@@ -1,16 +1,19 @@
 #!/usr/bin/env python
-"""Benchmark of the B200-native PARSeq engine: images/sec, PARSeq-S 32x128, AR + 1 refine iteration
+"""Benchmark of the H100-native (sm_90a) PARSeq engine: images/sec, PARSeq-S 32x128, AR + 1 refine iteration
 (BASELINE.json metric; configs[1]: bs=512 per GPU, bf16 tensor-core operands, synthetic crops / seeded
 random weights), end to end through the host-buffer C-ABI call, p50 latency at bs=1 (engine call and the
 reference's own `model(x)` protocol), roofline entries for every kernel kind >= 10 % of the step, a parity
 check of the timed batch against the fp32 oracle, the other BASELINE configs, and the reference's CPU path
 timed beside it.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One JSON line on stdout (rank 0).  "step" = one forward of `batch` images per GPU (weak scaling:
 images are independent, no data-path collective; model.py:105-169 has no cross-image dependency).
+--dump-outputs DIR writes what the last timed step returned (logits, ids, steps of rank 0) as DIR/<name>.npy in
+float32, at most 64 MB (larger batches: a fixed seeded sample of image rows, indices in rows.npy); weights and inputs
+are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -45,12 +48,12 @@ def parse_args():
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--no-pdl", action="store_true")
     ap.add_argument("--fuse-ln", type=int, default=-1, help="bit 0: attn.proj, bit 1: mlp.fc2 fused with the following LayerNorm (engine default 3)")
-    ap.add_argument("--attn-impl", type=int, default=-1, help="encoder attention: 1 tcgen05 (default), 0 mma.sync")
+    ap.add_argument("--attn-impl", type=int, default=-1, help="encoder attention: 0 mma.sync (default), 1 wgmma")
     ap.add_argument("--ar-kernel", type=int, default=-1, help="AR loop: 2 cluster kernel (default), 1 grid-barrier kernel, 0 separate kernels")
     ap.add_argument("--cta-group", type=int, default=0, help="GEMM tile: 0 auto, 1 single CTA, 2 CTA pair")
     ap.add_argument("--ln-cta-group", type=int, default=0, help="fused GEMM+LN tile: 0 auto, 1 single CTA, 2 CTA pair")
     ap.add_argument("--pair-pdl", type=int, default=-1, help="experiments: PDL attribute on CTA-pair launches")
-    ap.add_argument("--ln-split", type=int, default=-1, help="fused GEMM+LN: 2 = column-split CTA-pair kernel (gemm_ln2.cuh), 1 = full-row kernel")
+    ap.add_argument("--ln-split", type=int, default=-1, help="fused GEMM+LN: 2 = column-split CTA-pair kernel, 1 = full-row kernel")
     ap.add_argument("--fuse-mlp", type=int, default=-1, help="1: fc1 + GELU + fc2 + residual + LayerNorm in one kernel (mlp_ln.cuh)")
     ap.add_argument("--block-n", type=int, default=0)
     ap.add_argument("--no-cpu-baseline", action="store_true")
@@ -58,7 +61,12 @@ def parse_args():
     ap.add_argument("--no-configs", action="store_true", help="skip the other BASELINE configs (C1, C4, C5)")
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--no-two-in-flight", action="store_true", help="skip the two-handles / two-threads end-to-end extra")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    return args
 
 
 def load_peaks():
@@ -67,7 +75,8 @@ def load_peaks():
         with open(p) as f:
             d = json.load(f)
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA's H100 SXM data sheet (700 W card): HBM3 bandwidth and dense BF16 tensor rate; never reached in practice
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -429,7 +438,7 @@ def main():
     B = args.batch
     st = torch.cuda.current_stream(dev)
 
-    # Inputs larger than L2: NROT distinct resident batches (NROT * 25.2 MB > 126 MB), rotated per step.
+    # Inputs larger than L2: NROT distinct resident batches (NROT * 25.2 MB > 50 MB), rotated per step.
     NROT = 8
     batches_cpu = [synth_images(cfg, B, 100 + rank * NROT + i) for i in range(NROT)]
     batches = [b.to(dev) for b in batches_cpu]
@@ -467,6 +476,20 @@ def main():
         dist.barrier()
     clocks = sampler.stop() if rank == 0 else {}
     value = world * B * args.steps / (ms / 1000.0)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        # at most 64 MB in all: above that, a fixed seeded sample of image rows (their indices go to rows.npy)
+        row_bytes = (logits[0].numel() + ids[0].numel()) * 4
+        keep = max(1, (64_000_000 - 4096) // (row_bytes + 4))
+        out = {"logits": logits, "ids": ids}
+        if B > keep:
+            rows = torch.randperm(B, generator=torch.Generator().manual_seed(0))[:keep].sort().values
+            out = {k: v[rows.to(dev)] for k, v in out.items()}
+            out["rows"] = rows
+        out["steps"] = steps_t
+        for name, t in out.items():
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), t.float().cpu().numpy())
 
     # ---- the one collective of the path, outside the throughput region: all-gather of the decoded ids over NCCL ----
     gather = None
@@ -598,7 +621,7 @@ def main():
         del model_b
 
     peaks, peak_src = load_peaks()
-    # kernels are timed inside a long step -> the sustained cuBLAS figure is the tensor denominator
+    # kernels are timed inside a long step -> a sustained (measured) rate is the tensor denominator where one is known
     peak_tf = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1400.0)))
     peak_hbm = float(peaks.get("hbm_gbs", 6650.0))
 
@@ -620,20 +643,12 @@ def main():
     tim = eng.get_timing()
     eng.set_option("timing", 0)
     total_timed = sum(v["ms"] for v in tim.values())
-    ncu = {}
-    for name in ("r2_ncu_traffic.json", "r1_gemm_ncu_traffic.json"):
-        tpath = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(tpath):          # dram__bytes_read+write per launch from the committed ncu --set full captures
-            with open(tpath) as f:
-                ncu = json.load(f)
-            ncu["_file"] = "profiles/" + name
-            break
     by_cat = {k: round(v["ms"], 4) for k, v in tim.items()}
     whole = (value / world) * ALG_GFLOP_PER_IMAGE * 1e9 / (peak_tf * 1e12)
     D_, T_, Mrows = cfg.embed_dim, cfg.enc_tokens, B * cfg.enc_tokens
     L_, C_, V_, Md_ = 26, cfg.num_classes, cfg.num_tokens, cfg.embed_dim * cfg.dec_mlp_ratio
 
-    def entry(cat, bound, kernel, alg_per_launch_total, unit, traffic_key, note=None):
+    def entry(cat, bound, kernel, alg_per_launch_total, unit, note=None):
         """alg_per_launch_total: algorithmic bytes (hbm) or flops (tensor) summed over the category's launches."""
         t = tim.get(cat)
         if not t or t["launches"] == 0 or t["ms"] <= 0:
@@ -642,7 +657,6 @@ def main():
         peak = peak_hbm if bound == "hbm" else peak_tf
         e = {"bound": bound, "kernel": kernel, "achieved": ach, "peak": peak, "unit": unit, "frac": ach / peak,
              "peak_source": f"{peak_src} " + ("hbm_gbs" if bound == "hbm" else "bf16_tflops_sustained"),
-             "traffic": ncu.get(traffic_key), "traffic_source": ncu.get("_file"),
              ("bytes_per_launch" if bound == "hbm" else "flops_per_launch"): alg_per_launch_total / t["launches"],
              "launches_per_step": t["launches"], "avg_launch_ms": t["ms"] / t["launches"],
              "share_of_step": t["ms"] / total_timed if total_timed else None,
@@ -661,20 +675,18 @@ def main():
     ar_bytes = sum(B * T_ * 2 * D_ * 2 + B * (s + 1) * 2 * D_ * 2 + (3 * D_ * D_ + 2 * D_ * Md_ + C_ * D_) * 2 + B * C_ * 4
                    for s in range(L_))
     entries = [
-        entry("enc_gemm", "tensor", "gemm_bf16_tcgen05_kernel (QKV, fc1+GELU, patch embedding)", tim["enc_gemm"]["flops"], "TFLOP/s",
-              "avg_dram_bytes_per_launch"),
-        entry("enc_gemm_ln", "hbm", "gemm_ln_fused_kernel (attn.proj) / gemm_ln_split_kernel (mlp.fc2): residual GEMM + the following LayerNorm",
-              (fused_bytes(D_) + fused_bytes(D_ * cfg.enc_mlp_ratio)) * (n_fused / 2.0), "GB/s", "fused_avg_dram_bytes_per_launch"),
+        entry("enc_gemm", "tensor", "gemm_bf16_wgmma_kernel (QKV, fc1+GELU, patch embedding)", tim["enc_gemm"]["flops"], "TFLOP/s"),
+        entry("enc_gemm_ln", "hbm", "gemm_ln_fused_kernel (attn.proj; mlp.fc2 on column-split CTA pairs): residual GEMM + the following LayerNorm",
+              (fused_bytes(D_) + fused_bytes(D_ * cfg.enc_mlp_ratio)) * (n_fused / 2.0), "GB/s"),
         entry("dec_ar", "hbm", "dec_ar2_kernel (whole AR loop: 26 steps; independent clusters of 6 / 8 CTAs, TMA producer warp)"
               if args.ar_kernel in (-1, 2) else "dec_ar_kernel (whole AR loop, grid barriers)",
-              ar_bytes * tim.get("dec_ar", {}).get("launches", 0), "GB/s", "dec_ar_dram_bytes_per_launch",
+              ar_bytes * tim.get("dec_ar", {}).get("launches", 0), "GB/s",
               note="bytes = 26 x (cross K/V cache of the batch + context K/V rows + decoder weights + logits row); the loop is "
-                   "a chain of 26 x 11 dependent phases per cluster (latency-bound: profiles/r2_ar_phase_stamps_bs512.txt), "
-                   "tensor view: see tflops"),
-        entry("enc_attn", "hbm", "enc_attention_tc_kernel (QK^T, softmax, PV per (image, head))",
-              (Mrows * 3 * D_ * 2 + Mrows * D_ * 2) * tim["enc_attn"]["launches"], "GB/s", "attn_dram_bytes_per_launch"),
-        entry("dec_gemm", "tensor", "gemm_bf16_tcgen05_kernel (cross K/V projection, refine-pass projections, head)",
-              tim["dec_gemm"]["flops"], "TFLOP/s", None),
+                   "a chain of 26 x 11 dependent phases per cluster (latency-bound), tensor view: see tflops"),
+        entry("enc_attn", "hbm", "enc_attention_kernel (QK^T, softmax, PV per (image, head), mma.sync)",
+              (Mrows * 3 * D_ * 2 + Mrows * D_ * 2) * tim["enc_attn"]["launches"], "GB/s"),
+        entry("dec_gemm", "tensor", "gemm_bf16_wgmma_kernel (cross K/V projection, refine-pass projections, head)",
+              tim["dec_gemm"]["flops"], "TFLOP/s"),
     ]   # dec_attn / layernorm / other are a few percent of the step: see by_category_ms
     entries = [e for e in entries if e is not None]
     entries.sort(key=lambda e: -(e["share_of_step"] or 0.0))
@@ -739,12 +751,13 @@ def main():
 
     line = {
         "metric": "images/sec PARSeq-S 32x128 AR+1refine", "value": value, "unit": "images/s",
-        "n_gpus": world, "steps": args.steps, "warmup": max(3, args.warmup), "ms_per_step": ms / args.steps,
+        "n_gpus": world, "device": torch.cuda.get_device_name(dev), "steps": args.steps, "warmup": max(3, args.warmup),
+        "ms_per_step": ms / args.steps,
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16",
         "data": "synthetic",
         "config": {"workload": "PARSeq-S 32x128 94-char max_len=25 bs=512/GPU AR + 1 refine (BASELINE configs[1])",
                    "batch_per_gpu": B, "global_batch": B * world, "parallelism": f"dp{world} (batch-sharded, no collective)",
-                   "l2": f"inputs rotate over {NROT} resident batches ({NROT * B * 49152 / 1e6:.0f} MB > 126 MB L2)",
+                   "l2": f"inputs rotate over {NROT} resident batches ({NROT * B * 49152 / 1e6:.0f} MB > 50 MB L2)",
                    "chunk": args.chunk or (args.max_batch or 512), "max_batch": args.max_batch or 512, "dec_chunk": args.dec_chunk or 128, "cuda_graph": not args.no_graph},
         "clocks": clocks,
         "e2e": {"value": e2e_val, "unit": "images/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,

@@ -1,5 +1,5 @@
 /*
- * parseq_b200.h - C ABI of the B200-native PARSeq inference engine (libparseq_b200.so).
+ * parseq_b200.h - C ABI of the H100-native (sm_90a) PARSeq inference engine (libparseq_b200.so).
  *
  * The reference (baudm/parseq) has no FFI / plugin boundary for this path: it sits behind the Python
  * class strhub.models.parseq.system.PARSeq (system.py:33-88) wrapping the nn.Module
@@ -30,7 +30,7 @@ typedef enum parseq_status {
   PARSEQ_ERR_UNSUPPORTED = -2,           /* configuration outside what the kernels cover */
   PARSEQ_ERR_CUDA = -3,
   PARSEQ_ERR_STATE = -4,                 /* e.g. forward before finalize, missing weight */
-  PARSEQ_ERR_NO_DEVICE = -5              /* no sm_100 device: there is NO CPU fallback */
+  PARSEQ_ERR_NO_DEVICE = -5              /* no sm_90 device: there is NO CPU fallback */
 } parseq_status;
 
 /* Architecture hyper-parameters: the ctor arguments of model.PARSeq (model.py:33-49) /
@@ -150,12 +150,14 @@ int64_t parseq_debug_int(parseq_engine* e, const char* name);
  * also produces the LayerNorm that follows it, used when the batch fills the machine at least twice with 128-row tiles; bit 2:
  * for any batch; default 3; 0: separate LayerNorm kernels), "ar_kernel" (AR loop: 2 = cluster-owned persistent kernel,
  * default; 1 = grid-barrier persistent kernel; 0 = chain of separate kernels), "fuse_mlp" (1: fc1 + GELU + fc2 + residual +
- * LayerNorm of an encoder block in one kernel where fuse_ln bit 1 applies - bit-identical results, slower on B200, default 0),
- * "attn_impl", "cta_group" / "ln_cta_group" / "mlp_cta_group" (0 auto, 1 single CTA, 2 CTA pair: GEMM / fused GEMM+LayerNorm /
- * one-kernel MLP), "ln_split" (fused GEMM+LayerNorm: 0 auto = the column-split CTA-pair kernel for K >= 768, 1 never, 2 always),
- * "pair_pdl", "gemm_stages", "tma_epilogue" (kernel-variant switches for tests).  Options are PER HANDLE; with
- * e == NULL the launch options (block_n, attn_impl, pdl, tma_epilogue, gemm_stages, cta_group, ln_cta_group, mlp_cta_group,
- * ln_split, pair_pdl) set the process defaults that the stand-alone kernel
+ * LayerNorm of an encoder block in one kernel where fuse_ln bit 1 applies - bit-identical results, default 0), "attn_impl"
+ * (encoder attention: 0 = mma.sync kernels, default; 1 = wgmma kernel), "cta_group" / "ln_cta_group" / "mlp_cta_group"
+ * (0 auto, 1 single CTA, 2 CTA pair sharing the weight tiles by TMA multicast: GEMM / fused GEMM+LayerNorm / one-kernel
+ * MLP), "ln_split" (fused GEMM+LayerNorm: 0 auto = the column-split CTA-pair kernel for K >= 768, 1 never,
+ * 2 always), "pair_pdl", "gemm_stages" (kernel-variant switches for tests).  Options are PER HANDLE; with
+ * e == NULL the launch options (block_n, attn_impl, pdl, gemm_stages, cta_group, ln_cta_group, mlp_cta_group, ln_split,
+ * pair_pdl) set the
+ * process defaults that the stand-alone kernel
  * entry points below use and that handles created afterwards inherit. */
 int parseq_set_option(parseq_engine* e, const char* name, int64_t value);
 /* After a synchronised forward with "timing"=1: device milliseconds, algorithmic FLOPs and launch count of
@@ -169,7 +171,7 @@ const char* parseq_last_error(void);
 const char* parseq_version(void);
 
 /* Stand-alone kernel entry points (unit tests of the building blocks; all pointers DEVICE). */
-/* C[M,N] = epilogue(A[M,K](bf16,row-major,lda) * W[N,K]^T(bf16,row-major,ldw) + bias) on tcgen05.
+/* C[M,N] = epilogue(A[M,K](bf16,row-major,lda) * W[N,K]^T(bf16,row-major,ldw) + bias) on wgmma.
  * mode: 0 -> fp32 out (alpha*(acc+bias) [+ resid[row % resid_mod or row]]), 1 -> bf16 out,
  *       2 -> bf16 gelu(acc+bias). */
 int parseq_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, const float* bias,
@@ -187,10 +189,6 @@ int parseq_gemm_ln_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, 
 int parseq_mlp_ln_bf16(const void* xn, const void* W1, const float* b1, const void* W2, const float* b2,
                        int M, int D, float* x_inout, const float* gamma, const float* beta, float eps,
                        void* xn_out_bf16, parseq_stream_t stream);
-/* Same with cycle counters of CTA 0 (16 x uint64, device) for tests/prof_mlp_ln.py. */
-int parseq_mlp_ln_bf16_prof(const void* xn, const void* W1, const float* b1, const void* W2, const float* b2,
-                            int M, int D, float* x_inout, const float* gamma, const float* beta, float eps,
-                            void* xn_out_bf16, unsigned long long* prof_dev, parseq_stream_t stream);
 /* y = bf16(LayerNorm(x; gamma, beta, eps)), x fp32 [M, D]. */
 int parseq_layernorm_bf16(const float* x, const float* gamma, const float* beta, float eps, int M,
                           int D, void* y_bf16, float* y_f32_or_null, parseq_stream_t stream);

@@ -119,6 +119,64 @@ def main(cases=None):
               f"min margin {o.min_margin.min().item():.2e} bf16-model err {bf16_err}")
 
 
+# Files under tests/golden stay below 1 MB: a set whose logits would not fit keeps the rest of them in <name>_tail.pt
+# (the tests concatenate blob["logits"] and the tail's "logits").
+GOLDEN_FILE_LIMIT = 1_000_000
+
+
+def save_filtered(blob, name):
+    tail = os.path.join(OUT, name + "_tail.pt")
+    if os.path.exists(tail):
+        os.remove(tail)
+    blob = dict(blob)
+    blob.pop("logits_tail", None)
+    lg = blob["logits"]
+    if lg.numel() * lg.element_size() > GOLDEN_FILE_LIMIT * 3 // 4:
+        half = lg.shape[0] // 2
+        blob["logits"], blob["logits_tail"] = lg[:half].clone(), name + "_tail.pt"
+        torch.save({"logits": lg[half:].clone()}, tail)
+    torch.save(blob, os.path.join(OUT, name + ".pt"))
+
+
+def load_filtered(name):
+    blob = torch.load(os.path.join(OUT, name + ".pt"), weights_only=False)
+    if "logits_tail" in blob:
+        tail = torch.load(os.path.join(OUT, blob.pop("logits_tail")), weights_only=False)["logits"]
+        blob["logits"] = torch.cat([blob["logits"], tail])
+    return blob
+
+
+def make_reference_checks():
+    """Outputs of the reference's own modules for the comparisons that used to import them live
+    (tests/test_oracle_golden.py, tests/test_host_api.py), under tests/golden/reference/."""
+    from parseq_b200.config import CHARSET_94
+    out = os.path.join(OUT, "reference")
+    os.makedirs(out, exist_ok=True)
+    cfg, sd = make_sd("parseq-tiny", 11, 0.0)
+    ref, tok = RL.build_reference_model(cfg, sd)
+    x = synth_images(cfg, 2, 12)
+    modes = []
+    for ar, ri, ml in [(True, 1, None), (False, 0, None), (True, 2, 4)]:
+        ref.decode_ar, ref.refine_iters = ar, ri
+        with torch.inference_mode():
+            modes.append(dict(decode_ar=ar, refine_iters=ri, max_length=ml, logits=ref(tok, x, ml).clone()))
+    torch.save(dict(experiment="parseq-tiny", weight_seed=11, image_seed=12, batch=2, sd_digest=state_dict_digest(sd),
+                    modes=modes), os.path.join(out, "ti_modes.pt"))
+    cfg_s, sd_s = make_sd("parseq", 0, 0.0)
+    ref_s, _ = RL.build_reference_model(cfg_s, sd_s)
+    _, RefTok = RL.load_reference_classes()
+    rt = RefTok(CHARSET_94)
+    probs = torch.zeros(2, 5, 95)
+    seq = [[11, 12, 0, 13, 14], [36 + 1, 1, 2, 3, 4]]
+    for b in range(2):
+        for i, t in enumerate(seq[b]):
+            probs[b, i, t] = 0.9
+    labels, ps = rt.decode(probs)
+    torch.save(dict(state_dict_keys=sorted(ref_s.state_dict()), tokenizer_encode=rt.encode(["ab", "hello!"]),
+                    tokenizer_probs=probs, tokenizer_labels=labels, tokenizer_label_probs=[p.clone() for p in ps]),
+               os.path.join(out, "api.pt"))
+
+
 def make_filtered(name, exp, wseed, ar, ri, ml, n_blocks, block, tau, first_block=0):
     """Margin-filtered free-running set (SURVEY.md 7.2-1d): candidates whose smallest top1-top2 margin over
     every argmax decision of the fp32 reference run exceeds `tau`; on these, decoded ids must be bit-identical
@@ -145,7 +203,7 @@ def make_filtered(name, exp, wseed, ar, ri, ml, n_blocks, block, tau, first_bloc
     blob = dict(name=name, experiment=exp, weight_seed=wseed, decode_ar=ar, refine_iters=ri, max_length=ml,
                 block=block, tau=tau, candidates=n_cand, acceptance_rate=len(picks) / max(1, n_cand), picks=picks, ids=torch.stack(ids),
                 logits=torch.stack(logits), margins=torch.tensor(margins), sd_digest=state_dict_digest(sd))
-    torch.save(blob, os.path.join(OUT, name + ".pt"))
+    save_filtered(blob, name)
 
 
 # (case name, config overrides, weight seed, batch, image seed, max_length)
@@ -197,8 +255,8 @@ if __name__ == "__main__":
         first, n = int(sys.argv[2]), int(sys.argv[3])
         make_filtered("filtered_s_ar1_part", "parseq", 0, True, 1, None, n, 256, 0.02, first_block=first)
     elif len(sys.argv) > 1 and sys.argv[1] == "filtered_merge":
-        a = torch.load(os.path.join(OUT, "filtered_s_ar1.pt"), weights_only=False)
-        b = torch.load(os.path.join(OUT, "filtered_s_ar1_part.pt"), weights_only=False)
+        a = load_filtered("filtered_s_ar1")
+        b = load_filtered("filtered_s_ar1_part")
         assert a["sd_digest"] == b["sd_digest"] and a["tau"] == b["tau"] and a["block"] == b["block"]
         assert not (set(a["picks"]) & set(b["picks"]))
         a["picks"] = a["picks"] + b["picks"]
@@ -206,9 +264,11 @@ if __name__ == "__main__":
             a[k] = torch.cat([a[k], b[k]])
         a["candidates"] += b["candidates"]
         a["acceptance_rate"] = len(a["picks"]) / a["candidates"]
-        torch.save(a, os.path.join(OUT, "filtered_s_ar1.pt"))
+        save_filtered(a, "filtered_s_ar1")
         os.remove(os.path.join(OUT, "filtered_s_ar1_part.pt"))
         print("merged:", len(a["picks"]), "picks of", a["candidates"], "candidates")
+    elif len(sys.argv) > 1 and sys.argv[1] == "reference_checks":
+        make_reference_checks()
     elif len(sys.argv) > 1 and sys.argv[1] == "filtered":
         # 176 blocks of 256 candidates: ~0.25 % pass the margin filter at full length (a property of the near-flat random-init
         # logits, not of the engine) -> >= 100 accepted sequences; ~25 CPU-minutes on 8 cores

@@ -1,6 +1,6 @@
 // Persistent autoregressive-decode kernel: the whole `decode_ar` loop of PARSeq.forward (model.py:119-147) for one
 // super-chunk of images in ONE launch.  The AR loop is a chain of tiny, strictly dependent operations (M = batch rows
-// per step); as separate kernels each link costs a kernel boundary (~10 us measured on B200, 10 links per step, 26
+// per step); as separate kernels each link costs a kernel boundary (a launch gap each, 10 links per step, 26
 // steps).  Here every step is 8 phases separated by a software grid barrier (~2 us):
 //   P1 self-attention over the (position, token) K/V table            (warp per (image, head))
 //   P2 y  = pos_queries[i] + out_proj(sa)                              (64x64 mma.sync tiles)
@@ -11,8 +11,8 @@
 //   P7 part[s] = linear2(hd) over K-slice s (3-way split-K, deterministic: no atomics)
 //   P8 logits[:, i] = head(LN3(y + part0 + part1 + part2)); ids[:, i+1] = argmax   (64x96 tiles, argmax in the epilogue)
 // The projections of one step are 1.7 GFLOP over M <= 512 rows: latency-, not throughput-bound, so they run on
-// warp-level mma.sync tiles fed by cp.async (no TMEM/TMA set-up cost per phase); the large-M refine / NAR passes and the
-// encoder stay on the tcgen05 GEMM.  Numerics: identical rounding points to the multi-kernel path (bf16 operands,
+// warp-level mma.sync tiles fed by cp.async (no TMA / mbarrier set-up cost per phase); the large-M refine / NAR passes and the
+// encoder stay on the wgmma GEMM.  Numerics: identical rounding points to the multi-kernel path (bf16 operands,
 // fp32 accumulation, fp32 residual stream y, fp32 LayerNorm / softmax statistics).
 #pragma once
 #include <type_traits>

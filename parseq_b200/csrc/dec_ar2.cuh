@@ -87,7 +87,7 @@ __device__ __forceinline__ uint32_t box_off(int r, int c) {
 
 template <int D, int MT, int CS_>
 struct A2Cfg {
-  static constexpr int CS = CS_;                       // CTAs per cluster (8; 6 packs 23 instead of 15 clusters on a B200)
+  static constexpr int CS = CS_;                       // CTAs per cluster (8; 6 can pack more SMs of a GPC)
   static constexpr int ROWS = 16 * MT;                 // rows (images) per cluster, padded
   static constexpr int OWN = (ROWS + CS - 1) / CS;     // rows owned by one CTA for the attention phases
   static constexpr int DS = D / CS;                    // column slice of a D-wide projection

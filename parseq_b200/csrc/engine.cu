@@ -1,7 +1,7 @@
-// libparseq_b200.so: host-side engine + C ABI (include/parseq_b200.h) of the B200-native PARSeq
+// libparseq_b200.so: host-side engine + C ABI (include/parseq_b200.h) of the H100-native (sm_90a) PARSeq
 // inference path.  Restates, as a fixed kernel schedule on one CUDA stream, what
 // strhub/models/parseq/model.py:105-169 (PARSeq.forward: encode, AR loop, NAR, cloze refinement)
-// does through nn.Module calls.  There is no CPU path: without an sm_100 device creation fails.
+// does through nn.Module calls.  There is no CPU path: without an sm_90 device creation fails.
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -18,10 +18,9 @@
 #include "kernels.cuh"
 #include "dec_ar.cuh"
 #include "dec_ar2.cuh"
-#include "attn_tc.cuh"
 #include "gemm_ln.cuh"
-#include "gemm_ln2.cuh"
 #include "mlp_ln.cuh"
+#include "attn_wgmma.cuh"
 
 namespace {
 
@@ -111,14 +110,13 @@ struct LaunchOpts {
   int sm_count = 0;
   bool use_pdl = true;          // programmatic dependent launch on every kernel of the forward chain
   int block_n = 0;              // 0 = auto
-  int cta_group = 0;            // 0 = auto, 1 / 2 = forced (tests)
+  int cta_group = 0;            // 0 = auto, 1 / 2 = forced (tests): CTA pairs share the W tile by TMA multicast
   int ln_cta_group = 0;         // same for the fused GEMM + LayerNorm kernel
-  int ln_split = 0;             // fused GEMM + LayerNorm: 2 = column-split CTA-pair kernel (gemm_ln2.cuh), 0 / 1 = gemm_ln.cuh
+  int ln_split = 0;             // fused GEMM + LayerNorm: 2 = column-split CTA-pair kernel (gemm_ln.cuh MODE 2), 0 = auto, 1 = never
   int mlp_cta_group = 0;        // one-kernel MLP (mlp_ln.cuh): 0 = auto (pairs), 1 / 2 = forced
   bool pair_pdl = false;        // experiments: programmatic dependent launch also on CTA-pair (cluster) launches
-  bool no_tma_epilogue = false; // tests: force the direct-store epilogue
   int gemm_stages = 0;          // experiments: cap the operand ring depth (0 = full)
-  int attn_impl = 1;            // 1: tcgen05 kernel (attn_tc.cuh), 0: mma.sync kernel (kernels.cuh)
+  int attn_impl = 0;            // 0: mma.sync kernels (kernels.cuh), the faster on H100; 1: wgmma kernel (attn_wgmma.cuh)
 };
 LaunchOpts g_default_opts;
 
@@ -149,19 +147,18 @@ int launch_k(const LaunchOpts& lo, void (*kern)(KArgs...), dim3 grid, dim3 block
 }
 
 template <int BN, int CG>
-int launch_gemm_cfg(const LaunchOpts& lo, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
-                    const pq::GemmParams& p, int tiles, cudaStream_t st) {
-  auto kern = pq::gemm_bf16_tcgen05_kernel<BN, CG>;
+int launch_gemm_cfg(const LaunchOpts& lo, const CUtensorMap& ta, const CUtensorMap& tb, const pq::GemmParams& p, int tiles,
+                    cudaStream_t st) {
+  auto kern = pq::gemm_bf16_wgmma_kernel<BN, CG>;
   using Cfg = pq::GemmCfg<BN, CG>;
   static bool attr_set = false;
   if (!attr_set) {
     PQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_set = true;
   }
-  const int max_groups = lo.sm_count / CG;
-  const int groups = tiles < max_groups ? tiles : max_groups;
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(groups * CG));
+  const int max_groups = lo.sm_count / CG;                 // persistent: one CTA (pair) per SM (pair), tiles strided
+  cfg.gridDim = dim3(static_cast<unsigned>((tiles < max_groups ? tiles : max_groups) * CG));
   cfg.blockDim = dim3(pq::GEMM_THREADS);
   cfg.dynamicSmemBytes = Cfg::kSmemBytes;
   cfg.stream = st;
@@ -174,14 +171,14 @@ int launch_gemm_cfg(const LaunchOpts& lo, const CUtensorMap& ta, const CUtensorM
   attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = (lo.use_pdl && (CG == 1 || lo.pair_pdl)) ? 2 : 1;
-  PQ_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, tc, p));
+  PQ_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, p));
   return PARSEQ_OK;
 }
 
 // instantiate + set the smem attribute of every configuration outside of any stream capture
 template <int BN, int CG>
 int warm_gemm_cfg() {
-  return cudaFuncSetAttribute(pq::gemm_bf16_tcgen05_kernel<BN, CG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  return cudaFuncSetAttribute(pq::gemm_bf16_wgmma_kernel<BN, CG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                               pq::GemmCfg<BN, CG>::kSmemBytes) == cudaSuccess ? PARSEQ_OK
                                                                                 : fail(PARSEQ_ERR_CUDA, "cudaFuncSetAttribute(gemm)");
 }
@@ -223,8 +220,27 @@ int ar2_set_attributes() {
   return PARSEQ_OK;
 }
 
+template <int D, int MODE>
+int gemm_ln_attr() {
+  PQ_CUDA(cudaFuncSetAttribute(pq::gemm_ln_fused_kernel<D, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               pq::GemmLnCfg<D, MODE>::kSmemBytes));
+  return PARSEQ_OK;
+}
+
+template <int D, int CG>
+int mlp_ln_attr() {
+  PQ_CUDA(cudaFuncSetAttribute(pq::mlp_ln_fused_kernel<D, CG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               pq::MlpLnCfg<D, CG>::kSmemBytes));
+  return PARSEQ_OK;
+}
+template <int NK>
+int attn_wgmma_attr() {
+  PQ_CUDA(cudaFuncSetAttribute(pq::enc_attention_wgmma_kernel<NK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               pq::atw_smem_bytes<NK>()));
+  return PARSEQ_OK;
+}
+
 int init_kernel_attributes() {
-  PQ_CUDA(cudaFuncSetAttribute(pq::enc_attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, pq::ATC_SMEM_BYTES));
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar_kernel<192, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pq::dec_ar_smem_bytes<192>())));
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar_kernel<192, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pq::dec_ar_smem_bytes<192>())));
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar_kernel<384, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pq::dec_ar_smem_bytes<384>())));
@@ -235,15 +251,10 @@ int init_kernel_attributes() {
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ln_head_argmax_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, 120 * 1024));
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ln_head_argmax_kernel<384>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ln_head_argmax_kernel<768>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-  PQ_CUDA(cudaFuncSetAttribute(pq::gemm_ln_fused_kernel<192, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, pq::GemmLnCfg<192, 1>::kSmemBytes));
-  PQ_CUDA(cudaFuncSetAttribute(pq::gemm_ln_fused_kernel<384, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, pq::GemmLnCfg<384, 1>::kSmemBytes));
-  PQ_CUDA(cudaFuncSetAttribute(pq::gemm_ln_fused_kernel<192, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, pq::GemmLnCfg<192, 2>::kSmemBytes));
-  PQ_CUDA(cudaFuncSetAttribute(pq::gemm_ln_fused_kernel<384, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, pq::GemmLnCfg<384, 2>::kSmemBytes));
-  PQ_CUDA(cudaFuncSetAttribute(pq::gemm_ln_split_kernel<384>, cudaFuncAttributeMaxDynamicSharedMemorySize, pq::GemmLn2Cfg<384>::kSmemBytes));
-  PQ_CUDA(cudaFuncSetAttribute(pq::mlp_ln_fused_kernel<192, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, pq::MlpLnCfg<192, 1>::kSmemBytes));
-  PQ_CUDA(cudaFuncSetAttribute(pq::mlp_ln_fused_kernel<384, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, pq::MlpLnCfg<384, 1>::kSmemBytes));
-  PQ_CUDA(cudaFuncSetAttribute(pq::mlp_ln_fused_kernel<192, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, pq::MlpLnCfg<192, 2>::kSmemBytes));
-  PQ_CUDA(cudaFuncSetAttribute(pq::mlp_ln_fused_kernel<384, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, pq::MlpLnCfg<384, 2>::kSmemBytes));
+  PQ_TRY((gemm_ln_attr<192, 0>())); PQ_TRY((gemm_ln_attr<384, 0>())); PQ_TRY((gemm_ln_attr<192, 1>()));
+  PQ_TRY((gemm_ln_attr<384, 1>())); PQ_TRY((gemm_ln_attr<384, 2>()));
+  PQ_TRY((mlp_ln_attr<192, 1>())); PQ_TRY((mlp_ln_attr<384, 1>())); PQ_TRY((mlp_ln_attr<192, 2>())); PQ_TRY((mlp_ln_attr<384, 2>()));
+  PQ_TRY((attn_wgmma_attr<128>())); PQ_TRY((attn_wgmma_attr<256>()));
   PQ_TRY((warm_gemm_cfg<64, 1>()));
   PQ_TRY((warm_gemm_cfg<128, 1>()));
   PQ_TRY((warm_gemm_cfg<192, 1>()));
@@ -260,13 +271,11 @@ int gemm_launch(LaunchOpts& lo, const void* A, long long lda, const void* W, lon
                 cudaStream_t st, long long blocked_rows = 0) {
   if (M <= 0 || N <= 0 || K <= 0) return fail(PARSEQ_ERR_INVALID_ARG, "gemm: empty problem");
   PQ_TRY(ensure_sm_count(lo));
-  // Tile choice from tests/bench_gemm.py on B200 (profiles/r1_gemm_microbench*.txt): single-CTA 128 x 256 tiles win
-  // for the wide projections (QKV 1152 -> 4.5 tiles, fc1 1536), 128 x 192 for N = 384 / 768 (no padded columns),
-  // 128 x 128 for the small decoder GEMMs.
-  // CTA pairs (cta_group::2: each CTA holds half of the W tile) win once the main loop is long enough to amortise the
-  // pair's per-tile handshakes: measured (profiles/r2_gemm_cta_pair_sweep.txt) 0.81 - 0.98x the single-CTA time for
-  // K >= 768 (D = 768 configs, unfused fc2), 1.05 - 1.21x for K = 384.  The accumulation order per output element is the
-  // same, so the choice does not change a single bit of the result (test_cta_pair_rows_equal_single_cta_rows).
+  // Tile choice: 128 x 256 tiles for the wide projections (QKV 1152 -> 4.5 tiles, fc1 1536), 128 x 192 for N = 384 / 768
+  // (no padded columns), 128 x 128 for the small decoder GEMMs.
+  // CTA pairs (a cluster of two CTAs on 256 rows, the W tile multicast into both) halve the W traffic per output row;
+  // used where the main loop is long (K >= 768).  The accumulation order per output element is the same, so the choice
+  // does not change a single bit of the result (test_cta_pair_rows_equal_single_cta_rows).
   int CG = (K >= 768 && M >= 1024) ? 2 : 1;
   if (lo.cta_group) CG = lo.cta_group;
   int BN;
@@ -276,129 +285,74 @@ int gemm_launch(LaunchOpts& lo, const void* A, long long lda, const void* W, lon
     BN = lo.block_n;
     if (CG == 2 && BN == 64) BN = 128;
   }
-  CUtensorMap ta, tb, tc;
+  CUtensorMap ta, tb;
   PQ_TRY(make_tmap(&ta, A, 2, M, K, lda, pq::GEMM_BLOCK_K, pq::GEMM_BLOCK_M));
   PQ_TRY(make_tmap(&tb, W, 2, N, K, ldw, pq::GEMM_BLOCK_K, BN / CG));
   pq::GemmParams p;
   p.M = M; p.N = N; p.K = K; p.mode = mode; p.alpha = alpha; p.bias = bias;
   p.resid = resid; p.ldr = ldr; p.resid_mod = resid_mod; p.out = out; p.ldo = ldo;
   const int esz = (mode == pq::EPI_F32) ? 4 : 2;
-  bool vec = ((reinterpret_cast<uintptr_t>(out) & 15u) == 0) && ((ldo * esz) % 16 == 0);
-  if (resid != nullptr) vec = vec && ((reinterpret_cast<uintptr_t>(resid) & 15u) == 0) && ((ldr * 4) % 16 == 0);
-  if (bias != nullptr) vec = vec && ((reinterpret_cast<uintptr_t>(bias) & 15u) == 0);
+  bool vec = ((reinterpret_cast<uintptr_t>(out) & 7u) == 0) && ((ldo * esz) % 8 == 0);
+  if (resid != nullptr) vec = vec && ((reinterpret_cast<uintptr_t>(resid) & 7u) == 0) && ((ldr * 4) % 8 == 0);
   p.vec_ok = vec ? 1 : 0;
-  // asynchronous TMA epilogue whenever the output is TMA-addressable; residual only as in-place accumulate
-  p.tma_out = 0;
-  const bool out_ok = ((reinterpret_cast<uintptr_t>(out) & 15u) == 0) && ((ldo * esz) % 16 == 0) && !lo.no_tma_epilogue;
-  if (out_ok) {
-    if (mode != pq::EPI_F32) p.tma_out = 3;
-    else if (resid == nullptr) p.tma_out = 1;
-    else if (resid == out && ldr == ldo && resid_mod == 0) p.tma_out = 2;
-  }
+  p.blocked_rows = 0;
   if (blocked_rows > 0) {
     if (mode == pq::EPI_F32 || N % 64 != 0 || blocked_rows < M || (reinterpret_cast<uintptr_t>(out) & 15u) != 0)
       return fail(PARSEQ_ERR_INVALID_ARG, "gemm: blocked output needs a bf16 epilogue, N % 64 == 0 and rows >= M");
-    p.tma_out = 4;
-    PQ_TRY(make_tmap3d(&tc, out, 64, blocked_rows, N / 64, 64, 64 * blocked_rows, 64, 32));
-  } else if (p.tma_out == 3) PQ_TRY(make_tmap(&tc, out, 2, M, N, ldo, 64, 32));
-  else if (p.tma_out != 0) PQ_TRY(make_tmap(&tc, out, 4, M, N, ldo, 32, 32));
-  else tc = ta;
+    p.blocked_rows = blocked_rows;
+    p.vec_ok = 1;
+  }
   const int tile_m = pq::GEMM_BLOCK_M * CG;
   p.max_stages = lo.gemm_stages;
   p.num_m_tiles = (M + tile_m - 1) / tile_m;
   p.num_n_tiles = (N + BN - 1) / BN;
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   if (CG == 2) {
-    if (BN == 256) return launch_gemm_cfg<256, 2>(lo, ta, tb, tc, p, tiles, st);
-    if (BN == 192) return launch_gemm_cfg<192, 2>(lo, ta, tb, tc, p, tiles, st);
-    return launch_gemm_cfg<128, 2>(lo, ta, tb, tc, p, tiles, st);
+    if (BN == 256) return launch_gemm_cfg<256, 2>(lo, ta, tb, p, tiles, st);
+    if (BN == 192) return launch_gemm_cfg<192, 2>(lo, ta, tb, p, tiles, st);
+    return launch_gemm_cfg<128, 2>(lo, ta, tb, p, tiles, st);
   }
-  if (BN == 256) return launch_gemm_cfg<256, 1>(lo, ta, tb, tc, p, tiles, st);
-  if (BN == 192) return launch_gemm_cfg<192, 1>(lo, ta, tb, tc, p, tiles, st);
-  if (BN == 64) return launch_gemm_cfg<64, 1>(lo, ta, tb, tc, p, tiles, st);
-  return launch_gemm_cfg<128, 1>(lo, ta, tb, tc, p, tiles, st);
+  if (BN == 256) return launch_gemm_cfg<256, 1>(lo, ta, tb, p, tiles, st);
+  if (BN == 192) return launch_gemm_cfg<192, 1>(lo, ta, tb, p, tiles, st);
+  if (BN == 64) return launch_gemm_cfg<64, 1>(lo, ta, tb, p, tiles, st);
+  return launch_gemm_cfg<128, 1>(lo, ta, tb, p, tiles, st);
 }
 
 // x[M, D] += A[M, K] * W[D, K]^T + bias (fp32, in place); xn[M, D] = bf16(LayerNorm(x; gamma, beta, eps))   (gemm_ln.cuh)
 bool gemm_ln_supported(int D) { return D == 192 || D == 384; }
-template <int D, int CG>
+template <int D, int MODE>
 int launch_gemm_ln(const LaunchOpts& lo, const void* A, long long lda, const void* W, long long ldw, const float* bias, int M, int K, float* x,
                    const float* gamma, const float* beta, float eps, void* xn, cudaStream_t st) {
-  using Cfg = pq::GemmLnCfg<D, CG>;
-  auto kern = pq::gemm_ln_fused_kernel<D, CG>;
+  using Cfg = pq::GemmLnCfg<D, MODE>;
   static bool attr_set = false;
   if (!attr_set) {
-    PQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    PQ_TRY((gemm_ln_attr<D, MODE>()));
     attr_set = true;
   }
-  CUtensorMap ta, tb, tx, tn;
-  PQ_TRY(make_tmap(&ta, A, 2, M, K, lda, pq::GEMM_BLOCK_K, pq::GEMM_BLOCK_M));
-  PQ_TRY(make_tmap(&tb, W, 2, D, K, ldw, pq::GEMM_BLOCK_K, Cfg::kBRows));
-  PQ_TRY(make_tmap(&tx, x, 4, M, D, D, 32, 32));
-  PQ_TRY(make_tmap(&tn, xn, 2, M, D, D, 64, 32));
+  CUtensorMap ta, tb;
+  PQ_TRY(make_tmap(&ta, A, 2, M, K, lda, pq::GEMM_BLOCK_K, pq::GLN_BLOCK_M));
+  PQ_TRY(make_tmap(&tb, W, 2, D, K, ldw, pq::GEMM_BLOCK_K, Cfg::kBox));
+  if ((reinterpret_cast<uintptr_t>(x) & 7u) != 0 || (reinterpret_cast<uintptr_t>(xn) & 3u) != 0)
+    return fail(PARSEQ_ERR_INVALID_ARG, "gemm_ln: x must be 8-byte and xn 4-byte aligned");
   pq::GemmLnParams p;
   p.M = M; p.K = K; p.bias = bias; p.gamma = gamma; p.beta = beta; p.eps = eps;
-  const int tile_m = pq::GEMM_BLOCK_M * CG;
+  const int tile_m = pq::GLN_BLOCK_M * (MODE == 1 ? 2 : 1);
   p.num_m_tiles = (M + tile_m - 1) / tile_m;
-  const int max_groups = lo.sm_count / CG;
-  const int groups = p.num_m_tiles < max_groups ? p.num_m_tiles : max_groups;
-  if constexpr (CG == 1) {
-    return launch_k(lo, kern, dim3(groups), dim3(pq::GLN_THREADS), Cfg::kSmemBytes, st, ta, tb, tx, tn, p);
-  } else {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(groups * CG));
-    cfg.blockDim = dim3(pq::GLN_THREADS);
-    cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CG;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = (lo.use_pdl && lo.pair_pdl) ? 2 : 1;
-    PQ_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, tx, tn, p));
-    return PARSEQ_OK;
-  }
-}
-// version 2 (gemm_ln2.cuh): the columns of a 128-row tile split over a CTA pair, double-buffered TMEM, statistics through DSMEM
-int launch_gemm_ln_split(const LaunchOpts& lo, const void* A, long long lda, const void* W, long long ldw, const float* bias, int M, int K,
-                         float* x, const float* gamma, const float* beta, float eps, void* xn, cudaStream_t st) {
-  constexpr int D = 384;
-  using Cfg = pq::GemmLn2Cfg<D>;
-  auto kern = pq::gemm_ln_split_kernel<D>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    PQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_set = true;
-  }
-  CUtensorMap ta, tb, tx, tn;
-  PQ_TRY(make_tmap(&ta, A, 2, M, K, lda, pq::GEMM_BLOCK_K, pq::GEMM_BLOCK_M));
-  PQ_TRY(make_tmap(&tb, W, 2, D, K, ldw, pq::GEMM_BLOCK_K, Cfg::kN));
-  PQ_TRY(make_tmap(&tx, x, 4, M, D, D, 32, 32));
-  PQ_TRY(make_tmap(&tn, xn, 2, M, D, D, 64, 32));
-  pq::GemmLnParams p;
-  p.M = M; p.K = K; p.bias = bias; p.gamma = gamma; p.beta = beta; p.eps = eps;
-  p.num_m_tiles = (M + pq::GEMM_BLOCK_M - 1) / pq::GEMM_BLOCK_M;
-  const int max_groups = lo.sm_count / 2;
-  const int groups = p.num_m_tiles < max_groups ? p.num_m_tiles : max_groups;
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(groups * 2));
+  cfg.gridDim = dim3(static_cast<unsigned>(p.num_m_tiles * Cfg::kCG));
   cfg.blockDim = dim3(pq::GLN_THREADS);
   cfg.dynamicSmemBytes = Cfg::kSmemBytes;
   cfg.stream = st;
   cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.x = Cfg::kCG;
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = lo.use_pdl ? 2 : 1;
-  PQ_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, tx, tn, p));
+  cfg.numAttrs = (lo.use_pdl && (MODE == 0 || lo.pair_pdl)) ? 2 : 1;
+  PQ_CUDA(cudaLaunchKernelEx(&cfg, pq::gemm_ln_fused_kernel<D, MODE>, ta, tb, x, reinterpret_cast<__nv_bfloat16*>(xn), p));
   return PARSEQ_OK;
 }
 int gemm_ln_launch(LaunchOpts& lo, const void* A, long long lda, const void* W, long long ldw, const float* bias, int M, int D,
@@ -406,83 +360,71 @@ int gemm_ln_launch(LaunchOpts& lo, const void* A, long long lda, const void* W, 
   if (M <= 0 || K <= 0) return fail(PARSEQ_ERR_INVALID_ARG, "gemm_ln: empty problem");
   PQ_TRY(ensure_sm_count(lo));
   PQ_TRY(load_driver_api());
-  // CTA pairs stage 30 % fewer operand bytes per row, bit-identical results - and no gain (profiles/r2_gemm_ln_cta_pair.txt:
-  // fc2' 124.5 -> 123.7 us, proj' 64.8 -> 71.6 us): this kernel is not operand-ingest bound.  Opt-in ("ln_cta_group").
-  // The column-split pair kernel (gemm_ln2.cuh) pays where the MMAs of a tile are long enough to be worth hiding under the
-  // previous tile's epilogue: fc2 (K = 1536) 124.6 -> 110.7 us, attn.proj (K = 384) 64.8 -> 68.1 us
-  // (profiles/r2_gemm_ln_split_pair.txt).  ln_split: 0 auto (K >= 768), 1 never, 2 always (D = 384).  Where the fused kernels are
-  // used at all is decided by the caller from the batch regime (encode_chunk).
-  if (D == 384 && (lo.ln_split == 2 || (lo.ln_split == 0 && K >= 768)))   // by K only: a row's bits must not depend on the batch
-    return launch_gemm_ln_split(lo, A, lda, W, ldw, bias, M, K, x, gamma, beta, eps, xn, st);
-  int CG = 1;
-  if (lo.ln_cta_group) CG = lo.ln_cta_group;
-  if (CG == 2) {
-    if (D == 384) return launch_gemm_ln<384, 2>(lo, A, lda, W, ldw, bias, M, K, x, gamma, beta, eps, xn, st);
-    if (D == 192) return launch_gemm_ln<192, 2>(lo, A, lda, W, ldw, bias, M, K, x, gamma, beta, eps, xn, st);
+  // MODE 2 (the columns of a 64-row tile split over a CTA pair) halves the W bytes each CTA stages per k-block, so the
+  // ring is twice as deep where the main loop is long (fc2, K = 1536).  ln_split: 0 auto (K >= 768), 1 never, 2 always
+  // (D = 384).  Selected by K only: a row's bits must not depend on the batch.  MODE 1 (ln_cta_group = 2) shares the W
+  // tile of two 64-row tiles by multicast.  Where the fused kernels are used at all is decided by the caller from the
+  // batch regime (encode_chunk).
+  if (D == 384 && (lo.ln_split == 2 || (lo.ln_split == 0 && K >= 768)))
+    return launch_gemm_ln<384, 2>(lo, A, lda, W, ldw, bias, M, K, x, gamma, beta, eps, xn, st);
+  if (lo.ln_cta_group == 2) {
+    if (D == 384) return launch_gemm_ln<384, 1>(lo, A, lda, W, ldw, bias, M, K, x, gamma, beta, eps, xn, st);
+    if (D == 192) return launch_gemm_ln<192, 1>(lo, A, lda, W, ldw, bias, M, K, x, gamma, beta, eps, xn, st);
   }
-  if (D == 384) return launch_gemm_ln<384, 1>(lo, A, lda, W, ldw, bias, M, K, x, gamma, beta, eps, xn, st);
-  if (D == 192) return launch_gemm_ln<192, 1>(lo, A, lda, W, ldw, bias, M, K, x, gamma, beta, eps, xn, st);
-  return fail(PARSEQ_ERR_UNSUPPORTED, "gemm_ln: embed_dim must be 192 or 384 (full rows in 512 TMEM columns)");
+  if (D == 384) return launch_gemm_ln<384, 0>(lo, A, lda, W, ldw, bias, M, K, x, gamma, beta, eps, xn, st);
+  if (D == 192) return launch_gemm_ln<192, 0>(lo, A, lda, W, ldw, bias, M, K, x, gamma, beta, eps, xn, st);
+  return fail(PARSEQ_ERR_UNSUPPORTED, "gemm_ln: embed_dim must be 192 or 384");
 }
 
 // x[M, D] += GELU(xn W1^T + b1) W2^T + b2 (fp32, in place); xn_out = bf16(LayerNorm(x; gamma, beta, eps))   (mlp_ln.cuh)
 template <int D, int CG>
 int launch_mlp_ln(const LaunchOpts& lo, const void* xn, const void* W1, const float* b1, const void* W2, const float* b2, int M,
-                  float* x, const float* gamma, const float* beta, float eps, void* xn_out, cudaStream_t st, unsigned long long* prof) {
+                  float* x, const float* gamma, const float* beta, float eps, void* xn_out, cudaStream_t st) {
   using Cfg = pq::MlpLnCfg<D, CG>;
-  auto kern = pq::mlp_ln_fused_kernel<D, CG>;
   static bool attr_set = false;
   if (!attr_set) {
-    PQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    PQ_TRY((mlp_ln_attr<D, CG>()));
     attr_set = true;
   }
-  CUtensorMap txn, tw1, tw2, tx, tn;
-  PQ_TRY(make_tmap(&txn, xn, 2, M, D, D, pq::GEMM_BLOCK_K, pq::GEMM_BLOCK_M));
-  PQ_TRY(make_tmap(&tw1, W1, 2, Cfg::kH, D, D, pq::GEMM_BLOCK_K, Cfg::kW1Rows));
-  PQ_TRY(make_tmap(&tw2, W2, 2, D, Cfg::kH, Cfg::kH, pq::GEMM_BLOCK_K, Cfg::kW2Rows));
-  PQ_TRY(make_tmap(&tx, x, 4, M, D, D, 32, 32));
-  PQ_TRY(make_tmap(&tn, xn_out, 2, M, D, D, 64, 32));
+  if ((reinterpret_cast<uintptr_t>(x) & 7u) != 0 || (reinterpret_cast<uintptr_t>(xn_out) & 3u) != 0)
+    return fail(PARSEQ_ERR_INVALID_ARG, "mlp_ln: x must be 8-byte and xn_out 4-byte aligned");
+  CUtensorMap txn, tw1, tw2;
+  PQ_TRY(make_tmap(&txn, xn, 2, M, D, D, 64, pq::GLN_BLOCK_M));
+  PQ_TRY(make_tmap(&tw1, W1, 2, Cfg::kH, D, D, 64, Cfg::kW1Rows));
+  PQ_TRY(make_tmap(&tw2, W2, 2, D, Cfg::kH, Cfg::kH, 64, Cfg::kW2Rows));
   pq::MlpLnParams p;
-  p.M = M; p.b1 = b1; p.b2 = b2; p.gamma = gamma; p.beta = beta; p.eps = eps; p.prof = prof;
-  const int tile_m = pq::GEMM_BLOCK_M * CG;
-  p.num_m_tiles = (M + tile_m - 1) / tile_m;
-  const int max_groups = lo.sm_count / CG;
-  const int groups = p.num_m_tiles < max_groups ? p.num_m_tiles : max_groups;
-  if constexpr (CG == 1) {
-    return launch_k(lo, kern, dim3(groups), dim3(pq::MLP_THREADS), Cfg::kSmemBytes, st, txn, tw1, tw2, tx, tn, p);
-  } else {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(groups * CG));
-    cfg.blockDim = dim3(pq::MLP_THREADS);
-    cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CG;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = (lo.use_pdl && lo.pair_pdl) ? 2 : 1;
-    PQ_CUDA(cudaLaunchKernelEx(&cfg, kern, txn, tw1, tw2, tx, tn, p));
-    return PARSEQ_OK;
-  }
+  p.M = M; p.b1 = b1; p.b2 = b2; p.gamma = gamma; p.beta = beta; p.eps = eps;
+  p.num_m_tiles = (M + pq::GLN_BLOCK_M * CG - 1) / (pq::GLN_BLOCK_M * CG);
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(static_cast<unsigned>(p.num_m_tiles * CG));
+  cfg.blockDim = dim3(pq::MLP_THREADS);
+  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[2];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = CG;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[1].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = (lo.use_pdl && (CG == 1 || lo.pair_pdl)) ? 2 : 1;
+  PQ_CUDA(cudaLaunchKernelEx(&cfg, pq::mlp_ln_fused_kernel<D, CG>, txn, tw1, tw2, x, reinterpret_cast<__nv_bfloat16*>(xn_out), p));
+  return PARSEQ_OK;
 }
 int mlp_ln_launch(LaunchOpts& lo, const void* xn, const void* W1, const float* b1, const void* W2, const float* b2, int M, int D,
-                  float* x, const float* gamma, const float* beta, float eps, void* xn_out, cudaStream_t st,
-                  unsigned long long* prof = nullptr) {
+                  float* x, const float* gamma, const float* beta, float eps, void* xn_out, cudaStream_t st) {
   if (M <= 0) return fail(PARSEQ_ERR_INVALID_ARG, "mlp_ln: empty problem");
   PQ_TRY(ensure_sm_count(lo));
   PQ_TRY(load_driver_api());
-  // CTA pairs stage half of every weight box per CTA: the same ring covers twice as many k-steps (mlp_ln.cuh)
+  // CTA pairs fetch every weight box once per 128 rows instead of 64 (multicast)
   const int CG = lo.mlp_cta_group ? lo.mlp_cta_group : 2;
   if (CG == 2) {
-    if (D == 384) return launch_mlp_ln<384, 2>(lo, xn, W1, b1, W2, b2, M, x, gamma, beta, eps, xn_out, st, prof);
-    if (D == 192) return launch_mlp_ln<192, 2>(lo, xn, W1, b1, W2, b2, M, x, gamma, beta, eps, xn_out, st, prof);
+    if (D == 384) return launch_mlp_ln<384, 2>(lo, xn, W1, b1, W2, b2, M, x, gamma, beta, eps, xn_out, st);
+    if (D == 192) return launch_mlp_ln<192, 2>(lo, xn, W1, b1, W2, b2, M, x, gamma, beta, eps, xn_out, st);
   }
-  if (D == 384) return launch_mlp_ln<384, 1>(lo, xn, W1, b1, W2, b2, M, x, gamma, beta, eps, xn_out, st, prof);
-  if (D == 192) return launch_mlp_ln<192, 1>(lo, xn, W1, b1, W2, b2, M, x, gamma, beta, eps, xn_out, st, prof);
+  if (D == 384) return launch_mlp_ln<384, 1>(lo, xn, W1, b1, W2, b2, M, x, gamma, beta, eps, xn_out, st);
+  if (D == 192) return launch_mlp_ln<192, 1>(lo, xn, W1, b1, W2, b2, M, x, gamma, beta, eps, xn_out, st);
   return fail(PARSEQ_ERR_UNSUPPORTED, "mlp_ln: embed_dim must be 192 or 384 (hidden width 4 * embed_dim)");
 }
 
@@ -501,35 +443,23 @@ int layernorm_launch(const LaunchOpts& lo, const float* x, const float* g, const
 
 int enc_attention_launch(const LaunchOpts& lo, const void* qkv, int B, int T, int D, int heads, void* out, cudaStream_t st) {
   if (D != heads * pq::ATT_DH) return fail(PARSEQ_ERR_UNSUPPORTED, "encoder attention kernels cover head_dim=64");
-  if (T != pq::ATT_T && lo.attn_impl == 1 && T <= 256) {   // general token count on tcgen05: 3D maps [image][token][channel]
-    static bool attr_set2 = false;
-    if (!attr_set2) {
-      PQ_CUDA(cudaFuncSetAttribute(pq::enc_attention_tc2_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, pq::atc2_smem_bytes<1>()));
-      PQ_CUDA(cudaFuncSetAttribute(pq::enc_attention_tc2_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, pq::atc2_smem_bytes<2>()));
-      attr_set2 = true;
-    }
-    CUtensorMap tq, to;
-    PQ_TRY(make_tmap3d(&tq, qkv, 3ll * D, T, B, 3ll * D, 3ll * D * T, 64, 128));
-    PQ_TRY(make_tmap3d(&to, out, D, T, B, D, 1ll * D * T, 64, 32));
-    const dim3 grid(static_cast<unsigned>(B * heads), static_cast<unsigned>((T + 127) / 128));
-    if (T <= 128)
-      return launch_k(lo, pq::enc_attention_tc2_kernel<1>, grid, dim3(pq::ATC_THREADS), pq::atc2_smem_bytes<1>(), st, tq, to, D, heads, T);
-    return launch_k(lo, pq::enc_attention_tc2_kernel<2>, grid, dim3(pq::ATC_THREADS), pq::atc2_smem_bytes<2>(), st, tq, to, D, heads, T);
-  }
-  if (T != pq::ATT_T) {   // attn_impl = 0: masked two-pass mma.sync kernel (reference implementation of the unit tests)
-    return launch_k(lo, pq::enc_attention_any_kernel, dim3(B * heads, (T + pq::ATT_T - 1) / pq::ATT_T), dim3(256), 0, st,
-                    reinterpret_cast<const __nv_bfloat16*>(qkv), reinterpret_cast<__nv_bfloat16*>(out), T, D, heads);
-  }
-  if (lo.attn_impl == 1) {
-    static bool attr_set = false;
+  if (lo.attn_impl == 1 && T <= 256) {
+    static bool attr_set = false;            // the bare kernel entry point may run before any engine handle exists
     if (!attr_set) {
-      PQ_CUDA(cudaFuncSetAttribute(pq::enc_attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, pq::ATC_SMEM_BYTES));
+      PQ_TRY((attn_wgmma_attr<128>()));
+      PQ_TRY((attn_wgmma_attr<256>()));
       attr_set = true;
     }
-    CUtensorMap tq, to;
-    PQ_TRY(make_tmap(&tq, qkv, 2, static_cast<long long>(B) * T, 3ll * D, 3ll * D, 64, 128));
-    PQ_TRY(make_tmap(&to, out, 2, static_cast<long long>(B) * T, D, D, 64, 32));
-    return launch_k(lo, pq::enc_attention_tc_kernel, dim3(B * heads), dim3(pq::ATC_THREADS), pq::ATC_SMEM_BYTES, st, tq, to, D, heads);
+    const dim3 grid(static_cast<unsigned>(B * heads), static_cast<unsigned>((T + 127) / 128));
+    const __nv_bfloat16* q = reinterpret_cast<const __nv_bfloat16*>(qkv);
+    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);
+    if (T <= 128)
+      return launch_k(lo, pq::enc_attention_wgmma_kernel<128>, grid, dim3(pq::ATW_THREADS), pq::atw_smem_bytes<128>(), st, q, o, T, D, heads);
+    return launch_k(lo, pq::enc_attention_wgmma_kernel<256>, grid, dim3(pq::ATW_THREADS), pq::atw_smem_bytes<256>(), st, q, o, T, D, heads);
+  }
+  if (T != pq::ATT_T) {   // masked two-pass mma.sync kernel, any token count
+    return launch_k(lo, pq::enc_attention_any_kernel, dim3(B * heads, (T + pq::ATT_T - 1) / pq::ATT_T), dim3(256), 0, st,
+                    reinterpret_cast<const __nv_bfloat16*>(qkv), reinterpret_cast<__nv_bfloat16*>(out), T, D, heads);
   }
   return launch_k(lo, pq::enc_attention_kernel, dim3(B * heads), dim3(256), 0, st,
                   reinterpret_cast<const __nv_bfloat16*>(qkv), reinterpret_cast<__nv_bfloat16*>(out), D, heads);
@@ -794,7 +724,7 @@ int encode_chunk(parseq_engine* e, const void* images_any, bool u8, int B, __nv_
                 e->wf("encoder.pos_embed") + D, D, e->Tp, tmp, D, st));
     TimedScope ts(e, st, CAT_MISC, 0.0);
     const long long total = 1ll * M * (D / 4);
-    const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, 148ll * 16));
+    const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, 132ll * 16));
     PQ_TRY(launch_k(e->lo, pq::cls_assemble_kernel, dim3(grid), dim3(256), 0, st, reinterpret_cast<const float4*>(tmp),
                     reinterpret_cast<const float4*>(e->wf("encoder.cls_token")),
                     reinterpret_cast<const float4*>(e->wf("encoder.pos_embed")), reinterpret_cast<float4*>(e->x), B, e->Tp,
@@ -803,9 +733,9 @@ int encode_chunk(parseq_engine* e, const void* images_any, bool u8, int B, __nv_
   // With fuse_ln the two residual GEMMs of a block also emit the LayerNorm that consumes their result (norm2 after
   // attn.proj; the next block's norm1 - or the final encoder.norm - after mlp.fc2): the fp32 residual stream is read
   // and written once per GEMM instead of once more per LayerNorm.
-  // The fused kernel owns whole 128-row tiles (one CTA per tile, both column halves in sequence): it pays off once
-  // the tiles fill the machine about twice; below that the N-split GEMM + LayerNorm pair has the lower latency
-  // (bs=1: 1.67 ms vs 1.93 ms p50).  "fuse_ln" bit 2 forces it for any M (tests).
+  // The fused kernel owns whole rows (the columns of a row are not spread over tiles): it is used once the 128-row
+  // tiles fill the machine about twice; below that the N-split GEMM + LayerNorm pair has more CTAs to spread over the
+  // SMs.  "fuse_ln" bit 2 forces it for any M (tests).
   const int Mr = (regime_batch > B ? regime_batch : B) * T;
   const bool big = (Mr + pq::GEMM_BLOCK_M - 1) / pq::GEMM_BLOCK_M >= 2 * e->lo.sm_count || (e->fuse_ln & 4);
   const bool fuse_proj = (e->fuse_ln & 1) && gemm_ln_supported(D) && big;
@@ -867,7 +797,7 @@ int vitstr_tail(parseq_engine* e, int B, int L, float* logits, int* ids_out, cud
   {
     TimedScope ts(e, st, CAT_MISC, 0.0);
     const long long total = 1ll * M * (D / 4);
-    const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, 148ll * 16));
+    const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, 132ll * 16));
     PQ_TRY(launch_k(e->lo, pq::gather_token_rows_kernel, dim3(grid), dim3(256), 0, st, reinterpret_cast<const float4*>(e->x),
                     reinterpret_cast<float4*>(e->vt_rows), B, e->T, 1, L, D / 4));
   }
@@ -911,7 +841,7 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
   if (ex != nullptr && (ex->qmask != nullptr || ex->pmask != nullptr)) {
     if (mode != 2) {                     // masks with the default queries: expand the table rows (tiny) so mode 2 applies
       const int n4 = nq * D / 4;
-      PQ_TRY(launch_k(e->lo, pq::bcast_rows_kernel, dim3(static_cast<unsigned>(std::min((B * n4 + 255) / 256, 148 * 8))), dim3(256), 0, st,
+      PQ_TRY(launch_k(e->lo, pq::bcast_rows_kernel, dim3(static_cast<unsigned>(std::min((B * n4 + 255) / 256, 132 * 8))), dim3(256), 0, st,
                       reinterpret_cast<const float4*>(e->qs + static_cast<long long>(q0) * D), reinterpret_cast<float4*>(sg.qc), n4, B));
       e->launches++;
       qself = sg.qc;
@@ -957,7 +887,7 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
     // PARSeq.decode returns the decoder output: final LayerNorm only (modules.py:123-125)
     PQ_TRY(layernorm(e, sg.y, "decoder.norm", 1e-5f, M, sg.yn, ex->out_norm, st));
   } else if (nq > 1 && ids_dst == nullptr) {
-    // multi-query passes (refine / NAR): LayerNorm kernel + tcgen05 GEMM for the head (weights read once per tile).
+    // multi-query passes (refine / NAR): LayerNorm kernel + wgmma GEMM for the head (weights read once per tile).
     // Chosen by pass type, not by batch size, so that a row's result does not depend on the batch it is computed in.
     PQ_TRY(layernorm(e, sg.y, "decoder.norm", 1e-5f, M, sg.yn, nullptr, st));
     PQ_TRY(gemm(e, sg.yn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, pq::EPI_F32, 1.0f, nullptr, 0, 0,
@@ -1081,9 +1011,9 @@ int ar2_launch(parseq_engine* e, const pq::DecAr2Params& p, int ncl, cudaStream_
   PQ_CUDA(cudaLaunchKernelEx(&cfg, pq::dec_ar2_kernel<D, MT, CS>, e->ar2_maps[CS == 6 ? 1 : 0], p));
   return PARSEQ_OK;
 }
-// Clusters of this instantiation that can be co-resident.  A cluster lives inside one GPC; on the B200s of this pool the
-// occupancy query answers 15 for 8-CTA clusters (measured: 15 clusters run in 1.89 ms, 16 in 3.72 ms = two waves), so
-// 512 images do not fit one wave of 32-row clusters of 8; clusters of 6 pack more SMs (23 x 6 = 138).
+// Clusters of this instantiation that can be co-resident, as the occupancy query answers for this device.  A cluster
+// lives inside one GPC, so clusters of 8 can leave SMs of a GPC idle and clusters of 6 may pack more SMs; a batch that
+// needs more clusters than fit runs in two waves.
 template <int D, int MT, int CS>
 int ar2_max_clusters(parseq_engine* e) {
   int& cache = e->ar2_clusters[MT][CS == 6 ? 1 : 0];
@@ -1396,7 +1326,7 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
 extern "C" {
 
 const char* parseq_last_error(void) { return g_last_error.c_str(); }
-const char* parseq_version(void) { return "parseq_b200 0.1 (sm_100a, tcgen05/TMA)"; }
+const char* parseq_version(void) { return "parseq_b200 0.1 (sm_90a, wgmma/TMA)"; }
 
 int parseq_create(const parseq_config* cfg, parseq_engine** out) {
   if (cfg == nullptr || out == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
@@ -1408,9 +1338,9 @@ int parseq_create(const parseq_config* cfg, parseq_engine** out) {
   PQ_CUDA(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   PQ_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10)
+  if (prop.major != 9 || prop.minor != 0)
     return fail(PARSEQ_ERR_NO_DEVICE, std::string("device is sm_") + std::to_string(prop.major * 10 + prop.minor) +
-                                          ", the kernels are sm_100a (B200) only");
+                                          ", the kernels are sm_90a (H100) only");
   const int sm_count = prop.multiProcessorCount;
   PQ_TRY(init_kernel_attributes());
   PQ_TRY(load_driver_api());
@@ -1456,8 +1386,8 @@ int parseq_create(const parseq_config* cfg, parseq_engine** out) {
   e->C = cfg->num_tokens - 2;
   e->dh_dec = D / cfg->dec_num_heads;
   e->max_batch = cfg->max_batch > 0 ? cfg->max_batch : 512;
-  // One pipeline stage per super-chunk by default: measured on B200 the decoder chain is latency-bound and the
-  // encoder GEMMs occupy every SM, so splitting into stages only shrinks the GEMMs ("chunk" option re-enables it).
+  // One pipeline stage per super-chunk by default: the decoder chain is latency-bound and the encoder GEMMs occupy
+  // every SM, so splitting into stages only shrinks the GEMMs ("chunk" option re-enables it).
   e->chunk = e->max_batch;
   e->dec_chunk = e->max_batch < 128 ? e->max_batch : 128;
   if (e->T > 256) {
@@ -1745,7 +1675,7 @@ int parseq_decode(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t num_
     const int Bc = (batch - b0 < e->dec_chunk) ? (batch - b0) : e->dec_chunk;
     // memory (fp32, caller's) -> bf16 operand -> cross K/V cache rows [0, Bc * T)
     const long long n4 = 1ll * Bc * T * D / 4;
-    pq::f32_to_bf16_kernel<<<static_cast<unsigned>(std::min<long long>((n4 + 255) / 256, 148ll * 8)), 256, 0, st>>>(
+    pq::f32_to_bf16_kernel<<<static_cast<unsigned>(std::min<long long>((n4 + 255) / 256, 132ll * 8)), 256, 0, st>>>(
         reinterpret_cast<const float4*>(memory + 1ll * b0 * T * D), reinterpret_cast<uint2*>(e->mem), n4);
     PQ_CUDA(cudaGetLastError());
     e->cur_cat = CAT_DEC_GEMM;
@@ -1780,7 +1710,7 @@ int parseq_head(parseq_engine* e, int32_t rows, const float* x, float* logits, p
   for (int r0 = 0; r0 < rows; r0 += cap) {
     const int n = (rows - r0 < cap) ? (rows - r0) : cap;
     const long long n4 = 1ll * n * D / 4;
-    pq::f32_to_bf16_kernel<<<static_cast<unsigned>(std::min<long long>((n4 + 255) / 256, 148ll * 8)), 256, 0, e->main>>>(
+    pq::f32_to_bf16_kernel<<<static_cast<unsigned>(std::min<long long>((n4 + 255) / 256, 132ll * 8)), 256, 0, e->main>>>(
         reinterpret_cast<const float4*>(x + 1ll * r0 * D), reinterpret_cast<uint2*>(sg.yn), n4);
     PQ_CUDA(cudaGetLastError());
     e->launches++;
@@ -1800,7 +1730,7 @@ int parseq_text_embed(parseq_engine* e, int32_t n, const int32_t* ids, float* ou
   if (!e->slots[e->index.at("text_embed.embedding.weight")].set) return fail(PARSEQ_ERR_STATE, "weights not set");
   PQ_CUDA(cudaSetDevice(e->cfg.device));
   const long long total = 1ll * n * e->D;
-  pq::text_embed_kernel<<<static_cast<unsigned>(std::min<long long>((total + 255) / 256, 148ll * 8)), 256, 0,
+  pq::text_embed_kernel<<<static_cast<unsigned>(std::min<long long>((total + 255) / 256, 132ll * 8)), 256, 0,
                           reinterpret_cast<cudaStream_t>(stream)>>>(ids, e->wf("text_embed.embedding.weight"), out, n, e->D, e->V,
                                                                     std::sqrt(static_cast<float>(e->D)));
   PQ_CUDA(cudaGetLastError());
@@ -1865,8 +1795,13 @@ int parseq_set_option(parseq_engine* e, const char* name, int64_t value) {
   }
   if (n == "attn_impl") { lo.attn_impl = value != 0 ? 1 : 0; if (e) drop_graphs(e); return PARSEQ_OK; }
   if (n == "pdl") { lo.use_pdl = value != 0; if (e) drop_graphs(e); return PARSEQ_OK; }
-  if (n == "tma_epilogue") { lo.no_tma_epilogue = (value == 0); if (e) drop_graphs(e); return PARSEQ_OK; }
-  if (n == "gemm_stages") { lo.gemm_stages = value > 0 ? static_cast<int>(value) : 0; if (e) drop_graphs(e); return PARSEQ_OK; }
+  if (n == "gemm_stages") {
+    // the MMA warpgroups release a stage once the next k-block's MMAs are queued: a ring needs at least two slots
+    if (value < 0 || value == 1) return fail(PARSEQ_ERR_INVALID_ARG, "gemm_stages: 0 (full ring) or >= 2");
+    lo.gemm_stages = static_cast<int>(value);
+    if (e) drop_graphs(e);
+    return PARSEQ_OK;
+  }
   if (n == "cta_group") {
     if (value < 0 || value > 2) return fail(PARSEQ_ERR_INVALID_ARG, "cta_group: 0 (auto) / 1 / 2");
     lo.cta_group = static_cast<int>(value);
@@ -2000,13 +1935,6 @@ int parseq_mlp_ln_bf16(const void* xn, const void* W1, const float* b1, const vo
                        float* x_inout, const float* gamma, const float* beta, float eps, void* xn_out_bf16, parseq_stream_t stream) {
   return mlp_ln_launch(g_default_opts, xn, W1, b1, W2, b2, M, D, x_inout, gamma, beta, eps, xn_out_bf16,
                        reinterpret_cast<cudaStream_t>(stream));
-}
-// same, with 16 cycle counters of CTA 0 written to `prof_dev` (tests/prof_mlp_ln.py; see mlp_ln.cuh for the slots)
-int parseq_mlp_ln_bf16_prof(const void* xn, const void* W1, const float* b1, const void* W2, const float* b2, int M, int D,
-                            float* x_inout, const float* gamma, const float* beta, float eps, void* xn_out_bf16,
-                            unsigned long long* prof_dev, parseq_stream_t stream) {
-  return mlp_ln_launch(g_default_opts, xn, W1, b1, W2, b2, M, D, x_inout, gamma, beta, eps, xn_out_bf16,
-                       reinterpret_cast<cudaStream_t>(stream), prof_dev);
 }
 int parseq_layernorm_bf16(const float* x, const float* gamma, const float* beta, float eps, int M, int D, void* y_bf16,
                           float* y_f32_or_null, parseq_stream_t stream) {

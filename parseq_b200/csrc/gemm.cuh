@@ -1,12 +1,13 @@
-// Persistent warp-specialised bf16 GEMM on tcgen05 (sm_100a):
+// Persistent warp-specialised bf16 GEMM on wgmma (sm_90a):
 //   out[M,N] = epilogue( A[M,K] * W[N,K]^T + bias )
-// A and W are bf16, K-contiguous ("K-major"); both are fetched by TMA into 128B-swizzled shared-memory
-// stages; one elected thread issues tcgen05.mma (UMMA 128 x BLOCK_N x 16) into a double-buffered fp32
-// accumulator in TMEM; four epilogue warps drain TMEM with tcgen05.ld (one accumulator row per thread)
-// while the next tile's MMAs run.  Every projection of the PARSeq path goes through this kernel:
-// patch-embed (K=96), QKV / proj / fc1 / fc2 of the 12 ViT blocks (reference: timm Attention/Mlp via
-// strhub/models/parseq/modules.py:145-165), the cross-attention K/V projection of the image memory,
-// the decoder's q / out projections, MLP (modules.py:69-77) and the character head (model.py:63).
+// A and W are bf16, K-contiguous ("K-major"); both are fetched by TMA into 128B-swizzled shared-memory stages of an
+// mbarrier ring.  Warpgroup 0 is the producer (one thread issues the TMA loads); warpgroups 1 and 2 each accumulate 64
+// rows of the 128 x BLOCK_N tile in registers with wgmma (m64 x BLOCK_N x k16) and store their rows straight from the
+// accumulator.  A CTA (pair) walks the tiles with a stride of the grid; the ring position carries over, so the producer
+// loads the next tile's operands while the MMA warpgroups run the epilogue of the current one.  Every projection of the PARSeq path goes through this kernel: patch-embed (K=96), QKV / proj / fc1 / fc2
+// of the 12 ViT blocks (reference: timm Attention/Mlp via strhub/models/parseq/modules.py:145-165), the
+// cross-attention K/V projection of the image memory, the decoder's q / out projections, MLP (modules.py:69-77) and
+// the character head (model.py:63).
 #pragma once
 #include <cuda.h>
 #include "ptx.cuh"
@@ -24,418 +25,216 @@ struct GemmParams {
   int mode;
   float alpha;
   const float* bias;   // [N] or nullptr
-  const float* resid;  // fp32 residual (may alias out) or nullptr
+  const float* resid;  // fp32 residual (may alias out: in-place accumulate) or nullptr
   long long ldr;
   int resid_mod;       // >0: residual row = row % resid_mod (broadcast tables: pos_embed, pos_queries)
   void* out;
   long long ldo;       // elements
-  int vec_ok;          // 16B-aligned rows: vector stores allowed
-  int tma_out;         // 0: direct stores (fallback), 1: TMA store fp32, 2: TMA reduce-add fp32 (out += ...),
-                       // 3: TMA store bf16 (mode EPI_BF16 / EPI_GELU_BF16)
-                       // 4: TMA store bf16 into a column-blocked buffer [N/64][rows][64] (3D tensor map)
+  int vec_ok;          // 8-byte aligned column pairs: paired stores allowed
+  long long blocked_rows;  // > 0: bf16 output in a column-blocked buffer [N/64][blocked_rows][64] (ldo unused)
   int num_m_tiles, num_n_tiles;  // in units of (128 * CG) x BLOCK_N
   int max_stages;                // 0: the full operand ring; n > 0: use only n slots (pipeline-depth experiments)
 };
 
-constexpr int GEMM_BLOCK_M = 128;  // rows per CTA (one TMEM lane per row)
+constexpr int GEMM_BLOCK_M = 128;  // rows per CTA (64 per MMA warpgroup)
 constexpr int GEMM_BLOCK_K = 64;   // 64 bf16 = 128 B = one swizzle row
-constexpr int GEMM_EPI_WARPS = 8;   // two warps per TMEM lane quarter (warp % 4), alternating 32/64-column chunks
-constexpr int GEMM_THREADS = 64 + 32 * GEMM_EPI_WARPS;  // warp0: TMA, warp1: MMA + TMEM alloc, warps 2..9: epilogue
+constexpr int GEMM_THREADS = 384;  // warpgroup 0: TMA producer, warpgroups 1, 2: MMA + epilogue
 
 // CG = 1: one CTA computes a 128 x BLOCK_N tile.
-// CG = 2: a CTA pair (cluster of 2, tcgen05 cta_group::2) computes a 256 x BLOCK_N tile: each CTA loads its own
-//         128 rows of A and HALF of the W tile (BLOCK_N/2 rows), the leader issues UMMA M=256; every operand byte
-//         is fetched from L2 and crosses shared memory once per 256 (instead of 128) output rows.
+// CG = 2: a cluster of two CTAs computes a 256 x BLOCK_N tile: each CTA loads its own 128 rows of A and HALF of the W
+//         tile, multicast into both CTAs, so every W byte is fetched from L2 once per 256 (instead of 128) output rows.
 template <int BLOCK_N, int CG>
 struct GemmCfg {
   static constexpr int kBRows = BLOCK_N / CG;                       // W rows loaded by one CTA
   static constexpr int kABytes = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;   // 16 KB
-  static constexpr int kBBytes = kBRows * GEMM_BLOCK_K * 2;
+  static constexpr int kBBytes = BLOCK_N * GEMM_BLOCK_K * 2;        // the whole W tile lands in every CTA
   static constexpr int kStageBytes = kABytes + kBBytes;
-  // Shared memory is what bounds the TMA pipeline depth, so the widest tile trades epilogue buffering for a 4th
-  // operand stage: BLOCK_N = 256 keeps ONE staging slab per epilogue warp (the previous store's smem read is
-  // hidden behind the next chunk's TMEM load + math) and ONE bias slice shared by all epilogue warps.
-  // (a CTA of a pair stages only half of W per k-block: its ring has room for two slabs per warp at every width)
-  static constexpr int kSlabs = (BLOCK_N == 256 && CG == 1) ? 1 : 2;   // staging slabs (32 rows x 128 B) per epilogue warp
-  static constexpr bool kSharedBias = (BLOCK_N == 256);
-  static constexpr int kEpiStageBytes = GEMM_EPI_WARPS * kSlabs * 4096;
-  static constexpr int kBiasBytes = (kSharedBias ? 1 : GEMM_EPI_WARPS) * BLOCK_N * 4;  // bias slice of the current tile
-  static constexpr int kStagesRaw = (232448 - 1024 - 256 - kEpiStageBytes - kBiasBytes) / kStageBytes;
-  static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
-  static constexpr int kTmemCols = (2 * BLOCK_N <= 32) ? 32 : (2 * BLOCK_N <= 64) ? 64 : (2 * BLOCK_N <= 128) ? 128
-                                   : (2 * BLOCK_N <= 256) ? 256 : 512;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kEpiStageBytes + kBiasBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-  static_assert(BLOCK_N % 32 == 0 && BLOCK_N >= 32 && BLOCK_N <= 256, "BLOCK_N");
+  static constexpr int kStagesRaw = (232448 - 1024 - 256) / kStageBytes;
+  static constexpr int kStages = kStagesRaw > 6 ? 6 : kStagesRaw;
+  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(BLOCK_N == 64 || BLOCK_N == 128 || BLOCK_N == 192 || BLOCK_N == 256, "BLOCK_N");
   static_assert(CG == 1 || CG == 2, "CG");
-  static_assert(kBBytes % 1024 == 0, "stage bases must stay 1024-B aligned");
+  static_assert((kBRows * GEMM_BLOCK_K * 2) % 1024 == 0, "multicast halves must stay 1024-B aligned");
   static_assert(kStages >= 3, "pipeline depth");
 };
 
-// named barrier over the 8 epilogue warps only (barrier 0 stays __syncthreads)
-__device__ __forceinline__ void epi_bar_sync() {
-  asm volatile("bar.sync 1, %0;" ::"n"(32 * GEMM_EPI_WARPS) : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------ epilogue bodies
-// One epilogue warp owns 32 accumulator rows (its TMEM lane quarter); the two warps of a quarter alternate chunks.
-// TMA path: TMEM -> registers -> (+bias, activation) -> 128B-swizzled smem slab (32 rows x 128 B) -> TMA store /
-// fp32 reduce-add; out-of-range rows / columns are clipped by the tensor map, nothing is ever loaded from global.
-template <int BLOCK_N, bool REDUCE, int SLABS>
-__device__ __forceinline__ void epi_tma_f32(const GemmParams& p, const CUtensorMap* tmC, uint32_t taddr, uint8_t* my_stage,
-                                            const float* my_bias, int n0, int row0, int half, int lane, int& it) {
-  // `it` counts this warp's TMA stores over the whole kernel: slab (it % SLABS) is free once at most SLABS-1 newer
-  // stores are still reading their source (bulk_wait_group_read<SLABS-1>), so the counter must NOT restart per tile.
-  const uint32_t sw = static_cast<uint32_t>(lane & 7);
-#pragma unroll 1
-  for (int c = half; c < BLOCK_N / 32; c += 2, ++it) {
-    const int col0 = n0 + c * 32;
-    if (col0 >= p.N) break;
-    uint32_t v[32];
-    tmem_ld_32x32b_x32(taddr + static_cast<uint32_t>(c * 32), v);
-    tmem_ld_wait();
-    const float* bb = my_bias + c * 32;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = __float_as_uint((__uint_as_float(v[j]) + bb[j]) * p.alpha);
-    if (lane == 0) bulk_wait_group_read<SLABS - 1>();
-    __syncwarp();
-    uint8_t* slab = my_stage + (it % SLABS) * 4096;
-    uint8_t* buf = slab + lane * 128;
-#pragma unroll
-    for (int jj = 0; jj < 8; ++jj)
-      *reinterpret_cast<uint4*>(buf + ((static_cast<uint32_t>(jj) ^ sw) << 4)) =
-          make_uint4(v[jj * 4 + 0], v[jj * 4 + 1], v[jj * 4 + 2], v[jj * 4 + 3]);
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) {
-      if (REDUCE) tma_reduce_add_2d(tmC, slab, col0, row0);
-      else tma_store_2d(tmC, slab, col0, row0);
-      bulk_commit_group();
+// ------------------------------------------------------------------------------------------------ operand ring
+// full[s]: stage s holds its A and B tiles (TMA transaction bytes).  empty[s]: every MMA warpgroup that reads stage s
+// has finished with it - in both CTAs of a pair when B is multicast (2 warpgroups x CG arrivals).
+//
+// Consumer side of the ring for one warpgroup: accumulates a 64 x N block over num_kb k-blocks.  a_off / b_off: byte
+// offsets of the warpgroup's A rows / B rows inside a stage; stage / phase: the ring position, carried over from tile to
+// tile.  A stage is released once the MMAs of the NEXT k-block are queued (wgmma_wait<1>), so the tensor cores never wait
+// for the release round trip; the last one once the accumulator is complete.  Hence a ring needs at least two stages.
+template <int N, bool PAIR>
+__device__ __forceinline__ void wg_mainloop(float (&acc)[N / 2], uint8_t* smem, int stage_bytes, int a_off, int b_off,
+                                            uint64_t* full_bar, uint64_t* empty_bar, int nstages, int num_kb, int& stage,
+                                            uint32_t& phase) {
+  const bool signal = (threadIdx.x & 127) == 0;
+  int prev = -1;
+  auto release = [&](int s) {
+    if (signal) {
+      mbar_arrive(&empty_bar[s]);
+      if constexpr (PAIR) mbar_arrive_cluster(mapa_cluster(smem_u32(&empty_bar[s]), cluster_ctarank() ^ 1u));
     }
+  };
+#pragma unroll 1
+  for (int kb = 0; kb < num_kb; ++kb) {
+    mbar_wait_mma(&full_bar[stage], phase);
+    const uint32_t base = smem_u32(smem + stage * stage_bytes);
+    const uint64_t da = make_desc_k_sw128(base + a_off);
+    const uint64_t db = make_desc_k_sw128(base + b_off);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < GEMM_BLOCK_K / 16; ++k)
+      wgmma_bf16<N>(acc, da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k),
+                    static_cast<uint32_t>((kb | k) != 0));
+    wgmma_commit();
+    if (prev >= 0) {
+      wgmma_wait<1>();
+      release(prev);
+    }
+    prev = stage;
+    if (++stage == nstages) { stage = 0; phase ^= 1u; }
   }
+  wgmma_wait<0>();
+  wgmma_reg_fence(acc);
+  if (prev >= 0) release(prev);
 }
 
-template <int BLOCK_N, bool GELU, int SLABS>
-__device__ __forceinline__ void epi_tma_bf16(const GemmParams& p, const CUtensorMap* tmC, uint32_t taddr, uint8_t* my_stage,
-                                             const float* my_bias, int n0, int row0, int half, int lane, int& it) {
-  const uint32_t sw = static_cast<uint32_t>(lane & 7);
-#pragma unroll 1
-  for (int c = half; c < BLOCK_N / 64; c += 2, ++it) {   // 64 bf16 columns = 128 B per row per TMA store
-    const int col0 = n0 + c * 64;
-    if (col0 >= p.N) break;
-    uint4 q[8];                          // this lane's 64 output columns, packed (held across the slab wait)
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      uint32_t v[32];
-      tmem_ld_32x32b_x32(taddr + static_cast<uint32_t>(c * 64 + h * 32), v);
-      tmem_ld_wait();
-      const float* bb = my_bias + c * 64 + h * 32;
-#pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        float f[8];
-        if constexpr (GELU) {
-#pragma unroll
-          for (int t = 0; t < 8; t += 2) {                 // two columns per FFMA2 / FADD2 issue slot
-            float a0, a1;
-            f2_unpack(f2_add(f2_pack(__uint_as_float(v[jj * 8 + t]), __uint_as_float(v[jj * 8 + t + 1])),
-                             *reinterpret_cast<const unsigned long long*>(bb + jj * 8 + t)), a0, a1);
-            gelu_erf_x2(a0, a1, f[t], f[t + 1]);
-          }
-        } else {
-#pragma unroll
-          for (int t = 0; t < 8; ++t) f[t] = (__uint_as_float(v[jj * 8 + t]) + bb[jj * 8 + t]) * p.alpha;
-        }
-        q[h * 4 + jj].x = pack_bf16(f[0], f[1]); q[h * 4 + jj].y = pack_bf16(f[2], f[3]);
-        q[h * 4 + jj].z = pack_bf16(f[4], f[5]); q[h * 4 + jj].w = pack_bf16(f[6], f[7]);
-      }
-    }
-    if (lane == 0) bulk_wait_group_read<SLABS - 1>();   // the store that last read this slab is done with it
-    __syncwarp();
-    uint8_t* slab = my_stage + (it % SLABS) * 4096;
-    uint8_t* buf = slab + lane * 128;
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-      *reinterpret_cast<uint4*>(buf + ((static_cast<uint32_t>(j) ^ sw) << 4)) = q[j];
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) {
-      if (p.tma_out == 4) tma_store_3d(tmC, slab, 0, row0, col0 >> 6);
-      else tma_store_2d(tmC, slab, col0, row0);
-      bulk_commit_group();
-    }
+// ------------------------------------------------------------------------------------------------ epilogue
+// Two columns of one accumulator row.  Each quad of lanes covers 8 consecutive columns of a row (32 B fp32, 16 B bf16).
+__device__ __forceinline__ void gemm_store_pair(const GemmParams& p, int row, int col, float v0, float v1, float b0,
+                                                float b1) {
+  const bool two = col + 1 < p.N;
+  float f0, f1;
+  if (p.mode == EPI_GELU_BF16) {
+    f0 = gelu_erf(v0 + b0);
+    f1 = gelu_erf(v1 + b1);
+  } else {
+    f0 = (v0 + b0) * p.alpha;
+    f1 = (v1 + b1) * p.alpha;
   }
-}
-
-// Direct-store fallback (outputs that are not TMA-addressable: odd row pitch of the [B,26,95] logits; residual read
-// from a different / broadcast tensor: + pos_embed, + pos_queries).  One accumulator row per thread.
-template <int BLOCK_N>
-__device__ __forceinline__ void epi_direct(const GemmParams& p, uint32_t taddr, int n0, int row, int half) {
-  const long long rrow = (p.resid_mod > 0) ? (row % p.resid_mod) : row;
-#pragma unroll 1
-  for (int c = half; c < BLOCK_N / 32; c += 2) {
-    const int col0 = n0 + c * 32;
-    if (col0 >= p.N) break;            // warp-uniform
-    uint32_t v[32];
-    tmem_ld_32x32b_x32(taddr + static_cast<uint32_t>(c * 32), v);
-    tmem_ld_wait();
-    if (row < p.M) {
-      const bool full = p.vec_ok && (col0 + 32 <= p.N);
-      float f[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-      if (p.bias != nullptr) {
-        if (col0 + 32 <= p.N) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + j));
-            f[j] += b.x; f[j + 1] += b.y; f[j + 2] += b.z; f[j + 3] += b.w;
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (col0 + j < p.N) f[j] += __ldg(p.bias + col0 + j);
-        }
-      }
-      if (p.mode == EPI_GELU_BF16) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) f[j] = gelu_erf(f[j]);
-      } else if (p.alpha != 1.0f) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) f[j] *= p.alpha;
-      }
-      if (p.mode == EPI_F32) {
-        float* o = reinterpret_cast<float*>(p.out) + static_cast<long long>(row) * p.ldo + col0;
-        const float* r = (p.resid != nullptr) ? (p.resid + rrow * p.ldr + col0) : nullptr;
-        if (full) {
-          if (r != nullptr) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 x = *reinterpret_cast<const float4*>(r + j);
-              f[j] += x.x; f[j + 1] += x.y; f[j + 2] += x.z; f[j + 3] += x.w;
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<float4*>(o + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (col0 + j < p.N) o[j] = f[j] + ((r != nullptr) ? r[j] : 0.0f);
-        }
+  if (p.mode == EPI_F32) {
+    float* o = reinterpret_cast<float*>(p.out) + static_cast<long long>(row) * p.ldo + col;
+    if (p.resid != nullptr) {
+      const long long rrow = (p.resid_mod > 0) ? (row % p.resid_mod) : row;
+      const float* r = p.resid + rrow * p.ldr + col;
+      if (two && p.vec_ok) {
+        const float2 x = *reinterpret_cast<const float2*>(r);
+        f0 += x.x;
+        f1 += x.y;
       } else {
-        __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + static_cast<long long>(row) * p.ldo + col0;
-        if (full) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            uint4 q;
-            q.x = pack_bf16(f[j], f[j + 1]);
-            q.y = pack_bf16(f[j + 2], f[j + 3]);
-            q.z = pack_bf16(f[j + 4], f[j + 5]);
-            q.w = pack_bf16(f[j + 6], f[j + 7]);
-            *reinterpret_cast<uint4*>(o + j) = q;
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (col0 + j < p.N) o[j] = __float2bfloat16_rn(f[j]);
-        }
+        f0 += r[0];
+        if (two) f1 += r[1];
       }
+    }
+    if (two && p.vec_ok) *reinterpret_cast<float2*>(o) = make_float2(f0, f1);
+    else {
+      o[0] = f0;
+      if (two) o[1] = f1;
+    }
+  } else {
+    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) +
+                       (p.blocked_rows > 0 ? blocked_off(p.blocked_rows, row, col) : static_cast<long long>(row) * p.ldo + col);
+    if (two && p.vec_ok) *reinterpret_cast<uint32_t*>(o) = pack_bf16(f0, f1);
+    else {
+      o[0] = __float2bfloat16_rn(f0);
+      if (two) o[1] = __float2bfloat16_rn(f1);
     }
   }
 }
 
 template <int BLOCK_N, int CG>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                         const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   using Cfg = GemmCfg<BLOCK_N, CG>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   const uint32_t pad = ((raw_addr + 1023u) & ~1023u) - raw_addr;
   uint8_t* smem = smem_raw + pad;                         // 1024-B aligned (SWIZZLE_128B requirement)
-  uint8_t* epi_base = smem + Cfg::kStages * Cfg::kStageBytes;        // 1024-B aligned staging tiles for TMA stores
-  float* bias_base = reinterpret_cast<float*>(epi_base + Cfg::kEpiStageBytes);
-  uint8_t* bar_base = epi_base + Cfg::kEpiStageBytes + Cfg::kBiasBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(bar_base);         // [kStages] TMA -> MMA (leader's copy is live)
-  uint64_t* empty_bar = full_bar + Cfg::kStages;                       // [kStages] MMA -> TMA (each CTA its own)
-  uint64_t* tfull_bar = empty_bar + Cfg::kStages;                      // [2] MMA -> epilogue (each CTA its own)
-  uint64_t* tempty_bar = tfull_bar + 2;                                // [2] epilogue -> MMA (leader's copy is live)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  uint64_t* empty_bar = full_bar + Cfg::kStages;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
   const uint32_t rank = (CG == 2) ? cluster_ctarank() : 0u;
-  const int cluster_id = blockIdx.x / CG;
+  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
   const int num_clusters = gridDim.x / CG;
-  const int num_tiles = p.num_m_tiles * p.num_n_tiles;    // tiles of (128*CG) x BLOCK_N
   const int num_kb = (p.K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K;
   const int nstages = (p.max_stages > 0 && p.max_stages < Cfg::kStages) ? p.max_stages : Cfg::kStages;
 
   grid_dep_launch();                       // PDL: the next kernel may start its own prologue
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
-    if (p.tma_out) prefetch_tmap(&tmC);
     for (int s = 0; s < Cfg::kStages; ++s) {
-      mbar_init(&full_bar[s], 1);         // the leader's arrive.expect_tx covers the bytes of BOTH CTAs' loads
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      // leader: its own 8 epilogue warps + ONE forwarded arrival for the peer's 8; peer: collects its 8 warps locally
-      mbar_init(&tempty_bar[s], (CG == 2 && rank == 0) ? GEMM_EPI_WARPS + 1 : GEMM_EPI_WARPS);
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 2 * CG);
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    if constexpr (CG == 2) tmem_alloc_pair<Cfg::kTmemCols>(tmem_slot);
-    else tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  }
-  tc_fence_before();
   if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   grid_dep_wait();                         // PDL: inputs of this GEMM are complete and visible from here on
 
-  if (warp == 0) {
-    // ===================== TMA producer (every CTA loads its own A rows and its share of W) =====================
-    if (lane == 0) {
+  if (threadIdx.x < 128) {
+    // ===================== TMA producer =====================
+    // runs ahead across tiles: the next tile's operands stream in while the MMA warpgroups store this one
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
+      for (int tile = blockIdx.x / CG; tile < num_tiles; tile += num_clusters) {
         const int m0 = (tile / p.num_n_tiles) * (GEMM_BLOCK_M * CG) + static_cast<int>(rank) * GEMM_BLOCK_M;
-        const int n0 = (tile % p.num_n_tiles) * BLOCK_N + static_cast<int>(rank) * Cfg::kBRows;
+        const int n0 = (tile % p.num_n_tiles) * BLOCK_N;
         for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
+          mbar_wait_mma(&empty_bar[stage], phase ^ 1u);
           uint8_t* sa = smem + stage * Cfg::kStageBytes;
           uint8_t* sb = sa + Cfg::kABytes;
+          mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+          tma_load_2d(sa, &tmA, &full_bar[stage], kb * GEMM_BLOCK_K, m0);
           if constexpr (CG == 1) {
-            mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-            tma_load_2d(sa, &tmA, &full_bar[stage], kb * GEMM_BLOCK_K, m0);
             tma_load_2d(sb, &tmB, &full_bar[stage], kb * GEMM_BLOCK_K, n0);
           } else {
-            // Both CTAs' loads complete on the LEADER's barrier; only the leader arrives (expecting the bytes of both).
-            // The peer must not arrive remotely per stage: `mbarrier.arrive.release.cluster` on a remote barrier costs
-            // the producer thread a cluster-scope release (~700 cycles) per k-block and paced the whole pair at half
-            // speed (ncu: same tensor-busy cycles, twice the wall time - profiles/r2_ncu_cta_pair_gemm.txt).  The peer
-            // only refills a stage after the leader's multicast commit, i.e. after the previous phase of the leader's
-            // barrier has completed, so its complete_tx can never land in the wrong phase.
-            const uint32_t leader_full = mapa_cluster(smem_u32(&full_bar[stage]), 0u);
-            if (rank == 0) mbar_expect_tx(&full_bar[stage], 2u * Cfg::kStageBytes);
-            tma_load_2d_pair(sa, &tmA, leader_full, kb * GEMM_BLOCK_K, m0);
-            tma_load_2d_pair(sb, &tmB, leader_full, kb * GEMM_BLOCK_K, n0);
+            const int r = static_cast<int>(rank);
+            tma_load_2d_mcast(sb + r * Cfg::kBRows * GEMM_BLOCK_K * 2, &tmB, &full_bar[stage], kb * GEMM_BLOCK_K,
+                              n0 + r * Cfg::kBRows, 0x3);
           }
           if (++stage == nstages) { stage = 0; phase ^= 1u; }
         }
       }
     }
-  } else if (warp == 1) {
-    if (CG == 2 && rank != 0) {
-      // ===================== peer CTA: forward "accumulator stage drained" to the leader =====================
-      // The peer's epilogue warps arrive on their LOCAL barrier; this idle warp turns each completed phase into one
-      // remote arrival on the leader's barrier, so that no epilogue warp pays a cluster-scope release per tile.
-      if (lane == 0) {
-        int as = 0;
-        uint32_t aphase = 0;
-        for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-          mbar_wait(&tempty_bar[as], aphase);
-          mbar_arrive_cluster(mapa_cluster(smem_u32(&tempty_bar[as]), 0u));
-          if (++as == 2) { as = 0; aphase ^= 1u; }
-        }
-      }
-    }
-    // ===================== MMA issuer (single thread of the leader CTA) =====================
-    if (lane == 0 && rank == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(GEMM_BLOCK_M * CG, BLOCK_N);
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-        mbar_wait(&tempty_bar[as], aphase ^ 1u);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(as * BLOCK_N);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-          const uint64_t adesc = make_desc_k_sw128(sa);
-          const uint64_t bdesc = make_desc_k_sw128(sa + Cfg::kABytes);
-#pragma unroll
-          for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) {
-            // advance 16 bf16 = 32 B along K inside the swizzle row: +2 in the (addr>>4) field
-            const uint32_t acc = static_cast<uint32_t>((kb | k) != 0);
-            if constexpr (CG == 2)
-              umma_bf16_pair(tmem_d, adesc + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k), idesc, acc);
-            else
-              umma_bf16(tmem_d, adesc + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k), idesc, acc);
-          }
-          // smem slot reusable (in every CTA of the group) once these MMAs have read it
-          if constexpr (CG == 2) umma_commit_pair(&empty_bar[stage], 0x3); else umma_commit(&empty_bar[stage]);
-          if (++stage == nstages) { stage = 0; phase ^= 1u; }
-        }
-        // accumulator complete (signalled to the epilogue warps of every CTA of the group)
-        if constexpr (CG == 2) umma_commit_pair(&tfull_bar[as], 0x3); else umma_commit(&tfull_bar[as]);
-        if (++as == 2) { as = 0; aphase ^= 1u; }
-      }
-    }
+    __syncwarp();
   } else {
-    // ===================== epilogue warps (8: two per TMEM lane quarter) =====================
-    const int quarter = warp & 3;          // TMEM lane quarter this warp may access
-    const int ew = warp - 2;               // 0..7
-    const int half = ew >> 2;              // which of the alternating column chunks this warp takes
-    const int row_in_tile = quarter * 32 + lane;
-    uint8_t* my_stage = epi_base + ew * (Cfg::kSlabs * 4096);
-    float* my_bias = Cfg::kSharedBias ? bias_base : bias_base + ew * BLOCK_N;
-    int as = 0;
-    uint32_t aphase = 0;
-    int store_it = 0;                      // running count of this warp's TMA stores (staging slab parity)
-    for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
+    // ===================== MMA warpgroups: rows [64 wg, 64 wg + 64) of the tile =====================
+    const int wg = (threadIdx.x >> 7) - 1;
+    int stage = 0;
+    uint32_t phase = 0;
+#pragma unroll 1
+    for (int tile = blockIdx.x / CG; tile < num_tiles; tile += num_clusters) {
       const int m0 = (tile / p.num_n_tiles) * (GEMM_BLOCK_M * CG) + static_cast<int>(rank) * GEMM_BLOCK_M;
       const int n0 = (tile % p.num_n_tiles) * BLOCK_N;
-      if (p.tma_out != 0) {                // bias slice of this tile -> smem (before the accumulator wait)
-        if constexpr (Cfg::kSharedBias) {  // one copy for the 8 epilogue warps, one element per thread
-          static_assert(!Cfg::kSharedBias || BLOCK_N == 32 * GEMM_EPI_WARPS, "one bias element per epilogue thread");
-          epi_bar_sync();                  // every warp is done reading the previous tile's slice
-          const int j = ew * 32 + lane;
-          bias_base[j] = (p.bias != nullptr && n0 + j < p.N) ? __ldg(p.bias + n0 + j) : 0.0f;
-          epi_bar_sync();
-        } else {
-          __syncwarp();
-          for (int j = lane; j < BLOCK_N; j += 32)
-            my_bias[j] = (p.bias != nullptr && n0 + j < p.N) ? __ldg(p.bias + n0 + j) : 0.0f;
-          __syncwarp();
+      float acc[BLOCK_N / 2];
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.0f;
+      wg_mainloop<BLOCK_N, CG == 2>(acc, smem, Cfg::kStageBytes, wg * (64 * GEMM_BLOCK_K * 2), Cfg::kABytes, full_bar,
+                                    empty_bar, nstages, num_kb, stage, phase);
+      const int t = threadIdx.x & 127;
+      const int lane = t & 31;
+      const int row_a = m0 + wg * 64 + (t >> 5) * 16 + (lane >> 2);
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 8; ++i) {
+        const int col = n0 + i * 8 + 2 * (lane & 3);
+        if (col >= p.N) continue;
+        float b0 = 0.0f, b1 = 0.0f;
+        if (p.bias != nullptr) {
+          b0 = __ldg(p.bias + col);
+          if (col + 1 < p.N) b1 = __ldg(p.bias + col + 1);
         }
+        if (row_a < p.M) gemm_store_pair(p, row_a, col, acc[4 * i], acc[4 * i + 1], b0, b1);
+        if (row_a + 8 < p.M) gemm_store_pair(p, row_a + 8, col, acc[4 * i + 2], acc[4 * i + 3], b0, b1);
       }
-      mbar_wait(&tfull_bar[as], aphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) +
-                             static_cast<uint32_t>(as * BLOCK_N);
-      const int row0 = m0 + quarter * 32;
-      if (p.tma_out == 2) epi_tma_f32<BLOCK_N, true, Cfg::kSlabs>(p, &tmC, taddr, my_stage, my_bias, n0, row0, half, lane, store_it);
-      else if (p.tma_out == 1) epi_tma_f32<BLOCK_N, false, Cfg::kSlabs>(p, &tmC, taddr, my_stage, my_bias, n0, row0, half, lane, store_it);
-      else if (p.tma_out >= 3) {
-        if (p.mode == EPI_GELU_BF16) epi_tma_bf16<BLOCK_N, true, Cfg::kSlabs>(p, &tmC, taddr, my_stage, my_bias, n0, row0, half, lane, store_it);
-        else epi_tma_bf16<BLOCK_N, false, Cfg::kSlabs>(p, &tmC, taddr, my_stage, my_bias, n0, row0, half, lane, store_it);
-      } else {
-        epi_direct<BLOCK_N>(p, taddr, n0, m0 + row_in_tile, half);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {                     // 8*CG warp arrivals free this accumulator stage (leader's barrier)
-        mbar_arrive(&tempty_bar[as]);      // local (the peer's arrivals are forwarded by its otherwise idle warp 1)
-      }
-      if (++as == 2) { as = 0; aphase ^= 1u; }
     }
-    if (p.tma_out != 0 && lane == 0) bulk_wait_group<0>();   // all TMA stores of this warp have completed
   }
-
-  tc_fence_before();
-  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();   // peer smem / barriers stay valid until all are done
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (CG == 2) tmem_dealloc_pair<Cfg::kTmemCols>(tmem_base);
-    else tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-  }
+  // a CTA of a pair must not exit while its peer may still multicast into it or arrive on its barriers
+  if constexpr (CG == 2) cluster_sync_all();
 }
 
 }  // namespace pq

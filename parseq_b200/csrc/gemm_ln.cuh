@@ -1,30 +1,25 @@
-// Residual GEMM fused with the LayerNorm that follows it (sm_100a, tcgen05 + TMA).
+// Residual GEMM fused with the LayerNorm that follows it (sm_90a, wgmma + TMA).
 //
 //   x[M, D]  (fp32, in place)  <-  x + A[M, K] * W[D, K]^T + bias            (timm Block: x = x + attn(..) / mlp(..))
 //   xn[M, D] (bf16)            <-  LayerNorm(x_new; gamma, beta, eps)         (norm2 / next block's norm1 / final norm)
 //
 // Why: as separate kernels the attention-projection and fc2 GEMMs are bound by the fp32 read-modify-write of the
-// residual stream and the LayerNorm re-reads it from HBM; here each updated row is normalised while it is still on
-// the SM (profiles/: proj 47 us + LN 31 us, fc2 92 us + LN 31 us at M = 65536 before the fusion).
+// residual stream and the LayerNorm re-reads it from HBM; here each updated row is normalised while it is still in
+// registers.
 //
-// One CTA owns 128 full rows (N = D) so the row statistics never leave the thread that owns the row:
-//   warp 0      TMA producer (A tile 128x64 + a HALF of W: D/2 x 64 per stage; the two column halves of a tile are
-//               accumulated one after the other so that a stage stays 40 KB and shared memory is left for the epilogue)
-//   warp 1      MMA issuer (UMMA 128 x D/2 x 16 into TMEM columns [h*D/2, (h+1)*D/2)), TMEM alloc / dealloc
-//   warps 2..9  epilogue, two per TMEM lane quarter, thread = row, the two warps of a quarter take alternate chunks:
-//       pass 1 (32-column chunks): x tile chunk arrives by TMA in a 128B-swizzled slab (3 slabs per warp are kept in
-//               flight), v = (acc + bias) + x is written back in place and stored with TMA, written back to TMEM, and
-//               accumulated into the row's shifted sum / sum of squares; pass 1 of half 0 overlaps the MMAs of half 1;
-//       the two partial (mean, M2) of a row are combined through shared memory (Chan's parallel variance);
-//       pass 2 (64-column chunks): v is read back from TMEM, normalised, packed to bf16 and TMA-stored to xn.
-// Rounding points are those of the unfused pair (TMA reduce-add epilogue + layernorm_kernel): fp32 x, bf16 xn.
+// A CTA owns 64 rows.  Warpgroup 0 is the TMA producer; warpgroups 1 and 2 each accumulate half of the CTA's columns
+// for all 64 rows (wgmma m64 x N x k16), so a row's values sit in two warpgroups (and, for MODE 2, two CTAs):
+//   pass 1: v = (acc + bias) + x is stored back to x and kept in the accumulator registers; row sums are reduced over
+//           the quad of lanes that holds a row, then over the column parts through shared memory;
+//   pass 2: the same for the squared deviations from the mean (two-pass variance, as layernorm_kernel);
+//   pass 3: normalise, pack to bf16, store xn.
+// Rounding points are those of the unfused pair (residual-accumulate GEMM epilogue + layernorm_kernel): fp32 x, bf16 xn.
 //
-// CG = 2 (CTA pair, tcgen05 cta_group::2): the pair computes 256 rows; each CTA still owns 128 FULL rows (same epilogue,
-// statistics stay local) but stages only HALF of each W column half (D/4 rows of W per stage; UMMA 256 x D/2 x 16 reads B
-// from both CTAs), so a stage is 28 KB instead of 40 KB and the operand bytes per 128 rows drop by 30 % - the main loop of
-// the K = 1536 launch (fc2) is operand-ingest bound.  Same k order per output element: results are bit-identical to CG = 1.
-// Pair plumbing as in gemm.cuh: loads of both CTAs complete on the leader's barrier, multicast commits, the peer's idle
-// warp 1 forwards one "TMEM half drained" arrival per tile and half.
+// MODE 0: one CTA per 64-row tile, all D columns.
+// MODE 1: a cluster of two CTAs on 128 rows; each CTA loads half of the W tile and multicasts it into both, so every W
+//         byte is fetched once per 128 rows.  Same work per row as MODE 0: bit-identical results.
+// MODE 2: a cluster of two CTAs on 64 rows, each CTA computing half of the columns (half of W per CTA, a ring twice as
+//         deep); the row statistics of the four column parts are exchanged through distributed shared memory.
 #pragma once
 #include "gemm.cuh"
 
@@ -36,326 +31,217 @@ struct GemmLnParams {
   const float* gamma;    // [D]
   const float* beta;     // [D]
   float eps;
-  int num_m_tiles;
+  int num_m_tiles;       // clusters (MODE 1 / 2) or CTAs (MODE 0)
 };
 
-constexpr int GLN_EPI_WARPS = 8;
-constexpr int GLN_THREADS = 64 + 32 * GLN_EPI_WARPS;
-constexpr int GLN_SLABS = 3;          // x chunks in flight per epilogue warp
+constexpr int GLN_THREADS = 384;
+constexpr int GLN_BLOCK_M = 64;
 
-template <int D, int CG = 1>
+template <int D, int MODE>
 struct GemmLnCfg {
-  static_assert(CG == 1 || CG == 2, "CG");
-  static constexpr int kNH = D / 2;                                   // columns accumulated per pass over K
-  static constexpr int kBRows = kNH / CG;                             // W rows this CTA stages per k-block
-  static constexpr int kABytes = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;     // 16 KB
-  static constexpr int kBBytes = kBRows * GEMM_BLOCK_K * 2;
+  static_assert(MODE >= 0 && MODE <= 2, "MODE");
+  static constexpr int kCG = MODE == 0 ? 1 : 2;                       // CTAs per cluster
+  static constexpr int kCols = MODE == 2 ? D / 2 : D;                 // columns per CTA
+  static constexpr int kNW = kCols / 2;                               // columns per MMA warpgroup
+  static constexpr int kParts = MODE == 2 ? 4 : 2;                    // column parts of a row
+  static constexpr int kLoadRows = MODE == 1 ? D / 2 : kCols;         // W rows this CTA loads per k-block
+  static constexpr int kBox = kLoadRows > 256 ? kLoadRows / 2 : kLoadRows;   // TMA box rows (at most 256)
+  static constexpr int kABytes = GLN_BLOCK_M * GEMM_BLOCK_K * 2;      // 8 KB
+  static constexpr int kBBytes = kCols * GEMM_BLOCK_K * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kSlabBytes = GLN_EPI_WARPS * GLN_SLABS * 4096;
-  static constexpr int kParamBytes = 3 * D * 4 + 4 * 2 * 32 * 8;      // bias, gamma, beta; (mean, M2) exchange of the warp pairs
-  static constexpr int kBarBytes = 512;
-  static constexpr int kStagesRaw = (232448 - 1024 - kBarBytes - kSlabBytes - kParamBytes) / kStageBytes;
+  static constexpr int kParamBytes = 3 * kCols * 4 + 2 * kParts * GLN_BLOCK_M * 4;   // bias, gamma, beta; row partials
+  static constexpr int kBarBytes = 256;
+  static constexpr int kStagesRaw = (232448 - 1024 - kBarBytes - kParamBytes) / kStageBytes;
   static constexpr int kStages = kStagesRaw > 6 ? 6 : kStagesRaw;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kSlabBytes + kParamBytes + kBarBytes + 1024;
-  static constexpr int kChunks = D / 32;                              // pass-1 chunks per row
-  static_assert(D == 192 || D == 384, "full rows must fit 512 TMEM columns and the UMMA N range");
-  static_assert(kNH % 16 == 0 && kNH <= 256, "UMMA N");
-  static_assert(kBBytes % 1024 == 0 && kStageBytes % 1024 == 0, "1024-B aligned operand tiles");
+  static constexpr int kSmemBytes = kStages * kStageBytes + kParamBytes + kBarBytes + 1024;
+  static_assert(D == 192 || D == 384, "embed_dim");
+  static_assert(kNW % 16 == 0 && kNW <= 256, "wgmma N");
+  static_assert((kNW * GEMM_BLOCK_K * 2) % 1024 == 0 && (kBox * GEMM_BLOCK_K * 2) % 1024 == 0, "1024-B aligned operand tiles");
   static_assert(kStages >= 3, "pipeline depth");
-  static constexpr int kMyChunks = kChunks / 2;                       // pass-1 chunks per epilogue warp
-  static constexpr int kRounds = kMyChunks / GLN_SLABS;               // phases every slab barrier completes per tile
-  static_assert(kMyChunks % GLN_SLABS == 0, "whole rounds of slabs per tile");
 };
 
-template <int D, int CG = 1>
+// Sum of one row's column parts, in a fixed order (every thread of every CTA that holds the row gets the same bits).
+template <int PARTS>
+__device__ __forceinline__ float gln_row_total(const float* s_part, int r) {
+  float t = s_part[r] + s_part[GLN_BLOCK_M + r];
+  if constexpr (PARTS == 4) t += s_part[2 * GLN_BLOCK_M + r] + s_part[3 * GLN_BLOCK_M + r];
+  return t;
+}
+
+// Epilogue shared by the fused kernels (this file, mlp_ln.cuh): `acc` holds the 64 x NW block of one MMA warpgroup
+// (rows m0.., columns c0 + wg * NW..); x += acc + bias in place, then xn = bf16(LayerNorm(x)) over the D columns of a row,
+// whose PARTS column parts are combined through s_part (and, for SPLIT, through the peer CTA's s_part: stat_bar).
+template <int D, int NW, int PARTS, bool SPLIT>
+__device__ __forceinline__ void gln_epilogue(float (&acc)[NW / 2], float* __restrict__ x, __nv_bfloat16* __restrict__ xn, int M,
+                                             float eps, int m0, int c0, int wg, uint32_t rank, const float* s_bias,
+                                             const float* s_gamma, const float* s_beta, float* s_part, uint64_t* stat_bar) {
+  constexpr int kNW = NW;
+  const int t = threadIdx.x & 127;
+  const int lane = t & 31;
+  const int lr = (t >> 5) * 16 + (lane >> 2);        // local rows lr, lr + 8
+  const bool ok_a = m0 + lr < M, ok_b = m0 + lr + 8 < M;
+  float* xa = x + static_cast<long long>(m0 + lr) * D + c0 + wg * kNW + 2 * (lane & 3);
+  float* xb = xa + 8ll * D;
+  const int part = (SPLIT ? static_cast<int>(rank) * 2 : 0) + wg;
+  const uint32_t peer = rank ^ 1u;
+
+  // pass 1: residual update, row sums
+  float sa = 0.f, sb = 0.f;
+#pragma unroll
+  for (int i = 0; i < kNW / 8; ++i) {
+    const int cl = wg * kNW + i * 8 + 2 * (lane & 3);   // column inside this CTA's part
+    const float b0 = s_bias[cl], b1 = s_bias[cl + 1];
+    float2 xo = ok_a ? *reinterpret_cast<const float2*>(xa + i * 8) : make_float2(0.f, 0.f);
+    acc[4 * i] = (acc[4 * i] + b0) + xo.x;
+    acc[4 * i + 1] = (acc[4 * i + 1] + b1) + xo.y;
+    if (ok_a) *reinterpret_cast<float2*>(xa + i * 8) = make_float2(acc[4 * i], acc[4 * i + 1]);
+    xo = ok_b ? *reinterpret_cast<const float2*>(xb + i * 8) : make_float2(0.f, 0.f);
+    acc[4 * i + 2] = (acc[4 * i + 2] + b0) + xo.x;
+    acc[4 * i + 3] = (acc[4 * i + 3] + b1) + xo.y;
+    if (ok_b) *reinterpret_cast<float2*>(xb + i * 8) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+    sa += acc[4 * i] + acc[4 * i + 1];
+    sb += acc[4 * i + 2] + acc[4 * i + 3];
+  }
+  float mean_a = 0.f, mean_b = 0.f, rstd_a = 0.f, rstd_b = 0.f;
+#pragma unroll
+  for (int round = 0; round < 2; ++round) {
+    if (round == 1) {                                // pass 2: squared deviations from the mean
+      sa = 0.f;
+      sb = 0.f;
+#pragma unroll
+      for (int i = 0; i < kNW / 8; ++i) {
+        const float a0 = acc[4 * i] - mean_a, a1 = acc[4 * i + 1] - mean_a;
+        const float d0 = acc[4 * i + 2] - mean_b, d1 = acc[4 * i + 3] - mean_b;
+        sa += a0 * a0 + a1 * a1;
+        sb += d0 * d0 + d1 * d1;
+      }
+    }
+    sa += __shfl_xor_sync(0xffffffffu, sa, 1);
+    sa += __shfl_xor_sync(0xffffffffu, sa, 2);
+    sb += __shfl_xor_sync(0xffffffffu, sb, 1);
+    sb += __shfl_xor_sync(0xffffffffu, sb, 2);
+    float* slot = s_part + (round * PARTS + part) * GLN_BLOCK_M;
+    if ((lane & 3) == 0) {
+      slot[lr] = sa;
+      slot[lr + 8] = sb;
+      if constexpr (SPLIT) {
+        st_cluster_f32(mapa_cluster(smem_u32(slot + lr), peer), sa);
+        st_cluster_f32(mapa_cluster(smem_u32(slot + lr + 8), peer), sb);
+      }
+    }
+    if constexpr (SPLIT) {
+      mbar_arrive(&stat_bar[round]);
+      mbar_arrive_cluster(mapa_cluster(smem_u32(&stat_bar[round]), peer));
+      mbar_wait_cluster(&stat_bar[round], 0);
+    } else {
+      asm volatile("bar.sync 1, 256;" ::: "memory");   // the two MMA warpgroups
+    }
+    const float* tot = s_part + round * PARTS * GLN_BLOCK_M;
+    const float ta = gln_row_total<PARTS>(tot, lr), tb = gln_row_total<PARTS>(tot, lr + 8);
+    if (round == 0) {
+      mean_a = ta * (1.0f / D);
+      mean_b = tb * (1.0f / D);
+    } else {
+      rstd_a = 1.0f / sqrtf(ta * (1.0f / D) + eps);
+      rstd_b = 1.0f / sqrtf(tb * (1.0f / D) + eps);
+    }
+  }
+  // pass 3: normalise, bf16
+  uint32_t* na = reinterpret_cast<uint32_t*>(xn + static_cast<long long>(m0 + lr) * D + c0 + wg * kNW + 2 * (lane & 3));
+  uint32_t* nb = na + 4ll * D;
+#pragma unroll
+  for (int i = 0; i < kNW / 8; ++i) {
+    const int cl = wg * kNW + i * 8 + 2 * (lane & 3);
+    const float g0 = s_gamma[cl], g1 = s_gamma[cl + 1], e0 = s_beta[cl], e1 = s_beta[cl + 1];
+    if (ok_a) na[i * 4] = pack_bf16((acc[4 * i] - mean_a) * rstd_a * g0 + e0, (acc[4 * i + 1] - mean_a) * rstd_a * g1 + e1);
+    if (ok_b) nb[i * 4] = pack_bf16((acc[4 * i + 2] - mean_b) * rstd_b * g0 + e0, (acc[4 * i + 3] - mean_b) * rstd_b * g1 + e1);
+  }
+}
+
+template <int D, int MODE>
 __global__ void __launch_bounds__(GLN_THREADS, 1)
 gemm_ln_fused_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                     const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmN,
-                     const GemmLnParams p) {
-  using Cfg = GemmLnCfg<D, CG>;
+                     float* __restrict__ x, __nv_bfloat16* __restrict__ xn, const GemmLnParams p) {
+  using Cfg = GemmLnCfg<D, MODE>;
+  constexpr int kNW = Cfg::kNW;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   const uint32_t pad = ((raw_addr + 1023u) & ~1023u) - raw_addr;
   uint8_t* smem = smem_raw + pad;
-  uint8_t* slab_base = smem + Cfg::kStages * Cfg::kStageBytes;                 // 1024-B aligned
-  float* s_bias = reinterpret_cast<float*>(slab_base + Cfg::kSlabBytes);
-  float* s_gamma = s_bias + D;
-  float* s_beta = s_gamma + D;
-  float2* s_stat = reinterpret_cast<float2*>(s_beta + D);             // [4 quarters][2 warps][32 rows] (mean, M2)
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(slab_base + Cfg::kSlabBytes + Cfg::kParamBytes);
+  float* s_bias = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  float* s_gamma = s_bias + Cfg::kCols;
+  float* s_beta = s_gamma + Cfg::kCols;
+  float* s_part = s_beta + Cfg::kCols;                 // [2 rounds][kParts][64 rows]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(s_bias) + Cfg::kParamBytes);
   uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* tfull_bar = empty_bar + Cfg::kStages;      // [2]: accumulator half h complete
-  uint64_t* tempty_bar = tfull_bar + 2;                // [2]: the epilogue is done with TMEM column half h of this tile
-  uint64_t* x_bar = tempty_bar + 2;                    // [GLN_EPI_WARPS][GLN_SLABS]: x chunk landed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(x_bar + GLN_EPI_WARPS * GLN_SLABS);
+  uint64_t* stat_bar = empty_bar + Cfg::kStages;       // [2 rounds] (MODE 2): the partials of both CTAs have landed
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const uint32_t rank = (MODE != 0) ? cluster_ctarank() : 0u;
+  const int cluster = blockIdx.x / Cfg::kCG;
+  const int m0 = (MODE == 1) ? cluster * 2 * GLN_BLOCK_M + static_cast<int>(rank) * GLN_BLOCK_M : cluster * GLN_BLOCK_M;
+  const int c0 = (MODE == 2) ? static_cast<int>(rank) * Cfg::kCols : 0;   // first column of this CTA
   const int num_kb = (p.K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K;
-  const uint32_t rank = (CG == 2) ? cluster_ctarank() : 0u;
-  const int first_tile = blockIdx.x / CG;                // tiles of 128 * CG rows
-  const int tile_step = gridDim.x / CG;
-  constexpr int kTileRows = GEMM_BLOCK_M * CG;
-  const int row_off = static_cast<int>(rank) * GEMM_BLOCK_M;
 
   grid_dep_launch();
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmA); prefetch_tmap(&tmB); prefetch_tmap(&tmX); prefetch_tmap(&tmN);
-    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(&tfull_bar[0], 1);
-    mbar_init(&tfull_bar[1], 1);
-    // pair leader: its own 8 epilogue warps + one forwarded arrival for the peer's 8
-    mbar_init(&tempty_bar[0], (CG == 2 && rank == 0) ? GLN_EPI_WARPS + 1 : GLN_EPI_WARPS);
-    mbar_init(&tempty_bar[1], (CG == 2 && rank == 0) ? GLN_EPI_WARPS + 1 : GLN_EPI_WARPS);
-    for (int i = 0; i < GLN_EPI_WARPS * GLN_SLABS; ++i) mbar_init(&x_bar[i], 1);
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmA);
+    prefetch_tmap(&tmB);
+    for (int s = 0; s < Cfg::kStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], MODE == 1 ? 4 : 2);
+    }
+    mbar_init(&stat_bar[0], 2 * 256);                  // every MMA thread of both CTAs
+    mbar_init(&stat_bar[1], 2 * 256);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    if constexpr (CG == 2) tmem_alloc_pair<512>(tmem_slot);
-    else tmem_alloc<512>(tmem_slot);
-  }
   // bias / gamma / beta are weights (never written by a preceding kernel): stage them before the dependency wait
-  for (int j = threadIdx.x; j < D; j += GLN_THREADS) {
-    s_bias[j] = (p.bias != nullptr) ? __ldg(p.bias + j) : 0.0f;
-    s_gamma[j] = __ldg(p.gamma + j);
-    s_beta[j] = __ldg(p.beta + j);
+  for (int j = threadIdx.x; j < Cfg::kCols; j += GLN_THREADS) {
+    s_bias[j] = (p.bias != nullptr) ? __ldg(p.bias + c0 + j) : 0.0f;
+    s_gamma[j] = __ldg(p.gamma + c0 + j);
+    s_beta[j] = __ldg(p.beta + c0 + j);
   }
-  tc_fence_before();
-  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if constexpr (MODE != 0) cluster_sync_all(); else __syncthreads();
   grid_dep_wait();
 
-  if (warp == 0) {
+  if (threadIdx.x < 128) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = first_tile; tile < p.num_m_tiles; tile += tile_step) {
-        const int m0 = tile * kTileRows + row_off;
-        for (int h = 0; h < 2; ++h) {
-          const int n0 = h * Cfg::kNH + static_cast<int>(rank) * Cfg::kBRows;
-          for (int kb = 0; kb < num_kb; ++kb) {
-            mbar_wait(&empty_bar[stage], phase ^ 1u);
-            uint8_t* sa = smem + stage * Cfg::kStageBytes;
-            if constexpr (CG == 1) {
-              mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-              tma_load_2d(sa, &tmA, &full_bar[stage], kb * GEMM_BLOCK_K, m0);
-              tma_load_2d(sa + Cfg::kABytes, &tmB, &full_bar[stage], kb * GEMM_BLOCK_K, n0);
-            } else {
-              // both CTAs' loads complete on the leader's barrier; only the leader arrives (gemm.cuh explains why)
-              const uint32_t leader_full = mapa_cluster(smem_u32(&full_bar[stage]), 0u);
-              if (rank == 0) mbar_expect_tx(&full_bar[stage], 2u * Cfg::kStageBytes);
-              tma_load_2d_pair(sa, &tmA, leader_full, kb * GEMM_BLOCK_K, m0);
-              tma_load_2d_pair(sa + Cfg::kABytes, &tmB, leader_full, kb * GEMM_BLOCK_K, n0);
-            }
-            if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (CG == 2 && rank != 0) {
-      // peer CTA: turn each completed local "TMEM half drained" phase into ONE remote arrival on the leader's barrier
-      if (lane == 0) {
-        uint32_t tphase = 0;
-        for (int tile = first_tile; tile < p.num_m_tiles; tile += tile_step) {
-          for (int h = 0; h < 2; ++h) {
-            mbar_wait(&tempty_bar[h], tphase);
-            mbar_arrive_cluster(mapa_cluster(smem_u32(&tempty_bar[h]), 0u));
-          }
-          tphase ^= 1u;
-        }
-      }
-    }
-    // ===================== MMA issuer (the leader CTA's) =====================
-    if (lane == 0 && rank == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(kTileRows, Cfg::kNH);
-      int stage = 0;
-      uint32_t phase = 0, tphase = 0;
-      for (int tile = first_tile; tile < p.num_m_tiles; tile += tile_step) {
-        for (int h = 0; h < 2; ++h) {
-          // the previous tile's rows have left this half of TMEM (pass 2 releases the low columns first, so the
-          // MMAs of half 0 overlap the rest of the previous tile's pass 2)
-          mbar_wait(&tempty_bar[h], tphase ^ 1u);
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(h * Cfg::kNH);
-          for (int kb = 0; kb < num_kb; ++kb) {
-            mbar_wait(&full_bar[stage], phase);
-            tc_fence_after();
-            const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-            const uint64_t adesc = make_desc_k_sw128(sa);
-            const uint64_t bdesc = make_desc_k_sw128(sa + Cfg::kABytes);
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait_mma(&empty_bar[stage], phase ^ 1u);
+        uint8_t* sa = smem + stage * Cfg::kStageBytes;
+        uint8_t* sb = sa + Cfg::kABytes;
+        mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+        tma_load_2d(sa, &tmA, &full_bar[stage], kb * GEMM_BLOCK_K, m0);
+        if constexpr (MODE == 1) {
+          const int r = static_cast<int>(rank);
+          tma_load_2d_mcast(sb + r * Cfg::kLoadRows * GEMM_BLOCK_K * 2, &tmB, &full_bar[stage], kb * GEMM_BLOCK_K,
+                            r * Cfg::kLoadRows, 0x3);
+        } else {
 #pragma unroll
-            for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) {
-              const uint32_t acc = static_cast<uint32_t>((kb | k) != 0);
-              if constexpr (CG == 2)
-                umma_bf16_pair(tmem_d, adesc + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k), idesc, acc);
-              else
-                umma_bf16(tmem_d, adesc + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k), idesc, acc);
-            }
-            if constexpr (CG == 2) umma_commit_pair(&empty_bar[stage], 0x3); else umma_commit(&empty_bar[stage]);
-            if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
-          }
-          if constexpr (CG == 2) umma_commit_pair(&tfull_bar[h], 0x3); else umma_commit(&tfull_bar[h]);
+          for (int b = 0; b < Cfg::kLoadRows / Cfg::kBox; ++b)
+            tma_load_2d(sb + b * Cfg::kBox * GEMM_BLOCK_K * 2, &tmB, &full_bar[stage], kb * GEMM_BLOCK_K, c0 + b * Cfg::kBox);
         }
-        tphase ^= 1u;
+        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
       }
     }
+    __syncwarp();
   } else {
-    // ===================== epilogue: thread = row; warp pair (w = 0, 1) of a quarter alternates chunks =====================
-    const int quarter = warp & 3;
-    const int ew = warp - 2;
-    const int w = ew >> 2;
-    uint8_t* my_slabs = slab_base + ew * (GLN_SLABS * 4096);
-    uint64_t* my_xbar = x_bar + ew * GLN_SLABS;
-    const uint32_t sw = static_cast<uint32_t>(lane & 7);
-    const uint32_t trow = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    uint32_t tphase = 0;
-    uint32_t xround = 0;                               // slab-barrier phases completed before this tile
-    for (int tile = first_tile; tile < p.num_m_tiles; tile += tile_step, xround += Cfg::kRounds) {
-      const int row0 = tile * kTileRows + row_off + quarter * 32;
-      // every slab is free here (first tile, or bulk_wait_group_read<0> at the end of the previous tile)
-      if (lane == 0) {
+    // ===================== MMA warpgroups: columns [kNW wg, kNW wg + kNW) of this CTA's part =====================
+    const int wg = (threadIdx.x >> 7) - 1;
+    float acc[kNW / 2];
 #pragma unroll
-        for (int i = 0; i < GLN_SLABS; ++i) {
-          mbar_expect_tx(&my_xbar[i], 4096);
-          tma_load_2d(my_slabs + i * 4096, &tmX, &my_xbar[i], (2 * i + w) * 32, row0);
-        }
-      }
-      float shift = 0.f, sum = 0.f, sq = 0.f;
-      bool half1_ready = false;
-#pragma unroll 1
-      for (int i = 0; i < Cfg::kMyChunks; ++i) {
-        const int c = 2 * i + w;                       // this warp's i-th 32-column chunk
-        if (i == 0) {                                  // accumulator half 0 ready
-          mbar_wait(&tfull_bar[0], tphase);
-          tc_fence_after();
-        }
-        if (c >= Cfg::kChunks / 2 && !half1_ready) {   // pass 1 of half 0 overlapped half 1's MMAs
-          mbar_wait(&tfull_bar[1], tphase);
-          tc_fence_after();
-          half1_ready = true;
-        }
-        const int s = i % GLN_SLABS;
-        mbar_wait(&my_xbar[s], (xround + static_cast<uint32_t>(i / GLN_SLABS)) & 1u);
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(trow + static_cast<uint32_t>(c * 32), v);
-        tmem_ld_wait();
-        uint8_t* slab = my_slabs + s * 4096;
-        uint8_t* buf = slab + lane * 128;
-        const float* bb = s_bias + c * 32;
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
-          float4* px = reinterpret_cast<float4*>(buf + ((static_cast<uint32_t>(jj) ^ sw) << 4));
-          const float4 xo = *px;
-          float4 r;
-          r.x = (__uint_as_float(v[jj * 4 + 0]) + bb[jj * 4 + 0]) + xo.x;
-          r.y = (__uint_as_float(v[jj * 4 + 1]) + bb[jj * 4 + 1]) + xo.y;
-          r.z = (__uint_as_float(v[jj * 4 + 2]) + bb[jj * 4 + 2]) + xo.z;
-          r.w = (__uint_as_float(v[jj * 4 + 3]) + bb[jj * 4 + 3]) + xo.w;
-          *px = r;
-          if (i == 0 && jj == 0) shift = r.x;          // shifted single-pass variance (shift = first element seen)
-          const float d0 = r.x - shift, d1 = r.y - shift, d2 = r.z - shift, d3 = r.w - shift;
-          sum += (d0 + d1) + (d2 + d3);
-          sq = fmaf(d0, d0, fmaf(d1, d1, fmaf(d2, d2, fmaf(d3, d3, sq))));
-          v[jj * 4 + 0] = __float_as_uint(r.x); v[jj * 4 + 1] = __float_as_uint(r.y);
-          v[jj * 4 + 2] = __float_as_uint(r.z); v[jj * 4 + 3] = __float_as_uint(r.w);
-        }
-        tmem_st_32x32b_x32(trow + static_cast<uint32_t>(c * 32), v);           // keep the updated row for pass 2
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(&tmX, slab, c * 32, row0);
-          bulk_commit_group();
-          // the slab of this warp's previous chunk is reusable once its store (the second newest group) has read it
-          if (i >= 1 && i - 1 + GLN_SLABS < Cfg::kMyChunks) {
-            bulk_wait_group_read<1>();
-            const int sp = (i - 1) % GLN_SLABS;
-            mbar_expect_tx(&my_xbar[sp], 4096);
-            tma_load_2d(my_slabs + sp * 4096, &tmX, &my_xbar[sp], (2 * (i - 1 + GLN_SLABS) + w) * 32, row0);
-          }
-        }
-      }
-      // ---- combine the two partial statistics of the row (each over D/2 columns) ----
-      constexpr float kHalfN = 0.5f * D;
-      const float md = sum * (1.0f / kHalfN);
-      const float my_mean = shift + md;
-      const float my_m2 = fmaxf(sq - sum * md, 0.0f);
-      s_stat[(quarter * 2 + w) * 32 + lane] = make_float2(my_mean, my_m2);
-      tmem_st_wait();                                  // (also orders this warp's TMEM stores before the pair barrier)
-      tc_fence_before();
-      asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");
-      tc_fence_after();
-      const float2 other = s_stat[(quarter * 2 + (w ^ 1)) * 32 + lane];
-      const float delta = other.x - my_mean;            // symmetric forms: both warps of the pair get identical bits
-      const float mean = 0.5f * (my_mean + other.x);
-      const float var = ((my_m2 + other.y) + delta * delta * (0.5f * kHalfN)) * (1.0f / D);
-      const float rstd = 1.0f / sqrtf(var + p.eps);
-      if (lane == 0) bulk_wait_group_read<0>();        // every slab of this warp is free again
-      __syncwarp();
-      // ---- pass 2: normalise, bf16, 64 columns (128 B) per row per TMA store; chunk c2 = 2 * i + w ----
-      int k2 = 0;
-      bool low_released = false;
-#pragma unroll 1
-      for (int c = w; c < D / 64; c += 2, ++k2) {
-        if (c * 64 >= Cfg::kNH && !low_released) {      // this warp has read its last chunk of TMEM columns [0, D/2)
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty_bar[0]);
-          low_released = true;
-        }
-        if (k2 >= GLN_SLABS) {                          // (never taken for D <= 384)
-          if (lane == 0) bulk_wait_group_read<GLN_SLABS - 1>();
-          __syncwarp();
-        }
-        uint8_t* slab = my_slabs + (k2 % GLN_SLABS) * 4096;
-        uint8_t* buf = slab + lane * 128;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(trow + static_cast<uint32_t>(c * 64 + h * 32), v);
-          tmem_ld_wait();
-          const float* gg = s_gamma + c * 64 + h * 32;
-          const float* be = s_beta + c * 64 + h * 32;
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            float f[8];
-#pragma unroll
-            for (int t = 0; t < 8; ++t)
-              f[t] = (__uint_as_float(v[jj * 8 + t]) - mean) * rstd * gg[jj * 8 + t] + be[jj * 8 + t];
-            uint4 q;
-            q.x = pack_bf16(f[0], f[1]); q.y = pack_bf16(f[2], f[3]);
-            q.z = pack_bf16(f[4], f[5]); q.w = pack_bf16(f[6], f[7]);
-            *reinterpret_cast<uint4*>(buf + ((static_cast<uint32_t>(h * 4 + jj) ^ sw) << 4)) = q;
-          }
-        }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(&tmN, slab, c * 64, row0);
-          bulk_commit_group();
-        }
-      }
-      tc_fence_before();
-      if (lane == 0) bulk_wait_group_read<0>();        // slabs free for the next tile's x loads
-      __syncwarp();
-      if (lane == 0) {
-        if (!low_released) mbar_arrive(&tempty_bar[0]);
-        mbar_arrive(&tempty_bar[1]);
-      }
-      tphase ^= 1u;
-    }
-    if (lane == 0) bulk_wait_group<0>();
+    for (int i = 0; i < kNW / 2; ++i) acc[i] = 0.0f;
+    int stage = 0;
+    uint32_t phase = 0;
+    wg_mainloop<kNW, MODE == 1>(acc, smem, Cfg::kStageBytes, 0, Cfg::kABytes + wg * kNW * GEMM_BLOCK_K * 2, full_bar,
+                                empty_bar, Cfg::kStages, num_kb, stage, phase);
+    gln_epilogue<D, kNW, Cfg::kParts, MODE == 2>(acc, x, xn, p.M, p.eps, m0, c0, wg, rank, s_bias, s_gamma, s_beta, s_part,
+                                                stat_bar);
   }
-
-  tc_fence_before();
-  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();   // peer smem / barriers stay valid until all are done
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (CG == 2) tmem_dealloc_pair<512>(tmem_base);
-    else tmem_dealloc<512>(tmem_base);
-  }
+  // a CTA of a pair must not exit while its peer may still write to its shared memory or arrive on its barriers
+  if constexpr (MODE != 0) cluster_sync_all();
 }
 
 }  // namespace pq

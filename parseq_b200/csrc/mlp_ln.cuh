@@ -1,34 +1,17 @@
-// The whole MLP of an encoder block + the LayerNorm that follows, in one kernel (sm_100a, tcgen05 + TMA).
+// The whole MLP of a timm Block + the LayerNorm that follows it in one kernel (sm_90a, wgmma + TMA):
 //
-//   h[128, 4D]   (bf16, never leaves the SM)  <-  GELU(xn * W1^T + b1)                       (timm Mlp.fc1 + act)
-//   x[M, D]      (fp32, in place)             <-  x + h * W2^T + b2                           (Mlp.fc2 + residual)
-//   xn_out[M, D] (bf16; may alias xn)         <-  LayerNorm(x_new; gamma, beta, eps)          (next norm1 / final norm)
+//   x[M, D]  (fp32, in place)  <-  x + GELU(xn W1^T + b1) W2^T + b2        (H = 4 D hidden columns)
+//   xn_out   (bf16)            <-  LayerNorm(x_new; gamma, beta, eps)      (may alias xn)
 //
-// Why: as two kernels (gemm.cuh with the GELU epilogue, gemm_ln.cuh) the hidden activation makes a 2 x 201 MB round trip
-// through HBM per block at M = 65536 and each launch pays its own prologue, tail and TMEM-drain epilogue.  Here one CTA
-// owns 128 full rows for the whole MLP; the hidden activation is produced 64 columns (= one k-block of fc2) at a time:
+// A CTA owns 64 rows; their xn tile stays in shared memory for the whole kernel.  The hidden activation never reaches
+// HBM: it is produced 64 columns at a time (fc1: each MMA warpgroup computes 32 of them, GELU, bf16, into a swizzled
+// shared-memory chunk, double-buffered) and consumed at once as one 64-wide k-block of fc2, whose accumulators (each
+// warpgroup half of the D output columns) live in registers across all H / 64 chunks.  The weights stream through one
+// TMA ring in a fixed order: per chunk, the D / 64 k-blocks of its W1 rows, then the two column halves of its W2 block.
+// Same k order and rounding points as the two-kernel path (GEMM with the GELU epilogue, then gemm_ln.cuh MODE 0):
+// bit-identical results.
 //
-//   warp 0       TMA producer: the xn tile (128 x D, resident for the tile) and a ring of 24 KB weight stages in the order
-//                the MMA warp consumes them: W1 rows of chunk j+1 (64 x D, D/192 stages), both column halves of W2's
-//                k-block j (D/2 x 64 each)
-//   warp 1       MMA issuer.  fc1 chunk j: UMMA 128 x 64 x 16 over K = D into one of two 64-column TMEM buffers;
-//                fc2 k-block j: UMMA 128 x D/2 x 16 x 2 halves, A = the bf16 chunk the epilogue warps left in shared memory,
-//                accumulating into TMEM columns [0, D).  Issue order MMA1(j+1), MMA2(j): the tensor pipe works on the next
-//                chunk while the epilogue warps turn chunk j into fc2's A operand.
-//   warps 2..17  GELU epilogue, four per TMEM lane quarter, 16 columns of the chunk each: TMEM -> +b1 -> GELU (FFMA2) ->
-//                bf16 -> the 128B-swizzled K-major tile a UMMA descriptor reads (same layout a TMA box would produce)
-//   warps 2..9   then run gemm_ln.cuh's residual + LayerNorm epilogue on the finished fc2 accumulator (their x staging
-//                slabs alias the xn tile, which is dead once the last fc1 chunk has been issued)
-//
-// CG = 2 (CTA pair, tcgen05 cta_group::2, UMMA M = 256): each CTA keeps its own 128 rows (xn tile, hidden chunk, epilogues)
-// but stages only HALF of every weight box (32 of the 64 W1 rows of a chunk, D/4 of the D/2 W2 rows of a half), so the same
-// ring holds twice as many k-steps.  That is what makes the kernel pay: single-CTA, 72 KB of ring cover 3/4 of one chunk's
-// weights and every chunk waits for a full TMA round trip (1.9 us per chunk for 0.8 us of tensor work).  Pair plumbing as
-// in gemm.cuh: all loads complete on the leader's barriers, commits are multicast, and the peer's idle warp 1 forwards
-// "hidden chunk ready" (per chunk) and "accumulator drained" (per tile) to the leader with one remote arrive each.
-//
-// Same k order per output element and same rounding points (bf16 hidden, fp32 x, bf16 xn) as the two-kernel path:
-// results are bit-identical to it (tests/test_gpu_kernels.py::test_mlp_ln_fused_equals_two_kernels).
+// CG = 2: a cluster of two CTAs on 128 rows; each CTA loads half of every weight box and multicasts it into both.
 #pragma once
 #include "gemm_ln.cuh"
 
@@ -41,485 +24,187 @@ struct MlpLnParams {
   const float* gamma;    // [D]
   const float* beta;     // [D]
   float eps;
-  int num_m_tiles;
-  unsigned long long* prof;   // optional [16] cycle counters of CTA 0 (tests/prof_mlp_ln.py); nullptr in production
+  int num_m_tiles;       // clusters of CG CTAs
 };
 
-constexpr int MLP_EPI_WARPS = 16;
-constexpr int MLP_LN_WARPS = GLN_EPI_WARPS;            // the first 8 epilogue warps also run the LayerNorm epilogue
-constexpr int MLP_THREADS = 64 + 32 * MLP_EPI_WARPS;
+constexpr int MLP_THREADS = 384;
 
-template <int D, int CG = 1>
+template <int D, int CG>
 struct MlpLnCfg {
-  static_assert(CG == 1 || CG == 2, "CG");
-  static constexpr int kH = 4 * D;                                    // hidden width (mlp_ratio 4)
-  static constexpr int kNC = kH / 64;                                 // hidden chunks = k-blocks of fc2
-  static constexpr int kKB1 = D / 64;                                 // k-blocks of fc1
-  static constexpr int kNH = D / 2;                                   // fc2 output columns per UMMA
-  static constexpr int kXnBytes = kKB1 * GEMM_BLOCK_M * 128;          // resident xn tile
-  static constexpr int kSlabBytes = MLP_LN_WARPS * GLN_SLABS * 4096;  // LayerNorm epilogue staging (aliases the xn tile)
-  static constexpr int kRegionBytes = kXnBytes > kSlabBytes ? kXnBytes : kSlabBytes;
-  static constexpr int kHBytes = GEMM_BLOCK_M * 128;                  // one bf16 hidden chunk 128 x 64
-  static constexpr int kStageBytes = 24576 / CG;                      // 3 W1 boxes [64/CG x 64] or one W2 box [D/2/CG x 64]
-  static constexpr int kW1Stages = kKB1 / 3;                          // ring stages per fc1 chunk
-  static constexpr int kW1Rows = 64 / CG;                             // W1 rows of a chunk this CTA stages
-  static constexpr int kW2Rows = kNH / CG;                            // W2 rows of a column half this CTA stages
-  static constexpr int kW1BoxBytes = kW1Rows * 128;
-  static constexpr int kW1Bytes = 3 * kW1BoxBytes;
-  static constexpr int kW2Bytes = kW2Rows * 128;
-  static constexpr int kParamBytes = kH * 4 + 3 * D * 4 + 4 * 2 * 32 * 8;
-  static constexpr int kBarBytes = 512;
-  static_assert(kW1BoxBytes % 1024 == 0 && kW2Bytes % 1024 == 0, "1024-B aligned operand tiles");
-  static constexpr int kStagesRaw = (232448 - 1024 - kBarBytes - kRegionBytes - 2 * kHBytes - kParamBytes) / kStageBytes;
+  static constexpr int kH = 4 * D;
+  static constexpr int kKC = D / 64;                                  // fc1 k-blocks per hidden chunk
+  static constexpr int kChunks = kH / 64;                             // hidden chunks = fc2 k-blocks
+  static constexpr int kW1Rows = 64 / CG;                             // W1 box rows loaded by one CTA
+  static constexpr int kW2Rows = D / 2 / CG;                          // W2 box rows loaded by one CTA
+  static constexpr int kW1Bytes = 64 * 64 * 2;
+  static constexpr int kW2Bytes = (D / 2) * 64 * 2;
+  static constexpr int kSlotBytes = kW2Bytes > kW1Bytes ? kW2Bytes : kW1Bytes;
+  static constexpr int kXsBytes = kKC * 64 * 64 * 2;                  // the CTA's xn rows
+  static constexpr int kHidBytes = 2 * 64 * 64 * 2;                   // two hidden chunks
+  static constexpr int kParamBytes = (kH + 3 * D) * 4 + 2 * 2 * GLN_BLOCK_M * 4;   // b1, b2, gamma, beta; row partials
+  static constexpr int kBarBytes = 256;
+  static constexpr int kStagesRaw = (232448 - 1024 - kBarBytes - kXsBytes - kHidBytes - kParamBytes) / kSlotBytes;
   static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
-  static constexpr int kSmemBytes = kRegionBytes + 2 * kHBytes + kStages * kStageBytes + kParamBytes + kBarBytes + 1024;
-  static_assert(D == 192 || D == 384, "full rows + two 64-column chunk buffers must fit 512 TMEM columns");
-  static_assert(kKB1 % 3 == 0 && kW1Bytes <= kStageBytes && kW2Bytes <= kStageBytes, "ring stage holds either operand");
-  static_assert(kNC % 2 == 0, "chunk buffers alternate evenly over a tile");
-  static_assert(kStages >= 3, "ring depth");
-  static_assert((kRegionBytes % 1024) == 0 && (kHBytes % 1024) == 0 && (kStageBytes % 1024) == 0, "1024-B aligned tiles");
-  using Ln = GemmLnCfg<D, 1>;                                         // chunking of the LayerNorm epilogue
+  static constexpr int kSmemBytes = kXsBytes + kHidBytes + kStages * kSlotBytes + kParamBytes + kBarBytes + 1024;
+  static_assert(D == 192 || D == 384, "embed_dim");
+  static_assert((kW1Rows * 128) % 1024 == 0 && (kW2Rows * 128) % 1024 == 0 && kSlotBytes % 1024 == 0, "1024-B aligned boxes");
+  static_assert(kStages >= 4, "pipeline depth");
 };
 
-// TMEM -> registers, 16 consecutive fp32 columns of this thread's lane
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-template <int D, int CG = 1>
+template <int D, int CG>
 __global__ void __launch_bounds__(MLP_THREADS, 1)
-mlp_ln_fused_kernel(const __grid_constant__ CUtensorMap tmXN, const __grid_constant__ CUtensorMap tmW1,
-                    const __grid_constant__ CUtensorMap tmW2, const __grid_constant__ CUtensorMap tmX,
-                    const __grid_constant__ CUtensorMap tmN, const MlpLnParams p) {
+mlp_ln_fused_kernel(const __grid_constant__ CUtensorMap tmXn, const __grid_constant__ CUtensorMap tmW1,
+                    const __grid_constant__ CUtensorMap tmW2, float* __restrict__ x, __nv_bfloat16* __restrict__ xn_out,
+                    const MlpLnParams p) {
   using Cfg = MlpLnCfg<D, CG>;
-  using Ln = typename Cfg::Ln;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   const uint32_t pad = ((raw_addr + 1023u) & ~1023u) - raw_addr;
-  uint8_t* region = smem_raw + pad;                                   // xn tile [kKB1][128 x 128 B]  /  LN slabs
-  uint8_t* hbuf = region + Cfg::kRegionBytes;                         // [2][128 x 128 B] bf16 hidden chunk, SW128 K-major
-  uint8_t* ring = hbuf + 2 * Cfg::kHBytes;
-  float* s_b1 = reinterpret_cast<float*>(ring + Cfg::kStages * Cfg::kStageBytes);
-  float* s_bias = s_b1 + Cfg::kH;
-  float* s_gamma = s_bias + D;
+  uint8_t* xs = smem_raw + pad;                                       // [kKC][64 rows][128 B], 1024-B aligned
+  uint8_t* hid = xs + Cfg::kXsBytes;                                  // [2][64 rows][128 B]
+  uint8_t* ring = hid + Cfg::kHidBytes;
+  float* s_b1 = reinterpret_cast<float*>(ring + Cfg::kStages * Cfg::kSlotBytes);
+  float* s_b2 = s_b1 + Cfg::kH;
+  float* s_gamma = s_b2 + D;
   float* s_beta = s_gamma + D;
-  float2* s_stat = reinterpret_cast<float2*>(s_beta + D);             // [4 quarters][2 warps][32 rows] (mean, M2)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(s_b1) + Cfg::kParamBytes);
-  uint64_t* full_bar = bars;                           // [kStages] ring: TMA -> MMA
-  uint64_t* empty_bar = full_bar + Cfg::kStages;       // [kStages] ring: MMA -> TMA
-  uint64_t* xn_full = empty_bar + Cfg::kStages;        // xn tile landed
-  uint64_t* xn_empty = xn_full + 1;                    // the LN epilogue is done with the region
-  uint64_t* a1_full = xn_empty + 1;                    // [2] fc1 chunk accumulated
-  uint64_t* h_full = a1_full + 2;                      // [2] bf16 chunk in shared memory (and its TMEM buffer drained)
-  uint64_t* h_empty = h_full + 2;                      // [2] fc2 has read the chunk
-  uint64_t* a2_full = h_empty + 2;                     // fc2 accumulator of the tile complete
-  uint64_t* a2_empty = a2_full + 1;                    // LN pass 2 has drained it
-  uint64_t* x_bar = a2_empty + 1;                      // [MLP_LN_WARPS][GLN_SLABS]: x chunk landed
-  uint64_t* hp_full = x_bar + MLP_LN_WARPS * GLN_SLABS; // [2] pair leader: the PEER's chunk is in its shared memory (forwarded)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(hp_full + 2);
+  float* s_part = s_beta + D;                                         // [2 rounds][2 parts][64 rows]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(s_b1) + Cfg::kParamBytes);
+  uint64_t* empty_bar = full_bar + Cfg::kStages;
+  uint64_t* xs_bar = empty_bar + Cfg::kStages;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
   const uint32_t rank = (CG == 2) ? cluster_ctarank() : 0u;
-  const int first_tile = blockIdx.x / CG;                // tiles of 128 * CG rows
-  const int tile_step = gridDim.x / CG;
-  constexpr int kTileRows = GEMM_BLOCK_M * CG;
-  const int row_off = static_cast<int>(rank) * GEMM_BLOCK_M;
+  const int m0 = (blockIdx.x / CG) * (GLN_BLOCK_M * CG) + static_cast<int>(rank) * GLN_BLOCK_M;
 
   grid_dep_launch();
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmXN); prefetch_tmap(&tmW1); prefetch_tmap(&tmW2); prefetch_tmap(&tmX); prefetch_tmap(&tmN);
-    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(xn_full, 1);
-    mbar_init(xn_empty, MLP_LN_WARPS);
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&a1_full[b], 1);
-      mbar_init(&h_full[b], MLP_EPI_WARPS);
-      mbar_init(&h_empty[b], 1);
-      mbar_init(&hp_full[b], 1);
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmXn);
+    prefetch_tmap(&tmW1);
+    prefetch_tmap(&tmW2);
+    for (int s = 0; s < Cfg::kStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 2 * CG);
     }
-    mbar_init(a2_full, 1);
-    mbar_init(a2_empty, (CG == 2 && rank == 0) ? MLP_LN_WARPS + 1 : MLP_LN_WARPS);
-    for (int i = 0; i < MLP_LN_WARPS * GLN_SLABS; ++i) mbar_init(&x_bar[i], 1);
+    mbar_init(xs_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    if constexpr (CG == 2) tmem_alloc_pair<512>(tmem_slot);
-    else tmem_alloc<512>(tmem_slot);
-  }
-  for (int j = threadIdx.x; j < Cfg::kH; j += MLP_THREADS) s_b1[j] = (p.b1 != nullptr) ? __ldg(p.b1 + j) : 0.0f;
+  for (int j = threadIdx.x; j < Cfg::kH; j += MLP_THREADS) s_b1[j] = __ldg(p.b1 + j);
   for (int j = threadIdx.x; j < D; j += MLP_THREADS) {
-    s_bias[j] = (p.b2 != nullptr) ? __ldg(p.b2 + j) : 0.0f;
+    s_b2[j] = __ldg(p.b2 + j);
     s_gamma[j] = __ldg(p.gamma + j);
     s_beta[j] = __ldg(p.beta + j);
   }
-  tc_fence_before();
   if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_a1 = tmem_base + static_cast<uint32_t>(D);      // two 64-column fc1 chunk buffers behind acc2
   grid_dep_wait();
 
-  if (warp == 0) {
+  if (threadIdx.x < 128) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
+      mbar_expect_tx(xs_bar, Cfg::kXsBytes);
+      for (int c = 0; c < Cfg::kKC; ++c) tma_load_2d(xs + c * 8192, &tmXn, xs_bar, c * 64, m0);
+      const int r = static_cast<int>(rank);
       int stage = 0;
-      uint32_t phase = 0, tphase = 0;
-      auto load_w1 = [&](int j) {                       // W1 rows [64 j, 64 j + 64), all of K = D
-#pragma unroll 1
-        for (int s = 0; s < Cfg::kW1Stages; ++s) {
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          uint8_t* sa = ring + stage * Cfg::kStageBytes;
-          const int r0 = j * 64 + static_cast<int>(rank) * Cfg::kW1Rows;
-          if constexpr (CG == 1) {
-            mbar_expect_tx(&full_bar[stage], Cfg::kW1Bytes);
-#pragma unroll
-            for (int t = 0; t < 3; ++t)
-              tma_load_2d(sa + t * Cfg::kW1BoxBytes, &tmW1, &full_bar[stage], (s * 3 + t) * 64, r0);
-          } else {
-            const uint32_t leader_full = mapa_cluster(smem_u32(&full_bar[stage]), 0u);
-            if (rank == 0) mbar_expect_tx(&full_bar[stage], 2u * Cfg::kW1Bytes);
-#pragma unroll
-            for (int t = 0; t < 3; ++t)
-              tma_load_2d_pair(sa + t * Cfg::kW1BoxBytes, &tmW1, leader_full, (s * 3 + t) * 64, r0);
-          }
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
-        }
+      uint32_t phase = 0;
+      auto next_slot = [&](int bytes) -> uint8_t* {
+        mbar_wait_mma(&empty_bar[stage], phase ^ 1u);
+        mbar_expect_tx(&full_bar[stage], bytes);
+        return ring + stage * Cfg::kSlotBytes;
       };
-      auto load_w2 = [&](int j) {                       // W2[:, 64 j .. 64 j + 64): the two halves of the output columns
-#pragma unroll 1
-        for (int h = 0; h < 2; ++h) {
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          uint8_t* sa = ring + stage * Cfg::kStageBytes;
-          const int r0 = h * Cfg::kNH + static_cast<int>(rank) * Cfg::kW2Rows;
-          if constexpr (CG == 1) {
-            mbar_expect_tx(&full_bar[stage], Cfg::kW2Bytes);
-            tma_load_2d(sa, &tmW2, &full_bar[stage], j * 64, r0);
-          } else {
-            const uint32_t leader_full = mapa_cluster(smem_u32(&full_bar[stage]), 0u);
-            if (rank == 0) mbar_expect_tx(&full_bar[stage], 2u * Cfg::kW2Bytes);
-            tma_load_2d_pair(sa, &tmW2, leader_full, j * 64, r0);
-          }
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
+      auto advance = [&]() { if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; } };
+      for (int j = 0; j < Cfg::kChunks; ++j) {
+        for (int c = 0; c < Cfg::kKC; ++c) {                         // W1 rows [64 j, 64 j + 64), k-block c
+          uint8_t* dst = next_slot(Cfg::kW1Bytes) + r * Cfg::kW1Rows * 128;
+          if constexpr (CG == 2) tma_load_2d_mcast(dst, &tmW1, &full_bar[stage], c * 64, j * 64 + r * Cfg::kW1Rows, 0x3);
+          else tma_load_2d(dst, &tmW1, &full_bar[stage], c * 64, j * 64);
+          advance();
         }
-      };
-      for (int tile = first_tile; tile < p.num_m_tiles; tile += tile_step) {
-        const int m0 = tile * kTileRows + row_off;
-        load_w1(0);                                     // weights do not wait for the previous tile's epilogue
-        mbar_wait(xn_empty, tphase ^ 1u);               // region free (the LN slabs of the previous tile alias it)
-        if constexpr (CG == 1) {
-          mbar_expect_tx(xn_full, Cfg::kXnBytes);
-#pragma unroll 1
-          for (int kb = 0; kb < Cfg::kKB1; ++kb) tma_load_2d(region + kb * 16384, &tmXN, xn_full, kb * 64, m0);
-        } else {
-          // The leader arms its barrier for the tiles of BOTH CTAs when its own region is free; the peer's bytes may land
-          // before or after that (the phase cannot complete without the leader's arrival).
-          const uint32_t leader_xn = mapa_cluster(smem_u32(xn_full), 0u);
-          if (rank == 0) mbar_expect_tx(xn_full, 2u * Cfg::kXnBytes);
-#pragma unroll 1
-          for (int kb = 0; kb < Cfg::kKB1; ++kb) tma_load_2d_pair(region + kb * 16384, &tmXN, leader_xn, kb * 64, m0);
-        }
-#pragma unroll 1
-        for (int j = 0; j < Cfg::kNC; ++j) {
-          if (j + 1 < Cfg::kNC) load_w1(j + 1);
-          load_w2(j);
-        }
-        tphase ^= 1u;
-      }
-    }
-  } else if (warp == 1) {
-    if (CG == 2 && rank != 0) {
-      // peer CTA: forward "my hidden chunk is in shared memory" (per chunk) and "my rows have left the fc2 accumulator"
-      // (per tile) to the leader: one remote arrive each, issued by this otherwise idle warp
-      if (lane == 0) {
-        uint32_t cc = 0, tphase = 0;
-        for (int tile = first_tile; tile < p.num_m_tiles; tile += tile_step) {
-          for (int j = 0; j < Cfg::kNC; ++j, ++cc) {
-            mbar_wait(&h_full[cc & 1u], (cc >> 1) & 1u);
-            mbar_arrive_cluster(mapa_cluster(smem_u32(&hp_full[cc & 1u]), 0u));
-          }
-          mbar_wait(a2_empty, tphase);
-          mbar_arrive_cluster(mapa_cluster(smem_u32(a2_empty), 0u));
-          tphase ^= 1u;
+        for (int h = 0; h < 2; ++h) {                                  // W2 rows [h D/2, (h+1) D/2), k-block j
+          uint8_t* dst = next_slot(Cfg::kW2Bytes) + r * Cfg::kW2Rows * 128;
+          if constexpr (CG == 2)
+            tma_load_2d_mcast(dst, &tmW2, &full_bar[stage], j * 64, h * (D / 2) + r * Cfg::kW2Rows, 0x3);
+          else tma_load_2d(dst, &tmW2, &full_bar[stage], j * 64, h * (D / 2));
+          advance();
         }
       }
     }
-    // ===================== MMA issuer (the leader CTA's) =====================
-    if (lane == 0 && rank == 0) {
-      constexpr uint32_t idesc1 = make_idesc_bf16(kTileRows, 64);
-      constexpr uint32_t idesc2 = make_idesc_bf16(kTileRows, Cfg::kNH);
-      auto mma = [](uint32_t d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
-        if constexpr (CG == 2) umma_bf16_pair(d, a, b, idesc, acc); else umma_bf16(d, a, b, idesc, acc);
-      };
-      auto commit = [](uint64_t* bar) {
-        if constexpr (CG == 2) umma_commit_pair(bar, 0x3); else umma_commit(bar);
-      };
-      int stage = 0;
-      uint32_t phase = 0, tphase = 0;
-      uint32_t cc = 0;                                  // running chunk count: buffer cc & 1, phase (cc >> 1) & 1
-      const uint32_t region_addr = smem_u32(region);
-      const bool prof = (p.prof != nullptr) && blockIdx.x == 0;
-      long long w_ring1 = 0, w_ring2 = 0, w_h = 0, w_hp = 0, w_xn = 0, w_a2 = 0, t_all = 0;
-      auto mma1 = [&](uint32_t c) {
-        const uint32_t b = c & 1u;
-        const uint32_t tmem_d = tmem_a1 + b * 64u;
-#pragma unroll 1
-        for (int s = 0; s < Cfg::kW1Stages; ++s) {
-          const long long t0 = prof ? clock64() : 0;
-          mbar_wait(&full_bar[stage], phase);
-          if (prof) w_ring1 += clock64() - t0;
-          tc_fence_after();
-          const uint32_t sa = smem_u32(ring + stage * Cfg::kStageBytes);
-#pragma unroll
-          for (int t = 0; t < 3; ++t) {
-            const int kb = s * 3 + t;
-            const uint64_t adesc = make_desc_k_sw128(region_addr + static_cast<uint32_t>(kb) * 16384u);
-            const uint64_t bdesc = make_desc_k_sw128(sa + static_cast<uint32_t>(t * Cfg::kW1BoxBytes));
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              mma(tmem_d, adesc + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k), idesc1,
-                  static_cast<uint32_t>((kb | k) != 0));
-          }
-          commit(&empty_bar[stage]);
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
-        }
-        commit(&a1_full[b]);
-      };
-      const long long t_begin = prof ? clock64() : 0;
-      for (int tile = first_tile; tile < p.num_m_tiles; tile += tile_step) {
-        long long t0 = prof ? clock64() : 0;
-        mbar_wait(xn_full, tphase);
-        if (prof) w_xn += clock64() - t0;
-        tc_fence_after();
-        mma1(cc);
-#pragma unroll 1
-        for (int j = 0; j < Cfg::kNC; ++j) {
-          // (buffer (cc + 1) & 1 was drained before chunk cc - 1's h_full, which the previous iteration waited for)
-          if (j + 1 < Cfg::kNC) mma1(cc + 1u);
-          const uint32_t b = cc & 1u;
-          t0 = prof ? clock64() : 0;
-          mbar_wait(&h_full[b], (cc >> 1) & 1u);
-          if (prof) { const long long t1 = clock64(); w_h += t1 - t0; t0 = t1; }
-          if constexpr (CG == 2) mbar_wait(&hp_full[b], (cc >> 1) & 1u);
-          if (prof) w_hp += clock64() - t0;
-          tc_fence_after();
-          if (j == 0) {                                 // the previous tile's rows have left the fc2 accumulator
-            t0 = prof ? clock64() : 0;
-            mbar_wait(a2_empty, tphase ^ 1u);
-            if (prof) w_a2 += clock64() - t0;
-            tc_fence_after();
-          }
-          const uint64_t adesc = make_desc_k_sw128(smem_u32(hbuf) + b * static_cast<uint32_t>(Cfg::kHBytes));
-#pragma unroll 1
-          for (int h = 0; h < 2; ++h) {
-            t0 = prof ? clock64() : 0;
-            mbar_wait(&full_bar[stage], phase);
-            if (prof) w_ring2 += clock64() - t0;
-            tc_fence_after();
-            const uint64_t bdesc = make_desc_k_sw128(smem_u32(ring + stage * Cfg::kStageBytes));
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              mma(tmem_base + static_cast<uint32_t>(h * Cfg::kNH), adesc + static_cast<uint64_t>(2 * k),
-                  bdesc + static_cast<uint64_t>(2 * k), idesc2, static_cast<uint32_t>((j | k) != 0));
-            commit(&empty_bar[stage]);
-            if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
-          }
-          commit(&h_empty[b]);
-          ++cc;
-        }
-        commit(a2_full);
-        tphase ^= 1u;
-      }
-      if (prof) {
-        t_all = clock64() - t_begin;
-        p.prof[0] = t_all; p.prof[1] = w_xn; p.prof[2] = w_ring1; p.prof[3] = w_h; p.prof[4] = w_hp; p.prof[5] = w_ring2;
-        p.prof[6] = w_a2;
-      }
-    }
+    __syncwarp();
   } else {
-    // ===================== epilogue warps =====================
-    const int quarter = warp & 3;                        // TMEM lane quarter this warp may access
-    const int ew = warp - 2;                             // 0..15
-    const int g = ew >> 2;                               // GELU: 16-column group of the chunk
-    const int w = ew >> 2;                               // LN (ew < 8): which of the alternating 32-column chunks
-    const uint32_t sw = static_cast<uint32_t>(lane & 7);
-    const uint32_t trow = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    uint8_t* my_slabs = region + (ew & (MLP_LN_WARPS - 1)) * (GLN_SLABS * 4096);
-    uint64_t* my_xbar = x_bar + (ew & (MLP_LN_WARPS - 1)) * GLN_SLABS;
-    uint32_t cc = 0, tphase = 0, xround = 0;
-    const bool prof = (p.prof != nullptr) && blockIdx.x == 0 && ew == 0 && lane == 0;
-    long long e_a1 = 0, e_ld = 0, e_he = 0, e_rest = 0, e_ln = 0;
-    for (int tile = first_tile; tile < p.num_m_tiles; tile += tile_step, xround += Ln::kRounds) {
-      // ---- fc1 epilogue: chunk -> + b1 -> GELU -> bf16 -> fc2's A operand in shared memory ----
+    // ===================== MMA warpgroups =====================
+    const int wg = (threadIdx.x >> 7) - 1;
+    const int t = threadIdx.x & 127;
+    const int lane = t & 31;
+    const bool signal = t == 0;
+    int stage = 0;
+    uint32_t phase = 0;
+    auto release = [&]() {
+      if (signal) {
+        mbar_arrive(&empty_bar[stage]);
+        if constexpr (CG == 2) mbar_arrive_cluster(mapa_cluster(smem_u32(&empty_bar[stage]), rank ^ 1u));
+      }
+      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
+    };
+    float acc[D / 4];                                                  // fc2: 64 rows x D/2 columns of this warpgroup
+#pragma unroll
+    for (int i = 0; i < D / 4; ++i) acc[i] = 0.0f;
+    mbar_wait_mma(xs_bar, 0);
 #pragma unroll 1
-      for (int j = 0; j < Cfg::kNC; ++j, ++cc) {
-        const uint32_t b = cc & 1u;
-        const uint32_t hp = (cc >> 1) & 1u;
-        long long t0 = prof ? clock64() : 0;
-        mbar_wait(&a1_full[b], hp);
-        if (prof) { const long long t1 = clock64(); e_a1 += t1 - t0; t0 = t1; }
-        tc_fence_after();
-        uint32_t v[16];
-        tmem_ld_32x32b_x16(trow + static_cast<uint32_t>(D) + b * 64u + static_cast<uint32_t>(g * 16), v);
-        tmem_ld_wait();
-        if (prof) { const long long t1 = clock64(); e_ld += t1 - t0; t0 = t1; }
-        const float* bb = s_b1 + j * 64 + g * 16;
-        uint32_t q[8];
+    for (int j = 0; j < Cfg::kChunks; ++j) {
+      // ---- fc1: hidden columns [64 j + 32 wg, +32) ----
+      float h1[16];
 #pragma unroll
-        for (int t = 0; t < 16; t += 2) {
-          float a0, a1, f0, f1;
-          f2_unpack(f2_add(f2_pack(__uint_as_float(v[t]), __uint_as_float(v[t + 1])),
-                           *reinterpret_cast<const unsigned long long*>(bb + t)), a0, a1);
-          gelu_erf_x2(a0, a1, f0, f1);
-          q[t >> 1] = pack_bf16(f0, f1);
-        }
-        if (prof) { const long long t1 = clock64(); e_rest += t1 - t0; t0 = t1; }
-        mbar_wait(&h_empty[b], hp ^ 1u);                 // fc2 of chunk cc - 2 has read this buffer
-        if (prof) { const long long t1 = clock64(); e_he += t1 - t0; t0 = t1; }
-        uint8_t* hrow = hbuf + b * Cfg::kHBytes + (quarter * 32 + lane) * 128;
-        *reinterpret_cast<uint4*>(hrow + ((static_cast<uint32_t>(2 * g) ^ sw) << 4)) = make_uint4(q[0], q[1], q[2], q[3]);
-        *reinterpret_cast<uint4*>(hrow + ((static_cast<uint32_t>(2 * g + 1) ^ sw) << 4)) = make_uint4(q[4], q[5], q[6], q[7]);
-        fence_proxy_async_smem();                        // generic-proxy stores -> visible to the tensor core's reads
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&h_full[b]);
-        if (prof) e_rest += clock64() - t0;
-      }
-      if (ew >= MLP_LN_WARPS) { tphase ^= 1u; continue; }
-      const long long t_ln = prof ? clock64() : 0;
-
-      // ---- residual + LayerNorm epilogue (gemm_ln.cuh), thread = row, warp pair (w = 0, 1) alternates chunks ----
-      const int row0 = tile * kTileRows + row_off + quarter * 32;
-      mbar_wait(a2_full, tphase);                        // every MMA of the tile is complete: the xn tile is dead
-      tc_fence_after();
-      if (lane == 0) {
-#pragma unroll
-        for (int i = 0; i < GLN_SLABS; ++i) {
-          mbar_expect_tx(&my_xbar[i], 4096);
-          tma_load_2d(my_slabs + i * 4096, &tmX, &my_xbar[i], (2 * i + w) * 32, row0);
-        }
-      }
-      float shift = 0.f, sum = 0.f, sq = 0.f;
+      for (int i = 0; i < 16; ++i) h1[i] = 0.0f;
 #pragma unroll 1
-      for (int i = 0; i < Ln::kMyChunks; ++i) {
-        const int c = 2 * i + w;
-        const int s = i % GLN_SLABS;
-        mbar_wait(&my_xbar[s], (xround + static_cast<uint32_t>(i / GLN_SLABS)) & 1u);
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(trow + static_cast<uint32_t>(c * 32), v);
-        tmem_ld_wait();
-        uint8_t* slab = my_slabs + s * 4096;
-        uint8_t* buf = slab + lane * 128;
-        const float* bb = s_bias + c * 32;
+      for (int c = 0; c < Cfg::kKC; ++c) {
+        mbar_wait_mma(&full_bar[stage], phase);
+        const uint64_t da = make_desc_k_sw128(smem_u32(xs + c * 8192));
+        const uint64_t db = make_desc_k_sw128(smem_u32(ring + stage * Cfg::kSlotBytes + wg * 32 * 128));
+        wgmma_fence();
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
-          float4* px = reinterpret_cast<float4*>(buf + ((static_cast<uint32_t>(jj) ^ sw) << 4));
-          const float4 xo = *px;
-          float4 r;
-          r.x = (__uint_as_float(v[jj * 4 + 0]) + bb[jj * 4 + 0]) + xo.x;
-          r.y = (__uint_as_float(v[jj * 4 + 1]) + bb[jj * 4 + 1]) + xo.y;
-          r.z = (__uint_as_float(v[jj * 4 + 2]) + bb[jj * 4 + 2]) + xo.z;
-          r.w = (__uint_as_float(v[jj * 4 + 3]) + bb[jj * 4 + 3]) + xo.w;
-          *px = r;
-          if (i == 0 && jj == 0) shift = r.x;
-          const float d0 = r.x - shift, d1 = r.y - shift, d2 = r.z - shift, d3 = r.w - shift;
-          sum += (d0 + d1) + (d2 + d3);
-          sq = fmaf(d0, d0, fmaf(d1, d1, fmaf(d2, d2, fmaf(d3, d3, sq))));
-          v[jj * 4 + 0] = __float_as_uint(r.x); v[jj * 4 + 1] = __float_as_uint(r.y);
-          v[jj * 4 + 2] = __float_as_uint(r.z); v[jj * 4 + 3] = __float_as_uint(r.w);
-        }
-        tmem_st_32x32b_x32(trow + static_cast<uint32_t>(c * 32), v);
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(&tmX, slab, c * 32, row0);
-          bulk_commit_group();
-          if (i >= 1 && i - 1 + GLN_SLABS < Ln::kMyChunks) {
-            bulk_wait_group_read<1>();
-            const int sp = (i - 1) % GLN_SLABS;
-            mbar_expect_tx(&my_xbar[sp], 4096);
-            tma_load_2d(my_slabs + sp * 4096, &tmX, &my_xbar[sp], (2 * (i - 1 + GLN_SLABS) + w) * 32, row0);
-          }
+        for (int k = 0; k < 4; ++k)
+          wgmma_bf16<32>(h1, da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k), static_cast<uint32_t>((c | k) != 0));
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_reg_fence(h1);
+        release();
+      }
+      // bias + GELU + bf16 (the GEMM's EPI_GELU_BF16 epilogue) into the swizzled hidden chunk j & 1
+      uint8_t* hb = hid + (j & 1) * 8192;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int col = wg * 32 + i * 8 + 2 * (lane & 3);              // column inside the chunk
+        const float b0 = s_b1[j * 64 + col], b1 = s_b1[j * 64 + col + 1];
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int row = (t >> 5) * 16 + (lane >> 2) + hr * 8;
+          const uint32_t v = pack_bf16(gelu_erf(h1[4 * i + 2 * hr] + b0), gelu_erf(h1[4 * i + 2 * hr + 1] + b1));
+          *reinterpret_cast<uint32_t*>(hb + row * 128 + ((static_cast<uint32_t>(col >> 3) ^ static_cast<uint32_t>(row & 7)) << 4) +
+                                       (col & 7) * 2) = v;
         }
       }
-      constexpr float kHalfN = 0.5f * D;
-      const float md = sum * (1.0f / kHalfN);
-      const float my_mean = shift + md;
-      const float my_m2 = fmaxf(sq - sum * md, 0.0f);
-      s_stat[(quarter * 2 + w) * 32 + lane] = make_float2(my_mean, my_m2);
-      tmem_st_wait();
-      tc_fence_before();
-      asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");
-      tc_fence_after();
-      const float2 other = s_stat[(quarter * 2 + (w ^ 1)) * 32 + lane];
-      const float delta = other.x - my_mean;
-      const float mean = 0.5f * (my_mean + other.x);
-      const float var = ((my_m2 + other.y) + delta * delta * (0.5f * kHalfN)) * (1.0f / D);
-      const float rstd = 1.0f / sqrtf(var + p.eps);
-      if (lane == 0) bulk_wait_group_read<0>();
-      __syncwarp();
-      int k2 = 0;
-#pragma unroll 1
-      for (int c = w; c < D / 64; c += 2, ++k2) {
-        if (k2 >= GLN_SLABS) {
-          if (lane == 0) bulk_wait_group_read<GLN_SLABS - 1>();
-          __syncwarp();
-        }
-        uint8_t* slab = my_slabs + (k2 % GLN_SLABS) * 4096;
-        uint8_t* buf = slab + lane * 128;
+      fence_proxy_async_smem();                                        // generic stores -> wgmma operand reads
+      asm volatile("bar.sync 1, 256;" ::: "memory");                   // both halves of the chunk are in place
+      // ---- fc2: k-block j, this warpgroup's W2 column half (the other half's slot is released unread) ----
+      const uint64_t da = make_desc_k_sw128(smem_u32(hb));
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(trow + static_cast<uint32_t>(c * 64 + h * 32), v);
-          tmem_ld_wait();
-          const float* gg = s_gamma + c * 64 + h * 32;
-          const float* be = s_beta + c * 64 + h * 32;
+      for (int h = 0; h < 2; ++h) {
+        mbar_wait_mma(&full_bar[stage], phase);
+        if (h == wg) {
+          const uint64_t db = make_desc_k_sw128(smem_u32(ring + stage * Cfg::kSlotBytes));
+          wgmma_fence();
 #pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            float f[8];
-#pragma unroll
-            for (int t = 0; t < 8; ++t)
-              f[t] = (__uint_as_float(v[jj * 8 + t]) - mean) * rstd * gg[jj * 8 + t] + be[jj * 8 + t];
-            uint4 qq;
-            qq.x = pack_bf16(f[0], f[1]); qq.y = pack_bf16(f[2], f[3]);
-            qq.z = pack_bf16(f[4], f[5]); qq.w = pack_bf16(f[6], f[7]);
-            *reinterpret_cast<uint4*>(buf + ((static_cast<uint32_t>(h * 4 + jj) ^ sw) << 4)) = qq;
-          }
+          for (int k = 0; k < 4; ++k)
+            wgmma_bf16<D / 2>(acc, da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k),
+                              static_cast<uint32_t>((j | k) != 0));
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_reg_fence(acc);
         }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(&tmN, slab, c * 64, row0);
-          bulk_commit_group();
-        }
+        release();
       }
-      tc_fence_before();
-      if (lane == 0) bulk_wait_group_read<0>();          // slabs (= the xn region) free for the next tile
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(a2_empty);
-        mbar_arrive(xn_empty);
-      }
-      if (prof) e_ln += clock64() - t_ln;
-      tphase ^= 1u;
     }
-    if (prof) { p.prof[8] = e_a1; p.prof[9] = e_ld; p.prof[10] = e_rest; p.prof[11] = e_he; p.prof[12] = e_ln; }
-    if (ew < MLP_LN_WARPS && lane == 0) bulk_wait_group<0>();
+    gln_epilogue<D, D / 2, 2, false>(acc, x, xn_out, p.M, p.eps, m0, 0, wg, 0u, s_b2, s_gamma, s_beta, s_part, nullptr);
   }
-
-  tc_fence_before();
-  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();   // peer smem / barriers stay valid until all are done
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (CG == 2) tmem_dealloc_pair<512>(tmem_base);
-    else tmem_dealloc<512>(tmem_base);
-  }
+  // a CTA of a pair must not exit while its peer may still multicast into it or arrive on its barriers
+  if constexpr (CG == 2) cluster_sync_all();
 }
 
 }  // namespace pq

@@ -1,5 +1,5 @@
 """ctypes binding of include/parseq_b200.h.  The library is the product; this file only marshals
-pointers.  There is no fallback: if the shared library is missing or no sm_100 device exists,
+pointers.  There is no fallback: if the shared library is missing or no sm_90 device exists,
 construction raises."""
 from __future__ import annotations
 
@@ -27,7 +27,7 @@ EXPORTS = [
     "parseq_create", "parseq_destroy", "parseq_set_weight", "parseq_num_weights", "parseq_weight_key",
     "parseq_finalize", "parseq_forward", "parseq_forward_host", "parseq_forward_u8", "parseq_forward_host_u8",
     "parseq_postprocess", "parseq_encode", "parseq_decode", "parseq_head", "parseq_text_embed", "parseq_kernel_launches", "parseq_debug_int", "parseq_bench_tma_stream",
-    "parseq_set_option", "parseq_get_timing", "parseq_get_ar_profile", "parseq_last_error", "parseq_version", "parseq_gemm_bf16", "parseq_gemm_ln_bf16", "parseq_mlp_ln_bf16", "parseq_mlp_ln_bf16_prof", "parseq_layernorm_bf16",
+    "parseq_set_option", "parseq_get_timing", "parseq_get_ar_profile", "parseq_last_error", "parseq_version", "parseq_gemm_bf16", "parseq_gemm_ln_bf16", "parseq_mlp_ln_bf16", "parseq_layernorm_bf16",
     "parseq_enc_attention",
 ]
 
@@ -78,8 +78,6 @@ def load_library(path: Optional[str] = None):
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p]
     lib.parseq_mlp_ln_bf16.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p]
-    lib.parseq_mlp_ln_bf16_prof.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
-                                            C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.parseq_layernorm_bf16.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int,
                                           C.c_void_p, C.c_void_p, C.c_void_p]
     lib.parseq_enc_attention.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]

@@ -5,7 +5,7 @@
 (`test_step` -> `BatchResult`, base.py:36-44,112-143,179-180; `.device`).  `ParseqModel` mirrors the
 inner `strhub.models.parseq.model.PARSeq` (model.py:31-169): same parameter names (so released
 `parseq-*.pt` state_dicts load), `encode`, `forward(tokenizer, images, max_length)`, `decode_ar`,
-`refine_iters`, `max_label_length`.  All arithmetic happens in libparseq_b200.so (sm_100a CUDA);
+`refine_iters`, `max_label_length`.  All arithmetic happens in libparseq_b200.so (sm_90a CUDA);
 these classes only own the parameters and marshal pointers.  There is no CPU or eager-PyTorch
 fallback: calling forward with non-CUDA tensors raises.
 """
@@ -147,7 +147,7 @@ class _EngineModule(nn.Module):
     def engine(self) -> Engine:
         dev = self._device
         if dev.type != "cuda":
-            raise RuntimeError("parseq_b200 runs on a CUDA (sm_100a) device only; move the model with .to('cuda') "
+            raise RuntimeError("parseq_b200 runs on a CUDA (sm_90a, H100) device only; move the model with .to('cuda') "
                                "— there is no CPU fallback")
         idx = dev.index if dev.index is not None else torch.cuda.current_device()
         if self._engine is None or self._engine.device != idx:

@@ -8,11 +8,10 @@ from parseq_b200.engine import load_library, check
 lib = load_library()
 st = torch.cuda.current_stream().cuda_stream
 
-def run(M, N, K, mode, resid_inplace, cg, bn, tma, iters=30, stages=0):
+def run(M, N, K, mode, resid_inplace, cg, bn, iters=30, stages=0):
     check(lib, lib.parseq_set_option(None, b"gemm_stages", stages))
     check(lib, lib.parseq_set_option(None, b"cta_group", cg))
     check(lib, lib.parseq_set_option(None, b"block_n", bn))
-    check(lib, lib.parseq_set_option(None, b"tma_epilogue", tma))
     A = torch.randn((M, K), device="cuda").bfloat16()
     W = (torch.randn((N, K), device="cuda") * 0.02).bfloat16()
     bias = torch.randn((N,), device="cuda")
@@ -32,18 +31,18 @@ def run(M, N, K, mode, resid_inplace, cg, bn, tma, iters=30, stages=0):
     return us, 2.0 * M * N * K / us / 1e6
 
 M = int(sys.argv[1]) if len(sys.argv) > 1 else 65536
-print("shape                mode        cg bn  tma |    us     TF/s")
+print("shape                mode        cg bn  |    us     TF/s")
 cases = [("qkv", 1152, 384, 1, False), ("proj", 384, 384, 0, True), ("fc1", 1536, 384, 2, False), ("fc2", 384, 1536, 0, True)]
 for name, N, K, mode, ri in cases:
-    for cg, bn, tma in [(1, 128, 1), (1, 192, 1), (1, 256, 1), (2, 256, 1)]:
+    for cg, bn in [(1, 128), (1, 192), (1, 256), (2, 256)]:
         if bn == 192 and N % 192: continue
-        us, tf = run(M, N, K, mode, ri, cg, bn, tma)
-        print(f"{name:5s} N={N:5d} K={K:5d} mode={mode} inplace={int(ri)} cg={cg} bn={bn:3d} tma={tma} | {us:8.1f} {tf:7.1f}")
+        us, tf = run(M, N, K, mode, ri, cg, bn)
+        print(f"{name:5s} N={N:5d} K={K:5d} mode={mode} inplace={int(ri)} cg={cg} bn={bn:3d} | {us:8.1f} {tf:7.1f}")
 print("--- K sweep, N=1536 bf16 out (epilogue cost fixed, main loop ~ K)")
 for K in (64, 384, 4096):
-    for cg, bn, tma in [(1, 128, 1), (1, 256, 1)]:
-        us, tf = run(M, 1536, K, 1, False, cg, bn, tma, iters=15)
-        print(f"K={K:5d} cg={cg} bn={bn:3d} tma={tma} | {us:8.1f} us {tf:7.1f} TF/s")
+    for cg, bn in [(1, 128), (1, 256)]:
+        us, tf = run(M, 1536, K, 1, False, cg, bn, iters=15)
+        print(f"K={K:5d} cg={cg} bn={bn:3d} | {us:8.1f} us {tf:7.1f} TF/s")
 print("--- operand-ring depth sweep (gemm_stages cap; full ring: bn256 -> 4, bn192 -> 4, bn128 -> 6)")
 for name, N, K, mode, ri in cases:
     for bn, depths in ((256, (2, 3, 4)), (128, (2, 3, 4, 6))):

@@ -35,7 +35,7 @@ for cg, pdl, split in ((1, 0, 1), (2, 0, 1), (1, 0, 2)):
     check(lib, lib.parseq_set_option(None, b"ln_cta_group", cg))
     check(lib, lib.parseq_set_option(None, b"pair_pdl", pdl))
     check(lib, lib.parseq_set_option(None, b"ln_split", split))
-    print(f"--- fused kernel: ln_cta_group={cg} pair_pdl={pdl} ln_split={split} (2 = column-split pair, gemm_ln2.cuh)", flush=True)
-    for M in (65536, 148 * 128 * 4):
+    print(f"--- fused kernel: ln_cta_group={cg} pair_pdl={pdl} ln_split={split} (2 = column-split pair)", flush=True)
+    for M in (65536, 132 * 128 * 4):
         for K in (384, 1536, 4096):
             run(M, K)

@@ -9,13 +9,13 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (sm_100a) GPU; run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a) GPU")
 
 
 def _has_gpu():
     try:
         import torch
-        return torch.cuda.is_available() and torch.cuda.get_device_capability(0)[0] == 10
+        return torch.cuda.is_available() and torch.cuda.get_device_capability(0) == (9, 0)
     except Exception:
         return False
 
@@ -23,7 +23,7 @@ def _has_gpu():
 def pytest_collection_modifyitems(config, items):
     if _has_gpu():
         return
-    skip = pytest.mark.skip(reason="no sm_100 GPU in this environment")
+    skip = pytest.mark.skip(reason="no sm_90 GPU in this environment")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

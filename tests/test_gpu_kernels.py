@@ -51,7 +51,7 @@ def test_gemm_f32_bias(lib, M, N, K):
 @pytest.mark.parametrize("cta_group,block_n", [(1, 64), (1, 128), (1, 256), (2, 128), (2, 192), (2, 256)])
 @pytest.mark.parametrize("M,N,K", [(700, 1536, 384), (8192, 1152, 384), (1000, 384, 1536), (130, 95, 384)])
 def test_gemm_tile_variants(lib, cta_group, block_n, M, N, K):
-    """Single-CTA tiles and CTA-pair (cta_group::2, UMMA M=256) tiles of every width, ragged M / N."""
+    """Single-CTA tiles and CTA-pair tiles (a cluster of two on 256 rows, W tile multicast) of every width, ragged M / N."""
     from parseq_b200.engine import check
     check(lib, lib.parseq_set_option(None, b"block_n", block_n))
     check(lib, lib.parseq_set_option(None, b"cta_group", cta_group))
@@ -153,7 +153,7 @@ def _gemm_ln(lib, A, W, bias, x, gamma, beta, eps):
 
 @pytest.fixture(params=[1, 2], ids=["full-row-cta", "column-split-pair"])
 def ln_split(request, lib):
-    """gemm_ln.cuh (one CTA owns full rows) / gemm_ln2.cuh (the columns of a tile split over a CTA pair; D = 384 only)."""
+    """gemm_ln.cuh: one CTA owns full rows / the columns of a tile split over a CTA pair (D = 384 only)."""
     from parseq_b200.engine import check
     check(lib, lib.parseq_set_option(None, b"ln_split", request.param))
     yield request.param
@@ -191,7 +191,7 @@ def test_gemm_ln_fused(lib, ln_split, M, D, K):
 @pytest.mark.parametrize("M,D,K", [(128, 384, 384), (129, 384, 1536), (300, 384, 384), (148 * 128 + 77, 384, 1536), (65536, 384, 1536),
                                    (513, 192, 192), (2000, 192, 768)])
 def test_gemm_ln_cta_pair_equals_single_cta(lib, M, D, K):
-    """The fused GEMM + LayerNorm kernel on CTA pairs (cta_group::2, each CTA stages half of each W column half) returns
+    """The fused GEMM + LayerNorm kernel on CTA pairs (each CTA loads half of the W tile and multicasts it into both) returns
     the bits of the single-CTA kernel: same k order per output element, same epilogue.  Ragged M: the last pair tile has
     an empty second CTA / a partial first one."""
     from parseq_b200.engine import check
@@ -323,7 +323,7 @@ def test_layernorm(lib, D, eps):
     assert (y.float() == y32.bfloat16().float()).all()
 
 
-@pytest.mark.parametrize("impl", [1, 0], ids=["tcgen05", "mma_sync"])
+@pytest.mark.parametrize("impl", [1, 0], ids=["wgmma", "mma_sync"])
 @pytest.mark.parametrize("B,heads", [(1, 6), (5, 6), (3, 3), (2, 12), (300, 6)])
 def test_enc_attention(lib, B, heads, impl):
     from parseq_b200.engine import check
@@ -345,11 +345,11 @@ def test_enc_attention(lib, B, heads, impl):
     assert err <= 2 ** -7 * ref.abs().max().item() + 1e-3, err
 
 
-@pytest.mark.parametrize("impl", [1, 0], ids=["tcgen05", "mma_sync"])
+@pytest.mark.parametrize("impl", [1, 0], ids=["wgmma", "mma_sync"])
 @pytest.mark.parametrize("B,heads,T", [(2, 6, 196), (3, 12, 240), (1, 3, 130), (2, 6, 64), (40, 6, 129), (2, 6, 256), (3, 3, 49)])
 def test_enc_attention_any_token_count(lib, B, heads, T, impl):
-    """Geometries that do not fill one 128-row tile per image: tcgen05 kernel with two key blocks and one CTA per
-    (image, head, 128-query tile) over 3D tensor maps, and the masked two-pass mma.sync kernel."""
+    """Geometries that do not fill one 128-row tile per image: the wgmma kernel with 128 or 256 keys per tile and one
+    CTA per (image, head, 128-query tile), and the masked two-pass mma.sync kernel."""
     from parseq_b200.engine import check
     check(lib, lib.parseq_set_option(None, b"attn_impl", impl))
     d = 64

@@ -1,4 +1,4 @@
-"""End-to-end parity of the CUDA engine (strhub-compatible module -> C ABI -> sm_100a kernels) with
+"""End-to-end parity of the CUDA engine (strhub-compatible module -> C ABI -> sm_90a kernels) with
   (a) the committed golden outputs of the reference's own modules (tests/golden, fp32), and
   (b) the CPU oracle recomputed here on the same seeded inputs.
 
@@ -54,7 +54,7 @@ def _decisions_ok(engine_logits, ref_logits, tau):
 CASES = sorted(p for p in glob.glob(os.path.join(GOLDEN, "*.pt")) if not os.path.basename(p).startswith(("filtered", "vitstr")))
 
 
-# The residual-GEMM + LayerNorm fusion (gemm_ln.cuh) is selected by batch size (it needs >= 2 x 148 row tiles); the
+# The residual-GEMM + LayerNorm fusion (gemm_ln.cuh) is selected by batch size (it needs >= 2 x 132 row tiles); the
 # goldens are small batches, so every case runs twice: engine default (N-split GEMM + LayerNorm kernels here) and with the
 # fused kernel forced ("fuse_ln" = 7).  D = 768 has no fused variant and runs once.
 @pytest.mark.parametrize("fuse", [None, 7], ids=["default", "fused_ln"])
@@ -129,6 +129,9 @@ def test_free_running_ids_bit_identical_on_margin_filtered_set(name, mode):
     from parseq_b200.weights import synth_images, state_dict_digest
     path = os.path.join(GOLDEN, name + ".pt")
     blob = torch.load(path, weights_only=False)
+    if "logits_tail" in blob:                   # the larger sets keep the rest of their logits in a second file (< 1 MB each)
+        tail = torch.load(os.path.join(GOLDEN, blob["logits_tail"]), weights_only=False)["logits"]
+        blob["logits"] = torch.cat([blob["logits"], tail])
     cfg, sd, m = _model(blob["experiment"], blob["weight_seed"], decode_ar=blob["decode_ar"],
                         refine_iters=blob["refine_iters"])
     assert state_dict_digest(sd) == blob["sd_digest"]
@@ -279,7 +282,7 @@ def test_host_entry_points_equal_device_entry_points(B):
 
 
 def test_cta_pair_rows_equal_single_cta_rows():
-    """GEMMs with K >= 768 and >= 1024 rows run on CTA pairs (cta_group::2); the same images in a batch small enough for
+    """GEMMs with K >= 768 and >= 1024 rows run on CTA pairs (W tile multicast); the same images in a batch small enough for
     the single-CTA tiles, or with the pair forced off, give identical bits (D = 768 config, encoder output)."""
     from parseq_b200.weights import synth_images
     cfg, sd, m = _model("parseq-base-48x160", 4)

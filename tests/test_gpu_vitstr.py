@@ -1,4 +1,4 @@
-"""GPU: ViTSTR (SURVEY.md 8f rank 3) through the strhub-compatible module -> C ABI -> the same sm_100a encoder kernels,
+"""GPU: ViTSTR (SURVEY.md 8f rank 3) through the strhub-compatible module -> C ABI -> the same sm_90a encoder kernels,
 against the golden outputs of the reference's own strhub.models.vitstr.model.ViTSTR and the CPU oracle.
 Tolerances: the bf16-operand contract of tests/test_gpu_parity.py (TOL_FP32_MAX / TOL_FP32_MEAN / TAU)."""
 import glob

@@ -42,7 +42,8 @@ typedef struct parseq_config {
   int32_t enc_num_heads, enc_mlp_ratio, enc_depth;
   int32_t dec_num_heads, dec_mlp_ratio, dec_depth;   /* dec_depth must be 1 (all reference configs) */
   int32_t max_label_length;              /* 25 -> 26 decode positions */
-  int32_t num_tokens;                    /* 97: EOS=0, chars 1..94, BOS=95, PAD=96 (data/utils.py:102-111) */
+  int32_t num_tokens;                    /* 97: EOS=0, chars 1..94, BOS=95, PAD=96 (data/utils.py:102-111); 4..16386
+                                            (at most 16384 head classes, e.g. CJK charsets) */
   int32_t max_batch;                     /* images per super-chunk / CUDA graph (workspace sizing); 0 = 512 */
   int32_t device;                        /* CUDA device ordinal */
   int32_t arch;                          /* 0: PARSeq (parseq/model.py); 1: ViTSTR (vitstr/model.py:14-28: the same ViT with
@@ -149,7 +150,7 @@ int64_t parseq_debug_int(parseq_engine* e, const char* name);
  * for parseq_get_timing; 0: off + clear), "block_n" (engine-independent GEMM tile override, tests), "fuse_ln" (bit 0: the attention-projection GEMM, bit 1: the fc2 GEMM
  * also produces the LayerNorm that follows it, used when the batch fills the machine at least twice with 128-row tiles; bit 2:
  * for any batch; default 3; 0: separate LayerNorm kernels), "ar_kernel" (AR loop: 2 = cluster-owned persistent kernel,
- * default; 1 = grid-barrier persistent kernel; 0 = chain of separate kernels), "fuse_mlp" (1: fc1 + GELU + fc2 + residual +
+ * default; 1 = grid-barrier persistent kernel, at most 128 head classes; 0 = chain of separate kernels), "fuse_mlp" (1: fc1 + GELU + fc2 + residual +
  * LayerNorm of an encoder block in one kernel where fuse_ln bit 1 applies - bit-identical results, default 0), "attn_impl"
  * (encoder attention: 0 = mma.sync kernels, default; 1 = wgmma kernel), "cta_group" / "ln_cta_group" / "mlp_cta_group"
  * (0 auto, 1 single CTA, 2 CTA pair sharing the weight tiles by TMA multicast: GEMM / fused GEMM+LayerNorm / one-kernel

@@ -17,7 +17,12 @@
 //     normalised bf16 rows, which are the A operand of the next projection;
 //   * linear2 is split over K (each CTA multiplies the hidden slice it just produced), partial sums are
 //     scattered to the column owners and added in fixed order (deterministic, batch-invariant);
-//   * the character head runs redundantly in every CTA, so every CTA derives the same greedy token locally.
+//   * the character head runs redundantly in every CTA, so every CTA derives the same greedy token locally - up to 96
+//     classes.  Larger heads (WIDE, > 128 classes) are split over the cluster: CTA k owns the classes
+//     [k*Cs, (k+1)*Cs), streams only that slice of head.weight through the ring in [128 x 64] boxes, stores its logits
+//     straight from the MMA fragments and exchanges one (max, lowest index) pair per row through distributed shared
+//     memory; every CTA merges the pairs in rank order (= class order), so all derive the same token, the first maximum
+//     as torch.argmax picks it.
 // Numerics: bf16 tensor-core operands, fp32 accumulation, fp32 residual / LayerNorm / softmax statistics, exact-erf
 // GELU polynomial (ptx.cuh) - the rounding points of the v1 kernel and of the multi-kernel path.
 #pragma once
@@ -135,7 +140,8 @@ constexpr size_t dec_ar2_smem_bytes() { return static_cast<size_t>(A2Cfg<D, MT, 
 
 // ------------------------------------------------------------------------------------------------------------------
 // TMA ring: a static per-step program of slot fills; one thread issues, everybody consumes in program order.
-template <int D, int MT, int CS>
+// WIDE: the head segment is this CTA's class slice, ceil(Cs / 128) chunks of KT [128 x 64] boxes.
+template <int D, int MT, int CS, bool WIDE = false>
 struct A2Ring {
   using Cfg = A2Cfg<D, MT, CS>;
   uint8_t* slots;
@@ -147,10 +153,13 @@ struct A2Ring {
   int items_per_step, total;
   int seg_b, seg_c, seg_d, seg_e, seg_f, seg_g;   // first item index of each segment
   int cons, prod;
+  int head_row0, head_rows;            // WIDE: first class of this CTA's slice, number of classes C
 
   // n_kv_units: (image, k-block) cross-attention units of this CTA: n_own * KT, or 0 / 1 in head-split mode
+  // head_chunks (WIDE): 128-class chunks of this CTA's slice
   __device__ void init(uint8_t* slots_, uint64_t* full_, const DecAr2Maps* maps_, int rank_, int n_own_, int img0_, int tbox_,
-                       int tb_, int T_, int steps, int n_kv_units, int hs_row_, int hs_kb_) {
+                       int tb_, int T_, int steps, int n_kv_units, int hs_row_, int hs_kb_, int head_chunks = 0,
+                       int head_row0_ = 0, int head_rows_ = 0) {
     slots = slots_; full = full_; maps = maps_; rank = rank_; n_own = n_own_; img0 = img0_; tbox = tbox_; tb = tb_; T = T_;
     hs_row = hs_row_; hs_kb = hs_kb_;
     seg_b = Cfg::NSL_S;
@@ -159,7 +168,12 @@ struct A2Ring {
     seg_e = seg_d + Cfg::NSL_S;
     seg_f = seg_e + Cfg::NCH1 * Cfg::KT;
     seg_g = seg_f + Cfg::NCH2 * Cfg::KT2;
-    items_per_step = seg_g + Cfg::KT;
+    if constexpr (WIDE) {
+      items_per_step = seg_g + head_chunks * Cfg::KT;
+      head_row0 = head_row0_; head_rows = head_rows_;
+    } else {
+      items_per_step = seg_g + Cfg::KT;
+    }
     total = items_per_step * steps;
     cons = 0; prod = 0;
   }
@@ -205,8 +219,17 @@ struct A2Ring {
       tma_load_2d(dst, &maps->w2, bar, rank * Cfg::MS + kb * 64, c * Cfg::NC2);
       return;
     }
-    mbar_expect_tx(bar, 96 * 128);       // head: [96 x 64] (row 95.. zero-filled by the tensor map bounds)
-    tma_load_2d(dst, &maps->wh, bar, (it - seg_g) * 64, 0);
+    if constexpr (WIDE) {                // head chunk c: classes [head_row0 + 128 c, +128), k-block kb
+      const int j = it - seg_g, c = j / Cfg::KT, kb = j % Cfg::KT;
+      // rows >= C are zero-filled by the tensor map bounds; a chunk that starts past C (an empty tail slice) reads
+      // in-bounds rows instead and none of its columns is used
+      const int row = head_row0 + c * 128;
+      mbar_expect_tx(bar, 128 * 128);
+      tma_load_2d(dst, &maps->wh, bar, kb * 64, row < head_rows ? row : head_rows - 1);
+    } else {
+      mbar_expect_tx(bar, 96 * 128);     // head: [96 x 64] (row 95.. zero-filled by the tensor map bounds)
+      tma_load_2d(dst, &maps->wh, bar, (it - seg_g) * 64, 0);
+    }
   }
   // ---- producer warp (warp 8): issues every item in program order; item i >= NSLOT waits on the named barrier of its
   //      slot until the 256 consumer threads have arrived there after item i - NSLOT
@@ -274,9 +297,10 @@ __device__ __forceinline__ void mma_box(float (&acc)[NTW][4], const uint8_t* ati
 
 // HS: head-split cross-attention (launch-wide: rows per cluster x k-blocks <= cluster size; see below).  A template flag
 // so that the throughput instantiations carry none of its registers / branches.
-template <int D, int MT, int CS, bool HS = false>
-__global__ void __launch_bounds__(A2_LAUNCH_THREADS, 1)
-dec_ar2_kernel(const __grid_constant__ DecAr2Maps maps, const DecAr2Params p) {
+// WIDE: the class-sliced head for C > 128 (see the top of the file); `maps.wh` then has [128 x 64] boxes.  The body is
+// shared by two kernels, dec_ar2_kernel (WIDE = false) and dec_ar2_wide_kernel (WIDE = true).
+template <int D, int MT, int CS, bool HS, bool WIDE>
+__device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr2Params p) {
   using Cfg = A2Cfg<D, MT, CS>;
   constexpr int ROWS = Cfg::ROWS, DS = Cfg::DS, KT = Cfg::KT, KT2 = Cfg::KT2, MS = Cfg::MS, MH = Cfg::MH, G = Cfg::G,
                 OWN = Cfg::OWN, H = Cfg::H;
@@ -332,8 +356,12 @@ dec_ar2_kernel(const __grid_constant__ DecAr2Maps maps, const DecAr2Params p) {
   const int hs_row = (hs && rank < nrows * KT) ? rank / KT : -1;
   const int hs_kb = hs ? rank % KT : 0;
   const int c_own = hs ? (hs_row >= 0 ? 1 : 0) : n_own;             // cross-attention passes of this CTA
-  A2Ring<D, MT, CS> ring;
-  ring.init(s_ring, s_bar, &maps, rank, n_own, img0, p.tbox, p.tb, p.T, p.L, hs ? c_own : n_own * KT, hs ? hs_row : -1, hs_kb);
+  A2Ring<D, MT, CS, WIDE> ring;
+  // WIDE: classes per CTA, a multiple of 8 (whole n8 tiles); the last slices may be short or empty
+  const int h_cs = WIDE ? (((p.C + CS - 1) / CS + 7) & ~7) : 0;
+  const int h_chunks = (h_cs + 127) / 128;
+  ring.init(s_ring, s_bar, &maps, rank, n_own, img0, p.tbox, p.tb, p.T, p.L, hs ? c_own : n_own * KT, hs ? hs_row : -1, hs_kb,
+            h_chunks, rank * h_cs, p.C);
   __syncthreads();
   cluster_sync_relacq();              // every CTA of the cluster is running (remote stores are legal) and zero-filled
 
@@ -366,7 +394,12 @@ dec_ar2_kernel(const __grid_constant__ DecAr2Maps maps, const DecAr2Params p) {
       csync_p();                                                   // (8)
       csync_p();                                                   // (9)
       csync_p();                                                   // (10)
-      ring.produce(KT);                                            // P8: head
+      if constexpr (WIDE) {
+        ring.produce(h_chunks * KT);                               // P8: this CTA's head slice
+        csync_p();                                                 // (11) argmax pairs exchanged
+      } else {
+        ring.produce(KT);                                          // P8: head
+      }
     }
     if (pending) cluster_wait_acquire();
   } else {
@@ -895,7 +928,97 @@ dec_ar2_kernel(const __grid_constant__ DecAr2Maps maps, const DecAr2Params p) {
     cluster_sync_relacq();                                                                            // (10) LN3(y) gathered
     A2_PROF(14);
     // ================= P8: logits[:, step] = head(LN3(y)) in every CTA; greedy token =================
-    {
+    if constexpr (WIDE) {
+      // class slice [c_lo, c_hi) of this CTA, 128 classes per chunk; every chunk multiplies all rows in the k order of
+      // mma_box; logits leave from the fragments; a running (max, lowest index) per (thread, row)
+      constexpr int NTH = 16;                                           // 128 columns
+      constexpr int NTWH = (((NTH + G - 1) / G) + 1) & ~1;
+      const int c_lo = rank * h_cs;
+      const int c_hi = (c_lo + h_cs < p.C) ? (c_lo + h_cs) : p.C;
+      const int r0 = mi * 16 + g;
+      float* lrow0 = p.logits + (static_cast<long long>(img0 + r0) * p.L + step) * p.C;
+      float* lrow1 = p.logits + (static_cast<long long>(img0 + r0 + 8) * p.L + step) * p.C;
+      const bool st0 = r0 < nrows, st1 = r0 + 8 < nrows;
+      float best0 = -INFINITY, best1 = -INFINITY;
+      int bi0 = 0x7fffffff, bi1 = 0x7fffffff;
+      for (int hc = 0; hc < h_chunks; ++hc) {
+        float acc[NTWH][4];
+#pragma unroll
+        for (int j = 0; j < NTWH; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+        for (int kb = 0; kb < KT; ++kb) {
+          const uint8_t* slot = ring.wait();
+          mma_box<NTWH>(acc, s_a1 + kb * ROWS * 128, mi, slot, ng * NTWH, lane);
+          ring.release();
+        }
+#pragma unroll
+        for (int j = 0; j < NTWH; ++j) {
+          const int nt = ng * NTWH + j;
+          if (nt < NTH) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {                               // columns in increasing order per thread
+              const int c = c_lo + hc * 128 + nt * 8 + 2 * t + e;
+              if (c < c_hi) {
+                const float b = __ldg(p.bh + c);
+                const float v0 = acc[j][e] + b, v1 = acc[j][2 + e] + b;
+                if (st0) lrow0[c] = v0;
+                if (st1) lrow1[c] = v1;
+                if (v0 > best0) { best0 = v0; bi0 = c; }
+                if (v1 > best1) { best1 = v1; bi1 = c; }
+              }
+            }
+          }
+        }
+      }
+      // quad (same rows, interleaved columns), then the G warps of the m16 tile: ties go to the lower index
+#pragma unroll
+      for (int o = 1; o < 4; o <<= 1) {
+        const float ov0 = __shfl_xor_sync(0xffffffffu, best0, o), ov1 = __shfl_xor_sync(0xffffffffu, best1, o);
+        const int oi0 = __shfl_xor_sync(0xffffffffu, bi0, o), oi1 = __shfl_xor_sync(0xffffffffu, bi1, o);
+        if (ov0 > best0 || (ov0 == best0 && oi0 < bi0)) { best0 = ov0; bi0 = oi0; }
+        if (ov1 > best1 || (ov1 == best1 && oi1 < bi1)) { best1 = ov1; bi1 = oi1; }
+      }
+      float* s_hv = s_log;                                              // [ROWS][G] warp maxima (P is dead here)
+      int* s_hi = reinterpret_cast<int*>(s_log + ROWS * G);
+      if (t == 0) {
+        s_hv[r0 * G + ng] = best0; s_hi[r0 * G + ng] = bi0;
+        s_hv[(r0 + 8) * G + ng] = best1; s_hi[(r0 + 8) * G + ng] = bi1;
+      }
+      a2_csync();
+      // this CTA's pair of row r -> s_st[rank][r] of every CTA (s_st is free: the LN3 statistics were read before (10))
+      if (tid < ROWS) {
+        float bv = s_hv[tid * G];
+        int bx = s_hi[tid * G];
+#pragma unroll
+        for (int w = 1; w < G; ++w) {
+          const float v = s_hv[tid * G + w];
+          const int x = s_hi[tid * G + w];
+          if (v > bv || (v == bv && x < bx)) { bv = v; bx = x; }
+        }
+        const uint32_t off = smem_u32(&s_st[rank * ROWS + tid]);
+#pragma unroll
+        for (int pe = 0; pe < CS; ++pe) st_cluster_v2f(mapa_cluster(off, static_cast<uint32_t>(pe)), bv, __int_as_float(bx));
+      }
+      cluster_sync_relacq();                                                                          // (11) pairs exchanged
+      // slices ascend with the rank: a strict > in rank order keeps the first maximum; the same result in every CTA
+      if (tid < nrows) {
+        const int r = tid;
+        const long long b = img0 + r;
+        float bv = s_st[r].x;
+        int bx = __float_as_int(s_st[r].y);
+#pragma unroll
+        for (int k = 1; k < CS; ++k) {
+          const float2 s = s_st[k * ROWS + r];
+          if (s.x > bv) { bv = s.x; bx = __float_as_int(s.y); }
+        }
+        if (step + 1 < p.L) {
+          int v = bx;
+          if (p.forced != nullptr) v = p.forced[b * p.forced_ld + step + 1];
+          s_ids[r * 32 + step + 1] = v;
+          if ((r % CS) == rank) p.ids[b * p.ids_ld + step + 1] = v;     // one CTA stores the row
+        }
+      }
+      a2_csync();
+    } else {
       constexpr int NTH = 12;                                           // 96 columns
       constexpr int NTWH = (((NTH + G - 1) / G) + 1) & ~1;
       float acc[NTWH][4];
@@ -952,6 +1075,17 @@ dec_ar2_kernel(const __grid_constant__ DecAr2Maps maps, const DecAr2Params p) {
 #undef A2_PROF4
   }
   cluster_sync_relacq();       // no CTA exits while a peer may still address its shared memory
+}
+
+template <int D, int MT, int CS, bool HS = false>
+__global__ void __launch_bounds__(A2_LAUNCH_THREADS, 1)
+dec_ar2_kernel(const __grid_constant__ DecAr2Maps maps, const DecAr2Params p) {
+  dec_ar2_body<D, MT, CS, HS, false>(maps, p);
+}
+template <int D, int MT, int CS, bool HS = false>
+__global__ void __launch_bounds__(A2_LAUNCH_THREADS, 1)
+dec_ar2_wide_kernel(const __grid_constant__ DecAr2Maps maps, const DecAr2Params p) {
+  dec_ar2_body<D, MT, CS, HS, true>(maps, p);
 }
 
 // ------------------------------------------------------------------------------------------------------------------

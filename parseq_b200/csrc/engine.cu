@@ -24,6 +24,8 @@
 
 namespace {
 
+constexpr int kMaxHeadClasses = 16384;    // num_tokens - 2 (parseq_create)
+
 thread_local std::string g_last_error;
 
 int fail(int code, const std::string& msg) {
@@ -203,20 +205,27 @@ int ln_head_argmax_launch(const LaunchOpts& lo, const float* y, const float* g, 
   }
 }
 
-template <int D, int MT, int CS>
+// the cluster AR kernel of a head width: WIDE (> 128 classes) is the class-sliced head
+template <int D, int MT, int CS, bool HS, bool WIDE>
+constexpr auto ar2_kernel() {
+  if constexpr (WIDE) return pq::dec_ar2_wide_kernel<D, MT, CS, HS>;
+  else return pq::dec_ar2_kernel<D, MT, CS, HS>;
+}
+template <int D, int MT, int CS, bool WIDE>
 int ar2_attr() {
-  PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar2_kernel<D, MT, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  PQ_CUDA(cudaFuncSetAttribute(ar2_kernel<D, MT, CS, false, WIDE>(), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                static_cast<int>(pq::dec_ar2_smem_bytes<D, MT, CS>())));
   if constexpr (MT == 1 && CS == 8 && D / 64 <= CS)      // head-split variant for tiny batches
-    PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar2_kernel<D, MT, CS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    PQ_CUDA(cudaFuncSetAttribute(ar2_kernel<D, MT, CS, true, WIDE>(), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  static_cast<int>(pq::dec_ar2_smem_bytes<D, MT, CS>())));
   return PARSEQ_OK;
 }
+template <bool WIDE>
 int ar2_set_attributes() {
-  PQ_TRY((ar2_attr<192, 1, 8>())); PQ_TRY((ar2_attr<192, 2, 8>())); PQ_TRY((ar2_attr<384, 1, 8>())); PQ_TRY((ar2_attr<384, 2, 8>()));
-  PQ_TRY((ar2_attr<768, 1, 8>()));
-  PQ_TRY((ar2_attr<192, 1, 6>())); PQ_TRY((ar2_attr<192, 2, 6>())); PQ_TRY((ar2_attr<384, 1, 6>())); PQ_TRY((ar2_attr<384, 2, 6>()));
-  PQ_TRY((ar2_attr<768, 1, 6>()));
+  PQ_TRY((ar2_attr<192, 1, 8, WIDE>())); PQ_TRY((ar2_attr<192, 2, 8, WIDE>())); PQ_TRY((ar2_attr<384, 1, 8, WIDE>()));
+  PQ_TRY((ar2_attr<384, 2, 8, WIDE>())); PQ_TRY((ar2_attr<768, 1, 8, WIDE>()));
+  PQ_TRY((ar2_attr<192, 1, 6, WIDE>())); PQ_TRY((ar2_attr<192, 2, 6, WIDE>())); PQ_TRY((ar2_attr<384, 1, 6, WIDE>()));
+  PQ_TRY((ar2_attr<384, 2, 6, WIDE>())); PQ_TRY((ar2_attr<768, 1, 6, WIDE>()));
   return PARSEQ_OK;
 }
 
@@ -247,7 +256,8 @@ int init_kernel_attributes() {
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar_kernel<384, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pq::dec_ar_smem_bytes<384>())));
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar_kernel<768, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pq::dec_ar_smem_bytes<768>())));
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar_kernel<768, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pq::dec_ar_smem_bytes<768>())));
-  PQ_TRY(ar2_set_attributes());
+  PQ_TRY(ar2_set_attributes<false>());
+  PQ_TRY(ar2_set_attributes<true>());
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ln_head_argmax_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, 120 * 1024));
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ln_head_argmax_kernel<384>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ln_head_argmax_kernel<768>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
@@ -892,6 +902,14 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
     PQ_TRY(layernorm(e, sg.y, "decoder.norm", 1e-5f, M, sg.yn, nullptr, st));
     PQ_TRY(gemm(e, sg.yn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, pq::EPI_F32, 1.0f, nullptr, 0, 0,
                 logits_out, logits_ld, st));
+  } else if (e->C > 128) {
+    // single-query tail of a head too large for the fused kernel's shared memory: LayerNorm, the wgmma GEMM and the
+    // greedy argmax (one AR step, nq == 1: row b of the step's logits is at logits_out + b * logits_ld)
+    PQ_TRY(layernorm(e, sg.y, "decoder.norm", 1e-5f, M, sg.yn, nullptr, st));
+    PQ_TRY(gemm(e, sg.yn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, pq::EPI_F32, 1.0f, nullptr, 0, 0,
+                logits_out, logits_ld, st));
+    if (ids_dst != nullptr)
+      PQ_TRY(argmax_rows(e, logits_out, static_cast<int>(logits_ld / e->C), B, nq, 0, ids_dst, 32, dst_off, forced, forced_ld, st));
   } else {
     TimedScope ts(e, st, CAT_DEC_GEMM, 2.0 * M * e->C * D);
     PQ_TRY(ln_head_argmax_launch(e->lo, sg.y, e->wf("decoder.norm.weight"), e->wf("decoder.norm.bias"), 1e-5f, e->wb("head.weight"),
@@ -955,9 +973,12 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
 
 
 // ---- cluster-owned AR kernel (dec_ar2.cuh) ----
+// Heads of <= 96 classes run redundantly in every CTA; > 128 classes take the class-sliced head (WIDE); 97..128 classes
+// stay on the grid-barrier kernel.
 bool ar2_supported(const parseq_engine* e) {
-  return e->arch == 0 && e->cfg.dec_mlp_ratio == 4 && e->C <= 96 && e->T <= 256 && e->dh_dec == 32;
+  return e->arch == 0 && e->cfg.dec_mlp_ratio == 4 && (e->C <= 96 || e->C > 128) && e->T <= 256 && e->dh_dec == 32;
 }
+bool ar2_wide(const parseq_engine* e) { return e->C > 128; }
 // weight descriptors: once per weight set (parseq_finalize); K/V cache descriptor: once per workspace
 int ar2_build_maps(parseq_engine* e) {
   const int D = e->D;
@@ -972,7 +993,7 @@ int ar2_build_maps(parseq_engine* e) {
     PQ_TRY(make_tmap(&m.wo_c, e->w(Ly + "cross_attn.out_proj.weight"), 2, D, D, D, 64, DS));
     PQ_TRY(make_tmap(&m.w1, e->w(Ly + "linear1.weight"), 2, e->Md, D, D, 64, NC1));
     PQ_TRY(make_tmap(&m.w2, e->w(Ly + "linear2.weight"), 2, D, e->Md, e->Md, 64, NC2));
-    PQ_TRY(make_tmap(&m.wh, e->w("head.weight"), 2, e->C, D, D, 64, 96));
+    PQ_TRY(make_tmap(&m.wh, e->w("head.weight"), 2, e->C, D, D, 64, ar2_wide(e) ? 128 : 96));
     const int tbox = e->T <= 64 ? 64 : 128;
     const long long kv_rows = 1ll * e->max_batch * e->T;     // column-blocked cache [2D/64][kv_rows][64]
     PQ_TRY(make_tmap3d(&m.ckv, e->ckv, 64, kv_rows, 2 * D / 64, 64, 64 * kv_rows, 64, tbox));
@@ -994,8 +1015,8 @@ void ar2_config(parseq_engine* e, cudaLaunchConfig_t& cfg, cudaLaunchAttribute* 
   cfg.attrs = attr;
   cfg.numAttrs = 1;
 }
-template <int D, int MT, int CS>
-int ar2_launch(parseq_engine* e, const pq::DecAr2Params& p, int ncl, cudaStream_t st) {
+template <int D, int MT, int CS, bool WIDE>
+int ar2_launch_t(parseq_engine* e, const pq::DecAr2Params& p, int ncl, cudaStream_t st) {
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[1];
   ar2_config<D, MT, CS>(e, cfg, attr, ncl, st);
@@ -1004,12 +1025,16 @@ int ar2_launch(parseq_engine* e, const pq::DecAr2Params& p, int ncl, cudaStream_
     // so few images per cluster that (images x head pairs) fit its CTAs: every CTA takes one (image, head pair) of the
     // cross-attention instead of whole images (bs = 1: 9 -> 2.5 us per step; same bits per head)
     if (p.per * (D / 64) <= CS) {
-      PQ_CUDA(cudaLaunchKernelEx(&cfg, pq::dec_ar2_kernel<D, MT, CS, true>, e->ar2_maps[0], p));
+      PQ_CUDA(cudaLaunchKernelEx(&cfg, ar2_kernel<D, MT, CS, true, WIDE>(), e->ar2_maps[0], p));
       return PARSEQ_OK;
     }
   }
-  PQ_CUDA(cudaLaunchKernelEx(&cfg, pq::dec_ar2_kernel<D, MT, CS>, e->ar2_maps[CS == 6 ? 1 : 0], p));
+  PQ_CUDA(cudaLaunchKernelEx(&cfg, ar2_kernel<D, MT, CS, false, WIDE>(), e->ar2_maps[CS == 6 ? 1 : 0], p));
   return PARSEQ_OK;
+}
+template <int D, int MT, int CS>
+int ar2_launch(parseq_engine* e, const pq::DecAr2Params& p, int ncl, cudaStream_t st) {
+  return ar2_wide(e) ? ar2_launch_t<D, MT, CS, true>(e, p, ncl, st) : ar2_launch_t<D, MT, CS, false>(e, p, ncl, st);
 }
 // Clusters of this instantiation that can be co-resident, as the occupancy query answers for this device.  A cluster
 // lives inside one GPC, so clusters of 8 can leave SMs of a GPC idle and clusters of 6 may pack more SMs; a batch that
@@ -1022,7 +1047,10 @@ int ar2_max_clusters(parseq_engine* e) {
   cudaLaunchAttribute attr[1];
   ar2_config<D, MT, CS>(e, cfg, attr, e->lo.sm_count / CS, nullptr);
   int n = 0;
-  if (cudaOccupancyMaxActiveClusters(&n, pq::dec_ar2_kernel<D, MT, CS>, &cfg) != cudaSuccess || n <= 0) {
+  // (the cache is per engine, and so is the head width)
+  const cudaError_t qe = ar2_wide(e) ? cudaOccupancyMaxActiveClusters(&n, ar2_kernel<D, MT, CS, false, true>(), &cfg)
+                                     : cudaOccupancyMaxActiveClusters(&n, ar2_kernel<D, MT, CS, false, false>(), &cfg);
+  if (qe != cudaSuccess || n <= 0) {
     cudaGetLastError();
     n = (CS == 8) ? (e->lo.sm_count / 10) : 1;   // unknown: a conservative guess for 8, "do not use" for 6
   }
@@ -1107,6 +1135,7 @@ int ar_decode(parseq_engine* e, const parseq_forward_args* a, int b0, int B, int
     }
     return PARSEQ_OK;
   }
+  if (e->C > 128) return fail(PARSEQ_ERR_UNSUPPORTED, "ar_kernel = 1 (grid-barrier AR kernel) covers at most 128 head classes");
   PQ_CUDA(cudaMemsetAsync(e->ar_bar, 0, 64, st));
   pq::DecArParams p;
   p.B = B; p.L = L; p.Md = e->Md; p.V = e->V; p.C = e->C; p.T = e->T; p.heads = e->cfg.dec_num_heads;
@@ -1198,7 +1227,8 @@ int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B,
     PQ_TRY(gemm(e, e->mem, D, Wkv, D, bkv, B * T, 2 * D, D, pq::EPI_BF16, 1.0f, nullptr, 0, 0, e->ckv, 2 * D, e->main,
                 1ll * e->max_batch * T));
   }
-  const bool ar_done = a->decode_ar && e->use_ar_kernel;
+  // a head of > 128 classes that the cluster kernel cannot take (e.g. dec_mlp_ratio != 4) runs the AR loop as a chain
+  const bool ar_done = a->decode_ar && e->use_ar_kernel && !(e->ar_impl == 2 && e->C > 128 && !ar2_supported(e));
   if (ar_done) {
     PQ_TRY(ar_decode(e, a, b0, B, L, logits, steps, e->main));
     if (a->refine_iters == 0) {      // nothing left for the chains but the final argmax
@@ -1354,10 +1384,11 @@ int parseq_create(const parseq_config* cfg, parseq_engine** out) {
   if (!vitstr && D != cfg->dec_num_heads * 32) return fail(PARSEQ_ERR_UNSUPPORTED, "decoder head_dim must be 32");
   if (cfg->max_label_length + 1 > 32) return fail(PARSEQ_ERR_UNSUPPORTED, "max_label_length must be <= 31");
   if (cfg->max_label_length < 0) return fail(PARSEQ_ERR_INVALID_ARG, "negative max_label_length");
-  // the head tiles of the decoder kernels hold one row of logits in 128 columns (charset_train of <= 126 characters;
-  // the reference's largest, 94_full, has 94)
-  if (cfg->num_tokens < 4 || cfg->num_tokens - 2 > 128)
-    return fail(PARSEQ_ERR_UNSUPPORTED, "num_tokens must be in [4, 130] (at most 128 head classes)");
+  // at most 16384 head classes (charset_train of <= 16383 characters): every index into the (position, token) K/V table
+  // [L * V, 2D] stays in int32 (32 * 16386 * 1536 < 2^31) and the table stays below 1.7 GB (DESIGN.md section 4)
+  if (cfg->num_tokens < 4 || cfg->num_tokens - 2 > kMaxHeadClasses)
+    return fail(PARSEQ_ERR_UNSUPPORTED, "num_tokens must be in [4, 16386] (at most 16384 head classes, charset_train of "
+                                        "at most 16383 characters)");
   if (cfg->enc_mlp_ratio < 1 || cfg->enc_depth < 1) return fail(PARSEQ_ERR_INVALID_ARG, "enc_mlp_ratio / enc_depth");
   // decoder MLP: 128-wide linear1 tiles and a 3-way split-K of linear2 in 64-element k-blocks
   if (!vitstr && (cfg->dec_mlp_ratio < 1 || (D * cfg->dec_mlp_ratio) % 384 != 0))
@@ -1863,6 +1894,9 @@ int parseq_set_option(parseq_engine* e, const char* name, int64_t value) {
   }
   if (n == "ar_kernel") {           // 0: AR loop as separate kernels, 1: grid-barrier kernel (dec_ar.cuh), 2: cluster kernel
     if (value < 0 || value > 2) return fail(PARSEQ_ERR_INVALID_ARG, "ar_kernel: 0 / 1 / 2");
+    if (value == 1 && e->C > 128)
+      return fail(PARSEQ_ERR_UNSUPPORTED, "ar_kernel = 1 (grid-barrier AR kernel) covers at most 128 head classes; "
+                                          "use ar_kernel 0 or 2");
     e->use_ar_kernel = value != 0;
     e->ar_impl = value == 1 ? 1 : 2;
     drop_graphs(e);

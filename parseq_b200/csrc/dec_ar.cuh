@@ -260,18 +260,13 @@ __device__ void dec_tile(const DecArParams& p, unsigned char* smem, const __nv_b
       if (m >= M) continue;                          // warp-uniform
       float* lrow = p.logits + (static_cast<long long>(m) * p.L + step) * p.C;
       float best = -INFINITY;
-      int bi = 0x7fffffff;
+      int bi = ARGMAX_NONE;
       for (int j = lane; j < N; j += 32) {
         const float v = s_log[r * 128 + j];
         lrow[j] = v;
-        if (v > best) { best = v; bi = j; }
+        argmax_scan(best, bi, v, j);
       }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
-      }
+      bi = argmax_finish(best, bi, s_log + r * 128, N, lane);
       if (lane == 0 && step + 1 < p.L) {
         int v = bi;
         if (p.forced != nullptr) v = p.forced[static_cast<long long>(m) * p.forced_ld + step + 1];

@@ -200,10 +200,10 @@ struct A2Ring {
         kv = j & 1;
         img = img0 + rank + CS * (j >> 1);
       }
+      // column-blocked cache [2D/64][max_batch][T][64] (engine.cu make_tmap_kv4d): keys t*128 .. of this image only;
+      // keys past T are zero-filled, and the fill counts towards the box's tx bytes
       mbar_expect_tx(bar, static_cast<uint32_t>(tbox * 128));
-      // column-blocked cache [2D/64][rows][64], row = image * T + key: one contiguous tbox x 128 B run (rows past the
-      // image's T keys belong to the next image or are out of bounds: masked by the softmax)
-      tma_load_3d(dst, &maps->ckv, bar, 0, img * T + t * 128, kv * Cfg::KT + kb);
+      tma_load_4d(dst, &maps->ckv, bar, 0, t * 128, img, kv * Cfg::KT + kb);
       return;
     }
     if (it < seg_e) { issue_slice(&maps->wo_c, it - seg_d, dst, bar); return; }
@@ -940,7 +940,7 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
       float* lrow1 = p.logits + (static_cast<long long>(img0 + r0 + 8) * p.L + step) * p.C;
       const bool st0 = r0 < nrows, st1 = r0 + 8 < nrows;
       float best0 = -INFINITY, best1 = -INFINITY;
-      int bi0 = 0x7fffffff, bi1 = 0x7fffffff;
+      int bi0 = ARGMAX_NONE, bi1 = ARGMAX_NONE;
       for (int hc = 0; hc < h_chunks; ++hc) {
         float acc[NTWH][4];
 #pragma unroll
@@ -962,21 +962,16 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
                 const float v0 = acc[j][e] + b, v1 = acc[j][2 + e] + b;
                 if (st0) lrow0[c] = v0;
                 if (st1) lrow1[c] = v1;
-                if (v0 > best0) { best0 = v0; bi0 = c; }
-                if (v1 > best1) { best1 = v1; bi1 = c; }
+                argmax_fold(best0, bi0, v0, c);
+                argmax_fold(best1, bi1, v1, c);
               }
             }
           }
         }
       }
-      // quad (same rows, interleaved columns), then the G warps of the m16 tile: ties go to the lower index
-#pragma unroll
-      for (int o = 1; o < 4; o <<= 1) {
-        const float ov0 = __shfl_xor_sync(0xffffffffu, best0, o), ov1 = __shfl_xor_sync(0xffffffffu, best1, o);
-        const int oi0 = __shfl_xor_sync(0xffffffffu, bi0, o), oi1 = __shfl_xor_sync(0xffffffffu, bi1, o);
-        if (ov0 > best0 || (ov0 == best0 && oi0 < bi0)) { best0 = ov0; bi0 = oi0; }
-        if (ov1 > best1 || (ov1 == best1 && oi1 < bi1)) { best1 = ov1; bi1 = oi1; }
-      }
+      // quad (same rows, interleaved columns), then the G warps of the m16 tile, in torch.argmax order (ptx.cuh)
+      argmax_shfl(best0, bi0, 1, 4);
+      argmax_shfl(best1, bi1, 1, 4);
       float* s_hv = s_log;                                              // [ROWS][G] warp maxima (P is dead here)
       int* s_hi = reinterpret_cast<int*>(s_log + ROWS * G);
       if (t == 0) {
@@ -989,17 +984,14 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
         float bv = s_hv[tid * G];
         int bx = s_hi[tid * G];
 #pragma unroll
-        for (int w = 1; w < G; ++w) {
-          const float v = s_hv[tid * G + w];
-          const int x = s_hi[tid * G + w];
-          if (v > bv || (v == bv && x < bx)) { bv = v; bx = x; }
-        }
+        for (int w = 1; w < G; ++w) argmax_fold(bv, bx, s_hv[tid * G + w], s_hi[tid * G + w]);
         const uint32_t off = smem_u32(&s_st[rank * ROWS + tid]);
 #pragma unroll
         for (int pe = 0; pe < CS; ++pe) st_cluster_v2f(mapa_cluster(off, static_cast<uint32_t>(pe)), bv, __int_as_float(bx));
       }
       cluster_sync_relacq();                                                                          // (11) pairs exchanged
-      // slices ascend with the rank: a strict > in rank order keeps the first maximum; the same result in every CTA
+      // every CTA folds the same CS pairs in rank order under the same total order: the same token in every CTA, the
+      // one torch.argmax picks (an empty tail slice sends ARGMAX_NONE, which never wins)
       if (tid < nrows) {
         const int r = tid;
         const long long b = img0 + r;
@@ -1008,7 +1000,7 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
 #pragma unroll
         for (int k = 1; k < CS; ++k) {
           const float2 s = s_st[k * ROWS + r];
-          if (s.x > bv) { bv = s.x; bx = __float_as_int(s.y); }
+          argmax_fold(bv, bx, s.x, __float_as_int(s.y));
         }
         if (step + 1 < p.L) {
           int v = bx;
@@ -1048,18 +1040,13 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
         float* lrow = p.logits + (b * p.L + step) * p.C;
         const bool writer = (r % CS) == rank;                        // one CTA stores the row
         float best = -INFINITY;
-        int bi = 0x7fffffff;
+        int bi = ARGMAX_NONE;
         for (int j = lane; j < p.C; j += 32) {
           const float v = s_log[r * A2_SLOG_LD + j];
           if (writer) lrow[j] = v;
-          if (v > best) { best = v; bi = j; }
+          argmax_scan(best, bi, v, j);
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-          const int oi2 = __shfl_xor_sync(0xffffffffu, bi, o);
-          if (ov > best || (ov == best && oi2 < bi)) { best = ov; bi = oi2; }
-        }
+        bi = argmax_finish(best, bi, s_log + r * A2_SLOG_LD, p.C, lane);
         if (lane == 0 && step + 1 < p.L) {
           int v = bi;
           if (p.forced != nullptr) v = p.forced[b * p.forced_ld + step + 1];

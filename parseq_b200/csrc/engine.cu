@@ -80,8 +80,8 @@ int make_tmap(CUtensorMap* tm, const void* ptr, int esize, long long rows, long 
   return PARSEQ_OK;
 }
 
-// 3D bf16 tensor map [d2][d1][d0] (d0 contiguous), strides in elements, box = box_d0 x box_d1 x 1, 128B swizzle:
-// the decoder's cross K/V cache viewed as [image][key][2D] (keys past T read as zeros).
+// 3D bf16 tensor map [d2][d1][d0] (d0 contiguous), strides in elements, box = box_d0 x box_d1 x 1, 128B swizzle.
+// Rows past d1 read as zeros.
 int make_tmap3d(CUtensorMap* tm, const void* ptr, long long d0, long long d1, long long d2, long long ld1, long long ld2,
                 int box_d0, int box_d1) {
   PQ_TRY(load_driver_api());
@@ -95,6 +95,26 @@ int make_tmap3d(CUtensorMap* tm, const void* ptr, long long d0, long long d1, lo
                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(PARSEQ_ERR_CUDA, "cuTensorMapEncodeTiled(3d) failed: " + std::to_string(int(r)));
+  return PARSEQ_OK;
+}
+
+// The decoder's column-blocked cross K/V cache [2D/64][kv_rows = max_batch * T][64] bf16 viewed as the 4D tensor
+// [2D/64][max_batch][T][64]: a box of {64, box_t, 1, 1} at (0, key0, image, panel) holds keys key0.. of ONE image, and
+// the keys past T of that image read as zeros (never the next image's keys, nor rows past the cache), so the softmax's
+// P = 0 for a masked key never meets a non-finite V.  128B swizzle.
+int make_tmap_kv4d(CUtensorMap* tm, const void* ptr, int T, int max_batch, int panels, int box_t) {
+  PQ_TRY(load_driver_api());
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15u) != 0)
+    return fail(PARSEQ_ERR_INVALID_ARG, "tensor map operand must be 16-byte aligned");
+  const cuuint64_t row = 128;                               // 64 bf16
+  cuuint64_t dims[4] = {64, static_cast<cuuint64_t>(T), static_cast<cuuint64_t>(max_batch), static_cast<cuuint64_t>(panels)};
+  cuuint64_t strides[3] = {row, row * T, row * T * max_batch};
+  cuuint32_t box[4] = {64, static_cast<cuuint32_t>(box_t), 1u, 1u};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = g_encode(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(PARSEQ_ERR_CUDA, "cuTensorMapEncodeTiled(K/V 4d) failed: " + std::to_string(int(r)));
   return PARSEQ_OK;
 }
 
@@ -995,8 +1015,7 @@ int ar2_build_maps(parseq_engine* e) {
     PQ_TRY(make_tmap(&m.w2, e->w(Ly + "linear2.weight"), 2, D, e->Md, e->Md, 64, NC2));
     PQ_TRY(make_tmap(&m.wh, e->w("head.weight"), 2, e->C, D, D, 64, ar2_wide(e) ? 128 : 96));
     const int tbox = e->T <= 64 ? 64 : 128;
-    const long long kv_rows = 1ll * e->max_batch * e->T;     // column-blocked cache [2D/64][kv_rows][64]
-    PQ_TRY(make_tmap3d(&m.ckv, e->ckv, 64, kv_rows, 2 * D / 64, 64, 64 * kv_rows, 64, tbox));
+    PQ_TRY(make_tmap_kv4d(&m.ckv, e->ckv, e->T, e->max_batch, 2 * D / 64, tbox));
   }
   e->ar2_maps_ok = true;
   return PARSEQ_OK;

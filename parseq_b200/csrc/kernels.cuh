@@ -410,7 +410,7 @@ __global__ void build_ctx_rows_kernel(const float* __restrict__ emb, const float
 }
 
 // ---------------------------------------------------------------------------------------------
-// Greedy argmax (first maximum wins, torch.argmax semantics) of logits rows -> token ids.
+// Greedy argmax (torch.argmax semantics: first NaN, else first maximum; ptx.cuh) of logits rows -> token ids.
 // One warp per row.  Row r = (b, s): reads logits[b, src_pos0 + s, :C], writes ids[b*ids_ld + dst_pos0 + s].
 // If `forced` != nullptr the written id is forced[b*forced_ld + dst_pos0 + s] (teacher forcing).
 __global__ void argmax_rows_kernel(const float* __restrict__ logits, int L, int C, int B, int nrows_per_b, int src_pos0,
@@ -424,17 +424,9 @@ __global__ void argmax_rows_kernel(const float* __restrict__ logits, int L, int 
   const int b = w / nrows_per_b, s = w % nrows_per_b;
   const float* row = logits + (static_cast<long long>(b) * L + src_pos0 + s) * C;
   float best = -INFINITY;
-  int bi = 0x7fffffff;
-  for (int j = lane; j < C; j += 32) {
-    const float v = row[j];
-    if (v > best) { best = v; bi = j; }    // strictly greater: keeps the lowest index within the lane
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
-  }
+  int bi = ARGMAX_NONE;
+  for (int j = lane; j < C; j += 32) argmax_scan(best, bi, row[j], j);
+  bi = argmax_finish(best, bi, row, C, lane);
   if (lane == 0) {
     int v = bi;
     if (forced != nullptr) v = forced[static_cast<long long>(b) * forced_ld + dst_pos0 + s];
@@ -811,23 +803,15 @@ __global__ void __launch_bounds__(384) dec_ln_head_argmax_kernel(
   }
   if (ids == nullptr) return;
   __syncthreads();
-  // ---- greedy argmax (first maximum wins), warp per row ----
+  // ---- greedy argmax (torch.argmax order), warp per row ----
   if (warp < HEAD_ROWS) {
     const int r = warp;
     const int row = row0 + r;
     if (row < M) {
       float best = -INFINITY;
-      int bi = 0x7fffffff;
-      for (int j = lane; j < C; j += 32) {
-        const float v = sl[r * 128 + j];
-        if (v > best) { best = v; bi = j; }
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
-      }
+      int bi = ARGMAX_NONE;
+      for (int j = lane; j < C; j += 32) argmax_scan(best, bi, sl[r * 128 + j], j);
+      bi = argmax_finish(best, bi, sl + r * 128, C, lane);
       if (lane == 0) {
         const int b = row / nq, qi = row % nq;
         int v = bi;
@@ -842,7 +826,8 @@ __global__ void __launch_bounds__(384) dec_ln_head_argmax_kernel(
 // Fused post-processing of the reference's test path (strhub/models/base.py:132-142 + Tokenizer._filter,
 // strhub/data/utils.py:120-129): per image  ids[i] = argmax_c logits[i, c]  (first maximum),  length = index of the
 // first EOS (L if none),  confidence = prod_{i <= min(length, L-1)} max_c softmax(logits[i])_c  (the EOS probability is
-// included).  One warp per image; only (length, confidence, ids) cross PCIe instead of the [B, L, C] probabilities.
+// included).  A row whose maximum is NaN or +-inf has an all-NaN softmax in torch: id 0 (EOS) with probability NaN.
+// One warp per image; only (length, confidence, ids) cross PCIe instead of the [B, L, C] probabilities.
 __global__ void postprocess_kernel(const float* __restrict__ logits, int B, int L, int C, int eos_id, int* __restrict__ ids,
                                    int* __restrict__ lengths, float* __restrict__ confidence) {
   const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -854,25 +839,23 @@ __global__ void postprocess_kernel(const float* __restrict__ logits, int B, int 
   for (int i = 0; i < L; ++i) {
     const float* row = logits + (static_cast<long long>(b) * L + i) * C;
     float best = -INFINITY;
-    int bi = 0x7fffffff;
-    for (int j = lane; j < C; j += 32) {
-      const float v = row[j];
-      if (v > best) { best = v; bi = j; }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
-    }
+    int bi = ARGMAX_NONE;
+    for (int j = lane; j < C; j += 32) argmax_scan(best, bi, row[j], j);
+    bi = argmax_finish(best, bi, row, C, lane);
+    best = row[bi];
+    // torch's softmax of a row whose maximum is not finite (it holds a NaN or a +inf, or is all -inf) is all NaN, and
+    // max() over it gives index 0 with probability NaN
+    const bool finite = isfinite(best);
     float se = 0.f;
-    for (int j = lane; j < C; j += 32) se += expf(row[j] - best);
+    if (finite)
+      for (int j = lane; j < C; j += 32) se += expf(row[j] - best);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
-    if (lane == 0) ids[static_cast<long long>(b) * L + i] = bi;
+    const int id = finite ? bi : 0;
+    if (lane == 0) ids[static_cast<long long>(b) * L + i] = id;
     if (!done) {
-      conf *= 1.0f / se;                 // max softmax probability of position i
-      if (bi == eos_id) { len = i; done = true; }
+      conf *= finite ? 1.0f / se : __int_as_float(0x7fc00000);   // max softmax probability of position i
+      if (id == eos_id) { len = i; done = true; }
     }
   }
   if (lane == 0) {

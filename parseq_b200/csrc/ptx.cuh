@@ -12,6 +12,52 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 }
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31u; }
 
+// ---------------------------------------------------------------- greedy argmax (torch.argmax order)
+// The order of every argmax in the engine is torch.argmax's: any NaN beats every number and the first NaN wins;
+// otherwise the larger value wins (+inf included, -0.0 == +0.0) and ties go to the lower index.  A running
+// (value, index) pair starts EMPTY (value -inf, index ARGMAX_NONE), which every real candidate beats, so a row of -inf
+// gives its first index and the result is always inside the row.
+//   * argmax_fold / argmax_shfl merge pairs under that order, in any order of arrival (register fragments, shuffles,
+//     shared memory, the CTAs of a cluster);
+//   * a warp that owns a row in memory scans its columns with argmax_scan (a plain `>`, which skips NaN and keeps a
+//     lane's lowest index) and ends with argmax_finish, which merges the lanes and then lets the row's first NaN win in
+//     a second, early-exit pass.  Keeping the NaN test out of the scan keeps the scan as cheap as a finite-only argmax
+//     (register pressure of the AR kernels' heads).
+constexpr int ARGMAX_NONE = 0x7fffffff;
+__device__ __forceinline__ bool argmax_better(float v, int j, float best, int bi) {
+  if (j == ARGMAX_NONE) return false;
+  if (bi == ARGMAX_NONE) return true;
+  const bool vn = isnan(v), bn = isnan(best);
+  if (vn != bn) return vn;
+  if (vn || v == best) return j < bi;
+  return v > best;
+}
+__device__ __forceinline__ void argmax_fold(float& best, int& bi, float v, int j) {
+  if (argmax_better(v, j, best, bi)) { best = v; bi = j; }
+}
+// merge the pairs of the lanes that differ in the offset bits [lo, hi) (xor butterfly: every lane ends with the result)
+__device__ __forceinline__ void argmax_shfl(float& best, int& bi, int lo = 1, int hi = 32) {
+#pragma unroll
+  for (int o = lo; o < hi; o <<= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    argmax_fold(best, bi, ov, oi);
+  }
+}
+__device__ __forceinline__ void argmax_scan(float& best, int& bi, float v, int j) {
+  if (v > best) { best = v; bi = j; }
+}
+// the warp's result for row[0, n) after every lane scanned columns lane, lane + 32, ... with argmax_scan
+__device__ __forceinline__ int argmax_finish(float best, int bi, const float* row, int n, int lane) {
+  argmax_shfl(best, bi);
+  int first_nan = ARGMAX_NONE;
+  for (int j = lane; j < n; j += 32)
+    if (isnan(row[j])) { first_nan = j; break; }
+  first_nan = __reduce_min_sync(0xffffffffu, first_nan);
+  if (first_nan != ARGMAX_NONE) return first_nan;
+  return bi == ARGMAX_NONE ? 0 : bi;                  // no NaN and nothing above -inf: a row of -inf
+}
+
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
@@ -107,6 +153,15 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, ui
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
+
+__device__ __forceinline__ void tma_load_4d(void* smem_dst, const void* tmap, uint64_t* bar, int32_t c0, int32_t c1,
+                                            int32_t c2, int32_t c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2),
+        "r"(c3)
       : "memory");
 }
 

@@ -147,14 +147,14 @@ int64_t parseq_debug_int(parseq_engine* e, const char* name);
 /* Options: "max_batch" (images per super-chunk = one CUDA graph), "chunk" (images per encoder pass inside a
  * super-chunk), "dec_chunk" (images per decoder chain; the chains of a super-chunk run concurrently on their own
  * streams), "use_graph" (0/1), "pdl" (programmatic dependent launch, 0/1), "timing" (1: record a CUDA-event pair around every launch
- * for parseq_get_timing; 0: off + clear), "block_n" (engine-independent GEMM tile override, tests), "fuse_ln" (bit 0: the attention-projection GEMM, bit 1: the fc2 GEMM
+ * for parseq_get_timing; 0: off + clear), "block_n" (accepted for compatibility: the GEMM has one 128 x 128 tile), "fuse_ln" (bit 0: the attention-projection GEMM, bit 1: the fc2 GEMM
  * also produces the LayerNorm that follows it, used when the batch fills the machine at least twice with 128-row tiles; bit 2:
  * for any batch; default 3; 0: separate LayerNorm kernels), "ar_kernel" (AR loop: 2 = cluster-owned persistent kernel,
  * default; 1 = grid-barrier persistent kernel, at most 128 head classes; 0 = chain of separate kernels), "fuse_mlp" (1: fc1 + GELU + fc2 + residual +
  * LayerNorm of an encoder block in one kernel where fuse_ln bit 1 applies - bit-identical results, default 0), "attn_impl"
- * (encoder attention: 0 = mma.sync kernels, default; 1 = wgmma kernel), "cta_group" / "ln_cta_group" / "mlp_cta_group"
- * (0 auto, 1 single CTA, 2 CTA pair sharing the weight tiles by TMA multicast: GEMM / fused GEMM+LayerNorm / one-kernel
- * MLP), "ln_split" (fused GEMM+LayerNorm: 0 auto = the column-split CTA-pair kernel for K >= 768, 1 never,
+ * (encoder attention: 0 = mma.sync kernels, default; 1 = wgmma kernel), "ln_cta_group" / "mlp_cta_group"
+ * (0 auto, 1 single CTA, 2 CTA pair sharing the weight tiles by TMA multicast: fused GEMM+LayerNorm / one-kernel
+ * MLP; "cta_group" is accepted for compatibility, the GEMM runs single-CTA tiles), "ln_split" (fused GEMM+LayerNorm: 0 auto = the column-split CTA-pair kernel for K >= 768, 1 never,
  * 2 always), "pair_pdl", "gemm_stages" (kernel-variant switches for tests).  Options are PER HANDLE; with
  * e == NULL the launch options (block_n, attn_impl, pdl, gemm_stages, cta_group, ln_cta_group, mlp_cta_group, ln_split,
  * pair_pdl) set the

@@ -131,8 +131,8 @@ uint16_t f32_to_bf16_rne(float f) {
 struct LaunchOpts {
   int sm_count = 0;
   bool use_pdl = true;          // programmatic dependent launch on every kernel of the forward chain
-  int block_n = 0;              // 0 = auto
-  int cta_group = 0;            // 0 = auto, 1 / 2 = forced (tests): CTA pairs share the W tile by TMA multicast
+  int block_n = 0;              // accepted (0/64/128/192/256); the GEMM has one 128 x 128 tile shape
+  int cta_group = 0;            // accepted (0/1/2); the GEMM runs single-CTA tiles
   int ln_cta_group = 0;         // same for the fused GEMM + LayerNorm kernel
   int ln_split = 0;             // fused GEMM + LayerNorm: 2 = column-split CTA-pair kernel (gemm_ln.cuh MODE 2), 0 = auto, 1 = never
   int mlp_cta_group = 0;        // one-kernel MLP (mlp_ln.cuh): 0 = auto (pairs), 1 / 2 = forced
@@ -168,42 +168,26 @@ int launch_k(const LaunchOpts& lo, void (*kern)(KArgs...), dim3 grid, dim3 block
   return PARSEQ_OK;
 }
 
-template <int BN, int CG>
-int launch_gemm_cfg(const LaunchOpts& lo, const CUtensorMap& ta, const CUtensorMap& tb, const pq::GemmParams& p, int tiles,
-                    cudaStream_t st) {
-  auto kern = pq::gemm_bf16_wgmma_kernel<BN, CG>;
-  using Cfg = pq::GemmCfg<BN, CG>;
-  static bool attr_set = false;
+// instantiate + set the smem attribute of every configuration outside of any stream capture
+template <int EPI, int STORE>
+int warm_gemm_cfg() {
+  return cudaFuncSetAttribute(pq::gemm_bf16_wgmma_kernel<EPI, STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              pq::GemmCfg::smem_bytes<STORE != pq::ST_REG>()) == cudaSuccess ? PARSEQ_OK
+                                                                      : fail(PARSEQ_ERR_CUDA, "cudaFuncSetAttribute(gemm)");
+}
+template <int EPI, int STORE>
+int launch_gemm_cfg(const LaunchOpts& lo, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to,
+                    const pq::GemmParams& p, int tiles, cudaStream_t st) {
+  static bool attr_set = false;            // the bare kernel entry point may run before any engine handle exists
   if (!attr_set) {
-    PQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    PQ_TRY((warm_gemm_cfg<EPI, STORE>()));
     attr_set = true;
   }
-  cudaLaunchConfig_t cfg{};
-  const int max_groups = lo.sm_count / CG;                 // persistent: one CTA (pair) per SM (pair), tiles strided
-  cfg.gridDim = dim3(static_cast<unsigned>((tiles < max_groups ? tiles : max_groups) * CG));
-  cfg.blockDim = dim3(pq::GEMM_THREADS);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CG;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = (lo.use_pdl && (CG == 1 || lo.pair_pdl)) ? 2 : 1;
-  PQ_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, p));
-  return PARSEQ_OK;
+  const int grid = tiles < lo.sm_count ? tiles : lo.sm_count;   // persistent: one CTA per SM, tiles strided
+  return launch_k(lo, pq::gemm_bf16_wgmma_kernel<EPI, STORE>, dim3(static_cast<unsigned>(grid)), dim3(pq::GEMM_THREADS),
+                  pq::GemmCfg::smem_bytes<STORE != pq::ST_REG>(), st, ta, tb, to, p);
 }
 
-// instantiate + set the smem attribute of every configuration outside of any stream capture
-template <int BN, int CG>
-int warm_gemm_cfg() {
-  return cudaFuncSetAttribute(pq::gemm_bf16_wgmma_kernel<BN, CG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                              pq::GemmCfg<BN, CG>::kSmemBytes) == cudaSuccess ? PARSEQ_OK
-                                                                                : fail(PARSEQ_ERR_CUDA, "cudaFuncSetAttribute(gemm)");
-}
 size_t head_smem_bytes(int C, int D) {
   return ((static_cast<size_t>(C) * (D / 2 + 1) * 4 + 15) / 16) * 16 + static_cast<size_t>(pq::HEAD_ROWS) * D * 4 +
          4 * pq::HEAD_ROWS * 128 * 4 + pq::HEAD_ROWS * 128 * 4;
@@ -285,13 +269,13 @@ int init_kernel_attributes() {
   PQ_TRY((gemm_ln_attr<384, 1>())); PQ_TRY((gemm_ln_attr<384, 2>()));
   PQ_TRY((mlp_ln_attr<192, 1>())); PQ_TRY((mlp_ln_attr<384, 1>())); PQ_TRY((mlp_ln_attr<192, 2>())); PQ_TRY((mlp_ln_attr<384, 2>()));
   PQ_TRY((attn_wgmma_attr<128>())); PQ_TRY((attn_wgmma_attr<256>()));
-  PQ_TRY((warm_gemm_cfg<64, 1>()));
-  PQ_TRY((warm_gemm_cfg<128, 1>()));
-  PQ_TRY((warm_gemm_cfg<192, 1>()));
-  PQ_TRY((warm_gemm_cfg<256, 1>()));
-  PQ_TRY((warm_gemm_cfg<128, 2>()));
-  PQ_TRY((warm_gemm_cfg<192, 2>()));
-  PQ_TRY((warm_gemm_cfg<256, 2>()));
+  PQ_TRY((warm_gemm_cfg<pq::EPI_F32, pq::ST_REG>()));
+  PQ_TRY((warm_gemm_cfg<pq::EPI_F32_RESID, pq::ST_REG>()));
+  PQ_TRY((warm_gemm_cfg<pq::EPI_BF16, pq::ST_REG>()));
+  PQ_TRY((warm_gemm_cfg<pq::EPI_BF16, pq::ST_TMA_2D>()));
+  PQ_TRY((warm_gemm_cfg<pq::EPI_BF16, pq::ST_TMA_3D>()));
+  PQ_TRY((warm_gemm_cfg<pq::EPI_GELU_BF16, pq::ST_REG>()));
+  PQ_TRY((warm_gemm_cfg<pq::EPI_GELU_BF16, pq::ST_TMA_2D>()));
   return PARSEQ_OK;
 }
 
@@ -300,52 +284,51 @@ int gemm_launch(LaunchOpts& lo, const void* A, long long lda, const void* W, lon
                 int K, int mode, float alpha, const float* resid, long long ldr, int resid_mod, void* out, long long ldo,
                 cudaStream_t st, long long blocked_rows = 0) {
   if (M <= 0 || N <= 0 || K <= 0) return fail(PARSEQ_ERR_INVALID_ARG, "gemm: empty problem");
+  if (mode != pq::EPI_F32 && mode != pq::EPI_BF16 && mode != pq::EPI_GELU_BF16)
+    return fail(PARSEQ_ERR_INVALID_ARG, "gemm: mode must be 0 (fp32), 1 (bf16) or 2 (GELU bf16)");
   PQ_TRY(ensure_sm_count(lo));
-  // Tile choice: 128 x 256 tiles for the wide projections (QKV 1152 -> 4.5 tiles, fc1 1536), 128 x 192 for N = 384 / 768
-  // (no padded columns), 128 x 128 for the small decoder GEMMs.
-  // CTA pairs (a cluster of two CTAs on 256 rows, the W tile multicast into both) halve the W traffic per output row;
-  // used where the main loop is long (K >= 768).  The accumulation order per output element is the same, so the choice
-  // does not change a single bit of the result (test_cta_pair_rows_equal_single_cta_rows).
-  int CG = (K >= 768 && M >= 1024) ? 2 : 1;
-  if (lo.cta_group) CG = lo.cta_group;
-  int BN;
-  if (CG == 2) BN = (N % 256 == 0) ? 256 : (N % 192 == 0) ? 192 : 128;
-  else BN = (N <= 64) ? 64 : (M < 1024) ? 128 : (N >= 1024) ? 256 : (N % 192 == 0) ? 192 : 128;
-  if (lo.block_n) {
-    BN = lo.block_n;
-    if (CG == 2 && BN == 64) BN = 128;
-  }
-  CUtensorMap ta, tb;
+  // One tile shape, 128 x 128, for every problem (the block_n / cta_group options are accepted and map onto it): QKV
+  // (1152) and fc1 (1536) have no padded n-tile, and each ping-pong warpgroup holds one tile's accumulator.  Tiles are
+  // numbered along N first, so the CTAs running at the same time share the rows of A they read (L2).
+  CUtensorMap ta, tb, to;
   PQ_TRY(make_tmap(&ta, A, 2, M, K, lda, pq::GEMM_BLOCK_K, pq::GEMM_BLOCK_M));
-  PQ_TRY(make_tmap(&tb, W, 2, N, K, ldw, pq::GEMM_BLOCK_K, BN / CG));
+  PQ_TRY(make_tmap(&tb, W, 2, N, K, ldw, pq::GEMM_BLOCK_K, pq::GEMM_BLOCK_N));
   pq::GemmParams p;
-  p.M = M; p.N = N; p.K = K; p.mode = mode; p.alpha = alpha; p.bias = bias;
+  p.M = M; p.N = N; p.K = K; p.alpha = alpha; p.bias = bias;
   p.resid = resid; p.ldr = ldr; p.resid_mod = resid_mod; p.out = out; p.ldo = ldo;
   const int esz = (mode == pq::EPI_F32) ? 4 : 2;
   bool vec = ((reinterpret_cast<uintptr_t>(out) & 7u) == 0) && ((ldo * esz) % 8 == 0);
   if (resid != nullptr) vec = vec && ((reinterpret_cast<uintptr_t>(resid) & 7u) == 0) && ((ldr * 4) % 8 == 0);
   p.vec_ok = vec ? 1 : 0;
-  p.blocked_rows = 0;
+  // bf16 tiles leave through a TMA store wherever the output is a valid tensor map (16-B aligned base and row pitch);
+  // otherwise (e.g. a logits slice with an odd pitch) every thread stores its own values
+  int store = pq::ST_REG;
   if (blocked_rows > 0) {
-    if (mode == pq::EPI_F32 || N % 64 != 0 || blocked_rows < M || (reinterpret_cast<uintptr_t>(out) & 15u) != 0)
+    if (mode != pq::EPI_BF16 || N % 64 != 0 || blocked_rows < M || (reinterpret_cast<uintptr_t>(out) & 15u) != 0)
       return fail(PARSEQ_ERR_INVALID_ARG, "gemm: blocked output needs a bf16 epilogue, N % 64 == 0 and rows >= M");
-    p.blocked_rows = blocked_rows;
-    p.vec_ok = 1;
+    // [N/64][blocked_rows][64] viewed as a 3D tensor of M rows per block: rows past M are never written
+    PQ_TRY(make_tmap3d(&to, out, 64, M, N / 64, 64, 64 * blocked_rows, 64, pq::GEMM_BLOCK_M));
+    store = pq::ST_TMA_3D;
+  } else if (mode != pq::EPI_F32 && (reinterpret_cast<uintptr_t>(out) & 15u) == 0 && (ldo * 2) % 16 == 0 && ldo >= N) {
+    PQ_TRY(make_tmap(&to, out, 2, M, N, ldo, 64, pq::GEMM_BLOCK_M));
+    store = pq::ST_TMA_2D;
+  } else {
+    to = ta;                                                  // unused by the register-store epilogues
   }
-  const int tile_m = pq::GEMM_BLOCK_M * CG;
   p.max_stages = lo.gemm_stages;
-  p.num_m_tiles = (M + tile_m - 1) / tile_m;
-  p.num_n_tiles = (N + BN - 1) / BN;
+  p.num_m_tiles = (M + pq::GEMM_BLOCK_M - 1) / pq::GEMM_BLOCK_M;
+  p.num_n_tiles = (N + pq::GEMM_BLOCK_N - 1) / pq::GEMM_BLOCK_N;
   const int tiles = p.num_m_tiles * p.num_n_tiles;
-  if (CG == 2) {
-    if (BN == 256) return launch_gemm_cfg<256, 2>(lo, ta, tb, p, tiles, st);
-    if (BN == 192) return launch_gemm_cfg<192, 2>(lo, ta, tb, p, tiles, st);
-    return launch_gemm_cfg<128, 2>(lo, ta, tb, p, tiles, st);
+  if (mode == pq::EPI_F32)
+    return resid != nullptr ? launch_gemm_cfg<pq::EPI_F32_RESID, pq::ST_REG>(lo, ta, tb, to, p, tiles, st)
+                            : launch_gemm_cfg<pq::EPI_F32, pq::ST_REG>(lo, ta, tb, to, p, tiles, st);
+  if (mode == pq::EPI_BF16) {
+    if (store == pq::ST_TMA_3D) return launch_gemm_cfg<pq::EPI_BF16, pq::ST_TMA_3D>(lo, ta, tb, to, p, tiles, st);
+    return store == pq::ST_TMA_2D ? launch_gemm_cfg<pq::EPI_BF16, pq::ST_TMA_2D>(lo, ta, tb, to, p, tiles, st)
+                                  : launch_gemm_cfg<pq::EPI_BF16, pq::ST_REG>(lo, ta, tb, to, p, tiles, st);
   }
-  if (BN == 256) return launch_gemm_cfg<256, 1>(lo, ta, tb, p, tiles, st);
-  if (BN == 192) return launch_gemm_cfg<192, 1>(lo, ta, tb, p, tiles, st);
-  if (BN == 64) return launch_gemm_cfg<64, 1>(lo, ta, tb, p, tiles, st);
-  return launch_gemm_cfg<128, 1>(lo, ta, tb, p, tiles, st);
+  return store == pq::ST_TMA_2D ? launch_gemm_cfg<pq::EPI_GELU_BF16, pq::ST_TMA_2D>(lo, ta, tb, to, p, tiles, st)
+                                : launch_gemm_cfg<pq::EPI_GELU_BF16, pq::ST_REG>(lo, ta, tb, to, p, tiles, st);
 }
 
 // x[M, D] += A[M, K] * W[D, K]^T + bias (fp32, in place); xn[M, D] = bf16(LayerNorm(x; gamma, beta, eps))   (gemm_ln.cuh)

@@ -1,13 +1,14 @@
 // Persistent warp-specialised bf16 GEMM on wgmma (sm_90a):
 //   out[M,N] = epilogue( A[M,K] * W[N,K]^T + bias )
 // A and W are bf16, K-contiguous ("K-major"); both are fetched by TMA into 128B-swizzled shared-memory stages of an
-// mbarrier ring.  Warpgroup 0 is the producer (one thread issues the TMA loads); warpgroups 1 and 2 each accumulate 64
-// rows of the 128 x BLOCK_N tile in registers with wgmma (m64 x BLOCK_N x k16) and store their rows straight from the
-// accumulator.  A CTA (pair) walks the tiles with a stride of the grid; the ring position carries over, so the producer
-// loads the next tile's operands while the MMA warpgroups run the epilogue of the current one.  Every projection of the PARSeq path goes through this kernel: patch-embed (K=96), QKV / proj / fc1 / fc2
-// of the 12 ViT blocks (reference: timm Attention/Mlp via strhub/models/parseq/modules.py:145-165), the
-// cross-attention K/V projection of the image memory, the decoder's q / out projections, MLP (modules.py:69-77) and
-// the character head (model.py:63).
+// mbarrier ring.  Warpgroup 0 is the producer (one thread issues the TMA loads); warpgroups 1 and 2 are "ping-pong"
+// consumers: each owns whole 128 x 128 output tiles (the CTA's tiles alternate between them) and accumulates one in
+// registers with wgmma (two m64n128k16 per k16 step).  An ordered pair of named barriers lets only one of them issue
+// its main loop at a time, so one warpgroup's epilogue (bias, GELU, rounding, store) runs under the other's MMAs.
+// A CTA walks the tiles with a stride of the grid; the ring position carries over from tile to tile.  Every projection
+// of the PARSeq path goes through this kernel: patch-embed (K=96), QKV / proj / fc1 / fc2 of the 12 ViT blocks
+// (reference: timm Attention/Mlp via strhub/models/parseq/modules.py:145-165), the cross-attention K/V projection of
+// the image memory, the decoder's q / out projections, MLP (modules.py:69-77) and the character head (model.py:63).
 #pragma once
 #include <cuda.h>
 #include "ptx.cuh"
@@ -18,45 +19,48 @@ enum GemmEpilogue : int {
   EPI_F32 = 0,        // out_f32 = alpha*(acc+bias) (+ resid[row or row%resid_mod])
   EPI_BF16 = 1,       // out_bf16 = bf16(alpha*(acc+bias))
   EPI_GELU_BF16 = 2,  // out_bf16 = bf16(gelu(acc+bias))
+  EPI_F32_RESID = 3,  // kernel instantiation of EPI_F32 with a residual (the API's mode stays EPI_F32)
 };
+// How the kernel stores its tiles.  TMA: bf16 tiles go through a 128B-swizzled shared-memory staging tile and one
+// thread stores them with cp.async.bulk.tensor, 2D row-major or 3D column-blocked ([N/64][rows][64]); the tensor map's
+// bounds clip ragged rows and columns.  REG: every thread stores its accumulator pairs (fp32, or a bf16 output that is
+// not a valid tensor map: base or row pitch not 16-B aligned).
+enum GemmStore : int { ST_REG = 0, ST_TMA_2D = 1, ST_TMA_3D = 2 };
 
 struct GemmParams {
   int M, N, K;
-  int mode;
   float alpha;
   const float* bias;   // [N] or nullptr
   const float* resid;  // fp32 residual (may alias out: in-place accumulate) or nullptr
   long long ldr;
   int resid_mod;       // >0: residual row = row % resid_mod (broadcast tables: pos_embed, pos_queries)
-  void* out;
+  void* out;           // register-store epilogues only (the TMA store writes through its tensor map)
   long long ldo;       // elements
   int vec_ok;          // 8-byte aligned column pairs: paired stores allowed
-  long long blocked_rows;  // > 0: bf16 output in a column-blocked buffer [N/64][blocked_rows][64] (ldo unused)
-  int num_m_tiles, num_n_tiles;  // in units of (128 * CG) x BLOCK_N
-  int max_stages;                // 0: the full operand ring; n > 0: use only n slots (pipeline-depth experiments)
+  int num_m_tiles, num_n_tiles;
+  int max_stages;      // 0: the full operand ring; n > 0: use only n slots (pipeline-depth experiments)
 };
 
-constexpr int GEMM_BLOCK_M = 128;  // rows per CTA (64 per MMA warpgroup)
+constexpr int GEMM_BLOCK_M = 128;  // rows per tile (two m64 halves, one warpgroup)
+constexpr int GEMM_BLOCK_N = 128;  // columns per tile: QKV (1152), fc1 (1536), D = 384 / 768 split without padding
 constexpr int GEMM_BLOCK_K = 64;   // 64 bf16 = 128 B = one swizzle row
-constexpr int GEMM_THREADS = 384;  // warpgroup 0: TMA producer, warpgroups 1, 2: MMA + epilogue
+constexpr int GEMM_THREADS = 384;  // warpgroup 0: TMA producer, warpgroups 1, 2: MMA + epilogue (ping-pong)
 
-// CG = 1: one CTA computes a 128 x BLOCK_N tile.
-// CG = 2: a cluster of two CTAs computes a 256 x BLOCK_N tile: each CTA loads its own 128 rows of A and HALF of the W
-//         tile, multicast into both CTAs, so every W byte is fetched from L2 once per 256 (instead of 128) output rows.
-template <int BLOCK_N, int CG>
 struct GemmCfg {
-  static constexpr int kBRows = BLOCK_N / CG;                       // W rows loaded by one CTA
   static constexpr int kABytes = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;   // 16 KB
-  static constexpr int kBBytes = BLOCK_N * GEMM_BLOCK_K * 2;        // the whole W tile lands in every CTA
+  static constexpr int kBBytes = GEMM_BLOCK_N * GEMM_BLOCK_K * 2;   // 16 KB
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStagesRaw = (232448 - 1024 - 256) / kStageBytes;
-  static constexpr int kStages = kStagesRaw > 6 ? 6 : kStagesRaw;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-  static_assert(BLOCK_N == 64 || BLOCK_N == 128 || BLOCK_N == 192 || BLOCK_N == 256, "BLOCK_N");
-  static_assert(CG == 1 || CG == 2, "CG");
-  static_assert((kBRows * GEMM_BLOCK_K * 2) % 1024 == 0, "multicast halves must stay 1024-B aligned");
-  static_assert(kStages >= 3, "pipeline depth");
+  static constexpr int kHalfOutBytes = GEMM_BLOCK_M * 64 * 2;       // one 128 x 64 bf16 box of the output tile
+  static constexpr int kOutBytes = 2 * kHalfOutBytes;               // one staging tile per consumer warpgroup
+  // Four stages run as fast as five at M = 65 536 (tests/bench_gemm_shapes.py, gemm_stages sweep) and leave shared
+  // memory to spare: 193 KB with the staging tiles, 129 KB for the register-store epilogues, which need none.
+  static constexpr int kStages = 4;
+  template <bool STAGING>
+  static constexpr int smem_bytes() {
+    return kStages * kStageBytes + (STAGING ? 2 * kOutBytes : 0) + 1024 /*align slack*/ + 256 /*barriers*/;
+  }
 };
+static_assert(GemmCfg::smem_bytes<true>() <= 232448, "shared memory");
 
 // ------------------------------------------------------------------------------------------------ operand ring
 // full[s]: stage s holds its A and B tiles (TMA transaction bytes).  empty[s]: every MMA warpgroup that reads stage s
@@ -66,6 +70,7 @@ struct GemmCfg {
 // offsets of the warpgroup's A rows / B rows inside a stage; stage / phase: the ring position, carried over from tile to
 // tile.  A stage is released once the MMAs of the NEXT k-block are queued (wgmma_wait<1>), so the tensor cores never wait
 // for the release round trip; the last one once the accumulator is complete.  Hence a ring needs at least two stages.
+// (Used by the fused GEMM + LayerNorm kernel, gemm_ln.cuh.)
 template <int N, bool PAIR>
 __device__ __forceinline__ void wg_mainloop(float (&acc)[N / 2], uint8_t* smem, int stage_bytes, int a_off, int b_off,
                                             uint64_t* full_bar, uint64_t* empty_bar, int nstages, int num_kb, int& stage,
@@ -102,22 +107,27 @@ __device__ __forceinline__ void wg_mainloop(float (&acc)[N / 2], uint8_t* smem, 
   if (prev >= 0) release(prev);
 }
 
+__device__ __forceinline__ void ring_advance(int& stage, uint32_t& phase, int n, int nstages) {
+  const int s = stage + n;
+  phase ^= static_cast<uint32_t>((s / nstages) & 1);
+  stage = s % nstages;
+}
+
 // ------------------------------------------------------------------------------------------------ epilogue
-// Two columns of one accumulator row.  Each quad of lanes covers 8 consecutive columns of a row (32 B fp32, 16 B bf16).
-__device__ __forceinline__ void gemm_store_pair(const GemmParams& p, int row, int col, float v0, float v1, float b0,
-                                                float b1) {
+template <int EPI>
+__device__ __forceinline__ float gemm_epi(float v, float b, float alpha) {
+  if constexpr (EPI == EPI_GELU_BF16) return gelu_erf(v + b);
+  else return (v + b) * alpha;
+}
+
+// Register-store epilogue: fp32 (EPI_F32_RESID: plus a residual or broadcast table), or bf16 where the output cannot
+// be a TMA tensor.  Two columns of one accumulator row per call.
+template <int EPI>
+__device__ __forceinline__ void gemm_store_pair(const GemmParams& p, int row, int col, float f0, float f1) {
   const bool two = col + 1 < p.N;
-  float f0, f1;
-  if (p.mode == EPI_GELU_BF16) {
-    f0 = gelu_erf(v0 + b0);
-    f1 = gelu_erf(v1 + b1);
-  } else {
-    f0 = (v0 + b0) * p.alpha;
-    f1 = (v1 + b1) * p.alpha;
-  }
-  if (p.mode == EPI_F32) {
+  if constexpr (EPI == EPI_F32 || EPI == EPI_F32_RESID) {
     float* o = reinterpret_cast<float*>(p.out) + static_cast<long long>(row) * p.ldo + col;
-    if (p.resid != nullptr) {
+    if constexpr (EPI == EPI_F32_RESID) {
       const long long rrow = (p.resid_mod > 0) ? (row % p.resid_mod) : row;
       const float* r = p.resid + rrow * p.ldr + col;
       if (two && p.vec_ok) {
@@ -135,8 +145,7 @@ __device__ __forceinline__ void gemm_store_pair(const GemmParams& p, int row, in
       if (two) o[1] = f1;
     }
   } else {
-    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) +
-                       (p.blocked_rows > 0 ? blocked_off(p.blocked_rows, row, col) : static_cast<long long>(row) * p.ldo + col);
+    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + static_cast<long long>(row) * p.ldo + col;
     if (two && p.vec_ok) *reinterpret_cast<uint32_t*>(o) = pack_bf16(f0, f1);
     else {
       o[0] = __float2bfloat16_rn(f0);
@@ -145,96 +154,166 @@ __device__ __forceinline__ void gemm_store_pair(const GemmParams& p, int row, in
   }
 }
 
-template <int BLOCK_N, int CG>
+template <int EPI, int STORE>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-  using Cfg = GemmCfg<BLOCK_N, CG>;
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                       const __grid_constant__ CUtensorMap tmOut, const GemmParams p) {
+  constexpr bool TMA_OUT = STORE != ST_REG;
+  static_assert(!TMA_OUT || EPI == EPI_BF16 || EPI == EPI_GELU_BF16, "the TMA store carries bf16 tiles");
+  using Cfg = GemmCfg;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   const uint32_t pad = ((raw_addr + 1023u) & ~1023u) - raw_addr;
   uint8_t* smem = smem_raw + pad;                         // 1024-B aligned (SWIZZLE_128B requirement)
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  uint8_t* out_stage = smem + Cfg::kStages * Cfg::kStageBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(out_stage + (TMA_OUT ? 2 * Cfg::kOutBytes : 0));
   uint64_t* empty_bar = full_bar + Cfg::kStages;
 
-  const uint32_t rank = (CG == 2) ? cluster_ctarank() : 0u;
   const int num_tiles = p.num_m_tiles * p.num_n_tiles;
-  const int num_clusters = gridDim.x / CG;
   const int num_kb = (p.K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K;
   const int nstages = (p.max_stages > 0 && p.max_stages < Cfg::kStages) ? p.max_stages : Cfg::kStages;
+  const int n_local = (num_tiles - 1 - static_cast<int>(blockIdx.x)) / static_cast<int>(gridDim.x) + 1;  // grid <= tiles
 
   grid_dep_launch();                       // PDL: the next kernel may start its own prologue
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
+    if constexpr (TMA_OUT) prefetch_tmap(&tmOut);
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2 * CG);
+      mbar_init(&empty_bar[s], 1);         // a stage is read by one consumer warpgroup
     }
     fence_mbar_init();
   }
-  if constexpr (CG == 2) cluster_sync_all(); else __syncthreads();
+  __syncthreads();
   grid_dep_wait();                         // PDL: inputs of this GEMM are complete and visible from here on
 
   if (threadIdx.x < 128) {
-    // ===================== TMA producer =====================
-    // runs ahead across tiles: the next tile's operands stream in while the MMA warpgroups store this one
+    // ===================== TMA producer: the CTA's tiles in order, running ahead across tiles =====================
+    setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = blockIdx.x / CG; tile < num_tiles; tile += num_clusters) {
-        const int m0 = (tile / p.num_n_tiles) * (GEMM_BLOCK_M * CG) + static_cast<int>(rank) * GEMM_BLOCK_M;
-        const int n0 = (tile % p.num_n_tiles) * BLOCK_N;
+      for (int j = 0; j < n_local; ++j) {
+        const int tile = static_cast<int>(blockIdx.x) + j * static_cast<int>(gridDim.x);
+        const int m0 = (tile / p.num_n_tiles) * GEMM_BLOCK_M;
+        const int n0 = (tile % p.num_n_tiles) * GEMM_BLOCK_N;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait_mma(&empty_bar[stage], phase ^ 1u);
           uint8_t* sa = smem + stage * Cfg::kStageBytes;
-          uint8_t* sb = sa + Cfg::kABytes;
           mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
           tma_load_2d(sa, &tmA, &full_bar[stage], kb * GEMM_BLOCK_K, m0);
-          if constexpr (CG == 1) {
-            tma_load_2d(sb, &tmB, &full_bar[stage], kb * GEMM_BLOCK_K, n0);
-          } else {
-            const int r = static_cast<int>(rank);
-            tma_load_2d_mcast(sb + r * Cfg::kBRows * GEMM_BLOCK_K * 2, &tmB, &full_bar[stage], kb * GEMM_BLOCK_K,
-                              n0 + r * Cfg::kBRows, 0x3);
-          }
+          tma_load_2d(sa + Cfg::kABytes, &tmB, &full_bar[stage], kb * GEMM_BLOCK_K, n0);
           if (++stage == nstages) { stage = 0; phase ^= 1u; }
         }
       }
     }
-    __syncwarp();
   } else {
-    // ===================== MMA warpgroups: rows [64 wg, 64 wg + 64) of the tile =====================
+    // ===================== MMA warpgroup wg: the CTA's local tiles wg, wg + 2, ... =====================
+    setmaxnreg_inc<232>();
     const int wg = (threadIdx.x >> 7) - 1;
+    const int t = threadIdx.x & 127;
+    const int lane = t & 31;
+    const int warp = t >> 5;
+    const bool leader = t == 0;
+    uint8_t* stage_out = out_stage + wg * Cfg::kOutBytes;
     int stage = 0;
     uint32_t phase = 0;
+    if (wg == 1) ring_advance(stage, phase, num_kb, nstages);     // local tile 0 belongs to warpgroup 0
 #pragma unroll 1
-    for (int tile = blockIdx.x / CG; tile < num_tiles; tile += num_clusters) {
-      const int m0 = (tile / p.num_n_tiles) * (GEMM_BLOCK_M * CG) + static_cast<int>(rank) * GEMM_BLOCK_M;
-      const int n0 = (tile % p.num_n_tiles) * BLOCK_N;
-      float acc[BLOCK_N / 2];
+    for (int j = wg; j < n_local; j += 2) {
+      const int tile = static_cast<int>(blockIdx.x) + j * static_cast<int>(gridDim.x);
+      const int m0 = (tile / p.num_n_tiles) * GEMM_BLOCK_M;
+      const int n0 = (tile % p.num_n_tiles) * GEMM_BLOCK_N;
+      // ordered main loops: wait until the other warpgroup has issued every MMA of local tile j - 1
+      if (j > 0) named_bar_sync(1 + wg, 256);
+      float acc0[64], acc1[64];            // rows [0, 64) and [64, 128) of the tile
 #pragma unroll
-      for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.0f;
-      wg_mainloop<BLOCK_N, CG == 2>(acc, smem, Cfg::kStageBytes, wg * (64 * GEMM_BLOCK_K * 2), Cfg::kABytes, full_bar,
-                                    empty_bar, nstages, num_kb, stage, phase);
-      const int t = threadIdx.x & 127;
-      const int lane = t & 31;
-      const int row_a = m0 + wg * 64 + (t >> 5) * 16 + (lane >> 2);
+      for (int i = 0; i < 64; ++i) { acc0[i] = 0.0f; acc1[i] = 0.0f; }
+      int prev = -1;
+#pragma unroll 1
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait_mma(&full_bar[stage], phase);
+        const uint32_t base = smem_u32(smem + stage * Cfg::kStageBytes);
+        const uint64_t da0 = make_desc_k_sw128(base);
+        const uint64_t da1 = make_desc_k_sw128(base + 64 * GEMM_BLOCK_K * 2);
+        const uint64_t db = make_desc_k_sw128(base + Cfg::kABytes);
+        wgmma_fence();
 #pragma unroll
-      for (int i = 0; i < BLOCK_N / 8; ++i) {
+        for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) {
+          const uint32_t accum = static_cast<uint32_t>((kb | k) != 0);
+          wgmma_bf16<128>(acc0, da0 + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k), accum);
+          wgmma_bf16<128>(acc1, da1 + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k), accum);
+        }
+        wgmma_commit();
+        if (prev >= 0) {
+          wgmma_wait<1>();
+          if (leader) mbar_arrive(&empty_bar[prev]);
+        }
+        prev = stage;
+        if (++stage == nstages) { stage = 0; phase ^= 1u; }
+      }
+      if (j + 1 < n_local) named_bar_arrive(1 + (wg ^ 1), 256);   // the other warpgroup may start its main loop
+      wgmma_wait<0>();
+      wgmma_reg_fence(acc0);
+      wgmma_reg_fence(acc1);
+      if (leader) mbar_arrive(&empty_bar[prev]);
+      ring_advance(stage, phase, num_kb, nstages);                 // skip the other warpgroup's tile j + 1
+
+      // ---- epilogue.  Accumulator layout (ptx.cuh wgmma_bf16): acc_h[4i + {0,1}] = row 64h + 16 warp + lane/4,
+      // columns 8i + 2(lane%4) + {0,1}; acc_h[4i + {2,3}] = the same columns 8 rows further down.
+      const int r0 = 16 * warp + (lane >> 2);
+      if constexpr (TMA_OUT) {
+        // the previous TMA store of this warpgroup has finished reading the staging tile
+        if (leader) bulk_wait_group_read<0>();
+        named_bar_sync(3 + wg, 128);
+      }
+#pragma unroll
+      for (int i = 0; i < GEMM_BLOCK_N / 8; ++i) {
         const int col = n0 + i * 8 + 2 * (lane & 3);
-        if (col >= p.N) continue;
         float b0 = 0.0f, b1 = 0.0f;
         if (p.bias != nullptr) {
-          b0 = __ldg(p.bias + col);
+          if (col < p.N) b0 = __ldg(p.bias + col);
           if (col + 1 < p.N) b1 = __ldg(p.bias + col + 1);
         }
-        if (row_a < p.M) gemm_store_pair(p, row_a, col, acc[4 * i], acc[4 * i + 1], b0, b1);
-        if (row_a + 8 < p.M) gemm_store_pair(p, row_a + 8, col, acc[4 * i + 2], acc[4 * i + 3], b0, b1);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {        // (half, +8 rows)
+          const float* acc = (q < 2) ? acc0 : acc1;
+          const int rl = 64 * (q >> 1) + r0 + 8 * (q & 1);
+          const float f0 = gemm_epi<EPI>(acc[4 * i + 2 * (q & 1)], b0, p.alpha);
+          const float f1 = gemm_epi<EPI>(acc[4 * i + 2 * (q & 1) + 1], b1, p.alpha);
+          if constexpr (TMA_OUT) {
+            // 128B swizzle: 16-B chunk c of row r sits at chunk c ^ (r % 8); r % 8 = lane / 4 here
+            uint8_t* dst = stage_out + (i >> 3) * Cfg::kHalfOutBytes + rl * 128 + ((((i & 7) ^ (lane >> 2))) << 4) +
+                           (lane & 3) * 4;
+            *reinterpret_cast<uint32_t*>(dst) = pack_bf16(f0, f1);
+          } else {
+            const int row = m0 + rl;
+            if (row < p.M && col < p.N) gemm_store_pair<EPI>(p, row, col, f0, f1);
+          }
+        }
+      }
+      if constexpr (TMA_OUT) {
+        fence_proxy_async_smem();            // the staging writes are visible to the TMA (async proxy)
+        named_bar_sync(3 + wg, 128);
+        if (leader) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int c0 = n0 + 64 * h;
+            if (c0 >= p.N) break;
+            if constexpr (STORE == ST_TMA_3D) tma_store_3d(&tmOut, stage_out + h * Cfg::kHalfOutBytes, 0, m0, c0 / 64);
+            else tma_store_2d(&tmOut, stage_out + h * Cfg::kHalfOutBytes, c0, m0);
+          }
+          bulk_commit_group();
+        }
       }
     }
+    if constexpr (TMA_OUT) {
+      // the last stores have read their staging tile before the CTA's shared memory is released; their global writes
+      // are part of this grid's results, visible to the next kernel once the grid completes
+      if (leader) bulk_wait_group_read<0>();
+    }
   }
-  // a CTA of a pair must not exit while its peer may still multicast into it or arrive on its barriers
-  if constexpr (CG == 2) cluster_sync_all();
 }
 
 }  // namespace pq

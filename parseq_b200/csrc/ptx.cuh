@@ -116,6 +116,21 @@ __device__ __forceinline__ void mbar_wait_mma(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void grid_dep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
+// ---------------------------------------------------------------- named barriers, register reallocation
+// bar.sync waits until `count` threads (a multiple of 32) have arrived on barrier `id`; bar.arrive only arrives.
+// Barrier 0 is __syncthreads().
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+// Warpgroup-wide change of the per-thread register budget (all 128 threads execute it).
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---------------------------------------------------------------- clusters (CTA pairs)
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;

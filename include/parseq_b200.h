@@ -154,8 +154,8 @@ int64_t parseq_debug_int(parseq_engine* e, const char* name);
  * LayerNorm of an encoder block in one kernel where fuse_ln bit 1 applies - bit-identical results, default 0), "attn_impl"
  * (encoder attention: 0 = mma.sync kernels, default; 1 = wgmma kernel), "ln_cta_group" / "mlp_cta_group"
  * (0 auto, 1 single CTA, 2 CTA pair sharing the weight tiles by TMA multicast: fused GEMM+LayerNorm / one-kernel
- * MLP; "cta_group" is accepted for compatibility, the GEMM runs single-CTA tiles), "ln_split" (fused GEMM+LayerNorm: 0 auto = the column-split CTA-pair kernel for K >= 768, 1 never,
- * 2 always), "pair_pdl", "gemm_stages" (kernel-variant switches for tests).  Options are PER HANDLE; with
+ * MLP; "cta_group" is accepted for compatibility, the GEMM runs single-CTA tiles), "ln_split" (fused GEMM+LayerNorm: 0 auto = the persistent column-split CTA-pair kernel at D = 384,
+ * 1 never = the full-row kernel (ln_cta_group picks its single-CTA or pair form), 2 always), "pair_pdl", "gemm_stages" (kernel-variant switches for tests).  Options are PER HANDLE; with
  * e == NULL the launch options (block_n, attn_impl, pdl, gemm_stages, cta_group, ln_cta_group, mlp_cta_group, ln_split,
  * pair_pdl) set the
  * process defaults that the stand-alone kernel

@@ -134,7 +134,7 @@ struct LaunchOpts {
   int block_n = 0;              // accepted (0/64/128/192/256); the GEMM has one 128 x 128 tile shape
   int cta_group = 0;            // accepted (0/1/2); the GEMM runs single-CTA tiles
   int ln_cta_group = 0;         // same for the fused GEMM + LayerNorm kernel
-  int ln_split = 0;             // fused GEMM + LayerNorm: 2 = column-split CTA-pair kernel (gemm_ln.cuh MODE 2), 0 = auto, 1 = never
+  int ln_split = 0;             // fused GEMM + LayerNorm: 2 = persistent column-split CTA pairs (gemm_ln.cuh MODE 2), 0 = auto (MODE 2 at D = 384), 1 = never
   int mlp_cta_group = 0;        // one-kernel MLP (mlp_ln.cuh): 0 = auto (pairs), 1 / 2 = forced
   bool pair_pdl = false;        // experiments: programmatic dependent launch also on CTA-pair (cluster) launches
   int gemm_stages = 0;          // experiments: cap the operand ring depth (0 = full)
@@ -342,17 +342,24 @@ int launch_gemm_ln(const LaunchOpts& lo, const void* A, long long lda, const voi
     PQ_TRY((gemm_ln_attr<D, MODE>()));
     attr_set = true;
   }
-  CUtensorMap ta, tb;
+  CUtensorMap ta, tb, tx;
   PQ_TRY(make_tmap(&ta, A, 2, M, K, lda, pq::GEMM_BLOCK_K, pq::GLN_BLOCK_M));
   PQ_TRY(make_tmap(&tb, W, 2, D, K, ldw, pq::GEMM_BLOCK_K, Cfg::kBox));
   if ((reinterpret_cast<uintptr_t>(x) & 7u) != 0 || (reinterpret_cast<uintptr_t>(xn) & 3u) != 0)
     return fail(PARSEQ_ERR_INVALID_ARG, "gemm_ln: x must be 8-byte and xn 4-byte aligned");
   pq::GemmLnParams p;
   p.M = M; p.K = K; p.bias = bias; p.gamma = gamma; p.beta = beta; p.eps = eps;
-  const int tile_m = pq::GLN_BLOCK_M * (MODE == 1 ? 2 : 1);
-  p.num_m_tiles = (M + tile_m - 1) / tile_m;
+  p.num_m_tiles = (M + Cfg::kTileM - 1) / Cfg::kTileM;
+  int clusters = p.num_m_tiles;
+  if constexpr (MODE == 2) {
+    // persistent: one cluster per SM pair; the tile's x slice is fetched by TMA (x: 16-B aligned)
+    PQ_TRY(make_tmap(&tx, x, 4, M, D, D, Cfg::kXBoxCols, Cfg::kTileM));
+    clusters = std::min(p.num_m_tiles, std::max(1, lo.sm_count / 2));
+  } else {
+    tx = ta;                                                  // unused by MODE 0 / 1
+  }
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(p.num_m_tiles * Cfg::kCG));
+  cfg.gridDim = dim3(static_cast<unsigned>(clusters * Cfg::kCG));
   cfg.blockDim = dim3(pq::GLN_THREADS);
   cfg.dynamicSmemBytes = Cfg::kSmemBytes;
   cfg.stream = st;
@@ -365,7 +372,7 @@ int launch_gemm_ln(const LaunchOpts& lo, const void* A, long long lda, const voi
   attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = (lo.use_pdl && (MODE == 0 || lo.pair_pdl)) ? 2 : 1;
-  PQ_CUDA(cudaLaunchKernelEx(&cfg, pq::gemm_ln_fused_kernel<D, MODE>, ta, tb, x, reinterpret_cast<__nv_bfloat16*>(xn), p));
+  PQ_CUDA(cudaLaunchKernelEx(&cfg, pq::gemm_ln_fused_kernel<D, MODE>, ta, tb, tx, x, reinterpret_cast<__nv_bfloat16*>(xn), p));
   return PARSEQ_OK;
 }
 int gemm_ln_launch(LaunchOpts& lo, const void* A, long long lda, const void* W, long long ldw, const float* bias, int M, int D,
@@ -373,12 +380,13 @@ int gemm_ln_launch(LaunchOpts& lo, const void* A, long long lda, const void* W, 
   if (M <= 0 || K <= 0) return fail(PARSEQ_ERR_INVALID_ARG, "gemm_ln: empty problem");
   PQ_TRY(ensure_sm_count(lo));
   PQ_TRY(load_driver_api());
-  // MODE 2 (the columns of a 64-row tile split over a CTA pair) halves the W bytes each CTA stages per k-block, so the
-  // ring is twice as deep where the main loop is long (fc2, K = 1536).  ln_split: 0 auto (K >= 768), 1 never, 2 always
-  // (D = 384).  Selected by K only: a row's bits must not depend on the batch.  MODE 1 (ln_cta_group = 2) shares the W
-  // tile of two 64-row tiles by multicast.  Where the fused kernels are used at all is decided by the caller from the
-  // batch regime (encode_chunk).
-  if (D == 384 && (lo.ln_split == 2 || (lo.ln_split == 0 && K >= 768)))
+  // MODE 2 (persistent CTA pairs on 128-row tiles, the columns split over the pair) runs every K at D = 384: W bytes per
+  // row are half of the full-row kernel's, A crosses L2 once per tile, and the residual arrives during the main loop.
+  // ln_split: 0 auto (D = 384), 1 never (the full-row MODE 0 / MODE 1 kernel), 2 always.  The row statistics order is
+  // chosen by K inside the kernel, never by the batch.  MODE 1 (ln_cta_group = 2 with ln_split = 1) shares the W tile
+  // of two 64-row tiles by multicast.  Where the fused kernels are used at all is decided by the caller from the batch
+  // regime (encode_chunk).
+  if (D == 384 && lo.ln_split != 1)
     return launch_gemm_ln<384, 2>(lo, A, lda, W, ldw, bias, M, K, x, gamma, beta, eps, xn, st);
   if (lo.ln_cta_group == 2) {
     if (D == 384) return launch_gemm_ln<384, 1>(lo, A, lda, W, ldw, bias, M, K, x, gamma, beta, eps, xn, st);

@@ -201,7 +201,7 @@ mlp_ln_fused_kernel(const __grid_constant__ CUtensorMap tmXn, const __grid_const
         release();
       }
     }
-    gln_epilogue<D, D / 2, 2, false>(acc, x, xn_out, p.M, p.eps, m0, 0, wg, 0u, s_b2, s_gamma, s_beta, s_part, nullptr);
+    gln_epilogue<D, D / 2>(acc, x, xn_out, p.M, p.eps, m0, wg, s_b2, s_gamma, s_beta, s_part);
   }
   // a CTA of a pair must not exit while its peer may still multicast into it or arrive on its barriers
   if constexpr (CG == 2) cluster_sync_all();

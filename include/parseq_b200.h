@@ -41,7 +41,7 @@ typedef struct parseq_config {
   int32_t embed_dim;
   int32_t enc_num_heads, enc_mlp_ratio, enc_depth;
   int32_t dec_num_heads, dec_mlp_ratio, dec_depth;   /* dec_depth must be 1 (all reference configs) */
-  int32_t max_label_length;              /* 25 -> 26 decode positions */
+  int32_t max_label_length;              /* 25 -> 26 decode positions; 0..63 (labels of up to 63 characters) */
   int32_t num_tokens;                    /* 97: EOS=0, chars 1..94, BOS=95, PAD=96 (data/utils.py:102-111); 4..16386
                                             (at most 16384 head classes, e.g. CJK charsets) */
   int32_t max_batch;                     /* images per super-chunk / CUDA graph (workspace sizing); 0 = 512 */
@@ -87,7 +87,8 @@ typedef struct parseq_forward_args {
 
 /* Replaces system.PARSeq.forward -> model.PARSeq.forward (system.py:87-88, model.py:105-169).
  *   images : DEVICE fp32 [N,3,H,W] (NCHW, values as produced by T.Normalize(0.5,0.5))
- *   logits : DEVICE fp32 [N, num_steps, num_tokens-2], num_steps = min(max_length,25)+1 (26 if -1)
+ *   logits : DEVICE fp32 [N, num_steps, num_tokens-2], num_steps = min(max_length, max_label_length)+1
+ *            (max_label_length+1 if -1)
  *   ids    : DEVICE int32 [N, num_steps] argmax of `logits` (may be NULL)
  *   steps  : DEVICE int32 [1] (may be NULL): S = number of AR steps the reference would have run
  *            before its batch-wide early exit (model.py:144); == num_steps when max_length >= 0,
@@ -142,7 +143,9 @@ int64_t parseq_kernel_launches(const parseq_engine* e);      /* cumulative count
  * 16 KB boxes each from `buf` through `nslot` slots, no compute. */
 int parseq_bench_tma_stream(void* buf, int64_t bytes, int cluster, int ctas, int nboxes, int nslot, int mode, void* sink,
                             parseq_stream_t stream);
-/* Debug counters by name ("ar2_occupancy_mt2", "ar2_clusters_mt2", "ar_last_per", "ar_last_clusters", "sm_count"); -1 if unknown. */
+/* Debug counters by name ("ar2_occupancy_mt2", "ar2_clusters_mt2", "ar_last_per", "ar_last_clusters", "sm_count"; the last
+ * cluster AR kernel instantiation: "ar_last_cluster_size", "ar_last_mt", "ar_last_head_split", "ar_last_wide",
+ * "ar_last_ids_pitch"); -1 if unknown. */
 int64_t parseq_debug_int(parseq_engine* e, const char* name);
 /* Options: "max_batch" (images per super-chunk = one CUDA graph), "chunk" (images per encoder pass inside a
  * super-chunk), "dec_chunk" (images per decoder chain; the chains of a super-chunk run concurrently on their own
@@ -150,7 +153,7 @@ int64_t parseq_debug_int(parseq_engine* e, const char* name);
  * for parseq_get_timing; 0: off + clear), "block_n" (accepted for compatibility: the GEMM has one 128 x 128 tile), "fuse_ln" (bit 0: the attention-projection GEMM, bit 1: the fc2 GEMM
  * also produces the LayerNorm that follows it, used when the batch fills the machine at least twice with 128-row tiles; bit 2:
  * for any batch; default 3; 0: separate LayerNorm kernels), "ar_kernel" (AR loop: 2 = cluster-owned persistent kernel,
- * default; 1 = grid-barrier persistent kernel, at most 128 head classes; 0 = chain of separate kernels), "fuse_mlp" (1: fc1 + GELU + fc2 + residual +
+ * default; 1 = grid-barrier persistent kernel, at most 128 head classes and max_label_length <= 31; 0 = chain of separate kernels), "fuse_mlp" (1: fc1 + GELU + fc2 + residual +
  * LayerNorm of an encoder block in one kernel where fuse_ln bit 1 applies - bit-identical results, default 0), "attn_impl"
  * (encoder attention: 0 = mma.sync kernels, default; 1 = wgmma kernel), "ln_cta_group" / "mlp_cta_group"
  * (0 auto, 1 single CTA, 2 CTA pair sharing the weight tiles by TMA multicast: fused GEMM+LayerNorm / one-kernel
@@ -166,7 +169,8 @@ int parseq_set_option(parseq_engine* e, const char* name, int64_t value);
  * 6 encoder residual GEMM fused with LayerNorm, 7 persistent AR-loop kernel. */
 int parseq_get_timing(parseq_engine* e, int category, double* ms, double* flops, int64_t* count);
 /* Debug: after a forward with option "ar_prof"=1, copies the [32 steps][16 slots] globaltimer (ns) stamps that block 0 of
- * the persistent AR kernel recorded at its phase boundaries. */
+ * the persistent AR kernel recorded at its phase boundaries.  Row 26 holds extra stamps of step 1 of the cluster kernel;
+ * with max_label_length > 31 only steps < 26 are recorded. */
 int parseq_get_ar_profile(parseq_engine* e, uint64_t* out512);
 const char* parseq_last_error(void);
 const char* parseq_version(void);

@@ -50,13 +50,14 @@ struct DecAr2Params {
   float* logits;                  // [B, L, C]
   const int* forced;              // optional teacher forcing [B, forced_ld]
   int forced_ld;
-  unsigned long long* prof;       // optional [L][16] globaltimer stamps of cluster 0 / rank 0, or nullptr
+  unsigned long long* prof;       // optional [32][16] globaltimer stamps of cluster 0 / rank 0, or nullptr (A2_PROF)
 };
 
 constexpr int A2_THREADS = 256;      // consumer threads (warps 0-7)
 constexpr int A2_LAUNCH_THREADS = 288;   // + warp 8: the TMA producer
 constexpr int A2_SLOT = 16384;      // ring slot bytes
 constexpr int A2_SLOG_LD = 104;     // fp32 row pitch of the staged logits
+constexpr int A2_PROF_STEPS = 26;   // steps with a row of their own in the [32][16] profile buffer (row 26: step 1 extras)
 
 __device__ __forceinline__ void cluster_sync_relacq() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -90,7 +91,8 @@ __device__ __forceinline__ uint32_t box_off(int r, int c) {
   return static_cast<uint32_t>(r * 128 + ((((c >> 3) ^ (r & 7)) << 4) | ((c & 7) << 1)));
 }
 
-template <int D, int MT, int CS_>
+// IDP: row pitch of the per-cluster id buffer s_ids, 32 (L <= 32) or 64 (L <= 64 decode positions)
+template <int D, int MT, int CS_, int IDP = 32>
 struct A2Cfg {
   static constexpr int CS = CS_;                       // CTAs per cluster (8; 6 can pack more SMs of a GPC)
   static constexpr int ROWS = 16 * MT;                 // rows (images) per cluster, padded
@@ -119,7 +121,7 @@ struct A2Cfg {
   static constexpr int CA_BYTES = D * 2;
   static constexpr int ST_BYTES = CS * ROWS * 8;
   static constexpr int RED_BYTES = 2 * 8 * MH * 16 * 4;
-  static constexpr int IDS_BYTES = ROWS * 32 * 4;
+  static constexpr int IDS_BYTES = ROWS * IDP * 4;
   static constexpr int SLOG_BYTES = ROWS * A2_SLOG_LD * 4;
   static constexpr int MISC_BYTES = 1024;              // mbarriers, row statistics
   static constexpr int PART_BYTES = 8 * D * 4;         // cross-attention partial outputs of the 8 key slices (one image)
@@ -131,19 +133,20 @@ struct A2Cfg {
   static constexpr int NSLOT = NSLOT_RAW > 8 ? 8 : NSLOT_RAW;
   static constexpr int SMEM = 1024 + NSLOT * A2_SLOT + FIXED;
   static_assert(NSLOT >= 3, "ring too shallow");
+  static_assert(IDP == 32 || IDP == 64, "id row pitch");
   static_assert(D % CS == 0 && DS % 8 == 0 && MS % 32 == 0, "slices");
   static_assert(DS * 128 <= A2_SLOT && NC1 * 128 <= A2_SLOT && NC2 * 128 <= A2_SLOT, "box fits a slot");
 };
 
-template <int D, int MT, int CS>
-constexpr size_t dec_ar2_smem_bytes() { return static_cast<size_t>(A2Cfg<D, MT, CS>::SMEM); }
+template <int D, int MT, int CS, int IDP = 32>
+constexpr size_t dec_ar2_smem_bytes() { return static_cast<size_t>(A2Cfg<D, MT, CS, IDP>::SMEM); }
 
 // ------------------------------------------------------------------------------------------------------------------
 // TMA ring: a static per-step program of slot fills; one thread issues, everybody consumes in program order.
 // WIDE: the head segment is this CTA's class slice, ceil(Cs / 128) chunks of KT [128 x 64] boxes.
-template <int D, int MT, int CS, bool WIDE = false>
+template <int D, int MT, int CS, bool WIDE = false, int IDP = 32>
 struct A2Ring {
-  using Cfg = A2Cfg<D, MT, CS>;
+  using Cfg = A2Cfg<D, MT, CS, IDP>;
   uint8_t* slots;
   uint64_t* full;
   const DecAr2Maps* maps;
@@ -299,9 +302,9 @@ __device__ __forceinline__ void mma_box(float (&acc)[NTW][4], const uint8_t* ati
 // so that the throughput instantiations carry none of its registers / branches.
 // WIDE: the class-sliced head for C > 128 (see the top of the file); `maps.wh` then has [128 x 64] boxes.  The body is
 // shared by two kernels, dec_ar2_kernel (WIDE = false) and dec_ar2_wide_kernel (WIDE = true).
-template <int D, int MT, int CS, bool HS, bool WIDE>
+template <int D, int MT, int CS, bool HS, bool WIDE, int IDP>
 __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr2Params p) {
-  using Cfg = A2Cfg<D, MT, CS>;
+  using Cfg = A2Cfg<D, MT, CS, IDP>;
   constexpr int ROWS = Cfg::ROWS, DS = Cfg::DS, KT = Cfg::KT, KT2 = Cfg::KT2, MS = Cfg::MS, MH = Cfg::MH, G = Cfg::G,
                 OWN = Cfg::OWN, H = Cfg::H;
   extern __shared__ uint8_t a2_smem_raw[];
@@ -318,7 +321,7 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
   __nv_bfloat16* s_ca = reinterpret_cast<__nv_bfloat16*>(sm);   sm += Cfg::CA_BYTES;
   float2* s_st = reinterpret_cast<float2*>(sm);                 sm += Cfg::ST_BYTES;    // [8 src][ROWS] (mean, M2)
   float* s_red = reinterpret_cast<float*>(sm);                  sm += Cfg::RED_BYTES;   // [2][8 warps][16 MH]
-  int* s_ids = reinterpret_cast<int*>(sm);                      sm += Cfg::IDS_BYTES;   // [ROWS][32]
+  int* s_ids = reinterpret_cast<int*>(sm);                      sm += Cfg::IDS_BYTES;   // [ROWS][IDP]
   float* s_log = reinterpret_cast<float*>(s_p);
   float2* s_mr = reinterpret_cast<float2*>(sm);                 sm += ROWS * 8;         // per row (mean, rstd)
   uint4* s_qf = reinterpret_cast<uint4*>(sm);                   sm += Cfg::QF_BYTES;    // [KT][4 k-steps][4 t]: hi01, hi89, lo01, lo89
@@ -345,8 +348,8 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
   for (int i = tid; i < (Cfg::A_BYTES + Cfg::R_BYTES + Cfg::HD_BYTES) / 16; i += A2_LAUNCH_THREADS)
     reinterpret_cast<uint4*>(s_a1)[i] = make_uint4(0u, 0u, 0u, 0u);
   grid_dep_wait();                    // weights / K/V cache / ids of the producing kernels are visible from here on
-  for (int i = tid; i < ROWS * 32; i += A2_LAUNCH_THREADS) {
-    const int r = i >> 5, c = i & 31;
+  for (int i = tid; i < ROWS * IDP; i += A2_LAUNCH_THREADS) {
+    const int r = i >> (IDP == 32 ? 5 : 6), c = i & (IDP - 1);
     s_ids[i] = (r < nrows) ? p.ids[static_cast<long long>(img0 + r) * p.ids_ld + c] : 0;
   }
   // Head-split cross-attention: with so few images that (images x 64-channel k-blocks) fit the cluster, every CTA takes ONE
@@ -356,7 +359,7 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
   const int hs_row = (hs && rank < nrows * KT) ? rank / KT : -1;
   const int hs_kb = hs ? rank % KT : 0;
   const int c_own = hs ? (hs_row >= 0 ? 1 : 0) : n_own;             // cross-attention passes of this CTA
-  A2Ring<D, MT, CS, WIDE> ring;
+  A2Ring<D, MT, CS, WIDE, IDP> ring;
   // WIDE: classes per CTA, a multiple of 8 (whole n8 tiles); the last slices may be short or empty
   const int h_cs = WIDE ? (((p.C + CS - 1) / CS + 7) & ~7) : 0;
   const int h_chunks = (h_cs + 127) / 128;
@@ -475,9 +478,12 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
   do {                                                                                                          \
     if (p.prof != nullptr && blockIdx.x == 0 && tid == 0 && step == 1) p.prof[26 * 16 + (slot)] = a2_timer_ns(); \
   } while (0)
+  // the [32][16] profile buffer: rows 0..25 are steps, row 26 the extra stamps of step 1 (A2_PROF4); the 64-pitch
+  // kernels (L > 32) record steps < 26 only
 #define A2_PROF(slot)                                                                                           \
   do {                                                                                                          \
-    if (p.prof != nullptr && blockIdx.x == 0 && tid == 0) p.prof[step * 16 + (slot)] = a2_timer_ns();           \
+    if (p.prof != nullptr && blockIdx.x == 0 && tid == 0 && (IDP == 32 || step < A2_PROF_STEPS))                \
+      p.prof[step * 16 + (slot)] = a2_timer_ns();                                                               \
   } while (0)
 
   for (int step = 0; step < p.L; ++step) {
@@ -493,7 +499,7 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
         const int itc = valid ? it : items - 1;
         const int oi = itc / (D / 8), ch = itc % (D / 8);
         const int r = rank + CS * oi;
-        const int* idr = s_ids + r * 32;
+        const int* idr = s_ids + r * IDP;
         float q[8];
         {
           const float4 q0 = __ldg(reinterpret_cast<const float4*>(p.qs + static_cast<long long>(step) * D + ch * 8));
@@ -1005,7 +1011,7 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
         if (step + 1 < p.L) {
           int v = bx;
           if (p.forced != nullptr) v = p.forced[b * p.forced_ld + step + 1];
-          s_ids[r * 32 + step + 1] = v;
+          s_ids[r * IDP + step + 1] = v;
           if ((r % CS) == rank) p.ids[b * p.ids_ld + step + 1] = v;     // one CTA stores the row
         }
       }
@@ -1050,7 +1056,7 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
         if (lane == 0 && step + 1 < p.L) {
           int v = bi;
           if (p.forced != nullptr) v = p.forced[b * p.forced_ld + step + 1];
-          s_ids[r * 32 + step + 1] = v;
+          s_ids[r * IDP + step + 1] = v;
           if (writer) p.ids[b * p.ids_ld + step + 1] = v;
         }
       }
@@ -1067,12 +1073,23 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
 template <int D, int MT, int CS, bool HS = false>
 __global__ void __launch_bounds__(A2_LAUNCH_THREADS, 1)
 dec_ar2_kernel(const __grid_constant__ DecAr2Maps maps, const DecAr2Params p) {
-  dec_ar2_body<D, MT, CS, HS, false>(maps, p);
+  dec_ar2_body<D, MT, CS, HS, false, 32>(maps, p);
 }
 template <int D, int MT, int CS, bool HS = false>
 __global__ void __launch_bounds__(A2_LAUNCH_THREADS, 1)
 dec_ar2_wide_kernel(const __grid_constant__ DecAr2Maps maps, const DecAr2Params p) {
-  dec_ar2_body<D, MT, CS, HS, true>(maps, p);
+  dec_ar2_body<D, MT, CS, HS, true, 32>(maps, p);
+}
+// labels of 32..63 characters (33..64 decode positions): ids rows of 64 in shared memory and in p.ids
+template <int D, int MT, int CS, bool HS = false>
+__global__ void __launch_bounds__(A2_LAUNCH_THREADS, 1)
+dec_ar2_long_kernel(const __grid_constant__ DecAr2Maps maps, const DecAr2Params p) {
+  dec_ar2_body<D, MT, CS, HS, false, 64>(maps, p);
+}
+template <int D, int MT, int CS, bool HS = false>
+__global__ void __launch_bounds__(A2_LAUNCH_THREADS, 1)
+dec_ar2_long_wide_kernel(const __grid_constant__ DecAr2Maps maps, const DecAr2Params p) {
+  dec_ar2_body<D, MT, CS, HS, true, 64>(maps, p);
 }
 
 // ------------------------------------------------------------------------------------------------------------------

@@ -25,6 +25,7 @@
 namespace {
 
 constexpr int kMaxHeadClasses = 16384;    // num_tokens - 2 (parseq_create)
+constexpr int kMaxLabelLength = 63;       // L = max_label_length + 1 <= 64 decode positions (parseq_create)
 
 thread_local std::string g_last_error;
 
@@ -209,27 +210,33 @@ int ln_head_argmax_launch(const LaunchOpts& lo, const float* y, const float* g, 
   }
 }
 
-// the cluster AR kernel of a head width: WIDE (> 128 classes) is the class-sliced head
-template <int D, int MT, int CS, bool HS, bool WIDE>
+// the cluster AR kernel of a head width and id row pitch: WIDE (> 128 classes) is the class-sliced head; IDP = 64 holds
+// labels of up to 63 characters (L <= 64), IDP = 32 the rest
+template <int D, int MT, int CS, bool HS, bool WIDE, int IDP>
 constexpr auto ar2_kernel() {
-  if constexpr (WIDE) return pq::dec_ar2_wide_kernel<D, MT, CS, HS>;
-  else return pq::dec_ar2_kernel<D, MT, CS, HS>;
+  if constexpr (IDP == 64) {
+    if constexpr (WIDE) return pq::dec_ar2_long_wide_kernel<D, MT, CS, HS>;
+    else return pq::dec_ar2_long_kernel<D, MT, CS, HS>;
+  } else {
+    if constexpr (WIDE) return pq::dec_ar2_wide_kernel<D, MT, CS, HS>;
+    else return pq::dec_ar2_kernel<D, MT, CS, HS>;
+  }
 }
-template <int D, int MT, int CS, bool WIDE>
+template <int D, int MT, int CS, bool WIDE, int IDP>
 int ar2_attr() {
-  PQ_CUDA(cudaFuncSetAttribute(ar2_kernel<D, MT, CS, false, WIDE>(), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               static_cast<int>(pq::dec_ar2_smem_bytes<D, MT, CS>())));
+  PQ_CUDA(cudaFuncSetAttribute(ar2_kernel<D, MT, CS, false, WIDE, IDP>(), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               static_cast<int>(pq::dec_ar2_smem_bytes<D, MT, CS, IDP>())));
   if constexpr (MT == 1 && CS == 8 && D / 64 <= CS)      // head-split variant for tiny batches
-    PQ_CUDA(cudaFuncSetAttribute(ar2_kernel<D, MT, CS, true, WIDE>(), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 static_cast<int>(pq::dec_ar2_smem_bytes<D, MT, CS>())));
+    PQ_CUDA(cudaFuncSetAttribute(ar2_kernel<D, MT, CS, true, WIDE, IDP>(), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 static_cast<int>(pq::dec_ar2_smem_bytes<D, MT, CS, IDP>())));
   return PARSEQ_OK;
 }
-template <bool WIDE>
+template <bool WIDE, int IDP>
 int ar2_set_attributes() {
-  PQ_TRY((ar2_attr<192, 1, 8, WIDE>())); PQ_TRY((ar2_attr<192, 2, 8, WIDE>())); PQ_TRY((ar2_attr<384, 1, 8, WIDE>()));
-  PQ_TRY((ar2_attr<384, 2, 8, WIDE>())); PQ_TRY((ar2_attr<768, 1, 8, WIDE>()));
-  PQ_TRY((ar2_attr<192, 1, 6, WIDE>())); PQ_TRY((ar2_attr<192, 2, 6, WIDE>())); PQ_TRY((ar2_attr<384, 1, 6, WIDE>()));
-  PQ_TRY((ar2_attr<384, 2, 6, WIDE>())); PQ_TRY((ar2_attr<768, 1, 6, WIDE>()));
+  PQ_TRY((ar2_attr<192, 1, 8, WIDE, IDP>())); PQ_TRY((ar2_attr<192, 2, 8, WIDE, IDP>())); PQ_TRY((ar2_attr<384, 1, 8, WIDE, IDP>()));
+  PQ_TRY((ar2_attr<384, 2, 8, WIDE, IDP>())); PQ_TRY((ar2_attr<768, 1, 8, WIDE, IDP>()));
+  PQ_TRY((ar2_attr<192, 1, 6, WIDE, IDP>())); PQ_TRY((ar2_attr<192, 2, 6, WIDE, IDP>())); PQ_TRY((ar2_attr<384, 1, 6, WIDE, IDP>()));
+  PQ_TRY((ar2_attr<384, 2, 6, WIDE, IDP>())); PQ_TRY((ar2_attr<768, 1, 6, WIDE, IDP>()));
   return PARSEQ_OK;
 }
 
@@ -260,8 +267,10 @@ int init_kernel_attributes() {
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar_kernel<384, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pq::dec_ar_smem_bytes<384>())));
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar_kernel<768, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pq::dec_ar_smem_bytes<768>())));
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar_kernel<768, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pq::dec_ar_smem_bytes<768>())));
-  PQ_TRY(ar2_set_attributes<false>());
-  PQ_TRY(ar2_set_attributes<true>());
+  PQ_TRY((ar2_set_attributes<false, 32>()));
+  PQ_TRY((ar2_set_attributes<true, 32>()));
+  PQ_TRY((ar2_set_attributes<false, 64>()));
+  PQ_TRY((ar2_set_attributes<true, 64>()));
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ln_head_argmax_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, 120 * 1024));
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ln_head_argmax_kernel<384>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
   PQ_CUDA(cudaFuncSetAttribute(pq::dec_ln_head_argmax_kernel<768>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
@@ -500,6 +509,7 @@ struct Slot {
 struct parseq_engine {
   parseq_config cfg;
   int D, T, Kp, Me, Md, L, V, C, gh, gw, dh_dec;   // T: tokens per image in the encoder (patches + class token if any)
+  int ids_ld = 32;                                   // row pitch of the decoder's id buffers: 32 (L <= 32) or 64 (L <= 64)
   int arch = 0, Tp = 0;                              // arch 1 = ViTSTR; Tp = gh * gw patches
   std::map<std::string, int> pub_index;
   float* vt_rows = nullptr;                          // ViTSTR tail: gathered token rows [chunk * L, D] fp32
@@ -534,21 +544,22 @@ struct parseq_engine {
   int ar2_occ[3][2] = {{0, 0}, {0, 0}, {0, 0}};        // what cudaOccupancyMaxActiveClusters answered (debug)
   int ar_last_cs = 0;
   int ar_last_per = 0, ar_last_ncl = 0;
+  int ar_last_mt = 0, ar_last_hs = 0, ar_last_wide = 0, ar_last_idp = 0;   // last cluster-kernel instantiation (debug)
   int ar_cs = 0;                    // option "ar_cluster_size": 0 = auto, 6 / 8 = forced
   int ar_clusters_override = 0;     // option "ar_clusters": clusters the AR kernel spreads a batch over (0 = derived)
   int fuse_mlp = 0;                 // fc1 + GELU + fc2 + residual + LayerNorm in one kernel (mlp_ln.cuh) where fuse_ln bit 1 applies
   int fuse_ln = 3;                  // bit 0: attn.proj, bit 1: mlp.fc2 also produce the LayerNorm that follows (gemm_ln.cuh)
   __nv_bfloat16 *ar_sa = nullptr, *ar_ca = nullptr, *ar_hd = nullptr;
   float *ar_y = nullptr, *ar_qc = nullptr, *ar_part = nullptr;
-  int* ar_ids = nullptr;
+  int* ar_ids = nullptr;            // [max_batch, ids_ld]
   unsigned int* ar_bar = nullptr;
-  unsigned long long* ar_prof = nullptr;   // [32][16] phase time stamps of the AR kernel (debug option "ar_prof")
+  unsigned long long* ar_prof = nullptr;   // [32][16] phase time stamps of the AR kernel (debug option "ar_prof"; DESIGN.md 4)
   bool ar_prof_on = false;
   cudaEvent_t ev_enc = nullptr;
   struct Stage {
     __nv_bfloat16 *sa = nullptr, *yn = nullptr, *ca = nullptr, *hd = nullptr;
     float *y = nullptr, *qc = nullptr;
-    int *ids_ar = nullptr, *ids_ctx = nullptr;
+    int *ids_ar = nullptr, *ids_ctx = nullptr;    // [dec_chunk, ids_ld]
     cudaStream_t stream = nullptr;
     cudaEvent_t ev_enc = nullptr, ev_done = nullptr;
   };
@@ -605,7 +616,7 @@ int alloc_workspace(parseq_engine* e) {
   PQ_TRY(dev_alloc(&e->ar_y, 1ll * e->max_batch * D));
   PQ_TRY(dev_alloc(&e->ar_qc, 1ll * e->max_batch * D));
   PQ_TRY(dev_alloc(&e->ar_part, 3ll * e->max_batch * D));
-  PQ_TRY(dev_alloc(&e->ar_ids, 1ll * e->max_batch * 32));
+  PQ_TRY(dev_alloc(&e->ar_ids, 1ll * e->max_batch * e->ids_ld));
   PQ_TRY(dev_alloc(&e->ar_bar, 64));
   PQ_TRY(dev_alloc(&e->ar_prof, 32 * 16));
   if (e->arch == 1) PQ_TRY(dev_alloc(&e->vt_rows, 1ll * e->chunk * e->L * D));
@@ -619,8 +630,8 @@ int alloc_workspace(parseq_engine* e) {
     PQ_TRY(dev_alloc(&sg.hd, Rd * e->Md));
     PQ_TRY(dev_alloc(&sg.y, Rd * D));
     PQ_TRY(dev_alloc(&sg.qc, Rd * D));
-    PQ_TRY(dev_alloc(&sg.ids_ar, static_cast<long long>(e->dec_chunk) * 32));
-    PQ_TRY(dev_alloc(&sg.ids_ctx, static_cast<long long>(e->dec_chunk) * 32));
+    PQ_TRY(dev_alloc(&sg.ids_ar, static_cast<long long>(e->dec_chunk) * e->ids_ld));
+    PQ_TRY(dev_alloc(&sg.ids_ctx, static_cast<long long>(e->dec_chunk) * e->ids_ld));
     PQ_CUDA(cudaStreamCreateWithFlags(&sg.stream, cudaStreamNonBlocking));
     PQ_CUDA(cudaEventCreateWithFlags(&sg.ev_enc, cudaEventDisableTiming));
     PQ_CUDA(cudaEventCreateWithFlags(&sg.ev_done, cudaEventDisableTiming));
@@ -831,7 +842,7 @@ int vitstr_tail(parseq_engine* e, int B, int L, float* logits, int* ids_out, cud
 
 // ---------------------------------------------------------------- one Decoder call (model.py:86-103, modules.py:55-125)
 // rows are (b, qi), qi in [0,nq); query position q0+qi; context ids[b, 0..nkeys-1].
-// Tail: LayerNorm(decoder.norm) + head + (optionally) greedy argmax -> ids_dst[b*32 + dst_off + qi] in one kernel.
+// Tail: LayerNorm(decoder.norm) + head + (optionally) greedy argmax -> ids_dst[b*ids_ld + dst_off + qi] in one kernel.
 // Caller-supplied pieces of PARSeq.decode (model.py:86-103) that the inference loops never use: explicit query rows,
 // explicit masks, decoder output instead of logits.
 struct DecodeExtras {
@@ -873,9 +884,10 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
   {
     TimedScope ts(e, st, CAT_DEC_ATTN, 4.0 * M * nkeys * D);
     const int qsplit = (nq >= 8) ? 4 : 1;
-    PQ_TRY(launch_k(e->lo, pq::dec_self_attn2_kernel, dim3(B * qsplit), dim3(D < 384 ? D : 384), 0, st, qself,
-                    static_cast<const __nv_bfloat16*>(e->kvtab), ids, 32, e->V, D, nq, q0, nkeys, mode, /*eos*/ 0, sg.sa,
-                    qsplit, qmask, pmask));
+    // one key per lane up to 32 keys, two up to 64 (the kernel of the engine's id pitch)
+    PQ_TRY(launch_k(e->lo, e->ids_ld == 32 ? pq::dec_self_attn2_kernel : pq::dec_self_attn2_long_kernel, dim3(B * qsplit),
+                    dim3(D < 384 ? D : 384), 0, st, qself, static_cast<const __nv_bfloat16*>(e->kvtab), ids, e->ids_ld, e->V,
+                    D, nq, q0, nkeys, mode, /*eos*/ 0, sg.sa, qsplit, qmask, pmask));
   }
   // y = query + out_proj(sa): the GEMM stores out_proj(sa) with its TMA epilogue, the LayerNorm kernel adds the query
   // residual (broadcast pos_queries[q0 + qi], or the caller's rows), writes y back and emits norm1(y)
@@ -920,11 +932,12 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
     PQ_TRY(gemm(e, sg.yn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, pq::EPI_F32, 1.0f, nullptr, 0, 0,
                 logits_out, logits_ld, st));
     if (ids_dst != nullptr)
-      PQ_TRY(argmax_rows(e, logits_out, static_cast<int>(logits_ld / e->C), B, nq, 0, ids_dst, 32, dst_off, forced, forced_ld, st));
+      PQ_TRY(argmax_rows(e, logits_out, static_cast<int>(logits_ld / e->C), B, nq, 0, ids_dst, e->ids_ld, dst_off, forced,
+                         forced_ld, st));
   } else {
     TimedScope ts(e, st, CAT_DEC_GEMM, 2.0 * M * e->C * D);
     PQ_TRY(ln_head_argmax_launch(e->lo, sg.y, e->wf("decoder.norm.weight"), e->wf("decoder.norm.bias"), 1e-5f, e->wb("head.weight"),
-                                 e->wf("head.bias"), M, e->C, D, logits_out, logits_ld, ids_dst, 32, nq, dst_off, forced,
+                                 e->wf("head.bias"), M, e->C, D, logits_out, logits_ld, ids_dst, e->ids_ld, nq, dst_off, forced,
                                  forced_ld, st));
   }
   return PARSEQ_OK;
@@ -951,7 +964,8 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
   if (a->decode_ar && ar_done) {
     // the AR loop of the whole super-chunk already ran in the persistent kernel (ar_decode)
   } else if (a->decode_ar) {
-    PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * 32 + 255) / 256), dim3(256), 0, st, sg.ids_ar, B, 32, bos, pad));
+    PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * e->ids_ld + 255) / 256), dim3(256), 0, st, sg.ids_ar, B, e->ids_ld,
+                    bos, pad));
     e->launches++;
     const int* forced = a->forced_ids ? a->forced_ids + static_cast<long long>(b0) * L : nullptr;
     for (int i = 0; i < L; ++i) {
@@ -960,22 +974,25 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
                          (i + 1 < L) ? sg.ids_ar : nullptr, i + 1, forced, L, st));
     }
     if (testing && steps != nullptr) {
-      PQ_TRY(launch_k(e->lo, pq::ar_steps_kernel, dim3(1), dim3(256), 0, st, static_cast<const int*>(sg.ids_ar), 32, B, L, 0, steps));
+      PQ_TRY(launch_k(e->lo, pq::ar_steps_kernel, dim3(1), dim3(256), 0, st, static_cast<const int*>(sg.ids_ar), e->ids_ld, B, L,
+                      0, steps));
       e->launches++;
     }
   } else {
-    PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * 32 + 255) / 256), dim3(256), 0, st, sg.ids_ctx, B, 32, bos, pad));
+    PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * e->ids_ld + 255) / 256), dim3(256), 0, st, sg.ids_ctx, B, e->ids_ld,
+                    bos, pad));
     e->launches++;
     PQ_TRY(decode_pass(e, sg, b_first, B, L, 0, 1, 0, sg.ids_ctx, logits, C, nullptr, 0, nullptr, 0, st));
   }
   for (int it = 0; it < a->refine_iters; ++it) {
-    PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * 32 + 255) / 256), dim3(256), 0, st, sg.ids_ctx, B, 32, bos, pad));
+    PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * e->ids_ld + 255) / 256), dim3(256), 0, st, sg.ids_ctx, B, e->ids_ld,
+                    bos, pad));
     e->launches++;
     const int* forced = a->forced_refine
                             ? a->forced_refine + (static_cast<long long>(it) * a->batch + b0) * L
                             : nullptr;
     // ctx = [BOS, argmax(logits[:, :L-1])]  (model.py:161)
-    PQ_TRY(argmax_rows(e, logits, L, B, L - 1, 0, sg.ids_ctx, 32, 1, forced, L, st));
+    PQ_TRY(argmax_rows(e, logits, L, B, L - 1, 0, sg.ids_ctx, e->ids_ld, 1, forced, L, st));
     PQ_TRY(decode_pass(e, sg, b_first, B, L, 0, L, 1, sg.ids_ctx, logits, C, nullptr, 0, nullptr, 0, st));
   }
   if (ids_out != nullptr) PQ_TRY(argmax_rows(e, logits, L, B, L, 0, ids_out, L, 0, nullptr, 0, st));
@@ -985,7 +1002,7 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
 
 // ---- cluster-owned AR kernel (dec_ar2.cuh) ----
 // Heads of <= 96 classes run redundantly in every CTA; > 128 classes take the class-sliced head (WIDE); 97..128 classes
-// stay on the grid-barrier kernel.
+// stay on the grid-barrier kernel (labels of up to 31 characters) or on the chain of separate kernels (longer labels).
 bool ar2_supported(const parseq_engine* e) {
   return e->arch == 0 && e->cfg.dec_mlp_ratio == 4 && (e->C <= 96 || e->C > 128) && e->T <= 256 && e->dh_dec == 32;
 }
@@ -1011,12 +1028,12 @@ int ar2_build_maps(parseq_engine* e) {
   e->ar2_maps_ok = true;
   return PARSEQ_OK;
 }
-template <int D, int MT, int CS>
+template <int D, int MT, int CS, int IDP>
 void ar2_config(parseq_engine* e, cudaLaunchConfig_t& cfg, cudaLaunchAttribute* attr, int ncl, cudaStream_t st) {
   cfg = cudaLaunchConfig_t{};
   cfg.gridDim = dim3(static_cast<unsigned>(ncl * CS));
   cfg.blockDim = dim3(pq::A2_LAUNCH_THREADS);
-  cfg.dynamicSmemBytes = pq::dec_ar2_smem_bytes<D, MT, CS>();
+  cfg.dynamicSmemBytes = pq::dec_ar2_smem_bytes<D, MT, CS, IDP>();
   cfg.stream = st;
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = CS;
@@ -1025,41 +1042,43 @@ void ar2_config(parseq_engine* e, cudaLaunchConfig_t& cfg, cudaLaunchAttribute* 
   cfg.attrs = attr;
   cfg.numAttrs = 1;
 }
-template <int D, int MT, int CS, bool WIDE>
+template <int D, int MT, int CS, bool WIDE, int IDP>
 int ar2_launch_t(parseq_engine* e, const pq::DecAr2Params& p, int ncl, cudaStream_t st) {
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[1];
-  ar2_config<D, MT, CS>(e, cfg, attr, ncl, st);
+  ar2_config<D, MT, CS, IDP>(e, cfg, attr, ncl, st);
   e->ar_last_per = p.per; e->ar_last_ncl = ncl; e->ar_last_cs = CS;
+  e->ar_last_mt = MT; e->ar_last_hs = 0; e->ar_last_wide = WIDE ? 1 : 0; e->ar_last_idp = IDP;
   if constexpr (MT == 1 && CS == 8 && D / 64 <= CS) {
     // so few images per cluster that (images x head pairs) fit its CTAs: every CTA takes one (image, head pair) of the
     // cross-attention instead of whole images (bs = 1: 9 -> 2.5 us per step; same bits per head)
     if (p.per * (D / 64) <= CS) {
-      PQ_CUDA(cudaLaunchKernelEx(&cfg, ar2_kernel<D, MT, CS, true, WIDE>(), e->ar2_maps[0], p));
+      e->ar_last_hs = 1;
+      PQ_CUDA(cudaLaunchKernelEx(&cfg, ar2_kernel<D, MT, CS, true, WIDE, IDP>(), e->ar2_maps[0], p));
       return PARSEQ_OK;
     }
   }
-  PQ_CUDA(cudaLaunchKernelEx(&cfg, ar2_kernel<D, MT, CS, false, WIDE>(), e->ar2_maps[CS == 6 ? 1 : 0], p));
+  PQ_CUDA(cudaLaunchKernelEx(&cfg, ar2_kernel<D, MT, CS, false, WIDE, IDP>(), e->ar2_maps[CS == 6 ? 1 : 0], p));
   return PARSEQ_OK;
 }
-template <int D, int MT, int CS>
+template <int D, int MT, int CS, int IDP>
 int ar2_launch(parseq_engine* e, const pq::DecAr2Params& p, int ncl, cudaStream_t st) {
-  return ar2_wide(e) ? ar2_launch_t<D, MT, CS, true>(e, p, ncl, st) : ar2_launch_t<D, MT, CS, false>(e, p, ncl, st);
+  return ar2_wide(e) ? ar2_launch_t<D, MT, CS, true, IDP>(e, p, ncl, st) : ar2_launch_t<D, MT, CS, false, IDP>(e, p, ncl, st);
 }
 // Clusters of this instantiation that can be co-resident, as the occupancy query answers for this device.  A cluster
 // lives inside one GPC, so clusters of 8 can leave SMs of a GPC idle and clusters of 6 may pack more SMs; a batch that
 // needs more clusters than fit runs in two waves.
-template <int D, int MT, int CS>
+template <int D, int MT, int CS, int IDP>
 int ar2_max_clusters(parseq_engine* e) {
   int& cache = e->ar2_clusters[MT][CS == 6 ? 1 : 0];
   if (cache > 0) return cache;
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[1];
-  ar2_config<D, MT, CS>(e, cfg, attr, e->lo.sm_count / CS, nullptr);
+  ar2_config<D, MT, CS, IDP>(e, cfg, attr, e->lo.sm_count / CS, nullptr);
   int n = 0;
-  // (the cache is per engine, and so is the head width)
-  const cudaError_t qe = ar2_wide(e) ? cudaOccupancyMaxActiveClusters(&n, ar2_kernel<D, MT, CS, false, true>(), &cfg)
-                                     : cudaOccupancyMaxActiveClusters(&n, ar2_kernel<D, MT, CS, false, false>(), &cfg);
+  // (the cache is per engine, and so are the head width and the id pitch)
+  const cudaError_t qe = ar2_wide(e) ? cudaOccupancyMaxActiveClusters(&n, ar2_kernel<D, MT, CS, false, true, IDP>(), &cfg)
+                                     : cudaOccupancyMaxActiveClusters(&n, ar2_kernel<D, MT, CS, false, false, IDP>(), &cfg);
   if (qe != cudaSuccess || n <= 0) {
     cudaGetLastError();
     n = (CS == 8) ? (e->lo.sm_count / 10) : 1;   // unknown: a conservative guess for 8, "do not use" for 6
@@ -1072,17 +1091,17 @@ int ar2_max_clusters(parseq_engine* e) {
 // Spread the batch over the co-resident clusters.  Candidates in order of per-step cost: clusters of 8 with one m16 row
 // tile, clusters of 8 with two, clusters of 6 (a third more weight bytes per CTA and step); the first that holds the
 // batch in ONE wave wins (the loop is latency-bound: a second wave doubles its time), else the fewest waves.
-template <int D>
+template <int D, int IDP>
 int ar2_dispatch(parseq_engine* e, pq::DecAr2Params& p, cudaStream_t st) {
   constexpr bool kHas2 = (D != 768);            // two m16 tiles of D = 768 rows do not fit shared memory
   struct Cand { int mt, cs, maxc, rows; };
   Cand c[4];
   int nc = 0;
   const bool allow6 = e->ar_cs != 8, allow8 = e->ar_cs != 6;
-  if (allow8) c[nc++] = Cand{1, 8, ar2_max_clusters<D, 1, 8>(e), 16};
-  if constexpr (kHas2) { if (allow8) c[nc++] = Cand{2, 8, ar2_max_clusters<D, 2, 8>(e), 32}; }
-  if (allow6) c[nc++] = Cand{1, 6, ar2_max_clusters<D, 1, 6>(e), 16};
-  if constexpr (kHas2) { if (allow6) c[nc++] = Cand{2, 6, ar2_max_clusters<D, 2, 6>(e), 32}; }
+  if (allow8) c[nc++] = Cand{1, 8, ar2_max_clusters<D, 1, 8, IDP>(e), 16};
+  if constexpr (kHas2) { if (allow8) c[nc++] = Cand{2, 8, ar2_max_clusters<D, 2, 8, IDP>(e), 32}; }
+  if (allow6) c[nc++] = Cand{1, 6, ar2_max_clusters<D, 1, 6, IDP>(e), 16};
+  if constexpr (kHas2) { if (allow6) c[nc++] = Cand{2, 6, ar2_max_clusters<D, 2, 6, IDP>(e), 32}; }
   int best = -1, best_waves = 1 << 30;
   for (int i = 0; i < nc; ++i) {
     const int need = (p.B + c[i].rows - 1) / c[i].rows;             // clusters at full rows
@@ -1096,11 +1115,11 @@ int ar2_dispatch(parseq_engine* e, pq::DecAr2Params& p, cudaStream_t st) {
   p.per = per;
   const int ncl = (p.B + per - 1) / per;
   if (k.cs == 8) {
-    if (k.mt == 1) return ar2_launch<D, 1, 8>(e, p, ncl, st);
-    if constexpr (kHas2) return ar2_launch<D, 2, 8>(e, p, ncl, st);
+    if (k.mt == 1) return ar2_launch<D, 1, 8, IDP>(e, p, ncl, st);
+    if constexpr (kHas2) return ar2_launch<D, 2, 8, IDP>(e, p, ncl, st);
   } else {
-    if (k.mt == 1) return ar2_launch<D, 1, 6>(e, p, ncl, st);
-    if constexpr (kHas2) return ar2_launch<D, 2, 6>(e, p, ncl, st);
+    if (k.mt == 1) return ar2_launch<D, 1, 6, IDP>(e, p, ncl, st);
+    if constexpr (kHas2) return ar2_launch<D, 2, 6, IDP>(e, p, ncl, st);
   }
   return fail(PARSEQ_ERR_STATE, "dec_ar2: no launch configuration");
 }
@@ -1110,7 +1129,8 @@ int ar_decode(parseq_engine* e, const parseq_forward_args* a, int b0, int B, int
   const int D = e->D;
   const std::string Ly = "decoder.layers.0.";
   const bool testing = a->max_length < 0;
-  PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * 32 + 255) / 256), dim3(256), 0, st, e->ar_ids, B, 32, e->V - 2, e->V - 1));
+  PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * e->ids_ld + 255) / 256), dim3(256), 0, st, e->ar_ids, B, e->ids_ld,
+                  e->V - 2, e->V - 1));
   e->launches++;
   if (e->ar_impl == 2 && ar2_supported(e)) {
     if (!e->ar2_maps_ok) PQ_TRY(ar2_build_maps(e));
@@ -1125,27 +1145,30 @@ int ar_decode(parseq_engine* e, const parseq_forward_args* a, int b0, int B, int
     q.g1 = e->wf(Ly + "norm1.weight"); q.be1 = e->wf(Ly + "norm1.bias");
     q.g2 = e->wf(Ly + "norm2.weight"); q.be2 = e->wf(Ly + "norm2.bias");
     q.g3 = e->wf("decoder.norm.weight"); q.be3 = e->wf("decoder.norm.bias");
-    q.ids = e->ar_ids; q.ids_ld = 32; q.logits = logits;
+    q.ids = e->ar_ids; q.ids_ld = e->ids_ld; q.logits = logits;
     q.forced = a->forced_ids ? a->forced_ids + static_cast<long long>(b0) * L : nullptr;
     q.forced_ld = L;
     q.prof = e->ar_prof_on ? e->ar_prof : nullptr;
     {
       const double macs = static_cast<double>(B) * L * (3.0 * D * D + 2.0 * D * e->Md + 1.0 * e->C * D + 2.0 * e->T * D);
       TimedScope ts(e, st, CAT_DEC_AR, 2.0 * macs);
+      const bool lng = e->ids_ld == 64;
       switch (D) {
-        case 192: PQ_TRY(ar2_dispatch<192>(e, q, st)); break;
-        case 384: PQ_TRY(ar2_dispatch<384>(e, q, st)); break;
-        case 768: PQ_TRY(ar2_dispatch<768>(e, q, st)); break;
+        case 192: PQ_TRY((lng ? ar2_dispatch<192, 64>(e, q, st) : ar2_dispatch<192, 32>(e, q, st))); break;
+        case 384: PQ_TRY((lng ? ar2_dispatch<384, 64>(e, q, st) : ar2_dispatch<384, 32>(e, q, st))); break;
+        case 768: PQ_TRY((lng ? ar2_dispatch<768, 64>(e, q, st) : ar2_dispatch<768, 32>(e, q, st))); break;
         default: return fail(PARSEQ_ERR_UNSUPPORTED, "dec_ar2: embed_dim must be 192, 384 or 768");
       }
     }
     if (testing && steps != nullptr) {
-      PQ_TRY(launch_k(e->lo, pq::ar_steps_kernel, dim3(1), dim3(256), 0, st, static_cast<const int*>(e->ar_ids), 32, B, L, 0, steps));
+      PQ_TRY(launch_k(e->lo, pq::ar_steps_kernel, dim3(1), dim3(256), 0, st, static_cast<const int*>(e->ar_ids), e->ids_ld, B, L,
+                      0, steps));
       e->launches++;
     }
     return PARSEQ_OK;
   }
   if (e->C > 128) return fail(PARSEQ_ERR_UNSUPPORTED, "ar_kernel = 1 (grid-barrier AR kernel) covers at most 128 head classes");
+  if (e->L > 32) return fail(PARSEQ_ERR_UNSUPPORTED, "ar_kernel = 1 (grid-barrier AR kernel) covers max_label_length <= 31");
   PQ_CUDA(cudaMemsetAsync(e->ar_bar, 0, 64, st));
   pq::DecArParams p;
   p.B = B; p.L = L; p.Md = e->Md; p.V = e->V; p.C = e->C; p.T = e->T; p.heads = e->cfg.dec_num_heads;
@@ -1160,7 +1183,7 @@ int ar_decode(parseq_engine* e, const parseq_forward_args* a, int b0, int B, int
   p.g1 = e->wf(Ly + "norm1.weight"); p.be1 = e->wf(Ly + "norm1.bias");
   p.g2 = e->wf(Ly + "norm2.weight"); p.be2 = e->wf(Ly + "norm2.bias");
   p.g3 = e->wf("decoder.norm.weight"); p.be3 = e->wf("decoder.norm.bias");
-  p.ckv = e->ckv; p.kv_rows = 1ll * e->max_batch * e->T; p.ids = e->ar_ids; p.ids_ld = 32;
+  p.ckv = e->ckv; p.kv_rows = 1ll * e->max_batch * e->T; p.ids = e->ar_ids; p.ids_ld = e->ids_ld;
   p.sa = e->ar_sa; p.ca = e->ar_ca; p.hd = e->ar_hd; p.y = e->ar_y; p.qc = e->ar_qc; p.part = e->ar_part;
   p.logits = logits;
   p.forced = a->forced_ids ? a->forced_ids + static_cast<long long>(b0) * L : nullptr;
@@ -1189,7 +1212,8 @@ int ar_decode(parseq_engine* e, const parseq_forward_args* a, int b0, int B, int
     }
   }
   if (testing && steps != nullptr) {
-    PQ_TRY(launch_k(e->lo, pq::ar_steps_kernel, dim3(1), dim3(256), 0, st, static_cast<const int*>(e->ar_ids), 32, B, L, 0, steps));
+    PQ_TRY(launch_k(e->lo, pq::ar_steps_kernel, dim3(1), dim3(256), 0, st, static_cast<const int*>(e->ar_ids), e->ids_ld, B, L, 0,
+                    steps));
     e->launches++;
   }
   return PARSEQ_OK;
@@ -1237,8 +1261,10 @@ int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B,
     PQ_TRY(gemm(e, e->mem, D, Wkv, D, bkv, B * T, 2 * D, D, pq::EPI_BF16, 1.0f, nullptr, 0, 0, e->ckv, 2 * D, e->main,
                 1ll * e->max_batch * T));
   }
-  // a head of > 128 classes that the cluster kernel cannot take (e.g. dec_mlp_ratio != 4) runs the AR loop as a chain
-  const bool ar_done = a->decode_ar && e->use_ar_kernel && !(e->ar_impl == 2 && e->C > 128 && !ar2_supported(e));
+  // an AR loop that the cluster kernel cannot take (e.g. dec_mlp_ratio != 4) runs on the grid-barrier kernel if that holds
+  // it (<= 128 classes, L <= 32), else as a chain of separate kernels
+  const bool ar_done = a->decode_ar && e->use_ar_kernel &&
+                       ((e->ar_impl == 2 && ar2_supported(e)) || (e->C <= 128 && e->L <= 32));
   if (ar_done) {
     PQ_TRY(ar_decode(e, a, b0, B, L, logits, steps, e->main));
     if (a->refine_iters == 0) {      // nothing left for the chains but the final argmax
@@ -1392,10 +1418,12 @@ int parseq_create(const parseq_config* cfg, parseq_engine** out) {
   if (D != 192 && D != 384 && D != 768) return fail(PARSEQ_ERR_UNSUPPORTED, "embed_dim must be 192, 384 or 768");
   if (D != cfg->enc_num_heads * 64) return fail(PARSEQ_ERR_UNSUPPORTED, "encoder head_dim must be 64");
   if (!vitstr && D != cfg->dec_num_heads * 32) return fail(PARSEQ_ERR_UNSUPPORTED, "decoder head_dim must be 32");
-  if (cfg->max_label_length + 1 > 32) return fail(PARSEQ_ERR_UNSUPPORTED, "max_label_length must be <= 31");
+  // L = max_label_length + 1 <= 64 decode positions: the decoder's id rows are 32 or 64 wide (DESIGN.md section 4)
+  if (cfg->max_label_length > kMaxLabelLength)
+    return fail(PARSEQ_ERR_UNSUPPORTED, "max_label_length must be <= 63 (labels of at most 63 characters)");
   if (cfg->max_label_length < 0) return fail(PARSEQ_ERR_INVALID_ARG, "negative max_label_length");
   // at most 16384 head classes (charset_train of <= 16383 characters): every index into the (position, token) K/V table
-  // [L * V, 2D] stays in int32 (32 * 16386 * 1536 < 2^31) and the table stays below 1.7 GB (DESIGN.md section 4)
+  // [L * V, 2D] stays in int32 (64 * 16386 * 1536 < 2^31); the table is at most 3.2 GB (DESIGN.md section 4)
   if (cfg->num_tokens < 4 || cfg->num_tokens - 2 > kMaxHeadClasses)
     return fail(PARSEQ_ERR_UNSUPPORTED, "num_tokens must be in [4, 16386] (at most 16384 head classes, charset_train of "
                                         "at most 16383 characters)");
@@ -1423,6 +1451,7 @@ int parseq_create(const parseq_config* cfg, parseq_engine** out) {
   e->Me = D * cfg->enc_mlp_ratio;
   e->Md = D * cfg->dec_mlp_ratio;
   e->L = cfg->max_label_length + 1;
+  e->ids_ld = e->L <= 32 ? 32 : 64;
   e->V = cfg->num_tokens;
   e->C = cfg->num_tokens - 2;
   e->dh_dec = D / cfg->dec_num_heads;
@@ -1722,7 +1751,7 @@ int parseq_decode(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t num_
     e->cur_cat = CAT_DEC_GEMM;
     PQ_TRY(gemm(e, e->mem, D, Wkv, D, bkv, Bc * T, 2 * D, D, pq::EPI_BF16, 1.0f, nullptr, 0, 0, e->ckv, 2 * D, st,
                 1ll * e->max_batch * T));
-    pq::copy_ids_kernel<<<(Bc * 32 + 255) / 256, 256, 0, st>>>(tgt + 1ll * b0 * J, J, sg.ids_ctx, Bc);
+    pq::copy_ids_kernel<<<(Bc * e->ids_ld + 255) / 256, 256, 0, st>>>(tgt + 1ll * b0 * J, J, sg.ids_ctx, Bc, e->ids_ld);
     PQ_CUDA(cudaGetLastError());
     e->launches += 2;
     DecodeExtras ex;
@@ -1816,6 +1845,10 @@ int64_t parseq_debug_int(parseq_engine* e, const char* name) {
   if (n == "ar_last_cluster_size") return e->ar_last_cs;
   if (n == "ar_last_per") return e->ar_last_per;
   if (n == "ar_last_clusters") return e->ar_last_ncl;
+  if (n == "ar_last_mt") return e->ar_last_mt;
+  if (n == "ar_last_head_split") return e->ar_last_hs;
+  if (n == "ar_last_wide") return e->ar_last_wide;
+  if (n == "ar_last_ids_pitch") return e->ar_last_idp;
   if (n == "sm_count") return e->lo.sm_count;
   return -1;
 }
@@ -1906,6 +1939,9 @@ int parseq_set_option(parseq_engine* e, const char* name, int64_t value) {
     if (value < 0 || value > 2) return fail(PARSEQ_ERR_INVALID_ARG, "ar_kernel: 0 / 1 / 2");
     if (value == 1 && e->C > 128)
       return fail(PARSEQ_ERR_UNSUPPORTED, "ar_kernel = 1 (grid-barrier AR kernel) covers at most 128 head classes; "
+                                          "use ar_kernel 0 or 2");
+    if (value == 1 && e->L > 32)
+      return fail(PARSEQ_ERR_UNSUPPORTED, "ar_kernel = 1 (grid-barrier AR kernel) covers max_label_length <= 31; "
                                           "use ar_kernel 0 or 2");
     e->use_ar_kernel = value != 0;
     e->ar_impl = value == 1 ? 1 : 2;

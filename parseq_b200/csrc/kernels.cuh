@@ -461,8 +461,9 @@ __global__ void set_int_kernel(int* p, int v) {
 
 // ---------------------------------------------------------------------------------------------
 // Decoder self-attention, one CTA per image, one warp per head (head dim 32), ALL nq queries of the pass:
-// the context K rows (lane = key, <= 32 keys) and V columns (lane = channel) of the head are gathered once from the
-// (position, token) table into registers, then every query costs ~130 warp instructions.
+// the context K rows (lane = key, KPL keys per lane: key lane + 32 u) and V columns (lane = channel) of the head are
+// gathered once from the (position, token) table into registers, then every query costs ~130 warp instructions per
+// 32 keys.  KPL = 1 holds up to 32 keys (L <= 32), KPL = 2 up to 64 (labels of up to 63 characters).
 // (DecoderLayer.forward_stream step 1, modules.py:69-72)
 //   q      : Qs[qpos] fp32 (W_q LN_q(pos_queries[qpos]) + b, pre-scaled by 1/sqrt(32); input independent)
 //   K/V    : kvtab[(k*V + ids[b,k]) * 2D + {0, D} + c] bf16   (the content stream is a function of
@@ -474,13 +475,16 @@ __global__ void set_int_kernel(int* p, int v) {
 //            mode 2 (PARSeq.decode with caller-supplied masks, model.py:86-103): Qs holds one query row per (image,
 //            query) [B*nq, D]; key k of query qi is masked iff qmask[qi*nkeys + k] or pmask[b*nkeys + k] (either may be
 //            null); a row with every key masked yields NaN, as torch's softmax over -inf does
-__global__ void dec_self_attn2_kernel(const float* __restrict__ Qs, const __nv_bfloat16* __restrict__ kvtab,
-                                      const int* __restrict__ ids, int ids_ld, int V, int D, int nq, int q0, int nkeys,
-                                      int mode, int eos_id, __nv_bfloat16* __restrict__ out, int qsplit,
-                                      const unsigned char* __restrict__ qmask = nullptr,
-                                      const unsigned char* __restrict__ pmask = nullptr) {
+template <int KPL>
+__device__ __forceinline__ void dec_self_attn2_body(const float* __restrict__ Qs, const __nv_bfloat16* __restrict__ kvtab,
+                                                    const int* __restrict__ ids, int ids_ld, int V, int D, int nq, int q0,
+                                                    int nkeys, int mode, int eos_id, __nv_bfloat16* __restrict__ out,
+                                                    int qsplit, const unsigned char* __restrict__ qmask,
+                                                    const unsigned char* __restrict__ pmask) {
+  constexpr int NK = 32 * KPL;                          // keys held by one warp
   // grid = B * qsplit: CTA (b, part) handles queries [part*nq/qsplit, (part+1)*nq/qsplit) of image b
-  __shared__ int s_ids[32];
+  __shared__ int s_ids[NK];
+  __shared__ unsigned s_eos[KPL];                       // EOS ballot of each 32-key group (KPL > 1)
   __shared__ int s_first_eos;
   grid_dep_launch();
   grid_dep_wait();
@@ -488,63 +492,139 @@ __global__ void dec_self_attn2_kernel(const float* __restrict__ Qs, const __nv_b
   const int q_begin = (part * nq) / qsplit, q_end = ((part + 1) * nq) / qsplit;
   const int lane = threadIdx.x & 31;
   const int heads = D >> 5, nwarps = blockDim.x >> 5;   // blockDim.x = min(D, 384): heads are looped when D > 384
-  if (threadIdx.x < 32) {
+  if (threadIdx.x < NK) {
     const int id = (threadIdx.x < nkeys) ? ids[static_cast<long long>(b) * ids_ld + threadIdx.x] : -1;
     s_ids[threadIdx.x] = id;
     const unsigned m = __ballot_sync(0xffffffffu, id == eos_id);
-    if (threadIdx.x == 0) s_first_eos = (m != 0u) ? (__ffs(m) - 1) : (1 << 30);
+    if constexpr (KPL == 1) {
+      if (threadIdx.x == 0) s_first_eos = (m != 0u) ? (__ffs(m) - 1) : (1 << 30);
+    } else {
+      if (lane == 0) s_eos[threadIdx.x >> 5] = m;
+    }
   }
   __syncthreads();
+  if constexpr (KPL > 1) {                              // the first EOS is in the first group whose ballot is not empty
+    if (threadIdx.x == 0) {
+      int f = 1 << 30;
+#pragma unroll
+      for (int u = KPL - 1; u >= 0; --u)
+        if (s_eos[u] != 0u) f = 32 * u + __ffs(s_eos[u]) - 1;
+      s_first_eos = f;
+    }
+    __syncthreads();
+  }
   const int first_eos = s_first_eos;
   for (int h = threadIdx.x >> 5; h < heads; h += nwarps) {
-  float kreg[32], vreg[32];
-  if (lane < nkeys) {
-    const uint4* kr = reinterpret_cast<const uint4*>(kvtab + (static_cast<long long>(lane) * V + s_ids[lane]) * 2 * D + h * 32);
+  float kreg[KPL][32], vreg[NK];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const uint4 u = __ldg(kr + j);
-      const __nv_bfloat162* p2 = reinterpret_cast<const __nv_bfloat162*>(&u);
+  for (int u = 0; u < KPL; ++u) {
+    const int key = lane + 32 * u;
+    if (key < nkeys) {
+      const uint4* kr = reinterpret_cast<const uint4*>(kvtab + (static_cast<long long>(key) * V + s_ids[key]) * 2 * D + h * 32);
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float2 f = __bfloat1622float2(p2[e]);
-        kreg[j * 8 + e * 2] = f.x;
-        kreg[j * 8 + e * 2 + 1] = f.y;
+      for (int j = 0; j < 4; ++j) {
+        const uint4 w = __ldg(kr + j);
+        const __nv_bfloat162* p2 = reinterpret_cast<const __nv_bfloat162*>(&w);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float2 f = __bfloat1622float2(p2[e]);
+          kreg[u][j * 8 + e * 2] = f.x;
+          kreg[u][j * 8 + e * 2 + 1] = f.y;
+        }
       }
-    }
-  } else {
+    } else {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) kreg[j] = 0.f;
+      for (int j = 0; j < 32; ++j) kreg[u][j] = 0.f;
+    }
   }
 #pragma unroll
-  for (int k = 0; k < 32; ++k)
+  for (int k = 0; k < NK; ++k)
     vreg[k] = (k < nkeys) ? __bfloat162float(kvtab[(static_cast<long long>(k) * V + s_ids[k]) * 2 * D + D + h * 32 + lane]) : 0.f;
   for (int qi = q_begin; qi < q_end; ++qi) {
     const int qpos = q0 + qi;
     const long long qrow = (mode == 2) ? (static_cast<long long>(b) * nq + qi) : qpos;
     const float qv = __ldg(Qs + qrow * D + h * 32 + lane);   // lane j holds q_j
-    float s = 0.f;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) s = fmaf(__shfl_sync(0xffffffffu, qv, j), kreg[j], s);
-    bool masked = (lane >= nkeys) || ((mode == 1) && (lane == qpos + 1 || lane >= first_eos));
-    if (mode == 2 && lane < nkeys) {
-      if (qmask != nullptr && qmask[qi * nkeys + lane] != 0) masked = true;
-      if (pmask != nullptr && pmask[static_cast<long long>(b) * nkeys + lane] != 0) masked = true;
-    }
-    if (masked) s = -INFINITY;
-    float mx = s;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    const float e = masked ? 0.f : expf(s - mx);
-    float sum = e;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    const float pme = e / sum;
     float acc = 0.f;
+    if constexpr (KPL == 1) {
+      float s = 0.f;
 #pragma unroll
-    for (int k = 0; k < 32; ++k) acc = fmaf(__shfl_sync(0xffffffffu, pme, k), vreg[k], acc);
+      for (int j = 0; j < 32; ++j) s = fmaf(__shfl_sync(0xffffffffu, qv, j), kreg[0][j], s);
+      bool masked = (lane >= nkeys) || ((mode == 1) && (lane == qpos + 1 || lane >= first_eos));
+      if (mode == 2 && lane < nkeys) {
+        if (qmask != nullptr && qmask[qi * nkeys + lane] != 0) masked = true;
+        if (pmask != nullptr && pmask[static_cast<long long>(b) * nkeys + lane] != 0) masked = true;
+      }
+      if (masked) s = -INFINITY;
+      float mx = s;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+      const float e = masked ? 0.f : expf(s - mx);
+      float sum = e;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+      const float pme = e / sum;
+#pragma unroll
+      for (int k = 0; k < 32; ++k) acc = fmaf(__shfl_sync(0xffffffffu, pme, k), vreg[k], acc);
+    } else {
+      // scores of keys lane and lane + 32 (and so on), one shared max / sum over all of them
+      float s[KPL];
+#pragma unroll
+      for (int u = 0; u < KPL; ++u) s[u] = 0.f;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const float qj = __shfl_sync(0xffffffffu, qv, j);
+#pragma unroll
+        for (int u = 0; u < KPL; ++u) s[u] = fmaf(qj, kreg[u][j], s[u]);
+      }
+      bool masked[KPL];
+#pragma unroll
+      for (int u = 0; u < KPL; ++u) {
+        const int key = lane + 32 * u;
+        masked[u] = (key >= nkeys) || ((mode == 1) && (key == qpos + 1 || key >= first_eos));
+        if (mode == 2 && key < nkeys) {
+          if (qmask != nullptr && qmask[qi * nkeys + key] != 0) masked[u] = true;
+          if (pmask != nullptr && pmask[static_cast<long long>(b) * nkeys + key] != 0) masked[u] = true;
+        }
+        if (masked[u]) s[u] = -INFINITY;
+      }
+      float mx = s[0];
+#pragma unroll
+      for (int u = 1; u < KPL; ++u) mx = fmaxf(mx, s[u]);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+      float e[KPL];
+#pragma unroll
+      for (int u = 0; u < KPL; ++u) e[u] = masked[u] ? 0.f : expf(s[u] - mx);
+      float sum = e[0];
+#pragma unroll
+      for (int u = 1; u < KPL; ++u) sum += e[u];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+#pragma unroll
+      for (int u = 0; u < KPL; ++u) {
+        const float pme = e[u] / sum;
+#pragma unroll
+        for (int k = 0; k < 32; ++k) acc = fmaf(__shfl_sync(0xffffffffu, pme, k), vreg[u * 32 + k], acc);
+      }
+    }
     out[(static_cast<long long>(b) * nq + qi) * D + h * 32 + lane] = __float2bfloat16_rn(acc);
   }
   }
+}
+// up to 32 keys (L <= 32)
+__global__ void dec_self_attn2_kernel(const float* __restrict__ Qs, const __nv_bfloat16* __restrict__ kvtab,
+                                      const int* __restrict__ ids, int ids_ld, int V, int D, int nq, int q0, int nkeys,
+                                      int mode, int eos_id, __nv_bfloat16* __restrict__ out, int qsplit,
+                                      const unsigned char* __restrict__ qmask = nullptr,
+                                      const unsigned char* __restrict__ pmask = nullptr) {
+  dec_self_attn2_body<1>(Qs, kvtab, ids, ids_ld, V, D, nq, q0, nkeys, mode, eos_id, out, qsplit, qmask, pmask);
+}
+// up to 64 keys (labels of up to 63 characters); 384 threads at most, so that K and V of 64 keys stay in registers
+__global__ void __launch_bounds__(384) dec_self_attn2_long_kernel(
+    const float* __restrict__ Qs, const __nv_bfloat16* __restrict__ kvtab, const int* __restrict__ ids, int ids_ld, int V,
+    int D, int nq, int q0, int nkeys, int mode, int eos_id, __nv_bfloat16* __restrict__ out, int qsplit,
+    const unsigned char* __restrict__ qmask = nullptr, const unsigned char* __restrict__ pmask = nullptr) {
+  dec_self_attn2_body<2>(Qs, kvtab, ids, ids_ld, V, D, nq, q0, nkeys, mode, eos_id, out, qsplit, qmask, pmask);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -879,10 +959,10 @@ __global__ void bcast_rows_kernel(const float4* __restrict__ src, float4* __rest
        i += static_cast<long long>(gridDim.x) * blockDim.x)
     dst[i] = src[i % n4];
 }
-// ids [B, J] (row pitch J) -> context buffer [B, 32]
-__global__ void copy_ids_kernel(const int* __restrict__ src, int J, int* __restrict__ dst, int B) {
+// ids [B, J] (row pitch J) -> context buffer [B, ld]
+__global__ void copy_ids_kernel(const int* __restrict__ src, int J, int* __restrict__ dst, int B, int ld) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < B * 32) dst[i] = ((i & 31) < J) ? src[(i >> 5) * J + (i & 31)] : 0;
+  if (i < B * ld) dst[i] = ((i % ld) < J) ? src[(i / ld) * J + (i % ld)] : 0;
 }
 // TokenEmbedding.forward (modules.py:175-176): out[i, :] = sqrt(D) * E[ids[i], :]
 __global__ void text_embed_kernel(const int* __restrict__ ids, const float* __restrict__ E, float* __restrict__ out, int n,

@@ -40,7 +40,7 @@ typedef struct parseq_config {
   int32_t patch_h, patch_w;              /* patch_size   */
   int32_t embed_dim;
   int32_t enc_num_heads, enc_mlp_ratio, enc_depth;
-  int32_t dec_num_heads, dec_mlp_ratio, dec_depth;   /* dec_depth must be 1 (all reference configs) */
+  int32_t dec_num_heads, dec_mlp_ratio, dec_depth;   /* dec_depth >= 1 decoder layers (1 in every reference config) */
   int32_t max_label_length;              /* 25 -> 26 decode positions; 0..63 (labels of up to 63 characters) */
   int32_t num_tokens;                    /* 97: EOS=0, chars 1..94, BOS=95, PAD=96 (data/utils.py:102-111); 4..16386
                                             (at most 16384 head classes, e.g. CJK charsets) */
@@ -121,16 +121,22 @@ int parseq_postprocess(const float* logits, int32_t batch, int32_t num_steps, in
 int parseq_encode(parseq_engine* e, int32_t batch, const float* images, float* memory,
                   parseq_stream_t stream);
 
-/* Replaces model.PARSeq.decode (strhub/models/parseq/model.py:86-103 -> modules.py:55-125, depth-1 decoder: query stream
- * only): tgt DEVICE int32 [N, J] context ids (tgt[:, 0] = BOS; token k >= 1 receives pos_queries[k-1], model.py:96-99),
+/* Replaces model.PARSeq.decode (strhub/models/parseq/model.py:86-103 -> modules.py:55-125): tgt DEVICE int32 [N, J] context ids (tgt[:, 0] = BOS; token k >= 1 receives pos_queries[k-1], model.py:96-99),
  * memory DEVICE fp32 [N, T, D] (what parseq_encode returns), query DEVICE fp32 [N, NQ, D] or NULL (= pos_queries[:NQ],
  * model.py:100-101), query_mask DEVICE uint8 [NQ, J] or NULL (1 = key masked for that query: the bool `tgt_query_mask`),
  * padding_mask DEVICE uint8 [N, J] or NULL (`tgt_padding_mask`); out DEVICE fp32 [N, NQ, D] = Decoder output including
  * the final LayerNorm (modules.py:123-125).  1 <= J, NQ <= max_label_length + 1.  A query whose keys are all masked
- * yields NaN, as the reference's softmax does.  `tgt_mask` (content stream) has no effect at decoder depth 1. */
+ * yields NaN, as the reference's softmax does.  Same as parseq_decode_ex with content_mask = NULL. */
 int parseq_decode(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t num_queries, const int32_t* tgt,
                   const float* memory, const float* query, const uint8_t* query_mask, const uint8_t* padding_mask,
                   float* out, parseq_stream_t stream);
+/* parseq_decode with the content-stream mask `tgt_mask`: content_mask DEVICE uint8 [J, J] or NULL (unmasked, as
+ * tgt_mask=None is), 1 = key masked for that context row; the padding mask applies to the content rows too.  Decoders of
+ * depth >= 2 update the content stream in every layer but the last (modules.py:117-123), so the mask acts there; at
+ * depth 1 the content stream is never updated and the mask has no effect. */
+int parseq_decode_ex(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t num_queries, const int32_t* tgt,
+                     const float* memory, const float* query, const uint8_t* query_mask, const uint8_t* padding_mask,
+                     const uint8_t* content_mask, float* out, parseq_stream_t stream);
 /* Replaces model.PARSeq.head (model.py:63: nn.Linear(embed_dim, num_tokens - 2)): x DEVICE fp32 [rows, D] ->
  * logits DEVICE fp32 [rows, num_tokens - 2] (bf16 tensor-core operands, fp32 accumulate). */
 int parseq_head(parseq_engine* e, int32_t rows, const float* x, float* logits, parseq_stream_t stream);
@@ -153,7 +159,7 @@ int64_t parseq_debug_int(parseq_engine* e, const char* name);
  * for parseq_get_timing; 0: off + clear), "block_n" (accepted for compatibility: the GEMM has one 128 x 128 tile), "fuse_ln" (bit 0: the attention-projection GEMM, bit 1: the fc2 GEMM
  * also produces the LayerNorm that follows it, used when the batch fills the machine at least twice with 128-row tiles; bit 2:
  * for any batch; default 3; 0: separate LayerNorm kernels), "ar_kernel" (AR loop: 2 = cluster-owned persistent kernel,
- * default; 1 = grid-barrier persistent kernel, at most 128 head classes and max_label_length <= 31; 0 = chain of separate kernels), "fuse_mlp" (1: fc1 + GELU + fc2 + residual +
+ * default, where it applies - decoders of depth >= 2 run the chain; 1 = grid-barrier persistent kernel, at most 128 head classes, max_label_length <= 31 and dec_depth 1; 0 = chain of separate kernels), "fuse_mlp" (1: fc1 + GELU + fc2 + residual +
  * LayerNorm of an encoder block in one kernel where fuse_ln bit 1 applies - bit-identical results, default 0), "attn_impl"
  * (encoder attention: 0 = mma.sync kernels, default; 1 = wgmma kernel), "ln_cta_group" / "mlp_cta_group"
  * (0 auto, 1 single CTA, 2 CTA pair sharing the weight tiles by TMA multicast: fused GEMM+LayerNorm / one-kernel

@@ -534,6 +534,7 @@ struct parseq_engine {
   float* x = nullptr;
   // per-stage decoder state: the decoder of stage s runs on its own stream while `main` encodes stage s+1
   __nv_bfloat16 *mem = nullptr, *ckv = nullptr;   // [max_batch*T, D] encoder output, [max_batch*T, 2D] cross K/V
+  std::vector<__nv_bfloat16*> ckv_deep;           // cross K/V of decoder layers 1..dec_depth-1, laid out as ckv
   int dec_chunk = 128;              // images per decoder chain (each chain runs on its own stream)
   // persistent AR-loop kernel state (whole super-chunk)
   bool use_ar_kernel = true;
@@ -560,6 +561,10 @@ struct parseq_engine {
     __nv_bfloat16 *sa = nullptr, *yn = nullptr, *ca = nullptr, *hd = nullptr;
     float *y = nullptr, *qc = nullptr;
     int *ids_ar = nullptr, *ids_ctx = nullptr;    // [dec_chunk, ids_ld]
+    // decoders of depth >= 2: content residual stream [dec_chunk * L, D] fp32, and the content K/V of layers
+    // 1..dec_depth-1, one [dec_chunk, L, 2D] bf16 cache per layer (layer 0 reads the (position, token) table)
+    float* cx = nullptr;
+    std::vector<__nv_bfloat16*> kvc;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev_enc = nullptr, ev_done = nullptr;
   };
@@ -610,6 +615,10 @@ int alloc_workspace(parseq_engine* e) {
   PQ_TRY(dev_alloc(&e->hid, R * e->Me));
   PQ_TRY(dev_alloc(&e->mem, RB * D));
   PQ_TRY(dev_alloc(&e->ckv, RB * 2 * D));
+  if (e->cfg.dec_depth > 1) {
+    e->ckv_deep.assign(static_cast<size_t>(e->cfg.dec_depth - 1), nullptr);
+    for (auto& c : e->ckv_deep) PQ_TRY(dev_alloc(&c, RB * 2 * D));
+  }
   PQ_TRY(dev_alloc(&e->ar_sa, 1ll * e->max_batch * D));
   PQ_TRY(dev_alloc(&e->ar_ca, 1ll * e->max_batch * D));
   PQ_TRY(dev_alloc(&e->ar_hd, 1ll * e->max_batch * e->Md));
@@ -632,6 +641,11 @@ int alloc_workspace(parseq_engine* e) {
     PQ_TRY(dev_alloc(&sg.qc, Rd * D));
     PQ_TRY(dev_alloc(&sg.ids_ar, static_cast<long long>(e->dec_chunk) * e->ids_ld));
     PQ_TRY(dev_alloc(&sg.ids_ctx, static_cast<long long>(e->dec_chunk) * e->ids_ld));
+    if (e->cfg.dec_depth > 1) {
+      PQ_TRY(dev_alloc(&sg.cx, Rd * D));
+      sg.kvc.assign(static_cast<size_t>(e->cfg.dec_depth - 1), nullptr);
+      for (auto& c : sg.kvc) PQ_TRY(dev_alloc(&c, Rd * 2 * D));
+    }
     PQ_CUDA(cudaStreamCreateWithFlags(&sg.stream, cudaStreamNonBlocking));
     PQ_CUDA(cudaEventCreateWithFlags(&sg.ev_enc, cudaEventDisableTiming));
     PQ_CUDA(cudaEventCreateWithFlags(&sg.ev_done, cudaEventDisableTiming));
@@ -660,6 +674,9 @@ void free_workspace(parseq_engine* e) {
   e->ar_sa = e->ar_ca = e->ar_hd = nullptr; e->ar_y = e->ar_qc = nullptr; e->ar_ids = nullptr; e->ar_bar = nullptr;
   for (void* p : ptrs)
     if (p) cudaFree(p);
+  for (auto p : e->ckv_deep)
+    if (p) cudaFree(p);
+  e->ckv_deep.clear();
   if (e->ev_enc) { cudaEventDestroy(e->ev_enc); e->ev_enc = nullptr; }
   e->a_pe = e->xn = e->qkv = e->att = e->hid = e->mem = e->ckv = nullptr;
   e->x = e->in_images = e->out_logits = nullptr;
@@ -667,6 +684,9 @@ void free_workspace(parseq_engine* e) {
   for (auto& sg : e->stages) {
     void* q[] = {sg.sa, sg.yn, sg.ca, sg.hd, sg.y, sg.qc, sg.ids_ar, sg.ids_ctx};
     for (void* p : q)
+      if (p) cudaFree(p);
+    if (sg.cx) cudaFree(sg.cx);
+    for (auto p : sg.kvc)
       if (p) cudaFree(p);
     if (sg.stream) cudaStreamDestroy(sg.stream);
     if (sg.ev_enc) cudaEventDestroy(sg.ev_enc);
@@ -849,17 +869,118 @@ struct DecodeExtras {
   const float* query = nullptr;          // [B*nq, D] fp32 raw queries (residual base); null -> pos_queries[q0 + qi]
   const unsigned char* qmask = nullptr;  // [nq, nkeys], 1 = masked
   const unsigned char* pmask = nullptr;  // [B, nkeys], 1 = masked
+  const unsigned char* cmask = nullptr;  // [nkeys, nkeys] content-stream mask (`tgt_mask`), 1 = masked; depth >= 2 only
   float* out_norm = nullptr;             // [B*nq, D] fp32: decoder.norm(y) is the result (no head)
 };
+
+const __nv_bfloat16* ckv_of(const parseq_engine* e, int layer) { return layer == 0 ? e->ckv : e->ckv_deep[layer - 1]; }
+
+// Self-attention with one query row per (image, query) (decoders of depth >= 2): over the (position, token) table
+// (kv = kvtab, layer 0) or over a content K/V cache of `pitch` key rows per image (cache = true).
+int self_attn_rows(parseq_engine* e, const float* q, const __nv_bfloat16* kv, bool cache, int pitch, const int* ids, int B,
+                   int nq, int q0, int nkeys, int mode, const unsigned char* qmask, const unsigned char* pmask,
+                   __nv_bfloat16* out, cudaStream_t st) {
+  const int D = e->D;
+  TimedScope ts(e, st, CAT_DEC_ATTN, 4.0 * B * nq * nkeys * D);
+  const int qsplit = (nq >= 8) ? 4 : 1;
+  auto kern = e->ids_ld == 32 ? (cache ? pq::dec_self_attn2_rows_kernel<true> : pq::dec_self_attn2_rows_kernel<false>)
+                              : (cache ? pq::dec_self_attn2_rows_long_kernel<true> : pq::dec_self_attn2_rows_long_kernel<false>);
+  return launch_k(e->lo, kern, dim3(B * qsplit), dim3(D < 384 ? D : 384), 0, st, q, kv, ids, e->ids_ld, cache ? pitch : e->V, D,
+                  nq, q0, nkeys, mode, /*eos*/ 0, out, qsplit, qmask, pmask);
+}
+
+// The rest of decoder layer `l` after its self-attention (modules.py:72-78) on a residual stream x [B*nq, D] (fp32, in
+// place): x += out_proj(sa); x += cross_attn(norm1(x)); x += MLP(norm2(x)).  add != null: x holds no residual yet,
+// the base is the broadcast table / caller rows `add` (row r adds add[r % add_mod]).
+int dec_layer_rest(parseq_engine* e, parseq_engine::Stage& sg, int l, int b_first, int B, int nq, float* x, const float* add,
+                   int add_mod, cudaStream_t st) {
+  const int D = e->D, M = B * nq;
+  const std::string Ly = "decoder.layers." + std::to_string(l) + ".";
+  const float qscale = 1.0f / std::sqrt(static_cast<float>(e->dh_dec));
+  if (add != nullptr) {
+    // y = query + out_proj(sa): the GEMM stores out_proj(sa) with its TMA epilogue, the LayerNorm kernel adds the query
+    // residual (broadcast pos_queries[q0 + qi], or the caller's rows), writes y back and emits norm1(y)
+    PQ_TRY(gemm(e, sg.sa, D, e->w(Ly + "self_attn.out_proj.weight"), D, e->wf(Ly + "self_attn.out_proj.bias"), M, D, D,
+                pq::EPI_F32, 1.0f, nullptr, 0, 0, x, D, st));
+    PQ_TRY(layernorm(e, x, Ly + "norm1", 1e-5f, M, sg.yn, nullptr, st, add, add_mod, x));
+  } else {
+    PQ_TRY(gemm(e, sg.sa, D, e->w(Ly + "self_attn.out_proj.weight"), D, e->wf(Ly + "self_attn.out_proj.bias"), M, D, D,
+                pq::EPI_F32, 1.0f, x, D, 0, x, D, st));
+    PQ_TRY(layernorm(e, x, Ly + "norm1", 1e-5f, M, sg.yn, nullptr, st));
+  }
+  PQ_TRY(gemm(e, sg.yn, D, e->wb(Ly + "cross_attn.in_proj_weight"), D, e->wf(Ly + "cross_attn.in_proj_bias"), M, D, D,
+              pq::EPI_F32, qscale, nullptr, 0, 0, sg.qc, D, st));
+  {
+    TimedScope ts(e, st, CAT_DEC_ATTN, 4.0 * M * e->T * D);
+    const long long kv_rows = 1ll * e->max_batch * e->T;
+    if (e->T <= 128)
+      PQ_TRY(launch_k(e->lo, pq::dec_cross_attn3_kernel<4>, dim3(B * e->cfg.dec_num_heads), dim3(128), 0, st,
+                      static_cast<const float*>(sg.qc), ckv_of(e, l), kv_rows, b_first, e->T, D,
+                      e->cfg.dec_num_heads, nq, sg.ca));
+    else
+      PQ_TRY(launch_k(e->lo, pq::dec_cross_attn3_kernel<8>, dim3(B * e->cfg.dec_num_heads), dim3(128), 0, st,
+                      static_cast<const float*>(sg.qc), ckv_of(e, l), kv_rows, b_first, e->T, D,
+                      e->cfg.dec_num_heads, nq, sg.ca));
+  }
+  PQ_TRY(gemm(e, sg.ca, D, e->w(Ly + "cross_attn.out_proj.weight"), D, e->wf(Ly + "cross_attn.out_proj.bias"), M, D, D,
+              pq::EPI_F32, 1.0f, x, D, 0, x, D, st));
+  PQ_TRY(layernorm(e, x, Ly + "norm2", 1e-5f, M, sg.yn, nullptr, st));
+  PQ_TRY(gemm(e, sg.yn, D, e->w(Ly + "linear1.weight"), D, e->wf(Ly + "linear1.bias"), M, e->Md, D, pq::EPI_GELU_BF16,
+              1.0f, nullptr, 0, 0, sg.hd, e->Md, st));
+  PQ_TRY(gemm(e, sg.hd, e->Md, e->w(Ly + "linear2.weight"), e->Md, e->wf(Ly + "linear2.bias"), M, D, e->Md, pq::EPI_F32,
+              1.0f, x, D, 0, x, D, st));
+  return PARSEQ_OK;
+}
+
+// Content stream of a decoder of depth >= 2 (modules.py:94-97, 119-123): context rows [k0, k0 + nc) of B images through
+// layers 0..depth-2, each appending its K/V rows of the next layer to that layer's cache (row b * pitch + k).  nc is 1
+// (an AR step, pitch L: the causal content rows of earlier positions do not change as the context grows) or nkeys = pitch
+// (a whole pass).  The content rows attend to keys 0..nkeys-1 under `mode` (0: all, 1: cloze + first EOS), or under the
+// caller's content / padding masks (decode API).
+int content_stream(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, int k0, int nc, int nkeys, int pitch,
+                   int mode, const int* ids, const unsigned char* cmask, const unsigned char* pmask, cudaStream_t st) {
+  const int D = e->D, M = B * nc;
+  const float qscale = 1.0f / std::sqrt(static_cast<float>(e->dh_dec));
+  {
+    TimedScope ts(e, st, CAT_MISC, 0.0);
+    const long long total = 1ll * M * D;
+    PQ_TRY(launch_k(e->lo, pq::gather_ctx_rows_kernel, dim3(static_cast<unsigned>(std::min<long long>((total + 255) / 256, 132ll * 8))),
+                    dim3(256), 0, st, e->wf("text_embed.embedding.weight"), e->wf("pos_queries"), ids, e->ids_ld, B, k0, nc, D,
+                    std::sqrt(static_cast<float>(D)), sg.cx));
+  }
+  if (cmask != nullptr || pmask != nullptr) mode = 2;
+  PQ_TRY(layernorm(e, sg.cx, "decoder.layers.0.norm_c", 1e-5f, M, sg.yn, nullptr, st));
+  const long long ldo = (nc == pitch ? 1ll : pitch) * 2 * D;
+  for (int l = 0; l + 1 < e->cfg.dec_depth; ++l) {
+    // sg.yn = norm_c_l(content_l): the content queries of layer l (its keys are the same rows' K/V, already stored)
+    const std::string Ly = "decoder.layers." + std::to_string(l) + ".";
+    PQ_TRY(gemm(e, sg.yn, D, e->w(Ly + "self_attn.in_proj_weight"), D, e->wf(Ly + "self_attn.in_proj_bias"), M, D, D,
+                pq::EPI_F32, qscale, nullptr, 0, 0, sg.qc, D, st));
+    PQ_TRY(self_attn_rows(e, sg.qc, l == 0 ? e->kvtab : sg.kvc[l - 1], l > 0, pitch, ids, B, nc, k0, nkeys, mode, cmask, pmask,
+                          sg.sa, st));
+    PQ_TRY(dec_layer_rest(e, sg, l, b_first, B, nc, sg.cx, nullptr, 0, st));
+    // K/V of layer l + 1 = W_kv norm_c_{l+1}(content_{l+1}) + b_kv, into rows k0.. of its cache
+    const std::string Ln = "decoder.layers." + std::to_string(l + 1) + ".";
+    PQ_TRY(layernorm(e, sg.cx, Ln + "norm_c", 1e-5f, M, sg.yn, nullptr, st));
+    PQ_TRY(gemm(e, sg.yn, D, e->wb(Ln + "self_attn.in_proj_weight") + 1ll * D * D, D, e->wf(Ln + "self_attn.in_proj_bias") + D,
+                M, 2 * D, D, pq::EPI_BF16, 1.0f, nullptr, 0, 0, sg.kvc[l] + 2ll * k0 * D, ldo, st));
+  }
+  return PARSEQ_OK;
+}
+
+// ar_step: an AR step (nq = 1, query position q0, keys 0..q0): the content stream computes row q0 only and appends it to
+// the caches of pitch L; otherwise it computes the whole context (nkeys rows per image, pitch nkeys)
 int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, int nq, int q0, int nkeys,
                 int mode, const int* ids, float* logits_out, long long logits_ld, int* ids_dst, int dst_off,
-                const int* forced, int forced_ld, cudaStream_t st, const DecodeExtras* ex = nullptr) {
+                const int* forced, int forced_ld, cudaStream_t st, const DecodeExtras* ex = nullptr, bool ar_step = false) {
   const int D = e->D, M = B * nq;
   const std::string Ly = "decoder.layers.0.";
   const float qscale = 1.0f / std::sqrt(static_cast<float>(e->dh_dec));
-  const __nv_bfloat16* Wc = e->wb(Ly + "cross_attn.in_proj_weight");
-  const float* bc = e->wf(Ly + "cross_attn.in_proj_bias");
   e->cur_cat = CAT_DEC_GEMM;
+  const int kv_pitch = ar_step ? e->L : nkeys;
+  if (e->cfg.dec_depth > 1)
+    PQ_TRY(content_stream(e, sg, b_first, B, ar_step ? q0 : 0, ar_step ? 1 : nkeys, nkeys, kv_pitch, mode, ids,
+                          ex != nullptr ? ex->cmask : nullptr, ex != nullptr ? ex->pmask : nullptr, st));
   const float* qself = e->qs;            // [L, D] table of W_q LN_q(pos_queries), pre-scaled
   const unsigned char *qmask = nullptr, *pmask = nullptr;
   if (ex != nullptr && ex->query != nullptr) {
@@ -889,33 +1010,19 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
                     dim3(D < 384 ? D : 384), 0, st, qself, static_cast<const __nv_bfloat16*>(e->kvtab), ids, e->ids_ld, e->V,
                     D, nq, q0, nkeys, mode, /*eos*/ 0, sg.sa, qsplit, qmask, pmask));
   }
-  // y = query + out_proj(sa): the GEMM stores out_proj(sa) with its TMA epilogue, the LayerNorm kernel adds the query
-  // residual (broadcast pos_queries[q0 + qi], or the caller's rows), writes y back and emits norm1(y)
   const bool own_q = ex != nullptr && ex->query != nullptr;
   const float* resid = own_q ? ex->query : e->wf("pos_queries") + static_cast<long long>(q0) * D;
-  PQ_TRY(gemm(e, sg.sa, D, e->w(Ly + "self_attn.out_proj.weight"), D, e->wf(Ly + "self_attn.out_proj.bias"), M, D, D,
-              pq::EPI_F32, 1.0f, nullptr, 0, 0, sg.y, D, st));
-  PQ_TRY(layernorm(e, sg.y, Ly + "norm1", 1e-5f, M, sg.yn, nullptr, st, resid, own_q ? M : nq, sg.y));
-  PQ_TRY(gemm(e, sg.yn, D, Wc, D, bc, M, D, D, pq::EPI_F32, qscale, nullptr, 0, 0, sg.qc, D, st));
-  {
-    TimedScope ts(e, st, CAT_DEC_ATTN, 4.0 * M * e->T * D);
-    const long long kv_rows = 1ll * e->max_batch * e->T;
-    if (e->T <= 128)
-      PQ_TRY(launch_k(e->lo, pq::dec_cross_attn3_kernel<4>, dim3(B * e->cfg.dec_num_heads), dim3(128), 0, st,
-                      static_cast<const float*>(sg.qc), static_cast<const __nv_bfloat16*>(e->ckv), kv_rows, b_first, e->T, D,
-                      e->cfg.dec_num_heads, nq, sg.ca));
-    else
-      PQ_TRY(launch_k(e->lo, pq::dec_cross_attn3_kernel<8>, dim3(B * e->cfg.dec_num_heads), dim3(128), 0, st,
-                      static_cast<const float*>(sg.qc), static_cast<const __nv_bfloat16*>(e->ckv), kv_rows, b_first, e->T, D,
-                      e->cfg.dec_num_heads, nq, sg.ca));
+  PQ_TRY(dec_layer_rest(e, sg, 0, b_first, B, nq, sg.y, resid, own_q ? M : nq, st));
+  // query stream of layers >= 1 (modules.py:91-93): its residual base is the previous layer's output, its keys the
+  // layer's content K/V cache
+  for (int l = 1; l < e->cfg.dec_depth; ++l) {
+    const std::string Ll = "decoder.layers." + std::to_string(l) + ".";
+    PQ_TRY(layernorm(e, sg.y, Ll + "norm_q", 1e-5f, M, sg.yn, nullptr, st));
+    PQ_TRY(gemm(e, sg.yn, D, e->w(Ll + "self_attn.in_proj_weight"), D, e->wf(Ll + "self_attn.in_proj_bias"), M, D, D,
+                pq::EPI_F32, qscale, nullptr, 0, 0, sg.qc, D, st));
+    PQ_TRY(self_attn_rows(e, sg.qc, sg.kvc[l - 1], true, kv_pitch, ids, B, nq, q0, nkeys, mode, qmask, pmask, sg.sa, st));
+    PQ_TRY(dec_layer_rest(e, sg, l, b_first, B, nq, sg.y, nullptr, 0, st));
   }
-  PQ_TRY(gemm(e, sg.ca, D, e->w(Ly + "cross_attn.out_proj.weight"), D, e->wf(Ly + "cross_attn.out_proj.bias"), M, D, D,
-              pq::EPI_F32, 1.0f, sg.y, D, 0, sg.y, D, st));
-  PQ_TRY(layernorm(e, sg.y, Ly + "norm2", 1e-5f, M, sg.yn, nullptr, st));
-  PQ_TRY(gemm(e, sg.yn, D, e->w(Ly + "linear1.weight"), D, e->wf(Ly + "linear1.bias"), M, e->Md, D, pq::EPI_GELU_BF16,
-              1.0f, nullptr, 0, 0, sg.hd, e->Md, st));
-  PQ_TRY(gemm(e, sg.hd, e->Md, e->w(Ly + "linear2.weight"), e->Md, e->wf(Ly + "linear2.bias"), M, D, e->Md, pq::EPI_F32,
-              1.0f, sg.y, D, 0, sg.y, D, st));
   if (ex != nullptr && ex->out_norm != nullptr) {
     // PARSeq.decode returns the decoder output: final LayerNorm only (modules.py:123-125)
     PQ_TRY(layernorm(e, sg.y, "decoder.norm", 1e-5f, M, sg.yn, ex->out_norm, st));
@@ -971,7 +1078,7 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
     for (int i = 0; i < L; ++i) {
       // step i: context ids[:, :i+1], query position i; the fused tail writes ids[:, i+1] = argmax (model.py:142)
       PQ_TRY(decode_pass(e, sg, b_first, B, 1, i, i + 1, 0, sg.ids_ar, logits + static_cast<long long>(i) * C, LC,
-                         (i + 1 < L) ? sg.ids_ar : nullptr, i + 1, forced, L, st));
+                         (i + 1 < L) ? sg.ids_ar : nullptr, i + 1, forced, L, st, nullptr, /*ar_step*/ true));
     }
     if (testing && steps != nullptr) {
       PQ_TRY(launch_k(e->lo, pq::ar_steps_kernel, dim3(1), dim3(256), 0, st, static_cast<const int*>(sg.ids_ar), e->ids_ld, B, L,
@@ -1004,7 +1111,7 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
 // Heads of <= 96 classes run redundantly in every CTA; > 128 classes take the class-sliced head (WIDE); 97..128 classes
 // stay on the grid-barrier kernel (labels of up to 31 characters) or on the chain of separate kernels (longer labels).
 bool ar2_supported(const parseq_engine* e) {
-  return e->arch == 0 && e->cfg.dec_mlp_ratio == 4 && (e->C <= 96 || e->C > 128) && e->T <= 256 && e->dh_dec == 32;
+  return e->arch == 0 && e->cfg.dec_depth == 1 && e->cfg.dec_mlp_ratio == 4 && (e->C <= 96 || e->C > 128) && e->T <= 256 && e->dh_dec == 32;
 }
 bool ar2_wide(const parseq_engine* e) { return e->C > 128; }
 // weight descriptors: once per weight set (parseq_finalize); K/V cache descriptor: once per workspace
@@ -1252,19 +1359,19 @@ int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B,
   }
   // cross-attention K/V of the image memory, once per image (the reference recomputes it in every decode call)
   e->cur_cat = CAT_DEC_GEMM;
-  {
-    const std::string Ly = "decoder.layers.0.";
+  for (int l = 0; l < e->cfg.dec_depth; ++l) {
+    const std::string Ly = "decoder.layers." + std::to_string(l) + ".";
     const __nv_bfloat16* Wkv = e->wb(Ly + "cross_attn.in_proj_weight") + static_cast<long long>(D) * D;
     const float* bkv = e->wf(Ly + "cross_attn.in_proj_bias") + D;
     // stored column-blocked [2D/64][max_batch * T][64]: an image's K (V) panel of 64 channels is one contiguous T x 128 B
     // run - what a TMA box of the AR kernel and a head of the refine-pass attention read
-    PQ_TRY(gemm(e, e->mem, D, Wkv, D, bkv, B * T, 2 * D, D, pq::EPI_BF16, 1.0f, nullptr, 0, 0, e->ckv, 2 * D, e->main,
-                1ll * e->max_batch * T));
+    PQ_TRY(gemm(e, e->mem, D, Wkv, D, bkv, B * T, 2 * D, D, pq::EPI_BF16, 1.0f, nullptr, 0, 0,
+                const_cast<__nv_bfloat16*>(ckv_of(e, l)), 2 * D, e->main, 1ll * e->max_batch * T));
   }
   // an AR loop that the cluster kernel cannot take (e.g. dec_mlp_ratio != 4) runs on the grid-barrier kernel if that holds
-  // it (<= 128 classes, L <= 32), else as a chain of separate kernels
+  // it (<= 128 classes, L <= 32), else as a chain of separate kernels; so does every decoder of depth >= 2
   const bool ar_done = a->decode_ar && e->use_ar_kernel &&
-                       ((e->ar_impl == 2 && ar2_supported(e)) || (e->C <= 128 && e->L <= 32));
+                       ((e->ar_impl == 2 && ar2_supported(e)) || (e->C <= 128 && e->L <= 32 && e->cfg.dec_depth == 1));
   if (ar_done) {
     PQ_TRY(ar_decode(e, a, b0, B, L, logits, steps, e->main));
     if (a->refine_iters == 0) {      // nothing left for the chains but the final argmax
@@ -1412,7 +1519,7 @@ int parseq_create(const parseq_config* cfg, parseq_engine** out) {
   PQ_TRY(load_driver_api());
   if (cfg->arch != 0 && cfg->arch != 1) return fail(PARSEQ_ERR_INVALID_ARG, "arch: 0 (PARSeq) or 1 (ViTSTR)");
   const bool vitstr = cfg->arch == 1;
-  if (!vitstr && cfg->dec_depth != 1) return fail(PARSEQ_ERR_UNSUPPORTED, "dec_depth must be 1");
+  if (!vitstr && cfg->dec_depth < 1) return fail(PARSEQ_ERR_UNSUPPORTED, "dec_depth must be >= 1 (decoder layers)");
   if (cfg->img_h % cfg->patch_h || cfg->img_w % cfg->patch_w) return fail(PARSEQ_ERR_INVALID_ARG, "img/patch mismatch");
   const int D = cfg->embed_dim;
   if (D != 192 && D != 384 && D != 768) return fail(PARSEQ_ERR_UNSUPPORTED, "embed_dim must be 192, 384 or 768");
@@ -1492,8 +1599,8 @@ int parseq_create(const parseq_config* cfg, parseq_engine** out) {
   }
   add_slot(e, "encoder.norm.weight", D, false);
   add_slot(e, "encoder.norm.bias", D, false);
-  const std::string Ly = "decoder.layers.0.";
-  if (!vitstr) {
+  for (int l = 0; !vitstr && l < cfg->dec_depth; ++l) {
+    const std::string Ly = "decoder.layers." + std::to_string(l) + ".";
     for (const char* att : {"self_attn", "cross_attn"}) {
       add_slot(e, Ly + att + ".in_proj_weight", 3ll * D * D, true);
       add_slot(e, Ly + att + ".in_proj_bias", 3 * D, false);
@@ -1508,6 +1615,8 @@ int parseq_create(const parseq_config* cfg, parseq_engine** out) {
       add_slot(e, Ly + n + ".weight", D, false);
       add_slot(e, Ly + n + ".bias", D, false);
     }
+  }
+  if (!vitstr) {
     add_slot(e, "decoder.norm.weight", D, false);
     add_slot(e, "decoder.norm.bias", D, false);
   }
@@ -1724,6 +1833,12 @@ int parseq_encode(parseq_engine* e, int32_t batch, const float* images, float* m
 int parseq_decode(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t num_queries, const int32_t* tgt, const float* memory,
                   const float* query, const uint8_t* query_mask, const uint8_t* padding_mask, float* out,
                   parseq_stream_t stream) {
+  return parseq_decode_ex(e, batch, ctx_len, num_queries, tgt, memory, query, query_mask, padding_mask, nullptr, out, stream);
+}
+
+int parseq_decode_ex(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t num_queries, const int32_t* tgt,
+                     const float* memory, const float* query, const uint8_t* query_mask, const uint8_t* padding_mask,
+                     const uint8_t* content_mask, float* out, parseq_stream_t stream) {
   if (e == nullptr || tgt == nullptr || memory == nullptr || out == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
   if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
   if (!e->finalized) return fail(PARSEQ_ERR_STATE, "parseq_finalize has not been called");
@@ -1736,9 +1851,6 @@ int parseq_decode(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t num_
   PQ_CUDA(cudaEventRecord(e->ev_in, user));
   PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_in, 0));
   const int D = e->D, T = e->T, J = ctx_len, NQ = num_queries;
-  const std::string Ly = "decoder.layers.0.";
-  const __nv_bfloat16* Wkv = e->wb(Ly + "cross_attn.in_proj_weight") + static_cast<long long>(D) * D;
-  const float* bkv = e->wf(Ly + "cross_attn.in_proj_bias") + D;
   parseq_engine::Stage& sg = e->stages[0];
   cudaStream_t st = e->main;
   for (int b0 = 0; b0 < batch; b0 += e->dec_chunk) {
@@ -1749,8 +1861,12 @@ int parseq_decode(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t num_
         reinterpret_cast<const float4*>(memory + 1ll * b0 * T * D), reinterpret_cast<uint2*>(e->mem), n4);
     PQ_CUDA(cudaGetLastError());
     e->cur_cat = CAT_DEC_GEMM;
-    PQ_TRY(gemm(e, e->mem, D, Wkv, D, bkv, Bc * T, 2 * D, D, pq::EPI_BF16, 1.0f, nullptr, 0, 0, e->ckv, 2 * D, st,
-                1ll * e->max_batch * T));
+    for (int l = 0; l < e->cfg.dec_depth; ++l) {
+      const std::string Ly = "decoder.layers." + std::to_string(l) + ".";
+      PQ_TRY(gemm(e, e->mem, D, e->wb(Ly + "cross_attn.in_proj_weight") + static_cast<long long>(D) * D, D,
+                  e->wf(Ly + "cross_attn.in_proj_bias") + D, Bc * T, 2 * D, D, pq::EPI_BF16, 1.0f, nullptr, 0, 0,
+                  const_cast<__nv_bfloat16*>(ckv_of(e, l)), 2 * D, st, 1ll * e->max_batch * T));
+    }
     pq::copy_ids_kernel<<<(Bc * e->ids_ld + 255) / 256, 256, 0, st>>>(tgt + 1ll * b0 * J, J, sg.ids_ctx, Bc, e->ids_ld);
     PQ_CUDA(cudaGetLastError());
     e->launches += 2;
@@ -1758,6 +1874,7 @@ int parseq_decode(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t num_
     ex.query = query ? query + 1ll * b0 * NQ * D : nullptr;
     ex.qmask = query_mask;
     ex.pmask = padding_mask ? padding_mask + 1ll * b0 * J : nullptr;
+    ex.cmask = content_mask;
     ex.out_norm = out + 1ll * b0 * NQ * D;
     PQ_TRY(decode_pass(e, sg, 0, Bc, NQ, 0, J, 0, sg.ids_ctx, nullptr, 0, nullptr, 0, nullptr, 0, st, &ex));
   }
@@ -1943,6 +2060,8 @@ int parseq_set_option(parseq_engine* e, const char* name, int64_t value) {
     if (value == 1 && e->L > 32)
       return fail(PARSEQ_ERR_UNSUPPORTED, "ar_kernel = 1 (grid-barrier AR kernel) covers max_label_length <= 31; "
                                           "use ar_kernel 0 or 2");
+    if (value == 1 && e->cfg.dec_depth > 1)
+      return fail(PARSEQ_ERR_UNSUPPORTED, "ar_kernel = 1 (grid-barrier AR kernel) covers dec_depth 1; use ar_kernel 0 or 2");
     e->use_ar_kernel = value != 0;
     e->ar_impl = value == 1 ? 1 : 2;
     drop_graphs(e);

@@ -475,7 +475,10 @@ __global__ void set_int_kernel(int* p, int v) {
 //            mode 2 (PARSeq.decode with caller-supplied masks, model.py:86-103): Qs holds one query row per (image,
 //            query) [B*nq, D]; key k of query qi is masked iff qmask[qi*nkeys + k] or pmask[b*nkeys + k] (either may be
 //            null); a row with every key masked yields NaN, as torch's softmax over -inf does
-template <int KPL>
+//            QROW (decoders of depth >= 2): Qs holds one query row per (image, query) [B*nq, D] in every mode
+//            CACHE (decoders of depth >= 2): K/V rows come from a per-image cache [B, V, 2D] (V = key rows per image),
+//            row b * V + k, instead of the (position, token) table
+template <int KPL, bool QROW = false, bool CACHE = false>
 __device__ __forceinline__ void dec_self_attn2_body(const float* __restrict__ Qs, const __nv_bfloat16* __restrict__ kvtab,
                                                     const int* __restrict__ ids, int ids_ld, int V, int D, int nq, int q0,
                                                     int nkeys, int mode, int eos_id, __nv_bfloat16* __restrict__ out,
@@ -520,7 +523,8 @@ __device__ __forceinline__ void dec_self_attn2_body(const float* __restrict__ Qs
   for (int u = 0; u < KPL; ++u) {
     const int key = lane + 32 * u;
     if (key < nkeys) {
-      const uint4* kr = reinterpret_cast<const uint4*>(kvtab + (static_cast<long long>(key) * V + s_ids[key]) * 2 * D + h * 32);
+      const long long kvrow = CACHE ? static_cast<long long>(b) * V + key : static_cast<long long>(key) * V + s_ids[key];
+      const uint4* kr = reinterpret_cast<const uint4*>(kvtab + kvrow * 2 * D + h * 32);
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const uint4 w = __ldg(kr + j);
@@ -539,10 +543,10 @@ __device__ __forceinline__ void dec_self_attn2_body(const float* __restrict__ Qs
   }
 #pragma unroll
   for (int k = 0; k < NK; ++k)
-    vreg[k] = (k < nkeys) ? __bfloat162float(kvtab[(static_cast<long long>(k) * V + s_ids[k]) * 2 * D + D + h * 32 + lane]) : 0.f;
+    vreg[k] = (k < nkeys) ? __bfloat162float(kvtab[(CACHE ? static_cast<long long>(b) * V + k : static_cast<long long>(k) * V + s_ids[k]) * 2 * D + D + h * 32 + lane]) : 0.f;
   for (int qi = q_begin; qi < q_end; ++qi) {
     const int qpos = q0 + qi;
-    const long long qrow = (mode == 2) ? (static_cast<long long>(b) * nq + qi) : qpos;
+    const long long qrow = (QROW || mode == 2) ? (static_cast<long long>(b) * nq + qi) : qpos;
     const float qv = __ldg(Qs + qrow * D + h * 32 + lane);   // lane j holds q_j
     float acc = 0.f;
     if constexpr (KPL == 1) {
@@ -625,6 +629,41 @@ __global__ void __launch_bounds__(384) dec_self_attn2_long_kernel(
     int D, int nq, int q0, int nkeys, int mode, int eos_id, __nv_bfloat16* __restrict__ out, int qsplit,
     const unsigned char* __restrict__ qmask = nullptr, const unsigned char* __restrict__ pmask = nullptr) {
   dec_self_attn2_body<2>(Qs, kvtab, ids, ids_ld, V, D, nq, q0, nkeys, mode, eos_id, out, qsplit, qmask, pmask);
+}
+
+// Decoders of depth >= 2: one query row per (image, query) - the content stream's own rows, or the query stream of a
+// layer >= 1 - over the (position, token) table (CACHE = false: layer 0) or a per-image K/V cache (CACHE = true)
+template <bool CACHE>
+__global__ void dec_self_attn2_rows_kernel(const float* __restrict__ Qs, const __nv_bfloat16* __restrict__ kv,
+                                           const int* __restrict__ ids, int ids_ld, int V, int D, int nq, int q0, int nkeys,
+                                           int mode, int eos_id, __nv_bfloat16* __restrict__ out, int qsplit,
+                                           const unsigned char* __restrict__ qmask, const unsigned char* __restrict__ pmask) {
+  dec_self_attn2_body<1, true, CACHE>(Qs, kv, ids, ids_ld, V, D, nq, q0, nkeys, mode, eos_id, out, qsplit, qmask, pmask);
+}
+template <bool CACHE>
+__global__ void __launch_bounds__(384) dec_self_attn2_rows_long_kernel(
+    const float* __restrict__ Qs, const __nv_bfloat16* __restrict__ kv, const int* __restrict__ ids, int ids_ld, int V,
+    int D, int nq, int q0, int nkeys, int mode, int eos_id, __nv_bfloat16* __restrict__ out, int qsplit,
+    const unsigned char* __restrict__ qmask, const unsigned char* __restrict__ pmask) {
+  dec_self_attn2_body<2, true, CACHE>(Qs, kv, ids, ids_ld, V, D, nq, q0, nkeys, mode, eos_id, out, qsplit, qmask, pmask);
+}
+// Layer-0 content rows of context positions [k0, k0 + nc) of B images (the rows build_ctx_rows_kernel puts into the
+// K/V table, same arithmetic): x[b * nc + c] = sqrt(D) E[ids[b, k]] + (k >= 1 ? pos_queries[k - 1] : 0), k = k0 + c
+__global__ void gather_ctx_rows_kernel(const float* __restrict__ emb, const float* __restrict__ posq, const int* __restrict__ ids,
+                                       int ids_ld, int B, int k0, int nc, int D, float sqrtD, float* __restrict__ x) {
+  grid_dep_launch();
+  grid_dep_wait();
+  const long long total = static_cast<long long>(B) * nc * D;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int c = static_cast<int>(i % D);
+    const long long row = i / D;
+    const int k = k0 + static_cast<int>(row % nc);
+    const int tok = ids[(row / nc) * ids_ld + k];
+    float v = sqrtD * emb[static_cast<long long>(tok) * D + c];
+    if (k >= 1) v = posq[static_cast<long long>(k - 1) * D + c] + v;
+    x[i] = v;
+  }
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -26,7 +26,7 @@ class ForwardArgsC(C.Structure):
 EXPORTS = [
     "parseq_create", "parseq_destroy", "parseq_set_weight", "parseq_num_weights", "parseq_weight_key",
     "parseq_finalize", "parseq_forward", "parseq_forward_host", "parseq_forward_u8", "parseq_forward_host_u8",
-    "parseq_postprocess", "parseq_encode", "parseq_decode", "parseq_head", "parseq_text_embed", "parseq_kernel_launches", "parseq_debug_int", "parseq_bench_tma_stream",
+    "parseq_postprocess", "parseq_encode", "parseq_decode", "parseq_decode_ex", "parseq_head", "parseq_text_embed", "parseq_kernel_launches", "parseq_debug_int", "parseq_bench_tma_stream",
     "parseq_set_option", "parseq_get_timing", "parseq_get_ar_profile", "parseq_last_error", "parseq_version", "parseq_gemm_bf16", "parseq_gemm_ln_bf16", "parseq_mlp_ln_bf16", "parseq_layernorm_bf16",
     "parseq_enc_attention",
 ]
@@ -66,6 +66,8 @@ def load_library(path: Optional[str] = None):
     lib.parseq_encode.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.parseq_decode.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.parseq_decode_ex.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.parseq_head.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.parseq_text_embed.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.parseq_set_option.argtypes = [C.c_void_p, C.c_char_p, C.c_int64]
@@ -203,9 +205,10 @@ class Engine:
     def encode(self, images_ptr, batch, memory_ptr, stream):
         check(self.lib, self.lib.parseq_encode(self.handle, batch, images_ptr, memory_ptr, stream))
 
-    def decode(self, batch, ctx_len, num_queries, tgt_ptr, memory_ptr, query_ptr, qmask_ptr, pmask_ptr, out_ptr, stream):
-        check(self.lib, self.lib.parseq_decode(self.handle, batch, ctx_len, num_queries, tgt_ptr, memory_ptr, query_ptr,
-                                               qmask_ptr, pmask_ptr, out_ptr, stream))
+    def decode(self, batch, ctx_len, num_queries, tgt_ptr, memory_ptr, query_ptr, qmask_ptr, pmask_ptr, out_ptr, stream,
+               cmask_ptr=None):
+        check(self.lib, self.lib.parseq_decode_ex(self.handle, batch, ctx_len, num_queries, tgt_ptr, memory_ptr, query_ptr,
+                                                  qmask_ptr, pmask_ptr, cmask_ptr, out_ptr, stream))
 
     def head(self, rows, x_ptr, logits_ptr, stream):
         check(self.lib, self.lib.parseq_head(self.handle, rows, x_ptr, logits_ptr, stream))

@@ -243,8 +243,8 @@ class ParseqModel(_EngineModule):
                tgt_padding_mask: Optional[Tensor] = None, tgt_query: Optional[Tensor] = None,
                tgt_query_mask: Optional[Tensor] = None) -> Tensor:
         """model.py:86-103: decoder output [N, NQ, D] (before `head`) for context ids `tgt` [N, J] and encoder `memory`
-        [N, T, D].  `tgt_mask` acts on the content stream only, which the depth-1 decoder never updates
-        (modules.py:117-123), so it is accepted and ignored."""
+        [N, T, D].  `tgt_mask` [J, J] acts on the content stream only, which the decoder updates in every layer but
+        the last (modules.py:117-123): it is honoured at dec_depth >= 2, and accepted and ignored at depth 1."""
         eng = self.engine()
         dev = memory.device
         if dev.type != "cuda" or tgt.device != dev:
@@ -262,10 +262,11 @@ class ParseqModel(_EngineModule):
             q = tgt_query.to(device=dev, dtype=torch.float32).expand(N, NQ, D).contiguous()
         qm = self._bool_mask(tgt_query_mask, (NQ, J), dev)
         pm = self._bool_mask(tgt_padding_mask, (N, J), dev)
+        cm = self._bool_mask(tgt_mask, (J, J), dev) if self.cfg.dec_depth > 1 else None
         out = torch.empty((N, NQ, D), dtype=torch.float32, device=dev)
         eng.decode(N, J, NQ, ids.data_ptr(), mem.data_ptr(), q.data_ptr() if q is not None else None,
                    qm.data_ptr() if qm is not None else None, pm.data_ptr() if pm is not None else None, out.data_ptr(),
-                   torch.cuda.current_stream(dev).cuda_stream)
+                   torch.cuda.current_stream(dev).cuda_stream, cm.data_ptr() if cm is not None else None)
         return out
 
     def forward(self, tokenizer: Tokenizer, images: Tensor, max_length: Optional[int] = None,

@@ -140,6 +140,7 @@ struct LaunchOpts {
   bool pair_pdl = false;        // experiments: programmatic dependent launch also on CTA-pair (cluster) launches
   int gemm_stages = 0;          // experiments: cap the operand ring depth (0 = full)
   int attn_impl = 0;            // 0: mma.sync kernels (kernels.cuh), the faster on H100; 1: wgmma kernel (attn_wgmma.cuh)
+  int ln_clusters = 0;          // co-resident clusters of the persistent GEMM + LayerNorm kernel (0: not queried yet)
 };
 LaunchOpts g_default_opts;
 
@@ -343,7 +344,7 @@ int gemm_launch(LaunchOpts& lo, const void* A, long long lda, const void* W, lon
 // x[M, D] += A[M, K] * W[D, K]^T + bias (fp32, in place); xn[M, D] = bf16(LayerNorm(x; gamma, beta, eps))   (gemm_ln.cuh)
 bool gemm_ln_supported(int D) { return D == 192 || D == 384; }
 template <int D, int MODE>
-int launch_gemm_ln(const LaunchOpts& lo, const void* A, long long lda, const void* W, long long ldw, const float* bias, int M, int K, float* x,
+int launch_gemm_ln(LaunchOpts& lo, const void* A, long long lda, const void* W, long long ldw, const float* bias, int M, int K, float* x,
                    const float* gamma, const float* beta, float eps, void* xn, cudaStream_t st) {
   using Cfg = pq::GemmLnCfg<D, MODE>;
   static bool attr_set = false;
@@ -352,7 +353,7 @@ int launch_gemm_ln(const LaunchOpts& lo, const void* A, long long lda, const voi
     attr_set = true;
   }
   CUtensorMap ta, tb, tx;
-  PQ_TRY(make_tmap(&ta, A, 2, M, K, lda, pq::GEMM_BLOCK_K, pq::GLN_BLOCK_M));
+  PQ_TRY(make_tmap(&ta, A, 2, M, K, lda, pq::GEMM_BLOCK_K, Cfg::kABox));
   PQ_TRY(make_tmap(&tb, W, 2, D, K, ldw, pq::GEMM_BLOCK_K, Cfg::kBox));
   if ((reinterpret_cast<uintptr_t>(x) & 7u) != 0 || (reinterpret_cast<uintptr_t>(xn) & 3u) != 0)
     return fail(PARSEQ_ERR_INVALID_ARG, "gemm_ln: x must be 8-byte and xn 4-byte aligned");
@@ -360,15 +361,7 @@ int launch_gemm_ln(const LaunchOpts& lo, const void* A, long long lda, const voi
   p.M = M; p.K = K; p.bias = bias; p.gamma = gamma; p.beta = beta; p.eps = eps;
   p.num_m_tiles = (M + Cfg::kTileM - 1) / Cfg::kTileM;
   int clusters = p.num_m_tiles;
-  if constexpr (MODE == 2) {
-    // persistent: one cluster per SM pair; the tile's x slice is fetched by TMA (x: 16-B aligned)
-    PQ_TRY(make_tmap(&tx, x, 4, M, D, D, Cfg::kXBoxCols, Cfg::kTileM));
-    clusters = std::min(p.num_m_tiles, std::max(1, lo.sm_count / 2));
-  } else {
-    tx = ta;                                                  // unused by MODE 0 / 1
-  }
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(clusters * Cfg::kCG));
   cfg.blockDim = dim3(pq::GLN_THREADS);
   cfg.dynamicSmemBytes = Cfg::kSmemBytes;
   cfg.stream = st;
@@ -380,6 +373,21 @@ int launch_gemm_ln(const LaunchOpts& lo, const void* A, long long lda, const voi
   attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  if constexpr (MODE == 2) {
+    // persistent: as many CTA pairs as the occupancy query admits on this device, each walking the tiles with the grid's
+    // stride; x slices are fetched by TMA (x: 16-B aligned)
+    PQ_TRY(make_tmap(&tx, x, 4, M, D, D, Cfg::kXBoxCols, pq::GLN_BLOCK_M));
+    if (lo.ln_clusters == 0) {
+      cfg.gridDim = dim3(static_cast<unsigned>(lo.sm_count / Cfg::kCG * Cfg::kCG));
+      PQ_CUDA(cudaOccupancyMaxActiveClusters(&lo.ln_clusters, pq::gemm_ln_fused_kernel<D, MODE>, &cfg));
+      if (lo.ln_clusters <= 0) return fail(PARSEQ_ERR_CUDA, "gemm_ln: no cluster of the persistent kernel fits the device");
+    }
+    clusters = std::min(p.num_m_tiles, lo.ln_clusters);
+  } else {
+    tx = ta;                                                  // unused by MODE 0 / 1
+  }
+  cfg.gridDim = dim3(static_cast<unsigned>(clusters * Cfg::kCG));
   cfg.numAttrs = (lo.use_pdl && (MODE == 0 || lo.pair_pdl)) ? 2 : 1;
   PQ_CUDA(cudaLaunchKernelEx(&cfg, pq::gemm_ln_fused_kernel<D, MODE>, ta, tb, tx, x, reinterpret_cast<__nv_bfloat16*>(xn), p));
   return PARSEQ_OK;
@@ -389,8 +397,8 @@ int gemm_ln_launch(LaunchOpts& lo, const void* A, long long lda, const void* W, 
   if (M <= 0 || K <= 0) return fail(PARSEQ_ERR_INVALID_ARG, "gemm_ln: empty problem");
   PQ_TRY(ensure_sm_count(lo));
   PQ_TRY(load_driver_api());
-  // MODE 2 (persistent CTA pairs on 128-row tiles, the columns split over the pair) runs every K at D = 384: W bytes per
-  // row are half of the full-row kernel's, A crosses L2 once per tile, and the residual arrives during the main loop.
+  // MODE 2 (persistent CTA pairs on 64-row tiles, the columns split over the pair, ping-pong MMA warpgroups) runs every
+  // K at D = 384: each tile's epilogue runs under the next tile's MMAs, and the residual arrives during the main loop.
   // ln_split: 0 auto (D = 384), 1 never (the full-row MODE 0 / MODE 1 kernel), 2 always.  The row statistics order is
   // chosen by K inside the kernel, never by the batch.  MODE 1 (ln_cta_group = 2 with ln_split = 1) shares the W tile
   // of two 64-row tiles by multicast.  Where the fused kernels are used at all is decided by the caller from the batch
@@ -1953,8 +1961,11 @@ int parseq_bench_tma_stream(void* buf, int64_t bytes, int cluster, int ctas, int
 }
 
 int64_t parseq_debug_int(parseq_engine* e, const char* name) {
-  if (e == nullptr || name == nullptr) return -1;
+  if (name == nullptr) return -1;
   const std::string n(name);
+  // launch options: per handle, or (NULL handle) those of the bare kernel exports; 0 until the first MODE 2 launch
+  if (n == "ln_clusters") return (e ? e->lo : g_default_opts).ln_clusters;
+  if (e == nullptr) return -1;
   if (n == "ar2_occupancy_mt1_cs8") return e->ar2_occ[1][0];
   if (n == "ar2_occupancy_mt2_cs8") return e->ar2_occ[2][0];
   if (n == "ar2_occupancy_mt1_cs6") return e->ar2_occ[1][1];

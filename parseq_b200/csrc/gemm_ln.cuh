@@ -18,12 +18,13 @@
 // MODE 0: one CTA per 64-row tile, all D columns; warpgroup w accumulates columns [D/2 w, D/2 (w + 1)).
 // MODE 1: a cluster of two CTAs on 128 rows; each CTA loads half of the W tile and multicasts it into both, so every W
 //         byte is fetched once per 128 rows.  Same work per row as MODE 0: bit-identical results.
-// MODE 2 (D = 384): persistent; a cluster of two CTAs walks 128-row tiles with the grid's stride.  CTA r computes the
-//         columns [192 r, 192 r + 192) of all 128 rows (warpgroup w: rows 64 w.., wgmma m64n192k16), staging only its
-//         half of W; each CTA loads 64 of the A rows and multicasts them into both.  The producer runs ahead into the
-//         next tile's k-blocks while the MMA warpgroups run the epilogue, and TMA-loads the tile's x slice into shared
-//         memory during the main loop.  The row statistics of the column parts are exchanged through distributed
-//         shared memory.  Their summation order reproduces the kernel each K used before (see gln_pair_epilogue).
+// MODE 2 (D = 384): persistent; a cluster of two CTAs walks 64-row tiles with the grid's stride.  CTA r computes the
+//         columns [192 r, 192 r + 192) (wgmma m64n192k16), staging its own A rows and only its half of W.  The two MMA
+//         warpgroups of a CTA take the cluster's tiles in turn ("ping-pong", as in gemm.cuh): one warpgroup's epilogue
+//         runs under the other's main loop.  The producer TMA-loads each tile's x slice into the warpgroup's own
+//         shared-memory buffer ahead of the main loop.  The row statistics of the column parts are exchanged through
+//         distributed shared memory.  Their summation order reproduces the kernel each K used before (see
+//         gln_pair_epilogue).
 #pragma once
 #include "gemm.cuh"
 
@@ -50,6 +51,7 @@ struct GemmLnCfg {
   static constexpr int kCols = D;                                     // columns per CTA
   static constexpr int kNW = kCols / 2;                               // columns per MMA warpgroup
   static constexpr int kParts = 2;                                    // column parts of a row
+  static constexpr int kABox = GLN_BLOCK_M;                           // A rows per TMA box
   static constexpr int kLoadRows = MODE == 1 ? D / 2 : kCols;         // W rows this CTA loads per k-block
   static constexpr int kBox = kLoadRows > 256 ? kLoadRows / 2 : kLoadRows;   // TMA box rows (at most 256)
   static constexpr int kABytes = GLN_BLOCK_M * GEMM_BLOCK_K * 2;      // 8 KB
@@ -66,24 +68,26 @@ struct GemmLnCfg {
   static_assert(kStages >= 3, "pipeline depth");
 };
 
-// MODE 2.  Shared memory: 3 operand stages (A 128 x 64 + W 192 x 64), the x slice of a tile (96 KB), the parameters.
+// MODE 2.  Shared memory: 3 operand stages (A 64 x 64 + W 192 x 64), one x slice per MMA warpgroup (2 x 48 KB), the
+// parameters.
 template <int D>
 struct GemmLnCfg<D, 2> {
   static_assert(D == 384, "the persistent column-split kernel is built for D = 384");
-  static constexpr int kCG = 2;
-  static constexpr int kTileM = 2 * GLN_BLOCK_M;                      // 128 rows per tile
+  static constexpr int kCG = 2;                                       // CTAs per cluster: the two column halves
+  static constexpr int kTileM = GLN_BLOCK_M;                          // 64 rows per tile
   static constexpr int kCols = D / 2;                                 // columns per CTA; one m64n192 per warpgroup
+  static constexpr int kABox = GLN_BLOCK_M;                           // A rows per TMA box
   static constexpr int kBox = kCols;                                  // W rows per TMA box
-  static constexpr int kABytes = kTileM * GEMM_BLOCK_K * 2;           // 16 KB: the 64-row halves of both CTAs
+  static constexpr int kABytes = GLN_BLOCK_M * GEMM_BLOCK_K * 2;      // 8 KB
   static constexpr int kBBytes = kCols * GEMM_BLOCK_K * 2;            // 24 KB
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = 3;
   static constexpr int kXBoxCols = 32;                                // fp32 x boxes: one 128-B swizzle row wide
-  static constexpr int kXBoxBytes = kTileM * kXBoxCols * 4;           // 16 KB
-  static constexpr int kXBytes = kTileM * kCols * 4;                  // 96 KB
+  static constexpr int kXBoxBytes = GLN_BLOCK_M * kXBoxCols * 4;      // 8 KB
+  static constexpr int kXBytes = GLN_BLOCK_M * kCols * 4;             // 48 KB: one warpgroup's tile
   static constexpr int kParamBytes = 3 * kCols * 4 + 2 * 2 * 4 * GLN_BLOCK_M * 4;   // bias, gamma, beta; [wg][round][part][row]
   static constexpr int kBarBytes = 256;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kXBytes + kParamBytes + kBarBytes + 1024;
+  static constexpr int kSmemBytes = kStages * kStageBytes + 2 * kXBytes + kParamBytes + kBarBytes + 1024;
   static_assert(kSmemBytes <= 232448, "shared memory");
 };
 
@@ -178,15 +182,15 @@ __device__ __forceinline__ void gln_epilogue(float (&acc)[NW / 2], float* __rest
   }
 }
 
-// Epilogue of MODE 2 for one MMA warpgroup: `acc` holds rows m0 + [0, 64) x the CTA's columns c0 + [0, D/2); the tile's
-// x slice is in shared memory (xs: D/64 TMA boxes of [128 rows][32] fp32, 128B swizzle; this warpgroup's rows start at
-// xs_row).  The x buffer is released on x_empty as soon as it has been read.  The row statistics are summed per column
-// part in the order of the kernel that ran this K before: PARTS = 4, 96-column parts (rank 2 + half), each thread
-// keeping one sum per half; PARTS = 2, one 192-column part per CTA, with the in-thread order of a MODE 0 warpgroup.
-// The partials go to both CTAs' s_part (this warpgroup's [round][part][row]); stat_bar[round] collects the arrivals of
-// this warpgroup and of the peer CTA's warpgroup with the same rows (completing once per tile, parity `par`).
+// Epilogue of MODE 2 for one MMA warpgroup: `acc` holds rows m0 + [0, 64) x the CTA's columns c0 + [0, D/2); their x
+// slice is in the warpgroup's shared-memory buffer (xs: D/64 TMA boxes of [64 rows][32] fp32, 128B swizzle).  The x
+// buffer is released on x_empty as soon as it has been read.  The row statistics are summed per column part in the order
+// of the kernel that ran this K before: PARTS = 4, 96-column parts (rank 2 + half), each thread keeping one sum per
+// half; PARTS = 2, one 192-column part per CTA, with the in-thread order of a MODE 0 warpgroup.  The partials go to both
+// CTAs' s_part (this warpgroup's [round][part][row]); stat_bar[round] collects the arrivals of this warpgroup and of the
+// peer CTA's warpgroup with the same rows (completing once per tile of the warpgroup, parity `par`).
 template <int D, int PARTS>
-__device__ __forceinline__ void gln_pair_epilogue(float (&acc)[D / 4], const uint8_t* xs, int xs_row, float* __restrict__ x,
+__device__ __forceinline__ void gln_pair_epilogue(float (&acc)[D / 4], const uint8_t* xs, float* __restrict__ x,
                                                   __nv_bfloat16* __restrict__ xn, int M, float eps, int m0, int c0,
                                                   uint32_t rank, const float* s_bias, const float* s_gamma,
                                                   const float* s_beta, float* s_part, uint64_t* stat_bar, uint32_t par,
@@ -201,7 +205,7 @@ __device__ __forceinline__ void gln_pair_epilogue(float (&acc)[D / 4], const uin
   float* xa = x + static_cast<long long>(m0 + lr) * D + c0 + 2 * (lane & 3);
   float* xb = xa + 8ll * D;
   // 128B swizzle: 16-B chunk c of row r sits at chunk c ^ (r % 8); r % 8 = lane / 4 for both rows
-  const uint8_t* xsa = xs + (xs_row + lr) * 128 + (lane & 1) * 8;
+  const uint8_t* xsa = xs + lr * 128 + (lane & 1) * 8;
   const uint8_t* xsb = xsa + 8 * 128;
   const uint32_t peer = rank ^ 1u;
 
@@ -249,7 +253,7 @@ __device__ __forceinline__ void gln_pair_epilogue(float (&acc)[D / 4], const uin
       sa[h] += __shfl_xor_sync(0xffffffffu, sa[h], 2);
       sb[h] += __shfl_xor_sync(0xffffffffu, sb[h], 1);
       sb[h] += __shfl_xor_sync(0xffffffffu, sb[h], 2);
-      float* slot = slots + (static_cast<int>(rank) * kH + h) * GLN_BLOCK_M;
+      float* slot = slots + (static_cast<int>(rank & 1u) * kH + h) * GLN_BLOCK_M;
       if ((lane & 3) == 0) {
         slot[lr] = sa[h];
         slot[lr + 8] = sb[h];
@@ -281,10 +285,12 @@ __device__ __forceinline__ void gln_pair_epilogue(float (&acc)[D / 4], const uin
   }
 }
 
-// MODE 2 (see the top of the file).  Grid: clusters of two CTAs, at most one per SM pair; cluster c takes the tiles
-// c, c + clusters, ...  Barriers: full/empty per operand stage (empty: the two MMA warpgroups of both CTAs, since every
-// stage holds A rows multicast by the peer), x_full / x_empty for the x buffer, stat_bar[wg][round] for the row
-// statistics of the warpgroup's rows.
+// MODE 2 (see the top of the file).  Grid: clusters of two CTAs; cluster c takes the 64-row tiles c, c + clusters, ...
+// and its j-th tile goes to MMA warpgroup j % 2 of both CTAs.  CTA r computes columns [192 r, 192 r + 192) and loads its
+// own A and W boxes: no operand is multicast, so a stage is free as soon as the warpgroup that read it releases it, and
+// neither CTA's ring waits on the other's.  Barriers: full/empty per operand stage, x_full[wg] / x_empty[wg] for the
+// warpgroups' x buffers, stat_bar[wg][round] for the row statistics of the warpgroup's rows.  Both CTAs walk every tile
+// of their cluster, also rows past M (TMA zero-fills them, the stores are guarded).
 template <int D>
 __device__ __forceinline__ void gln_pair_persistent(const CUtensorMap* tmA, const CUtensorMap* tmB, const CUtensorMap* tmX,
                                                     float* __restrict__ x, __nv_bfloat16* __restrict__ xn,
@@ -294,20 +300,20 @@ __device__ __forceinline__ void gln_pair_persistent(const CUtensorMap* tmA, cons
   const uint32_t raw_addr = smem_u32(smem_raw);
   const uint32_t pad = ((raw_addr + 1023u) & ~1023u) - raw_addr;
   uint8_t* smem = smem_raw + pad;
-  uint8_t* xs = smem + Cfg::kStages * Cfg::kStageBytes;
-  float* s_bias = reinterpret_cast<float*>(xs + Cfg::kXBytes);
+  uint8_t* xs = smem + Cfg::kStages * Cfg::kStageBytes;  // [wg][48 KB]
+  float* s_bias = reinterpret_cast<float*>(xs + 2 * Cfg::kXBytes);
   float* s_gamma = s_bias + Cfg::kCols;
   float* s_beta = s_gamma + Cfg::kCols;
   float* s_part = s_beta + Cfg::kCols;                 // [wg][round][4 parts][64 rows]
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(s_bias) + Cfg::kParamBytes);
   uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* x_full = empty_bar + Cfg::kStages;
-  uint64_t* x_empty = x_full + 1;
-  uint64_t* stat_bar = x_empty + 1;                    // [wg][round]
+  uint64_t* x_full = empty_bar + Cfg::kStages;         // [wg]
+  uint64_t* x_empty = x_full + 2;                      // [wg]
+  uint64_t* stat_bar = x_empty + 2;                    // [wg][round]
 
   const uint32_t rank = cluster_ctarank();
-  const int cluster = static_cast<int>(blockIdx.x) / 2, clusters = static_cast<int>(gridDim.x) / 2;
-  const int c0 = static_cast<int>(rank) * Cfg::kCols;   // first column of this CTA
+  const int cluster = static_cast<int>(blockIdx.x / Cfg::kCG), clusters = static_cast<int>(gridDim.x / Cfg::kCG);
+  const int c0 = static_cast<int>(rank & 1u) * Cfg::kCols;   // first column of this CTA
   const int num_kb = (p.K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K;
 
   grid_dep_launch();
@@ -317,11 +323,13 @@ __device__ __forceinline__ void gln_pair_persistent(const CUtensorMap* tmA, cons
     prefetch_tmap(tmX);
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 4);
+      mbar_init(&empty_bar[s], 1);                     // the one warpgroup that reads the stage
     }
-    mbar_init(x_full, 1);
-    mbar_init(x_empty, 256);                           // every MMA thread
-    for (int i = 0; i < 4; ++i) mbar_init(&stat_bar[i], 2 * 128);   // a warpgroup and its peer
+    for (int w = 0; w < 2; ++w) {
+      mbar_init(&x_full[w], 1);
+      mbar_init(&x_empty[w], 128);                     // every thread of the warpgroup
+    }
+    for (int i = 0; i < 4; ++i) mbar_init(&stat_bar[i], 2 * 128);   // a warpgroup and its peer's
     fence_mbar_init();
   }
   // bias / gamma / beta are weights (never written by a preceding kernel): stage them before the dependency wait
@@ -338,54 +346,79 @@ __device__ __forceinline__ void gln_pair_persistent(const CUtensorMap* tmA, cons
     setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
       int stage = 0;
-      uint32_t phase = 0, xphase = 0;
-      // the x slice of a tile is requested after its first k-blocks: those fill the ring while the MMA warpgroups
-      // still run the previous tile's epilogue, which frees the x buffer in its first pass
-      const int x_at = num_kb < Cfg::kStages ? num_kb : Cfg::kStages;
-      for (int tile = cluster; tile < p.num_m_tiles; tile += clusters) {
+      uint32_t phase = 0;
+      int j = 0;
+      for (int tile = cluster; tile < p.num_m_tiles; tile += clusters, ++j) {
         const int m0 = tile * Cfg::kTileM;
+        // the x slice first: its buffer was freed by pass 1 of the warpgroup's previous tile's epilogue, and the
+        // warpgroup finishes that epilogue before it needs this tile's operands
+        const int w = j & 1;
+        mbar_wait_mma(&x_empty[w], ((j >> 1) & 1) ^ 1u);
+        mbar_expect_tx(&x_full[w], Cfg::kXBytes);
+#pragma unroll
+        for (int b = 0; b < Cfg::kCols / Cfg::kXBoxCols; ++b)
+          tma_load_2d(xs + w * Cfg::kXBytes + b * Cfg::kXBoxBytes, tmX, &x_full[w], c0 + b * Cfg::kXBoxCols, m0);
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait_mma(&empty_bar[stage], phase ^ 1u);
           uint8_t* sa = smem + stage * Cfg::kStageBytes;
           mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-          tma_load_2d_mcast(sa + rank * (Cfg::kABytes / 2), tmA, &full_bar[stage], kb * GEMM_BLOCK_K,
-                            m0 + static_cast<int>(rank) * GLN_BLOCK_M, 0x3);
+          tma_load_2d(sa, tmA, &full_bar[stage], kb * GEMM_BLOCK_K, m0);
           tma_load_2d(sa + Cfg::kABytes, tmB, &full_bar[stage], kb * GEMM_BLOCK_K, c0);
           if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
-          if (kb + 1 == x_at) {
-            mbar_wait_mma(x_empty, xphase ^ 1u);
-            mbar_expect_tx(x_full, Cfg::kXBytes);
-#pragma unroll
-            for (int b = 0; b < Cfg::kCols / Cfg::kXBoxCols; ++b)
-              tma_load_2d(xs + b * Cfg::kXBoxBytes, tmX, x_full, c0 + b * Cfg::kXBoxCols, m0);
-            xphase ^= 1u;
-          }
         }
       }
     }
     __syncwarp();
   } else {
-    // ===================== MMA warpgroup wg: rows [64 wg, 64 wg + 64) of every tile, the CTA's columns =====================
+    // ===================== MMA warpgroup wg: the cluster's tiles wg, wg + 2, ... (ping-pong) =====================
     setmaxnreg_inc<232>();                              // 96 accumulators, and the epilogue's state next to them
     const int wg = (threadIdx.x >> 7) - 1;
     const bool parts4 = p.K >= GLN_PARTS4_MIN_K;
+    const bool leader = (threadIdx.x & 127) == 0;
+    uint8_t* xw = xs + wg * Cfg::kXBytes;
     int stage = 0;
     uint32_t phase = 0, par = 0;
+    if (wg == 1) ring_advance(stage, phase, num_kb, Cfg::kStages);   // tile 0 belongs to warpgroup 0
 #pragma unroll 1
-    for (int tile = cluster; tile < p.num_m_tiles; tile += clusters) {
-      const int m0 = tile * Cfg::kTileM + wg * GLN_BLOCK_M;
+    for (int tile = cluster + wg * clusters; tile < p.num_m_tiles; tile += 2 * clusters) {
+      const int m0 = tile * Cfg::kTileM;
+      // ordered main loops: wait until the other warpgroup has issued every MMA of the cluster's previous tile
+      if (tile != cluster) named_bar_sync(1 + wg, 256);
       float acc[Cfg::kCols / 2];
 #pragma unroll
       for (int i = 0; i < Cfg::kCols / 2; ++i) acc[i] = 0.0f;
-      wg_mainloop<Cfg::kCols, true>(acc, smem, Cfg::kStageBytes, wg * (Cfg::kABytes / 2), Cfg::kABytes, full_bar, empty_bar,
-                                    Cfg::kStages, num_kb, stage, phase);
-      mbar_wait_mma(x_full, par);
+      int prev = -1;
+#pragma unroll 1
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait_mma(&full_bar[stage], phase);
+        const uint32_t base = smem_u32(smem + stage * Cfg::kStageBytes);
+        const uint64_t da = make_desc_k_sw128(base);
+        const uint64_t db = make_desc_k_sw128(base + Cfg::kABytes);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < GEMM_BLOCK_K / 16; ++k)
+          wgmma_bf16<Cfg::kCols>(acc, da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k),
+                                 static_cast<uint32_t>((kb | k) != 0));
+        wgmma_commit();
+        if (prev >= 0) {                                 // the MMAs of this k-block are queued: free the previous stage
+          wgmma_wait<1>();
+          if (leader) mbar_arrive(&empty_bar[prev]);
+        }
+        prev = stage;
+        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
+      }
+      if (tile + clusters < p.num_m_tiles) named_bar_arrive(1 + (wg ^ 1), 256);   // the other warpgroup may start its main loop
+      wgmma_wait<0>();
+      wgmma_reg_fence(acc);
+      if (leader) mbar_arrive(&empty_bar[prev]);
+      ring_advance(stage, phase, num_kb, Cfg::kStages);            // skip the other warpgroup's next tile
+      mbar_wait_mma(&x_full[wg], par);
       if (parts4)
-        gln_pair_epilogue<D, 4>(acc, xs, wg * GLN_BLOCK_M, x, xn, p.M, p.eps, m0, c0, rank, s_bias, s_gamma, s_beta,
-                                s_part + wg * 2 * 4 * GLN_BLOCK_M, stat_bar + 2 * wg, par, x_empty);
+        gln_pair_epilogue<D, 4>(acc, xw, x, xn, p.M, p.eps, m0, c0, rank, s_bias, s_gamma, s_beta,
+                                s_part + wg * 2 * 4 * GLN_BLOCK_M, stat_bar + 2 * wg, par, &x_empty[wg]);
       else
-        gln_pair_epilogue<D, 2>(acc, xs, wg * GLN_BLOCK_M, x, xn, p.M, p.eps, m0, c0, rank, s_bias, s_gamma, s_beta,
-                                s_part + wg * 2 * 4 * GLN_BLOCK_M, stat_bar + 2 * wg, par, x_empty);
+        gln_pair_epilogue<D, 2>(acc, xw, x, xn, p.M, p.eps, m0, c0, rank, s_bias, s_gamma, s_beta,
+                                s_part + wg * 2 * 4 * GLN_BLOCK_M, stat_bar + 2 * wg, par, &x_empty[wg]);
       par ^= 1u;
     }
   }

@@ -10,7 +10,10 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <mutex>
+#include <set>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/parseq_b200.h"
@@ -132,9 +135,7 @@ uint16_t f32_to_bf16_rne(float f) {
 struct LaunchOpts {
   int sm_count = 0;
   bool use_pdl = true;          // programmatic dependent launch on every kernel of the forward chain
-  int block_n = 0;              // accepted (0/64/128/192/256); the GEMM has one 128 x 128 tile shape
-  int cta_group = 0;            // accepted (0/1/2); the GEMM runs single-CTA tiles
-  int ln_cta_group = 0;         // same for the fused GEMM + LayerNorm kernel
+  int ln_cta_group = 0;         // fused GEMM + LayerNorm full-row kernel: 2 = CTA pairs (MODE 1), else single CTAs (MODE 0)
   int ln_split = 0;             // fused GEMM + LayerNorm: 2 = persistent column-split CTA pairs (gemm_ln.cuh MODE 2), 0 = auto (MODE 2 at D = 384), 1 = never
   int mlp_cta_group = 0;        // one-kernel MLP (mlp_ln.cuh): 0 = auto (pairs), 1 / 2 = forced
   bool pair_pdl = false;        // experiments: programmatic dependent launch also on CTA-pair (cluster) launches
@@ -153,38 +154,63 @@ int ensure_sm_count(LaunchOpts& o) {
   return PARSEQ_OK;
 }
 
-// cudaLaunchKernelEx wrapper: optional PDL attribute (the kernels call griddepcontrol.{launch_dependents,wait}).
-template <typename... KArgs, typename... Args>
-int launch_k(const LaunchOpts& lo, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
+// The configuration of one cudaLaunchKernelEx call.  cluster > 0 sets a cluster dimension of cluster x 1 x 1 (a cluster
+// of 1 is an explicit attribute too); pdl allows programmatic dependent launch (the kernels call
+// griddepcontrol.{launch_dependents,wait}).  Not copyable: `cfg.attrs` points into the object.  The occupancy queries
+// take `cfg` as well.
+struct LaunchConfig {
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = lo.use_pdl ? 1 : 0;
-  PQ_CUDA(cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...));
+  cudaLaunchAttribute attr[2];
+  LaunchConfig(dim3 grid, dim3 block, size_t smem, cudaStream_t st, unsigned cluster, bool pdl) {
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cfg.attrs = attr;
+    if (cluster > 0) {
+      attr[cfg.numAttrs].id = cudaLaunchAttributeClusterDimension;
+      attr[cfg.numAttrs].val.clusterDim.x = cluster;
+      attr[cfg.numAttrs].val.clusterDim.y = 1;
+      attr[cfg.numAttrs].val.clusterDim.z = 1;
+      ++cfg.numAttrs;
+    }
+    if (pdl) {
+      attr[cfg.numAttrs].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+      attr[cfg.numAttrs].val.programmaticStreamSerializationAllowed = 1;
+      ++cfg.numAttrs;
+    }
+  }
+  LaunchConfig(const LaunchConfig&) = delete;
+  LaunchConfig& operator=(const LaunchConfig&) = delete;
+};
+
+template <typename... KArgs, typename... Args>
+int launch_ex(const LaunchConfig& lc, void (*kern)(KArgs...), Args... args) {
+  PQ_CUDA(cudaLaunchKernelEx(&lc.cfg, kern, static_cast<KArgs>(args)...));
   return PARSEQ_OK;
 }
-
-// instantiate + set the smem attribute of every configuration outside of any stream capture
-template <int EPI, int STORE>
-int warm_gemm_cfg() {
-  return cudaFuncSetAttribute(pq::gemm_bf16_wgmma_kernel<EPI, STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                              pq::GemmCfg::smem_bytes<STORE != pq::ST_REG>()) == cudaSuccess ? PARSEQ_OK
-                                                                      : fail(PARSEQ_ERR_CUDA, "cudaFuncSetAttribute(gemm)");
+// a launch without a cluster attribute, with PDL as the options say
+template <typename... KArgs, typename... Args>
+int launch_k(const LaunchOpts& lo, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
+  return launch_ex(LaunchConfig(grid, block, smem, st, 0, lo.use_pdl), kern, args...);
 }
+// PDL on a launch of cg-CTA clusters of the forward chain: CTA pairs take it only with the "pair_pdl" option
+bool cluster_pdl(const LaunchOpts& lo, int cg) { return lo.use_pdl && (cg == 1 || lo.pair_pdl); }
+
+// Calls f(std::integral_constant<int, D>) for the embedding widths the kernels are instantiated for.
+template <typename F>
+int dispatch_width(int D, const char* what, F&& f) {
+  switch (D) {
+    case 192: return f(std::integral_constant<int, 192>{});
+    case 384: return f(std::integral_constant<int, 384>{});
+    case 768: return f(std::integral_constant<int, 768>{});
+    default: return fail(PARSEQ_ERR_UNSUPPORTED, std::string(what) + ": embed_dim must be 192, 384 or 768");
+  }
+}
+
 template <int EPI, int STORE>
 int launch_gemm_cfg(const LaunchOpts& lo, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to,
                     const pq::GemmParams& p, int tiles, cudaStream_t st) {
-  static bool attr_set = false;            // the bare kernel entry point may run before any engine handle exists
-  if (!attr_set) {
-    PQ_TRY((warm_gemm_cfg<EPI, STORE>()));
-    attr_set = true;
-  }
   const int grid = tiles < lo.sm_count ? tiles : lo.sm_count;   // persistent: one CTA per SM, tiles strided
   return launch_k(lo, pq::gemm_bf16_wgmma_kernel<EPI, STORE>, dim3(static_cast<unsigned>(grid)), dim3(pq::GEMM_THREADS),
                   pq::GemmCfg::smem_bytes<STORE != pq::ST_REG>(), st, ta, tb, to, p);
@@ -223,13 +249,16 @@ constexpr auto ar2_kernel() {
     else return pq::dec_ar2_kernel<D, MT, CS, HS>;
   }
 }
+template <typename... KArgs>
+int set_smem(void (*kern)(KArgs...), size_t bytes) {
+  PQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes)));
+  return PARSEQ_OK;
+}
 template <int D, int MT, int CS, bool WIDE, int IDP>
 int ar2_attr() {
-  PQ_CUDA(cudaFuncSetAttribute(ar2_kernel<D, MT, CS, false, WIDE, IDP>(), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               static_cast<int>(pq::dec_ar2_smem_bytes<D, MT, CS, IDP>())));
+  PQ_TRY(set_smem(ar2_kernel<D, MT, CS, false, WIDE, IDP>(), pq::dec_ar2_smem_bytes<D, MT, CS, IDP>()));
   if constexpr (MT == 1 && CS == 8 && D / 64 <= CS)      // head-split variant for tiny batches
-    PQ_CUDA(cudaFuncSetAttribute(ar2_kernel<D, MT, CS, true, WIDE, IDP>(), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 static_cast<int>(pq::dec_ar2_smem_bytes<D, MT, CS, IDP>())));
+    PQ_TRY(set_smem(ar2_kernel<D, MT, CS, true, WIDE, IDP>(), pq::dec_ar2_smem_bytes<D, MT, CS, IDP>()));
   return PARSEQ_OK;
 }
 template <bool WIDE, int IDP>
@@ -242,50 +271,56 @@ int ar2_set_attributes() {
 }
 
 template <int D, int MODE>
-int gemm_ln_attr() {
-  PQ_CUDA(cudaFuncSetAttribute(pq::gemm_ln_fused_kernel<D, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               pq::GemmLnCfg<D, MODE>::kSmemBytes));
-  return PARSEQ_OK;
-}
-
+int gemm_ln_attr() { return set_smem(pq::gemm_ln_fused_kernel<D, MODE>, pq::GemmLnCfg<D, MODE>::kSmemBytes); }
 template <int D, int CG>
-int mlp_ln_attr() {
-  PQ_CUDA(cudaFuncSetAttribute(pq::mlp_ln_fused_kernel<D, CG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               pq::MlpLnCfg<D, CG>::kSmemBytes));
-  return PARSEQ_OK;
-}
+int mlp_ln_attr() { return set_smem(pq::mlp_ln_fused_kernel<D, CG>, pq::MlpLnCfg<D, CG>::kSmemBytes); }
 template <int NK>
-int attn_wgmma_attr() {
-  PQ_CUDA(cudaFuncSetAttribute(pq::enc_attention_wgmma_kernel<NK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               pq::atw_smem_bytes<NK>()));
-  return PARSEQ_OK;
-}
+int attn_wgmma_attr() { return set_smem(pq::enc_attention_wgmma_kernel<NK>, pq::atw_smem_bytes<NK>()); }
+template <int EPI, int STORE>
+int gemm_attr() { return set_smem(pq::gemm_bf16_wgmma_kernel<EPI, STORE>, pq::GemmCfg::smem_bytes<STORE != pq::ST_REG>()); }
+constexpr int kTmaBenchSmem = 12 * pq::A2_SLOT + 1024 + 256;
 
+// The dynamic shared memory limit of every engine kernel that needs more than the default.  cudaFuncSetAttribute acts on
+// the current device and must not run under stream capture: call through ensure_kernel_attributes.
 int init_kernel_attributes() {
-  PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar_kernel<192, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pq::dec_ar_smem_bytes<192>())));
-  PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar_kernel<192, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pq::dec_ar_smem_bytes<192>())));
-  PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar_kernel<384, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pq::dec_ar_smem_bytes<384>())));
-  PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar_kernel<384, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pq::dec_ar_smem_bytes<384>())));
-  PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar_kernel<768, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pq::dec_ar_smem_bytes<768>())));
-  PQ_CUDA(cudaFuncSetAttribute(pq::dec_ar_kernel<768, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pq::dec_ar_smem_bytes<768>())));
+  PQ_TRY(set_smem(pq::dec_ar_kernel<192, 1>, pq::dec_ar_smem_bytes<192>()));
+  PQ_TRY(set_smem(pq::dec_ar_kernel<192, 2>, pq::dec_ar_smem_bytes<192>()));
+  PQ_TRY(set_smem(pq::dec_ar_kernel<384, 1>, pq::dec_ar_smem_bytes<384>()));
+  PQ_TRY(set_smem(pq::dec_ar_kernel<384, 2>, pq::dec_ar_smem_bytes<384>()));
+  PQ_TRY(set_smem(pq::dec_ar_kernel<768, 1>, pq::dec_ar_smem_bytes<768>()));
+  PQ_TRY(set_smem(pq::dec_ar_kernel<768, 2>, pq::dec_ar_smem_bytes<768>()));
   PQ_TRY((ar2_set_attributes<false, 32>()));
   PQ_TRY((ar2_set_attributes<true, 32>()));
   PQ_TRY((ar2_set_attributes<false, 64>()));
   PQ_TRY((ar2_set_attributes<true, 64>()));
-  PQ_CUDA(cudaFuncSetAttribute(pq::dec_ln_head_argmax_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, 120 * 1024));
-  PQ_CUDA(cudaFuncSetAttribute(pq::dec_ln_head_argmax_kernel<384>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-  PQ_CUDA(cudaFuncSetAttribute(pq::dec_ln_head_argmax_kernel<768>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+  PQ_TRY(set_smem(pq::dec_ln_head_argmax_kernel<192>, 120 * 1024));
+  PQ_TRY(set_smem(pq::dec_ln_head_argmax_kernel<384>, 160 * 1024));
+  PQ_TRY(set_smem(pq::dec_ln_head_argmax_kernel<768>, 226 * 1024));
   PQ_TRY((gemm_ln_attr<192, 0>())); PQ_TRY((gemm_ln_attr<384, 0>())); PQ_TRY((gemm_ln_attr<192, 1>()));
   PQ_TRY((gemm_ln_attr<384, 1>())); PQ_TRY((gemm_ln_attr<384, 2>()));
   PQ_TRY((mlp_ln_attr<192, 1>())); PQ_TRY((mlp_ln_attr<384, 1>())); PQ_TRY((mlp_ln_attr<192, 2>())); PQ_TRY((mlp_ln_attr<384, 2>()));
   PQ_TRY((attn_wgmma_attr<128>())); PQ_TRY((attn_wgmma_attr<256>()));
-  PQ_TRY((warm_gemm_cfg<pq::EPI_F32, pq::ST_REG>()));
-  PQ_TRY((warm_gemm_cfg<pq::EPI_F32_RESID, pq::ST_REG>()));
-  PQ_TRY((warm_gemm_cfg<pq::EPI_BF16, pq::ST_REG>()));
-  PQ_TRY((warm_gemm_cfg<pq::EPI_BF16, pq::ST_TMA_2D>()));
-  PQ_TRY((warm_gemm_cfg<pq::EPI_BF16, pq::ST_TMA_3D>()));
-  PQ_TRY((warm_gemm_cfg<pq::EPI_GELU_BF16, pq::ST_REG>()));
-  PQ_TRY((warm_gemm_cfg<pq::EPI_GELU_BF16, pq::ST_TMA_2D>()));
+  PQ_TRY((gemm_attr<pq::EPI_F32, pq::ST_REG>()));
+  PQ_TRY((gemm_attr<pq::EPI_F32_RESID, pq::ST_REG>()));
+  PQ_TRY((gemm_attr<pq::EPI_BF16, pq::ST_REG>()));
+  PQ_TRY((gemm_attr<pq::EPI_BF16, pq::ST_TMA_2D>()));
+  PQ_TRY((gemm_attr<pq::EPI_BF16, pq::ST_TMA_3D>()));
+  PQ_TRY((gemm_attr<pq::EPI_GELU_BF16, pq::ST_REG>()));
+  PQ_TRY((gemm_attr<pq::EPI_GELU_BF16, pq::ST_TMA_2D>()));
+  PQ_TRY(set_smem(pq::tma_stream_bench_kernel, kTmaBenchSmem));
+  return PARSEQ_OK;
+}
+
+// init_kernel_attributes once per device: by parseq_create, and by the bare kernel exports, which may run without a handle
+int ensure_kernel_attributes() {
+  static std::mutex mu;
+  static std::set<int> done;
+  int dev = 0;
+  PQ_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(mu);
+  if (done.count(dev) != 0) return PARSEQ_OK;
+  PQ_TRY(init_kernel_attributes());
+  done.insert(dev);
   return PARSEQ_OK;
 }
 
@@ -347,11 +382,6 @@ template <int D, int MODE>
 int launch_gemm_ln(LaunchOpts& lo, const void* A, long long lda, const void* W, long long ldw, const float* bias, int M, int K, float* x,
                    const float* gamma, const float* beta, float eps, void* xn, cudaStream_t st) {
   using Cfg = pq::GemmLnCfg<D, MODE>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    PQ_TRY((gemm_ln_attr<D, MODE>()));
-    attr_set = true;
-  }
   CUtensorMap ta, tb, tx;
   PQ_TRY(make_tmap(&ta, A, 2, M, K, lda, pq::GEMM_BLOCK_K, Cfg::kABox));
   PQ_TRY(make_tmap(&tb, W, 2, D, K, ldw, pq::GEMM_BLOCK_K, Cfg::kBox));
@@ -361,36 +391,23 @@ int launch_gemm_ln(LaunchOpts& lo, const void* A, long long lda, const void* W, 
   p.M = M; p.K = K; p.bias = bias; p.gamma = gamma; p.beta = beta; p.eps = eps;
   p.num_m_tiles = (M + Cfg::kTileM - 1) / Cfg::kTileM;
   int clusters = p.num_m_tiles;
-  cudaLaunchConfig_t cfg{};
-  cfg.blockDim = dim3(pq::GLN_THREADS);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = Cfg::kCG;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
   if constexpr (MODE == 2) {
     // persistent: as many CTA pairs as the occupancy query admits on this device, each walking the tiles with the grid's
     // stride; x slices are fetched by TMA (x: 16-B aligned)
     PQ_TRY(make_tmap(&tx, x, 4, M, D, D, Cfg::kXBoxCols, pq::GLN_BLOCK_M));
     if (lo.ln_clusters == 0) {
-      cfg.gridDim = dim3(static_cast<unsigned>(lo.sm_count / Cfg::kCG * Cfg::kCG));
-      PQ_CUDA(cudaOccupancyMaxActiveClusters(&lo.ln_clusters, pq::gemm_ln_fused_kernel<D, MODE>, &cfg));
+      const LaunchConfig occ(dim3(static_cast<unsigned>(lo.sm_count / Cfg::kCG * Cfg::kCG)), dim3(pq::GLN_THREADS),
+                             Cfg::kSmemBytes, st, Cfg::kCG, false);
+      PQ_CUDA(cudaOccupancyMaxActiveClusters(&lo.ln_clusters, pq::gemm_ln_fused_kernel<D, MODE>, &occ.cfg));
       if (lo.ln_clusters <= 0) return fail(PARSEQ_ERR_CUDA, "gemm_ln: no cluster of the persistent kernel fits the device");
     }
     clusters = std::min(p.num_m_tiles, lo.ln_clusters);
   } else {
     tx = ta;                                                  // unused by MODE 0 / 1
   }
-  cfg.gridDim = dim3(static_cast<unsigned>(clusters * Cfg::kCG));
-  cfg.numAttrs = (lo.use_pdl && (MODE == 0 || lo.pair_pdl)) ? 2 : 1;
-  PQ_CUDA(cudaLaunchKernelEx(&cfg, pq::gemm_ln_fused_kernel<D, MODE>, ta, tb, tx, x, reinterpret_cast<__nv_bfloat16*>(xn), p));
-  return PARSEQ_OK;
+  return launch_ex(LaunchConfig(dim3(static_cast<unsigned>(clusters * Cfg::kCG)), dim3(pq::GLN_THREADS), Cfg::kSmemBytes, st,
+                                Cfg::kCG, cluster_pdl(lo, Cfg::kCG)),
+                   pq::gemm_ln_fused_kernel<D, MODE>, ta, tb, tx, x, reinterpret_cast<__nv_bfloat16*>(xn), p);
 }
 int gemm_ln_launch(LaunchOpts& lo, const void* A, long long lda, const void* W, long long ldw, const float* bias, int M, int D,
                    int K, float* x, const float* gamma, const float* beta, float eps, void* xn, cudaStream_t st) {
@@ -419,11 +436,6 @@ template <int D, int CG>
 int launch_mlp_ln(const LaunchOpts& lo, const void* xn, const void* W1, const float* b1, const void* W2, const float* b2, int M,
                   float* x, const float* gamma, const float* beta, float eps, void* xn_out, cudaStream_t st) {
   using Cfg = pq::MlpLnCfg<D, CG>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    PQ_TRY((mlp_ln_attr<D, CG>()));
-    attr_set = true;
-  }
   if ((reinterpret_cast<uintptr_t>(x) & 7u) != 0 || (reinterpret_cast<uintptr_t>(xn_out) & 3u) != 0)
     return fail(PARSEQ_ERR_INVALID_ARG, "mlp_ln: x must be 8-byte and xn_out 4-byte aligned");
   CUtensorMap txn, tw1, tw2;
@@ -433,22 +445,9 @@ int launch_mlp_ln(const LaunchOpts& lo, const void* xn, const void* W1, const fl
   pq::MlpLnParams p;
   p.M = M; p.b1 = b1; p.b2 = b2; p.gamma = gamma; p.beta = beta; p.eps = eps;
   p.num_m_tiles = (M + pq::GLN_BLOCK_M * CG - 1) / (pq::GLN_BLOCK_M * CG);
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(p.num_m_tiles * CG));
-  cfg.blockDim = dim3(pq::MLP_THREADS);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CG;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = (lo.use_pdl && (CG == 1 || lo.pair_pdl)) ? 2 : 1;
-  PQ_CUDA(cudaLaunchKernelEx(&cfg, pq::mlp_ln_fused_kernel<D, CG>, txn, tw1, tw2, x, reinterpret_cast<__nv_bfloat16*>(xn_out), p));
-  return PARSEQ_OK;
+  return launch_ex(LaunchConfig(dim3(static_cast<unsigned>(p.num_m_tiles * CG)), dim3(pq::MLP_THREADS), Cfg::kSmemBytes, st, CG,
+                                cluster_pdl(lo, CG)),
+                   pq::mlp_ln_fused_kernel<D, CG>, txn, tw1, tw2, x, reinterpret_cast<__nv_bfloat16*>(xn_out), p);
 }
 int mlp_ln_launch(LaunchOpts& lo, const void* xn, const void* W1, const float* b1, const void* W2, const float* b2, int M, int D,
                   float* x, const float* gamma, const float* beta, float eps, void* xn_out, cudaStream_t st) {
@@ -482,12 +481,6 @@ int layernorm_launch(const LaunchOpts& lo, const float* x, const float* g, const
 int enc_attention_launch(const LaunchOpts& lo, const void* qkv, int B, int T, int D, int heads, void* out, cudaStream_t st) {
   if (D != heads * pq::ATT_DH) return fail(PARSEQ_ERR_UNSUPPORTED, "encoder attention kernels cover head_dim=64");
   if (lo.attn_impl == 1 && T <= 256) {
-    static bool attr_set = false;            // the bare kernel entry point may run before any engine handle exists
-    if (!attr_set) {
-      PQ_TRY((attn_wgmma_attr<128>()));
-      PQ_TRY((attn_wgmma_attr<256>()));
-      attr_set = true;
-    }
     const dim3 grid(static_cast<unsigned>(B * heads), static_cast<unsigned>((T + 127) / 128));
     const __nv_bfloat16* q = reinterpret_cast<const __nv_bfloat16*>(qkv);
     __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);
@@ -545,8 +538,7 @@ struct parseq_engine {
   std::vector<__nv_bfloat16*> ckv_deep;           // cross K/V of decoder layers 1..dec_depth-1, laid out as ckv
   int dec_chunk = 128;              // images per decoder chain (each chain runs on its own stream)
   // persistent AR-loop kernel state (whole super-chunk)
-  bool use_ar_kernel = true;
-  int ar_impl = 2;                  // 2: cluster-owned kernel (dec_ar2.cuh), 1: grid-barrier kernel (dec_ar.cuh)
+  int ar_kernel = 2;                // option "ar_kernel": 0 chain, 1 grid-barrier kernel, 2 cluster kernel where it applies (ar_path)
   pq::DecAr2Maps ar2_maps[2];       // TMA descriptors (decoder weights, K/V cache) for cluster size 8 [0] and 6 [1]
   bool ar2_maps_ok = false;
   int ar2_clusters[3][2] = {{0, 0}, {0, 0}, {0, 0}};   // max co-resident clusters, index [MT][cluster size 6 ? 1 : 0]
@@ -1115,12 +1107,30 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
 }
 
 
-// ---- cluster-owned AR kernel (dec_ar2.cuh) ----
-// Heads of <= 96 classes run redundantly in every CTA; > 128 classes take the class-sliced head (WIDE); 97..128 classes
-// stay on the grid-barrier kernel (labels of up to 31 characters) or on the chain of separate kernels (longer labels).
-bool ar2_supported(const parseq_engine* e) {
-  return e->arch == 0 && e->cfg.dec_depth == 1 && e->cfg.dec_mlp_ratio == 4 && (e->C <= 96 || e->C > 128) && e->T <= 256 && e->dh_dec == 32;
+// ---- which implementation runs the AR loop ----
+// Why the grid-barrier kernel (dec_ar.cuh) cannot take this engine's AR loop, or nullptr if it can.
+const char* grid_barrier_limit(const parseq_engine* e) {
+  if (e->C > 128) return "ar_kernel = 1 (grid-barrier AR kernel) covers at most 128 head classes; use ar_kernel 0 or 2";
+  if (e->L > 32) return "ar_kernel = 1 (grid-barrier AR kernel) covers max_label_length <= 31; use ar_kernel 0 or 2";
+  if (e->cfg.dec_depth > 1) return "ar_kernel = 1 (grid-barrier AR kernel) covers dec_depth 1; use ar_kernel 0 or 2";
+  return nullptr;
 }
+enum class ArPath { Chain, GridBarrier, Cluster };
+// Option "ar_kernel" 2 (default) runs the cluster kernel (dec_ar2.cuh) where it applies: heads of <= 96 classes run
+// redundantly in every CTA, > 128 classes take the class-sliced head.  Anything else it cannot take (97..128 classes,
+// dec_mlp_ratio != 4) runs on the grid-barrier kernel if that holds it, else on the chain of separate kernels, as do
+// decoders of depth >= 2.  "ar_kernel" 1 (accepted only where the grid-barrier kernel applies) forces that kernel, 0 the
+// chain.
+ArPath ar_path(const parseq_engine* e) {
+  if (e->arch != 0 || e->ar_kernel == 0) return ArPath::Chain;
+  if (e->ar_kernel == 2 && e->cfg.dec_depth == 1 && e->cfg.dec_mlp_ratio == 4 && (e->C <= 96 || e->C > 128) && e->T <= 256 &&
+      e->dh_dec == 32)
+    return ArPath::Cluster;
+  if (grid_barrier_limit(e) == nullptr) return ArPath::GridBarrier;
+  return ArPath::Chain;
+}
+
+// ---- cluster-owned AR kernel (dec_ar2.cuh) ----
 bool ar2_wide(const parseq_engine* e) { return e->C > 128; }
 // weight descriptors: once per weight set (parseq_finalize); K/V cache descriptor: once per workspace
 int ar2_build_maps(parseq_engine* e) {
@@ -1143,25 +1153,15 @@ int ar2_build_maps(parseq_engine* e) {
   e->ar2_maps_ok = true;
   return PARSEQ_OK;
 }
+// ncl clusters of CS CTAs; the AR kernel is never launched with PDL
 template <int D, int MT, int CS, int IDP>
-void ar2_config(parseq_engine* e, cudaLaunchConfig_t& cfg, cudaLaunchAttribute* attr, int ncl, cudaStream_t st) {
-  cfg = cudaLaunchConfig_t{};
-  cfg.gridDim = dim3(static_cast<unsigned>(ncl * CS));
-  cfg.blockDim = dim3(pq::A2_LAUNCH_THREADS);
-  cfg.dynamicSmemBytes = pq::dec_ar2_smem_bytes<D, MT, CS, IDP>();
-  cfg.stream = st;
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CS;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
+LaunchConfig ar2_config(int ncl, cudaStream_t st) {
+  return LaunchConfig(dim3(static_cast<unsigned>(ncl * CS)), dim3(pq::A2_LAUNCH_THREADS), pq::dec_ar2_smem_bytes<D, MT, CS, IDP>(),
+                      st, CS, false);
 }
 template <int D, int MT, int CS, bool WIDE, int IDP>
 int ar2_launch_t(parseq_engine* e, const pq::DecAr2Params& p, int ncl, cudaStream_t st) {
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  ar2_config<D, MT, CS, IDP>(e, cfg, attr, ncl, st);
+  const LaunchConfig lc = ar2_config<D, MT, CS, IDP>(ncl, st);
   e->ar_last_per = p.per; e->ar_last_ncl = ncl; e->ar_last_cs = CS;
   e->ar_last_mt = MT; e->ar_last_hs = 0; e->ar_last_wide = WIDE ? 1 : 0; e->ar_last_idp = IDP;
   if constexpr (MT == 1 && CS == 8 && D / 64 <= CS) {
@@ -1169,12 +1169,10 @@ int ar2_launch_t(parseq_engine* e, const pq::DecAr2Params& p, int ncl, cudaStrea
     // cross-attention instead of whole images (bs = 1: 9 -> 2.5 us per step; same bits per head)
     if (p.per * (D / 64) <= CS) {
       e->ar_last_hs = 1;
-      PQ_CUDA(cudaLaunchKernelEx(&cfg, ar2_kernel<D, MT, CS, true, WIDE, IDP>(), e->ar2_maps[0], p));
-      return PARSEQ_OK;
+      return launch_ex(lc, ar2_kernel<D, MT, CS, true, WIDE, IDP>(), e->ar2_maps[0], p);
     }
   }
-  PQ_CUDA(cudaLaunchKernelEx(&cfg, ar2_kernel<D, MT, CS, false, WIDE, IDP>(), e->ar2_maps[CS == 6 ? 1 : 0], p));
-  return PARSEQ_OK;
+  return launch_ex(lc, ar2_kernel<D, MT, CS, false, WIDE, IDP>(), e->ar2_maps[CS == 6 ? 1 : 0], p);
 }
 template <int D, int MT, int CS, int IDP>
 int ar2_launch(parseq_engine* e, const pq::DecAr2Params& p, int ncl, cudaStream_t st) {
@@ -1187,13 +1185,11 @@ template <int D, int MT, int CS, int IDP>
 int ar2_max_clusters(parseq_engine* e) {
   int& cache = e->ar2_clusters[MT][CS == 6 ? 1 : 0];
   if (cache > 0) return cache;
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  ar2_config<D, MT, CS, IDP>(e, cfg, attr, e->lo.sm_count / CS, nullptr);
+  const LaunchConfig lc = ar2_config<D, MT, CS, IDP>(e->lo.sm_count / CS, nullptr);
   int n = 0;
   // (the cache is per engine, and so are the head width and the id pitch)
-  const cudaError_t qe = ar2_wide(e) ? cudaOccupancyMaxActiveClusters(&n, ar2_kernel<D, MT, CS, false, true, IDP>(), &cfg)
-                                     : cudaOccupancyMaxActiveClusters(&n, ar2_kernel<D, MT, CS, false, false, IDP>(), &cfg);
+  const cudaError_t qe = ar2_wide(e) ? cudaOccupancyMaxActiveClusters(&n, ar2_kernel<D, MT, CS, false, true, IDP>(), &lc.cfg)
+                                     : cudaOccupancyMaxActiveClusters(&n, ar2_kernel<D, MT, CS, false, false, IDP>(), &lc.cfg);
   if (qe != cudaSuccess || n <= 0) {
     cudaGetLastError();
     n = (CS == 8) ? (e->lo.sm_count / 10) : 1;   // unknown: a conservative guess for 8, "do not use" for 6
@@ -1239,94 +1235,68 @@ int ar2_dispatch(parseq_engine* e, pq::DecAr2Params& p, cudaStream_t st) {
   return fail(PARSEQ_ERR_STATE, "dec_ar2: no launch configuration");
 }
 
-// The whole AR loop (model.py:119-147) of B images in one persistent launch (csrc/dec_ar.cuh).
-int ar_decode(parseq_engine* e, const parseq_forward_args* a, int b0, int B, int L, float* logits, int* steps, cudaStream_t st) {
+// The whole AR loop (model.py:119-147) of B images in one persistent launch: the cluster kernel (dec_ar2.cuh) or the
+// grid-barrier kernel (dec_ar.cuh), as ar_path chose.
+int ar_decode(parseq_engine* e, ArPath path, const parseq_forward_args* a, int b0, int B, int L, float* logits, int* steps,
+              cudaStream_t st) {
   const int D = e->D;
   const std::string Ly = "decoder.layers.0.";
-  const bool testing = a->max_length < 0;
   PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * e->ids_ld + 255) / 256), dim3(256), 0, st, e->ar_ids, B, e->ids_ld,
                   e->V - 2, e->V - 1));
   e->launches++;
-  if (e->ar_impl == 2 && ar2_supported(e)) {
-    if (!e->ar2_maps_ok) PQ_TRY(ar2_build_maps(e));
-    pq::DecAr2Params q;
-    q.B = B; q.L = L; q.V = e->V; q.C = e->C; q.T = e->T; q.per = 0;
-    q.tbox = e->T <= 64 ? 64 : 128; q.tb = (e->T + 127) / 128;
-    q.qscale = 1.0f / std::sqrt(static_cast<float>(e->dh_dec));
-    q.qs = e->qs; q.kvtab = e->kvtab; q.posq = e->wf("pos_queries");
-    q.bo_s = e->wf(Ly + "self_attn.out_proj.bias"); q.bq_c = e->wf(Ly + "cross_attn.in_proj_bias");
-    q.bo_c = e->wf(Ly + "cross_attn.out_proj.bias"); q.b1 = e->wf(Ly + "linear1.bias"); q.b2 = e->wf(Ly + "linear2.bias");
-    q.bh = e->wf("head.bias");
-    q.g1 = e->wf(Ly + "norm1.weight"); q.be1 = e->wf(Ly + "norm1.bias");
-    q.g2 = e->wf(Ly + "norm2.weight"); q.be2 = e->wf(Ly + "norm2.bias");
-    q.g3 = e->wf("decoder.norm.weight"); q.be3 = e->wf("decoder.norm.bias");
-    q.ids = e->ar_ids; q.ids_ld = e->ids_ld; q.logits = logits;
-    q.forced = a->forced_ids ? a->forced_ids + static_cast<long long>(b0) * L : nullptr;
-    q.forced_ld = L;
-    q.prof = e->ar_prof_on ? e->ar_prof : nullptr;
-    {
-      const double macs = static_cast<double>(B) * L * (3.0 * D * D + 2.0 * D * e->Md + 1.0 * e->C * D + 2.0 * e->T * D);
-      TimedScope ts(e, st, CAT_DEC_AR, 2.0 * macs);
-      const bool lng = e->ids_ld == 64;
-      switch (D) {
-        case 192: PQ_TRY((lng ? ar2_dispatch<192, 64>(e, q, st) : ar2_dispatch<192, 32>(e, q, st))); break;
-        case 384: PQ_TRY((lng ? ar2_dispatch<384, 64>(e, q, st) : ar2_dispatch<384, 32>(e, q, st))); break;
-        case 768: PQ_TRY((lng ? ar2_dispatch<768, 64>(e, q, st) : ar2_dispatch<768, 32>(e, q, st))); break;
-        default: return fail(PARSEQ_ERR_UNSUPPORTED, "dec_ar2: embed_dim must be 192, 384 or 768");
-      }
-    }
-    if (testing && steps != nullptr) {
-      PQ_TRY(launch_k(e->lo, pq::ar_steps_kernel, dim3(1), dim3(256), 0, st, static_cast<const int*>(e->ar_ids), e->ids_ld, B, L,
-                      0, steps));
-      e->launches++;
-    }
-    return PARSEQ_OK;
-  }
-  if (e->C > 128) return fail(PARSEQ_ERR_UNSUPPORTED, "ar_kernel = 1 (grid-barrier AR kernel) covers at most 128 head classes");
-  if (e->L > 32) return fail(PARSEQ_ERR_UNSUPPORTED, "ar_kernel = 1 (grid-barrier AR kernel) covers max_label_length <= 31");
-  PQ_CUDA(cudaMemsetAsync(e->ar_bar, 0, 64, st));
+  // what both kernels read: the decoder's tables, bias and LayerNorm vectors, the id rows and the logits
+  auto common = [&](auto& p) {
+    p.B = B; p.L = L; p.V = e->V; p.C = e->C; p.T = e->T;
+    p.qscale = 1.0f / std::sqrt(static_cast<float>(e->dh_dec));
+    p.qs = e->qs; p.kvtab = e->kvtab; p.posq = e->wf("pos_queries");
+    p.bo_s = e->wf(Ly + "self_attn.out_proj.bias"); p.bq_c = e->wf(Ly + "cross_attn.in_proj_bias");
+    p.bo_c = e->wf(Ly + "cross_attn.out_proj.bias"); p.b1 = e->wf(Ly + "linear1.bias"); p.b2 = e->wf(Ly + "linear2.bias");
+    p.bh = e->wf("head.bias");
+    p.g1 = e->wf(Ly + "norm1.weight"); p.be1 = e->wf(Ly + "norm1.bias");
+    p.g2 = e->wf(Ly + "norm2.weight"); p.be2 = e->wf(Ly + "norm2.bias");
+    p.g3 = e->wf("decoder.norm.weight"); p.be3 = e->wf("decoder.norm.bias");
+    p.ids = e->ar_ids; p.ids_ld = e->ids_ld; p.logits = logits;
+    p.forced = a->forced_ids ? a->forced_ids + static_cast<long long>(b0) * L : nullptr;
+    p.forced_ld = L;
+    p.prof = e->ar_prof_on ? e->ar_prof : nullptr;
+  };
+  pq::DecAr2Params q;
   pq::DecArParams p;
-  p.B = B; p.L = L; p.Md = e->Md; p.V = e->V; p.C = e->C; p.T = e->T; p.heads = e->cfg.dec_num_heads;
-  p.qscale = 1.0f / std::sqrt(static_cast<float>(e->dh_dec));
-  p.qs = e->qs; p.kvtab = e->kvtab; p.posq = e->wf("pos_queries");
-  p.Wo_s = e->wb(Ly + "self_attn.out_proj.weight"); p.bo_s = e->wf(Ly + "self_attn.out_proj.bias");
-  p.Wq_c = e->wb(Ly + "cross_attn.in_proj_weight"); p.bq_c = e->wf(Ly + "cross_attn.in_proj_bias");
-  p.Wo_c = e->wb(Ly + "cross_attn.out_proj.weight"); p.bo_c = e->wf(Ly + "cross_attn.out_proj.bias");
-  p.W1 = e->wb(Ly + "linear1.weight"); p.b1 = e->wf(Ly + "linear1.bias");
-  p.W2 = e->wb(Ly + "linear2.weight"); p.b2 = e->wf(Ly + "linear2.bias");
-  p.Wh = e->wb("head.weight"); p.bh = e->wf("head.bias");
-  p.g1 = e->wf(Ly + "norm1.weight"); p.be1 = e->wf(Ly + "norm1.bias");
-  p.g2 = e->wf(Ly + "norm2.weight"); p.be2 = e->wf(Ly + "norm2.bias");
-  p.g3 = e->wf("decoder.norm.weight"); p.be3 = e->wf("decoder.norm.bias");
-  p.ckv = e->ckv; p.kv_rows = 1ll * e->max_batch * e->T; p.ids = e->ar_ids; p.ids_ld = e->ids_ld;
-  p.sa = e->ar_sa; p.ca = e->ar_ca; p.hd = e->ar_hd; p.y = e->ar_y; p.qc = e->ar_qc; p.part = e->ar_part;
-  p.logits = logits;
-  p.forced = a->forced_ids ? a->forced_ids + static_cast<long long>(b0) * L : nullptr;
-  p.forced_ld = L;
-  p.bar = e->ar_bar;
-  p.prof = e->ar_prof_on ? e->ar_prof : nullptr;
+  if (path == ArPath::Cluster) {
+    if (!e->ar2_maps_ok) PQ_TRY(ar2_build_maps(e));
+    common(q);
+    q.per = 0;
+    q.tbox = e->T <= 64 ? 64 : 128; q.tb = (e->T + 127) / 128;
+  } else {
+    PQ_CUDA(cudaMemsetAsync(e->ar_bar, 0, 64, st));
+    common(p);
+    p.Md = e->Md; p.heads = e->cfg.dec_num_heads;
+    p.Wo_s = e->wb(Ly + "self_attn.out_proj.weight"); p.Wq_c = e->wb(Ly + "cross_attn.in_proj_weight");
+    p.Wo_c = e->wb(Ly + "cross_attn.out_proj.weight"); p.W1 = e->wb(Ly + "linear1.weight"); p.W2 = e->wb(Ly + "linear2.weight");
+    p.Wh = e->wb("head.weight");
+    p.ckv = e->ckv; p.kv_rows = 1ll * e->max_batch * e->T;
+    p.sa = e->ar_sa; p.ca = e->ar_ca; p.hd = e->ar_hd; p.y = e->ar_y; p.qc = e->ar_qc; p.part = e->ar_part;
+    p.bar = e->ar_bar;
+  }
   {
     // per image and step: 3 D^2 (self out, cross q, cross out) + 2 D Md (MLP) + C D (head) + attention dots
     const double macs = static_cast<double>(B) * L * (3.0 * D * D + 2.0 * D * e->Md + 1.0 * e->C * D + 2.0 * e->T * D);
     TimedScope ts(e, st, CAT_DEC_AR, 2.0 * macs);
-    const dim3 grid(static_cast<unsigned>(e->lo.sm_count)), block(pq::DEC_THREADS);
-    switch (D) {
-      case 192:
-        if (e->T <= 128) PQ_TRY(launch_k(e->lo, pq::dec_ar_kernel<192, 1>, grid, block, pq::dec_ar_smem_bytes<192>(), st, p));
-        else PQ_TRY(launch_k(e->lo, pq::dec_ar_kernel<192, 2>, grid, block, pq::dec_ar_smem_bytes<192>(), st, p));
-        break;
-      case 384:
-        if (e->T <= 128) PQ_TRY(launch_k(e->lo, pq::dec_ar_kernel<384, 1>, grid, block, pq::dec_ar_smem_bytes<384>(), st, p));
-        else PQ_TRY(launch_k(e->lo, pq::dec_ar_kernel<384, 2>, grid, block, pq::dec_ar_smem_bytes<384>(), st, p));
-        break;
-      case 768:
-        if (e->T <= 128) PQ_TRY(launch_k(e->lo, pq::dec_ar_kernel<768, 1>, grid, block, pq::dec_ar_smem_bytes<768>(), st, p));
-        else PQ_TRY(launch_k(e->lo, pq::dec_ar_kernel<768, 2>, grid, block, pq::dec_ar_smem_bytes<768>(), st, p));
-        break;
-      default: return fail(PARSEQ_ERR_UNSUPPORTED, "dec_ar: embed_dim must be 192, 384 or 768");
+    if (path == ArPath::Cluster) {
+      PQ_TRY(dispatch_width(D, "dec_ar2", [&](auto w) {
+        constexpr int W = decltype(w)::value;
+        return e->ids_ld == 64 ? ar2_dispatch<W, 64>(e, q, st) : ar2_dispatch<W, 32>(e, q, st);
+      }));
+    } else {
+      PQ_TRY(dispatch_width(D, "dec_ar", [&](auto w) {
+        constexpr int W = decltype(w)::value;
+        const dim3 grid(static_cast<unsigned>(e->lo.sm_count)), block(pq::DEC_THREADS);
+        return e->T <= 128 ? launch_k(e->lo, pq::dec_ar_kernel<W, 1>, grid, block, pq::dec_ar_smem_bytes<W>(), st, p)
+                           : launch_k(e->lo, pq::dec_ar_kernel<W, 2>, grid, block, pq::dec_ar_smem_bytes<W>(), st, p);
+      }));
     }
   }
-  if (testing && steps != nullptr) {
+  if (a->max_length < 0 && steps != nullptr) {
     PQ_TRY(launch_k(e->lo, pq::ar_steps_kernel, dim3(1), dim3(256), 0, st, static_cast<const int*>(e->ar_ids), e->ids_ld, B, L, 0,
                     steps));
     e->launches++;
@@ -1376,12 +1346,10 @@ int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B,
     PQ_TRY(gemm(e, e->mem, D, Wkv, D, bkv, B * T, 2 * D, D, pq::EPI_BF16, 1.0f, nullptr, 0, 0,
                 const_cast<__nv_bfloat16*>(ckv_of(e, l)), 2 * D, e->main, 1ll * e->max_batch * T));
   }
-  // an AR loop that the cluster kernel cannot take (e.g. dec_mlp_ratio != 4) runs on the grid-barrier kernel if that holds
-  // it (<= 128 classes, L <= 32), else as a chain of separate kernels; so does every decoder of depth >= 2
-  const bool ar_done = a->decode_ar && e->use_ar_kernel &&
-                       ((e->ar_impl == 2 && ar2_supported(e)) || (e->C <= 128 && e->L <= 32 && e->cfg.dec_depth == 1));
+  const ArPath path = ar_path(e);
+  const bool ar_done = a->decode_ar && path != ArPath::Chain;
   if (ar_done) {
-    PQ_TRY(ar_decode(e, a, b0, B, L, logits, steps, e->main));
+    PQ_TRY(ar_decode(e, path, a, b0, B, L, logits, steps, e->main));
     if (a->refine_iters == 0) {      // nothing left for the chains but the final argmax
       if (ids_out != nullptr) PQ_TRY(argmax_rows(e, logits, L, B, L, 0, ids_out, L, 0, nullptr, 0, e->main));
       return PARSEQ_OK;
@@ -1523,7 +1491,7 @@ int parseq_create(const parseq_config* cfg, parseq_engine** out) {
     return fail(PARSEQ_ERR_NO_DEVICE, std::string("device is sm_") + std::to_string(prop.major * 10 + prop.minor) +
                                           ", the kernels are sm_90a (H100) only");
   const int sm_count = prop.multiProcessorCount;
-  PQ_TRY(init_kernel_attributes());
+  PQ_TRY(ensure_kernel_attributes());
   PQ_TRY(load_driver_api());
   if (cfg->arch != 0 && cfg->arch != 1) return fail(PARSEQ_ERR_INVALID_ARG, "arch: 0 (PARSeq) or 1 (ViTSTR)");
   const bool vitstr = cfg->arch == 1;
@@ -1747,7 +1715,7 @@ int parseq_finalize(parseq_engine* e, parseq_stream_t stream) {
   if (r != PARSEQ_OK) return r;
   if (ce != cudaSuccess) return fail(PARSEQ_ERR_CUDA, std::string("finalize: ") + cudaGetErrorString(ce));
   e->ar2_maps_ok = false;
-  if (ar2_supported(e)) PQ_TRY(ar2_build_maps(e));
+  if (ar_path(e) == ArPath::Cluster) PQ_TRY(ar2_build_maps(e));
   e->finalized = true;
   return PARSEQ_OK;
 }
@@ -1939,25 +1907,13 @@ int parseq_bench_tma_stream(void* buf, int64_t bytes, int cluster, int ctas, int
   const long long rows_total = 8192;                         // rows per 64-column block
   const int blocks = static_cast<int>(bytes / (rows_total * 128));
   if (blocks < 1) return fail(PARSEQ_ERR_INVALID_ARG, "bench_tma_stream: buffer too small");
+  PQ_TRY(ensure_kernel_attributes());
   CUtensorMap map;
   PQ_TRY(make_tmap3d(&map, buf, 64, rows_total, blocks, 64, 64 * rows_total, 64, 128));
-  const int smem = 12 * pq::A2_SLOT + 1024 + 256;
-  PQ_CUDA(cudaFuncSetAttribute(pq::tma_stream_bench_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(ctas));
-  cfg.blockDim = dim3(pq::A2_THREADS + 32);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = reinterpret_cast<cudaStream_t>(stream);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = static_cast<unsigned>(cluster);
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = cluster > 1 ? 1 : 0;
-  PQ_CUDA(cudaLaunchKernelEx(&cfg, pq::tma_stream_bench_kernel, map, nboxes, nslot, static_cast<int>(rows_total / 128), blocks, mode,
-                             static_cast<unsigned int*>(sink)));
-  return PARSEQ_OK;
+  return launch_ex(LaunchConfig(dim3(static_cast<unsigned>(ctas)), dim3(pq::A2_THREADS + 32), kTmaBenchSmem,
+                                reinterpret_cast<cudaStream_t>(stream), cluster > 1 ? static_cast<unsigned>(cluster) : 0, false),
+                   pq::tma_stream_bench_kernel, map, nboxes, nslot, static_cast<int>(rows_total / 128), blocks, mode,
+                   static_cast<unsigned int*>(sink));
 }
 
 int64_t parseq_debug_int(parseq_engine* e, const char* name) {
@@ -1988,11 +1944,14 @@ int parseq_set_option(parseq_engine* e, const char* name, int64_t value) {
   // launch options: per handle; with a NULL handle they set the process defaults used by the bare kernel exports
   // (parseq_gemm_bf16 & co.) and inherited by handles created afterwards
   LaunchOpts& lo = e ? e->lo : g_default_opts;
+  // "block_n" and "cta_group" are accepted for compatibility and ignored: the GEMM has one 128 x 128 single-CTA tile
   if (n == "block_n") {
     if (value != 0 && value != 64 && value != 128 && value != 192 && value != 256)
       return fail(PARSEQ_ERR_INVALID_ARG, "block_n: 0/64/128/192/256");
-    lo.block_n = static_cast<int>(value);
-    if (e) drop_graphs(e);
+    return PARSEQ_OK;
+  }
+  if (n == "cta_group") {
+    if (value < 0 || value > 2) return fail(PARSEQ_ERR_INVALID_ARG, "cta_group: 0 (auto) / 1 / 2");
     return PARSEQ_OK;
   }
   if (n == "attn_impl") { lo.attn_impl = value != 0 ? 1 : 0; if (e) drop_graphs(e); return PARSEQ_OK; }
@@ -2001,12 +1960,6 @@ int parseq_set_option(parseq_engine* e, const char* name, int64_t value) {
     // the MMA warpgroups release a stage once the next k-block's MMAs are queued: a ring needs at least two slots
     if (value < 0 || value == 1) return fail(PARSEQ_ERR_INVALID_ARG, "gemm_stages: 0 (full ring) or >= 2");
     lo.gemm_stages = static_cast<int>(value);
-    if (e) drop_graphs(e);
-    return PARSEQ_OK;
-  }
-  if (n == "cta_group") {
-    if (value < 0 || value > 2) return fail(PARSEQ_ERR_INVALID_ARG, "cta_group: 0 (auto) / 1 / 2");
-    lo.cta_group = static_cast<int>(value);
     if (e) drop_graphs(e);
     return PARSEQ_OK;
   }
@@ -2063,18 +2016,11 @@ int parseq_set_option(parseq_engine* e, const char* name, int64_t value) {
     drop_graphs(e);
     return PARSEQ_OK;
   }
-  if (n == "ar_kernel") {           // 0: AR loop as separate kernels, 1: grid-barrier kernel (dec_ar.cuh), 2: cluster kernel
+  if (n == "ar_kernel") {           // 0: AR loop as separate kernels, 1: grid-barrier kernel, 2: cluster kernel (ar_path)
     if (value < 0 || value > 2) return fail(PARSEQ_ERR_INVALID_ARG, "ar_kernel: 0 / 1 / 2");
-    if (value == 1 && e->C > 128)
-      return fail(PARSEQ_ERR_UNSUPPORTED, "ar_kernel = 1 (grid-barrier AR kernel) covers at most 128 head classes; "
-                                          "use ar_kernel 0 or 2");
-    if (value == 1 && e->L > 32)
-      return fail(PARSEQ_ERR_UNSUPPORTED, "ar_kernel = 1 (grid-barrier AR kernel) covers max_label_length <= 31; "
-                                          "use ar_kernel 0 or 2");
-    if (value == 1 && e->cfg.dec_depth > 1)
-      return fail(PARSEQ_ERR_UNSUPPORTED, "ar_kernel = 1 (grid-barrier AR kernel) covers dec_depth 1; use ar_kernel 0 or 2");
-    e->use_ar_kernel = value != 0;
-    e->ar_impl = value == 1 ? 1 : 2;
+    if (value == 1)
+      if (const char* why = grid_barrier_limit(e)) return fail(PARSEQ_ERR_UNSUPPORTED, why);
+    e->ar_kernel = static_cast<int>(value);
     drop_graphs(e);
     return PARSEQ_OK;
   }
@@ -2133,24 +2079,29 @@ int parseq_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, con
                      int mode, float alpha, const float* resid, int64_t ldr, int resid_mod, void* out, int64_t ldo,
                      parseq_stream_t stream) {
   if (mode < 0 || mode > 2) return fail(PARSEQ_ERR_INVALID_ARG, "bad epilogue mode");
+  PQ_TRY(ensure_kernel_attributes());
   return gemm_launch(g_default_opts, A, lda, W, ldw, bias, M, N, K, mode, alpha, resid, ldr, resid_mod, out, ldo,
                      reinterpret_cast<cudaStream_t>(stream));
 }
 int parseq_gemm_ln_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, const float* bias, int M, int D, int K,
                          float* x_inout, const float* gamma, const float* beta, float eps, void* xn_bf16,
                          parseq_stream_t stream) {
+  PQ_TRY(ensure_kernel_attributes());
   return gemm_ln_launch(g_default_opts, A, lda, W, ldw, bias, M, D, K, x_inout, gamma, beta, eps, xn_bf16, reinterpret_cast<cudaStream_t>(stream));
 }
 int parseq_mlp_ln_bf16(const void* xn, const void* W1, const float* b1, const void* W2, const float* b2, int M, int D,
                        float* x_inout, const float* gamma, const float* beta, float eps, void* xn_out_bf16, parseq_stream_t stream) {
+  PQ_TRY(ensure_kernel_attributes());
   return mlp_ln_launch(g_default_opts, xn, W1, b1, W2, b2, M, D, x_inout, gamma, beta, eps, xn_out_bf16,
                        reinterpret_cast<cudaStream_t>(stream));
 }
 int parseq_layernorm_bf16(const float* x, const float* gamma, const float* beta, float eps, int M, int D, void* y_bf16,
                           float* y_f32_or_null, parseq_stream_t stream) {
+  PQ_TRY(ensure_kernel_attributes());
   return layernorm_launch(g_default_opts, x, gamma, beta, eps, M, D, y_bf16, y_f32_or_null, reinterpret_cast<cudaStream_t>(stream));
 }
 int parseq_enc_attention(const void* qkv_bf16, int B, int T, int D, int heads, void* out_bf16, parseq_stream_t stream) {
+  PQ_TRY(ensure_kernel_attributes());
   PQ_TRY(ensure_sm_count(g_default_opts));
   return enc_attention_launch(g_default_opts, qkv_bf16, B, T, D, heads, out_bf16, reinterpret_cast<cudaStream_t>(stream));
 }

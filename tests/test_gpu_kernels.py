@@ -323,11 +323,23 @@ def test_layernorm(lib, D, eps):
     assert (y.float() == y32.bfloat16().float()).all()
 
 
-@pytest.mark.parametrize("impl", [1, 0], ids=["wgmma", "mma_sync"])
-@pytest.mark.parametrize("B,heads", [(1, 6), (5, 6), (3, 3), (2, 12), (300, 6)])
-def test_enc_attention(lib, B, heads, impl):
+@pytest.fixture
+def attn_impl(request, lib):
+    """Encoder attention: 1 = the wgmma kernel (attn_wgmma.cuh), 0 = the mma.sync kernels (kernels.cuh, the default), which
+    later tests in the same process get back."""
     from parseq_b200.engine import check
-    check(lib, lib.parseq_set_option(None, b"attn_impl", impl))
+    check(lib, lib.parseq_set_option(None, b"attn_impl", request.param))
+    yield request.param
+    check(lib, lib.parseq_set_option(None, b"attn_impl", 0))
+
+
+ATTN_IMPLS = pytest.mark.parametrize("attn_impl", [1, 0], ids=["wgmma", "mma_sync"], indirect=True)
+
+
+@ATTN_IMPLS
+@pytest.mark.parametrize("B,heads", [(1, 6), (5, 6), (3, 3), (2, 12), (300, 6)])
+def test_enc_attention(lib, B, heads, attn_impl):
+    from parseq_b200.engine import check
     T, d = 128, 64
     D = heads * d
     g = torch.Generator(device="cuda").manual_seed(B * 10 + heads)
@@ -341,17 +353,15 @@ def test_enc_attention(lib, B, heads, impl):
     o = (e.bfloat16().float() @ v) / e.sum(-1, keepdim=True)
     ref = o.permute(0, 2, 1, 3).reshape(B * T, D)
     err = (out.float() - ref).abs().max().item()
-    check(lib, lib.parseq_set_option(None, b"attn_impl", 1))
     assert err <= 2 ** -7 * ref.abs().max().item() + 1e-3, err
 
 
-@pytest.mark.parametrize("impl", [1, 0], ids=["wgmma", "mma_sync"])
+@ATTN_IMPLS
 @pytest.mark.parametrize("B,heads,T", [(2, 6, 196), (3, 12, 240), (1, 3, 130), (2, 6, 64), (40, 6, 129), (2, 6, 256), (3, 3, 49)])
-def test_enc_attention_any_token_count(lib, B, heads, T, impl):
+def test_enc_attention_any_token_count(lib, B, heads, T, attn_impl):
     """Geometries that do not fill one 128-row tile per image: the wgmma kernel with 128 or 256 keys per tile and one
     CTA per (image, head, 128-query tile), and the masked two-pass mma.sync kernel."""
     from parseq_b200.engine import check
-    check(lib, lib.parseq_set_option(None, b"attn_impl", impl))
     d = 64
     D = heads * d
     g = torch.Generator(device="cuda").manual_seed(B * 10 + heads + T)
@@ -365,5 +375,4 @@ def test_enc_attention_any_token_count(lib, B, heads, T, impl):
     o = (e.bfloat16().float() @ v) / e.sum(-1, keepdim=True)
     ref = o.permute(0, 2, 1, 3).reshape(B * T, D)
     err = (out.float() - ref).abs().max().item()
-    check(lib, lib.parseq_set_option(None, b"attn_impl", 1))
     assert err <= 2 ** -7 * ref.abs().max().item() + 1e-3, err

@@ -110,6 +110,27 @@ int parseq_forward_u8(parseq_engine* e, const parseq_forward_args* args, const u
                       float* logits, int32_t* ids, int32_t* steps, parseq_stream_t stream);
 int parseq_forward_host_u8(parseq_engine* e, const parseq_forward_args* args, const uint8_t* images_hwc_host,
                            float* logits_host, int32_t* ids_host, int32_t* steps_host, parseq_stream_t stream);
+/* Raw crops of any size: the whole reference transform (strhub/data/module.py:69-82: Image.rotate(rotation, expand=True),
+ * T.Resize(img_size, BICUBIC) of the uint8 RGB image, ToTensor, Normalize(0.5, 0.5)) runs on the device.  The resize is
+ * byte-identical to PIL's; the results are bit-identical to parseq_forward_u8 on the PIL-resized crops.  Each
+ * super-chunk of max_batch crops is resized into the engine's static uint8 input, in front of the CUDA graph.  The only
+ * device memory that grows with the crops is the staging copy of a super-chunk's bytes in the host variant. */
+typedef struct parseq_crops {
+  const uint8_t* data;     /* packed HWC RGB bytes of all crops: DEVICE (forward_crops, resize_crops) or HOST (forward_host_crops) */
+  int64_t data_bytes;
+  const int64_t* offsets;  /* HOST int64 [N]: byte offset of crop i in data */
+  const int32_t* sizes;    /* HOST int32 [N][2]: (h, w) of crop i before rotation, 1 <= h, w <= 8192 */
+  int32_t rotation;        /* 0, 90, 180, 270: PIL Image.rotate(r, expand=True), counter-clockwise */
+} parseq_crops;
+/* out_hwc: DEVICE uint8 [N, img_h, img_w, 3], what T.Resize(img_size, BICUBIC) makes of each (rotated) crop.  The
+ * metadata is checked on the host before anything is launched (PARSEQ_ERR_INVALID_ARG). */
+int parseq_resize_crops(parseq_engine* e, int32_t batch, const parseq_crops* crops, uint8_t* out_hwc, parseq_stream_t stream);
+/* parseq_forward_u8 / parseq_forward_host_u8 on the resized crops; args->batch = N.  No teacher forcing.  The host
+ * variant uploads each super-chunk's bytes on the engine's copy stream (in two halves from 256 crops up, PARSeq). */
+int parseq_forward_crops(parseq_engine* e, const parseq_forward_args* args, const parseq_crops* crops, float* logits,
+                         int32_t* ids, int32_t* steps, parseq_stream_t stream);
+int parseq_forward_host_crops(parseq_engine* e, const parseq_forward_args* args, const parseq_crops* crops,
+                              float* logits_host, int32_t* ids_host, int32_t* steps_host, parseq_stream_t stream);
 /* Fused post-processing of BaseSystem._eval_step (strhub/models/base.py:132-142) + Tokenizer._filter
  * (strhub/data/utils.py:120-129): DEVICE logits [N, num_steps, num_classes] -> ids [N, num_steps] (greedy), lengths [N]
  * (index of the first EOS, num_steps if none) and confidence [N] (product of the max softmax probabilities up to and

@@ -24,6 +24,7 @@
 #include "gemm_ln.cuh"
 #include "mlp_ln.cuh"
 #include "attn_wgmma.cuh"
+#include "crops.cuh"
 
 namespace {
 
@@ -308,6 +309,10 @@ int init_kernel_attributes() {
   PQ_TRY((gemm_attr<pq::EPI_GELU_BF16, pq::ST_REG>()));
   PQ_TRY((gemm_attr<pq::EPI_GELU_BF16, pq::ST_TMA_2D>()));
   PQ_TRY(set_smem(pq::tma_stream_bench_kernel, kTmaBenchSmem));
+  int dev = 0, optin = 0;
+  PQ_CUDA(cudaGetDevice(&dev));
+  PQ_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  PQ_TRY(set_smem(pq::crop_resize_bicubic_kernel, static_cast<size_t>(optin)));   // sized per launch by the largest crop
   return PARSEQ_OK;
 }
 
@@ -577,6 +582,13 @@ struct parseq_engine {
   // static I/O buffers the CUDA graphs are captured on
   float* in_images = nullptr; float* out_logits = nullptr; int* out_ids = nullptr; int* out_steps = nullptr;
   uint8_t* in_images_u8 = nullptr;  // static input of the uint8 HWC entry points
+  // raw-crop entry points (crops.cuh): the resize kernel's crop table [max_batch], its host copy for the current
+  // super-chunk, and the device copy of a super-chunk's packed bytes for the host entry point (grown on demand)
+  pq::CropDesc* crop_tab = nullptr;
+  std::vector<pq::CropDesc> crop_descs;
+  long long crop_base = 0;
+  uint8_t* crop_stage = nullptr;
+  long long crop_stage_bytes = 0;
   bool use_graph = true;
   struct GraphEntry { cudaGraphExec_t exec; long long kernels; };
   std::map<std::vector<int>, GraphEntry> graphs;
@@ -653,6 +665,7 @@ int alloc_workspace(parseq_engine* e) {
   const long long NB = e->max_batch;
   PQ_TRY(dev_alloc(&e->in_images, NB * 3 * e->cfg.img_h * e->cfg.img_w));
   PQ_TRY(dev_alloc(&e->in_images_u8, NB * 3 * e->cfg.img_h * e->cfg.img_w));
+  PQ_TRY(dev_alloc(&e->crop_tab, NB));
   PQ_TRY(dev_alloc(&e->out_logits, NB * e->L * e->C));
   PQ_TRY(dev_alloc(&e->out_ids, NB * e->L));
   PQ_TRY(dev_alloc(&e->out_steps, 4));
@@ -668,8 +681,8 @@ void free_workspace(parseq_engine* e) {
   drop_graphs(e);
   e->ar2_maps_ok = false;           // holds the address of the K/V cache
   void* ptrs[] = {e->a_pe, e->x, e->xn, e->qkv, e->att, e->hid, e->mem, e->ckv, e->in_images, e->out_logits, e->out_ids,
-                  e->out_steps, e->in_images_u8, e->ar_sa, e->ar_ca, e->ar_hd, e->ar_y, e->ar_qc, e->ar_part, e->ar_ids, e->ar_bar, e->ar_prof};
-  e->ar_part = nullptr; e->ar_prof = nullptr; e->in_images_u8 = nullptr;
+                  e->out_steps, e->in_images_u8, e->crop_tab, e->ar_sa, e->ar_ca, e->ar_hd, e->ar_y, e->ar_qc, e->ar_part, e->ar_ids, e->ar_bar, e->ar_prof};
+  e->ar_part = nullptr; e->ar_prof = nullptr; e->in_images_u8 = nullptr; e->crop_tab = nullptr;
   if (e->vt_rows) { cudaFree(e->vt_rows); e->vt_rows = nullptr; }
   e->ar_sa = e->ar_ca = e->ar_hd = nullptr; e->ar_y = e->ar_qc = nullptr; e->ar_ids = nullptr; e->ar_bar = nullptr;
   for (void* p : ptrs)
@@ -1409,9 +1422,146 @@ int run_graph(parseq_engine* e, const parseq_forward_args* a, int Bc, int L, boo
   return PARSEQ_OK;
 }
 
+// ---------------------------------------------------------------- raw crops of any size (crops.cuh)
+// The crops of one parseq_forward_crops / parseq_forward_host_crops / parseq_resize_crops call, metadata validated.
+struct CropBatch {
+  const parseq_crops* c;
+  bool host;                        // c->data is host memory: each super-chunk's bytes are staged in e->crop_stage
+};
+
+// The crop metadata, on the host alone (no handle or device needed).  These checks, and check_crop_smem, run before
+// the first launch of a call: on failure nothing is enqueued.
+int check_crops(int batch, const parseq_crops* c) {
+  if (c == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  if (batch == 0) return PARSEQ_OK;
+  if (c->data == nullptr || c->offsets == nullptr || c->sizes == nullptr)
+    return fail(PARSEQ_ERR_INVALID_ARG, "null crop data, offsets or sizes");
+  if (c->rotation != 0 && c->rotation != 90 && c->rotation != 180 && c->rotation != 270)
+    return fail(PARSEQ_ERR_INVALID_ARG, "rotation must be 0, 90, 180 or 270");
+  for (int i = 0; i < batch; ++i) {
+    const int h = c->sizes[2 * i], w = c->sizes[2 * i + 1];
+    if (h < 1 || w < 1 || h > pq::CROP_MAX_SIDE || w > pq::CROP_MAX_SIDE)
+      return fail(PARSEQ_ERR_INVALID_ARG, "crop " + std::to_string(i) + ": size " + std::to_string(h) + " x " +
+                                              std::to_string(w) + ", sides must be in [1, 8192]");
+    if (c->offsets[i] < 0 || c->offsets[i] > c->data_bytes - 3ll * h * w)
+      return fail(PARSEQ_ERR_INVALID_ARG, "crop " + std::to_string(i) + ": offset + 3 h w exceeds data_bytes");
+  }
+  return PARSEQ_OK;
+}
+
+// The resize kernel's coefficient tables of every crop fit in shared memory (always at img_size 32 x 128 and 224 x 224).
+int check_crop_smem(const parseq_engine* e, int batch, const parseq_crops* c) {
+  int optin = 0;
+  PQ_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, e->cfg.device));
+  const bool turn = c->rotation == 90 || c->rotation == 270;
+  for (int i = 0; i < batch; ++i) {
+    const int h = c->sizes[2 * i], w = c->sizes[2 * i + 1];
+    if (4ll * pq::crop_smem_ints(turn ? w : h, turn ? h : w, e->cfg.img_h, e->cfg.img_w) > optin)
+      return fail(PARSEQ_ERR_UNSUPPORTED, "crop " + std::to_string(i) + ": resize tables exceed shared memory at this img_size");
+  }
+  return PARSEQ_OK;
+}
+
+// Crop i as the kernel reads it, rotated counter-clockwise by c->rotation (np.rot90(crop, rotation / 90)), its bytes
+// at data + offsets[i] - base.
+pq::CropDesc crop_desc(const parseq_crops* c, int i, long long base) {
+  const int h = c->sizes[2 * i], w = c->sizes[2 * i + 1], row = 3 * w;
+  const long long o = c->offsets[i] - base;
+  switch (c->rotation) {
+    case 90: return pq::CropDesc{o + 3ll * (w - 1), -3, row, w, h};
+    case 180: return pq::CropDesc{o + 1ll * row * (h - 1) + 3ll * (w - 1), -row, -3, h, w};
+    case 270: return pq::CropDesc{o + 1ll * row * (h - 1), 3, -row, w, h};
+    default: return pq::CropDesc{o, row, 3, h, w};
+  }
+}
+
+// Bytes [lo, hi) of data that crops [i0, i1) occupy.
+void crop_range(const parseq_crops* c, int i0, int i1, long long* lo, long long* hi) {
+  *lo = c->offsets[i0];
+  *hi = 0;
+  for (int i = i0; i < i1; ++i) {
+    const long long o = c->offsets[i];
+    *lo = o < *lo ? o : *lo;
+    const long long end = o + 3ll * c->sizes[2 * i] * c->sizes[2 * i + 1];
+    *hi = end > *hi ? end : *hi;
+  }
+}
+
+// Host crops: grows the staging buffer to the largest super-chunk of the call, before anything of the call is enqueued.
+int crops_reserve(parseq_engine* e, const CropBatch& cb, int batch) {
+  if (!cb.host) return PARSEQ_OK;
+  long long need = 0;
+  for (int b0 = 0; b0 < batch; b0 += e->max_batch) {
+    long long lo, hi;
+    crop_range(cb.c, b0, (batch - b0 < e->max_batch) ? batch : b0 + e->max_batch, &lo, &hi);
+    need = hi - lo > need ? hi - lo : need;
+  }
+  if (need <= e->crop_stage_bytes) return PARSEQ_OK;
+  PQ_CUDA(cudaStreamSynchronize(e->main));
+  PQ_CUDA(cudaStreamSynchronize(e->copy));
+  if (e->crop_stage) cudaFree(e->crop_stage);
+  e->crop_stage = nullptr;
+  e->crop_stage_bytes = 0;
+  PQ_TRY(dev_alloc(&e->crop_stage, need));
+  e->crop_stage_bytes = need;
+  return PARSEQ_OK;
+}
+
+// Uploads the crop table of super-chunk [b0, b0 + Bc) on `st`.
+int crops_table(parseq_engine* e, const CropBatch& cb, int b0, int Bc, cudaStream_t st) {
+  long long lo = 0, hi = 0;
+  if (cb.host) crop_range(cb.c, b0, b0 + Bc, &lo, &hi);
+  e->crop_base = lo;
+  e->crop_descs.resize(static_cast<size_t>(Bc));
+  for (int i = 0; i < Bc; ++i) e->crop_descs[static_cast<size_t>(i)] = crop_desc(cb.c, b0 + i, lo);
+  // pageable source: the call returns once the table is staged, so crop_descs may change afterwards
+  PQ_CUDA(cudaMemcpyAsync(e->crop_tab, e->crop_descs.data(), sizeof(pq::CropDesc) * Bc, cudaMemcpyHostToDevice, st));
+  return PARSEQ_OK;
+}
+
+// Crops [b0 + i0, b0 + i1) of the super-chunk whose table is uploaded -> out [i1 - i0, img_h, img_w, 3] on `st` (host
+// crops: their bytes are uploaded first, on the same stream).
+int crops_resize(parseq_engine* e, const CropBatch& cb, int b0, int i0, int i1, uint8_t* out, cudaStream_t st) {
+  const uint8_t* data = cb.c->data;
+  if (cb.host) {
+    long long lo, hi;
+    crop_range(cb.c, b0 + i0, b0 + i1, &lo, &hi);
+    PQ_CUDA(cudaMemcpyAsync(e->crop_stage + (lo - e->crop_base), data + lo, static_cast<size_t>(hi - lo), cudaMemcpyHostToDevice, st));
+    data = e->crop_stage;
+  }
+  const int H = e->cfg.img_h, W = e->cfg.img_w;
+  int smem = 0;
+  for (int i = i0; i < i1; ++i) {
+    const pq::CropDesc& d = e->crop_descs[static_cast<size_t>(i)];
+    const int s = 4 * pq::crop_smem_ints(d.h, d.w, H, W);
+    smem = s > smem ? s : smem;
+  }
+  const int lines = H > W ? H : W;          // second-pass lines: out_h, or out_w for tall crops
+  const dim3 grid((lines + pq::CROP_BAND - 1) / pq::CROP_BAND, i1 - i0);
+  TimedScope ts(e, st, CAT_MISC, 0.0);
+  // no PDL: the kernel reads what the copies and the previous forward left behind
+  return launch_ex(LaunchConfig(grid, dim3(pq::CROP_THREADS), static_cast<size_t>(smem), st, 0, false),
+                   pq::crop_resize_bicubic_kernel, data, static_cast<const pq::CropDesc*>(e->crop_tab + i0), H, W,
+                   out + 3ll * H * W * i0);
+}
+
+// Shared checks of the forward entry points of raw crops; teacher forcing is a float-input debug feature.
+int check_crops_call(parseq_engine* e, const parseq_forward_args* a, const parseq_crops* crops, const float* logits) {
+  if (a == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  if (a->batch < 0 || a->refine_iters < 0) return fail(PARSEQ_ERR_INVALID_ARG, "negative batch / refine_iters");
+  if (a->forced_ids != nullptr || a->forced_refine != nullptr)
+    return fail(PARSEQ_ERR_INVALID_ARG, "teacher forcing is a device-pointer API (parseq_forward)");
+  PQ_TRY(check_crops(a->batch, crops));
+  if (e == nullptr || logits == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
+  if (!e->finalized) return fail(PARSEQ_ERR_STATE, "parseq_finalize has not been called after the last weight update");
+  return check_crop_smem(e, a->batch, crops);
+}
+
 // Common driver of parseq_forward / parseq_forward_host. `host` selects H2D/D2H vs D2D staging copies.
+// `crops` (raw crops of any size, u8): each super-chunk is resized into the static uint8 input in place of the copy.
 int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* images_any, float* logits, int32_t* ids,
-                 int32_t* steps, cudaStream_t user, bool host, bool u8 = false) {
+                 int32_t* steps, cudaStream_t user, bool host, bool u8 = false, const CropBatch* crops = nullptr) {
   const int L = num_steps_of(e, a->max_length);
   const bool testing = a->max_length < 0;
   const long long img_sz = 3ll * e->cfg.img_h * e->cfg.img_w * (u8 ? 1 : 4);   // bytes per image
@@ -1429,7 +1579,14 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
   for (int b0 = 0; b0 < a->batch; b0 += e->max_batch) {
     const int Bc = (a->batch - b0 < e->max_batch) ? (a->batch - b0) : e->max_batch;
     if (eager && !host) {
-      PQ_TRY(forward_super(e, a, b0, Bc, L, images + b0 * img_sz, u8, logits + 1ll * b0 * L * e->C,
+      const char* in = reinterpret_cast<const char*>(e->in_images_u8);
+      if (crops) {
+        PQ_TRY(crops_table(e, *crops, b0, Bc, e->main));
+        PQ_TRY(crops_resize(e, *crops, b0, 0, Bc, e->in_images_u8, e->main));
+      } else {
+        in = images + b0 * img_sz;
+      }
+      PQ_TRY(forward_super(e, a, b0, Bc, L, in, u8, logits + 1ll * b0 * L * e->C,
                            ids ? ids + 1ll * b0 * L : nullptr, e->out_steps));
       continue;
     }
@@ -1438,10 +1595,19 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
       const int split = ((Bc / 2 + 7) / 8) * 8;
       PQ_CUDA(cudaEventRecord(e->ev_c[2], e->main));                       // previous work on `main` (and the caller's stream)
       PQ_CUDA(cudaStreamWaitEvent(e->copy, e->ev_c[2], 0));
-      PQ_CUDA(cudaMemcpyAsync(in_static, images + b0 * img_sz, static_cast<size_t>(split * img_sz), kin, e->copy));
+      if (crops) {
+        PQ_TRY(crops_table(e, *crops, b0, Bc, e->copy));
+        PQ_TRY(crops_resize(e, *crops, b0, 0, split, e->in_images_u8, e->copy));
+      } else {
+        PQ_CUDA(cudaMemcpyAsync(in_static, images + b0 * img_sz, static_cast<size_t>(split * img_sz), kin, e->copy));
+      }
       PQ_CUDA(cudaEventRecord(e->ev_c[0], e->copy));
-      PQ_CUDA(cudaMemcpyAsync(static_cast<char*>(in_static) + split * img_sz, images + (b0 + split) * img_sz,
-                              static_cast<size_t>((Bc - split) * img_sz), kin, e->copy));
+      if (crops) {
+        PQ_TRY(crops_resize(e, *crops, b0, split, Bc, e->in_images_u8, e->copy));
+      } else {
+        PQ_CUDA(cudaMemcpyAsync(static_cast<char*>(in_static) + split * img_sz, images + (b0 + split) * img_sz,
+                                static_cast<size_t>((Bc - split) * img_sz), kin, e->copy));
+      }
       PQ_CUDA(cudaEventRecord(e->ev_c[1], e->copy));
       PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_c[0], 0));
       PQ_TRY(run_graph(e, a, Bc, L, u8, 1, split));
@@ -1452,7 +1618,12 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
       if (ids) PQ_CUDA(cudaMemcpyAsync(ids + 1ll * b0 * L, e->out_ids, static_cast<size_t>(1ll * Bc * L) * 4, kout, e->main));
       continue;
     }
-    PQ_CUDA(cudaMemcpyAsync(in_static, images + b0 * img_sz, static_cast<size_t>(Bc * img_sz), kin, e->main));
+    if (crops) {
+      PQ_TRY(crops_table(e, *crops, b0, Bc, e->main));
+      PQ_TRY(crops_resize(e, *crops, b0, 0, Bc, e->in_images_u8, e->main));
+    } else {
+      PQ_CUDA(cudaMemcpyAsync(in_static, images + b0 * img_sz, static_cast<size_t>(Bc * img_sz), kin, e->main));
+    }
     if (eager) {
       PQ_TRY(forward_super(e, a, b0, Bc, L, in_static, u8, e->out_logits, e->out_ids, e->out_steps));
     } else {
@@ -1632,6 +1803,7 @@ void parseq_destroy(parseq_engine* e) {
     if (s.dev) cudaFree(s.dev);
   if (e->kvtab) cudaFree(e->kvtab);
   if (e->qs) cudaFree(e->qs);
+  if (e->crop_stage) cudaFree(e->crop_stage);
   free_workspace(e);
   if (e->main) cudaStreamDestroy(e->main);
   if (e->copy) cudaStreamDestroy(e->copy);
@@ -1773,6 +1945,49 @@ int parseq_forward_host_u8(parseq_engine* e, const parseq_forward_args* a, const
     return fail(PARSEQ_ERR_INVALID_ARG, "teacher forcing is a device-pointer API (parseq_forward)");
   PQ_CUDA(cudaSetDevice(e->cfg.device));
   PQ_TRY(forward_impl(e, a, images_hwc_host, logits_host, ids_host, steps_host, reinterpret_cast<cudaStream_t>(stream), true, true));
+  PQ_CUDA(cudaStreamSynchronize(e->main));
+  return PARSEQ_OK;
+}
+
+int parseq_resize_crops(parseq_engine* e, int32_t batch, const parseq_crops* crops, uint8_t* out_hwc, parseq_stream_t stream) {
+  if (batch < 0) return fail(PARSEQ_ERR_INVALID_ARG, "negative batch");
+  PQ_TRY(check_crops(batch, crops));
+  if (e == nullptr || out_hwc == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
+  PQ_TRY(check_crop_smem(e, batch, crops));
+  if (batch == 0) return PARSEQ_OK;
+  PQ_CUDA(cudaSetDevice(e->cfg.device));
+  cudaStream_t user = reinterpret_cast<cudaStream_t>(stream);
+  const CropBatch cb{crops, false};
+  PQ_CUDA(cudaEventRecord(e->ev_in, user));
+  PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_in, 0));
+  for (int b0 = 0; b0 < batch; b0 += e->max_batch) {
+    const int Bc = (batch - b0 < e->max_batch) ? (batch - b0) : e->max_batch;
+    PQ_TRY(crops_table(e, cb, b0, Bc, e->main));
+    PQ_TRY(crops_resize(e, cb, b0, 0, Bc, out_hwc + 3ll * e->cfg.img_h * e->cfg.img_w * b0, e->main));
+  }
+  PQ_CUDA(cudaEventRecord(e->ev_out, e->main));
+  PQ_CUDA(cudaStreamWaitEvent(user, e->ev_out, 0));
+  return PARSEQ_OK;
+}
+
+int parseq_forward_crops(parseq_engine* e, const parseq_forward_args* a, const parseq_crops* crops, float* logits, int32_t* ids,
+                         int32_t* steps, parseq_stream_t stream) {
+  PQ_TRY(check_crops_call(e, a, crops, logits));
+  if (a->batch == 0) return PARSEQ_OK;
+  PQ_CUDA(cudaSetDevice(e->cfg.device));
+  const CropBatch cb{crops, false};
+  return forward_impl(e, a, nullptr, logits, ids, steps, reinterpret_cast<cudaStream_t>(stream), false, true, &cb);
+}
+
+int parseq_forward_host_crops(parseq_engine* e, const parseq_forward_args* a, const parseq_crops* crops, float* logits_host,
+                              int32_t* ids_host, int32_t* steps_host, parseq_stream_t stream) {
+  PQ_TRY(check_crops_call(e, a, crops, logits_host));
+  if (a->batch == 0) return PARSEQ_OK;
+  PQ_CUDA(cudaSetDevice(e->cfg.device));
+  const CropBatch cb{crops, true};
+  PQ_TRY(crops_reserve(e, cb, a->batch));
+  PQ_TRY(forward_impl(e, a, nullptr, logits_host, ids_host, steps_host, reinterpret_cast<cudaStream_t>(stream), true, true, &cb));
   PQ_CUDA(cudaStreamSynchronize(e->main));
   return PARSEQ_OK;
 }

@@ -23,9 +23,15 @@ class ForwardArgsC(C.Structure):
                 ("refine_iters", C.c_int32), ("forced_ids", C.c_void_p), ("forced_refine", C.c_void_p)]
 
 
+class CropsC(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("data_bytes", C.c_int64), ("offsets", C.c_void_p), ("sizes", C.c_void_p),
+                ("rotation", C.c_int32)]
+
+
 EXPORTS = [
     "parseq_create", "parseq_destroy", "parseq_set_weight", "parseq_num_weights", "parseq_weight_key",
     "parseq_finalize", "parseq_forward", "parseq_forward_host", "parseq_forward_u8", "parseq_forward_host_u8",
+    "parseq_resize_crops", "parseq_forward_crops", "parseq_forward_host_crops",
     "parseq_postprocess", "parseq_encode", "parseq_decode", "parseq_decode_ex", "parseq_head", "parseq_text_embed", "parseq_kernel_launches", "parseq_debug_int", "parseq_bench_tma_stream",
     "parseq_set_option", "parseq_get_timing", "parseq_get_ar_profile", "parseq_last_error", "parseq_version", "parseq_gemm_bf16", "parseq_gemm_ln_bf16", "parseq_mlp_ln_bf16", "parseq_layernorm_bf16",
     "parseq_enc_attention",
@@ -61,6 +67,10 @@ def load_library(path: Optional[str] = None):
     lib.parseq_forward_host.argtypes = lib.parseq_forward.argtypes
     lib.parseq_forward_u8.argtypes = lib.parseq_forward.argtypes
     lib.parseq_forward_host_u8.argtypes = lib.parseq_forward.argtypes
+    lib.parseq_resize_crops.argtypes = [C.c_void_p, C.c_int32, C.POINTER(CropsC), C.c_void_p, C.c_void_p]
+    lib.parseq_forward_crops.argtypes = [C.c_void_p, C.POINTER(ForwardArgsC), C.POINTER(CropsC), C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p]
+    lib.parseq_forward_host_crops.argtypes = lib.parseq_forward_crops.argtypes
     lib.parseq_postprocess.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p]
     lib.parseq_encode.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -197,6 +207,15 @@ class Engine:
         a = self._args(batch, max_length, decode_ar, refine_iters)
         fn = self.lib.parseq_forward_host_u8 if host else self.lib.parseq_forward_u8
         check(self.lib, fn(self.handle, C.byref(a), images_ptr, logits_ptr, ids_ptr, steps_ptr, stream))
+
+    def resize_crops(self, crops: CropsC, batch, out_ptr, stream):
+        check(self.lib, self.lib.parseq_resize_crops(self.handle, batch, C.byref(crops), out_ptr, stream))
+
+    def forward_crops(self, crops: CropsC, batch, logits_ptr, ids_ptr, steps_ptr, stream, max_length=None, decode_ar=True,
+                      refine_iters=1, host=False):
+        a = self._args(batch, max_length, decode_ar, refine_iters)
+        fn = self.lib.parseq_forward_host_crops if host else self.lib.parseq_forward_crops
+        check(self.lib, fn(self.handle, C.byref(a), C.byref(crops), logits_ptr, ids_ptr, steps_ptr, stream))
 
     def postprocess(self, logits_ptr, batch, num_steps, ids_ptr, lengths_ptr, conf_ptr, stream, eos_id=0):
         check(self.lib, self.lib.parseq_postprocess(logits_ptr, batch, num_steps, self.cfg.num_classes, eos_id, ids_ptr,

@@ -14,13 +14,13 @@ from __future__ import annotations
 import math
 from dataclasses import dataclass
 from types import SimpleNamespace
-from typing import Any, Dict, Optional, Sequence
+from typing import Any, Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 from torch import Tensor, nn
 
 from .config import ParseqConfig, make_config
-from .engine import Engine, EngineError
+from .engine import CropsC, Engine, EngineError
 from .tokenizer import CharsetAdapter, Tokenizer
 
 
@@ -52,6 +52,57 @@ def edit_distance(a: str, b: str) -> int:
             cur.append(min(prev[j] + 1, cur[j - 1] + 1, prev[j - 1] + (ca != cb)))
         prev = cur
     return prev[-1]
+
+
+def _crop_tensor(c) -> Tensor:
+    """A raw crop as a uint8 [h, w, 3] tensor: a tensor as given, or the pixels of a PIL image in mode RGB."""
+    if isinstance(c, Tensor):
+        if c.dtype != torch.uint8:
+            raise TypeError(f"a crop must be a uint8 tensor, got {c.dtype}")
+        if c.dim() != 3 or c.shape[2] != 3:
+            raise ValueError(f"a crop must be [h, w, 3] (HWC RGB), got {tuple(c.shape)}")
+        return c
+    try:
+        from PIL import Image
+    except ImportError:             # pragma: no cover
+        Image = None
+    if Image is not None and isinstance(c, Image.Image):
+        if c.mode != "RGB":
+            raise ValueError(f"a PIL crop must be in mode RGB, got {c.mode} (convert it, as read.py does)")
+        import numpy as np
+        return torch.from_numpy(np.asarray(c).copy())
+    raise TypeError(f"a crop must be a uint8 [h, w, 3] tensor or a PIL image, got {type(c).__name__}")
+
+
+def pack_crops(crops: Sequence[Any], pin_memory: bool = False) -> Tuple[Tensor, Tensor, Tensor]:
+    """Packs a list of raw crops of any size for the engine's crop entry points: (data, offsets, sizes), with data the
+    crops' HWC bytes back to back on the crops' device (pinned if asked, for CPU crops), offsets int64 [N] and sizes
+    int32 [N, 2] = (h, w) on the CPU.  All crops must be on one device; PIL images count as CPU crops."""
+    if not isinstance(crops, (list, tuple)):
+        raise TypeError("crops must be a list of uint8 [h, w, 3] tensors or PIL images")
+    if len(crops) == 0:
+        raise ValueError("empty crop list")
+    ts = [_crop_tensor(c) for c in crops]
+    devs = {t.device for t in ts}
+    if len(devs) != 1:
+        raise ValueError(f"all crops must be on one device, got {sorted(str(d) for d in devs)}")
+    sizes = torch.tensor([[t.shape[0], t.shape[1]] for t in ts], dtype=torch.int32)
+    nbytes = sizes[:, 0].to(torch.int64) * sizes[:, 1].to(torch.int64) * 3
+    offsets = torch.zeros(len(ts), dtype=torch.int64)
+    if len(ts) > 1:
+        offsets[1:] = torch.cumsum(nbytes, 0)[:-1]
+    dev = ts[0].device
+    if dev.type == "cuda":
+        data = torch.cat([t.reshape(-1) for t in ts])
+    else:
+        data = torch.empty(int(nbytes.sum()), dtype=torch.uint8, pin_memory=pin_memory)
+        for t, o, n in zip(ts, offsets.tolist(), nbytes.tolist()):
+            data[o:o + n].copy_(t.reshape(-1))
+    return data, offsets, sizes
+
+
+def _crops_c(data: Tensor, offsets: Tensor, sizes: Tensor, rotation: int) -> CropsC:
+    return CropsC(data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), int(rotation))
 
 
 class _Holder(nn.Module):
@@ -190,7 +241,48 @@ class _EngineModule(nn.Module):
         eng.encode(img.data_ptr(), img.shape[0], mem.data_ptr(), torch.cuda.current_stream(img.device).cuda_stream)
         return mem
 
-    def _run(self, images: Tensor, max_length, decode_ar, refine_iters, forced_ids=None, forced_refine=None):
+    def preprocess(self, crops: Sequence[Any], rotation: int = 0) -> Tensor:
+        """CUDA uint8 [N, H, W, 3]: each crop rotated by `rotation` (counter-clockwise) and resized to img_size on the
+        device, byte-identical to the reference's Image.rotate(rotation, expand=True) + T.Resize(img_size, BICUBIC)."""
+        eng = self.engine()
+        dev = self._device
+        data, offsets, sizes = pack_crops(crops, pin_memory=True)
+        if data.device.type == "cuda" and data.device != dev:
+            raise ValueError(f"crops are on {data.device}, the model on {dev}")
+        data = data.to(dev, non_blocking=True)
+        H, W = self.cfg.img_size
+        out = torch.empty((len(crops), H, W, 3), dtype=torch.uint8, device=dev)
+        eng.resize_crops(_crops_c(data, offsets, sizes, rotation), len(crops), out.data_ptr(),
+                         torch.cuda.current_stream(dev).cuda_stream)
+        return out
+
+    def _run_crops(self, crops, max_length, decode_ar, refine_iters, rotation):
+        """Raw crops of any size: CUDA crops run parseq_forward_crops and return CUDA tensors; CPU crops and PIL images
+        run parseq_forward_host_crops (pinned upload, host outputs) and return CPU tensors."""
+        eng = self.engine()
+        dev = self._device
+        data, offsets, sizes = pack_crops(crops, pin_memory=True)
+        host = data.device.type != "cuda"
+        if not host and data.device != dev:
+            raise ValueError(f"crops are on {data.device}, the model on {dev}")
+        N = len(crops)
+        L = eng.num_steps(max_length)
+        out_dev = torch.device("cpu") if host else dev
+        logits = torch.empty((N, L, self.cfg.num_classes), dtype=torch.float32, device=out_dev, pin_memory=host)
+        ids = torch.empty((N, L), dtype=torch.int32, device=out_dev, pin_memory=host)
+        steps = torch.empty((1,), dtype=torch.int32, device=out_dev, pin_memory=host)
+        eng.forward_crops(_crops_c(data, offsets, sizes, rotation), N, logits.data_ptr(), ids.data_ptr(), steps.data_ptr(),
+                          torch.cuda.current_stream(dev).cuda_stream, max_length, decode_ar, refine_iters, host=host)
+        return logits, ids, steps
+
+    def _run(self, images: Union[Tensor, List[Any]], max_length, decode_ar, refine_iters, forced_ids=None,
+             forced_refine=None, rotation: int = 0):
+        if isinstance(images, (list, tuple)):
+            if forced_ids is not None or forced_refine is not None:
+                raise ValueError("teacher forcing takes normalised float images")
+            return self._run_crops(images, max_length, decode_ar, refine_iters, rotation)
+        if rotation:
+            raise ValueError("rotation applies to lists of raw crops; a tensor input is already at img_size")
         eng = self.engine()
         images = self._check_images(images)
         dev = images.device
@@ -269,10 +361,14 @@ class ParseqModel(_EngineModule):
                    torch.cuda.current_stream(dev).cuda_stream, cm.data_ptr() if cm is not None else None)
         return out
 
-    def forward(self, tokenizer: Tokenizer, images: Tensor, max_length: Optional[int] = None,
+    def forward(self, tokenizer: Tokenizer, images: Union[Tensor, List[Any]], max_length: Optional[int] = None,
                 return_ids: bool = False, forced_ids: Optional[Tensor] = None,
-                forced_refine: Optional[Tensor] = None):
-        logits, ids, steps = self._run(images, max_length, self.decode_ar, self.refine_iters, forced_ids, forced_refine)
+                forced_refine: Optional[Tensor] = None, *, rotation: int = 0):
+        """`images`: normalised float [N, 3, H, W], uint8 [N, H, W, 3] at img_size, or a list of raw crops of any size
+        (uint8 [h, w, 3] tensors, all CUDA or all CPU, or PIL images in mode RGB) that the engine rotates by `rotation`
+        and resizes as the reference's test transform does."""
+        logits, ids, steps = self._run(images, max_length, self.decode_ar, self.refine_iters, forced_ids, forced_refine,
+                                       rotation)
         if max_length is None and self.decode_ar and not self.refine_iters:
             # model.py:144-147: with no refinement the reference returns only the S steps it ran
             S = int(steps.item())
@@ -289,9 +385,11 @@ class VitstrModel(_EngineModule):
     def forward_features(self, x: Tensor) -> Tensor:
         return self._features(x)
 
-    def forward_tokens(self, images: Tensor, max_length: Optional[int] = None, return_ids: bool = False):
-        """`self.forward(images, max_length + 2)[:, 1:]` (vitstr/system.py:65-71) in one engine call."""
-        logits, ids, _ = self._run(images, max_length, False, 0)
+    def forward_tokens(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, return_ids: bool = False,
+                       *, rotation: int = 0):
+        """`self.forward(images, max_length + 2)[:, 1:]` (vitstr/system.py:65-71) in one engine call; `images` as in
+        ParseqModel.forward."""
+        logits, ids, _ = self._run(images, max_length, False, 0, rotation=rotation)
         return (logits, ids) if return_ids else logits
 
     def forward(self, x: Tensor, seqlen: int = 25) -> Tensor:
@@ -323,6 +421,11 @@ class _System(nn.Module):
     @property
     def device(self) -> torch.device:
         return self.model._device
+
+    def preprocess(self, crops: Sequence[Any], rotation: int = 0) -> Tensor:
+        """The reference's test transform up to the uint8 image (module.py:69-82: rotate, T.Resize(img_size, BICUBIC)) of
+        a list of raw crops, on the device: CUDA uint8 [N, H, W, 3], what `forward` takes as a tensor."""
+        return self.model.preprocess(crops, rotation)
 
     def postprocess(self, logits: Tensor):
         """Device-side greedy decode of logits [N, L, C]: (labels, confidences) with the semantics of
@@ -401,8 +504,9 @@ class PARSeq(_System):
         except EngineError as e:  # pragma: no cover
             raise InvalidModelError(str(e)) from e
 
-    def forward(self, images: Tensor, max_length: Optional[int] = None) -> Tensor:
-        return self.model.forward(self.tokenizer, images, max_length)
+    def forward(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *, rotation: int = 0) -> Tensor:
+        """`images`: a tensor, as the reference takes, or a list of raw crops of any size (ParseqModel.forward)."""
+        return self.model.forward(self.tokenizer, images, max_length, rotation=rotation)
 
 
 class ViTSTR(_System):
@@ -430,8 +534,8 @@ class ViTSTR(_System):
         except EngineError as e:  # pragma: no cover
             raise InvalidModelError(str(e)) from e
 
-    def forward(self, images: Tensor, max_length: Optional[int] = None) -> Tensor:
-        return self.model.forward_tokens(images, max_length)
+    def forward(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *, rotation: int = 0) -> Tensor:
+        return self.model.forward_tokens(images, max_length, rotation=rotation)
 
     @classmethod
     def load_from_checkpoint(cls, checkpoint_path: str, map_location="cpu", **kwargs):

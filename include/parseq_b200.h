@@ -228,6 +228,12 @@ int parseq_layernorm_bf16(const float* x, const float* gamma, const float* beta,
 /* out[B*T, D] = softmax(QK^T/sqrt(64)) V per (image, head) from packed qkv bf16 [B*T, 3D]. */
 int parseq_enc_attention(const void* qkv_bf16, int B, int T, int D, int heads, void* out_bf16,
                          parseq_stream_t stream);
+/* The QKV projection and the attention core in one kernel: out[B*T, D] = softmax(QK^T/sqrt(64)) V per (image, head) with
+ * [Q | K | V] = bf16(xn[B*T, D] * W_qkv[3D, D]^T + b_qkv) (b_qkv may be NULL); qkv never leaves the SM.  Bit-identical to
+ * parseq_gemm_bf16 (mode 1) followed by parseq_enc_attention.  T = 128, D = 64 * heads in {192, 384}; anything else
+ * returns PARSEQ_ERR_UNSUPPORTED. */
+int parseq_qkv_attention_bf16(const void* xn_bf16, const void* W_qkv, const float* b_qkv, int B, int T, int D,
+                              int heads, void* out_bf16, parseq_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -24,6 +24,7 @@
 #include "gemm_ln.cuh"
 #include "mlp_ln.cuh"
 #include "attn_wgmma.cuh"
+#include "qkv_attn.cuh"
 #include "crops.cuh"
 
 namespace {
@@ -277,6 +278,8 @@ template <int D, int CG>
 int mlp_ln_attr() { return set_smem(pq::mlp_ln_fused_kernel<D, CG>, pq::MlpLnCfg<D, CG>::kSmemBytes); }
 template <int NK>
 int attn_wgmma_attr() { return set_smem(pq::enc_attention_wgmma_kernel<NK>, pq::atw_smem_bytes<NK>()); }
+template <int D>
+int qkv_attn_attr() { return set_smem(pq::enc_qkv_attn_kernel<D>, pq::QkvAttnCfg::kSmemBytes); }
 template <int EPI, int STORE>
 int gemm_attr() { return set_smem(pq::gemm_bf16_wgmma_kernel<EPI, STORE>, pq::GemmCfg::smem_bytes<STORE != pq::ST_REG>()); }
 constexpr int kTmaBenchSmem = 12 * pq::A2_SLOT + 1024 + 256;
@@ -301,6 +304,7 @@ int init_kernel_attributes() {
   PQ_TRY((gemm_ln_attr<384, 1>())); PQ_TRY((gemm_ln_attr<384, 2>()));
   PQ_TRY((mlp_ln_attr<192, 1>())); PQ_TRY((mlp_ln_attr<384, 1>())); PQ_TRY((mlp_ln_attr<192, 2>())); PQ_TRY((mlp_ln_attr<384, 2>()));
   PQ_TRY((attn_wgmma_attr<128>())); PQ_TRY((attn_wgmma_attr<256>()));
+  PQ_TRY((qkv_attn_attr<192>())); PQ_TRY((qkv_attn_attr<384>()));
   PQ_TRY((gemm_attr<pq::EPI_F32, pq::ST_REG>()));
   PQ_TRY((gemm_attr<pq::EPI_F32_RESID, pq::ST_REG>()));
   PQ_TRY((gemm_attr<pq::EPI_BF16, pq::ST_REG>()));
@@ -499,6 +503,27 @@ int enc_attention_launch(const LaunchOpts& lo, const void* qkv, int B, int T, in
   }
   return launch_k(lo, pq::enc_attention_kernel, dim3(B * heads), dim3(256), 0, st,
                   reinterpret_cast<const __nv_bfloat16*>(qkv), reinterpret_cast<__nv_bfloat16*>(out), D, heads);
+}
+
+// out[B*T, D] = attention(bf16(xn W_qkv^T + b_qkv)) in one kernel (qkv_attn.cuh): T = 128, head_dim 64, D in {192, 384}.
+// Bit-identical to the QKV gemm (EPI_BF16) followed by enc_attention_launch with attn_impl = 0.
+bool qkv_attn_supported(int T, int D, int heads) { return T == pq::ATT_T && D == heads * pq::ATT_DH && (D == 192 || D == 384); }
+int qkv_attn_launch(LaunchOpts& lo, const void* xn, const void* W, const float* bias, int B, int T, int D, int heads, void* out,
+                    cudaStream_t st) {
+  if (B <= 0) return fail(PARSEQ_ERR_INVALID_ARG, "qkv_attn: empty batch");
+  if (!qkv_attn_supported(T, D, heads))
+    return fail(PARSEQ_ERR_UNSUPPORTED, "qkv_attn: T = 128, head_dim 64 and embed_dim 192 or 384 only");
+  if ((reinterpret_cast<uintptr_t>(out) & 15u) != 0) return fail(PARSEQ_ERR_INVALID_ARG, "qkv_attn: out must be 16-byte aligned");
+  PQ_TRY(ensure_sm_count(lo));
+  CUtensorMap tx, tw;
+  PQ_TRY(make_tmap(&tx, xn, 2, static_cast<long long>(B) * T, D, D, pq::GEMM_BLOCK_K, pq::ATT_T));
+  PQ_TRY(make_tmap(&tw, W, 2, 3 * D, D, D, pq::GEMM_BLOCK_K, pq::ATT_DH));
+  const int items = B * heads;
+  const dim3 grid(static_cast<unsigned>(items < lo.sm_count ? items : lo.sm_count));   // persistent: one CTA per SM
+  __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);
+  if (D == 192)
+    return launch_k(lo, pq::enc_qkv_attn_kernel<192>, grid, dim3(pq::QA_THREADS), pq::QkvAttnCfg::kSmemBytes, st, tx, tw, bias, o, items);
+  return launch_k(lo, pq::enc_qkv_attn_kernel<384>, grid, dim3(pq::QA_THREADS), pq::QkvAttnCfg::kSmemBytes, st, tx, tw, bias, o, items);
 }
 
 struct Slot {
@@ -806,14 +831,22 @@ int encode_chunk(parseq_engine* e, const void* images_any, bool u8, int B, __nv_
   const bool fuse_proj = (e->fuse_ln & 1) && gemm_ln_supported(D) && big;
   const bool fuse_fc2 = (e->fuse_ln & 2) && gemm_ln_supported(D) && big;
   const bool fuse_mlp = e->fuse_mlp && fuse_fc2 && e->Me == 4 * D;
+  // QKV + attention in one kernel wherever it applies (bit-identical to the pair, so at every batch size); the wgmma
+  // attention (attn_impl = 1) and the other token counts keep the QKV GEMM + attention kernel pair
+  const bool fuse_qkv_attn = e->lo.attn_impl == 0 && qkv_attn_supported(T, D, e->cfg.enc_num_heads);
   bool final_done = false;
   for (int i = 0; i < e->cfg.enc_depth; ++i) {
     const std::string p = "encoder.blocks." + std::to_string(i) + ".";
     const bool last = (i == e->cfg.enc_depth - 1);
     if (!(fuse_fc2 && i > 0)) PQ_TRY(layernorm(e, e->x, p + "norm1", 1e-6f, M, e->xn, nullptr, st));
-    PQ_TRY(gemm(e, e->xn, D, e->w(p + "attn.qkv.weight"), D, e->wf(p + "attn.qkv.bias"), M, 3 * D, D, pq::EPI_BF16,
-                1.0f, nullptr, 0, 0, e->qkv, 3 * D, st));
-    {
+    if (fuse_qkv_attn) {
+      // the QKV projection and the attention core in one kernel: qkv stays on the SM
+      TimedScope ts(e, st, CAT_ENC_GEMM, 2.0 * M * 3 * D * D + 4.0 * B * T * T * D);
+      PQ_TRY(qkv_attn_launch(e->lo, e->xn, e->w(p + "attn.qkv.weight"), e->wf(p + "attn.qkv.bias"), B, T, D,
+                             e->cfg.enc_num_heads, e->att, st));
+    } else {
+      PQ_TRY(gemm(e, e->xn, D, e->w(p + "attn.qkv.weight"), D, e->wf(p + "attn.qkv.bias"), M, 3 * D, D, pq::EPI_BF16,
+                  1.0f, nullptr, 0, 0, e->qkv, 3 * D, st));
       TimedScope ts(e, st, CAT_ENC_ATTN, 4.0 * B * T * T * D);
       PQ_TRY(enc_attention_launch(e->lo, e->qkv, B, T, D, e->cfg.enc_num_heads, e->att, st));
     }
@@ -2319,6 +2352,11 @@ int parseq_enc_attention(const void* qkv_bf16, int B, int T, int D, int heads, v
   PQ_TRY(ensure_kernel_attributes());
   PQ_TRY(ensure_sm_count(g_default_opts));
   return enc_attention_launch(g_default_opts, qkv_bf16, B, T, D, heads, out_bf16, reinterpret_cast<cudaStream_t>(stream));
+}
+int parseq_qkv_attention_bf16(const void* xn_bf16, const void* W_qkv, const float* b_qkv, int B, int T, int D, int heads,
+                              void* out_bf16, parseq_stream_t stream) {
+  PQ_TRY(ensure_kernel_attributes());
+  return qkv_attn_launch(g_default_opts, xn_bf16, W_qkv, b_qkv, B, T, D, heads, out_bf16, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -6,7 +6,8 @@
 // registers with wgmma (two m64n128k16 per k16 step).  An ordered pair of named barriers lets only one of them issue
 // its main loop at a time, so one warpgroup's epilogue (bias, GELU, rounding, store) runs under the other's MMAs.
 // A CTA walks the tiles with a stride of the grid; the ring position carries over from tile to tile.  Every projection
-// of the PARSeq path goes through this kernel: patch-embed (K=96), QKV / proj / fc1 / fc2 of the 12 ViT blocks
+// of the PARSeq path goes through this kernel (QKV only where the fused QKV + attention kernel of qkv_attn.cuh does not
+// apply): patch-embed (K=96), QKV / proj / fc1 / fc2 of the 12 ViT blocks
 // (reference: timm Attention/Mlp via strhub/models/parseq/modules.py:145-165), the cross-attention K/V projection of
 // the image memory, the decoder's q / out projections, MLP (modules.py:69-77) and the character head (model.py:63).
 #pragma once

@@ -139,29 +139,12 @@ constexpr int ATT_DH = 64;
 __device__ __forceinline__ uint32_t att_swz(int r, int c) {  // element offset of (row r, col c), c%8==0 chunks
   return static_cast<uint32_t>(r * ATT_DH + ((((c >> 3) ^ (r & 7)) << 3) | (c & 7)));
 }
-__global__ void __launch_bounds__(256, 2) enc_attention_kernel(const __nv_bfloat16* __restrict__ qkv,
-                                                            __nv_bfloat16* __restrict__ out, int D, int heads) {
-  grid_dep_launch();
-  grid_dep_wait();
-  __shared__ __align__(128) __nv_bfloat16 sQ[ATT_T * ATT_DH];
-  __shared__ __align__(128) __nv_bfloat16 sK[ATT_T * ATT_DH];
-  __shared__ __align__(128) __nv_bfloat16 sV[ATT_T * ATT_DH];
-  const int b = blockIdx.x / heads, h = blockIdx.x % heads;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const long long ld = 3ll * D;
-  const __nv_bfloat16* base = qkv + static_cast<long long>(b) * ATT_T * ld + h * ATT_DH;
-  // 3 matrices x 128 rows x 8 chunks of 16 B
-  for (int i = tid; i < 3 * ATT_T * 8; i += 256) {
-    const int m = i / (ATT_T * 8);
-    const int r = (i / 8) % ATT_T;
-    const int ck = i % 8;
-    const __nv_bfloat16* src = base + static_cast<long long>(r) * ld + m * D + ck * 8;
-    __nv_bfloat16* dstm = (m == 0) ? sQ : (m == 1) ? sK : sV;
-    cp_async_16(smem_u32(dstm + att_swz(r, ck * 8)), src);
-  }
-  cp_async_wait_all();
-  __syncthreads();
-
+// The arithmetic of one (image, head) once its Q/K/V tiles (att_swz layout) are in shared memory: warp `warp` (0..7) of
+// the 8 that run it computes query rows [16 warp, 16 warp + 16) and stores them to obase (row pitch D elements).  The
+// warp's rows of sQ are overwritten (output staging); sK / sV are only read.  Shared by enc_attention_kernel and the
+// fused QKV + attention kernel (qkv_attn.cuh), so both compute the same bits.
+__device__ __forceinline__ void att_tile_128(__nv_bfloat16* sQ, const __nv_bfloat16* sK, const __nv_bfloat16* sV,
+                                             __nv_bfloat16* __restrict__ obase, int D, int warp, int lane) {
   const int r0 = warp * 16;
   // ---- Q fragments for the 4 k-steps over d ----
   uint32_t qf[4][4];
@@ -244,7 +227,6 @@ __global__ void __launch_bounds__(256, 2) enc_attention_kernel(const __nv_bfloat
     *reinterpret_cast<uint32_t*>(sQ + att_swz(r0 + g + 8, col)) = pack_bf16(oacc[nt][2] * inv1, oacc[nt][3] * inv1);
   }
   __syncwarp();
-  __nv_bfloat16* obase = out + static_cast<long long>(b) * ATT_T * D + h * ATT_DH;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int idx = i * 32 + lane;       // 16 rows x 8 chunks
@@ -252,6 +234,31 @@ __global__ void __launch_bounds__(256, 2) enc_attention_kernel(const __nv_bfloat
     const uint4 val = *reinterpret_cast<const uint4*>(sQ + att_swz(r, ck * 8));
     *reinterpret_cast<uint4*>(obase + static_cast<long long>(r) * D + ck * 8) = val;
   }
+}
+
+__global__ void __launch_bounds__(256, 2) enc_attention_kernel(const __nv_bfloat16* __restrict__ qkv,
+                                                            __nv_bfloat16* __restrict__ out, int D, int heads) {
+  grid_dep_launch();
+  grid_dep_wait();
+  __shared__ __align__(128) __nv_bfloat16 sQ[ATT_T * ATT_DH];
+  __shared__ __align__(128) __nv_bfloat16 sK[ATT_T * ATT_DH];
+  __shared__ __align__(128) __nv_bfloat16 sV[ATT_T * ATT_DH];
+  const int b = blockIdx.x / heads, h = blockIdx.x % heads;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const long long ld = 3ll * D;
+  const __nv_bfloat16* base = qkv + static_cast<long long>(b) * ATT_T * ld + h * ATT_DH;
+  // 3 matrices x 128 rows x 8 chunks of 16 B
+  for (int i = tid; i < 3 * ATT_T * 8; i += 256) {
+    const int m = i / (ATT_T * 8);
+    const int r = (i / 8) % ATT_T;
+    const int ck = i % 8;
+    const __nv_bfloat16* src = base + static_cast<long long>(r) * ld + m * D + ck * 8;
+    __nv_bfloat16* dstm = (m == 0) ? sQ : (m == 1) ? sK : sV;
+    cp_async_16(smem_u32(dstm + att_swz(r, ck * 8)), src);
+  }
+  cp_async_wait_all();
+  __syncthreads();
+  att_tile_128(sQ, sK, sV, out + static_cast<long long>(b) * ATT_T * D + h * ATT_DH, D, warp, lane);
 }
 
 // ---------------------------------------------------------------------------------------------

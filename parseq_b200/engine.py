@@ -34,7 +34,7 @@ EXPORTS = [
     "parseq_resize_crops", "parseq_forward_crops", "parseq_forward_host_crops",
     "parseq_postprocess", "parseq_encode", "parseq_decode", "parseq_decode_ex", "parseq_head", "parseq_text_embed", "parseq_kernel_launches", "parseq_debug_int", "parseq_bench_tma_stream",
     "parseq_set_option", "parseq_get_timing", "parseq_get_ar_profile", "parseq_last_error", "parseq_version", "parseq_gemm_bf16", "parseq_gemm_ln_bf16", "parseq_mlp_ln_bf16", "parseq_layernorm_bf16",
-    "parseq_enc_attention",
+    "parseq_enc_attention", "parseq_qkv_attention_bf16",
 ]
 
 
@@ -93,6 +93,8 @@ def load_library(path: Optional[str] = None):
     lib.parseq_layernorm_bf16.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int,
                                           C.c_void_p, C.c_void_p, C.c_void_p]
     lib.parseq_enc_attention.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    lib.parseq_qkv_attention_bf16.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                              C.c_void_p, C.c_void_p]
     if path is None:
         _lib = lib
     return lib

@@ -83,6 +83,15 @@ typedef struct parseq_forward_args {
   const int32_t* forced_ids;
   /* Optional: device int32 [refine_iters, batch, num_steps] contexts (BOS included) for the cloze passes. */
   const int32_t* forced_refine;
+  /* Optional per-image character allowlist: uint32 [batch][ceil(C / 32)] words, C = num_tokens - 2; bit c % 32 of word
+   * c / 32 of row b allows class c for image b.  The result is that of the reference with its character head wrapped as
+   * head(x)[b, :, c] = -inf for every disallowed c: every greedy decision (AR feedback, refine contexts, ids, the step
+   * count S) is the argmax of the masked row, a disallowed class never wins (not even with a NaN or +inf raw logit),
+   * and the returned logits hold exactly -inf there.  EOS (class 0) is always allowed, so an empty row decodes to the
+   * empty label; an all-ones row gives the bits of an unmasked call.  NULL = no constraint, and no extra copy or
+   * launch.  Same memory as the entry point's images: DEVICE for parseq_forward / _u8 / _crops, HOST for
+   * the *_host* variants (uploaded with each super-chunk).  PARSeq and ViTSTR; not with forced_ids / forced_refine. */
+  const uint32_t* class_mask;
 } parseq_forward_args;
 
 /* Replaces system.PARSeq.forward -> model.PARSeq.forward (system.py:87-88, model.py:105-169).

@@ -40,6 +40,7 @@ struct DecArParams {
   float* logits;                  // [B, L, C]
   const int* forced;              // optional teacher forcing [B, forced_ld]
   int forced_ld;
+  const uint32_t* mask;           // optional class allowlist [B, ceil(C / 32)] words (ptx.cuh class_allowed)
   unsigned int* bar;              // grid-barrier counter, zero on entry
   unsigned long long* prof;       // optional [L][16] globaltimer stamps of block 0 (phase boundaries), or nullptr
 };
@@ -259,10 +260,12 @@ __device__ void dec_tile(const DecArParams& p, unsigned char* smem, const __nv_b
       const int m = row0 + r;
       if (m >= M) continue;                          // warp-uniform
       float* lrow = p.logits + (static_cast<long long>(m) * p.L + step) * p.C;
+      const uint32_t* mrow = p.mask != nullptr ? p.mask + static_cast<long long>(m) * class_mask_words(N) : nullptr;
       float best = -INFINITY;
       int bi = ARGMAX_NONE;
       for (int j = lane; j < N; j += 32) {
-        const float v = s_log[r * 128 + j];
+        float v = s_log[r * 128 + j];
+        if (mrow != nullptr && !class_allowed(mrow, j)) { v = -INFINITY; s_log[r * 128 + j] = v; }   // (argmax_finish)
         lrow[j] = v;
         argmax_scan(best, bi, v, j);
       }

@@ -50,6 +50,7 @@ struct DecAr2Params {
   float* logits;                  // [B, L, C]
   const int* forced;              // optional teacher forcing [B, forced_ld]
   int forced_ld;
+  const uint32_t* mask;           // optional class allowlist [B, ceil(C / 32)] words (ptx.cuh class_allowed)
   unsigned long long* prof;       // optional [32][16] globaltimer stamps of cluster 0 / rank 0, or nullptr (A2_PROF)
 };
 
@@ -945,6 +946,9 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
       float* lrow0 = p.logits + (static_cast<long long>(img0 + r0) * p.L + step) * p.C;
       float* lrow1 = p.logits + (static_cast<long long>(img0 + r0 + 8) * p.L + step) * p.C;
       const bool st0 = r0 < nrows, st1 = r0 + 8 < nrows;
+      // allowlist words of the two rows, read through L2 per column (a row is up to 512 words: not staged)
+      const uint32_t* mrow0 = (p.mask != nullptr && st0) ? p.mask + (img0 + r0) * class_mask_words(p.C) : nullptr;
+      const uint32_t* mrow1 = (p.mask != nullptr && st1) ? p.mask + (img0 + r0 + 8) * class_mask_words(p.C) : nullptr;
       float best0 = -INFINITY, best1 = -INFINITY;
       int bi0 = ARGMAX_NONE, bi1 = ARGMAX_NONE;
       for (int hc = 0; hc < h_chunks; ++hc) {
@@ -965,7 +969,9 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
               const int c = c_lo + hc * 128 + nt * 8 + 2 * t + e;
               if (c < c_hi) {
                 const float b = __ldg(p.bh + c);
-                const float v0 = acc[j][e] + b, v1 = acc[j][2 + e] + b;
+                float v0 = acc[j][e] + b, v1 = acc[j][2 + e] + b;
+                if (mrow0 != nullptr && !class_allowed(mrow0, c)) v0 = -INFINITY;
+                if (mrow1 != nullptr && !class_allowed(mrow1, c)) v1 = -INFINITY;
                 if (st0) lrow0[c] = v0;
                 if (st1) lrow1[c] = v1;
                 argmax_fold(best0, bi0, v0, c);
@@ -1041,6 +1047,14 @@ __device__ __forceinline__ void dec_ar2_body(const DecAr2Maps& maps, const DecAr
         }
       }
       a2_csync();
+      if (p.mask != nullptr) {
+        // allowlist: the same (warp, lane) -> (row, column) map as the store / argmax loop below, so no barrier between
+        for (int r = warp; r < nrows; r += 8) {
+          const uint32_t* mrow = p.mask + (img0 + r) * class_mask_words(p.C);
+          for (int j = lane; j < p.C; j += 32)
+            if (!class_allowed(mrow, j)) s_log[r * A2_SLOG_LD + j] = -INFINITY;
+        }
+      }
       for (int r = warp; r < nrows; r += 8) {
         const long long b = img0 + r;
         float* lrow = p.logits + (b * p.L + step) * p.C;

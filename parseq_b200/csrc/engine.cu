@@ -224,17 +224,17 @@ size_t head_smem_bytes(int C, int D) {
 }
 int ln_head_argmax_launch(const LaunchOpts& lo, const float* y, const float* g, const float* b, float eps, const __nv_bfloat16* Wh, const float* bh,
                           int M, int C, int D, float* logits, long long logits_ld, int* ids, int ids_ld, int nq, int dst_off,
-                          const int* forced, int forced_ld, cudaStream_t st) {
+                          const int* forced, int forced_ld, const uint32_t* mask, cudaStream_t st) {
   if (C > 128) return fail(PARSEQ_ERR_UNSUPPORTED, "head kernel covers at most 128 classes");
   const dim3 grid((M + pq::HEAD_ROWS - 1) / pq::HEAD_ROWS), block(384);
   const size_t sm = head_smem_bytes(C, D);
   switch (D) {
     case 192: return launch_k(lo, pq::dec_ln_head_argmax_kernel<192>, grid, block, sm, st, y, g, b, eps, Wh, bh, M, C, logits,
-                              logits_ld, ids, ids_ld, nq, dst_off, forced, forced_ld);
+                              logits_ld, ids, ids_ld, nq, dst_off, forced, forced_ld, mask);
     case 384: return launch_k(lo, pq::dec_ln_head_argmax_kernel<384>, grid, block, sm, st, y, g, b, eps, Wh, bh, M, C, logits,
-                              logits_ld, ids, ids_ld, nq, dst_off, forced, forced_ld);
+                              logits_ld, ids, ids_ld, nq, dst_off, forced, forced_ld, mask);
     case 768: return launch_k(lo, pq::dec_ln_head_argmax_kernel<768>, grid, block, sm, st, y, g, b, eps, Wh, bh, M, C, logits,
-                              logits_ld, ids, ids_ld, nq, dst_off, forced, forced_ld);
+                              logits_ld, ids, ids_ld, nq, dst_off, forced, forced_ld, mask);
     default: return fail(PARSEQ_ERR_UNSUPPORTED, "head kernel: embed_dim must be 192, 384 or 768");
   }
 }
@@ -607,6 +607,8 @@ struct parseq_engine {
   // static I/O buffers the CUDA graphs are captured on
   float* in_images = nullptr; float* out_logits = nullptr; int* out_ids = nullptr; int* out_steps = nullptr;
   uint8_t* in_images_u8 = nullptr;  // static input of the uint8 HWC entry points
+  uint32_t* in_mask = nullptr;      // [max_batch, mask_ld] class allowlist rows of the super-chunk (graphs, host entry points)
+  int mask_ld = 0;                  // words per allowlist row: ceil(C / 32)
   // raw-crop entry points (crops.cuh): the resize kernel's crop table [max_batch], its host copy for the current
   // super-chunk, and the device copy of a super-chunk's packed bytes for the host entry point (grown on demand)
   pq::CropDesc* crop_tab = nullptr;
@@ -691,6 +693,7 @@ int alloc_workspace(parseq_engine* e) {
   PQ_TRY(dev_alloc(&e->in_images, NB * 3 * e->cfg.img_h * e->cfg.img_w));
   PQ_TRY(dev_alloc(&e->in_images_u8, NB * 3 * e->cfg.img_h * e->cfg.img_w));
   PQ_TRY(dev_alloc(&e->crop_tab, NB));
+  PQ_TRY(dev_alloc(&e->in_mask, NB * e->mask_ld));
   PQ_TRY(dev_alloc(&e->out_logits, NB * e->L * e->C));
   PQ_TRY(dev_alloc(&e->out_ids, NB * e->L));
   PQ_TRY(dev_alloc(&e->out_steps, 4));
@@ -706,8 +709,9 @@ void free_workspace(parseq_engine* e) {
   drop_graphs(e);
   e->ar2_maps_ok = false;           // holds the address of the K/V cache
   void* ptrs[] = {e->a_pe, e->x, e->xn, e->qkv, e->att, e->hid, e->mem, e->ckv, e->in_images, e->out_logits, e->out_ids,
-                  e->out_steps, e->in_images_u8, e->crop_tab, e->ar_sa, e->ar_ca, e->ar_hd, e->ar_y, e->ar_qc, e->ar_part, e->ar_ids, e->ar_bar, e->ar_prof};
-  e->ar_part = nullptr; e->ar_prof = nullptr; e->in_images_u8 = nullptr; e->crop_tab = nullptr;
+                  e->out_steps, e->in_images_u8, e->crop_tab, e->in_mask, e->ar_sa, e->ar_ca, e->ar_hd, e->ar_y, e->ar_qc, e->ar_part,
+                  e->ar_ids, e->ar_bar, e->ar_prof};
+  e->ar_part = nullptr; e->ar_prof = nullptr; e->in_images_u8 = nullptr; e->crop_tab = nullptr; e->in_mask = nullptr;
   if (e->vt_rows) { cudaFree(e->vt_rows); e->vt_rows = nullptr; }
   e->ar_sa = e->ar_ca = e->ar_hd = nullptr; e->ar_y = e->ar_qc = nullptr; e->ar_ids = nullptr; e->ar_bar = nullptr;
   for (void* p : ptrs)
@@ -888,9 +892,9 @@ int encode_chunk(parseq_engine* e, const void* images_any, bool u8, int B, __nv_
 // ---------------------------------------------------------------- ViTSTR tail (vitstr/model.py:19-28, vitstr/system.py:65-71)
 // logits[b, j] = head(norm(x[b, 1 + j])), j < L = max_length + 1: the reference computes tokens [0, max_length + 2) and
 // drops token 0 (the class token); norm and head are row-wise, so only the kept rows are gathered and computed.
-int argmax_rows(parseq_engine* e, const float* logits, int L, int B, int nrows, int src0, int* ids, int ids_ld, int dst0,
-                const int* forced, int forced_ld, cudaStream_t st);
-int vitstr_tail(parseq_engine* e, int B, int L, float* logits, int* ids_out, cudaStream_t st) {
+int argmax_rows(parseq_engine* e, float* logits, int L, int B, int nrows, int src0, int* ids, int ids_ld, int dst0,
+                const int* forced, int forced_ld, const uint32_t* mask, cudaStream_t st);
+int vitstr_tail(parseq_engine* e, int B, int L, float* logits, int* ids_out, const uint32_t* mask, cudaStream_t st) {
   const int D = e->D, M = B * L;
   {
     TimedScope ts(e, st, CAT_MISC, 0.0);
@@ -902,7 +906,8 @@ int vitstr_tail(parseq_engine* e, int B, int L, float* logits, int* ids_out, cud
   PQ_TRY(layernorm(e, e->vt_rows, "encoder.norm", 1e-6f, M, e->xn, nullptr, st));
   PQ_TRY(gemm(e, e->xn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, pq::EPI_F32, 1.0f, nullptr, 0, 0, logits,
               e->C, st));
-  if (ids_out != nullptr) PQ_TRY(argmax_rows(e, logits, L, B, L, 0, ids_out, L, 0, nullptr, 0, st));
+  // vitstr/model.py:26 applies the head to [B * s, D] rows: row r belongs to image r / s, the allowlist row it takes
+  if (ids_out != nullptr || mask != nullptr) PQ_TRY(argmax_rows(e, logits, L, B, L, 0, ids_out, L, 0, nullptr, 0, mask, st));
   return PARSEQ_OK;
 }
 
@@ -1018,7 +1023,8 @@ int content_stream(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int 
 // the caches of pitch L; otherwise it computes the whole context (nkeys rows per image, pitch nkeys)
 int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, int nq, int q0, int nkeys,
                 int mode, const int* ids, float* logits_out, long long logits_ld, int* ids_dst, int dst_off,
-                const int* forced, int forced_ld, cudaStream_t st, const DecodeExtras* ex = nullptr, bool ar_step = false) {
+                const int* forced, int forced_ld, const uint32_t* mask, cudaStream_t st, const DecodeExtras* ex = nullptr,
+                bool ar_step = false) {
   const int D = e->D, M = B * nq;
   const std::string Ly = "decoder.layers.0.";
   const float qscale = 1.0f / std::sqrt(static_cast<float>(e->dh_dec));
@@ -1086,29 +1092,33 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
                 logits_out, logits_ld, st));
     if (ids_dst != nullptr)
       PQ_TRY(argmax_rows(e, logits_out, static_cast<int>(logits_ld / e->C), B, nq, 0, ids_dst, e->ids_ld, dst_off, forced,
-                         forced_ld, st));
+                         forced_ld, mask, st));
   } else {
     TimedScope ts(e, st, CAT_DEC_GEMM, 2.0 * M * e->C * D);
     PQ_TRY(ln_head_argmax_launch(e->lo, sg.y, e->wf("decoder.norm.weight"), e->wf("decoder.norm.bias"), 1e-5f, e->wb("head.weight"),
                                  e->wf("head.bias"), M, e->C, D, logits_out, logits_ld, ids_dst, e->ids_ld, nq, dst_off, forced,
-                                 forced_ld, st));
+                                 forced_ld, mask, st));
   }
   return PARSEQ_OK;
 }
 
-int argmax_rows(parseq_engine* e, const float* logits, int L, int B, int nrows, int src0, int* ids, int ids_ld, int dst0,
-                const int* forced, int forced_ld, cudaStream_t st) {
+// Greedy ids of B images x nrows logits rows; with an allowlist (`mask`: the images' rows) the disallowed logits are set to
+// -inf in place first, and `ids` may be null.
+int argmax_rows(parseq_engine* e, float* logits, int L, int B, int nrows, int src0, int* ids, int ids_ld, int dst0,
+                const int* forced, int forced_ld, const uint32_t* mask, cudaStream_t st) {
   const int warps = B * nrows;
   if (warps <= 0) return PARSEQ_OK;
   TimedScope ts(e, st, CAT_MISC, 0.0);
   return launch_k(e->lo, pq::argmax_rows_kernel, dim3((warps + 7) / 8), dim3(256), 0, st, logits, L, e->C, B, nrows, src0, ids, ids_ld,
-                  dst0, forced, forced_ld);
+                  dst0, forced, forced_ld, mask);
 }
 
 // Decoder chain of one group of B <= dec_chunk images (their cross K/V is at `ckv`): AR loop / NAR pass, cloze
-// refinement, final argmax.  model.py:113-169.
+// refinement, final argmax.  model.py:113-169.  `mask`: the group's class allowlist rows, or null.  Every head output
+// that the multi-query passes (and the chain's large-head AR steps) leave unmasked is masked by the argmax that reads it,
+// and the final argmax runs with a mask even when the caller wants no ids, so no unmasked logit is returned.
 int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const parseq_forward_args* a, int b0,
-                 int B, int L, float* logits, int* ids_out, int* steps, cudaStream_t st, bool ar_done) {
+                 int B, int L, float* logits, int* ids_out, int* steps, const uint32_t* mask, cudaStream_t st, bool ar_done) {
   // b_first: index of the group's first image inside the super-chunk (row of the K/V cache); b0: inside the caller's batch
   const int C = e->C;
   const int bos = e->V - 2, pad = e->V - 1;
@@ -1124,7 +1134,7 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
     for (int i = 0; i < L; ++i) {
       // step i: context ids[:, :i+1], query position i; the fused tail writes ids[:, i+1] = argmax (model.py:142)
       PQ_TRY(decode_pass(e, sg, b_first, B, 1, i, i + 1, 0, sg.ids_ar, logits + static_cast<long long>(i) * C, LC,
-                         (i + 1 < L) ? sg.ids_ar : nullptr, i + 1, forced, L, st, nullptr, /*ar_step*/ true));
+                         (i + 1 < L) ? sg.ids_ar : nullptr, i + 1, forced, L, mask, st, nullptr, /*ar_step*/ true));
     }
     if (testing && steps != nullptr) {
       PQ_TRY(launch_k(e->lo, pq::ar_steps_kernel, dim3(1), dim3(256), 0, st, static_cast<const int*>(sg.ids_ar), e->ids_ld, B, L,
@@ -1135,7 +1145,7 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
     PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * e->ids_ld + 255) / 256), dim3(256), 0, st, sg.ids_ctx, B, e->ids_ld,
                     bos, pad));
     e->launches++;
-    PQ_TRY(decode_pass(e, sg, b_first, B, L, 0, 1, 0, sg.ids_ctx, logits, C, nullptr, 0, nullptr, 0, st));
+    PQ_TRY(decode_pass(e, sg, b_first, B, L, 0, 1, 0, sg.ids_ctx, logits, C, nullptr, 0, nullptr, 0, mask, st));
   }
   for (int it = 0; it < a->refine_iters; ++it) {
     PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * e->ids_ld + 255) / 256), dim3(256), 0, st, sg.ids_ctx, B, e->ids_ld,
@@ -1145,10 +1155,10 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
                             ? a->forced_refine + (static_cast<long long>(it) * a->batch + b0) * L
                             : nullptr;
     // ctx = [BOS, argmax(logits[:, :L-1])]  (model.py:161)
-    PQ_TRY(argmax_rows(e, logits, L, B, L - 1, 0, sg.ids_ctx, e->ids_ld, 1, forced, L, st));
-    PQ_TRY(decode_pass(e, sg, b_first, B, L, 0, L, 1, sg.ids_ctx, logits, C, nullptr, 0, nullptr, 0, st));
+    PQ_TRY(argmax_rows(e, logits, L, B, L - 1, 0, sg.ids_ctx, e->ids_ld, 1, forced, L, mask, st));
+    PQ_TRY(decode_pass(e, sg, b_first, B, L, 0, L, 1, sg.ids_ctx, logits, C, nullptr, 0, nullptr, 0, mask, st));
   }
-  if (ids_out != nullptr) PQ_TRY(argmax_rows(e, logits, L, B, L, 0, ids_out, L, 0, nullptr, 0, st));
+  if (ids_out != nullptr || mask != nullptr) PQ_TRY(argmax_rows(e, logits, L, B, L, 0, ids_out, L, 0, nullptr, 0, mask, st));
   return PARSEQ_OK;
 }
 
@@ -1284,7 +1294,7 @@ int ar2_dispatch(parseq_engine* e, pq::DecAr2Params& p, cudaStream_t st) {
 // The whole AR loop (model.py:119-147) of B images in one persistent launch: the cluster kernel (dec_ar2.cuh) or the
 // grid-barrier kernel (dec_ar.cuh), as ar_path chose.
 int ar_decode(parseq_engine* e, ArPath path, const parseq_forward_args* a, int b0, int B, int L, float* logits, int* steps,
-              cudaStream_t st) {
+              const uint32_t* mask, cudaStream_t st) {
   const int D = e->D;
   const std::string Ly = "decoder.layers.0.";
   PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * e->ids_ld + 255) / 256), dim3(256), 0, st, e->ar_ids, B, e->ids_ld,
@@ -1304,6 +1314,7 @@ int ar_decode(parseq_engine* e, ArPath path, const parseq_forward_args* a, int b
     p.ids = e->ar_ids; p.ids_ld = e->ids_ld; p.logits = logits;
     p.forced = a->forced_ids ? a->forced_ids + static_cast<long long>(b0) * L : nullptr;
     p.forced_ld = L;
+    p.mask = mask;
     p.prof = e->ar_prof_on ? e->ar_prof : nullptr;
   };
   pq::DecAr2Params q;
@@ -1356,8 +1367,9 @@ int ar_decode(parseq_engine* e, ArPath path, const parseq_forward_args* a, int b
 // part 0: the whole super-chunk.  part 1 / 2 (host entry points, PARSeq only): the encoder of images [0, split) alone /
 // the encoder of images [split, B) and everything after it - two graphs, so that the second half of the input is still
 // uploading while the first half is being encoded.
+// `mask`: the super-chunk's class allowlist rows (mask_ld words per image), or null.
 int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B, int L, const void* images, bool u8,
-                  float* logits, int* ids_out, int* steps, int part = 0, int split = 0) {
+                  float* logits, int* ids_out, int* steps, const uint32_t* mask, int part = 0, int split = 0) {
   const long long img_sz = 3ll * e->cfg.img_h * e->cfg.img_w * (u8 ? 1 : 4);   // bytes per image
   const int D = e->D, T = e->T;
   if (part == 1)
@@ -1366,7 +1378,8 @@ int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B,
     for (int o = 0; o < B; o += e->chunk) {
       const int Bs = (B - o < e->chunk) ? (B - o) : e->chunk;
       PQ_TRY(encode_chunk(e, static_cast<const char*>(images) + o * img_sz, u8, Bs, nullptr, nullptr, e->main, false));
-      PQ_TRY(vitstr_tail(e, Bs, L, logits + 1ll * o * L * e->C, ids_out ? ids_out + 1ll * o * L : nullptr, e->main));
+      PQ_TRY(vitstr_tail(e, Bs, L, logits + 1ll * o * L * e->C, ids_out ? ids_out + 1ll * o * L : nullptr,
+                         mask ? mask + 1ll * o * e->mask_ld : nullptr, e->main));
     }
     return PARSEQ_OK;
   }
@@ -1395,9 +1408,9 @@ int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B,
   const ArPath path = ar_path(e);
   const bool ar_done = a->decode_ar && path != ArPath::Chain;
   if (ar_done) {
-    PQ_TRY(ar_decode(e, path, a, b0, B, L, logits, steps, e->main));
-    if (a->refine_iters == 0) {      // nothing left for the chains but the final argmax
-      if (ids_out != nullptr) PQ_TRY(argmax_rows(e, logits, L, B, L, 0, ids_out, L, 0, nullptr, 0, e->main));
+    PQ_TRY(ar_decode(e, path, a, b0, B, L, logits, steps, mask, e->main));
+    if (a->refine_iters == 0) {      // nothing left for the chains but the final argmax (the AR kernels masked the logits)
+      if (ids_out != nullptr) PQ_TRY(argmax_rows(e, logits, L, B, L, 0, ids_out, L, 0, nullptr, 0, nullptr, e->main));
       return PARSEQ_OK;
     }
   }
@@ -1411,7 +1424,8 @@ int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B,
     cudaStream_t ds = fork ? sg.stream : e->main;
     if (fork) PQ_CUDA(cudaStreamWaitEvent(ds, e->ev_enc, 0));
     PQ_TRY(decode_stage(e, sg, o, a, b0 + o, Bs, L, logits + 1ll * o * L * e->C,
-                        ids_out ? ids_out + 1ll * o * L : nullptr, steps, ds, ar_done));
+                        ids_out ? ids_out + 1ll * o * L : nullptr, steps, mask ? mask + 1ll * o * e->mask_ld : nullptr, ds,
+                        ar_done));
     if (fork) PQ_CUDA(cudaEventRecord(sg.ev_done, ds));
   }
   if (fork)
@@ -1425,9 +1439,12 @@ int num_steps_of(const parseq_engine* e, int max_length) {
   return ml + 1;
 }
 
-// Replays (capturing on first use) the CUDA graph of one super-chunk of Bc images on the static I/O buffers.
+// Replays (capturing on first use) the CUDA graph of one super-chunk of Bc images on the static I/O buffers (a call with
+// an allowlist: its rows are in e->in_mask).
 int run_graph(parseq_engine* e, const parseq_forward_args* a, int Bc, int L, bool u8, int part = 0, int split = 0) {
-  std::vector<int> key = {Bc, L, a->max_length < 0 ? 1 : 0, a->decode_ar ? 1 : 0, a->refine_iters, u8 ? 1 : 0, part, split};
+  const bool masked = a->class_mask != nullptr;
+  std::vector<int> key = {Bc, L, a->max_length < 0 ? 1 : 0, a->decode_ar ? 1 : 0, a->refine_iters, u8 ? 1 : 0, part, split,
+                          masked ? 1 : 0};
   auto it = e->graphs.find(key);
   if (it == e->graphs.end()) {
     parseq_forward_args aa = *a;
@@ -1437,7 +1454,7 @@ int run_graph(parseq_engine* e, const parseq_forward_args* a, int Bc, int L, boo
     const long long before = e->launches;
     PQ_CUDA(cudaStreamBeginCapture(e->main, cudaStreamCaptureModeThreadLocal));
     int r = forward_super(e, &aa, 0, Bc, L, u8 ? static_cast<const void*>(e->in_images_u8) : static_cast<const void*>(e->in_images),
-                          u8, e->out_logits, e->out_ids, e->out_steps, part, split);
+                          u8, e->out_logits, e->out_ids, e->out_steps, masked ? e->in_mask : nullptr, part, split);
     cudaGraph_t g = nullptr;
     cudaError_t ce = cudaStreamEndCapture(e->main, &g);
     if (r != PARSEQ_OK) { if (g) cudaGraphDestroy(g); return r; }
@@ -1595,6 +1612,8 @@ int check_crops_call(parseq_engine* e, const parseq_forward_args* a, const parse
 // `crops` (raw crops of any size, u8): each super-chunk is resized into the static uint8 input in place of the copy.
 int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* images_any, float* logits, int32_t* ids,
                  int32_t* steps, cudaStream_t user, bool host, bool u8 = false, const CropBatch* crops = nullptr) {
+  if (a->class_mask != nullptr && (a->forced_ids != nullptr || a->forced_refine != nullptr))
+    return fail(PARSEQ_ERR_INVALID_ARG, "class_mask cannot be combined with teacher forcing");
   const int L = num_steps_of(e, a->max_length);
   const bool testing = a->max_length < 0;
   const long long img_sz = 3ll * e->cfg.img_h * e->cfg.img_w * (u8 ? 1 : 4);   // bytes per image
@@ -1603,6 +1622,15 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
   const bool eager = !e->use_graph || e->timing || a->forced_ids != nullptr || a->forced_refine != nullptr;
   const cudaMemcpyKind kin = host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
   const cudaMemcpyKind kout = host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+  // the allowlist rows of super-chunk [b0, b0 + Bc) -> the static rows the graphs read (on `main`: after the previous
+  // super-chunk's graph has read them); nothing at all for a call without one
+  const long long mask_row_bytes = 4ll * e->mask_ld;
+  auto stage_mask = [&](int b0, int Bc) -> int {
+    if (a->class_mask == nullptr) return PARSEQ_OK;
+    PQ_CUDA(cudaMemcpyAsync(e->in_mask, a->class_mask + 1ll * b0 * e->mask_ld, static_cast<size_t>(Bc * mask_row_bytes), kin,
+                            e->main));
+    return PARSEQ_OK;
+  };
   // user stream -> main
   PQ_CUDA(cudaEventRecord(e->ev_in, user));
   PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_in, 0));
@@ -1619,8 +1647,8 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
       } else {
         in = images + b0 * img_sz;
       }
-      PQ_TRY(forward_super(e, a, b0, Bc, L, in, u8, logits + 1ll * b0 * L * e->C,
-                           ids ? ids + 1ll * b0 * L : nullptr, e->out_steps));
+      PQ_TRY(forward_super(e, a, b0, Bc, L, in, u8, logits + 1ll * b0 * L * e->C, ids ? ids + 1ll * b0 * L : nullptr,
+                           e->out_steps, a->class_mask ? a->class_mask + 1ll * b0 * e->mask_ld : nullptr));
       continue;
     }
     if (host && !eager && e->arch == 0 && Bc >= 256 && e->chunk >= Bc) {
@@ -1642,6 +1670,7 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
                                 static_cast<size_t>((Bc - split) * img_sz), kin, e->copy));
       }
       PQ_CUDA(cudaEventRecord(e->ev_c[1], e->copy));
+      PQ_TRY(stage_mask(b0, Bc));
       PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_c[0], 0));
       PQ_TRY(run_graph(e, a, Bc, L, u8, 1, split));
       PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_c[1], 0));
@@ -1657,8 +1686,10 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
     } else {
       PQ_CUDA(cudaMemcpyAsync(in_static, images + b0 * img_sz, static_cast<size_t>(Bc * img_sz), kin, e->main));
     }
+    PQ_TRY(stage_mask(b0, Bc));
     if (eager) {
-      PQ_TRY(forward_super(e, a, b0, Bc, L, in_static, u8, e->out_logits, e->out_ids, e->out_steps));
+      PQ_TRY(forward_super(e, a, b0, Bc, L, in_static, u8, e->out_logits, e->out_ids, e->out_steps,
+                           a->class_mask ? e->in_mask : nullptr));
     } else {
       PQ_TRY(run_graph(e, a, Bc, L, u8));
     }
@@ -1741,6 +1772,7 @@ int parseq_create(const parseq_config* cfg, parseq_engine** out) {
   e->ids_ld = e->L <= 32 ? 32 : 64;
   e->V = cfg->num_tokens;
   e->C = cfg->num_tokens - 2;
+  e->mask_ld = (e->C + 31) / 32;
   e->dh_dec = D / cfg->dec_num_heads;
   e->max_batch = cfg->max_batch > 0 ? cfg->max_batch : 512;
   // One pipeline stage per super-chunk by default: the decoder chain is latency-bound and the encoder GEMMs occupy
@@ -2100,7 +2132,7 @@ int parseq_decode_ex(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t n
     ex.pmask = padding_mask ? padding_mask + 1ll * b0 * J : nullptr;
     ex.cmask = content_mask;
     ex.out_norm = out + 1ll * b0 * NQ * D;
-    PQ_TRY(decode_pass(e, sg, 0, Bc, NQ, 0, J, 0, sg.ids_ctx, nullptr, 0, nullptr, 0, nullptr, 0, st, &ex));
+    PQ_TRY(decode_pass(e, sg, 0, Bc, NQ, 0, J, 0, sg.ids_ctx, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, st, &ex));
   }
   PQ_CUDA(cudaEventRecord(e->ev_out, e->main));
   PQ_CUDA(cudaStreamWaitEvent(user, e->ev_out, 0));

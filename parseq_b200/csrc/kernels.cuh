@@ -420,21 +420,32 @@ __global__ void build_ctx_rows_kernel(const float* __restrict__ emb, const float
 // Greedy argmax (torch.argmax semantics: first NaN, else first maximum; ptx.cuh) of logits rows -> token ids.
 // One warp per row.  Row r = (b, s): reads logits[b, src_pos0 + s, :C], writes ids[b*ids_ld + dst_pos0 + s].
 // If `forced` != nullptr the written id is forced[b*forced_ld + dst_pos0 + s] (teacher forcing).
-__global__ void argmax_rows_kernel(const float* __restrict__ logits, int L, int C, int B, int nrows_per_b, int src_pos0,
+// If `mask` != nullptr (class allowlist rows of the B images, ptx.cuh class_allowed) the disallowed logits of the row are
+// set to -inf in place before the argmax; `ids` may then be nullptr (masking only).
+__global__ void argmax_rows_kernel(float* __restrict__ logits, int L, int C, int B, int nrows_per_b, int src_pos0,
                                    int* __restrict__ ids, int ids_ld, int dst_pos0, const int* __restrict__ forced,
-                                   int forced_ld) {
+                                   int forced_ld, const uint32_t* __restrict__ mask) {
   grid_dep_launch();
   grid_dep_wait();
   const int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (w >= B * nrows_per_b) return;
   const int lane = threadIdx.x & 31;
   const int b = w / nrows_per_b, s = w % nrows_per_b;
-  const float* row = logits + (static_cast<long long>(b) * L + src_pos0 + s) * C;
+  float* row = logits + (static_cast<long long>(b) * L + src_pos0 + s) * C;
   float best = -INFINITY;
   int bi = ARGMAX_NONE;
-  for (int j = lane; j < C; j += 32) argmax_scan(best, bi, row[j], j);
+  if (mask != nullptr) {
+    const uint32_t* mrow = mask + static_cast<long long>(b) * class_mask_words(C);
+    for (int j = lane; j < C; j += 32) {
+      float v = row[j];
+      if (!class_allowed(mrow, j)) { v = -INFINITY; row[j] = v; }   // argmax_finish below re-reads this lane's columns
+      argmax_scan(best, bi, v, j);
+    }
+  } else {
+    for (int j = lane; j < C; j += 32) argmax_scan(best, bi, row[j], j);
+  }
   bi = argmax_finish(best, bi, row, C, lane);
-  if (lane == 0) {
+  if (lane == 0 && ids != nullptr) {
     int v = bi;
     if (forced != nullptr) v = forced[static_cast<long long>(b) * forced_ld + dst_pos0 + s];
     ids[static_cast<long long>(b) * ids_ld + dst_pos0 + s] = v;
@@ -828,13 +839,14 @@ __global__ void gather_token_rows_kernel(const float4* __restrict__ x, float4* _
 // conflict-free); each warp computes a (32 classes x 4 rows) partial over a quarter of K; the normalised rows are
 // rounded to bf16 exactly like a tensor-core A operand.
 // logits fp32: row r -> logits[r * logits_ld .. + C); ids (optional): row r = (b, qi) -> ids[b*ids_ld + dst_off + qi].
+// mask (optional): class allowlist rows of the images, row r = (b, qi) reads image b's (ptx.cuh class_allowed).
 constexpr int HEAD_ROWS = 4;
 template <int D>
 __global__ void __launch_bounds__(384) dec_ln_head_argmax_kernel(
     const float* __restrict__ y, const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
     const __nv_bfloat16* __restrict__ Wh, const float* __restrict__ bh, int M, int C, float* __restrict__ logits,
     long long logits_ld, int* __restrict__ ids, int ids_ld, int nq, int dst_off, const int* __restrict__ forced,
-    int forced_ld) {
+    int forced_ld, const uint32_t* __restrict__ mask) {
   extern __shared__ __align__(16) unsigned char head_smem[];
   constexpr int WP = D / 2 + 1;                         // weight row pitch in 32-bit words (odd -> conflict-free)
   uint32_t* sW = reinterpret_cast<uint32_t*>(head_smem);            // [C][WP] bf16x2
@@ -921,10 +933,13 @@ __global__ void __launch_bounds__(384) dec_ln_head_argmax_kernel(
   __syncthreads();
   for (int i = tid; i < HEAD_ROWS * C; i += blockDim.x) {
     const int r = i / C, c = i % C;
-    const float l = ((spart[(0 * HEAD_ROWS + r) * 128 + c] + spart[(1 * HEAD_ROWS + r) * 128 + c]) +
-                     (spart[(2 * HEAD_ROWS + r) * 128 + c] + spart[(3 * HEAD_ROWS + r) * 128 + c])) + __ldg(bh + c);
-    sl[r * 128 + c] = l;
+    float l = ((spart[(0 * HEAD_ROWS + r) * 128 + c] + spart[(1 * HEAD_ROWS + r) * 128 + c]) +
+               (spart[(2 * HEAD_ROWS + r) * 128 + c] + spart[(3 * HEAD_ROWS + r) * 128 + c])) + __ldg(bh + c);
     const int row = row0 + r;
+    if (mask != nullptr && row < M &&
+        !class_allowed(mask + static_cast<long long>(row / nq) * class_mask_words(C), c))
+      l = -INFINITY;
+    sl[r * 128 + c] = l;
     if (row < M) logits[static_cast<long long>(row) * logits_ld + c] = l;
   }
   if (ids == nullptr) return;

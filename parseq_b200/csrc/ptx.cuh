@@ -57,6 +57,13 @@ __device__ __forceinline__ int argmax_finish(float best, int bi, const float* ro
   if (first_nan != ARGMAX_NONE) return first_nan;
   return bi == ARGMAX_NONE ? 0 : bi;                  // no NaN and nothing above -inf: a row of -inf
 }
+// Per-image class allowlist (parseq_forward_args.class_mask): `row` is the image's [ceil(C / 32)] words, bit c % 32 of
+// word c / 32 allows class c.  EOS (class 0) is always allowed.  A disallowed logit becomes -inf before it is stored
+// and before it enters an argmax, so it never wins (not even over a NaN or +inf raw value).
+__device__ __forceinline__ bool class_allowed(const uint32_t* row, int c) {
+  return c == 0 || ((__ldg(row + (c >> 5)) >> (c & 31)) & 1u);
+}
+__device__ __forceinline__ int class_mask_words(int C) { return (C + 31) >> 5; }
 
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {

@@ -101,6 +101,52 @@ def pack_crops(crops: Sequence[Any], pin_memory: bool = False) -> Tuple[Tensor, 
     return data, offsets, sizes
 
 
+Allowlist = Union[None, str, Sequence[Optional[str]]]
+
+
+def allowlist_mask(tokenizer: Tokenizer, allowlist: Allowlist, batch: int, num_classes: int) -> Optional[Tensor]:
+    """The engine's per-image class allowlist (parseq_forward_args.class_mask) as CPU int32 [batch, ceil(C / 32)] words:
+    bit c % 32 of word c / 32 of row b allows head class c (= token id c) for image b.  `allowlist` is None (no
+    constraint: None is returned), one string for every image, or one Optional[str] per image (None: every class).  EOS
+    is always allowed, so an empty string decodes to the empty label."""
+    if allowlist is None:
+        return None
+    if isinstance(allowlist, str):
+        rows: List[Optional[str]] = [allowlist] * batch
+    else:
+        rows = list(allowlist)
+        if len(rows) != batch:
+            raise ValueError(f"allowlist has {len(rows)} entries for {batch} images")
+        if all(r is None for r in rows):
+            return None
+    words = (num_classes + 31) // 32
+    bits = torch.zeros((batch, words * 32), dtype=torch.bool)
+    cache: Dict[str, Tensor] = {}
+    for b, r in enumerate(rows):
+        if r is None:
+            bits[b, :num_classes] = True
+            continue
+        if not isinstance(r, str):
+            raise TypeError(f"allowlist entry {b} must be a string or None, got {type(r).__name__}")
+        if r not in cache:
+            unknown = sorted({ch for ch in r if ch not in tokenizer._stoi or tokenizer._stoi[ch] >= num_classes
+                              or tokenizer._stoi[ch] == tokenizer.eos_id})
+            if unknown:
+                raise ValueError(f"allowlist characters not in charset_train: {''.join(unknown)!r}")
+            ids = torch.tensor([tokenizer.eos_id] + tokenizer._tok2ids(r), dtype=torch.long)
+            row = torch.zeros(words * 32, dtype=torch.bool)
+            row[ids] = True
+            cache[r] = row
+        bits[b] = cache[r]
+    weights = torch.tensor([1 << i for i in range(32)], dtype=torch.int64)
+    packed = (bits.view(batch, words, 32).to(torch.int64) * weights).sum(-1)
+    return torch.where(packed >= 1 << 31, packed - (1 << 32), packed).to(torch.int32)
+
+
+def _mask_ptr(mask: Optional[Tensor]):
+    return mask.data_ptr() if mask is not None else None
+
+
 def _crops_c(data: Tensor, offsets: Tensor, sizes: Tensor, rotation: int) -> CropsC:
     return CropsC(data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), int(rotation))
 
@@ -256,9 +302,10 @@ class _EngineModule(nn.Module):
                          torch.cuda.current_stream(dev).cuda_stream)
         return out
 
-    def _run_crops(self, crops, max_length, decode_ar, refine_iters, rotation):
+    def _run_crops(self, crops, max_length, decode_ar, refine_iters, rotation, class_mask=None):
         """Raw crops of any size: CUDA crops run parseq_forward_crops and return CUDA tensors; CPU crops and PIL images
-        run parseq_forward_host_crops (pinned upload, host outputs) and return CPU tensors."""
+        run parseq_forward_host_crops (pinned upload, host outputs) and return CPU tensors.  `class_mask`: the CPU
+        allowlist words of allowlist_mask, or None."""
         eng = self.engine()
         dev = self._device
         data, offsets, sizes = pack_crops(crops, pin_memory=True)
@@ -271,16 +318,21 @@ class _EngineModule(nn.Module):
         logits = torch.empty((N, L, self.cfg.num_classes), dtype=torch.float32, device=out_dev, pin_memory=host)
         ids = torch.empty((N, L), dtype=torch.int32, device=out_dev, pin_memory=host)
         steps = torch.empty((1,), dtype=torch.int32, device=out_dev, pin_memory=host)
+        if class_mask is not None:
+            class_mask = class_mask.pin_memory() if host else class_mask.to(dev, non_blocking=True)
         eng.forward_crops(_crops_c(data, offsets, sizes, rotation), N, logits.data_ptr(), ids.data_ptr(), steps.data_ptr(),
-                          torch.cuda.current_stream(dev).cuda_stream, max_length, decode_ar, refine_iters, host=host)
+                          torch.cuda.current_stream(dev).cuda_stream, max_length, decode_ar, refine_iters, host=host,
+                          class_mask_ptr=_mask_ptr(class_mask))
         return logits, ids, steps
 
     def _run(self, images: Union[Tensor, List[Any]], max_length, decode_ar, refine_iters, forced_ids=None,
-             forced_refine=None, rotation: int = 0):
+             forced_refine=None, rotation: int = 0, class_mask: Optional[Tensor] = None):
+        if class_mask is not None and (forced_ids is not None or forced_refine is not None):
+            raise ValueError("an allowlist cannot be combined with teacher forcing")
         if isinstance(images, (list, tuple)):
             if forced_ids is not None or forced_refine is not None:
                 raise ValueError("teacher forcing takes normalised float images")
-            return self._run_crops(images, max_length, decode_ar, refine_iters, rotation)
+            return self._run_crops(images, max_length, decode_ar, refine_iters, rotation, class_mask)
         if rotation:
             raise ValueError("rotation applies to lists of raw crops; a tensor input is already at img_size")
         eng = self.engine()
@@ -294,13 +346,17 @@ class _EngineModule(nn.Module):
         fi = forced_ids.to(device=dev, dtype=torch.int32).contiguous() if forced_ids is not None else None
         fr = forced_refine.to(device=dev, dtype=torch.int32).contiguous() if forced_refine is not None else None
         st = torch.cuda.current_stream(dev).cuda_stream
+        if class_mask is not None:
+            if tuple(class_mask.shape) != (N, (self.cfg.num_classes + 31) // 32) or class_mask.dtype != torch.int32:
+                raise ValueError(f"class_mask must be int32 [{N}, {(self.cfg.num_classes + 31) // 32}]")
+            class_mask = class_mask.to(dev, non_blocking=True).contiguous()
         if images.dtype == torch.uint8:
             eng.forward_u8(images.data_ptr(), N, logits.data_ptr(), ids.data_ptr(), steps.data_ptr(), st, max_length,
-                           decode_ar, refine_iters)
+                           decode_ar, refine_iters, class_mask_ptr=_mask_ptr(class_mask))
         else:
             eng.forward(images.data_ptr(), N, logits.data_ptr(), ids.data_ptr(), steps.data_ptr(), st, max_length,
                         decode_ar, refine_iters, fi.data_ptr() if fi is not None else None,
-                        fr.data_ptr() if fr is not None else None)
+                        fr.data_ptr() if fr is not None else None, _mask_ptr(class_mask))
         return logits, ids, steps
 
 
@@ -363,12 +419,12 @@ class ParseqModel(_EngineModule):
 
     def forward(self, tokenizer: Tokenizer, images: Union[Tensor, List[Any]], max_length: Optional[int] = None,
                 return_ids: bool = False, forced_ids: Optional[Tensor] = None,
-                forced_refine: Optional[Tensor] = None, *, rotation: int = 0):
+                forced_refine: Optional[Tensor] = None, *, rotation: int = 0, class_mask: Optional[Tensor] = None):
         """`images`: normalised float [N, 3, H, W], uint8 [N, H, W, 3] at img_size, or a list of raw crops of any size
         (uint8 [h, w, 3] tensors, all CUDA or all CPU, or PIL images in mode RGB) that the engine rotates by `rotation`
-        and resizes as the reference's test transform does."""
+        and resizes as the reference's test transform does.  `class_mask`: per-image allowlist words (allowlist_mask)."""
         logits, ids, steps = self._run(images, max_length, self.decode_ar, self.refine_iters, forced_ids, forced_refine,
-                                       rotation)
+                                       rotation, class_mask)
         if max_length is None and self.decode_ar and not self.refine_iters:
             # model.py:144-147: with no refinement the reference returns only the S steps it ran
             S = int(steps.item())
@@ -386,10 +442,10 @@ class VitstrModel(_EngineModule):
         return self._features(x)
 
     def forward_tokens(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, return_ids: bool = False,
-                       *, rotation: int = 0):
-        """`self.forward(images, max_length + 2)[:, 1:]` (vitstr/system.py:65-71) in one engine call; `images` as in
-        ParseqModel.forward."""
-        logits, ids, _ = self._run(images, max_length, False, 0, rotation=rotation)
+                       *, rotation: int = 0, class_mask: Optional[Tensor] = None):
+        """`self.forward(images, max_length + 2)[:, 1:]` (vitstr/system.py:65-71) in one engine call; `images` and
+        `class_mask` as in ParseqModel.forward."""
+        logits, ids, _ = self._run(images, max_length, False, 0, rotation=rotation, class_mask=class_mask)
         return (logits, ids) if return_ids else logits
 
     def forward(self, x: Tensor, seqlen: int = 25) -> Tensor:
@@ -426,6 +482,10 @@ class _System(nn.Module):
         """The reference's test transform up to the uint8 image (module.py:69-82: rotate, T.Resize(img_size, BICUBIC)) of
         a list of raw crops, on the device: CUDA uint8 [N, H, W, 3], what `forward` takes as a tensor."""
         return self.model.preprocess(crops, rotation)
+
+    def allowlist_mask(self, allowlist: Allowlist, batch: int) -> Optional[Tensor]:
+        """`allowlist` of `forward` as the engine's per-image class mask (module function allowlist_mask)."""
+        return allowlist_mask(self.tokenizer, allowlist, batch, self.model.cfg.num_classes)
 
     def postprocess(self, logits: Tensor):
         """Device-side greedy decode of logits [N, L, C]: (labels, confidences) with the semantics of
@@ -504,9 +564,14 @@ class PARSeq(_System):
         except EngineError as e:  # pragma: no cover
             raise InvalidModelError(str(e)) from e
 
-    def forward(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *, rotation: int = 0) -> Tensor:
-        """`images`: a tensor, as the reference takes, or a list of raw crops of any size (ParseqModel.forward)."""
-        return self.model.forward(self.tokenizer, images, max_length, rotation=rotation)
+    def forward(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *, rotation: int = 0,
+                allowlist: Allowlist = None) -> Tensor:
+        """`images`: a tensor, as the reference takes, or a list of raw crops of any size (ParseqModel.forward).
+        `allowlist`: None, one string for every image, or one Optional[str] per image: the characters each image may
+        decode to.  Every greedy decision (AR loop, refinement, NAR) is constrained on the device, as if the reference's
+        head returned -inf for every other character; those logits come back as -inf."""
+        mask = self.allowlist_mask(allowlist, len(images) if isinstance(images, (list, tuple)) else images.shape[0])
+        return self.model.forward(self.tokenizer, images, max_length, rotation=rotation, class_mask=mask)
 
 
 class ViTSTR(_System):
@@ -534,8 +599,11 @@ class ViTSTR(_System):
         except EngineError as e:  # pragma: no cover
             raise InvalidModelError(str(e)) from e
 
-    def forward(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *, rotation: int = 0) -> Tensor:
-        return self.model.forward_tokens(images, max_length, rotation=rotation)
+    def forward(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *, rotation: int = 0,
+                allowlist: Allowlist = None) -> Tensor:
+        """`allowlist` as in PARSeq.forward: it constrains the argmax of every token position."""
+        mask = self.allowlist_mask(allowlist, len(images) if isinstance(images, (list, tuple)) else images.shape[0])
+        return self.model.forward_tokens(images, max_length, rotation=rotation, class_mask=mask)
 
     @classmethod
     def load_from_checkpoint(cls, checkpoint_path: str, map_location="cpu", **kwargs):

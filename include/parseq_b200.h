@@ -181,8 +181,9 @@ int parseq_bench_tma_stream(void* buf, int64_t bytes, int cluster, int ctas, int
                             parseq_stream_t stream);
 /* Debug counters by name ("ar2_occupancy_mt2", "ar2_clusters_mt2", "ar_last_per", "ar_last_clusters", "sm_count"; the last
  * cluster AR kernel instantiation: "ar_last_cluster_size", "ar_last_mt", "ar_last_head_split", "ar_last_wide",
- * "ar_last_ids_pitch"; "ln_clusters": the clusters the persistent GEMM + LayerNorm kernel runs on, 0 before its first
- * launch, also with e = NULL for the bare kernel exports); -1 if unknown. */
+ * "ar_last_ids_pitch"; "ar_last_path": the AR loop of the last PARSeq forward, 0 the chain of separate kernels, 1 the
+ * grid-barrier kernel, 2 the cluster kernel, -1 no AR loop; "ln_clusters": the clusters the persistent GEMM + LayerNorm
+ * kernel runs on, 0 before its first launch, also with e = NULL for the bare kernel exports); -1 if unknown. */
 int64_t parseq_debug_int(parseq_engine* e, const char* name);
 /* Options: "max_batch" (images per super-chunk = one CUDA graph), "chunk" (images per encoder pass inside a
  * super-chunk), "dec_chunk" (images per decoder chain; the chains of a super-chunk run concurrently on their own

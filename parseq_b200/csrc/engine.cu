@@ -576,6 +576,7 @@ struct parseq_engine {
   int ar_last_cs = 0;
   int ar_last_per = 0, ar_last_ncl = 0;
   int ar_last_mt = 0, ar_last_hs = 0, ar_last_wide = 0, ar_last_idp = 0;   // last cluster-kernel instantiation (debug)
+  int ar_last_path = -1;            // AR loop of the last forward: ArPath (0 chain, 1 grid barrier, 2 cluster), -1 none (debug)
   int ar_cs = 0;                    // option "ar_cluster_size": 0 = auto, 6 / 8 = forced
   int ar_clusters_override = 0;     // option "ar_clusters": clusters the AR kernel spreads a batch over (0 = derived)
   int fuse_mlp = 0;                 // fc1 + GELU + fc2 + residual + LayerNorm in one kernel (mlp_ln.cuh) where fuse_ln bit 1 applies
@@ -1407,6 +1408,7 @@ int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B,
   }
   const ArPath path = ar_path(e);
   const bool ar_done = a->decode_ar && path != ArPath::Chain;
+  e->ar_last_path = a->decode_ar ? static_cast<int>(path) : -1;
   if (ar_done) {
     PQ_TRY(ar_decode(e, path, a, b0, B, L, logits, steps, mask, e->main));
     if (a->refine_iters == 0) {      // nothing left for the chains but the final argmax (the AR kernels masked the logits)
@@ -2213,6 +2215,7 @@ int64_t parseq_debug_int(parseq_engine* e, const char* name) {
   if (n == "ar_last_head_split") return e->ar_last_hs;
   if (n == "ar_last_wide") return e->ar_last_wide;
   if (n == "ar_last_ids_pitch") return e->ar_last_idp;
+  if (n == "ar_last_path") return e->ar_last_path;
   if (n == "sm_count") return e->lo.sm_count;
   return -1;
 }

@@ -140,6 +140,34 @@ int parseq_forward_crops(parseq_engine* e, const parseq_forward_args* args, cons
                          int32_t* ids, int32_t* steps, parseq_stream_t stream);
 int parseq_forward_host_crops(parseq_engine* e, const parseq_forward_args* args, const parseq_crops* crops,
                               float* logits_host, int32_t* ids_host, int32_t* steps_host, parseq_stream_t stream);
+/* Candidate scoring: the log-likelihood of given labels for each image, e.g. to pick the best word of a lexicon.
+ * PARSeq: score(x, c) = sum_{i=0..n} log_softmax(head(decode(tgt_in, memory, content_mask, query_mask)))[i, t_i] with
+ * tgt_in = [BOS, c_1..c_n] (Tokenizer.encode, strhub/data/utils.py:113-118, without its last column), the targets
+ * t = (c_1..c_n, EOS) and the masks of the canonical left-to-right permutation (generate_attn_masks,
+ * strhub/models/parseq/system.py:153-167): minus the summed cross-entropy terms of permutation 0 of training_step
+ * (system.py:169-197).  ViTSTR: sum_{i=0..n} log_softmax(head(norm(x))[:, 1:])[i, t_i], minus the summed terms of
+ * CrossEntropySystem.forward_logits_loss (strhub/models/base.py:194-201).  Each term equals torch.log_softmax(row, -1)[t]
+ * of the fp32 logits row up to fp32 rounding (a row holding NaN or +inf gives NaN); the logits never reach memory.  The
+ * encoder runs once per image, the decoder once per candidate over its n + 1 positions.  Runs eagerly (no CUDA graph);
+ * the first call allocates the scoring buffers. */
+typedef struct parseq_score_args {
+  int32_t batch;               /* N images */
+  int32_t num_candidates;      /* M = sum of per_image */
+  const int32_t* per_image;    /* HOST int32 [N]: candidates of image b, >= 1; candidates are image-major */
+  const int32_t* targets;      /* HOST int32 [M][max_label_length + 1]: c_1..c_n (head classes 1..C-1), EOS (0), rest ignored */
+  const int32_t* lengths;      /* HOST int32 [M]: n, 0 <= n <= max_label_length */
+} parseq_score_args;
+/* images as parseq_forward / parseq_forward_u8 take them; scores DEVICE fp32 [M]; token_logprobs DEVICE fp32
+ * [M][max_label_length + 1] or NULL (term i of candidate m, 0 past n).  All metadata is checked on the host before anything
+ * is launched (PARSEQ_ERR_INVALID_ARG): the counts need no handle, the targets are checked against the handle's
+ * configuration (ids, EOS at position n and nowhere before, no BOS / PAD). */
+int parseq_score(parseq_engine* e, const parseq_score_args* a, const float* images, float* scores, float* token_logprobs,
+                 parseq_stream_t stream);
+int parseq_score_u8(parseq_engine* e, const parseq_score_args* a, const uint8_t* images_hwc, float* scores,
+                    float* token_logprobs, parseq_stream_t stream);
+/* The host checks of parseq_score against a configuration, without a handle or a device. */
+int parseq_score_check(const parseq_config* cfg, const parseq_score_args* a);
+
 /* Fused post-processing of BaseSystem._eval_step (strhub/models/base.py:132-142) + Tokenizer._filter
  * (strhub/data/utils.py:120-129): DEVICE logits [N, num_steps, num_classes] -> ids [N, num_steps] (greedy), lengths [N]
  * (index of the first EOS, num_steps if none) and confidence [N] (product of the max softmax probabilities up to and
@@ -204,7 +232,8 @@ int64_t parseq_debug_int(parseq_engine* e, const char* name);
 int parseq_set_option(parseq_engine* e, const char* name, int64_t value);
 /* After a synchronised forward with "timing"=1: device milliseconds, algorithmic FLOPs and launch count of
  * category 0 encoder GEMM, 1 encoder attention, 2 LayerNorm, 3 decoder GEMM, 4 decoder attention, 5 other,
- * 6 encoder residual GEMM fused with LayerNorm, 7 persistent AR-loop kernel. */
+ * 6 encoder residual GEMM fused with LayerNorm, 7 persistent AR-loop kernel, 8 scoring tail (head GEMM with the log-sum-exp
+ * epilogue and the per-candidate reduce of parseq_score). */
 int parseq_get_timing(parseq_engine* e, int category, double* ms, double* flops, int64_t* count);
 /* Debug: after a forward with option "ar_prof"=1, copies the [32 steps][16 slots] globaltimer (ns) stamps that block 0 of
  * the persistent AR kernel recorded at its phase boundaries.  Row 26 holds extra stamps of step 1 of the cluster kernel;

@@ -312,6 +312,7 @@ int init_kernel_attributes() {
   PQ_TRY((gemm_attr<pq::EPI_BF16, pq::ST_TMA_3D>()));
   PQ_TRY((gemm_attr<pq::EPI_GELU_BF16, pq::ST_REG>()));
   PQ_TRY((gemm_attr<pq::EPI_GELU_BF16, pq::ST_TMA_2D>()));
+  PQ_TRY(set_smem(pq::gemm_bf16_lse_kernel, pq::GemmCfg::smem_bytes<false>()));
   PQ_TRY(set_smem(pq::tma_stream_bench_kernel, kTmaBenchSmem));
   int dev = 0, optin = 0;
   PQ_CUDA(cudaGetDevice(&dev));
@@ -383,6 +384,29 @@ int gemm_launch(LaunchOpts& lo, const void* A, long long lda, const void* W, lon
   }
   return store == pq::ST_TMA_2D ? launch_gemm_cfg<pq::EPI_GELU_BF16, pq::ST_TMA_2D>(lo, ta, tb, to, p, tiles, st)
                                 : launch_gemm_cfg<pq::EPI_GELU_BF16, pq::ST_REG>(lo, ta, tb, to, p, tiles, st);
+}
+
+// The head GEMM with the log-sum-exp epilogue (gemm.cuh, gemm_bf16_lse_kernel): A[M, K] * W[N, K]^T + bias never leaves the registers;
+// part[M][ceil(N / 128)] float2 per-tile (max, sum exp) partials, tlogit[row] = the logit of class tgt[row] (tgt may be
+// null: partials only)
+int gemm_lse_launch(LaunchOpts& lo, const void* A, long long lda, const void* W, long long ldw, const float* bias, int M, int N,
+                    int K, const int* tgt, float2* part, float* tlogit, cudaStream_t st) {
+  if (M <= 0 || N <= 0 || K <= 0) return fail(PARSEQ_ERR_INVALID_ARG, "gemm: empty problem");
+  PQ_TRY(ensure_sm_count(lo));
+  CUtensorMap ta, tb;
+  PQ_TRY(make_tmap(&ta, A, 2, M, K, lda, pq::GEMM_BLOCK_K, pq::GEMM_BLOCK_M));
+  PQ_TRY(make_tmap(&tb, W, 2, N, K, ldw, pq::GEMM_BLOCK_K, pq::GEMM_BLOCK_N));
+  pq::GemmParams p{};
+  p.M = M; p.N = N; p.K = K; p.alpha = 1.0f; p.bias = bias;
+  p.out = part;
+  p.max_stages = lo.gemm_stages;
+  p.num_m_tiles = (M + pq::GEMM_BLOCK_M - 1) / pq::GEMM_BLOCK_M;
+  p.num_n_tiles = (N + pq::GEMM_BLOCK_N - 1) / pq::GEMM_BLOCK_N;
+  p.lse_tgt = tgt;
+  p.lse_tlogit = tlogit;
+  const int tiles = p.num_m_tiles * p.num_n_tiles;
+  return launch_k(lo, pq::gemm_bf16_lse_kernel, dim3(static_cast<unsigned>(tiles < lo.sm_count ? tiles : lo.sm_count)),
+                  dim3(pq::GEMM_THREADS), pq::GemmCfg::smem_bytes<false>(), st, ta, tb, ta, p);
 }
 
 // x[M, D] += A[M, K] * W[D, K]^T + bias (fp32, in place); xn[M, D] = bf16(LayerNorm(x; gamma, beta, eps))   (gemm_ln.cuh)
@@ -596,6 +620,13 @@ struct parseq_engine {
     // 1..dec_depth-1, one [dec_chunk, L, 2D] bf16 cache per layer (layer 0 reads the (position, token) table)
     float* cx = nullptr;
     std::vector<__nv_bfloat16*> kvc;
+    // candidate scoring (parseq_score), allocated by the first score call: per-tile log-sum-exp partials
+    // [dec_chunk * L][ceil(C / 128)] and target logits of the chain's rows; while a group is decoded, cand_off (device,
+    // candidates of each of its images) routes the cross-attention rows to their image (dec_layer_rest)
+    float2* lse_part = nullptr;
+    float* lse_tlogit = nullptr;
+    const int* cand_off = nullptr;
+    int cand_imgs = 0, cand_max_rows = 0;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev_enc = nullptr, ev_done = nullptr;
   };
@@ -617,6 +648,12 @@ struct parseq_engine {
   long long crop_base = 0;
   uint8_t* crop_stage = nullptr;
   long long crop_stage_bytes = 0;
+  // candidate scoring: the call's metadata (ids, targets, row tables; grown on demand), one causal [P][P] mask per
+  // P = 1..L (mask of P at sc_causal + (P - 1) * L * L), and ViTSTR's LSE partials of a chunk's (image, position) rows
+  int* sc_meta = nullptr;
+  long long sc_meta_ints = 0;
+  unsigned char* sc_causal = nullptr;
+  float2* sc_vt_part = nullptr;
   bool use_graph = true;
   struct GraphEntry { cudaGraphExec_t exec; long long kernels; };
   std::map<std::vector<int>, GraphEntry> graphs;
@@ -720,6 +757,10 @@ void free_workspace(parseq_engine* e) {
   for (auto p : e->ckv_deep)
     if (p) cudaFree(p);
   e->ckv_deep.clear();
+  void* sc[] = {e->sc_meta, e->sc_causal, e->sc_vt_part};
+  for (void* p : sc)
+    if (p) cudaFree(p);
+  e->sc_meta = nullptr; e->sc_meta_ints = 0; e->sc_causal = nullptr; e->sc_vt_part = nullptr;
   if (e->ev_enc) { cudaEventDestroy(e->ev_enc); e->ev_enc = nullptr; }
   e->a_pe = e->xn = e->qkv = e->att = e->hid = e->mem = e->ckv = nullptr;
   e->x = e->in_images = e->out_logits = nullptr;
@@ -729,6 +770,8 @@ void free_workspace(parseq_engine* e) {
     for (void* p : q)
       if (p) cudaFree(p);
     if (sg.cx) cudaFree(sg.cx);
+    if (sg.lse_part) cudaFree(sg.lse_part);
+    if (sg.lse_tlogit) cudaFree(sg.lse_tlogit);
     for (auto p : sg.kvc)
       if (p) cudaFree(p);
     if (sg.stream) cudaStreamDestroy(sg.stream);
@@ -738,9 +781,10 @@ void free_workspace(parseq_engine* e) {
   e->stages.clear();
 }
 
-// categories: 0 encoder GEMM, 1 encoder attention, 2 LayerNorm, 3 decoder GEMM, 4 decoder attention, 5 other
+// categories: 0 encoder GEMM, 1 encoder attention, 2 LayerNorm, 3 decoder GEMM, 4 decoder attention, 5 other,
+// 6 encoder residual GEMM + LayerNorm, 7 AR-loop kernel, 8 scoring tail (head GEMM with the LSE epilogue + reduce)
 enum { CAT_ENC_GEMM = 0, CAT_ENC_ATTN = 1, CAT_LN = 2, CAT_DEC_GEMM = 3, CAT_DEC_ATTN = 4, CAT_MISC = 5, CAT_ENC_GEMM_LN = 6, CAT_DEC_AR = 7,
-       CAT_COUNT = 8 };
+       CAT_SCORE = 8, CAT_COUNT = 9 };
 
 cudaEvent_t pool_event(parseq_engine* e) {
   if (!e->event_pool.empty()) { cudaEvent_t ev = e->event_pool.back(); e->event_pool.pop_back(); return ev; }
@@ -895,7 +939,8 @@ int encode_chunk(parseq_engine* e, const void* images_any, bool u8, int B, __nv_
 // drops token 0 (the class token); norm and head are row-wise, so only the kept rows are gathered and computed.
 int argmax_rows(parseq_engine* e, float* logits, int L, int B, int nrows, int src0, int* ids, int ids_ld, int dst0,
                 const int* forced, int forced_ld, const uint32_t* mask, cudaStream_t st);
-int vitstr_tail(parseq_engine* e, int B, int L, float* logits, int* ids_out, const uint32_t* mask, cudaStream_t st) {
+// e->xn [B * L, D] = bf16(norm(x[b, 1 + j])), j < L: the rows the head reads
+int vitstr_rows(parseq_engine* e, int B, int L, cudaStream_t st) {
   const int D = e->D, M = B * L;
   {
     TimedScope ts(e, st, CAT_MISC, 0.0);
@@ -904,7 +949,11 @@ int vitstr_tail(parseq_engine* e, int B, int L, float* logits, int* ids_out, con
     PQ_TRY(launch_k(e->lo, pq::gather_token_rows_kernel, dim3(grid), dim3(256), 0, st, reinterpret_cast<const float4*>(e->x),
                     reinterpret_cast<float4*>(e->vt_rows), B, e->T, 1, L, D / 4));
   }
-  PQ_TRY(layernorm(e, e->vt_rows, "encoder.norm", 1e-6f, M, e->xn, nullptr, st));
+  return layernorm(e, e->vt_rows, "encoder.norm", 1e-6f, M, e->xn, nullptr, st);
+}
+int vitstr_tail(parseq_engine* e, int B, int L, float* logits, int* ids_out, const uint32_t* mask, cudaStream_t st) {
+  const int D = e->D, M = B * L;
+  PQ_TRY(vitstr_rows(e, B, L, st));
   PQ_TRY(gemm(e, e->xn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, pq::EPI_F32, 1.0f, nullptr, 0, 0, logits,
               e->C, st));
   // vitstr/model.py:26 applies the head to [B * s, D] rows: row r belongs to image r / s, the allowlist row it takes
@@ -923,6 +972,8 @@ struct DecodeExtras {
   const unsigned char* pmask = nullptr;  // [B, nkeys], 1 = masked
   const unsigned char* cmask = nullptr;  // [nkeys, nkeys] content-stream mask (`tgt_mask`), 1 = masked; depth >= 2 only
   float* out_norm = nullptr;             // [B*nq, D] fp32: decoder.norm(y) is the result (no head)
+  const int* lse_tgt = nullptr;          // [B*nq] target class per row: the head runs with the LSE epilogue into the
+                                         // stage's lse_part / lse_tlogit (candidate scoring), no logits are stored
 };
 
 const __nv_bfloat16* ckv_of(const parseq_engine* e, int layer) { return layer == 0 ? e->ckv : e->ckv_deep[layer - 1]; }
@@ -965,7 +1016,17 @@ int dec_layer_rest(parseq_engine* e, parseq_engine::Stage& sg, int l, int b_firs
   {
     TimedScope ts(e, st, CAT_DEC_ATTN, 4.0 * M * e->T * D);
     const long long kv_rows = 1ll * e->max_batch * e->T;
-    if (e->T <= 128)
+    if (sg.cand_off != nullptr) {
+      // candidate scoring: the rows of each image's candidates attend to that image (64 rows per CTA)
+      constexpr int kRows = 64;
+      const dim3 grid(static_cast<unsigned>(sg.cand_imgs * e->cfg.dec_num_heads), static_cast<unsigned>((sg.cand_max_rows + kRows - 1) / kRows));
+      if (e->T <= 128)
+        PQ_TRY(launch_k(e->lo, pq::dec_cross_attn3_grouped_kernel<4>, grid, dim3(128), 0, st, static_cast<const float*>(sg.qc),
+                        ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, sg.cand_off, kRows, sg.ca));
+      else
+        PQ_TRY(launch_k(e->lo, pq::dec_cross_attn3_grouped_kernel<8>, grid, dim3(128), 0, st, static_cast<const float*>(sg.qc),
+                        ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, sg.cand_off, kRows, sg.ca));
+    } else if (e->T <= 128)
       PQ_TRY(launch_k(e->lo, pq::dec_cross_attn3_kernel<4>, dim3(B * e->cfg.dec_num_heads), dim3(128), 0, st,
                       static_cast<const float*>(sg.qc), ckv_of(e, l), kv_rows, b_first, e->T, D,
                       e->cfg.dec_num_heads, nq, sg.ca));
@@ -1046,9 +1107,13 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
   }
   if (ex != nullptr && (ex->qmask != nullptr || ex->pmask != nullptr)) {
     if (mode != 2) {                     // masks with the default queries: expand the table rows (tiny) so mode 2 applies
+      // launched without PDL: the kernel has no griddepcontrol.wait, so as a PDL launch it could start under the previous
+      // kernel on the stream (an early-triggering GEMM: the cross K/V, or the previous scoring group's head), and every
+      // later kernel of this pass, which waits only for its own predecessor, would lose its order after that kernel
       const int n4 = nq * D / 4;
-      PQ_TRY(launch_k(e->lo, pq::bcast_rows_kernel, dim3(static_cast<unsigned>(std::min((B * n4 + 255) / 256, 132 * 8))), dim3(256), 0, st,
-                      reinterpret_cast<const float4*>(e->qs + static_cast<long long>(q0) * D), reinterpret_cast<float4*>(sg.qc), n4, B));
+      PQ_TRY(launch_ex(LaunchConfig(dim3(static_cast<unsigned>(std::min((B * n4 + 255) / 256, 132 * 8))), dim3(256), 0, st, 0, false),
+                       pq::bcast_rows_kernel, reinterpret_cast<const float4*>(e->qs + static_cast<long long>(q0) * D),
+                       reinterpret_cast<float4*>(sg.qc), n4, B));
       e->launches++;
       qself = sg.qc;
       mode = 2;
@@ -1079,6 +1144,13 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
   if (ex != nullptr && ex->out_norm != nullptr) {
     // PARSeq.decode returns the decoder output: final LayerNorm only (modules.py:123-125)
     PQ_TRY(layernorm(e, sg.y, "decoder.norm", 1e-5f, M, sg.yn, ex->out_norm, st));
+  } else if (ex != nullptr && ex->lse_tgt != nullptr) {
+    // candidate scoring: the multi-query head's LayerNorm, then the head GEMM whose epilogue keeps only the per-row
+    // log-sum-exp partials and target logits (score_reduce_kernel finishes the terms)
+    PQ_TRY(layernorm(e, sg.y, "decoder.norm", 1e-5f, M, sg.yn, nullptr, st));
+    TimedScope ts(e, st, CAT_SCORE, 2.0 * M * e->C * D);
+    PQ_TRY(gemm_lse_launch(e->lo, sg.yn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, ex->lse_tgt, sg.lse_part,
+                           sg.lse_tlogit, st));
   } else if (nq > 1 && ids_dst == nullptr) {
     // multi-query passes (refine / NAR): LayerNorm kernel + wgmma GEMM for the head (weights read once per tile).
     // Chosen by pass type, not by batch size, so that a row's result does not depend on the batch it is computed in.
@@ -1369,6 +1441,23 @@ int ar_decode(parseq_engine* e, ArPath path, const parseq_forward_args* a, int b
 // the encoder of images [split, B) and everything after it - two graphs, so that the second half of the input is still
 // uploading while the first half is being encoded.
 // `mask`: the super-chunk's class allowlist rows (mask_ld words per image), or null.
+// Cross-attention K/V of every decoder layer from the memory of the super-chunk's B images, once per image (the
+// reference recomputes it in every decode call).
+int cross_kv(parseq_engine* e, int B) {
+  const int D = e->D, T = e->T;
+  e->cur_cat = CAT_DEC_GEMM;
+  for (int l = 0; l < e->cfg.dec_depth; ++l) {
+    const std::string Ly = "decoder.layers." + std::to_string(l) + ".";
+    const __nv_bfloat16* Wkv = e->wb(Ly + "cross_attn.in_proj_weight") + static_cast<long long>(D) * D;
+    const float* bkv = e->wf(Ly + "cross_attn.in_proj_bias") + D;
+    // stored column-blocked [2D/64][max_batch * T][64]: an image's K (V) panel of 64 channels is one contiguous T x 128 B
+    // run - what a TMA box of the AR kernel and a head of the refine-pass attention read
+    PQ_TRY(gemm(e, e->mem, D, Wkv, D, bkv, B * T, 2 * D, D, pq::EPI_BF16, 1.0f, nullptr, 0, 0,
+                const_cast<__nv_bfloat16*>(ckv_of(e, l)), 2 * D, e->main, 1ll * e->max_batch * T));
+  }
+  return PARSEQ_OK;
+}
+
 int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B, int L, const void* images, bool u8,
                   float* logits, int* ids_out, int* steps, const uint32_t* mask, int part = 0, int split = 0) {
   const long long img_sz = 3ll * e->cfg.img_h * e->cfg.img_w * (u8 ? 1 : 4);   // bytes per image
@@ -1395,17 +1484,7 @@ int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B,
                           true, B));
     }
   }
-  // cross-attention K/V of the image memory, once per image (the reference recomputes it in every decode call)
-  e->cur_cat = CAT_DEC_GEMM;
-  for (int l = 0; l < e->cfg.dec_depth; ++l) {
-    const std::string Ly = "decoder.layers." + std::to_string(l) + ".";
-    const __nv_bfloat16* Wkv = e->wb(Ly + "cross_attn.in_proj_weight") + static_cast<long long>(D) * D;
-    const float* bkv = e->wf(Ly + "cross_attn.in_proj_bias") + D;
-    // stored column-blocked [2D/64][max_batch * T][64]: an image's K (V) panel of 64 channels is one contiguous T x 128 B
-    // run - what a TMA box of the AR kernel and a head of the refine-pass attention read
-    PQ_TRY(gemm(e, e->mem, D, Wkv, D, bkv, B * T, 2 * D, D, pq::EPI_BF16, 1.0f, nullptr, 0, 0,
-                const_cast<__nv_bfloat16*>(ckv_of(e, l)), 2 * D, e->main, 1ll * e->max_batch * T));
-  }
+  PQ_TRY(cross_kv(e, B));
   const ArPath path = ar_path(e);
   const bool ar_done = a->decode_ar && path != ArPath::Chain;
   e->ar_last_path = a->decode_ar ? static_cast<int>(path) : -1;
@@ -1704,6 +1783,236 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
   PQ_CUDA(cudaEventRecord(e->ev_out, e->main));
   PQ_CUDA(cudaStreamWaitEvent(user, e->ev_out, 0));
   return PARSEQ_OK;
+}
+
+// ---------------------------------------------------------------- candidate scoring (parseq_score)
+// The metadata of a score call, on the host alone (no handle or device needed).  max_label_length < 0: the counts only.
+// Target row m (pitch max_label_length + 1) holds c_1..c_n (head classes 1..C-1) and EOS (0) at position n.
+int check_score(const parseq_score_args* a, int max_label_length, int num_classes) {
+  if (a == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  if (a->batch < 0 || a->num_candidates < 0) return fail(PARSEQ_ERR_INVALID_ARG, "negative batch / num_candidates");
+  if (a->batch == 0) return a->num_candidates == 0 ? PARSEQ_OK : fail(PARSEQ_ERR_INVALID_ARG, "candidates without images");
+  if (a->per_image == nullptr || a->targets == nullptr || a->lengths == nullptr)
+    return fail(PARSEQ_ERR_INVALID_ARG, "null per_image, targets or lengths");
+  long long sum = 0;
+  for (int b = 0; b < a->batch; ++b) {
+    if (a->per_image[b] < 1) return fail(PARSEQ_ERR_INVALID_ARG, "image " + std::to_string(b) + ": per_image must be >= 1");
+    sum += a->per_image[b];
+  }
+  if (sum != a->num_candidates)
+    return fail(PARSEQ_ERR_INVALID_ARG, "per_image sums to " + std::to_string(sum) + ", num_candidates is " +
+                                            std::to_string(a->num_candidates));
+  if (max_label_length < 0) return PARSEQ_OK;
+  const int L = max_label_length + 1, C = num_classes;
+  for (int m = 0; m < a->num_candidates; ++m) {
+    const std::string who = "candidate " + std::to_string(m) + ": ";
+    const int n = a->lengths[m];
+    if (n < 0 || n > max_label_length)
+      return fail(PARSEQ_ERR_INVALID_ARG, who + "length " + std::to_string(n) + " outside [0, max_label_length = " +
+                                              std::to_string(max_label_length) + "]");
+    const int32_t* t = a->targets + 1ll * m * L;
+    for (int i = 0; i < n; ++i) {
+      if (t[i] == 0) return fail(PARSEQ_ERR_INVALID_ARG, who + "EOS at position " + std::to_string(i) + ", before its end " + std::to_string(n));
+      if (t[i] == C || t[i] == C + 1) return fail(PARSEQ_ERR_INVALID_ARG, who + "BOS or PAD id at position " + std::to_string(i));
+      if (t[i] < 1 || t[i] > C + 1)
+        return fail(PARSEQ_ERR_INVALID_ARG, who + "id " + std::to_string(t[i]) + " at position " + std::to_string(i) +
+                                                " outside the character classes [1, " + std::to_string(C - 1) + "]");
+    }
+    if (t[n] != 0) return fail(PARSEQ_ERR_INVALID_ARG, who + "no EOS (0) at position n = " + std::to_string(n));
+  }
+  return PARSEQ_OK;
+}
+
+// Scoring buffers, on the first score call (an engine that never scores allocates none of them): the chains' LSE
+// partials and target logits (PARSeq), ViTSTR's partials of a chunk, and the causal masks of every row count P.
+int score_reserve(parseq_engine* e) {
+  const int L = e->L;
+  const long long ntiles = (e->C + pq::GEMM_BLOCK_N - 1) / pq::GEMM_BLOCK_N;
+  const long long Rd = 1ll * e->dec_chunk * L;
+  if (e->arch == 0) {
+    for (auto& sg : e->stages) {
+      if (sg.lse_part != nullptr) continue;
+      PQ_TRY(dev_alloc(&sg.lse_part, Rd * ntiles));
+      PQ_TRY(dev_alloc(&sg.lse_tlogit, Rd));
+    }
+    if (e->sc_causal == nullptr) {
+      // the canonical left-to-right permutation (system.py:153-167): query i and content row i see keys 0..i
+      std::vector<unsigned char> h(static_cast<size_t>(L) * L * L, 0);
+      for (int P = 1; P <= L; ++P)
+        for (int q = 0; q < P; ++q)
+          for (int k = 0; k < P; ++k) h[static_cast<size_t>(P - 1) * L * L + static_cast<size_t>(q) * P + k] = k > q ? 1 : 0;
+      PQ_TRY(dev_alloc(&e->sc_causal, static_cast<long long>(h.size())));
+      PQ_CUDA(cudaMemcpy(e->sc_causal, h.data(), h.size(), cudaMemcpyHostToDevice));
+    }
+  } else if (e->sc_vt_part == nullptr) {
+    PQ_TRY(dev_alloc(&e->sc_vt_part, 1ll * e->chunk * L * ntiles));
+  }
+  return PARSEQ_OK;
+}
+
+// A group of candidates decoded in one pass of a chain: candidates [m0, m1) of images [b_lo, b_lo + nimg), P rows each
+// (P = the longest label + 1), at most dec_chunk * L rows.  Offsets index the call's metadata (ints).
+struct ScoreGroup {
+  int m0, m1, P, b_lo, nimg, max_rows;
+  long long ids_off, tgt_off, cand_off;
+};
+
+// Scores candidate labels of a batch of images (parseq_score): encoder and cross K/V once per super-chunk, then the
+// candidates of its images in groups over the chains (PARSeq), or the head's LSE partials once per (image, position)
+// and a gather per candidate (ViTSTR).
+int score_impl(parseq_engine* e, const parseq_score_args* a, const void* images_any, bool u8, float* scores, float* token_lp,
+               cudaStream_t user) {
+  const int L = e->L, D = e->D, T = e->T, N = a->batch, M = a->num_candidates;
+  const int bos = e->V - 2, pad = e->V - 1;
+  const int ntiles = (e->C + pq::GEMM_BLOCK_N - 1) / pq::GEMM_BLOCK_N;
+  const long long img_sz = 3ll * e->cfg.img_h * e->cfg.img_w * (u8 ? 1 : 4);
+  const char* images = static_cast<const char*>(images_any);
+  PQ_TRY(score_reserve(e));
+  // host metadata: lengths [M], then per arch the candidates' targets / images or the groups' ids, targets, offsets
+  std::vector<int> first(static_cast<size_t>(N) + 1, 0);              // first candidate of image b
+  for (int b = 0; b < N; ++b) first[b + 1] = first[b] + a->per_image[b];
+  std::vector<int> h(a->lengths, a->lengths + M);
+  const long long len_off = 0;
+  long long vt_tgt_off = 0, vt_img_off = 0;
+  std::vector<ScoreGroup> groups;
+  if (e->arch == 1) {
+    vt_tgt_off = static_cast<long long>(h.size());
+    for (int m = 0; m < M; ++m)
+      for (int i = 0; i < L; ++i) h.push_back(i <= a->lengths[m] ? a->targets[1ll * m * L + i] : -1);
+    vt_img_off = static_cast<long long>(h.size());
+    for (int b = 0; b < N; ++b) h.insert(h.end(), static_cast<size_t>(a->per_image[b]), b);
+  } else {
+    const long long cap = 1ll * e->dec_chunk * L;
+    std::vector<int> img_of(static_cast<size_t>(M));
+    for (int b = 0; b < N; ++b) std::fill(img_of.begin() + first[b], img_of.begin() + first[b + 1], b);
+    for (int b0 = 0; b0 < N; b0 += e->max_batch) {                    // groups never span super-chunks
+      const int m_end = first[std::min(N, b0 + e->max_batch)];
+      for (int m = first[b0]; m < m_end;) {
+        ScoreGroup g{m, m, 0, img_of[m], 0, 0, 0, 0, 0};
+        while (g.m1 < m_end) {
+          const int P = std::max(g.P, a->lengths[g.m1] + 1);
+          if (1ll * (g.m1 + 1 - g.m0) * P > cap) break;
+          g.P = P;
+          ++g.m1;
+        }
+        g.nimg = img_of[g.m1 - 1] - g.b_lo + 1;
+        g.ids_off = static_cast<long long>(h.size());
+        for (int c = g.m0; c < g.m1; ++c) {
+          const size_t r = h.size();
+          h.resize(r + e->ids_ld, pad);
+          h[r] = bos;
+          for (int i = 0; i < a->lengths[c]; ++i) h[r + 1 + i] = a->targets[1ll * c * L + i];
+        }
+        g.tgt_off = static_cast<long long>(h.size());
+        for (int c = g.m0; c < g.m1; ++c)
+          for (int i = 0; i < g.P; ++i) h.push_back(i <= a->lengths[c] ? a->targets[1ll * c * L + i] : -1);
+        g.cand_off = static_cast<long long>(h.size());
+        for (int j = 0; j <= g.nimg; ++j) {
+          const int b = g.b_lo + j;
+          const int c = (j == g.nimg) ? g.m1 : std::max(first[b], g.m0);
+          h.push_back(c - g.m0);
+          if (j > 0) g.max_rows = std::max(g.max_rows, (h.back() - h[h.size() - 2]) * g.P);
+        }
+        groups.push_back(g);
+        m = g.m1;
+      }
+    }
+  }
+  if (static_cast<long long>(h.size()) > e->sc_meta_ints) {
+    PQ_CUDA(cudaStreamSynchronize(e->main));                          // the previous call's kernels may still read it
+    if (e->sc_meta) cudaFree(e->sc_meta);
+    e->sc_meta = nullptr;
+    e->sc_meta_ints = 0;
+    PQ_TRY(dev_alloc(&e->sc_meta, static_cast<long long>(h.size())));
+    e->sc_meta_ints = static_cast<long long>(h.size());
+  }
+  const int* meta = e->sc_meta;
+  PQ_CUDA(cudaEventRecord(e->ev_in, user));
+  PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_in, 0));
+  // pageable source: the copy is staged before the call returns, so `h` may go
+  PQ_CUDA(cudaMemcpyAsync(e->sc_meta, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice, e->main));
+  size_t gi = 0;
+  for (int b0 = 0; b0 < N; b0 += e->max_batch) {
+    const int Bc = std::min(N - b0, e->max_batch);
+    if (e->arch == 1) {
+      for (int o = 0; o < Bc; o += e->chunk) {
+        const int Bs = std::min(Bc - o, e->chunk), b = b0 + o;
+        PQ_TRY(encode_chunk(e, images + b * img_sz, u8, Bs, nullptr, nullptr, e->main, false));
+        PQ_TRY(vitstr_rows(e, Bs, L, e->main));
+        {
+          TimedScope ts(e, e->main, CAT_SCORE, 2.0 * Bs * L * e->C * D);
+          PQ_TRY(gemm_lse_launch(e->lo, e->xn, D, e->w("head.weight"), D, e->wf("head.bias"), Bs * L, e->C, D, nullptr,
+                                 e->sc_vt_part, nullptr, e->main));
+        }
+        const int m0 = first[b], nc = first[b + Bs] - m0;
+        TimedScope ts(e, e->main, CAT_SCORE, 0.0);
+        PQ_TRY(launch_k(e->lo, pq::score_reduce_kernel, dim3(static_cast<unsigned>(nc)), dim3(64), 0, e->main,
+                        static_cast<const float2*>(e->sc_vt_part), ntiles, static_cast<const float*>(nullptr),
+                        meta + vt_tgt_off + 1ll * m0 * L, meta + len_off, meta + vt_img_off, m0, b, L,
+                        static_cast<const __nv_bfloat16*>(e->xn), e->wb("head.weight"), e->wf("head.bias"), D, scores, token_lp, L));
+      }
+      continue;
+    }
+    for (int o = 0; o < Bc; o += e->chunk) {
+      const int Bs = std::min(Bc - o, e->chunk);
+      // kernel regime from the super-chunk, as forward_super: the memory bits equal the forward's
+      PQ_TRY(encode_chunk(e, images + (b0 + o) * img_sz, u8, Bs, e->mem + 1ll * o * T * D, nullptr, e->main, true, Bc));
+    }
+    PQ_TRY(cross_kv(e, Bc));
+    size_t g_end = gi;
+    while (g_end < groups.size() && groups[g_end].b_lo < b0 + Bc) ++g_end;
+    const int ns = static_cast<int>(e->stages.size());
+    const int used = static_cast<int>(std::min<size_t>(g_end - gi, static_cast<size_t>(ns)));
+    const bool fork = used > 1 && !e->timing;            // timing mode: everything on `main` (isolated kernel times)
+    if (fork) PQ_CUDA(cudaEventRecord(e->ev_enc, e->main));
+    for (int s = 0; s < used; ++s)
+      if (fork) PQ_CUDA(cudaStreamWaitEvent(e->stages[static_cast<size_t>(s)].stream, e->ev_enc, 0));
+    for (size_t k = gi; k < g_end; ++k) {
+      const ScoreGroup& g = groups[k];
+      parseq_engine::Stage& sg = e->stages[(k - gi) % static_cast<size_t>(ns)];
+      cudaStream_t ds = fork ? sg.stream : e->main;
+      const int B = g.m1 - g.m0;
+      const unsigned char* causal = e->sc_causal + 1ll * (g.P - 1) * L * L;
+      DecodeExtras ex;
+      ex.qmask = causal;
+      ex.cmask = e->cfg.dec_depth > 1 ? causal : nullptr;
+      ex.lse_tgt = meta + g.tgt_off;
+      sg.cand_off = meta + g.cand_off;
+      sg.cand_imgs = g.nimg;
+      sg.cand_max_rows = g.max_rows;
+      const int rc = decode_pass(e, sg, g.b_lo - b0, B, g.P, 0, g.P, 0, meta + g.ids_off, nullptr, 0, nullptr, 0, nullptr, 0,
+                                 nullptr, ds, &ex);
+      sg.cand_off = nullptr;
+      PQ_TRY(rc);
+      TimedScope ts(e, ds, CAT_SCORE, 0.0);
+      PQ_TRY(launch_k(e->lo, pq::score_reduce_kernel, dim3(static_cast<unsigned>(B)), dim3(64), 0, ds,
+                      static_cast<const float2*>(sg.lse_part), ntiles, static_cast<const float*>(sg.lse_tlogit),
+                      static_cast<const int*>(nullptr), meta + len_off, static_cast<const int*>(nullptr), g.m0, 0, g.P,
+                      static_cast<const __nv_bfloat16*>(nullptr), static_cast<const __nv_bfloat16*>(nullptr),
+                      static_cast<const float*>(nullptr), D, scores, token_lp, L));
+    }
+    if (fork) {
+      for (int s = 0; s < used; ++s) {
+        parseq_engine::Stage& sg = e->stages[static_cast<size_t>(s)];
+        PQ_CUDA(cudaEventRecord(sg.ev_done, sg.stream));
+        PQ_CUDA(cudaStreamWaitEvent(e->main, sg.ev_done, 0));
+      }
+    }
+    gi = g_end;
+  }
+  PQ_CUDA(cudaEventRecord(e->ev_out, e->main));
+  PQ_CUDA(cudaStreamWaitEvent(user, e->ev_out, 0));
+  return PARSEQ_OK;
+}
+
+// Shared checks of the score entry points: the counts first (a NULL handle is enough for them), then the handle, then
+// the targets against its configuration.
+int check_score_call(parseq_engine* e, const parseq_score_args* a, const void* images, const float* scores) {
+  PQ_TRY(check_score(a, -1, 0));
+  if (e == nullptr || images == nullptr || scores == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
+  if (!e->finalized) return fail(PARSEQ_ERR_STATE, "parseq_finalize has not been called after the last weight update");
+  return check_score(a, e->cfg.max_label_length, e->C);
 }
 
 }  // namespace
@@ -2057,6 +2366,27 @@ int parseq_forward_host_crops(parseq_engine* e, const parseq_forward_args* a, co
   PQ_TRY(forward_impl(e, a, nullptr, logits_host, ids_host, steps_host, reinterpret_cast<cudaStream_t>(stream), true, true, &cb));
   PQ_CUDA(cudaStreamSynchronize(e->main));
   return PARSEQ_OK;
+}
+
+int parseq_score_check(const parseq_config* cfg, const parseq_score_args* a) {
+  if (cfg == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  return check_score(a, cfg->max_label_length, cfg->num_tokens - 2);
+}
+
+int parseq_score(parseq_engine* e, const parseq_score_args* a, const float* images, float* scores, float* token_logprobs,
+                 parseq_stream_t stream) {
+  PQ_TRY(check_score_call(e, a, images, scores));
+  if (a->batch == 0) return PARSEQ_OK;
+  PQ_CUDA(cudaSetDevice(e->cfg.device));
+  return score_impl(e, a, images, false, scores, token_logprobs, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int parseq_score_u8(parseq_engine* e, const parseq_score_args* a, const uint8_t* images_hwc, float* scores, float* token_logprobs,
+                    parseq_stream_t stream) {
+  PQ_TRY(check_score_call(e, a, images_hwc, scores));
+  if (a->batch == 0) return PARSEQ_OK;
+  PQ_CUDA(cudaSetDevice(e->cfg.device));
+  return score_impl(e, a, images_hwc, true, scores, token_logprobs, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int parseq_postprocess(const float* logits, int32_t batch, int32_t num_steps, int32_t num_classes, int32_t eos_id, int32_t* ids,

@@ -21,6 +21,7 @@ enum GemmEpilogue : int {
   EPI_BF16 = 1,       // out_bf16 = bf16(alpha*(acc+bias))
   EPI_GELU_BF16 = 2,  // out_bf16 = bf16(gelu(acc+bias))
   EPI_F32_RESID = 3,  // kernel instantiation of EPI_F32 with a residual (the API's mode stays EPI_F32)
+  EPI_LSE = 4,        // no output tile: per-row log-sum-exp partials of the tile (gemm_lse_epilogue), candidate scoring
 };
 // How the kernel stores its tiles.  TMA: bf16 tiles go through a 128B-swizzled shared-memory staging tile and one
 // thread stores them with cp.async.bulk.tensor, 2D row-major or 3D column-blocked ([N/64][rows][64]); the tensor map's
@@ -40,6 +41,9 @@ struct GemmParams {
   int vec_ok;          // 8-byte aligned column pairs: paired stores allowed
   int num_m_tiles, num_n_tiles;
   int max_stages;      // 0: the full operand ring; n > 0: use only n slots (pipeline-depth experiments)
+  // EPI_LSE only: target class of each row (< 0: none) and where its logit goes; `out` holds the float2 partials
+  const int* lse_tgt;
+  float* lse_tlogit;
 };
 
 constexpr int GEMM_BLOCK_M = 128;  // rows per tile (two m64 halves, one warpgroup)
@@ -155,166 +159,65 @@ __device__ __forceinline__ void gemm_store_pair(const GemmParams& p, int row, in
   }
 }
 
+// EPI_LSE: the logits of a 128 x 128 tile stay in the accumulator registers.  For each row the tile leaves (max, sum of
+// exp(v - max)) over its columns < N in out[row * num_n_tiles + tile column] (float2), and the logit of the row's
+// target class, if that class is one of the tile's columns, in lse_tlogit[row].  v = (acc + bias) * alpha is the value
+// EPI_F32 stores, formed once per row into v[32].  Next to the 128 accumulators this costs a 48-byte stack frame (ptxas);
+// forming v twice instead (max pass, sum pass) has no spill but halved the epilogue's throughput (104-110 against
+// 238-250 TFLOP/s at 16384 classes, H100 80GB HBM3, 700 W), so v stays.  A tile whose max is -inf sums exp(v) instead,
+// so that it contributes 0, or NaN if it holds a NaN; NaN and +inf propagate through the sum as they do through torch's
+// log_softmax.  expf, not __expf: the partials carry fp32 rounding only.  The four lanes of a row (lane % 4) combine
+// with a fixed xor-shuffle order.
+__device__ __forceinline__ void gemm_lse_epilogue(const GemmParams& p, const float (&acc0)[64], const float (&acc1)[64],
+                                                  int m0, int n0, int r0, int lane) {
+  float2* part = reinterpret_cast<float2*>(p.out);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {        // (half, +8 rows)
+    const float* acc = (q < 2) ? acc0 : acc1;
+    const int row = m0 + 64 * (q >> 1) + r0 + 8 * (q & 1);
+    const int tgt = (row < p.M && p.lse_tgt != nullptr) ? __ldg(p.lse_tgt + row) : -1;
+    float v[32];
+    float mx = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < GEMM_BLOCK_N / 8; ++i) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = n0 + i * 8 + 2 * (lane & 3) + e;
+        const float b = (p.bias != nullptr && col < p.N) ? __ldg(p.bias + col) : 0.0f;
+        const float f = gemm_epi<EPI_F32>(acc[4 * i + 2 * (q & 1) + e], b, p.alpha);
+        v[2 * i + e] = col < p.N ? f : -INFINITY;
+        mx = fmaxf(mx, v[2 * i + e]);
+        if (col == tgt) p.lse_tlogit[row] = f;
+      }
+    }
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+    const float base = (mx == -INFINITY) ? 0.0f : mx;
+    float s = 0.0f;
+#pragma unroll
+    for (int k = 0; k < 32; ++k) s += expf(v[k] - base);
+    s += __shfl_xor_sync(0xffffffffu, s, 1);
+    s += __shfl_xor_sync(0xffffffffu, s, 2);
+    if ((lane & 3) == 0 && row < p.M)
+      part[static_cast<long long>(row) * p.num_n_tiles + n0 / GEMM_BLOCK_N] = make_float2(mx, s);
+  }
+}
+
+// The kernel body lives in gemm_body.inc, included by each kernel below with EPI and STORE in scope.
 template <int EPI, int STORE>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                        const __grid_constant__ CUtensorMap tmOut, const GemmParams p) {
-  constexpr bool TMA_OUT = STORE != ST_REG;
-  static_assert(!TMA_OUT || EPI == EPI_BF16 || EPI == EPI_GELU_BF16, "the TMA store carries bf16 tiles");
-  using Cfg = GemmCfg;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  const uint32_t pad = ((raw_addr + 1023u) & ~1023u) - raw_addr;
-  uint8_t* smem = smem_raw + pad;                         // 1024-B aligned (SWIZZLE_128B requirement)
-  uint8_t* out_stage = smem + Cfg::kStages * Cfg::kStageBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(out_stage + (TMA_OUT ? 2 * Cfg::kOutBytes : 0));
-  uint64_t* empty_bar = full_bar + Cfg::kStages;
+#include "gemm_body.inc"
+}
 
-  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
-  const int num_kb = (p.K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K;
-  const int nstages = (p.max_stages > 0 && p.max_stages < Cfg::kStages) ? p.max_stages : Cfg::kStages;
-  const int n_local = (num_tiles - 1 - static_cast<int>(blockIdx.x)) / static_cast<int>(gridDim.x) + 1;  // grid <= tiles
-
-  grid_dep_launch();                       // PDL: the next kernel may start its own prologue
-  if (threadIdx.x == 0) {
-    prefetch_tmap(&tmA);
-    prefetch_tmap(&tmB);
-    if constexpr (TMA_OUT) prefetch_tmap(&tmOut);
-    for (int s = 0; s < Cfg::kStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);         // a stage is read by one consumer warpgroup
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  grid_dep_wait();                         // PDL: inputs of this GEMM are complete and visible from here on
-
-  if (threadIdx.x < 128) {
-    // ===================== TMA producer: the CTA's tiles in order, running ahead across tiles =====================
-    setmaxnreg_dec<40>();
-    if (threadIdx.x == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int j = 0; j < n_local; ++j) {
-        const int tile = static_cast<int>(blockIdx.x) + j * static_cast<int>(gridDim.x);
-        const int m0 = (tile / p.num_n_tiles) * GEMM_BLOCK_M;
-        const int n0 = (tile % p.num_n_tiles) * GEMM_BLOCK_N;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait_mma(&empty_bar[stage], phase ^ 1u);
-          uint8_t* sa = smem + stage * Cfg::kStageBytes;
-          mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-          tma_load_2d(sa, &tmA, &full_bar[stage], kb * GEMM_BLOCK_K, m0);
-          tma_load_2d(sa + Cfg::kABytes, &tmB, &full_bar[stage], kb * GEMM_BLOCK_K, n0);
-          if (++stage == nstages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else {
-    // ===================== MMA warpgroup wg: the CTA's local tiles wg, wg + 2, ... =====================
-    setmaxnreg_inc<232>();
-    const int wg = (threadIdx.x >> 7) - 1;
-    const int t = threadIdx.x & 127;
-    const int lane = t & 31;
-    const int warp = t >> 5;
-    const bool leader = t == 0;
-    uint8_t* stage_out = out_stage + wg * Cfg::kOutBytes;
-    int stage = 0;
-    uint32_t phase = 0;
-    if (wg == 1) ring_advance(stage, phase, num_kb, nstages);     // local tile 0 belongs to warpgroup 0
-#pragma unroll 1
-    for (int j = wg; j < n_local; j += 2) {
-      const int tile = static_cast<int>(blockIdx.x) + j * static_cast<int>(gridDim.x);
-      const int m0 = (tile / p.num_n_tiles) * GEMM_BLOCK_M;
-      const int n0 = (tile % p.num_n_tiles) * GEMM_BLOCK_N;
-      // ordered main loops: wait until the other warpgroup has issued every MMA of local tile j - 1
-      if (j > 0) named_bar_sync(1 + wg, 256);
-      float acc0[64], acc1[64];            // rows [0, 64) and [64, 128) of the tile
-#pragma unroll
-      for (int i = 0; i < 64; ++i) { acc0[i] = 0.0f; acc1[i] = 0.0f; }
-      int prev = -1;
-#pragma unroll 1
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait_mma(&full_bar[stage], phase);
-        const uint32_t base = smem_u32(smem + stage * Cfg::kStageBytes);
-        const uint64_t da0 = make_desc_k_sw128(base);
-        const uint64_t da1 = make_desc_k_sw128(base + 64 * GEMM_BLOCK_K * 2);
-        const uint64_t db = make_desc_k_sw128(base + Cfg::kABytes);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) {
-          const uint32_t accum = static_cast<uint32_t>((kb | k) != 0);
-          wgmma_bf16<128>(acc0, da0 + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k), accum);
-          wgmma_bf16<128>(acc1, da1 + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k), accum);
-        }
-        wgmma_commit();
-        if (prev >= 0) {
-          wgmma_wait<1>();
-          if (leader) mbar_arrive(&empty_bar[prev]);
-        }
-        prev = stage;
-        if (++stage == nstages) { stage = 0; phase ^= 1u; }
-      }
-      if (j + 1 < n_local) named_bar_arrive(1 + (wg ^ 1), 256);   // the other warpgroup may start its main loop
-      wgmma_wait<0>();
-      wgmma_reg_fence(acc0);
-      wgmma_reg_fence(acc1);
-      if (leader) mbar_arrive(&empty_bar[prev]);
-      ring_advance(stage, phase, num_kb, nstages);                 // skip the other warpgroup's tile j + 1
-
-      // ---- epilogue.  Accumulator layout (ptx.cuh wgmma_bf16): acc_h[4i + {0,1}] = row 64h + 16 warp + lane/4,
-      // columns 8i + 2(lane%4) + {0,1}; acc_h[4i + {2,3}] = the same columns 8 rows further down.
-      const int r0 = 16 * warp + (lane >> 2);
-      if constexpr (TMA_OUT) {
-        // the previous TMA store of this warpgroup has finished reading the staging tile
-        if (leader) bulk_wait_group_read<0>();
-        named_bar_sync(3 + wg, 128);
-      }
-#pragma unroll
-      for (int i = 0; i < GEMM_BLOCK_N / 8; ++i) {
-        const int col = n0 + i * 8 + 2 * (lane & 3);
-        float b0 = 0.0f, b1 = 0.0f;
-        if (p.bias != nullptr) {
-          if (col < p.N) b0 = __ldg(p.bias + col);
-          if (col + 1 < p.N) b1 = __ldg(p.bias + col + 1);
-        }
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {        // (half, +8 rows)
-          const float* acc = (q < 2) ? acc0 : acc1;
-          const int rl = 64 * (q >> 1) + r0 + 8 * (q & 1);
-          const float f0 = gemm_epi<EPI>(acc[4 * i + 2 * (q & 1)], b0, p.alpha);
-          const float f1 = gemm_epi<EPI>(acc[4 * i + 2 * (q & 1) + 1], b1, p.alpha);
-          if constexpr (TMA_OUT) {
-            // 128B swizzle: 16-B chunk c of row r sits at chunk c ^ (r % 8); r % 8 = lane / 4 here
-            uint8_t* dst = stage_out + (i >> 3) * Cfg::kHalfOutBytes + rl * 128 + ((((i & 7) ^ (lane >> 2))) << 4) +
-                           (lane & 3) * 4;
-            *reinterpret_cast<uint32_t*>(dst) = pack_bf16(f0, f1);
-          } else {
-            const int row = m0 + rl;
-            if (row < p.M && col < p.N) gemm_store_pair<EPI>(p, row, col, f0, f1);
-          }
-        }
-      }
-      if constexpr (TMA_OUT) {
-        fence_proxy_async_smem();            // the staging writes are visible to the TMA (async proxy)
-        named_bar_sync(3 + wg, 128);
-        if (leader) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int c0 = n0 + 64 * h;
-            if (c0 >= p.N) break;
-            if constexpr (STORE == ST_TMA_3D) tma_store_3d(&tmOut, stage_out + h * Cfg::kHalfOutBytes, 0, m0, c0 / 64);
-            else tma_store_2d(&tmOut, stage_out + h * Cfg::kHalfOutBytes, c0, m0);
-          }
-          bulk_commit_group();
-        }
-      }
-    }
-    if constexpr (TMA_OUT) {
-      // the last stores have read their staging tile before the CTA's shared memory is released; their global writes
-      // are part of this grid's results, visible to the next kernel once the grid completes
-      if (leader) bulk_wait_group_read<0>();
-    }
-  }
+// The head GEMM of candidate scoring: the same body with the log-sum-exp epilogue (EPI_LSE, register path).  A kernel of
+// its own name rather than one more gemm_bf16_wgmma_kernel instantiation, which keeps that kernel's set unchanged.
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_bf16_lse_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                     const __grid_constant__ CUtensorMap tmOut, const GemmParams p) {
+  constexpr int EPI = EPI_LSE, STORE = ST_REG;
+#include "gemm_body.inc"
 }
 
 }  // namespace pq

@@ -791,6 +791,180 @@ __global__ void __launch_bounds__(128) dec_cross_attn3_kernel(const float* __res
   }
 }
 
+// Candidate scoring: the query rows of image b_first + j are rows [cand_off[j] * nq, cand_off[j + 1] * nq) (candidates
+// are image-major, nq rows each).  CTA (j * heads + h, y) stages the image's K/V of head h once and serves rows
+// [y * rows_per_cta, (y + 1) * rows_per_cta) of the image, grid.y covering the image with the most rows.  Apart from
+// that row mapping this is dec_cross_attn3_kernel line for line (kept separate so that the existing kernel's code is
+// untouched), so every row is computed as there and its bits do not depend on how many candidates share its image.
+template <int NR>
+__global__ void __launch_bounds__(128) dec_cross_attn3_grouped_kernel(const float* __restrict__ q,
+                                                                      const __nv_bfloat16* __restrict__ kv, long long kv_rows,
+                                                                      int b_first, int T, int D, int heads, int nq,
+                                                                      const int* __restrict__ cand_off, int rows_per_cta,
+                                                                      __nv_bfloat16* __restrict__ out) {
+  constexpr int TK = 32 * NR;
+  __shared__ uint32_t sK[TK * 17];                        // bf16x2 words, pitch 17 (odd)
+  __shared__ __align__(16) __nv_bfloat16 sV[TK * 32];
+  grid_dep_launch();
+  grid_dep_wait();
+  const int b = blockIdx.x / heads, h = blockIdx.x % heads;
+  const long long row0 = static_cast<long long>(cand_off[b]) * nq;
+  const int rows = (cand_off[b + 1] - cand_off[b]) * nq;
+  const int q_begin = static_cast<int>(blockIdx.y) * rows_per_cta;
+  if (q_begin >= rows) return;
+  const int q_end = q_begin + rows_per_cta < rows ? q_begin + rows_per_cta : rows;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const long long row_b = static_cast<long long>(b_first + b) * T;
+  for (int t = tid; t < TK; t += 128) {
+    uint4* vd = reinterpret_cast<uint4*>(sV + t * 32);
+    if (t < T) {
+      const uint4* kr = reinterpret_cast<const uint4*>(kv + blocked_off(kv_rows, row_b + t, h * 32));
+      const uint4* vr = reinterpret_cast<const uint4*>(kv + blocked_off(kv_rows, row_b + t, D + h * 32));
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint4 u = __ldg(kr + j);
+        sK[t * 17 + j * 4 + 0] = u.x; sK[t * 17 + j * 4 + 1] = u.y;
+        sK[t * 17 + j * 4 + 2] = u.z; sK[t * 17 + j * 4 + 3] = u.w;
+        vd[j] = __ldg(vr + j);
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 16; ++j) sK[t * 17 + j] = 0u;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) vd[j] = make_uint4(0u, 0u, 0u, 0u);
+    }
+  }
+  __syncthreads();
+  for (int qi = q_begin + warp; qi < q_end; qi += 4) {
+    const long long row = row0 + qi;
+    const float qv = q[row * D + h * 32 + lane];          // lane j holds q_j
+    float sc[NR];
+#pragma unroll
+    for (int r = 0; r < NR; ++r) sc[r] = 0.f;
+#pragma unroll
+    for (int w = 0; w < 16; ++w) {
+      const float qa = __shfl_sync(0xffffffffu, qv, 2 * w), qb = __shfl_sync(0xffffffffu, qv, 2 * w + 1);
+#pragma unroll
+      for (int r = 0; r < NR; ++r) {
+        const uint32_t kw = sK[(r * 32 + lane) * 17 + w];
+        sc[r] = fmaf(qb, __uint_as_float(kw & 0xffff0000u), fmaf(qa, __uint_as_float(kw << 16), sc[r]));
+      }
+    }
+    float mx = -INFINITY;
+#pragma unroll
+    for (int r = 0; r < NR; ++r) {
+      if (r * 32 + lane >= T) sc[r] = -INFINITY;
+      mx = fmaxf(mx, sc[r]);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    float sum = 0.f;
+#pragma unroll
+    for (int r = 0; r < NR; ++r) {
+      sc[r] = expf(sc[r] - mx);
+      sum += sc[r];
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    // P.V with 16-byte smem reads: lane = (key group kg = lane>>2, 8-channel chunk cc = lane&3); 4*NR iterations cover
+    // the keys; the 8 key groups are then summed with xor-shuffles and lanes 0..3 hold the 32 output channels.
+    const int kg = lane >> 2, cc = lane & 3;
+    float o[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) o[j] = 0.f;
+#pragma unroll
+    for (int it = 0; it < 4 * NR; ++it) {              // key = it*8 + kg -> register sc[it>>2], source lane (it&3)*8 + kg
+      const int key = it * 8 + kg;
+      const uint4 vvv = *reinterpret_cast<const uint4*>(sV + key * 32 + cc * 8);
+      const float pk = __shfl_sync(0xffffffffu, sc[it >> 2], (it & 3) * 8 + kg);
+      const __nv_bfloat162* p2 = reinterpret_cast<const __nv_bfloat162*>(&vvv);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 f = __bfloat1622float2(p2[e]);
+        o[e * 2] = fmaf(pk, f.x, o[e * 2]);
+        o[e * 2 + 1] = fmaf(pk, f.y, o[e * 2 + 1]);
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      o[j] += __shfl_xor_sync(0xffffffffu, o[j], 4);
+      o[j] += __shfl_xor_sync(0xffffffffu, o[j], 8);
+      o[j] += __shfl_xor_sync(0xffffffffu, o[j], 16);
+    }
+    if (kg == 0) {
+      const float inv = 1.0f / sum;
+      uint4 q4;
+      q4.x = pack_bf16(o[0] * inv, o[1] * inv); q4.y = pack_bf16(o[2] * inv, o[3] * inv);
+      q4.z = pack_bf16(o[4] * inv, o[5] * inv); q4.w = pack_bf16(o[6] * inv, o[7] * inv);
+      *reinterpret_cast<uint4*>(out + row * D + h * 32 + cc * 8) = q4;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Candidate scoring, last step: one CTA per candidate m, thread i = position i <= n_m (n_m = lengths[m]).  The term of
+// position i is log_softmax(logits row)[t_i] = (t - M) - log(S), with M, S the merge of the row's per-tile partials
+// (gemm_lse_epilogue) in column order: M = max of the tile maxima, S = sum of s_j exp(m_j - M).  The candidate's score is
+// the sum of its terms in position order (thread 0).  Rows: the partial row of (m, i) is prow_m * P + i with prow_m =
+// m - m0 (PARSeq: rows are (candidate, position)) or cand_img[m] - img0 (ViTSTR: rows are (image, position), shared by
+// the image's candidates); the target logit is tlogit[(m - m0) * P + i], or, with xn != null (ViTSTR), the dot product
+// of the bf16 row xn[prow] with the bf16 head row W[t] plus bias[t]: warp w takes positions w, w + 2, ..., its lanes
+// read both rows as bf16 pairs (coalesced) and sum in fp32 with a fixed xor-shuffle order.  token_lp (may be null):
+// [M][L] terms, 0 past n_m.
+// No early griddepcontrol.launch_dependents: the next kernel on the stream (the next group of candidates, which
+// rewrites the chain's LayerNorm, partial and target-logit buffers) may start only once this grid has exited, and this
+// grid's wait orders it after the head GEMM that wrote what it reads.
+__global__ void __launch_bounds__(64) score_reduce_kernel(const float2* __restrict__ part, int ntiles,
+                                                          const float* __restrict__ tlogit, const int* __restrict__ tgt,
+                                                          const int* __restrict__ lengths, const int* __restrict__ cand_img,
+                                                          int m0, int img0, int P, const __nv_bfloat16* __restrict__ xn,
+                                                          const __nv_bfloat16* __restrict__ W, const float* __restrict__ bias,
+                                                          int D, float* __restrict__ scores, float* __restrict__ token_lp,
+                                                          int L) {
+  __shared__ float s_term[64];
+  __shared__ float s_tl[64];
+  grid_dep_wait();
+  const int m = m0 + static_cast<int>(blockIdx.x), i = threadIdx.x;
+  const int n = lengths[m];
+  const long long prow0 = static_cast<long long>(cand_img != nullptr ? cand_img[m] - img0 : m - m0) * P;
+  const long long trow0 = static_cast<long long>(m - m0) * P;
+  if (xn != nullptr) {
+    const int warp = i >> 5, lane = i & 31;
+    for (int k = warp; k <= n; k += 2) {
+      const int c = tgt[trow0 + k];
+      const __nv_bfloat162* x = reinterpret_cast<const __nv_bfloat162*>(xn + (prow0 + k) * D);
+      const __nv_bfloat162* w = reinterpret_cast<const __nv_bfloat162*>(W + static_cast<long long>(c) * D);
+      float t = 0.0f;
+      for (int j = lane; j < D / 2; j += 32) {
+        const float2 a = __bfloat1622float2(x[j]), b = __bfloat1622float2(w[j]);
+        t = fmaf(a.y, b.y, fmaf(a.x, b.x, t));
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+      if (lane == 0) s_tl[k] = t + bias[c];
+    }
+    __syncthreads();
+  }
+  float term = 0.0f;
+  if (i <= n) {
+    const float2* pr = part + (prow0 + i) * ntiles;
+    float M = -INFINITY;
+    for (int j = 0; j < ntiles; ++j) M = fmaxf(M, pr[j].x);
+    float S = 0.0f;
+    for (int j = 0; j < ntiles; ++j) S += pr[j].y * expf(pr[j].x - M);
+    const float t = xn != nullptr ? s_tl[i] : tlogit[trow0 + i];
+    term = (t - M) - logf(S);
+  }
+  if (token_lp != nullptr && i < L) token_lp[static_cast<long long>(m) * L + i] = term;
+  s_term[i] = term;
+  __syncthreads();
+  if (i == 0) {
+    float s = 0.0f;
+    for (int k = 0; k <= n; ++k) s += s_term[k];
+    scores[m] = s;
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // ViTSTR (vitstr/model.py:14-28 over timm VisionTransformer._pos_embed): token 0 of every image is
 // cls_token + pos_embed[0]; tokens 1..Tp are the patch embeddings (pos_embed[1..Tp] already added by the patch GEMM).

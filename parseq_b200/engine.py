@@ -29,10 +29,16 @@ class CropsC(C.Structure):
                 ("rotation", C.c_int32)]
 
 
+class ScoreArgsC(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("num_candidates", C.c_int32), ("per_image", C.c_void_p), ("targets", C.c_void_p),
+                ("lengths", C.c_void_p)]
+
+
 EXPORTS = [
     "parseq_create", "parseq_destroy", "parseq_set_weight", "parseq_num_weights", "parseq_weight_key",
     "parseq_finalize", "parseq_forward", "parseq_forward_host", "parseq_forward_u8", "parseq_forward_host_u8",
     "parseq_resize_crops", "parseq_forward_crops", "parseq_forward_host_crops",
+    "parseq_score", "parseq_score_u8", "parseq_score_check",
     "parseq_postprocess", "parseq_encode", "parseq_decode", "parseq_decode_ex", "parseq_head", "parseq_text_embed", "parseq_kernel_launches", "parseq_debug_int", "parseq_bench_tma_stream",
     "parseq_set_option", "parseq_get_timing", "parseq_get_ar_profile", "parseq_last_error", "parseq_version", "parseq_gemm_bf16", "parseq_gemm_ln_bf16", "parseq_mlp_ln_bf16", "parseq_layernorm_bf16",
     "parseq_enc_attention", "parseq_qkv_attention_bf16",
@@ -72,6 +78,9 @@ def load_library(path: Optional[str] = None):
     lib.parseq_forward_crops.argtypes = [C.c_void_p, C.POINTER(ForwardArgsC), C.POINTER(CropsC), C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p]
     lib.parseq_forward_host_crops.argtypes = lib.parseq_forward_crops.argtypes
+    lib.parseq_score.argtypes = [C.c_void_p, C.POINTER(ScoreArgsC), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.parseq_score_u8.argtypes = lib.parseq_score.argtypes
+    lib.parseq_score_check.argtypes = [C.POINTER(ParseqConfigC), C.POINTER(ScoreArgsC)]
     lib.parseq_postprocess.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p]
     lib.parseq_encode.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -110,16 +119,20 @@ def check(lib, rc: int):
         raise EngineError(f"parseq_b200 error {rc}: {lib.parseq_last_error().decode()}")
 
 
+def config_c(cfg, device: int = 0, max_batch: int = 0) -> ParseqConfigC:
+    return ParseqConfigC(cfg.img_size[0], cfg.img_size[1], cfg.patch_size[0], cfg.patch_size[1], cfg.embed_dim,
+                         cfg.enc_num_heads, cfg.enc_mlp_ratio, cfg.enc_depth, cfg.dec_num_heads, cfg.dec_mlp_ratio,
+                         cfg.dec_depth, cfg.max_label_length, cfg.num_tokens, max_batch, device,
+                         1 if getattr(cfg, "arch", "parseq") == "vitstr" else 0)
+
+
 class Engine:
     """Owns one `parseq_engine*`."""
 
     def __init__(self, cfg, device: int = 0, max_batch: int = 0):
         self.lib = load_library()
         self.cfg = cfg
-        c = ParseqConfigC(cfg.img_size[0], cfg.img_size[1], cfg.patch_size[0], cfg.patch_size[1], cfg.embed_dim,
-                          cfg.enc_num_heads, cfg.enc_mlp_ratio, cfg.enc_depth, cfg.dec_num_heads, cfg.dec_mlp_ratio,
-                          cfg.dec_depth, cfg.max_label_length, cfg.num_tokens, max_batch, device,
-                          1 if getattr(cfg, "arch", "parseq") == "vitstr" else 0)
+        c = config_c(cfg, device, max_batch)
         h = C.c_void_p()
         check(self.lib, self.lib.parseq_create(C.byref(c), C.byref(h)))
         self.handle = h
@@ -162,7 +175,8 @@ class Engine:
     def set_option(self, name: str, value: int):
         check(self.lib, self.lib.parseq_set_option(self.handle, name.encode(), int(value)))
 
-    TIMING_CATEGORIES = ("enc_gemm", "enc_attn", "layernorm", "dec_gemm", "dec_attn", "other", "enc_gemm_ln", "dec_ar")
+    TIMING_CATEGORIES = ("enc_gemm", "enc_attn", "layernorm", "dec_gemm", "dec_attn", "other", "enc_gemm_ln", "dec_ar",
+                         "score_tail")
 
     def get_timing(self):
         out = {}
@@ -220,6 +234,12 @@ class Engine:
         a = self._args(batch, max_length, decode_ar, refine_iters, class_mask=class_mask_ptr)
         fn = self.lib.parseq_forward_host_crops if host else self.lib.parseq_forward_crops
         check(self.lib, fn(self.handle, C.byref(a), C.byref(crops), logits_ptr, ids_ptr, steps_ptr, stream))
+
+    # per_image / targets / lengths: CPU int32 tensors (parseq_score_args); scores / token_lp: device pointers
+    def score(self, images_ptr, batch, per_image, targets, lengths, scores_ptr, token_lp_ptr, stream, u8=False):
+        a = ScoreArgsC(batch, int(targets.shape[0]), per_image.data_ptr(), targets.data_ptr(), lengths.data_ptr())
+        fn = self.lib.parseq_score_u8 if u8 else self.lib.parseq_score
+        check(self.lib, fn(self.handle, C.byref(a), images_ptr, scores_ptr, token_lp_ptr, stream))
 
     def postprocess(self, logits_ptr, batch, num_steps, ids_ptr, lengths_ptr, conf_ptr, stream, eos_id=0):
         check(self.lib, self.lib.parseq_postprocess(logits_ptr, batch, num_steps, self.cfg.num_classes, eos_id, ids_ptr,

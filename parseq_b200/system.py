@@ -143,6 +143,50 @@ def allowlist_mask(tokenizer: Tokenizer, allowlist: Allowlist, batch: int, num_c
     return torch.where(packed >= 1 << 31, packed - (1 << 32), packed).to(torch.int32)
 
 
+Candidates = Union[Sequence[str], Sequence[Sequence[str]]]
+
+
+def pack_candidates(tokenizer: Tokenizer, candidates: Candidates, batch: int, max_label_length: int,
+                    num_classes: int) -> Tuple[Tensor, Tensor, Tensor]:
+    """The candidate labels of a score call as the engine takes them (parseq_score_args): CPU int32 targets
+    [M, max_label_length + 1] = (c_1..c_n, EOS, 0...), lengths [M] and per_image [batch].  `candidates` is one list of
+    strings for every image (a lexicon) or one non-empty list per image; candidates are image-major."""
+    if isinstance(candidates, str) or not isinstance(candidates, (list, tuple)) or len(candidates) == 0:
+        raise TypeError("candidates must be a non-empty list of strings, or one non-empty list of strings per image")
+    shared = all(isinstance(c, str) for c in candidates)
+    if shared:
+        rows: List[Sequence[str]] = [candidates] * batch
+    else:
+        rows = list(candidates)
+        if len(rows) != batch:
+            raise ValueError(f"candidates has {len(rows)} lists for {batch} images")
+        for b, r in enumerate(rows):
+            if isinstance(r, str) or not isinstance(r, (list, tuple)) or len(r) == 0 or not all(isinstance(s, str) for s in r):
+                raise TypeError(f"candidates of image {b} must be a non-empty list of strings")
+    words = sorted(set(candidates) if shared else {s for r in rows for s in r})
+    unknown = sorted({ch for s in words for ch in s
+                      if ch not in tokenizer._stoi or not 1 <= tokenizer._stoi[ch] < num_classes})
+    if unknown:
+        raise ValueError(f"candidate characters not in charset_train: {''.join(unknown)!r}")
+    too_long = [s for s in words if len(s) > max_label_length]
+    if too_long:
+        raise ValueError(f"candidate {too_long[0]!r} has {len(too_long[0])} characters, more than max_label_length = "
+                         f"{max_label_length}")
+    # one target row per distinct word, then a gather: a lexicon shared by 512 images costs one row per word
+    L = max_label_length + 1
+    index = {s: i for i, s in enumerate(words)}
+    table = torch.zeros((len(words), L), dtype=torch.int32)
+    for s, i in index.items():
+        table[i, :len(s) + 1] = torch.tensor(tokenizer._tok2ids(s) + [tokenizer.eos_id], dtype=torch.int32)
+    word_len = torch.tensor([len(s) for s in words], dtype=torch.int32)
+    if shared:
+        pick = torch.tensor([index[s] for s in candidates], dtype=torch.long).repeat(batch)
+    else:
+        pick = torch.tensor([index[s] for r in rows for s in r], dtype=torch.long)
+    per_image = torch.tensor([len(r) for r in rows], dtype=torch.int32)
+    return table[pick], word_len[pick], per_image
+
+
 def _mask_ptr(mask: Optional[Tensor]):
     return mask.data_ptr() if mask is not None else None
 
@@ -301,6 +345,35 @@ class _EngineModule(nn.Module):
         eng.resize_crops(_crops_c(data, offsets, sizes, rotation), len(crops), out.data_ptr(),
                          torch.cuda.current_stream(dev).cuda_stream)
         return out
+
+    def score(self, images: Union[Tensor, List[Any]], targets: Tensor, lengths: Tensor, per_image: Tensor, *,
+              rotation: int = 0, return_token_logprobs: bool = False):
+        """Log-likelihoods of candidate labels (parseq_score): `targets` int32 [M, max_label_length + 1] (c_1..c_n, EOS),
+        `lengths` [M], `per_image` [N] as pack_candidates makes them (CPU).  Returns fp32 scores [M] on the device, and
+        with return_token_logprobs the per-position terms [M, max_label_length + 1] (0 past each label's EOS).
+        `images` as forward takes them; raw crops are resized on the device first (preprocess)."""
+        eng = self.engine()
+        if isinstance(images, (list, tuple)):
+            images = self.preprocess(images, rotation)
+        elif rotation:
+            raise ValueError("rotation applies to lists of raw crops; a tensor input is already at img_size")
+        images = self._check_images(images)
+        dev = images.device
+        L = self.cfg.max_label_length + 1
+        targets = targets.to(device="cpu", dtype=torch.int32).contiguous()
+        lengths = lengths.to(device="cpu", dtype=torch.int32).contiguous()
+        per_image = per_image.to(device="cpu", dtype=torch.int32).contiguous()
+        if targets.dim() != 2 or targets.shape[1] != L or lengths.shape != (targets.shape[0],):
+            raise ValueError(f"targets must be int32 [M, {L}] and lengths [M]")
+        if per_image.shape != (images.shape[0],):
+            raise ValueError(f"per_image must have one entry per image ({images.shape[0]})")
+        M = targets.shape[0]
+        scores = torch.empty((M,), dtype=torch.float32, device=dev)
+        tlp = torch.empty((M, L), dtype=torch.float32, device=dev) if return_token_logprobs else None
+        eng.score(images.data_ptr(), images.shape[0], per_image, targets, lengths, scores.data_ptr(),
+                  tlp.data_ptr() if tlp is not None else None, torch.cuda.current_stream(dev).cuda_stream,
+                  u8=images.dtype == torch.uint8)
+        return (scores, tlp) if return_token_logprobs else scores
 
     def _run_crops(self, crops, max_length, decode_ar, refine_iters, rotation, class_mask=None):
         """Raw crops of any size: CUDA crops run parseq_forward_crops and return CUDA tensors; CPU crops and PIL images
@@ -502,6 +575,50 @@ class _System(nn.Module):
         ids_h, len_h, conf_h = ids.cpu().tolist(), lengths.cpu().tolist(), conf.cpu().tolist()
         labels = [self.tokenizer._ids2tok(row[:n], True) for row, n in zip(ids_h, len_h)]
         return labels, conf_h
+
+    def score(self, images: Union[Tensor, List[Any]], candidates: Candidates, *, rotation: int = 0,
+              return_token_logprobs: bool = False):
+        """Log-likelihood of each candidate label for each image: fp32 [N, Kmax], -inf past an image's own candidates.
+        PARSeq: sum over i = 0..n of log_softmax(head(decode(...)))[i, t_i] under the canonical left-to-right masks, with
+        targets t = (c_1..c_n, EOS) - minus the summed cross-entropy of permutation 0 of the reference's training_step.
+        ViTSTR: the same sum over its per-token logits.  `candidates`: one list of strings for every image (a lexicon),
+        or one non-empty list per image.  With return_token_logprobs also the terms [N, Kmax, max_label_length + 1]
+        (0 past each label's EOS and past an image's candidates).  `images` as forward takes them; the result is on
+        the images' device (CPU for CPU crops)."""
+        N = len(images) if isinstance(images, (list, tuple)) else images.shape[0]
+        cfg = self.model.cfg
+        targets, lengths, per_image = pack_candidates(self.tokenizer, candidates, N, cfg.max_label_length, cfg.num_classes)
+        out = self.model.score(images, targets, lengths, per_image, rotation=rotation,
+                               return_token_logprobs=return_token_logprobs)
+        scores, tlp = out if return_token_logprobs else (out, None)
+        K = int(per_image.max())
+        dev = scores.device
+        img = torch.repeat_interleave(torch.arange(N), per_image.long())
+        col = torch.arange(len(img)) - torch.repeat_interleave(torch.cumsum(per_image.long(), 0) - per_image.long(),
+                                                                per_image.long())
+        idx = (img * K + col).to(dev)
+        grid = torch.full((N * K,), float("-inf"), dtype=torch.float32, device=dev)
+        grid[idx] = scores
+        if isinstance(images, (list, tuple)) and all(not (isinstance(c, Tensor) and c.is_cuda) for c in images):
+            dev = torch.device("cpu")
+        grid = grid.view(N, K).to(dev)
+        if not return_token_logprobs:
+            return grid
+        L = cfg.max_label_length + 1
+        terms = torch.zeros((N * K, L), dtype=torch.float32, device=tlp.device)
+        terms[idx] = tlp
+        return grid, terms.view(N, K, L).to(dev)
+
+    def lexicon_decode(self, images: Union[Tensor, List[Any]], lexicon: Candidates, *, rotation: int = 0):
+        """Lexicon-constrained recognition: for each image the candidate the model rates most likely (score), as
+        (labels, log_probs).  The pick is torch.argmax of the image's scores: the first maximum, or the first NaN."""
+        scores = self.score(images, lexicon, rotation=rotation)
+        N = scores.shape[0]
+        rows = [lexicon] * N if all(isinstance(c, str) for c in lexicon) else list(lexicon)
+        best = scores.argmax(-1)
+        best_h = best.tolist()
+        labels = [rows[b][k] for b, k in enumerate(best_h)]
+        return labels, scores.gather(1, best[:, None])[:, 0]
 
     # base.py:112-143,179-180 (test path only; validation loss is a training concern)
     def _eval_step(self, batch, validation: bool = False):

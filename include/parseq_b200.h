@@ -168,6 +168,34 @@ int parseq_score_u8(parseq_engine* e, const parseq_score_args* a, const uint8_t*
 /* The host checks of parseq_score against a configuration, without a handle or a device. */
 int parseq_score_check(const parseq_config* cfg, const parseq_score_args* a);
 
+/* Beam search: the K most likely readings of each image with their log-likelihoods (the quantity parseq_score computes).
+ * One search per image, beam width K, over num_steps = min(max_length, max_label_length) + 1 positions:
+ *   - K slots per image; slot 0 starts as [BOS] with score 0, the others empty (score -inf).
+ *   - Step i: every active slot runs the AR step at query position i over its own prefix (model.py:124-142 for one row).
+ *     Over the allowed classes of its logits row, LSE = log-sum-exp (NaN if one is NaN or +inf); a class's term is logit - LSE (fp32) and a child's
+ *     score is parent + term.  The slot expands its K best classes in the row order: NaN logits first (lowest class
+ *     first), then logit descending, ties to the lower class.  Classes the allowlist masks or whose logit is -inf never
+ *     expand.
+ *   - A child that takes EOS is finished with its length n; one that reaches num_steps characters without EOS is finished
+ *     with num_steps characters.  A finished slot is carried unchanged into every later pool.
+ *   - The pool, in slot order, holds each finished slot and each active slot's expansions in row order; the K best by
+ *     score are kept by a stable sort (NaN after every number; -inf never kept).  They are the next step's slots.
+ * PARSeq runs the AR decoder whatever decode_ar / refine_iters say and never refines; ViTSTR applies the same rule to its
+ * per-position logits head(norm(x))[:, 1:] (the row of step i is the image's position-i row for every slot).  With K = 1
+ * the ids through the first EOS are the greedy AR ids.  Runs eagerly (no CUDA graph); the first call allocates the beam
+ * buffers.  Arguments are checked on the host before anything is launched (PARSEQ_ERR_INVALID_ARG). */
+typedef struct parseq_beam_args {
+  int32_t batch, beam_width, max_length;   /* 1 <= beam_width <= 16 (PARSeq: and <= option dec_chunk); max_length -1 = None */
+  const uint32_t* class_mask;              /* DEVICE allowlist rows as parseq_forward_args.class_mask, or NULL */
+} parseq_beam_args;
+/* images as parseq_forward / parseq_forward_u8 take them; all outputs DEVICE, hypotheses best first:
+ * ids int32 [N][K][num_steps] = c_1..c_n, then 0 (EOS / padding); lengths int32 [N][K] = n, -1 for a missing hypothesis;
+ * scores fp32 [N][K], -inf for a missing hypothesis (e.g. allowlist "": the only reading is "" with score 0). */
+int parseq_beam_search(parseq_engine* e, const parseq_beam_args* a, const float* images, int32_t* ids, int32_t* lengths,
+                       float* scores, parseq_stream_t stream);
+int parseq_beam_search_u8(parseq_engine* e, const parseq_beam_args* a, const uint8_t* images_hwc, int32_t* ids,
+                          int32_t* lengths, float* scores, parseq_stream_t stream);
+
 /* Fused post-processing of BaseSystem._eval_step (strhub/models/base.py:132-142) + Tokenizer._filter
  * (strhub/data/utils.py:120-129): DEVICE logits [N, num_steps, num_classes] -> ids [N, num_steps] (greedy), lengths [N]
  * (index of the first EOS, num_steps if none) and confidence [N] (product of the max softmax probabilities up to and
@@ -211,7 +239,8 @@ int parseq_bench_tma_stream(void* buf, int64_t bytes, int cluster, int ctas, int
  * cluster AR kernel instantiation: "ar_last_cluster_size", "ar_last_mt", "ar_last_head_split", "ar_last_wide",
  * "ar_last_ids_pitch"; "ar_last_path": the AR loop of the last PARSeq forward, 0 the chain of separate kernels, 1 the
  * grid-barrier kernel, 2 the cluster kernel, -1 no AR loop; "ln_clusters": the clusters the persistent GEMM + LayerNorm
- * kernel runs on, 0 before its first launch, also with e = NULL for the bare kernel exports); -1 if unknown. */
+ * kernel runs on, 0 before its first launch, also with e = NULL for the bare kernel exports; "beam_bytes": device bytes of
+ * the beam-search buffers, 0 until the first parseq_beam_search call); -1 if unknown. */
 int64_t parseq_debug_int(parseq_engine* e, const char* name);
 /* Options: "max_batch" (images per super-chunk = one CUDA graph), "chunk" (images per encoder pass inside a
  * super-chunk), "dec_chunk" (images per decoder chain; the chains of a super-chunk run concurrently on their own
@@ -233,7 +262,8 @@ int parseq_set_option(parseq_engine* e, const char* name, int64_t value);
 /* After a synchronised forward with "timing"=1: device milliseconds, algorithmic FLOPs and launch count of
  * category 0 encoder GEMM, 1 encoder attention, 2 LayerNorm, 3 decoder GEMM, 4 decoder attention, 5 other,
  * 6 encoder residual GEMM fused with LayerNorm, 7 persistent AR-loop kernel, 8 scoring tail (head GEMM with the log-sum-exp
- * epilogue and the per-candidate reduce of parseq_score). */
+ * epilogue and the per-candidate reduce of parseq_score), 9 beam selection (the selection kernel and, at dec_depth >= 2,
+ * the K/V cache gather of parseq_beam_search). */
 int parseq_get_timing(parseq_engine* e, int category, double* ms, double* flops, int64_t* count);
 /* Debug: after a forward with option "ar_prof"=1, copies the [32 steps][16 slots] globaltimer (ns) stamps that block 0 of
  * the persistent AR kernel recorded at its phase boundaries.  Row 26 holds extra stamps of step 1 of the cluster kernel;

@@ -313,6 +313,7 @@ int init_kernel_attributes() {
   PQ_TRY((gemm_attr<pq::EPI_GELU_BF16, pq::ST_REG>()));
   PQ_TRY((gemm_attr<pq::EPI_GELU_BF16, pq::ST_TMA_2D>()));
   PQ_TRY(set_smem(pq::gemm_bf16_lse_kernel, pq::GemmCfg::smem_bytes<false>()));
+  PQ_TRY(set_smem(pq::gemm_bf16_topk_kernel, pq::GemmCfg::smem_bytes<false>()));
   PQ_TRY(set_smem(pq::tma_stream_bench_kernel, kTmaBenchSmem));
   int dev = 0, optin = 0;
   PQ_CUDA(cudaGetDevice(&dev));
@@ -406,6 +407,31 @@ int gemm_lse_launch(LaunchOpts& lo, const void* A, long long lda, const void* W,
   p.lse_tlogit = tlogit;
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   return launch_k(lo, pq::gemm_bf16_lse_kernel, dim3(static_cast<unsigned>(tiles < lo.sm_count ? tiles : lo.sm_count)),
+                  dim3(pq::GEMM_THREADS), pq::GemmCfg::smem_bytes<false>(), st, ta, tb, ta, p);
+}
+
+// The head GEMM with the top-K epilogue (gemm.cuh, gemm_bf16_topk_kernel): per row and 128-column tile the (max, sum exp)
+// partial of the allowed classes in part[M][ceil(N / 128)] and the tile's k best keys in keys[M][ceil(N / 128)][16];
+// allowlist row of row r: mask + (r / mask_div) * ceil(N / 32), or no mask
+int gemm_topk_launch(LaunchOpts& lo, const void* A, long long lda, const void* W, long long ldw, const float* bias, int M, int N,
+                     int K, int k, const uint32_t* mask, int mask_div, float2* part, unsigned long long* keys, cudaStream_t st) {
+  if (M <= 0 || N <= 0 || K <= 0) return fail(PARSEQ_ERR_INVALID_ARG, "gemm: empty problem");
+  PQ_TRY(ensure_sm_count(lo));
+  CUtensorMap ta, tb;
+  PQ_TRY(make_tmap(&ta, A, 2, M, K, lda, pq::GEMM_BLOCK_K, pq::GEMM_BLOCK_M));
+  PQ_TRY(make_tmap(&tb, W, 2, N, K, ldw, pq::GEMM_BLOCK_K, pq::GEMM_BLOCK_N));
+  pq::GemmParams p{};
+  p.M = M; p.N = N; p.K = K; p.alpha = 1.0f; p.bias = bias;
+  p.out = part;
+  p.max_stages = lo.gemm_stages;
+  p.num_m_tiles = (M + pq::GEMM_BLOCK_M - 1) / pq::GEMM_BLOCK_M;
+  p.num_n_tiles = (N + pq::GEMM_BLOCK_N - 1) / pq::GEMM_BLOCK_N;
+  p.topk_keys = keys;
+  p.topk_k = k;
+  p.topk_mask = mask;
+  p.topk_mask_div = mask_div;
+  const int tiles = p.num_m_tiles * p.num_n_tiles;
+  return launch_k(lo, pq::gemm_bf16_topk_kernel, dim3(static_cast<unsigned>(tiles < lo.sm_count ? tiles : lo.sm_count)),
                   dim3(pq::GEMM_THREADS), pq::GemmCfg::smem_bytes<false>(), st, ta, tb, ta, p);
 }
 
@@ -627,6 +653,23 @@ struct parseq_engine {
     float* lse_tlogit = nullptr;
     const int* cand_off = nullptr;
     int cand_imgs = 0, cand_max_rows = 0;
+    // beam search (parseq_beam_search), allocated by the first beam call: double-buffered state of `rows` beam rows
+    // (ids [rows][ids_ld], score, len, st; kernels.cuh beam_select_kernel), the parent row of each new beam, what the
+    // head leaves of one step's rows (ViTSTR: of `rows / BEAM_MAX` images' positions) - the logits at <= 128 classes, the
+    // top-K epilogue's partials and keys above - and at depth >= 2 a second content K/V cache per layer that the parents'
+    // rows are gathered into
+    struct Beam {
+      int rows = 0;
+      int* ids[2] = {nullptr, nullptr};
+      float* score[2] = {nullptr, nullptr};
+      int* len[2] = {nullptr, nullptr};
+      int* st[2] = {nullptr, nullptr};
+      int* parent = nullptr;
+      float* logits = nullptr;              // <= 128 classes: the step's logits
+      float2* part = nullptr;               // > 128 classes: the top-K epilogue's LSE partials [lrows][ceil(C / 128)]
+      unsigned long long* keys = nullptr;   //   and keys [lrows][ceil(C / 128)][BEAM_TOPK_LD]
+      std::vector<__nv_bfloat16*> kvc;
+    } bm;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev_enc = nullptr, ev_done = nullptr;
   };
@@ -654,6 +697,7 @@ struct parseq_engine {
   long long sc_meta_ints = 0;
   unsigned char* sc_causal = nullptr;
   float2* sc_vt_part = nullptr;
+  long long beam_bytes = 0;         // device bytes of the beam-search buffers (0 until the first beam call)
   bool use_graph = true;
   struct GraphEntry { cudaGraphExec_t exec; long long kernels; };
   std::map<std::vector<int>, GraphEntry> graphs;
@@ -761,6 +805,7 @@ void free_workspace(parseq_engine* e) {
   for (void* p : sc)
     if (p) cudaFree(p);
   e->sc_meta = nullptr; e->sc_meta_ints = 0; e->sc_causal = nullptr; e->sc_vt_part = nullptr;
+  e->beam_bytes = 0;
   if (e->ev_enc) { cudaEventDestroy(e->ev_enc); e->ev_enc = nullptr; }
   e->a_pe = e->xn = e->qkv = e->att = e->hid = e->mem = e->ckv = nullptr;
   e->x = e->in_images = e->out_logits = nullptr;
@@ -772,6 +817,12 @@ void free_workspace(parseq_engine* e) {
     if (sg.cx) cudaFree(sg.cx);
     if (sg.lse_part) cudaFree(sg.lse_part);
     if (sg.lse_tlogit) cudaFree(sg.lse_tlogit);
+    void* bq[] = {sg.bm.ids[0], sg.bm.ids[1], sg.bm.score[0], sg.bm.score[1], sg.bm.len[0], sg.bm.len[1], sg.bm.st[0],
+                  sg.bm.st[1], sg.bm.parent, sg.bm.logits, sg.bm.part, sg.bm.keys};
+    for (void* p : bq)
+      if (p) cudaFree(p);
+    for (auto p : sg.bm.kvc)
+      if (p) cudaFree(p);
     for (auto p : sg.kvc)
       if (p) cudaFree(p);
     if (sg.stream) cudaStreamDestroy(sg.stream);
@@ -782,9 +833,10 @@ void free_workspace(parseq_engine* e) {
 }
 
 // categories: 0 encoder GEMM, 1 encoder attention, 2 LayerNorm, 3 decoder GEMM, 4 decoder attention, 5 other,
-// 6 encoder residual GEMM + LayerNorm, 7 AR-loop kernel, 8 scoring tail (head GEMM with the LSE epilogue + reduce)
+// 6 encoder residual GEMM + LayerNorm, 7 AR-loop kernel, 8 scoring tail (head GEMM with the LSE epilogue + reduce),
+// 9 beam selection (beam_select_kernel and the K/V gather of parseq_beam_search)
 enum { CAT_ENC_GEMM = 0, CAT_ENC_ATTN = 1, CAT_LN = 2, CAT_DEC_GEMM = 3, CAT_DEC_ATTN = 4, CAT_MISC = 5, CAT_ENC_GEMM_LN = 6, CAT_DEC_AR = 7,
-       CAT_SCORE = 8, CAT_COUNT = 9 };
+       CAT_SCORE = 8, CAT_BEAM = 9, CAT_COUNT = 10 };
 
 cudaEvent_t pool_event(parseq_engine* e) {
   if (!e->event_pool.empty()) { cudaEvent_t ev = e->event_pool.back(); e->event_pool.pop_back(); return ev; }
@@ -974,6 +1026,14 @@ struct DecodeExtras {
   float* out_norm = nullptr;             // [B*nq, D] fp32: decoder.norm(y) is the result (no head)
   const int* lse_tgt = nullptr;          // [B*nq] target class per row: the head runs with the LSE epilogue into the
                                          // stage's lse_part / lse_tlogit (candidate scoring), no logits are stored
+  int beam = 1;                          // beam search: B counts beam rows, `beam` consecutive rows per image; the rows'
+                                         // self-attention reads their own ids, their cross-attention their image
+  // beam search above 128 classes: the head GEMM runs the top-K epilogue (beam_k keys per row and tile, the images'
+  // allowlist rows beam_mask) into these, and no logits are stored
+  float2* beam_part = nullptr;
+  unsigned long long* beam_keys = nullptr;
+  int beam_k = 0;
+  const uint32_t* beam_mask = nullptr;
 };
 
 const __nv_bfloat16* ckv_of(const parseq_engine* e, int layer) { return layer == 0 ? e->ckv : e->ckv_deep[layer - 1]; }
@@ -1050,8 +1110,10 @@ int dec_layer_rest(parseq_engine* e, parseq_engine::Stage& sg, int l, int b_firs
 // (an AR step, pitch L: the causal content rows of earlier positions do not change as the context grows) or nkeys = pitch
 // (a whole pass).  The content rows attend to keys 0..nkeys-1 under `mode` (0: all, 1: cloze + first EOS), or under the
 // caller's content / padding masks (decode API).
+// rpi > 1 (beam search, nc = 1): the B rows are rpi consecutive beams of each of B / rpi images.
 int content_stream(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, int k0, int nc, int nkeys, int pitch,
-                   int mode, const int* ids, const unsigned char* cmask, const unsigned char* pmask, cudaStream_t st) {
+                   int mode, const int* ids, const unsigned char* cmask, const unsigned char* pmask, cudaStream_t st,
+                   int rpi = 1) {
   const int D = e->D, M = B * nc;
   const float qscale = 1.0f / std::sqrt(static_cast<float>(e->dh_dec));
   {
@@ -1071,7 +1133,7 @@ int content_stream(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int 
                 pq::EPI_F32, qscale, nullptr, 0, 0, sg.qc, D, st));
     PQ_TRY(self_attn_rows(e, sg.qc, l == 0 ? e->kvtab : sg.kvc[l - 1], l > 0, pitch, ids, B, nc, k0, nkeys, mode, cmask, pmask,
                           sg.sa, st));
-    PQ_TRY(dec_layer_rest(e, sg, l, b_first, B, nc, sg.cx, nullptr, 0, st));
+    PQ_TRY(dec_layer_rest(e, sg, l, b_first, B / rpi, nc * rpi, sg.cx, nullptr, 0, st));
     // K/V of layer l + 1 = W_kv norm_c_{l+1}(content_{l+1}) + b_kv, into rows k0.. of its cache
     const std::string Ln = "decoder.layers." + std::to_string(l + 1) + ".";
     PQ_TRY(layernorm(e, sg.cx, Ln + "norm_c", 1e-5f, M, sg.yn, nullptr, st));
@@ -1092,9 +1154,10 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
   const float qscale = 1.0f / std::sqrt(static_cast<float>(e->dh_dec));
   e->cur_cat = CAT_DEC_GEMM;
   const int kv_pitch = ar_step ? e->L : nkeys;
+  const int rpi = ex != nullptr ? ex->beam : 1;   // rows per image of the cross-attention (beam search)
   if (e->cfg.dec_depth > 1)
     PQ_TRY(content_stream(e, sg, b_first, B, ar_step ? q0 : 0, ar_step ? 1 : nkeys, nkeys, kv_pitch, mode, ids,
-                          ex != nullptr ? ex->cmask : nullptr, ex != nullptr ? ex->pmask : nullptr, st));
+                          ex != nullptr ? ex->cmask : nullptr, ex != nullptr ? ex->pmask : nullptr, st, rpi));
   const float* qself = e->qs;            // [L, D] table of W_q LN_q(pos_queries), pre-scaled
   const unsigned char *qmask = nullptr, *pmask = nullptr;
   if (ex != nullptr && ex->query != nullptr) {
@@ -1130,7 +1193,7 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
   }
   const bool own_q = ex != nullptr && ex->query != nullptr;
   const float* resid = own_q ? ex->query : e->wf("pos_queries") + static_cast<long long>(q0) * D;
-  PQ_TRY(dec_layer_rest(e, sg, 0, b_first, B, nq, sg.y, resid, own_q ? M : nq, st));
+  PQ_TRY(dec_layer_rest(e, sg, 0, b_first, B / rpi, nq * rpi, sg.y, resid, own_q ? M : nq, st));
   // query stream of layers >= 1 (modules.py:91-93): its residual base is the previous layer's output, its keys the
   // layer's content K/V cache
   for (int l = 1; l < e->cfg.dec_depth; ++l) {
@@ -1139,7 +1202,7 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
     PQ_TRY(gemm(e, sg.yn, D, e->w(Ll + "self_attn.in_proj_weight"), D, e->wf(Ll + "self_attn.in_proj_bias"), M, D, D,
                 pq::EPI_F32, qscale, nullptr, 0, 0, sg.qc, D, st));
     PQ_TRY(self_attn_rows(e, sg.qc, sg.kvc[l - 1], true, kv_pitch, ids, B, nq, q0, nkeys, mode, qmask, pmask, sg.sa, st));
-    PQ_TRY(dec_layer_rest(e, sg, l, b_first, B, nq, sg.y, nullptr, 0, st));
+    PQ_TRY(dec_layer_rest(e, sg, l, b_first, B / rpi, nq * rpi, sg.y, nullptr, 0, st));
   }
   if (ex != nullptr && ex->out_norm != nullptr) {
     // PARSeq.decode returns the decoder output: final LayerNorm only (modules.py:123-125)
@@ -1151,6 +1214,11 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
     TimedScope ts(e, st, CAT_SCORE, 2.0 * M * e->C * D);
     PQ_TRY(gemm_lse_launch(e->lo, sg.yn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, ex->lse_tgt, sg.lse_part,
                            sg.lse_tlogit, st));
+  } else if (ex != nullptr && ex->beam_keys != nullptr) {
+    PQ_TRY(layernorm(e, sg.y, "decoder.norm", 1e-5f, M, sg.yn, nullptr, st));
+    TimedScope ts(e, st, CAT_DEC_GEMM, 2.0 * M * e->C * D);
+    PQ_TRY(gemm_topk_launch(e->lo, sg.yn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, ex->beam_k, ex->beam_mask,
+                            rpi, ex->beam_part, ex->beam_keys, st));
   } else if (nq > 1 && ids_dst == nullptr) {
     // multi-query passes (refine / NAR): LayerNorm kernel + wgmma GEMM for the head (weights read once per tile).
     // Chosen by pass type, not by batch size, so that a row's result does not depend on the batch it is computed in.
@@ -2015,6 +2083,197 @@ int check_score_call(parseq_engine* e, const parseq_score_args* a, const void* i
   return check_score(a, e->cfg.max_label_length, e->C);
 }
 
+// ---------------------------------------------------------------- beam search (parseq_beam_search)
+// ViTSTR: images whose [L, C] logits one beam group holds (the head runs once per group, the selection once per position)
+int beam_vt_images(const parseq_engine* e) { return std::min(e->chunk, 32); }
+
+// Beam buffers, on the first beam call (an engine that never beam-searches allocates none of them).  PARSeq: every stage
+// holds dec_chunk beam rows, whatever the beam width; ViTSTR: stage 0 holds beam_vt_images images of BEAM_MAX slots.
+int beam_reserve(parseq_engine* e) {
+  const size_t nst = e->arch == 0 ? e->stages.size() : 1;
+  const int D = e->D;
+  auto grab = [&](auto** p, long long n) -> int {
+    if (*p != nullptr) return PARSEQ_OK;
+    PQ_TRY(dev_alloc(p, n));
+    e->beam_bytes += n * static_cast<long long>(sizeof(**p));
+    return PARSEQ_OK;
+  };
+  for (size_t s = 0; s < nst; ++s) {
+    parseq_engine::Stage::Beam& bm = e->stages[s].bm;
+    if (bm.rows > 0) continue;
+    const int rows = e->arch == 0 ? e->dec_chunk : beam_vt_images(e) * pq::BEAM_MAX;
+    const long long lrows = e->arch == 0 ? rows : 1ll * beam_vt_images(e) * e->L;
+    for (int h = 0; h < 2; ++h) {
+      PQ_TRY(grab(&bm.ids[h], 1ll * rows * e->ids_ld));
+      PQ_TRY(grab(&bm.score[h], rows));
+      PQ_TRY(grab(&bm.len[h], rows));
+      PQ_TRY(grab(&bm.st[h], rows));
+    }
+    PQ_TRY(grab(&bm.parent, rows));
+    const long long ntiles = (e->C + pq::GEMM_BLOCK_N - 1) / pq::GEMM_BLOCK_N;
+    if (e->C <= 128) {
+      PQ_TRY(grab(&bm.logits, lrows * e->C));
+    } else {
+      PQ_TRY(grab(&bm.part, lrows * ntiles));
+      PQ_TRY(grab(&bm.keys, lrows * ntiles * pq::BEAM_TOPK_LD));
+    }
+    if (e->arch == 0 && e->cfg.dec_depth > 1) {
+      bm.kvc.resize(static_cast<size_t>(e->cfg.dec_depth - 1), nullptr);
+      for (auto& c : bm.kvc) PQ_TRY(grab(&c, 1ll * e->dec_chunk * e->L * 2 * D));
+    }
+    bm.rows = rows;
+  }
+  return PARSEQ_OK;
+}
+
+// Beam search over a batch of images (parseq_beam_search).  PARSeq: the encoder and the cross K/V once per super-chunk as
+// forward_super runs them, then groups of dec_chunk / K images (all K beams of an image in one group) round-robin over
+// the stages' streams; each step is one decoder pass over the group's beam rows (decode_pass with DecodeExtras::beam),
+// the head's logits of the step, and beam_select_kernel.  ViTSTR: the head once over a group's [B * L] token rows, then
+// beam_select_kernel once per position.
+int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_any, bool u8, int* ids, int* lengths,
+              float* scores, cudaStream_t user) {
+  const int N = a->batch, K = a->beam_width, D = e->D, T = e->T, C = e->C, L = e->L;
+  const int S = num_steps_of(e, a->max_length);
+  const long long img_sz = 3ll * e->cfg.img_h * e->cfg.img_w * (u8 ? 1 : 4);
+  const char* images = static_cast<const char*>(images_any);
+  PQ_TRY(beam_reserve(e));
+  auto init = [&](parseq_engine::Stage::Beam& bm, int B, cudaStream_t st) {
+    const int n = B * K * e->ids_ld;
+    e->launches++;
+    return launch_k(e->lo, pq::beam_init_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, bm.ids[0],
+                    bm.score[0], bm.len[0], bm.st[0], B * K, K, e->ids_ld, e->V - 2, e->V - 1);
+  };
+  // step `step` of the group whose first image is g0 (in the call's batch)
+  const bool wide = C > 128;
+  const int ntiles = (C + pq::GEMM_BLOCK_N - 1) / pq::GEMM_BLOCK_N;
+  auto select = [&](parseq_engine::Stage::Beam& bm, int B, int step, long long row0, long long img_stride,
+                    long long slot_stride, int g0, cudaStream_t st) {
+    const int cur = step & 1, nxt = cur ^ 1;
+    TimedScope ts(e, st, CAT_BEAM, 0.0);
+    return launch_k(e->lo, pq::beam_select_kernel, dim3(static_cast<unsigned>(B)), dim3(pq::BEAM_THREADS), 0, st,
+                    static_cast<const float*>(bm.logits), static_cast<const float2*>(bm.part),
+                    static_cast<const unsigned long long*>(bm.keys), ntiles, row0, img_stride, slot_stride, C, K, step, S, a->class_mask ? a->class_mask + 1ll * g0 * e->mask_ld : nullptr, e->mask_ld,
+                    static_cast<const int*>(bm.ids[cur]), static_cast<const float*>(bm.score[cur]),
+                    static_cast<const int*>(bm.len[cur]), static_cast<const int*>(bm.st[cur]), bm.ids[nxt], bm.score[nxt],
+                    bm.len[nxt], bm.st[nxt], bm.parent, e->ids_ld, ids + 1ll * g0 * K * S, lengths + 1ll * g0 * K,
+                    scores + 1ll * g0 * K);
+  };
+  PQ_CUDA(cudaEventRecord(e->ev_in, user));
+  PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_in, 0));
+  for (int b0 = 0; b0 < N; b0 += e->max_batch) {
+    const int Bc = std::min(N - b0, e->max_batch);
+    if (e->arch == 1) {
+      parseq_engine::Stage::Beam& bm = e->stages[0].bm;
+      const int G = beam_vt_images(e);
+      for (int o = 0; o < Bc; o += e->chunk) {
+        const int Bs = std::min(Bc - o, e->chunk);
+        PQ_TRY(encode_chunk(e, images + (b0 + o) * img_sz, u8, Bs, nullptr, nullptr, e->main, false));
+        PQ_TRY(vitstr_rows(e, Bs, L, e->main));
+        for (int g = 0; g < Bs; g += G) {
+          const int Bg = std::min(G, Bs - g);
+          if (wide) {
+            // the top-K epilogue over the group's [Bg * L] token rows: row r belongs to image r / L
+            TimedScope ts(e, e->main, CAT_DEC_GEMM, 2.0 * Bg * L * C * D);
+            PQ_TRY(gemm_topk_launch(e->lo, e->xn + 1ll * g * L * D, D, e->w("head.weight"), D, e->wf("head.bias"), Bg * L, C, D, K,
+                                    a->class_mask ? a->class_mask + 1ll * (b0 + o + g) * e->mask_ld : nullptr, L, bm.part,
+                                    bm.keys, e->main));
+          } else {
+            PQ_TRY(gemm(e, e->xn + 1ll * g * L * D, D, e->w("head.weight"), D, e->wf("head.bias"), Bg * L, C, D, pq::EPI_F32,
+                        1.0f, nullptr, 0, 0, bm.logits, C, e->main));
+          }
+          PQ_TRY(init(bm, Bg, e->main));
+          for (int step = 0; step < S; ++step) PQ_TRY(select(bm, Bg, step, step, L, 0, b0 + o + g, e->main));
+        }
+      }
+      continue;
+    }
+    for (int o = 0; o < Bc; o += e->chunk) {
+      const int Bs = std::min(Bc - o, e->chunk);
+      // kernel regime from the super-chunk, as forward_super: the memory bits equal the forward's
+      PQ_TRY(encode_chunk(e, images + (b0 + o) * img_sz, u8, Bs, e->mem + 1ll * o * T * D, nullptr, e->main, true, Bc));
+    }
+    PQ_TRY(cross_kv(e, Bc));
+    const int G = e->dec_chunk / K;                    // images per group: G * K beam rows fill a stage's buffers
+    const int ngroups = (Bc + G - 1) / G;
+    const int ns = static_cast<int>(e->stages.size());
+    const int used = std::min(ngroups, ns);
+    const bool fork = used > 1 && !e->timing;            // timing mode: everything on `main` (isolated kernel times)
+    if (fork) {
+      PQ_CUDA(cudaEventRecord(e->ev_enc, e->main));
+      for (int s = 0; s < used; ++s) PQ_CUDA(cudaStreamWaitEvent(e->stages[static_cast<size_t>(s)].stream, e->ev_enc, 0));
+    }
+    for (int gi = 0; gi < ngroups; ++gi) {
+      parseq_engine::Stage& sg = e->stages[static_cast<size_t>(gi % ns)];
+      parseq_engine::Stage::Beam& bm = sg.bm;
+      cudaStream_t ds = fork ? sg.stream : e->main;
+      const int g0 = gi * G, Bg = std::min(G, Bc - g0), R = Bg * K;
+      PQ_TRY(init(bm, Bg, ds));
+      DecodeExtras ex;
+      ex.beam = K;
+      if (wide) {
+        ex.beam_part = bm.part;
+        ex.beam_keys = bm.keys;
+        ex.beam_k = K;
+        ex.beam_mask = a->class_mask ? a->class_mask + 1ll * (b0 + g0) * e->mask_ld : nullptr;
+      }
+      const std::vector<__nv_bfloat16*> kvc0 = sg.kvc;
+      int rc = PARSEQ_OK;
+      for (int step = 0; step < S && rc == PARSEQ_OK; ++step) {
+        // query position `step` over keys 0..step of every beam row; the head leaves row r's logits at bm.logits + r * C
+        // (<= 128 classes) or its partials and top-K keys (above)
+        rc = decode_pass(e, sg, g0, R, 1, step, step + 1, 0, bm.ids[step & 1], bm.logits, C, nullptr, 0, nullptr, 0, nullptr,
+                         ds, &ex, /*ar_step*/ true);
+        if (rc == PARSEQ_OK) rc = select(bm, Bg, step, 0, K, 1, b0 + g0, ds);
+        if (rc != PARSEQ_OK || e->cfg.dec_depth == 1 || step + 1 == S) continue;
+        // depth >= 2: each new beam row continues its parent's content K/V cache rows 0..step
+        TimedScope ts(e, ds, CAT_BEAM, 0.0);
+        const long long pitch4 = 1ll * L * 2 * D * 2 / 16;
+        const int n4 = (step + 1) * 2 * D * 2 / 16;
+        for (size_t l = 0; l < sg.kvc.size() && rc == PARSEQ_OK; ++l) {
+          const long long total = 1ll * R * n4;
+          rc = launch_k(e->lo, pq::beam_kv_gather_kernel, dim3(static_cast<unsigned>(std::min<long long>((total + 255) / 256, 132ll * 8))),
+                        dim3(256), 0, ds, reinterpret_cast<const uint4*>(sg.kvc[l]), reinterpret_cast<uint4*>(bm.kvc[l]),
+                        static_cast<const int*>(bm.parent), R, pitch4, n4);
+          std::swap(sg.kvc[l], bm.kvc[l]);
+        }
+      }
+      // the stage's own cache pointers back (their contents are scratch between calls)
+      for (size_t l = 0; l < sg.kvc.size(); ++l)
+        if (sg.kvc[l] != kvc0[l]) std::swap(sg.kvc[l], bm.kvc[l]);
+      PQ_TRY(rc);
+    }
+    if (fork) {
+      for (int s = 0; s < used; ++s) {
+        parseq_engine::Stage& sg = e->stages[static_cast<size_t>(s)];
+        PQ_CUDA(cudaEventRecord(sg.ev_done, sg.stream));
+        PQ_CUDA(cudaStreamWaitEvent(e->main, sg.ev_done, 0));
+      }
+    }
+  }
+  PQ_CUDA(cudaEventRecord(e->ev_out, e->main));
+  PQ_CUDA(cudaStreamWaitEvent(user, e->ev_out, 0));
+  return PARSEQ_OK;
+}
+
+// Checks of the beam entry points, all on the host before anything is launched.
+int check_beam_call(parseq_engine* e, const parseq_beam_args* a, const void* images, const int* ids, const int* lengths,
+                    const float* scores) {
+  if (a == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  if (a->batch < 0) return fail(PARSEQ_ERR_INVALID_ARG, "negative batch");
+  if (a->beam_width < 1 || a->beam_width > pq::BEAM_MAX)
+    return fail(PARSEQ_ERR_INVALID_ARG, "beam_width " + std::to_string(a->beam_width) + " outside [1, 16]");
+  if (a->max_length < -1) return fail(PARSEQ_ERR_INVALID_ARG, "max_length must be -1 (None) or >= 0");
+  if (e == nullptr || (a->batch > 0 && (images == nullptr || ids == nullptr || lengths == nullptr || scores == nullptr)))
+    return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
+  if (!e->finalized) return fail(PARSEQ_ERR_STATE, "parseq_finalize has not been called after the last weight update");
+  if (e->arch == 0 && a->beam_width > e->dec_chunk)
+    return fail(PARSEQ_ERR_INVALID_ARG, "beam_width " + std::to_string(a->beam_width) + " exceeds the decoder chunk (option "
+                                        "dec_chunk = " + std::to_string(e->dec_chunk) + ")");
+  return PARSEQ_OK;
+}
+
 }  // namespace
 
 // =============================================================================== C ABI
@@ -2389,6 +2648,22 @@ int parseq_score_u8(parseq_engine* e, const parseq_score_args* a, const uint8_t*
   return score_impl(e, a, images_hwc, true, scores, token_logprobs, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int parseq_beam_search(parseq_engine* e, const parseq_beam_args* a, const float* images, int32_t* ids, int32_t* lengths,
+                       float* scores, parseq_stream_t stream) {
+  PQ_TRY(check_beam_call(e, a, images, ids, lengths, scores));
+  if (a->batch == 0) return PARSEQ_OK;
+  PQ_CUDA(cudaSetDevice(e->cfg.device));
+  return beam_impl(e, a, images, false, ids, lengths, scores, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int parseq_beam_search_u8(parseq_engine* e, const parseq_beam_args* a, const uint8_t* images_hwc, int32_t* ids,
+                          int32_t* lengths, float* scores, parseq_stream_t stream) {
+  PQ_TRY(check_beam_call(e, a, images_hwc, ids, lengths, scores));
+  if (a->batch == 0) return PARSEQ_OK;
+  PQ_CUDA(cudaSetDevice(e->cfg.device));
+  return beam_impl(e, a, images_hwc, true, ids, lengths, scores, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int parseq_postprocess(const float* logits, int32_t batch, int32_t num_steps, int32_t num_classes, int32_t eos_id, int32_t* ids,
                        int32_t* lengths, float* confidence, parseq_stream_t stream) {
   if (logits == nullptr || ids == nullptr || lengths == nullptr || confidence == nullptr)
@@ -2547,6 +2822,7 @@ int64_t parseq_debug_int(parseq_engine* e, const char* name) {
   if (n == "ar_last_ids_pitch") return e->ar_last_idp;
   if (n == "ar_last_path") return e->ar_last_path;
   if (n == "sm_count") return e->lo.sm_count;
+  if (n == "beam_bytes") return e->beam_bytes;
   return -1;
 }
 int64_t parseq_kernel_launches(const parseq_engine* e) { return e ? e->launches : 0; }

@@ -22,6 +22,7 @@ enum GemmEpilogue : int {
   EPI_GELU_BF16 = 2,  // out_bf16 = bf16(gelu(acc+bias))
   EPI_F32_RESID = 3,  // kernel instantiation of EPI_F32 with a residual (the API's mode stays EPI_F32)
   EPI_LSE = 4,        // no output tile: per-row log-sum-exp partials of the tile (gemm_lse_epilogue), candidate scoring
+  EPI_TOPK = 5,       // EPI_LSE partials of the allowed classes plus each row's top-K classes of the tile (beam search)
 };
 // How the kernel stores its tiles.  TMA: bf16 tiles go through a 128B-swizzled shared-memory staging tile and one
 // thread stores them with cp.async.bulk.tensor, 2D row-major or 3D column-blocked ([N/64][rows][64]); the tensor map's
@@ -44,6 +45,12 @@ struct GemmParams {
   // EPI_LSE only: target class of each row (< 0: none) and where its logit goes; `out` holds the float2 partials
   const int* lse_tgt;
   float* lse_tlogit;
+  // EPI_TOPK only: per row and tile the K best (beam_order_key) of the allowed classes, BEAM_TOPK_LD keys per (row, tile),
+  // 0 past the last; allowlist rows (ceil(N / 32) words; row r reads word row r / topk_mask_div), or null
+  unsigned long long* topk_keys;
+  int topk_k;
+  const uint32_t* topk_mask;
+  int topk_mask_div;
 };
 
 constexpr int GEMM_BLOCK_M = 128;  // rows per tile (two m64 halves, one warpgroup)
@@ -203,6 +210,66 @@ __device__ __forceinline__ void gemm_lse_epilogue(const GemmParams& p, const flo
   }
 }
 
+// EPI_TOPK: the EPI_LSE body over the allowed classes (a masked class counts as -inf, so it adds 0 to the sum), and each
+// row's K best allowed classes of the tile (-inf never listed).  The four lanes of a row hold 32 columns each: K rounds
+// of a masked arg-max over a lane's 32 values (a 32-bit "taken" mask), merged over the four lanes with the xor-shuffle
+// order of the LSE.  No logit reaches memory.
+__device__ __forceinline__ void gemm_topk_epilogue(const GemmParams& p, const float (&acc0)[64], const float (&acc1)[64],
+                                                   int m0, int n0, int r0, int lane) {
+  float2* part = reinterpret_cast<float2*>(p.out);
+  const int words = (p.N + 31) >> 5;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {        // (half, +8 rows)
+    const float* acc = (q < 2) ? acc0 : acc1;
+    const int row = m0 + 64 * (q >> 1) + r0 + 8 * (q & 1);
+    const uint32_t* mrow = (p.topk_mask != nullptr && row < p.M)
+                               ? p.topk_mask + static_cast<long long>(row / p.topk_mask_div) * words : nullptr;
+    float v[32];
+    float mx = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < GEMM_BLOCK_N / 8; ++i) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = n0 + i * 8 + 2 * (lane & 3) + e;
+        const float b = (p.bias != nullptr && col < p.N) ? __ldg(p.bias + col) : 0.0f;
+        const float f = gemm_epi<EPI_F32>(acc[4 * i + 2 * (q & 1) + e], b, p.alpha);
+        const bool ok = col < p.N && (mrow == nullptr || class_allowed(mrow, col));
+        v[2 * i + e] = ok ? f : -INFINITY;
+        mx = fmaxf(mx, v[2 * i + e]);
+      }
+    }
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+    const float base = (mx == -INFINITY) ? 0.0f : mx;
+    float s = 0.0f;
+#pragma unroll
+    for (int k = 0; k < 32; ++k) s += expf(v[k] - base);
+    s += __shfl_xor_sync(0xffffffffu, s, 1);
+    s += __shfl_xor_sync(0xffffffffu, s, 2);
+    const int tile = n0 / GEMM_BLOCK_N;
+    if ((lane & 3) == 0 && row < p.M) part[static_cast<long long>(row) * p.num_n_tiles + tile] = make_float2(mx, s);
+    unsigned long long* keys = p.topk_keys + (static_cast<long long>(row) * p.num_n_tiles + tile) * BEAM_TOPK_LD;
+    uint32_t taken = 0u;
+#pragma unroll 1
+    for (int r = 0; r < p.topk_k; ++r) {
+      unsigned long long best = 0ull;
+      int bk = -1;
+#pragma unroll
+      for (int k = 0; k < 32; ++k) {
+        const int col = n0 + (k >> 1) * 8 + 2 * (lane & 3) + (k & 1);
+        const unsigned long long key =
+            (((taken >> k) & 1u) || v[k] == -INFINITY) ? 0ull : beam_order_key(v[k], col);
+        if (key > best) { best = key; bk = k; }
+      }
+      unsigned long long w = best;
+      w = max(w, __shfl_xor_sync(0xffffffffu, w, 1));
+      w = max(w, __shfl_xor_sync(0xffffffffu, w, 2));
+      if (w != 0ull && w == best) taken |= 1u << bk;   // keys are unique within a row: one lane takes it
+      if ((lane & 3) == 0 && row < p.M) keys[r] = w;
+    }
+  }
+}
+
 // The kernel body lives in gemm_body.inc, included by each kernel below with EPI and STORE in scope.
 template <int EPI, int STORE>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
@@ -217,6 +284,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_lse_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                      const __grid_constant__ CUtensorMap tmOut, const GemmParams p) {
   constexpr int EPI = EPI_LSE, STORE = ST_REG;
+#include "gemm_body.inc"
+}
+
+// The head GEMM of beam search above 128 classes: the same body with the top-K epilogue (EPI_TOPK, register path).
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_bf16_topk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                      const __grid_constant__ CUtensorMap tmOut, const GemmParams p) {
+  constexpr int EPI = EPI_TOPK, STORE = ST_REG;
 #include "gemm_body.inc"
 }
 

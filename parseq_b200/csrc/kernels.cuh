@@ -914,6 +914,14 @@ __global__ void __launch_bounds__(128) dec_cross_attn3_grouped_kernel(const floa
 // No early griddepcontrol.launch_dependents: the next kernel on the stream (the next group of candidates, which
 // rewrites the chain's LayerNorm, partial and target-logit buffers) may start only once this grid has exited, and this
 // grid's wait orders it after the head GEMM that wrote what it reads.
+// The merge of a row's per-tile (max, sum exp) partials (gemm_lse_epilogue, gemm_topk_epilogue) in column order:
+// M = max of the tile maxima, S = sum of s_j exp(m_j - M); the row's log-sum-exp is M + log(S).
+__device__ __forceinline__ void lse_merge(const float2* pr, int ntiles, float& M, float& S) {
+  M = -INFINITY;
+  for (int j = 0; j < ntiles; ++j) M = fmaxf(M, pr[j].x);
+  S = 0.0f;
+  for (int j = 0; j < ntiles; ++j) S += pr[j].y * expf(pr[j].x - M);
+}
 __global__ void __launch_bounds__(64) score_reduce_kernel(const float2* __restrict__ part, int ntiles,
                                                           const float* __restrict__ tlogit, const int* __restrict__ tgt,
                                                           const int* __restrict__ lengths, const int* __restrict__ cand_img,
@@ -947,11 +955,8 @@ __global__ void __launch_bounds__(64) score_reduce_kernel(const float2* __restri
   }
   float term = 0.0f;
   if (i <= n) {
-    const float2* pr = part + (prow0 + i) * ntiles;
-    float M = -INFINITY;
-    for (int j = 0; j < ntiles; ++j) M = fmaxf(M, pr[j].x);
-    float S = 0.0f;
-    for (int j = 0; j < ntiles; ++j) S += pr[j].y * expf(pr[j].x - M);
+    float M, S;
+    lse_merge(part + (prow0 + i) * ntiles, ntiles, M, S);
     const float t = xn != nullptr ? s_tl[i] : tlogit[trow0 + i];
     term = (t - M) - logf(S);
   }
@@ -962,6 +967,228 @@ __global__ void __launch_bounds__(64) score_reduce_kernel(const float2* __restri
     float s = 0.0f;
     for (int k = 0; k <= n; ++k) s += s_term[k];
     scores[m] = s;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Beam search (parseq_beam_search).  A group's state has one row r = b * K + k per (image b, slot k): ids[r][ids_ld]
+// (BOS, c_1.., then PAD; the EOS of a finished label stays in its row), score[r], len[r] (characters so far, -1 empty)
+// and st[r] (BEAM_ACTIVE / BEAM_DONE / BEAM_EMPTY).  Every beam row of every step reads a valid token id, so the decoder
+// runs on all rows without a branch; only the selection looks at the state.
+constexpr int BEAM_MAX = 16;
+constexpr int BEAM_ACTIVE = 0, BEAM_DONE = 1, BEAM_EMPTY = 2;
+constexpr int BEAM_THREADS = 32 * BEAM_MAX;
+
+// slot 0 of every image active with [BOS] and score 0, the other slots empty
+__global__ void beam_init_kernel(int* __restrict__ ids, float* __restrict__ score, int* __restrict__ len, int* __restrict__ st,
+                                 int rows, int K, int ids_ld, int bos, int pad) {
+  grid_dep_launch();
+  grid_dep_wait();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < rows * ids_ld) ids[i] = ((i % ids_ld) == 0) ? bos : pad;
+  if (i < rows) {
+    const bool first = (i % K) == 0;
+    score[i] = first ? 0.0f : -INFINITY;
+    len[i] = first ? 0 : -1;
+    st[i] = first ? BEAM_ACTIVE : BEAM_EMPTY;
+  }
+}
+
+// One beam step of a group: one CTA per image, warp k < K expands slot k.  The row of (b, k) is row0 + b * img_stride +
+// k * slot_stride (PARSeq: the step's b * K + k; ViTSTR: the image's position-`step` row for every slot).
+//   1. Each active slot takes its row's log-sum-exp over the allowed classes and its K best classes in row order
+//      (beam_order_key; masked and -inf classes never expand):
+//      - at <= 128 classes (topk null) the lanes scan the logits row [C] for the max m and the sum s of exp(x - m) (m = -inf:
+//        exp(x)), LSE = m + log(s), and keep their K best keys in registers;
+//      - above 128 classes the head GEMM's top-K epilogue left per 128-column tile the (max, sum) partial `part` [ntiles]
+//        and the tile's K best keys `topk` [ntiles][BEAM_TOPK_LD] of the allowed classes: lane 0 merges the partials in
+//        column order (lse_merge, as score_reduce_kernel), the lanes keep the K best of the tiles' keys.
+//      A NaN or +inf allowed logit makes the LSE NaN.  K rounds of a warp arg-max over the lanes' list heads
+//      (xor-shuffle butterfly) give the slot's K expansions in row order.
+//   2. Thread 0 builds the pool in slot order: a finished slot contributes itself, an active slot its expansions, each
+//      with score parent + (logit - LSE) in fp32 (the logit is read back from its key).
+//   3. Every entry counts the entries that rank before it (higher score, or equal and earlier; NaN after every number;
+//      -inf never kept): the K first are the new slots.
+//   4. The new state goes to the *_out buffers, parent[r] = the state row each new slot came from (the K/V cache rows
+//      follow it at depth >= 2), and after the last step the results: out_ids [K][num_steps] per image (c_1..c_n, then
+//      0 = EOS / padding), out_len (-1 empty), out_score (-inf empty).
+// No early griddepcontrol.launch_dependents: what comes next reads the state this grid writes.
+__global__ void __launch_bounds__(BEAM_THREADS) beam_select_kernel(
+    const float* __restrict__ logits, const float2* __restrict__ part, const unsigned long long* __restrict__ topk,
+    int ntiles, long long row0, long long img_stride, long long slot_stride, int C, int K, int step, int num_steps,
+    const uint32_t* __restrict__ mask, int mask_ld, const int* __restrict__ ids_in, const float* __restrict__ score_in,
+    const int* __restrict__ len_in, const int* __restrict__ st_in, int* __restrict__ ids_out, float* __restrict__ score_out,
+    int* __restrict__ len_out, int* __restrict__ st_out, int* __restrict__ parent, int ids_ld, int* __restrict__ out_ids,
+    int* __restrict__ out_len, float* __restrict__ out_score) {
+  __shared__ unsigned long long s_key[BEAM_MAX][BEAM_MAX];
+  __shared__ float s_lse[BEAM_MAX];
+  __shared__ float p_score[BEAM_MAX * BEAM_MAX];
+  __shared__ int p_slot[BEAM_MAX * BEAM_MAX], p_cls[BEAM_MAX * BEAM_MAX];
+  __shared__ int s_sel[BEAM_MAX];
+  __shared__ int s_n;
+  grid_dep_wait();
+  const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int r0 = b * K;
+  const uint32_t* mrow = mask != nullptr ? mask + static_cast<long long>(b) * mask_ld : nullptr;
+  if (tid < BEAM_MAX) s_sel[tid] = -1;
+  if (warp < K && st_in[r0 + warp] == BEAM_ACTIVE) {
+    const long long row = row0 + b * img_stride + warp * slot_stride;
+    unsigned long long top[BEAM_MAX];
+#pragma unroll
+    for (int j = 0; j < BEAM_MAX; ++j) top[j] = 0ull;
+    unsigned long long thr = 0ull;
+    auto insert = [&](unsigned long long v) {
+      if (v <= thr) return;
+#pragma unroll
+      for (int j = 0; j < BEAM_MAX; ++j) {        // insertion into the lane's descending list
+        const unsigned long long t = top[j];
+        const bool sw = v > t;
+        top[j] = sw ? v : t;
+        v = sw ? t : v;
+      }
+#pragma unroll
+      for (int j = 0; j < BEAM_MAX; ++j)
+        if (j == K - 1) thr = top[j];
+    };
+    float lse;
+    if (topk == nullptr) {
+      const float* lr = logits + row * C;
+      float m = -INFINITY;
+      for (int c = lane; c < C; c += 32) {
+        if (mrow != nullptr && !class_allowed(mrow, c)) continue;
+        const float x = lr[c];
+        m = fmaxf(m, x);
+        if (x != -INFINITY) insert(beam_order_key(x, c));
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+      const float base = (m == -INFINITY) ? 0.0f : m;
+      float s = 0.0f;
+      for (int c = lane; c < C; c += 32)
+        if (mrow == nullptr || class_allowed(mrow, c)) s += expf(lr[c] - base);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      lse = m + logf(s);
+    } else {
+      const unsigned long long* kr = topk + row * ntiles * BEAM_TOPK_LD;
+      for (int i = lane; i < ntiles * K; i += 32) {
+        const int t = i / K, j = i - t * K;
+        const unsigned long long v = kr[t * BEAM_TOPK_LD + j];
+        if (v != 0ull) insert(v);
+      }
+      float M = 0.0f, S = 0.0f;
+      if (lane == 0) lse_merge(part + row * ntiles, ntiles, M, S);
+      lse = __shfl_sync(0xffffffffu, M + logf(S), 0);
+    }
+    int h = 0;
+    for (int r = 0; r < K; ++r) {
+      unsigned long long cand = 0ull;
+#pragma unroll
+      for (int j = 0; j < BEAM_MAX; ++j)
+        if (j == h && j < K) cand = top[j];
+      unsigned long long best = cand;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long u = __shfl_xor_sync(0xffffffffu, best, o);
+        best = u > best ? u : best;
+      }
+      if (best != 0ull && cand == best) ++h;     // keys are unique within a row: one lane advances
+      if (lane == 0) s_key[warp][r] = best;
+    }
+    if (lane == 0) s_lse[warp] = lse;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    int n = 0;
+    for (int k = 0; k < K; ++k) {
+      const int sk = st_in[r0 + k];
+      const float ps = score_in[r0 + k];
+      if (sk == BEAM_DONE) {
+        p_score[n] = ps; p_slot[n] = k; p_cls[n] = -1; ++n;
+      } else if (sk == BEAM_ACTIVE) {
+        for (int j = 0; j < K && s_key[k][j] != 0ull; ++j) {
+          const int c = beam_key_class(s_key[k][j]);
+          p_score[n] = ps + (beam_key_value(s_key[k][j]) - s_lse[k]); p_slot[n] = k; p_cls[n] = c; ++n;
+        }
+      }
+    }
+    s_n = n;
+  }
+  __syncthreads();
+  const int n = s_n;
+  if (tid < n) {
+    const float v = p_score[tid];
+    if (v != -INFINITY) {
+      const bool vn = isnan(v);
+      int rank = 0;
+      for (int j = 0; j < n && rank < K; ++j) {
+        const float u = p_score[j];
+        if (j == tid || u == -INFINITY) continue;
+        const bool un = isnan(u);
+        rank += (un != vn) ? vn : ((!un && u > v) || ((un || u == v) && j < tid));
+      }
+      if (rank < K) s_sel[rank] = tid;
+    }
+  }
+  __syncthreads();
+  for (int idx = tid; idx < K * ids_ld; idx += blockDim.x) {
+    const int k = idx / ids_ld, t = idx - k * ids_ld;
+    const int e = s_sel[k];
+    int v = ids_in[static_cast<long long>(r0 + k) * ids_ld + t];      // an empty slot keeps a row of valid ids
+    if (e >= 0) {
+      const int c = p_cls[e];
+      v = (c >= 0 && t == step + 1) ? c : ids_in[static_cast<long long>(r0 + p_slot[e]) * ids_ld + t];
+    }
+    ids_out[static_cast<long long>(r0 + k) * ids_ld + t] = v;
+  }
+  const bool last = step + 1 == num_steps;
+  if (tid < K) {
+    const int k = tid, e = s_sel[k];
+    float sc = -INFINITY;
+    int ln = -1, sn = BEAM_EMPTY, par = k;
+    if (e >= 0) {
+      const int c = p_cls[e];
+      par = p_slot[e];
+      sc = p_score[e];
+      if (c < 0) { ln = len_in[r0 + par]; sn = BEAM_DONE; }
+      else if (c == 0) { ln = step; sn = BEAM_DONE; }
+      else { ln = step + 1; sn = last ? BEAM_DONE : BEAM_ACTIVE; }
+    }
+    score_out[r0 + k] = sc;
+    len_out[r0 + k] = ln;
+    st_out[r0 + k] = sn;
+    parent[r0 + k] = r0 + par;
+    if (last) {
+      out_len[r0 + k] = ln;
+      out_score[r0 + k] = sc;
+    }
+  }
+  if (last) {
+    for (int idx = tid; idx < K * num_steps; idx += blockDim.x) {
+      const int k = idx / num_steps, t = idx - k * num_steps;
+      const int e = s_sel[k];
+      int v = 0;
+      if (e >= 0) {
+        const int c = p_cls[e], p = p_slot[e];
+        const int ln = c < 0 ? len_in[r0 + p] : (c == 0 ? step : step + 1);
+        if (t < ln) v = t < step ? ids_in[static_cast<long long>(r0 + p) * ids_ld + t + 1] : c;
+      }
+      out_ids[static_cast<long long>(r0 + k) * num_steps + t] = v;
+    }
+  }
+}
+
+// Depth >= 2: the content K/V cache rows 0..n-1 of every new beam row come from its parent's row (cache [rows][pitch][2D]
+// bf16, in 16-byte units: pitch4 per row, n4 valid)
+__global__ void beam_kv_gather_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, const int* __restrict__ parent,
+                                      int rows, long long pitch4, int n4) {
+  grid_dep_launch();
+  grid_dep_wait();
+  const long long total = static_cast<long long>(rows) * n4;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int r = static_cast<int>(i / n4), j = static_cast<int>(i % n4);
+    dst[r * pitch4 + j] = src[parent[r] * pitch4 + j];
   }
 }
 

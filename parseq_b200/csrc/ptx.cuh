@@ -64,6 +64,28 @@ __device__ __forceinline__ bool class_allowed(const uint32_t* row, int c) {
   return c == 0 || ((__ldg(row + (c >> 5)) >> (c & 31)) & 1u);
 }
 __device__ __forceinline__ int class_mask_words(int C) { return (C + 31) >> 5; }
+constexpr int BEAM_TOPK_LD = 16;   // keys per (row, 128-column tile) of the beam head's top-K epilogue: the largest beam width
+// The order in which beam search expands a row's classes, as one 64-bit key (larger = earlier; 0 = none): NaN logits
+// first, then the logit descending, ties (and NaNs) to the lower class.  -0 counts as +0.  beam_key_value inverts it.
+__device__ __forceinline__ unsigned long long beam_order_key(float x, int c) {
+  uint32_t o;
+  if (isnan(x)) {
+    o = 0xffffffffu;
+  } else {
+    const uint32_t u = __float_as_uint(x == 0.0f ? 0.0f : x);
+    o = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+  }
+  return (static_cast<unsigned long long>(o) << 32) | (0xffffffffu - static_cast<uint32_t>(c));
+}
+__device__ __forceinline__ float beam_key_value(unsigned long long key) {
+  const uint32_t o = static_cast<uint32_t>(key >> 32);
+  if (o == 0xffffffffu) return __int_as_float(0x7fffffff);
+  return __uint_as_float((o & 0x80000000u) ? (o & 0x7fffffffu) : ~o);
+}
+__device__ __forceinline__ int beam_key_class(unsigned long long key) {
+  return static_cast<int>(0xffffffffu - static_cast<uint32_t>(key));
+}
+
 
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {

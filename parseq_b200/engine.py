@@ -34,11 +34,15 @@ class ScoreArgsC(C.Structure):
                 ("lengths", C.c_void_p)]
 
 
+class BeamArgsC(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("beam_width", C.c_int32), ("max_length", C.c_int32), ("class_mask", C.c_void_p)]
+
+
 EXPORTS = [
     "parseq_create", "parseq_destroy", "parseq_set_weight", "parseq_num_weights", "parseq_weight_key",
     "parseq_finalize", "parseq_forward", "parseq_forward_host", "parseq_forward_u8", "parseq_forward_host_u8",
     "parseq_resize_crops", "parseq_forward_crops", "parseq_forward_host_crops",
-    "parseq_score", "parseq_score_u8", "parseq_score_check",
+    "parseq_score", "parseq_score_u8", "parseq_score_check", "parseq_beam_search", "parseq_beam_search_u8",
     "parseq_postprocess", "parseq_encode", "parseq_decode", "parseq_decode_ex", "parseq_head", "parseq_text_embed", "parseq_kernel_launches", "parseq_debug_int", "parseq_bench_tma_stream",
     "parseq_set_option", "parseq_get_timing", "parseq_get_ar_profile", "parseq_last_error", "parseq_version", "parseq_gemm_bf16", "parseq_gemm_ln_bf16", "parseq_mlp_ln_bf16", "parseq_layernorm_bf16",
     "parseq_enc_attention", "parseq_qkv_attention_bf16",
@@ -81,6 +85,9 @@ def load_library(path: Optional[str] = None):
     lib.parseq_score.argtypes = [C.c_void_p, C.POINTER(ScoreArgsC), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.parseq_score_u8.argtypes = lib.parseq_score.argtypes
     lib.parseq_score_check.argtypes = [C.POINTER(ParseqConfigC), C.POINTER(ScoreArgsC)]
+    lib.parseq_beam_search.argtypes = [C.c_void_p, C.POINTER(BeamArgsC), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p]
+    lib.parseq_beam_search_u8.argtypes = lib.parseq_beam_search.argtypes
     lib.parseq_postprocess.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p]
     lib.parseq_encode.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -176,7 +183,7 @@ class Engine:
         check(self.lib, self.lib.parseq_set_option(self.handle, name.encode(), int(value)))
 
     TIMING_CATEGORIES = ("enc_gemm", "enc_attn", "layernorm", "dec_gemm", "dec_attn", "other", "enc_gemm_ln", "dec_ar",
-                         "score_tail")
+                         "score_tail", "beam_select")
 
     def get_timing(self):
         out = {}
@@ -240,6 +247,13 @@ class Engine:
         a = ScoreArgsC(batch, int(targets.shape[0]), per_image.data_ptr(), targets.data_ptr(), lengths.data_ptr())
         fn = self.lib.parseq_score_u8 if u8 else self.lib.parseq_score
         check(self.lib, fn(self.handle, C.byref(a), images_ptr, scores_ptr, token_lp_ptr, stream))
+
+    # ids [N, K, num_steps] / lengths [N, K] / scores [N, K]: device pointers; class_mask_ptr as in forward
+    def beam_search(self, images_ptr, batch, beam_width, ids_ptr, lengths_ptr, scores_ptr, stream, max_length=None,
+                    class_mask_ptr=None, u8=False):
+        a = BeamArgsC(batch, int(beam_width), -1 if max_length is None else int(max_length), class_mask_ptr)
+        fn = self.lib.parseq_beam_search_u8 if u8 else self.lib.parseq_beam_search
+        check(self.lib, fn(self.handle, C.byref(a), images_ptr, ids_ptr, lengths_ptr, scores_ptr, stream))
 
     def postprocess(self, logits_ptr, batch, num_steps, ids_ptr, lengths_ptr, conf_ptr, stream, eos_id=0):
         check(self.lib, self.lib.parseq_postprocess(logits_ptr, batch, num_steps, self.cfg.num_classes, eos_id, ids_ptr,

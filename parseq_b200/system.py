@@ -187,6 +187,16 @@ def pack_candidates(tokenizer: Tokenizer, candidates: Candidates, batch: int, ma
     return table[pick], word_len[pick], per_image
 
 
+BEAM_WIDTH_MAX = 16
+
+
+def check_beam_width(beam_width) -> int:
+    """The beam width of a beam_search call: an int in [1, BEAM_WIDTH_MAX] (ValueError otherwise)."""
+    if isinstance(beam_width, bool) or not isinstance(beam_width, int) or not 1 <= beam_width <= BEAM_WIDTH_MAX:
+        raise ValueError(f"beam_width must be an int in [1, {BEAM_WIDTH_MAX}], got {beam_width!r}")
+    return beam_width
+
+
 def _mask_ptr(mask: Optional[Tensor]):
     return mask.data_ptr() if mask is not None else None
 
@@ -374,6 +384,35 @@ class _EngineModule(nn.Module):
                   tlp.data_ptr() if tlp is not None else None, torch.cuda.current_stream(dev).cuda_stream,
                   u8=images.dtype == torch.uint8)
         return (scores, tlp) if return_token_logprobs else scores
+
+    def beam_search(self, images: Union[Tensor, List[Any]], beam_width: int = 5, max_length: Optional[int] = None, *,
+                    rotation: int = 0, class_mask: Optional[Tensor] = None):
+        """Beam search (parseq_beam_search): the `beam_width` most likely readings of each image, best first, as raw
+        (ids int32 [N, K, num_steps] = c_1..c_n then 0, lengths int32 [N, K] (-1: no hypothesis), scores fp32 [N, K]
+        (-inf: no hypothesis)) on the device.  A hypothesis's score is its AR log-likelihood, the quantity `score`
+        computes.  `images` as forward takes them; `class_mask`: per-image allowlist words (allowlist_mask)."""
+        check_beam_width(beam_width)
+        if max_length is not None and int(max_length) < 0:
+            raise ValueError(f"max_length must be None or >= 0, got {max_length}")
+        eng = self.engine()
+        if isinstance(images, (list, tuple)):
+            images = self.preprocess(images, rotation)
+        elif rotation:
+            raise ValueError("rotation applies to lists of raw crops; a tensor input is already at img_size")
+        images = self._check_images(images)
+        dev = images.device
+        N, K, S = images.shape[0], int(beam_width), eng.num_steps(max_length)
+        if class_mask is not None:
+            if tuple(class_mask.shape) != (N, (self.cfg.num_classes + 31) // 32) or class_mask.dtype != torch.int32:
+                raise ValueError(f"class_mask must be int32 [{N}, {(self.cfg.num_classes + 31) // 32}]")
+            class_mask = class_mask.to(dev, non_blocking=True).contiguous()
+        ids = torch.empty((N, K, S), dtype=torch.int32, device=dev)
+        lengths = torch.empty((N, K), dtype=torch.int32, device=dev)
+        scores = torch.empty((N, K), dtype=torch.float32, device=dev)
+        eng.beam_search(images.data_ptr(), N, K, ids.data_ptr(), lengths.data_ptr(), scores.data_ptr(),
+                        torch.cuda.current_stream(dev).cuda_stream, max_length, _mask_ptr(class_mask),
+                        u8=images.dtype == torch.uint8)
+        return ids, lengths, scores
 
     def _run_crops(self, crops, max_length, decode_ar, refine_iters, rotation, class_mask=None):
         """Raw crops of any size: CUDA crops run parseq_forward_crops and return CUDA tensors; CPU crops and PIL images
@@ -619,6 +658,25 @@ class _System(nn.Module):
         best_h = best.tolist()
         labels = [rows[b][k] for b, k in enumerate(best_h)]
         return labels, scores.gather(1, best[:, None])[:, 0]
+
+    def beam_search(self, images: Union[Tensor, List[Any]], beam_width: int = 5, max_length: Optional[int] = None, *,
+                    rotation: int = 0, allowlist: Allowlist = None):
+        """The `beam_width` most likely readings of each image by beam search on the device, as (labels, scores):
+        labels[b] lists image b's hypotheses best first (fewer than beam_width when fewer exist), scores is fp32
+        [N, beam_width], -inf padded, with each hypothesis's AR log-likelihood (what `score` returns for that label).
+        PARSeq runs its AR decoder without refinement, whatever decode_ar / refine_iters say; ViTSTR searches over its
+        per-position logits.  With beam_width = 1 the label is the greedy AR reading.  `images` as forward takes them;
+        `allowlist` as in forward.  The scores are on the images' device (CPU for CPU crops)."""
+        check_beam_width(beam_width)
+        N = len(images) if isinstance(images, (list, tuple)) else images.shape[0]
+        mask = self.allowlist_mask(allowlist, N)
+        ids, lengths, scores = self.model.beam_search(images, beam_width, max_length, rotation=rotation, class_mask=mask)
+        ids_h, len_h = ids.cpu().tolist(), lengths.cpu().tolist()
+        labels = [[self.tokenizer._ids2tok(ids_h[b][k][:n], True) for k, n in enumerate(len_h[b]) if n >= 0]
+                  for b in range(N)]
+        if isinstance(images, (list, tuple)) and all(not (isinstance(c, Tensor) and c.is_cuda) for c in images):
+            scores = scores.cpu()
+        return labels, scores
 
     # base.py:112-143,179-180 (test path only; validation loss is a training concern)
     def _eval_step(self, batch, validation: bool = False):

@@ -196,6 +196,50 @@ int parseq_beam_search(parseq_engine* e, const parseq_beam_args* a, const float*
 int parseq_beam_search_u8(parseq_engine* e, const parseq_beam_args* a, const uint8_t* images_hwc, int32_t* ids,
                           int32_t* lengths, float* scores, parseq_stream_t stream);
 
+/* Lexicon-constrained beam search: every hypothesis is a word of a lexicon, at a cost that depends on the beam width and
+ * not on the lexicon's size.  A lexicon is a set of words over the head classes 1..C-1, compiled to a rooted DAG in
+ * topological numbering (a trie is one): nodes 0..V-1, terminal[v] != 0 when the path from a root to v spells a word, and
+ * the edges of node v at first_edge[v] .. first_edge[v+1]-1, each with a head class edge_class (1..C-1, strictly
+ * increasing within a node) and a child edge_child (> v).  Image b starts at node roots[b].
+ * The rule is parseq_beam_search's, except that each slot also carries its node v.  At step i an active slot
+ *   - takes its LSE exactly as there: over the allowlist-allowed classes of the whole row, not over v's children (the
+ *     lexicon restricts the hypotheses, it does not renormalise the model);
+ *   - may expand EOS iff terminal[v], and each edge class c of v iff the allowlist allows c, logit[c] != -inf and
+ *     i + 1 < num_steps (a character leaves room for its EOS);
+ *   - expands its K best expandable classes in the row order; a character moves the child to edge_child, EOS finishes it
+ *     with length i.
+ * The pool, the stable sort, NaN ranking and -inf handling are unchanged.  So every hypothesis is a word of at most
+ * num_steps - 1 characters that ended with EOS, and its score is parseq_score's for that word; with K >= the number of
+ * words and no allowlist or -inf pruning the search is exhaustive (distinct prefixes of one length are distinct words). */
+typedef struct parseq_lexicon parseq_lexicon;   /* a lexicon on an engine's device (parseq_lexicon_create) */
+typedef struct parseq_lexicon_desc {
+  int32_t num_nodes, num_edges;   /* V >= 1, E >= 0 (E = 0: the lexicon {""}) */
+  const int32_t* first_edge;      /* HOST int32 [V + 1], non-decreasing, first_edge[0] = 0, first_edge[V] = E */
+  const int32_t* edge_class;      /* HOST int32 [E] */
+  const int32_t* edge_child;      /* HOST int32 [E] */
+  const uint8_t* terminal;        /* HOST uint8 [V], nonzero where the node ends a word */
+} parseq_lexicon_desc;
+/* The host checks of a lexicon against a configuration, without a handle or a device (PARSEQ_ERR_INVALID_ARG): counts,
+ * first_edge monotone and ending at E, classes in 1..C-1 and strictly increasing within a node, children in v+1..V-1, and
+ * no path longer than max_label_length edges. */
+int parseq_lexicon_check(const parseq_config* cfg, const parseq_lexicon_desc* d);
+/* Checks the lexicon against the engine's configuration, then uploads it to the engine's device on `stream` (the call
+ * returns once the copy is done; the host arrays are not kept).  The handle may serve any engine on that device with the
+ * same number of classes, and outlives the engine it was made with. */
+int parseq_lexicon_create(parseq_engine* e, const parseq_lexicon_desc* d, parseq_lexicon** out, parseq_stream_t stream);
+void parseq_lexicon_destroy(parseq_lexicon* lx);
+/* parseq_beam_search under a lexicon; `roots` HOST int32 [batch] (each in 0..V-1; pageable or pinned, copied before the
+ * call returns, so the buffer may be reused at once) or NULL for node 0 everywhere.  Outputs as parseq_beam_search.  Checked on the host before anything is launched: the lexicon is
+ * on the engine's device with the engine's number of classes, and every root is a node.  The first lexicon call allocates
+ * the lexicon's beam state (a node per beam row, double-buffered) and, above 128 classes, one fp32 logits buffer per stage:
+ * the lexicon step reads the chain's logits rows rather than the top-K epilogue's keys, whose classes need not be
+ * children of the slot's node. */
+int parseq_beam_search_lexicon(parseq_engine* e, const parseq_beam_args* a, const parseq_lexicon* lx, const int32_t* roots,
+                               const float* images, int32_t* ids, int32_t* lengths, float* scores, parseq_stream_t stream);
+int parseq_beam_search_lexicon_u8(parseq_engine* e, const parseq_beam_args* a, const parseq_lexicon* lx,
+                                  const int32_t* roots, const uint8_t* images_hwc, int32_t* ids, int32_t* lengths,
+                                  float* scores, parseq_stream_t stream);
+
 /* Fused post-processing of BaseSystem._eval_step (strhub/models/base.py:132-142) + Tokenizer._filter
  * (strhub/data/utils.py:120-129): DEVICE logits [N, num_steps, num_classes] -> ids [N, num_steps] (greedy), lengths [N]
  * (index of the first EOS, num_steps if none) and confidence [N] (product of the max softmax probabilities up to and

@@ -669,6 +669,9 @@ struct parseq_engine {
       float2* part = nullptr;               // > 128 classes: the top-K epilogue's LSE partials [lrows][ceil(C / 128)]
       unsigned long long* keys = nullptr;   //   and keys [lrows][ceil(C / 128)][BEAM_TOPK_LD]
       std::vector<__nv_bfloat16*> kvc;
+      // lexicon search (parseq_beam_search_lexicon), allocated by the first lexicon call: each beam row's lexicon node,
+      // double-buffered; above 128 classes `logits` is allocated then as well (the lexicon step reads whole rows)
+      int* node[2] = {nullptr, nullptr};
     } bm;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev_enc = nullptr, ev_done = nullptr;
@@ -698,6 +701,8 @@ struct parseq_engine {
   unsigned char* sc_causal = nullptr;
   float2* sc_vt_part = nullptr;
   long long beam_bytes = 0;         // device bytes of the beam-search buffers (0 until the first beam call)
+  int* lex_roots = nullptr;         // the lexicon call's roots [lex_roots_cap] (grown on demand)
+  int lex_roots_cap = 0;
   bool use_graph = true;
   struct GraphEntry { cudaGraphExec_t exec; long long kernels; };
   std::map<std::vector<int>, GraphEntry> graphs;
@@ -705,6 +710,15 @@ struct parseq_engine {
   void* w(const std::string& k) const { return slots[index.at(k)].dev; }
   const float* wf(const std::string& k) const { return reinterpret_cast<const float*>(w(k)); }
   const __nv_bfloat16* wb(const std::string& k) const { return reinterpret_cast<const __nv_bfloat16*>(w(k)); }
+};
+
+// A lexicon DAG on one device (parseq_lexicon_create): the CSR arrays of parseq_lexicon_desc
+struct parseq_lexicon {
+  int device = 0, C = 0, V = 0, E = 0;
+  int* first_edge = nullptr;        // [V + 1]
+  int* edge_class = nullptr;        // [max(E, 1)]
+  int* edge_child = nullptr;        // [max(E, 1)]
+  unsigned char* terminal = nullptr;   // [V]
 };
 
 namespace {
@@ -806,6 +820,8 @@ void free_workspace(parseq_engine* e) {
     if (p) cudaFree(p);
   e->sc_meta = nullptr; e->sc_meta_ints = 0; e->sc_causal = nullptr; e->sc_vt_part = nullptr;
   e->beam_bytes = 0;
+  if (e->lex_roots) { cudaFree(e->lex_roots); e->lex_roots = nullptr; }
+  e->lex_roots_cap = 0;
   if (e->ev_enc) { cudaEventDestroy(e->ev_enc); e->ev_enc = nullptr; }
   e->a_pe = e->xn = e->qkv = e->att = e->hid = e->mem = e->ckv = nullptr;
   e->x = e->in_images = e->out_logits = nullptr;
@@ -818,7 +834,7 @@ void free_workspace(parseq_engine* e) {
     if (sg.lse_part) cudaFree(sg.lse_part);
     if (sg.lse_tlogit) cudaFree(sg.lse_tlogit);
     void* bq[] = {sg.bm.ids[0], sg.bm.ids[1], sg.bm.score[0], sg.bm.score[1], sg.bm.len[0], sg.bm.len[1], sg.bm.st[0],
-                  sg.bm.st[1], sg.bm.parent, sg.bm.logits, sg.bm.part, sg.bm.keys};
+                  sg.bm.st[1], sg.bm.parent, sg.bm.logits, sg.bm.part, sg.bm.keys, sg.bm.node[0], sg.bm.node[1]};
     for (void* p : bq)
       if (p) cudaFree(p);
     for (auto p : sg.bm.kvc)
@@ -2126,18 +2142,47 @@ int beam_reserve(parseq_engine* e) {
   return PARSEQ_OK;
 }
 
+// ViTSTR under a lexicon: images per beam group.  Its head writes the group's [G * L, C] fp32 logits, which above 128
+// classes can be large: the group holds at most 2^21 logits (8 MB; e.g. 4 images at 16384 classes and L = 26) or one image.
+// At <= 128 classes this is beam_vt_images, so the plain beam's logits buffer serves.
+int beam_lex_vt_images(const parseq_engine* e) {
+  const long long per = 1ll * e->L * e->C;
+  return static_cast<int>(std::max(1ll, std::min<long long>(beam_vt_images(e), (1ll << 21) / per)));
+}
+
+// Lexicon buffers, on the first lexicon call (after beam_reserve; counted in beam_bytes): each beam row's node,
+// double-buffered, and above 128 classes the fp32 logits of a stage's rows (PARSeq: dec_chunk rows, 8 MB at 16384 classes
+// and dec_chunk 128; ViTSTR: beam_lex_vt_images images' L positions).
+int lexicon_reserve(parseq_engine* e) {
+  const size_t nst = e->arch == 0 ? e->stages.size() : 1;
+  auto grab = [&](auto** p, long long n) -> int {
+    if (*p != nullptr) return PARSEQ_OK;
+    PQ_TRY(dev_alloc(p, n));
+    e->beam_bytes += n * static_cast<long long>(sizeof(**p));
+    return PARSEQ_OK;
+  };
+  for (size_t s = 0; s < nst; ++s) {
+    parseq_engine::Stage::Beam& bm = e->stages[s].bm;
+    for (int h = 0; h < 2; ++h) PQ_TRY(grab(&bm.node[h], bm.rows));
+    const long long lrows = e->arch == 0 ? e->dec_chunk : 1ll * beam_lex_vt_images(e) * e->L;
+    PQ_TRY(grab(&bm.logits, lrows * e->C));
+  }
+  return PARSEQ_OK;
+}
+
 // Beam search over a batch of images (parseq_beam_search).  PARSeq: the encoder and the cross K/V once per super-chunk as
 // forward_super runs them, then groups of dec_chunk / K images (all K beams of an image in one group) round-robin over
 // the stages' streams; each step is one decoder pass over the group's beam rows (decode_pass with DecodeExtras::beam),
 // the head's logits of the step, and beam_select_kernel.  ViTSTR: the head once over a group's [B * L] token rows, then
 // beam_select_kernel once per position.
 int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_any, bool u8, int* ids, int* lengths,
-              float* scores, cudaStream_t user) {
+              float* scores, cudaStream_t user, const parseq_lexicon* lx = nullptr, const int* roots = nullptr) {
   const int N = a->batch, K = a->beam_width, D = e->D, T = e->T, C = e->C, L = e->L;
   const int S = num_steps_of(e, a->max_length);
   const long long img_sz = 3ll * e->cfg.img_h * e->cfg.img_w * (u8 ? 1 : 4);
   const char* images = static_cast<const char*>(images_any);
   PQ_TRY(beam_reserve(e));
+  if (lx != nullptr) PQ_TRY(lexicon_reserve(e));
   auto init = [&](parseq_engine::Stage::Beam& bm, int B, cudaStream_t st) {
     const int n = B * K * e->ids_ld;
     e->launches++;
@@ -2146,33 +2191,57 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
   };
   // step `step` of the group whose first image is g0 (in the call's batch)
   const bool wide = C > 128;
+  const bool topk = wide && lx == nullptr;           // the head's top-K epilogue (the lexicon step reads whole rows)
   const int ntiles = (C + pq::GEMM_BLOCK_N - 1) / pq::GEMM_BLOCK_N;
+  if (lx != nullptr && roots != nullptr) {
+    // `roots`: the checked host copy of the call's roots (beam_lexicon_call), uploaded below
+    if (e->lex_roots_cap < N) {
+      if (e->lex_roots != nullptr) {
+        PQ_CUDA(cudaStreamSynchronize(e->main));                      // the previous call's kernels may still read it
+        PQ_CUDA(cudaFree(e->lex_roots));
+        e->beam_bytes -= 4ll * e->lex_roots_cap;
+        e->lex_roots = nullptr;
+        e->lex_roots_cap = 0;
+      }
+      PQ_TRY(dev_alloc(&e->lex_roots, N));
+      e->lex_roots_cap = N;
+      e->beam_bytes += 4ll * N;
+    }
+  }
   auto select = [&](parseq_engine::Stage::Beam& bm, int B, int step, long long row0, long long img_stride,
                     long long slot_stride, int g0, cudaStream_t st) {
     const int cur = step & 1, nxt = cur ^ 1;
     TimedScope ts(e, st, CAT_BEAM, 0.0);
-    return launch_k(e->lo, pq::beam_select_kernel, dim3(static_cast<unsigned>(B)), dim3(pq::BEAM_THREADS), 0, st,
+    pq::BeamLex bl{};
+    if (lx != nullptr)
+      bl = pq::BeamLex{lx->first_edge, lx->edge_class, lx->edge_child, lx->terminal,
+                       roots != nullptr ? e->lex_roots + g0 : nullptr, bm.node[cur], bm.node[nxt]};
+    return launch_k(e->lo, lx != nullptr ? pq::beam_select_kernel<true> : pq::beam_select_kernel<false>,
+                    dim3(static_cast<unsigned>(B)), dim3(pq::BEAM_THREADS), 0, st,
                     static_cast<const float*>(bm.logits), static_cast<const float2*>(bm.part),
-                    static_cast<const unsigned long long*>(bm.keys), ntiles, row0, img_stride, slot_stride, C, K, step, S, a->class_mask ? a->class_mask + 1ll * g0 * e->mask_ld : nullptr, e->mask_ld,
+                    static_cast<const unsigned long long*>(topk ? bm.keys : nullptr), ntiles, row0, img_stride, slot_stride, C, K, step, S, a->class_mask ? a->class_mask + 1ll * g0 * e->mask_ld : nullptr, e->mask_ld,
                     static_cast<const int*>(bm.ids[cur]), static_cast<const float*>(bm.score[cur]),
                     static_cast<const int*>(bm.len[cur]), static_cast<const int*>(bm.st[cur]), bm.ids[nxt], bm.score[nxt],
                     bm.len[nxt], bm.st[nxt], bm.parent, e->ids_ld, ids + 1ll * g0 * K * S, lengths + 1ll * g0 * K,
-                    scores + 1ll * g0 * K);
+                    scores + 1ll * g0 * K, bl);
   };
   PQ_CUDA(cudaEventRecord(e->ev_in, user));
   PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_in, 0));
+  // pageable source (a std::vector of beam_lexicon_call): the copy is staged before the call returns
+  if (lx != nullptr && roots != nullptr)
+    PQ_CUDA(cudaMemcpyAsync(e->lex_roots, roots, 4ull * N, cudaMemcpyHostToDevice, e->main));
   for (int b0 = 0; b0 < N; b0 += e->max_batch) {
     const int Bc = std::min(N - b0, e->max_batch);
     if (e->arch == 1) {
       parseq_engine::Stage::Beam& bm = e->stages[0].bm;
-      const int G = beam_vt_images(e);
+      const int G = lx != nullptr ? beam_lex_vt_images(e) : beam_vt_images(e);
       for (int o = 0; o < Bc; o += e->chunk) {
         const int Bs = std::min(Bc - o, e->chunk);
         PQ_TRY(encode_chunk(e, images + (b0 + o) * img_sz, u8, Bs, nullptr, nullptr, e->main, false));
         PQ_TRY(vitstr_rows(e, Bs, L, e->main));
         for (int g = 0; g < Bs; g += G) {
           const int Bg = std::min(G, Bs - g);
-          if (wide) {
+          if (topk) {
             // the top-K epilogue over the group's [Bg * L] token rows: row r belongs to image r / L
             TimedScope ts(e, e->main, CAT_DEC_GEMM, 2.0 * Bg * L * C * D);
             PQ_TRY(gemm_topk_launch(e->lo, e->xn + 1ll * g * L * D, D, e->w("head.weight"), D, e->wf("head.bias"), Bg * L, C, D, K,
@@ -2211,7 +2280,7 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
       PQ_TRY(init(bm, Bg, ds));
       DecodeExtras ex;
       ex.beam = K;
-      if (wide) {
+      if (topk) {
         ex.beam_part = bm.part;
         ex.beam_keys = bm.keys;
         ex.beam_k = K;
@@ -2221,7 +2290,8 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
       int rc = PARSEQ_OK;
       for (int step = 0; step < S && rc == PARSEQ_OK; ++step) {
         // query position `step` over keys 0..step of every beam row; the head leaves row r's logits at bm.logits + r * C
-        // (<= 128 classes) or its partials and top-K keys (above)
+        // (<= 128 classes, and at every C under a lexicon: the chain's head GEMM, no argmax) or its partials and top-K
+        // keys (above)
         rc = decode_pass(e, sg, g0, R, 1, step, step + 1, 0, bm.ids[step & 1], bm.logits, C, nullptr, 0, nullptr, 0, nullptr,
                          ds, &ex, /*ar_step*/ true);
         if (rc == PARSEQ_OK) rc = select(bm, Bg, step, 0, K, 1, b0 + g0, ds);
@@ -2256,6 +2326,40 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
   return PARSEQ_OK;
 }
 
+// The host checks of a lexicon (parseq_lexicon_check) against C head classes and labels of at most max_label_length
+int check_lexicon(const parseq_lexicon_desc* d, int num_classes, int max_label_length) {
+  if (d == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  const int V = d->num_nodes, E = d->num_edges;
+  if (V <= 0 || E < 0) return fail(PARSEQ_ERR_INVALID_ARG, "lexicon: num_nodes must be >= 1 and num_edges >= 0");
+  if (d->first_edge == nullptr || d->terminal == nullptr || (E > 0 && (d->edge_class == nullptr || d->edge_child == nullptr)))
+    return fail(PARSEQ_ERR_INVALID_ARG, "lexicon: null array");
+  if (d->first_edge[0] != 0 || d->first_edge[V] != E)
+    return fail(PARSEQ_ERR_INVALID_ARG, "lexicon: first_edge must start at 0 and end at num_edges = " + std::to_string(E));
+  std::vector<int> depth(static_cast<size_t>(V), 0);   // longest path ending at each node, in index order
+  for (int v = 0; v < V; ++v) {
+    const int e0 = d->first_edge[v], e1 = d->first_edge[v + 1];
+    if (e1 < e0 || e1 > E) return fail(PARSEQ_ERR_INVALID_ARG, "lexicon: first_edge is not monotone at node " + std::to_string(v));
+    for (int j = e0; j < e1; ++j) {
+      const int c = d->edge_class[j], ch = d->edge_child[j];
+      if (c < 1 || c >= num_classes)
+        return fail(PARSEQ_ERR_INVALID_ARG, "lexicon: edge " + std::to_string(j) + " has class " + std::to_string(c) +
+                                                ", outside 1.." + std::to_string(num_classes - 1));
+      if (j > e0 && c <= d->edge_class[j - 1])
+        return fail(PARSEQ_ERR_INVALID_ARG, "lexicon: edge classes of node " + std::to_string(v) +
+                                                " are not strictly increasing");
+      if (ch <= v || ch >= V)
+        return fail(PARSEQ_ERR_INVALID_ARG, "lexicon: edge " + std::to_string(j) + " of node " + std::to_string(v) +
+                                                " has child " + std::to_string(ch) + ", not in " + std::to_string(v + 1) +
+                                                ".." + std::to_string(V - 1));
+      depth[static_cast<size_t>(ch)] = std::max(depth[static_cast<size_t>(ch)], depth[static_cast<size_t>(v)] + 1);
+    }
+    if (depth[static_cast<size_t>(v)] > max_label_length)
+      return fail(PARSEQ_ERR_INVALID_ARG, "lexicon: a path of " + std::to_string(depth[static_cast<size_t>(v)]) +
+                                              " characters, more than max_label_length = " + std::to_string(max_label_length));
+  }
+  return PARSEQ_OK;
+}
+
 // Checks of the beam entry points, all on the host before anything is launched.
 int check_beam_call(parseq_engine* e, const parseq_beam_args* a, const void* images, const int* ids, const int* lengths,
                     const float* scores) {
@@ -2272,6 +2376,32 @@ int check_beam_call(parseq_engine* e, const parseq_beam_args* a, const void* ima
     return fail(PARSEQ_ERR_INVALID_ARG, "beam_width " + std::to_string(a->beam_width) + " exceeds the decoder chunk (option "
                                         "dec_chunk = " + std::to_string(e->dec_chunk) + ")");
   return PARSEQ_OK;
+}
+
+// The lexicon beam entry points: the beam checks, the lexicon against the engine, every root a node; then beam_impl
+int beam_lexicon_call(parseq_engine* e, const parseq_beam_args* a, const parseq_lexicon* lx, const int32_t* roots,
+                      const void* images, bool u8, int32_t* ids, int32_t* lengths, float* scores, parseq_stream_t stream) {
+  PQ_TRY(check_beam_call(e, a, images, ids, lengths, scores));
+  if (lx == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null lexicon");
+  if (lx->device != e->cfg.device || lx->C != e->C)
+    return fail(PARSEQ_ERR_INVALID_ARG, "lexicon was made for device " + std::to_string(lx->device) + " and " +
+                                            std::to_string(lx->C) + " classes, the engine has device " +
+                                            std::to_string(e->cfg.device) + " and " + std::to_string(e->C));
+  // the roots are read once, into a host copy that is checked and then uploaded: the caller's buffer (pageable or
+  // pinned) may change as soon as the call returns, and the device only ever sees checked values
+  std::vector<int> rv;
+  if (roots != nullptr) {
+    rv.assign(roots, roots + a->batch);
+    for (int b = 0; b < a->batch; ++b)
+      if (rv[static_cast<size_t>(b)] < 0 || rv[static_cast<size_t>(b)] >= lx->V)
+        return fail(PARSEQ_ERR_INVALID_ARG, "root " + std::to_string(rv[static_cast<size_t>(b)]) + " of image " +
+                                                std::to_string(b) + " is not a node of the lexicon (0.." +
+                                                std::to_string(lx->V - 1) + ")");
+  }
+  if (a->batch == 0) return PARSEQ_OK;
+  PQ_CUDA(cudaSetDevice(e->cfg.device));
+  return beam_impl(e, a, images, u8, ids, lengths, scores, reinterpret_cast<cudaStream_t>(stream), lx,
+                   roots != nullptr ? rv.data() : nullptr);
 }
 
 }  // namespace
@@ -2662,6 +2792,61 @@ int parseq_beam_search_u8(parseq_engine* e, const parseq_beam_args* a, const uin
   if (a->batch == 0) return PARSEQ_OK;
   PQ_CUDA(cudaSetDevice(e->cfg.device));
   return beam_impl(e, a, images_hwc, true, ids, lengths, scores, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int parseq_lexicon_check(const parseq_config* cfg, const parseq_lexicon_desc* d) {
+  if (cfg == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  return check_lexicon(d, cfg->num_tokens - 2, cfg->max_label_length);
+}
+
+int parseq_lexicon_create(parseq_engine* e, const parseq_lexicon_desc* d, parseq_lexicon** out, parseq_stream_t stream) {
+  if (e == nullptr || out == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  *out = nullptr;
+  PQ_TRY(check_lexicon(d, e->C, e->cfg.max_label_length));
+  PQ_CUDA(cudaSetDevice(e->cfg.device));
+  auto* lx = new parseq_lexicon();
+  lx->device = e->cfg.device; lx->C = e->C; lx->V = d->num_nodes; lx->E = d->num_edges;
+  const long long E1 = std::max(d->num_edges, 1);
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int rc = dev_alloc(&lx->first_edge, lx->V + 1ll);
+  if (rc == PARSEQ_OK) rc = dev_alloc(&lx->edge_class, E1);
+  if (rc == PARSEQ_OK) rc = dev_alloc(&lx->edge_child, E1);
+  if (rc == PARSEQ_OK) rc = dev_alloc(&lx->terminal, lx->V);
+  auto up = [&](void* dst, const void* src, long long bytes) {
+    if (rc == PARSEQ_OK && bytes > 0 && cudaMemcpyAsync(dst, src, static_cast<size_t>(bytes), cudaMemcpyHostToDevice, st) != cudaSuccess)
+      rc = fail(PARSEQ_ERR_CUDA, "lexicon upload failed");
+  };
+  up(lx->first_edge, d->first_edge, 4ll * (lx->V + 1));
+  up(lx->edge_class, d->edge_class, 4ll * lx->E);
+  up(lx->edge_child, d->edge_child, 4ll * lx->E);
+  up(lx->terminal, d->terminal, lx->V);
+  if (rc == PARSEQ_OK && cudaStreamSynchronize(st) != cudaSuccess) rc = fail(PARSEQ_ERR_CUDA, "lexicon upload failed");
+  if (rc != PARSEQ_OK) {
+    parseq_lexicon_destroy(lx);
+    return rc;
+  }
+  *out = lx;
+  return PARSEQ_OK;
+}
+
+void parseq_lexicon_destroy(parseq_lexicon* lx) {
+  if (lx == nullptr) return;
+  cudaSetDevice(lx->device);
+  void* p[] = {lx->first_edge, lx->edge_class, lx->edge_child, lx->terminal};
+  for (void* q : p)
+    if (q) cudaFree(q);
+  delete lx;
+}
+
+int parseq_beam_search_lexicon(parseq_engine* e, const parseq_beam_args* a, const parseq_lexicon* lx, const int32_t* roots,
+                               const float* images, int32_t* ids, int32_t* lengths, float* scores, parseq_stream_t stream) {
+  return beam_lexicon_call(e, a, lx, roots, images, false, ids, lengths, scores, stream);
+}
+
+int parseq_beam_search_lexicon_u8(parseq_engine* e, const parseq_beam_args* a, const parseq_lexicon* lx,
+                                  const int32_t* roots, const uint8_t* images_hwc, int32_t* ids, int32_t* lengths,
+                                  float* scores, parseq_stream_t stream) {
+  return beam_lexicon_call(e, a, lx, roots, images_hwc, true, ids, lengths, scores, stream);
 }
 
 int parseq_postprocess(const float* logits, int32_t batch, int32_t num_steps, int32_t num_classes, int32_t eos_id, int32_t* ids,

@@ -1012,20 +1012,38 @@ __global__ void beam_init_kernel(int* __restrict__ ids, float* __restrict__ scor
 //   4. The new state goes to the *_out buffers, parent[r] = the state row each new slot came from (the K/V cache rows
 //      follow it at depth >= 2), and after the last step the results: out_ids [K][num_steps] per image (c_1..c_n, then
 //      0 = EOS / padding), out_len (-1 empty), out_score (-inf empty).
+// LEX (parseq_beam_search_lexicon): each slot also walks a lexicon DAG (BeamLex).  Its LSE is taken exactly as above
+// from the whole logits row (the lexicon step always has the row: topk is null at every C), but only the node's
+// expandable classes enter the lanes' lists: the lanes stride over the node's edges (class allowed, logit != -inf, and
+// step + 1 < num_steps so that a character leaves room for its EOS), lane 0 adds EOS when the node is terminal.  Lanes
+// k < K then find the child of the slot's k-th expansion by binary search over the node's sorted edge classes; the child
+// travels with the pool entry into node_out (-1 for a finished or empty slot).  Step 0 takes slot 0's node from roots.
 // No early griddepcontrol.launch_dependents: what comes next reads the state this grid writes.
+struct BeamLex {
+  const int* first_edge;            // [V + 1]
+  const int* edge_class;            // [E], strictly increasing within a node
+  const int* edge_child;            // [E]
+  const unsigned char* terminal;    // [V]
+  const int* roots;                 // [images of the group] or null (node 0)
+  const int* node_in;               // [rows]
+  int* node_out;                    // [rows]
+};
+template <bool LEX>
 __global__ void __launch_bounds__(BEAM_THREADS) beam_select_kernel(
     const float* __restrict__ logits, const float2* __restrict__ part, const unsigned long long* __restrict__ topk,
     int ntiles, long long row0, long long img_stride, long long slot_stride, int C, int K, int step, int num_steps,
     const uint32_t* __restrict__ mask, int mask_ld, const int* __restrict__ ids_in, const float* __restrict__ score_in,
     const int* __restrict__ len_in, const int* __restrict__ st_in, int* __restrict__ ids_out, float* __restrict__ score_out,
     int* __restrict__ len_out, int* __restrict__ st_out, int* __restrict__ parent, int ids_ld, int* __restrict__ out_ids,
-    int* __restrict__ out_len, float* __restrict__ out_score) {
+    int* __restrict__ out_len, float* __restrict__ out_score, BeamLex lex) {
   __shared__ unsigned long long s_key[BEAM_MAX][BEAM_MAX];
   __shared__ float s_lse[BEAM_MAX];
   __shared__ float p_score[BEAM_MAX * BEAM_MAX];
   __shared__ int p_slot[BEAM_MAX * BEAM_MAX], p_cls[BEAM_MAX * BEAM_MAX];
   __shared__ int s_sel[BEAM_MAX];
   __shared__ int s_n;
+  __shared__ int s_child[LEX ? BEAM_MAX : 1][BEAM_MAX];
+  __shared__ int p_child[LEX ? BEAM_MAX * BEAM_MAX : 1];
   grid_dep_wait();
   const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int r0 = b * K;
@@ -1051,14 +1069,14 @@ __global__ void __launch_bounds__(BEAM_THREADS) beam_select_kernel(
         if (j == K - 1) thr = top[j];
     };
     float lse;
-    if (topk == nullptr) {
+    if (LEX || topk == nullptr) {
       const float* lr = logits + row * C;
       float m = -INFINITY;
       for (int c = lane; c < C; c += 32) {
         if (mrow != nullptr && !class_allowed(mrow, c)) continue;
         const float x = lr[c];
         m = fmaxf(m, x);
-        if (x != -INFINITY) insert(beam_order_key(x, c));
+        if (!LEX && x != -INFINITY) insert(beam_order_key(x, c));
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
@@ -1080,6 +1098,22 @@ __global__ void __launch_bounds__(BEAM_THREADS) beam_select_kernel(
       if (lane == 0) lse_merge(part + row * ntiles, ntiles, M, S);
       lse = __shfl_sync(0xffffffffu, M + logf(S), 0);
     }
+    int e0 = 0, e1 = 0;
+    if constexpr (LEX) {
+      const int v = step == 0 ? (lex.roots != nullptr ? lex.roots[b] : 0) : lex.node_in[r0 + warp];
+      const float* lr = logits + row * C;
+      e0 = lex.first_edge[v];
+      e1 = lex.first_edge[v + 1];
+      if (step + 1 < num_steps) {
+        for (int ei = e0 + lane; ei < e1; ei += 32) {
+          const int c = lex.edge_class[ei];
+          if (mrow != nullptr && !class_allowed(mrow, c)) continue;
+          const float x = lr[c];
+          if (x != -INFINITY) insert(beam_order_key(x, c));
+        }
+      }
+      if (lane == 0 && lex.terminal[v] != 0 && lr[0] != -INFINITY) insert(beam_order_key(lr[0], 0));
+    }
     int h = 0;
     for (int r = 0; r < K; ++r) {
       unsigned long long cand = 0ull;
@@ -1096,6 +1130,23 @@ __global__ void __launch_bounds__(BEAM_THREADS) beam_select_kernel(
       if (lane == 0) s_key[warp][r] = best;
     }
     if (lane == 0) s_lse[warp] = lse;
+    if constexpr (LEX) {
+      __syncwarp();
+      if (lane < K) {
+        const unsigned long long key = s_key[warp][lane];
+        const int c = key != 0ull ? beam_key_class(key) : 0;
+        int child = -1;
+        if (c != 0) {
+          int lo = e0, hi = e1 - 1;
+          while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (lex.edge_class[mid] < c) lo = mid + 1; else hi = mid;
+          }
+          child = lex.edge_child[lo];
+        }
+        s_child[warp][lane] = child;
+      }
+    }
   }
   __syncthreads();
   if (tid == 0) {
@@ -1104,11 +1155,15 @@ __global__ void __launch_bounds__(BEAM_THREADS) beam_select_kernel(
       const int sk = st_in[r0 + k];
       const float ps = score_in[r0 + k];
       if (sk == BEAM_DONE) {
-        p_score[n] = ps; p_slot[n] = k; p_cls[n] = -1; ++n;
+        p_score[n] = ps; p_slot[n] = k; p_cls[n] = -1;
+        if constexpr (LEX) p_child[n] = -1;
+        ++n;
       } else if (sk == BEAM_ACTIVE) {
         for (int j = 0; j < K && s_key[k][j] != 0ull; ++j) {
           const int c = beam_key_class(s_key[k][j]);
-          p_score[n] = ps + (beam_key_value(s_key[k][j]) - s_lse[k]); p_slot[n] = k; p_cls[n] = c; ++n;
+          p_score[n] = ps + (beam_key_value(s_key[k][j]) - s_lse[k]); p_slot[n] = k; p_cls[n] = c;
+          if constexpr (LEX) p_child[n] = s_child[k][j];
+          ++n;
         }
       }
     }
@@ -1158,6 +1213,7 @@ __global__ void __launch_bounds__(BEAM_THREADS) beam_select_kernel(
     len_out[r0 + k] = ln;
     st_out[r0 + k] = sn;
     parent[r0 + k] = r0 + par;
+    if constexpr (LEX) lex.node_out[r0 + k] = e >= 0 ? p_child[e] : -1;
     if (last) {
       out_len[r0 + k] = ln;
       out_score[r0 + k] = sc;

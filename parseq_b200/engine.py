@@ -38,11 +38,39 @@ class BeamArgsC(C.Structure):
     _fields_ = [("batch", C.c_int32), ("beam_width", C.c_int32), ("max_length", C.c_int32), ("class_mask", C.c_void_p)]
 
 
+class LexiconDescC(C.Structure):
+    _fields_ = [("num_nodes", C.c_int32), ("num_edges", C.c_int32), ("first_edge", C.c_void_p), ("edge_class", C.c_void_p),
+                ("edge_child", C.c_void_p), ("terminal", C.c_void_p)]
+
+
+def lexicon_desc(first_edge, edge_class, edge_child, terminal) -> LexiconDescC:
+    """parseq_lexicon_desc over contiguous numpy arrays (int32, int32, int32, uint8); the caller keeps them alive."""
+    return LexiconDescC(int(terminal.shape[0]), int(edge_class.shape[0]), first_edge.ctypes.data, edge_class.ctypes.data,
+                        edge_child.ctypes.data, terminal.ctypes.data)
+
+
+class LexiconHandle:
+    """Owns one `parseq_lexicon*` (a lexicon on one device)."""
+
+    def __init__(self, lib, ptr):
+        self.lib, self.ptr = lib, ptr
+
+    def __del__(self):
+        try:
+            if self.ptr:
+                self.lib.parseq_lexicon_destroy(self.ptr)
+                self.ptr = None
+        except Exception:
+            pass
+
+
 EXPORTS = [
     "parseq_create", "parseq_destroy", "parseq_set_weight", "parseq_num_weights", "parseq_weight_key",
     "parseq_finalize", "parseq_forward", "parseq_forward_host", "parseq_forward_u8", "parseq_forward_host_u8",
     "parseq_resize_crops", "parseq_forward_crops", "parseq_forward_host_crops",
     "parseq_score", "parseq_score_u8", "parseq_score_check", "parseq_beam_search", "parseq_beam_search_u8",
+    "parseq_lexicon_check", "parseq_lexicon_create", "parseq_lexicon_destroy", "parseq_beam_search_lexicon",
+    "parseq_beam_search_lexicon_u8",
     "parseq_postprocess", "parseq_encode", "parseq_decode", "parseq_decode_ex", "parseq_head", "parseq_text_embed", "parseq_kernel_launches", "parseq_debug_int", "parseq_bench_tma_stream",
     "parseq_set_option", "parseq_get_timing", "parseq_get_ar_profile", "parseq_last_error", "parseq_version", "parseq_gemm_bf16", "parseq_gemm_ln_bf16", "parseq_mlp_ln_bf16", "parseq_layernorm_bf16",
     "parseq_enc_attention", "parseq_qkv_attention_bf16",
@@ -88,6 +116,13 @@ def load_library(path: Optional[str] = None):
     lib.parseq_beam_search.argtypes = [C.c_void_p, C.POINTER(BeamArgsC), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p]
     lib.parseq_beam_search_u8.argtypes = lib.parseq_beam_search.argtypes
+    lib.parseq_lexicon_check.argtypes = [C.POINTER(ParseqConfigC), C.POINTER(LexiconDescC)]
+    lib.parseq_lexicon_create.argtypes = [C.c_void_p, C.POINTER(LexiconDescC), C.POINTER(C.c_void_p), C.c_void_p]
+    lib.parseq_lexicon_destroy.argtypes = [C.c_void_p]
+    lib.parseq_lexicon_destroy.restype = None
+    lib.parseq_beam_search_lexicon.argtypes = [C.c_void_p, C.POINTER(BeamArgsC), C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.parseq_beam_search_lexicon_u8.argtypes = lib.parseq_beam_search_lexicon.argtypes
     lib.parseq_postprocess.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p]
     lib.parseq_encode.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -248,12 +283,25 @@ class Engine:
         fn = self.lib.parseq_score_u8 if u8 else self.lib.parseq_score
         check(self.lib, fn(self.handle, C.byref(a), images_ptr, scores_ptr, token_lp_ptr, stream))
 
-    # ids [N, K, num_steps] / lengths [N, K] / scores [N, K]: device pointers; class_mask_ptr as in forward
+    # ids [N, K, num_steps] / lengths [N, K] / scores [N, K]: device pointers; class_mask_ptr as in forward; lexicon: a
+    # LexiconHandle of this engine's device, roots a CPU int32 tensor [N] or None
     def beam_search(self, images_ptr, batch, beam_width, ids_ptr, lengths_ptr, scores_ptr, stream, max_length=None,
-                    class_mask_ptr=None, u8=False):
+                    class_mask_ptr=None, u8=False, lexicon=None, roots=None):
         a = BeamArgsC(batch, int(beam_width), -1 if max_length is None else int(max_length), class_mask_ptr)
-        fn = self.lib.parseq_beam_search_u8 if u8 else self.lib.parseq_beam_search
-        check(self.lib, fn(self.handle, C.byref(a), images_ptr, ids_ptr, lengths_ptr, scores_ptr, stream))
+        if lexicon is None:
+            fn = self.lib.parseq_beam_search_u8 if u8 else self.lib.parseq_beam_search
+            check(self.lib, fn(self.handle, C.byref(a), images_ptr, ids_ptr, lengths_ptr, scores_ptr, stream))
+            return
+        fn = self.lib.parseq_beam_search_lexicon_u8 if u8 else self.lib.parseq_beam_search_lexicon
+        check(self.lib, fn(self.handle, C.byref(a), lexicon.ptr, roots.data_ptr() if roots is not None else None,
+                           images_ptr, ids_ptr, lengths_ptr, scores_ptr, stream))
+
+    def lexicon_create(self, first_edge, edge_class, edge_child, terminal, stream) -> LexiconHandle:
+        """Uploads a lexicon (numpy CSR arrays, parseq_lexicon_desc) to this engine's device."""
+        d = lexicon_desc(first_edge, edge_class, edge_child, terminal)
+        h = C.c_void_p()
+        check(self.lib, self.lib.parseq_lexicon_create(self.handle, C.byref(d), C.byref(h), stream))
+        return LexiconHandle(self.lib, h)
 
     def postprocess(self, logits_ptr, batch, num_steps, ids_ptr, lengths_ptr, conf_ptr, stream, eos_id=0):
         check(self.lib, self.lib.parseq_postprocess(logits_ptr, batch, num_steps, self.cfg.num_classes, eos_id, ids_ptr,

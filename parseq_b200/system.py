@@ -21,6 +21,7 @@ from torch import Tensor, nn
 
 from .config import ParseqConfig, make_config
 from .engine import CropsC, Engine, EngineError
+from .lexicon import Lexicon, check_words, lexicon_rows
 from .tokenizer import CharsetAdapter, Tokenizer
 
 
@@ -151,27 +152,11 @@ def pack_candidates(tokenizer: Tokenizer, candidates: Candidates, batch: int, ma
     """The candidate labels of a score call as the engine takes them (parseq_score_args): CPU int32 targets
     [M, max_label_length + 1] = (c_1..c_n, EOS, 0...), lengths [M] and per_image [batch].  `candidates` is one list of
     strings for every image (a lexicon) or one non-empty list per image; candidates are image-major."""
-    if isinstance(candidates, str) or not isinstance(candidates, (list, tuple)) or len(candidates) == 0:
-        raise TypeError("candidates must be a non-empty list of strings, or one non-empty list of strings per image")
-    shared = all(isinstance(c, str) for c in candidates)
+    shared, rows = lexicon_rows(candidates, batch)
     if shared:
-        rows: List[Sequence[str]] = [candidates] * batch
-    else:
-        rows = list(candidates)
-        if len(rows) != batch:
-            raise ValueError(f"candidates has {len(rows)} lists for {batch} images")
-        for b, r in enumerate(rows):
-            if isinstance(r, str) or not isinstance(r, (list, tuple)) or len(r) == 0 or not all(isinstance(s, str) for s in r):
-                raise TypeError(f"candidates of image {b} must be a non-empty list of strings")
+        rows = [candidates] * batch
     words = sorted(set(candidates) if shared else {s for r in rows for s in r})
-    unknown = sorted({ch for s in words for ch in s
-                      if ch not in tokenizer._stoi or not 1 <= tokenizer._stoi[ch] < num_classes})
-    if unknown:
-        raise ValueError(f"candidate characters not in charset_train: {''.join(unknown)!r}")
-    too_long = [s for s in words if len(s) > max_label_length]
-    if too_long:
-        raise ValueError(f"candidate {too_long[0]!r} has {len(too_long[0])} characters, more than max_label_length = "
-                         f"{max_label_length}")
+    check_words(tokenizer, words, max_label_length, num_classes)
     # one target row per distinct word, then a gather: a lexicon shared by 512 images costs one row per word
     L = max_label_length + 1
     index = {s: i for i, s in enumerate(words)}
@@ -386,12 +371,17 @@ class _EngineModule(nn.Module):
         return (scores, tlp) if return_token_logprobs else scores
 
     def beam_search(self, images: Union[Tensor, List[Any]], beam_width: int = 5, max_length: Optional[int] = None, *,
-                    rotation: int = 0, class_mask: Optional[Tensor] = None):
+                    rotation: int = 0, class_mask: Optional[Tensor] = None, lexicon: Optional[Lexicon] = None,
+                    roots: Optional[Tensor] = None):
         """Beam search (parseq_beam_search): the `beam_width` most likely readings of each image, best first, as raw
         (ids int32 [N, K, num_steps] = c_1..c_n then 0, lengths int32 [N, K] (-1: no hypothesis), scores fp32 [N, K]
         (-inf: no hypothesis)) on the device.  A hypothesis's score is its AR log-likelihood, the quantity `score`
-        computes.  `images` as forward takes them; `class_mask`: per-image allowlist words (allowlist_mask)."""
+        computes.  `images` as forward takes them; `class_mask`: per-image allowlist words (allowlist_mask).
+        `lexicon` (a compiled Lexicon) restricts every hypothesis to its words (parseq_beam_search_lexicon); `roots`:
+        CPU int32 [N], the node each image starts at (Lexicon.roots_for), or None for node 0."""
         check_beam_width(beam_width)
+        if lexicon is None and roots is not None:
+            raise ValueError("roots need a lexicon")
         if max_length is not None and int(max_length) < 0:
             raise ValueError(f"max_length must be None or >= 0, got {max_length}")
         eng = self.engine()
@@ -409,9 +399,19 @@ class _EngineModule(nn.Module):
         ids = torch.empty((N, K, S), dtype=torch.int32, device=dev)
         lengths = torch.empty((N, K), dtype=torch.int32, device=dev)
         scores = torch.empty((N, K), dtype=torch.float32, device=dev)
+        lex = None
+        if lexicon is not None:
+            if lexicon.num_classes != self.cfg.num_classes:
+                raise ValueError(f"lexicon was compiled for {lexicon.num_classes} classes, the model has "
+                                 f"{self.cfg.num_classes}")
+            lex = lexicon.handle(eng)
+            if roots is not None:
+                roots = roots.to(device="cpu", dtype=torch.int32).contiguous()
+                if roots.shape != (N,):
+                    raise ValueError(f"roots must be int32 [{N}]")
         eng.beam_search(images.data_ptr(), N, K, ids.data_ptr(), lengths.data_ptr(), scores.data_ptr(),
                         torch.cuda.current_stream(dev).cuda_stream, max_length, _mask_ptr(class_mask),
-                        u8=images.dtype == torch.uint8)
+                        u8=images.dtype == torch.uint8, lexicon=lex, roots=roots)
         return ids, lengths, scores
 
     def _run_crops(self, crops, max_length, decode_ar, refine_iters, rotation, class_mask=None):
@@ -648,9 +648,27 @@ class _System(nn.Module):
         terms[idx] = tlp
         return grid, terms.view(N, K, L).to(dev)
 
-    def lexicon_decode(self, images: Union[Tensor, List[Any]], lexicon: Candidates, *, rotation: int = 0):
+    def compile_lexicon(self, candidates: Candidates) -> Lexicon:
+        """A word list (shared by every image) or one list per image, compiled for beam_search(lexicon=) and
+        lexicon_decode(beam_width=): checked as score checks candidates, de-duplicated, and built into a prefix trie
+        (a forest with one root per distinct per-image list).  Words match charset_train exactly (no case folding).
+        Compiling once saves the trie build on every call; the device copy is made once per engine."""
+        cfg = self.model.cfg
+        return Lexicon(self.tokenizer, candidates, cfg.max_label_length, cfg.num_classes)
+
+    def lexicon_decode(self, images: Union[Tensor, List[Any]], lexicon: Union[Candidates, Lexicon], *,
+                       rotation: int = 0, beam_width: Optional[int] = None):
         """Lexicon-constrained recognition: for each image the candidate the model rates most likely (score), as
-        (labels, log_probs).  The pick is torch.argmax of the image's scores: the first maximum, or the first NaN."""
+        (labels, log_probs).  The pick is torch.argmax of the image's scores: the first maximum, or the first NaN.
+        With `beam_width` the pick is the best hypothesis of a lexicon-constrained beam search of that width instead,
+        at a cost that does not grow with the lexicon (`lexicon` may then be a compiled Lexicon); an image with no
+        reachable word gets label None and -inf."""
+        if beam_width is not None:
+            labels, scores = self.beam_search(images, beam_width, rotation=rotation, lexicon=lexicon)
+            return [h[0] if h else None for h in labels], scores[:, 0]
+        if isinstance(lexicon, Lexicon):
+            raise TypeError("a compiled Lexicon serves the beam search only: pass beam_width, or the word lists to score "
+                            "every word")
         scores = self.score(images, lexicon, rotation=rotation)
         N = scores.shape[0]
         rows = [lexicon] * N if all(isinstance(c, str) for c in lexicon) else list(lexicon)
@@ -660,17 +678,27 @@ class _System(nn.Module):
         return labels, scores.gather(1, best[:, None])[:, 0]
 
     def beam_search(self, images: Union[Tensor, List[Any]], beam_width: int = 5, max_length: Optional[int] = None, *,
-                    rotation: int = 0, allowlist: Allowlist = None):
+                    rotation: int = 0, allowlist: Allowlist = None, lexicon: Union[Candidates, Lexicon, None] = None):
         """The `beam_width` most likely readings of each image by beam search on the device, as (labels, scores):
         labels[b] lists image b's hypotheses best first (fewer than beam_width when fewer exist), scores is fp32
         [N, beam_width], -inf padded, with each hypothesis's AR log-likelihood (what `score` returns for that label).
         PARSeq runs its AR decoder without refinement, whatever decode_ar / refine_iters say; ViTSTR searches over its
         per-position logits.  With beam_width = 1 the label is the greedy AR reading.  `images` as forward takes them;
-        `allowlist` as in forward.  The scores are on the images' device (CPU for CPU crops)."""
+        `allowlist` as in forward.  The scores are on the images' device (CPU for CPU crops).
+        `lexicon` (a word list for every image, one list per image, or a compiled Lexicon) restricts every hypothesis to
+        a word of the image's list that ends with EOS within max_length characters; the log-sum-exp of each step stays
+        over all allowed classes, so a score is still `score`'s for that word."""
         check_beam_width(beam_width)
         N = len(images) if isinstance(images, (list, tuple)) else images.shape[0]
         mask = self.allowlist_mask(allowlist, N)
-        ids, lengths, scores = self.model.beam_search(images, beam_width, max_length, rotation=rotation, class_mask=mask)
+        roots = None
+        if lexicon is not None:
+            if not isinstance(lexicon, Lexicon):
+                lexicon_rows(lexicon, N)                   # the image count of per-image lists, before the trie build
+                lexicon = self.compile_lexicon(lexicon)
+            roots = lexicon.roots_for(N)
+        ids, lengths, scores = self.model.beam_search(images, beam_width, max_length, rotation=rotation, class_mask=mask,
+                                                      lexicon=lexicon, roots=roots)
         ids_h, len_h = ids.cpu().tolist(), lengths.cpu().tolist()
         labels = [[self.tokenizer._ids2tok(ids_h[b][k][:n], True) for k, n in enumerate(len_h[b]) if n >= 0]
                   for b in range(N)]

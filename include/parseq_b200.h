@@ -92,6 +92,19 @@ typedef struct parseq_forward_args {
    * launch.  Same memory as the entry point's images: DEVICE for parseq_forward / _u8 / _crops, HOST for
    * the *_host* variants (uploaded with each super-chunk).  PARSeq and ViTSTR; not with forced_ids / forced_refine. */
   const uint32_t* class_mask;
+  /* Optional output: fp32 [batch][num_steps][T] cross-attention maps, T = (img_h / patch_h) * (img_w / patch_w) image
+   * tokens in the patch-embed flatten order (row-major over the patch grid).  maps[b][i][t] is ca_weights of the query
+   * stream of the last decoder layer (strhub/models/parseq/modules.py:74, nn.MultiheadAttention's head average) in the
+   * pass that produced logits[b][i]: the last cloze refinement pass (refine_iters >= 1), the NAR pass (decode_ar = 0), or
+   * AR step i's query (decode_ar = 1, no refinement; computed by one teacher-forced pass over the AR loop's own ids [BOS,
+   * ids[:, :num_steps-1]] under the causal masks, so it is the same whichever AR loop ran).  Rows follow the allowlist's
+   * ids; rows past the early-exit length S are computed and may be dropped with the logits.  The logits, ids and steps
+   * are bit-identical to the call without maps.  Same memory as the entry point's logits: DEVICE for parseq_forward /
+   * _u8 / _crops, HOST for the *_host* variants.  NULL = no maps, no extra launch or allocation; the first call with maps
+   * allocates a static [max_batch][max_label_length + 1][T] buffer (the first AR-only one also the causal masks of its
+   * map pass, uploaded synchronously, so make it outside a stream capture).  PARSeq only (ViTSTR: PARSEQ_ERR_UNSUPPORTED); not
+   * with forced_ids / forced_refine (PARSEQ_ERR_INVALID_ARG). */
+  float* attn_maps;
 } parseq_forward_args;
 
 /* Replaces system.PARSeq.forward -> model.PARSeq.forward (system.py:87-88, model.py:105-169).
@@ -307,7 +320,8 @@ int parseq_set_option(parseq_engine* e, const char* name, int64_t value);
  * category 0 encoder GEMM, 1 encoder attention, 2 LayerNorm, 3 decoder GEMM, 4 decoder attention, 5 other,
  * 6 encoder residual GEMM fused with LayerNorm, 7 persistent AR-loop kernel, 8 scoring tail (head GEMM with the log-sum-exp
  * epilogue and the per-candidate reduce of parseq_score), 9 beam selection (the selection kernel and, at dec_depth >= 2,
- * the K/V cache gather of parseq_beam_search). */
+ * the K/V cache gather of parseq_beam_search), 10 cross-attention maps (the maps kernel of parseq_forward_args.attn_maps;
+ * the AR-only map pass's other kernels count in their own categories). */
 int parseq_get_timing(parseq_engine* e, int category, double* ms, double* flops, int64_t* count);
 /* Debug: after a forward with option "ar_prof"=1, copies the [32 steps][16 slots] globaltimer (ns) stamps that block 0 of
  * the persistent AR kernel recorded at its phase boundaries.  Row 26 holds extra stamps of step 1 of the cluster kernel;

@@ -684,6 +684,7 @@ struct parseq_engine {
   cudaEvent_t ev_in = nullptr, ev_out = nullptr;
   // static I/O buffers the CUDA graphs are captured on
   float* in_images = nullptr; float* out_logits = nullptr; int* out_ids = nullptr; int* out_steps = nullptr;
+  float* out_maps = nullptr;        // [max_batch, L, T] cross-attention maps, allocated by the first call that asks for them
   uint8_t* in_images_u8 = nullptr;  // static input of the uint8 HWC entry points
   uint32_t* in_mask = nullptr;      // [max_batch, mask_ld] class allowlist rows of the super-chunk (graphs, host entry points)
   int mask_ld = 0;                  // words per allowlist row: ceil(C / 32)
@@ -820,6 +821,7 @@ void free_workspace(parseq_engine* e) {
     if (p) cudaFree(p);
   e->sc_meta = nullptr; e->sc_meta_ints = 0; e->sc_causal = nullptr; e->sc_vt_part = nullptr;
   e->beam_bytes = 0;
+  if (e->out_maps) { cudaFree(e->out_maps); e->out_maps = nullptr; }
   if (e->lex_roots) { cudaFree(e->lex_roots); e->lex_roots = nullptr; }
   e->lex_roots_cap = 0;
   if (e->ev_enc) { cudaEventDestroy(e->ev_enc); e->ev_enc = nullptr; }
@@ -850,9 +852,10 @@ void free_workspace(parseq_engine* e) {
 
 // categories: 0 encoder GEMM, 1 encoder attention, 2 LayerNorm, 3 decoder GEMM, 4 decoder attention, 5 other,
 // 6 encoder residual GEMM + LayerNorm, 7 AR-loop kernel, 8 scoring tail (head GEMM with the LSE epilogue + reduce),
-// 9 beam selection (beam_select_kernel and the K/V gather of parseq_beam_search)
+// 9 beam selection (beam_select_kernel and the K/V gather of parseq_beam_search), 10 cross-attention maps
+// (dec_cross_attn_maps_kernel)
 enum { CAT_ENC_GEMM = 0, CAT_ENC_ATTN = 1, CAT_LN = 2, CAT_DEC_GEMM = 3, CAT_DEC_ATTN = 4, CAT_MISC = 5, CAT_ENC_GEMM_LN = 6, CAT_DEC_AR = 7,
-       CAT_SCORE = 8, CAT_BEAM = 9, CAT_COUNT = 10 };
+       CAT_SCORE = 8, CAT_BEAM = 9, CAT_MAPS = 10, CAT_COUNT = 11 };
 
 cudaEvent_t pool_event(parseq_engine* e) {
   if (!e->event_pool.empty()) { cudaEvent_t ev = e->event_pool.back(); e->event_pool.pop_back(); return ev; }
@@ -1050,6 +1053,11 @@ struct DecodeExtras {
   unsigned long long* beam_keys = nullptr;
   int beam_k = 0;
   const uint32_t* beam_mask = nullptr;
+  // cross-attention maps (parseq_forward_args.attn_maps): the query stream of the last layer writes the head-averaged
+  // weights of row (b, qi) to maps + (b * nq + qi) * T; maps_only: the pass ends there (no cross-attention output, MLP
+  // or head)
+  float* maps = nullptr;
+  bool maps_only = false;
 };
 
 const __nv_bfloat16* ckv_of(const parseq_engine* e, int layer) { return layer == 0 ? e->ckv : e->ckv_deep[layer - 1]; }
@@ -1072,7 +1080,7 @@ int self_attn_rows(parseq_engine* e, const float* q, const __nv_bfloat16* kv, bo
 // place): x += out_proj(sa); x += cross_attn(norm1(x)); x += MLP(norm2(x)).  add != null: x holds no residual yet,
 // the base is the broadcast table / caller rows `add` (row r adds add[r % add_mod]).
 int dec_layer_rest(parseq_engine* e, parseq_engine::Stage& sg, int l, int b_first, int B, int nq, float* x, const float* add,
-                   int add_mod, cudaStream_t st) {
+                   int add_mod, cudaStream_t st, float* maps = nullptr, bool maps_only = false) {
   const int D = e->D, M = B * nq;
   const std::string Ly = "decoder.layers." + std::to_string(l) + ".";
   const float qscale = 1.0f / std::sqrt(static_cast<float>(e->dh_dec));
@@ -1089,6 +1097,19 @@ int dec_layer_rest(parseq_engine* e, parseq_engine::Stage& sg, int l, int b_firs
   }
   PQ_TRY(gemm(e, sg.yn, D, e->wb(Ly + "cross_attn.in_proj_weight"), D, e->wf(Ly + "cross_attn.in_proj_bias"), M, D, D,
               pq::EPI_F32, qscale, nullptr, 0, 0, sg.qc, D, st));
+  if (maps != nullptr) {
+    // the head-averaged weights of these query rows, from the q just projected and the layer's K (reads only)
+    TimedScope ts(e, st, CAT_MAPS, 2.0 * M * e->T * D);
+    const dim3 grid(static_cast<unsigned>(B), static_cast<unsigned>((nq + pq::AMAP_ROWS - 1) / pq::AMAP_ROWS));
+    const long long kv_rows = 1ll * e->max_batch * e->T;
+    if (e->T <= 128)
+      PQ_TRY(launch_k(e->lo, pq::dec_cross_attn_maps_kernel<4>, grid, dim3(pq::AMAP_THREADS), 0, st, static_cast<const float*>(sg.qc),
+                      ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, maps));
+    else
+      PQ_TRY(launch_k(e->lo, pq::dec_cross_attn_maps_kernel<8>, grid, dim3(pq::AMAP_THREADS), 0, st, static_cast<const float*>(sg.qc),
+                      ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, maps));
+    if (maps_only) return PARSEQ_OK;
+  }
   {
     TimedScope ts(e, st, CAT_DEC_ATTN, 4.0 * M * e->T * D);
     const long long kv_rows = 1ll * e->max_batch * e->T;
@@ -1209,7 +1230,11 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
   }
   const bool own_q = ex != nullptr && ex->query != nullptr;
   const float* resid = own_q ? ex->query : e->wf("pos_queries") + static_cast<long long>(q0) * D;
-  PQ_TRY(dec_layer_rest(e, sg, 0, b_first, B / rpi, nq * rpi, sg.y, resid, own_q ? M : nq, st));
+  const int last = e->cfg.dec_depth - 1;
+  float* maps = ex != nullptr ? ex->maps : nullptr;
+  const bool maps_only = maps != nullptr && ex->maps_only;
+  PQ_TRY(dec_layer_rest(e, sg, 0, b_first, B / rpi, nq * rpi, sg.y, resid, own_q ? M : nq, st, last == 0 ? maps : nullptr,
+                        maps_only));
   // query stream of layers >= 1 (modules.py:91-93): its residual base is the previous layer's output, its keys the
   // layer's content K/V cache
   for (int l = 1; l < e->cfg.dec_depth; ++l) {
@@ -1218,9 +1243,11 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
     PQ_TRY(gemm(e, sg.yn, D, e->w(Ll + "self_attn.in_proj_weight"), D, e->wf(Ll + "self_attn.in_proj_bias"), M, D, D,
                 pq::EPI_F32, qscale, nullptr, 0, 0, sg.qc, D, st));
     PQ_TRY(self_attn_rows(e, sg.qc, sg.kvc[l - 1], true, kv_pitch, ids, B, nq, q0, nkeys, mode, qmask, pmask, sg.sa, st));
-    PQ_TRY(dec_layer_rest(e, sg, l, b_first, B / rpi, nq * rpi, sg.y, nullptr, 0, st));
+    PQ_TRY(dec_layer_rest(e, sg, l, b_first, B / rpi, nq * rpi, sg.y, nullptr, 0, st, l == last ? maps : nullptr, maps_only));
   }
-  if (ex != nullptr && ex->out_norm != nullptr) {
+  if (maps_only) {
+    // the map pass of an AR-only schedule stops after the last layer's maps
+  } else if (ex != nullptr && ex->out_norm != nullptr) {
     // PARSeq.decode returns the decoder output: final LayerNorm only (modules.py:123-125)
     PQ_TRY(layernorm(e, sg.y, "decoder.norm", 1e-5f, M, sg.yn, ex->out_norm, st));
   } else if (ex != nullptr && ex->lse_tgt != nullptr) {
@@ -1270,12 +1297,33 @@ int argmax_rows(parseq_engine* e, float* logits, int L, int B, int nrows, int sr
                   dst0, forced, forced_ld, mask);
 }
 
+// The cross-attention maps of an AR-only schedule (no refinement): row i is AR step i's query.  Under teacher forcing
+// step i is a fixed function of the memory and the context 0..i, so one pass over the AR loop's own ids
+// [BOS, ids[:, :L-1]] (`ids`: its [B, ids_ld] id rows) under the causal query mask, and at depth >= 2 the causal content
+// mask, computes every step's query at once (the argument parseq_score rests on).  It stops after the last layer's maps
+// and writes nothing else the caller sees; whichever AR loop ran, the maps depend only on the ids.
+int ar_maps_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, int L, const int* ids, float* maps,
+                 cudaStream_t st) {
+  const unsigned char* causal = e->sc_causal + 1ll * (L - 1) * e->L * e->L;
+  DecodeExtras ex;
+  ex.qmask = causal;
+  ex.cmask = e->cfg.dec_depth > 1 ? causal : nullptr;
+  ex.maps = maps;
+  ex.maps_only = true;
+  return decode_pass(e, sg, b_first, B, L, 0, L, 0, ids, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, st, &ex);
+}
+
 // Decoder chain of one group of B <= dec_chunk images (their cross K/V is at `ckv`): AR loop / NAR pass, cloze
 // refinement, final argmax.  model.py:113-169.  `mask`: the group's class allowlist rows, or null.  Every head output
 // that the multi-query passes (and the chain's large-head AR steps) leave unmasked is masked by the argmax that reads it,
 // and the final argmax runs with a mask even when the caller wants no ids, so no unmasked logit is returned.
+// `maps` (the group's [B, L, T] cross-attention maps, or null): written by the pass that produced the returned logits.
 int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const parseq_forward_args* a, int b0,
-                 int B, int L, float* logits, int* ids_out, int* steps, const uint32_t* mask, cudaStream_t st, bool ar_done) {
+                 int B, int L, float* logits, int* ids_out, int* steps, const uint32_t* mask, cudaStream_t st, bool ar_done,
+                 float* maps) {
+  DecodeExtras mx;                  // the final pass's extras: its maps
+  mx.maps = maps;
+  const DecodeExtras* last_ex = maps != nullptr ? &mx : nullptr;
   // b_first: index of the group's first image inside the super-chunk (row of the K/V cache); b0: inside the caller's batch
   const int C = e->C;
   const int bos = e->V - 2, pad = e->V - 1;
@@ -1302,7 +1350,8 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
     PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * e->ids_ld + 255) / 256), dim3(256), 0, st, sg.ids_ctx, B, e->ids_ld,
                     bos, pad));
     e->launches++;
-    PQ_TRY(decode_pass(e, sg, b_first, B, L, 0, 1, 0, sg.ids_ctx, logits, C, nullptr, 0, nullptr, 0, mask, st));
+    PQ_TRY(decode_pass(e, sg, b_first, B, L, 0, 1, 0, sg.ids_ctx, logits, C, nullptr, 0, nullptr, 0, mask, st,
+                       a->refine_iters == 0 ? last_ex : nullptr));
   }
   for (int it = 0; it < a->refine_iters; ++it) {
     PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * e->ids_ld + 255) / 256), dim3(256), 0, st, sg.ids_ctx, B, e->ids_ld,
@@ -1313,9 +1362,11 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
                             : nullptr;
     // ctx = [BOS, argmax(logits[:, :L-1])]  (model.py:161)
     PQ_TRY(argmax_rows(e, logits, L, B, L - 1, 0, sg.ids_ctx, e->ids_ld, 1, forced, L, mask, st));
-    PQ_TRY(decode_pass(e, sg, b_first, B, L, 0, L, 1, sg.ids_ctx, logits, C, nullptr, 0, nullptr, 0, mask, st));
+    PQ_TRY(decode_pass(e, sg, b_first, B, L, 0, L, 1, sg.ids_ctx, logits, C, nullptr, 0, nullptr, 0, mask, st,
+                       it + 1 == a->refine_iters ? last_ex : nullptr));
   }
   if (ids_out != nullptr || mask != nullptr) PQ_TRY(argmax_rows(e, logits, L, B, L, 0, ids_out, L, 0, nullptr, 0, mask, st));
+  if (maps != nullptr && a->decode_ar && a->refine_iters == 0) PQ_TRY(ar_maps_pass(e, sg, b_first, B, L, sg.ids_ar, maps, st));
   return PARSEQ_OK;
 }
 
@@ -1543,7 +1594,7 @@ int cross_kv(parseq_engine* e, int B) {
 }
 
 int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B, int L, const void* images, bool u8,
-                  float* logits, int* ids_out, int* steps, const uint32_t* mask, int part = 0, int split = 0) {
+                  float* logits, int* ids_out, int* steps, const uint32_t* mask, float* maps, int part = 0, int split = 0) {
   const long long img_sz = 3ll * e->cfg.img_h * e->cfg.img_w * (u8 ? 1 : 4);   // bytes per image
   const int D = e->D, T = e->T;
   if (part == 1)
@@ -1576,6 +1627,9 @@ int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B,
     PQ_TRY(ar_decode(e, path, a, b0, B, L, logits, steps, mask, e->main));
     if (a->refine_iters == 0) {      // nothing left for the chains but the final argmax (the AR kernels masked the logits)
       if (ids_out != nullptr) PQ_TRY(argmax_rows(e, logits, L, B, L, 0, ids_out, L, 0, nullptr, 0, nullptr, e->main));
+      for (int o = 0; maps != nullptr && o < B; o += e->dec_chunk)
+        PQ_TRY(ar_maps_pass(e, e->stages[static_cast<size_t>(o / e->dec_chunk)], o, std::min(B - o, e->dec_chunk), L,
+                            e->ar_ids + 1ll * o * e->ids_ld, maps + 1ll * o * L * T, e->main));
       return PARSEQ_OK;
     }
   }
@@ -1590,7 +1644,7 @@ int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B,
     if (fork) PQ_CUDA(cudaStreamWaitEvent(ds, e->ev_enc, 0));
     PQ_TRY(decode_stage(e, sg, o, a, b0 + o, Bs, L, logits + 1ll * o * L * e->C,
                         ids_out ? ids_out + 1ll * o * L : nullptr, steps, mask ? mask + 1ll * o * e->mask_ld : nullptr, ds,
-                        ar_done));
+                        ar_done, maps ? maps + 1ll * o * L * T : nullptr));
     if (fork) PQ_CUDA(cudaEventRecord(sg.ev_done, ds));
   }
   if (fork)
@@ -1610,6 +1664,8 @@ int run_graph(parseq_engine* e, const parseq_forward_args* a, int Bc, int L, boo
   const bool masked = a->class_mask != nullptr;
   std::vector<int> key = {Bc, L, a->max_length < 0 ? 1 : 0, a->decode_ar ? 1 : 0, a->refine_iters, u8 ? 1 : 0, part, split,
                           masked ? 1 : 0};
+  // the graphs of calls without maps keep their keys; part 1 (the first half's encoder) never touches the maps
+  if (a->attn_maps != nullptr && part != 1) key.push_back(1);
   auto it = e->graphs.find(key);
   if (it == e->graphs.end()) {
     parseq_forward_args aa = *a;
@@ -1619,7 +1675,8 @@ int run_graph(parseq_engine* e, const parseq_forward_args* a, int Bc, int L, boo
     const long long before = e->launches;
     PQ_CUDA(cudaStreamBeginCapture(e->main, cudaStreamCaptureModeThreadLocal));
     int r = forward_super(e, &aa, 0, Bc, L, u8 ? static_cast<const void*>(e->in_images_u8) : static_cast<const void*>(e->in_images),
-                          u8, e->out_logits, e->out_ids, e->out_steps, masked ? e->in_mask : nullptr, part, split);
+                          u8, e->out_logits, e->out_ids, e->out_steps, masked ? e->in_mask : nullptr,
+                          a->attn_maps != nullptr ? e->out_maps : nullptr, part, split);
     cudaGraph_t g = nullptr;
     cudaError_t ce = cudaStreamEndCapture(e->main, &g);
     if (r != PARSEQ_OK) { if (g) cudaGraphDestroy(g); return r; }
@@ -1773,12 +1830,40 @@ int check_crops_call(parseq_engine* e, const parseq_forward_args* a, const parse
   return check_crop_smem(e, a->batch, crops);
 }
 
+// The causal masks of every row count P (scoring, and the map pass of AR-only schedules), on first use.
+int causal_reserve(parseq_engine* e) {
+  if (e->sc_causal != nullptr) return PARSEQ_OK;
+  const int L = e->L;
+  // the canonical left-to-right permutation (system.py:153-167): query i and content row i see keys 0..i
+  std::vector<unsigned char> h(static_cast<size_t>(L) * L * L, 0);
+  for (int P = 1; P <= L; ++P)
+    for (int q = 0; q < P; ++q)
+      for (int k = 0; k < P; ++k) h[static_cast<size_t>(P - 1) * L * L + static_cast<size_t>(q) * P + k] = k > q ? 1 : 0;
+  PQ_TRY(dev_alloc(&e->sc_causal, static_cast<long long>(h.size())));
+  PQ_CUDA(cudaMemcpy(e->sc_causal, h.data(), h.size(), cudaMemcpyHostToDevice));
+  return PARSEQ_OK;
+}
+
+// Cross-attention map buffers, on the first call that asks for maps: the static maps the graphs write, and the causal
+// masks only for an AR-only schedule (the one whose map pass reads them).
+int maps_reserve(parseq_engine* e, const parseq_forward_args* a) {
+  if (e->out_maps == nullptr) PQ_TRY(dev_alloc(&e->out_maps, 1ll * e->max_batch * e->L * e->T));
+  return a->decode_ar && a->refine_iters == 0 ? causal_reserve(e) : PARSEQ_OK;
+}
+
 // Common driver of parseq_forward / parseq_forward_host. `host` selects H2D/D2H vs D2D staging copies.
 // `crops` (raw crops of any size, u8): each super-chunk is resized into the static uint8 input in place of the copy.
 int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* images_any, float* logits, int32_t* ids,
                  int32_t* steps, cudaStream_t user, bool host, bool u8 = false, const CropBatch* crops = nullptr) {
   if (a->class_mask != nullptr && (a->forced_ids != nullptr || a->forced_refine != nullptr))
     return fail(PARSEQ_ERR_INVALID_ARG, "class_mask cannot be combined with teacher forcing");
+  float* const maps = a->attn_maps;
+  if (maps != nullptr) {
+    if (e->arch != 0) return fail(PARSEQ_ERR_UNSUPPORTED, "attn_maps: ViTSTR has no decoder cross-attention");
+    if (a->forced_ids != nullptr || a->forced_refine != nullptr)
+      return fail(PARSEQ_ERR_INVALID_ARG, "attn_maps cannot be combined with teacher forcing");
+    PQ_TRY(maps_reserve(e, a));
+  }
   const int L = num_steps_of(e, a->max_length);
   const bool testing = a->max_length < 0;
   const long long img_sz = 3ll * e->cfg.img_h * e->cfg.img_w * (u8 ? 1 : 4);   // bytes per image
@@ -1794,6 +1879,12 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
     if (a->class_mask == nullptr) return PARSEQ_OK;
     PQ_CUDA(cudaMemcpyAsync(e->in_mask, a->class_mask + 1ll * b0 * e->mask_ld, static_cast<size_t>(Bc * mask_row_bytes), kin,
                             e->main));
+    return PARSEQ_OK;
+  };
+  // the static maps of super-chunk [b0, b0 + Bc) -> the caller's, as the logits
+  auto copy_maps = [&](int b0, int Bc) -> int {
+    if (maps == nullptr) return PARSEQ_OK;
+    PQ_CUDA(cudaMemcpyAsync(maps + 1ll * b0 * L * e->T, e->out_maps, static_cast<size_t>(1ll * Bc * L * e->T) * 4, kout, e->main));
     return PARSEQ_OK;
   };
   // user stream -> main
@@ -1813,7 +1904,8 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
         in = images + b0 * img_sz;
       }
       PQ_TRY(forward_super(e, a, b0, Bc, L, in, u8, logits + 1ll * b0 * L * e->C, ids ? ids + 1ll * b0 * L : nullptr,
-                           e->out_steps, a->class_mask ? a->class_mask + 1ll * b0 * e->mask_ld : nullptr));
+                           e->out_steps, a->class_mask ? a->class_mask + 1ll * b0 * e->mask_ld : nullptr,
+                           maps ? maps + 1ll * b0 * L * e->T : nullptr));
       continue;
     }
     if (host && !eager && e->arch == 0 && Bc >= 256 && e->chunk >= Bc) {
@@ -1843,6 +1935,7 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
       PQ_CUDA(cudaMemcpyAsync(logits + 1ll * b0 * L * e->C, e->out_logits, static_cast<size_t>(1ll * Bc * L * e->C) * 4, kout,
                               e->main));
       if (ids) PQ_CUDA(cudaMemcpyAsync(ids + 1ll * b0 * L, e->out_ids, static_cast<size_t>(1ll * Bc * L) * 4, kout, e->main));
+      PQ_TRY(copy_maps(b0, Bc));
       continue;
     }
     if (crops) {
@@ -1854,13 +1947,14 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
     PQ_TRY(stage_mask(b0, Bc));
     if (eager) {
       PQ_TRY(forward_super(e, a, b0, Bc, L, in_static, u8, e->out_logits, e->out_ids, e->out_steps,
-                           a->class_mask ? e->in_mask : nullptr));
+                           a->class_mask ? e->in_mask : nullptr, maps ? e->out_maps : nullptr));
     } else {
       PQ_TRY(run_graph(e, a, Bc, L, u8));
     }
     PQ_CUDA(cudaMemcpyAsync(logits + 1ll * b0 * L * e->C, e->out_logits, static_cast<size_t>(1ll * Bc * L * e->C) * 4, kout,
                             e->main));
     if (ids) PQ_CUDA(cudaMemcpyAsync(ids + 1ll * b0 * L, e->out_ids, static_cast<size_t>(1ll * Bc * L) * 4, kout, e->main));
+    PQ_TRY(copy_maps(b0, Bc));
   }
   if (steps) PQ_CUDA(cudaMemcpyAsync(steps, e->out_steps, 4, kout, e->main));
   // main -> user stream
@@ -1919,15 +2013,7 @@ int score_reserve(parseq_engine* e) {
       PQ_TRY(dev_alloc(&sg.lse_part, Rd * ntiles));
       PQ_TRY(dev_alloc(&sg.lse_tlogit, Rd));
     }
-    if (e->sc_causal == nullptr) {
-      // the canonical left-to-right permutation (system.py:153-167): query i and content row i see keys 0..i
-      std::vector<unsigned char> h(static_cast<size_t>(L) * L * L, 0);
-      for (int P = 1; P <= L; ++P)
-        for (int q = 0; q < P; ++q)
-          for (int k = 0; k < P; ++k) h[static_cast<size_t>(P - 1) * L * L + static_cast<size_t>(q) * P + k] = k > q ? 1 : 0;
-      PQ_TRY(dev_alloc(&e->sc_causal, static_cast<long long>(h.size())));
-      PQ_CUDA(cudaMemcpy(e->sc_causal, h.data(), h.size(), cudaMemcpyHostToDevice));
-    }
+    PQ_TRY(causal_reserve(e));
   } else if (e->sc_vt_part == nullptr) {
     PQ_TRY(dev_alloc(&e->sc_vt_part, 1ll * e->chunk * L * ntiles));
   }
@@ -2410,7 +2496,7 @@ int beam_lexicon_call(parseq_engine* e, const parseq_beam_args* a, const parseq_
 extern "C" {
 
 const char* parseq_last_error(void) { return g_last_error.c_str(); }
-const char* parseq_version(void) { return "parseq_b200 0.1 (sm_90a, wgmma/TMA)"; }
+const char* parseq_version(void) { return "parseq_b200 0.2 (sm_90a, wgmma/TMA)"; }
 
 int parseq_create(const parseq_config* cfg, parseq_engine** out) {
   if (cfg == nullptr || out == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");

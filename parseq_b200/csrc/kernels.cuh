@@ -902,6 +902,102 @@ __global__ void __launch_bounds__(128) dec_cross_attn3_grouped_kernel(const floa
 }
 
 // ---------------------------------------------------------------------------------------------
+// Cross-attention maps (parseq_forward_args.attn_maps): maps[row, t] = (1 / heads) * sum_h softmax_t(q_h . k_h,t) of
+// the query rows of one decoder pass, the head-averaged weights nn.MultiheadAttention returns.  One CTA of 8 warps per
+// (image, block of AMAP_ROWS query rows); the heads are visited in order, each head's K staged as dec_cross_attn3_kernel
+// stages it, and the probabilities are computed with that kernel's arithmetic (the fmaf order over the 16 bf16x2 words,
+// expf(s - max), the xor-shuffle sum): the exponentials and their sum are bitwise those of its P.V, which scales
+// sum(e * v) by 1 / sum where this kernel stores p = e * (1 / sum) per key.
+// Each warp keeps its AMAP_ROWS / 8 rows' running sums in registers; the heads are summed in fixed order, so the maps
+// are bitwise reproducible and independent of the batch.  q fp32 [B*nq, D] pre-scaled; maps fp32 [B*nq, T].
+constexpr int AMAP_ROWS = 32;
+constexpr int AMAP_THREADS = 256;
+template <int NR>   // keys per lane: T <= 32 * NR
+__global__ void __launch_bounds__(AMAP_THREADS, 1) dec_cross_attn_maps_kernel(const float* __restrict__ q,
+                                                                         const __nv_bfloat16* __restrict__ kv,
+                                                                         long long kv_rows, int b_first, int T, int D,
+                                                                         int heads, int nq, float* __restrict__ maps) {
+  constexpr int TK = 32 * NR, WARPS = AMAP_THREADS / 32, RPW = AMAP_ROWS / WARPS;
+  __shared__ uint32_t sK[TK * 17];                        // bf16x2 words, pitch 17 (odd)
+  grid_dep_launch();
+  grid_dep_wait();
+  const int b = blockIdx.x, q_begin = static_cast<int>(blockIdx.y) * AMAP_ROWS;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const long long row_b = static_cast<long long>(b_first + b) * T;
+  float acc[RPW][NR];
+#pragma unroll
+  for (int j = 0; j < RPW; ++j)
+#pragma unroll
+    for (int r = 0; r < NR; ++r) acc[j][r] = 0.f;
+  for (int h = 0; h < heads; ++h) {
+    if (h > 0) __syncthreads();                          // every warp is done with the previous head's K
+    for (int t = tid; t < TK; t += AMAP_THREADS) {
+      if (t < T) {
+        const uint4* kr = reinterpret_cast<const uint4*>(kv + blocked_off(kv_rows, row_b + t, h * 32));
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const uint4 u = __ldg(kr + j);
+          sK[t * 17 + j * 4 + 0] = u.x; sK[t * 17 + j * 4 + 1] = u.y;
+          sK[t * 17 + j * 4 + 2] = u.z; sK[t * 17 + j * 4 + 3] = u.w;
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < 16; ++j) sK[t * 17 + j] = 0u;
+      }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int j = 0; j < RPW; ++j) {
+      const int qi = q_begin + warp + j * WARPS;
+      if (qi >= nq) continue;                            // warp-uniform
+      const long long row = static_cast<long long>(b) * nq + qi;
+      const float qv = q[row * D + h * 32 + lane];        // lane j holds q_j
+      float sc[NR];
+#pragma unroll
+      for (int r = 0; r < NR; ++r) sc[r] = 0.f;
+#pragma unroll
+      for (int w = 0; w < 16; ++w) {
+        const float qa = __shfl_sync(0xffffffffu, qv, 2 * w), qb = __shfl_sync(0xffffffffu, qv, 2 * w + 1);
+#pragma unroll
+        for (int r = 0; r < NR; ++r) {
+          const uint32_t kw = sK[(r * 32 + lane) * 17 + w];
+          sc[r] = fmaf(qb, __uint_as_float(kw & 0xffff0000u), fmaf(qa, __uint_as_float(kw << 16), sc[r]));
+        }
+      }
+      float mx = -INFINITY;
+#pragma unroll
+      for (int r = 0; r < NR; ++r) {
+        if (r * 32 + lane >= T) sc[r] = -INFINITY;
+        mx = fmaxf(mx, sc[r]);
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+      float sum = 0.f;
+#pragma unroll
+      for (int r = 0; r < NR; ++r) {
+        sc[r] = expf(sc[r] - mx);
+        sum += sc[r];
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+      const float inv = 1.0f / sum;
+#pragma unroll
+      for (int r = 0; r < NR; ++r) acc[j][r] += sc[r] * inv;
+    }
+  }
+  const float rh = static_cast<float>(heads);
+#pragma unroll
+  for (int j = 0; j < RPW; ++j) {
+    const int qi = q_begin + warp + j * WARPS;
+    if (qi >= nq) continue;
+    float* out = maps + (static_cast<long long>(b) * nq + qi) * T;
+#pragma unroll
+    for (int r = 0; r < NR; ++r)
+      if (r * 32 + lane < T) out[r * 32 + lane] = acc[j][r] / rh;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // Candidate scoring, last step: one CTA per candidate m, thread i = position i <= n_m (n_m = lengths[m]).  The term of
 // position i is log_softmax(logits row)[t_i] = (t - M) - log(S), with M, S the merge of the row's per-tile partials
 // (gemm_lse_epilogue) in column order: M = max of the tile maxima, S = sum of s_j exp(m_j - M).  The candidate's score is

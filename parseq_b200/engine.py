@@ -21,7 +21,7 @@ class ParseqConfigC(C.Structure):
 class ForwardArgsC(C.Structure):
     _fields_ = [("batch", C.c_int32), ("max_length", C.c_int32), ("decode_ar", C.c_int32),
                 ("refine_iters", C.c_int32), ("forced_ids", C.c_void_p), ("forced_refine", C.c_void_p),
-                ("class_mask", C.c_void_p)]
+                ("class_mask", C.c_void_p), ("attn_maps", C.c_void_p)]
 
 
 class CropsC(C.Structure):
@@ -218,7 +218,7 @@ class Engine:
         check(self.lib, self.lib.parseq_set_option(self.handle, name.encode(), int(value)))
 
     TIMING_CATEGORIES = ("enc_gemm", "enc_attn", "layernorm", "dec_gemm", "dec_attn", "other", "enc_gemm_ln", "dec_ar",
-                         "score_tail", "beam_select")
+                         "score_tail", "beam_select", "attn_maps")
 
     def get_timing(self):
         out = {}
@@ -245,26 +245,30 @@ class Engine:
         ml = self.cfg.max_label_length if max_length is None else min(int(max_length), self.cfg.max_label_length)
         return ml + 1
 
-    def _args(self, batch, max_length, decode_ar, refine_iters, forced_ids=None, forced_refine=None, class_mask=None):
+    def _args(self, batch, max_length, decode_ar, refine_iters, forced_ids=None, forced_refine=None, class_mask=None,
+              attn_maps=None):
         return ForwardArgsC(batch, -1 if max_length is None else int(max_length), int(bool(decode_ar)),
-                            int(refine_iters), forced_ids, forced_refine, class_mask)
+                            int(refine_iters), forced_ids, forced_refine, class_mask, attn_maps)
 
-    # class_mask_ptr: the per-image allowlist words (parseq_forward_args.class_mask), in the memory of the images
+    # class_mask_ptr: the per-image allowlist words (parseq_forward_args.class_mask), in the memory of the images;
+    # attn_maps_ptr: fp32 [batch, num_steps, T] cross-attention maps (parseq_forward_args.attn_maps), in the memory of the
+    # logits
     def forward(self, images_ptr, batch, logits_ptr, ids_ptr, steps_ptr, stream, max_length=None, decode_ar=True,
-                refine_iters=1, forced_ids_ptr=None, forced_refine_ptr=None, class_mask_ptr=None):
-        a = self._args(batch, max_length, decode_ar, refine_iters, forced_ids_ptr, forced_refine_ptr, class_mask_ptr)
+                refine_iters=1, forced_ids_ptr=None, forced_refine_ptr=None, class_mask_ptr=None, attn_maps_ptr=None):
+        a = self._args(batch, max_length, decode_ar, refine_iters, forced_ids_ptr, forced_refine_ptr, class_mask_ptr,
+                       attn_maps_ptr)
         check(self.lib, self.lib.parseq_forward(self.handle, C.byref(a), images_ptr, logits_ptr, ids_ptr, steps_ptr,
                                                 stream))
 
     def forward_host(self, images_ptr, batch, logits_ptr, ids_ptr, steps_ptr, stream, max_length=None,
-                     decode_ar=True, refine_iters=1, class_mask_ptr=None):
-        a = self._args(batch, max_length, decode_ar, refine_iters, class_mask=class_mask_ptr)
+                     decode_ar=True, refine_iters=1, class_mask_ptr=None, attn_maps_ptr=None):
+        a = self._args(batch, max_length, decode_ar, refine_iters, class_mask=class_mask_ptr, attn_maps=attn_maps_ptr)
         check(self.lib, self.lib.parseq_forward_host(self.handle, C.byref(a), images_ptr, logits_ptr, ids_ptr,
                                                      steps_ptr, stream))
 
     def forward_u8(self, images_ptr, batch, logits_ptr, ids_ptr, steps_ptr, stream, max_length=None, decode_ar=True,
-                   refine_iters=1, host=False, class_mask_ptr=None):
-        a = self._args(batch, max_length, decode_ar, refine_iters, class_mask=class_mask_ptr)
+                   refine_iters=1, host=False, class_mask_ptr=None, attn_maps_ptr=None):
+        a = self._args(batch, max_length, decode_ar, refine_iters, class_mask=class_mask_ptr, attn_maps=attn_maps_ptr)
         fn = self.lib.parseq_forward_host_u8 if host else self.lib.parseq_forward_u8
         check(self.lib, fn(self.handle, C.byref(a), images_ptr, logits_ptr, ids_ptr, steps_ptr, stream))
 
@@ -272,8 +276,8 @@ class Engine:
         check(self.lib, self.lib.parseq_resize_crops(self.handle, batch, C.byref(crops), out_ptr, stream))
 
     def forward_crops(self, crops: CropsC, batch, logits_ptr, ids_ptr, steps_ptr, stream, max_length=None, decode_ar=True,
-                      refine_iters=1, host=False, class_mask_ptr=None):
-        a = self._args(batch, max_length, decode_ar, refine_iters, class_mask=class_mask_ptr)
+                      refine_iters=1, host=False, class_mask_ptr=None, attn_maps_ptr=None):
+        a = self._args(batch, max_length, decode_ar, refine_iters, class_mask=class_mask_ptr, attn_maps=attn_maps_ptr)
         fn = self.lib.parseq_forward_host_crops if host else self.lib.parseq_forward_crops
         check(self.lib, fn(self.handle, C.byref(a), C.byref(crops), logits_ptr, ids_ptr, steps_ptr, stream))
 

@@ -186,8 +186,76 @@ def _mask_ptr(mask: Optional[Tensor]):
     return mask.data_ptr() if mask is not None else None
 
 
+def _ptr(t: Optional[Tensor]):
+    return t.data_ptr() if t is not None else None
+
+
 def _crops_c(data: Tensor, offsets: Tensor, sizes: Tensor, rotation: int) -> CropsC:
     return CropsC(data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), int(rotation))
+
+
+def _crop_hw(c) -> Tuple[int, int]:
+    """(h, w) of a raw crop as pack_crops takes it."""
+    if isinstance(c, Tensor):
+        return int(c.shape[0]), int(c.shape[1])
+    if hasattr(c, "size") and not callable(c.size):        # PIL: size = (w, h)
+        return int(c.size[1]), int(c.size[0])
+    t = _crop_tensor(c)
+    return int(t.shape[0]), int(t.shape[1])
+
+
+def attention_centers_boxes(maps: Tensor, patch_size: Sequence[int], threshold: float = 0.5) -> Tuple[Tensor, Tensor]:
+    """Where each map row points, in the pixels of the img_size image: maps fp32 [n, gh, gw] (one row per character)
+    -> centers [n, 2] = (x, y), the map-weighted centroid of the patch-cell centres, and boxes [n, 4] = (x0, y0, x1, y1),
+    the extent of the cells whose weight is >= threshold * the row's maximum.  Cell (r, c) covers x in [c pw, (c+1) pw),
+    y in [r ph, (r+1) ph)."""
+    ph, pw = int(patch_size[0]), int(patch_size[1])
+    n, gh, gw = maps.shape
+    m = maps.to(torch.float32)
+    ys = (torch.arange(gh, dtype=torch.float32, device=m.device) + 0.5) * ph
+    xs = (torch.arange(gw, dtype=torch.float32, device=m.device) + 0.5) * pw
+    tot = m.sum(dim=(1, 2)).clamp_min(torch.finfo(torch.float32).tiny)
+    cx = (m.sum(dim=1) * xs).sum(-1) / tot
+    cy = (m.sum(dim=2) * ys).sum(-1) / tot
+    keep = m >= threshold * m.amax(dim=(1, 2), keepdim=True)
+    rows, cols = keep.any(dim=2), keep.any(dim=1)                  # [n, gh], [n, gw]
+    r_idx = torch.arange(gh, device=m.device).expand(n, gh)
+    c_idx = torch.arange(gw, device=m.device).expand(n, gw)
+    r0 = torch.where(rows, r_idx, gh).amin(-1)
+    r1 = torch.where(rows, r_idx, -1).amax(-1) + 1
+    c0 = torch.where(cols, c_idx, gw).amin(-1)
+    c1 = torch.where(cols, c_idx, -1).amax(-1) + 1
+    boxes = torch.stack([c0 * pw, r0 * ph, c1 * pw, r1 * ph], dim=-1).to(torch.float32)
+    return torch.stack([cx, cy], dim=-1), boxes
+
+
+def unrotate_points(xy: Tensor, crop_hw: Sequence[int], img_size: Sequence[int], rotation: int) -> Tensor:
+    """Points (x, y) [..., 2] in the pixels of the img_size image that get_transform made of a crop of size crop_hw
+    (strhub/data/module.py:69-82: Image.rotate(rotation, expand=True), counter-clockwise, then T.Resize(img_size))
+    -> the same points in the crop's own pixels: the resize scale is undone per axis, then the rotation."""
+    h, w = int(crop_hw[0]), int(crop_hw[1])
+    H, W = int(img_size[0]), int(img_size[1])
+    rh, rw = (w, h) if rotation in (90, 270) else (h, w)          # the rotated crop's size
+    xr = xy[..., 0] * (rw / W)
+    yr = xy[..., 1] * (rh / H)
+    if rotation == 0:
+        x, y = xr, yr
+    elif rotation == 90:
+        x, y = w - yr, xr
+    elif rotation == 180:
+        x, y = w - xr, h - yr
+    elif rotation == 270:
+        x, y = yr, h - xr
+    else:
+        raise ValueError(f"rotation must be 0, 90, 180 or 270, got {rotation}")
+    return torch.stack([x, y], dim=-1)
+
+
+def unrotate_boxes(boxes: Tensor, crop_hw: Sequence[int], img_size: Sequence[int], rotation: int) -> Tensor:
+    """Boxes (x0, y0, x1, y1) [n, 4] of the img_size image -> the crop's pixels (unrotate_points of two corners)."""
+    a = unrotate_points(boxes[:, :2], crop_hw, img_size, rotation)
+    b = unrotate_points(boxes[:, 2:], crop_hw, img_size, rotation)
+    return torch.cat([torch.minimum(a, b), torch.maximum(a, b)], dim=-1)
 
 
 class _Holder(nn.Module):
@@ -414,10 +482,11 @@ class _EngineModule(nn.Module):
                         u8=images.dtype == torch.uint8, lexicon=lex, roots=roots)
         return ids, lengths, scores
 
-    def _run_crops(self, crops, max_length, decode_ar, refine_iters, rotation, class_mask=None):
+    def _run_crops(self, crops, max_length, decode_ar, refine_iters, rotation, class_mask=None, attn_maps=False):
         """Raw crops of any size: CUDA crops run parseq_forward_crops and return CUDA tensors; CPU crops and PIL images
         run parseq_forward_host_crops (pinned upload, host outputs) and return CPU tensors.  `class_mask`: the CPU
-        allowlist words of allowlist_mask, or None."""
+        allowlist words of allowlist_mask, or None.  attn_maps: also return the fp32 [N, num_steps, T] cross-attention
+        maps (else None)."""
         eng = self.engine()
         dev = self._device
         data, offsets, sizes = pack_crops(crops, pin_memory=True)
@@ -430,21 +499,26 @@ class _EngineModule(nn.Module):
         logits = torch.empty((N, L, self.cfg.num_classes), dtype=torch.float32, device=out_dev, pin_memory=host)
         ids = torch.empty((N, L), dtype=torch.int32, device=out_dev, pin_memory=host)
         steps = torch.empty((1,), dtype=torch.int32, device=out_dev, pin_memory=host)
+        maps = (torch.empty((N, L, self.cfg.enc_tokens), dtype=torch.float32, device=out_dev, pin_memory=host)
+                if attn_maps else None)
         if class_mask is not None:
             class_mask = class_mask.pin_memory() if host else class_mask.to(dev, non_blocking=True)
         eng.forward_crops(_crops_c(data, offsets, sizes, rotation), N, logits.data_ptr(), ids.data_ptr(), steps.data_ptr(),
                           torch.cuda.current_stream(dev).cuda_stream, max_length, decode_ar, refine_iters, host=host,
-                          class_mask_ptr=_mask_ptr(class_mask))
-        return logits, ids, steps
+                          class_mask_ptr=_mask_ptr(class_mask), attn_maps_ptr=_ptr(maps))
+        return logits, ids, steps, maps
 
     def _run(self, images: Union[Tensor, List[Any]], max_length, decode_ar, refine_iters, forced_ids=None,
-             forced_refine=None, rotation: int = 0, class_mask: Optional[Tensor] = None):
+             forced_refine=None, rotation: int = 0, class_mask: Optional[Tensor] = None, attn_maps: bool = False):
+        """(logits, ids, steps, maps) of one engine forward; maps is None unless attn_maps."""
         if class_mask is not None and (forced_ids is not None or forced_refine is not None):
             raise ValueError("an allowlist cannot be combined with teacher forcing")
+        if attn_maps and (forced_ids is not None or forced_refine is not None):
+            raise ValueError("attention maps cannot be combined with teacher forcing")
         if isinstance(images, (list, tuple)):
             if forced_ids is not None or forced_refine is not None:
                 raise ValueError("teacher forcing takes normalised float images")
-            return self._run_crops(images, max_length, decode_ar, refine_iters, rotation, class_mask)
+            return self._run_crops(images, max_length, decode_ar, refine_iters, rotation, class_mask, attn_maps)
         if rotation:
             raise ValueError("rotation applies to lists of raw crops; a tensor input is already at img_size")
         eng = self.engine()
@@ -455,6 +529,7 @@ class _EngineModule(nn.Module):
         logits = torch.empty((N, L, self.cfg.num_classes), dtype=torch.float32, device=dev)
         ids = torch.empty((N, L), dtype=torch.int32, device=dev)
         steps = torch.empty((1,), dtype=torch.int32, device=dev)
+        maps = torch.empty((N, L, self.cfg.enc_tokens), dtype=torch.float32, device=dev) if attn_maps else None
         fi = forced_ids.to(device=dev, dtype=torch.int32).contiguous() if forced_ids is not None else None
         fr = forced_refine.to(device=dev, dtype=torch.int32).contiguous() if forced_refine is not None else None
         st = torch.cuda.current_stream(dev).cuda_stream
@@ -464,12 +539,12 @@ class _EngineModule(nn.Module):
             class_mask = class_mask.to(dev, non_blocking=True).contiguous()
         if images.dtype == torch.uint8:
             eng.forward_u8(images.data_ptr(), N, logits.data_ptr(), ids.data_ptr(), steps.data_ptr(), st, max_length,
-                           decode_ar, refine_iters, class_mask_ptr=_mask_ptr(class_mask))
+                           decode_ar, refine_iters, class_mask_ptr=_mask_ptr(class_mask), attn_maps_ptr=_ptr(maps))
         else:
             eng.forward(images.data_ptr(), N, logits.data_ptr(), ids.data_ptr(), steps.data_ptr(), st, max_length,
                         decode_ar, refine_iters, fi.data_ptr() if fi is not None else None,
-                        fr.data_ptr() if fr is not None else None, _mask_ptr(class_mask))
-        return logits, ids, steps
+                        fr.data_ptr() if fr is not None else None, _mask_ptr(class_mask), _ptr(maps))
+        return logits, ids, steps, maps
 
 
 class ParseqModel(_EngineModule):
@@ -535,8 +610,8 @@ class ParseqModel(_EngineModule):
         """`images`: normalised float [N, 3, H, W], uint8 [N, H, W, 3] at img_size, or a list of raw crops of any size
         (uint8 [h, w, 3] tensors, all CUDA or all CPU, or PIL images in mode RGB) that the engine rotates by `rotation`
         and resizes as the reference's test transform does.  `class_mask`: per-image allowlist words (allowlist_mask)."""
-        logits, ids, steps = self._run(images, max_length, self.decode_ar, self.refine_iters, forced_ids, forced_refine,
-                                       rotation, class_mask)
+        logits, ids, steps, _ = self._run(images, max_length, self.decode_ar, self.refine_iters, forced_ids, forced_refine,
+                                          rotation, class_mask)
         if max_length is None and self.decode_ar and not self.refine_iters:
             # model.py:144-147: with no refinement the reference returns only the S steps it ran
             S = int(steps.item())
@@ -544,6 +619,19 @@ class ParseqModel(_EngineModule):
         if return_ids:
             return logits, ids
         return logits
+
+    def forward_with_attention(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *,
+                               rotation: int = 0, class_mask: Optional[Tensor] = None):
+        """forward(tokenizer, images, max_length, return_ids=True) plus the cross-attention maps of the decoder's last
+        layer (parseq_forward_args.attn_maps): (logits [N, S, C], ids [N, S], maps fp32 [N, S, T]), maps[b, i] the
+        head-averaged weights over the T image tokens of the query that produced logits[b, i].  The logits and ids are
+        bit-identical to forward's."""
+        logits, ids, steps, maps = self._run(images, max_length, self.decode_ar, self.refine_iters, rotation=rotation,
+                                             class_mask=class_mask, attn_maps=True)
+        if max_length is None and self.decode_ar and not self.refine_iters:
+            S = int(steps.item())
+            logits, ids, maps = logits[:, :S], ids[:, :S], maps[:, :S]
+        return logits, ids, maps
 
 
 class VitstrModel(_EngineModule):
@@ -557,7 +645,7 @@ class VitstrModel(_EngineModule):
                        *, rotation: int = 0, class_mask: Optional[Tensor] = None):
         """`self.forward(images, max_length + 2)[:, 1:]` (vitstr/system.py:65-71) in one engine call; `images` and
         `class_mask` as in ParseqModel.forward."""
-        logits, ids, _ = self._run(images, max_length, False, 0, rotation=rotation, class_mask=class_mask)
+        logits, ids, _, _ = self._run(images, max_length, False, 0, rotation=rotation, class_mask=class_mask)
         return (logits, ids) if return_ids else logits
 
     def forward(self, x: Tensor, seqlen: int = 25) -> Tensor:
@@ -776,6 +864,42 @@ class PARSeq(_System):
         mask = self.allowlist_mask(allowlist, len(images) if isinstance(images, (list, tuple)) else images.shape[0])
         return self.model.forward(self.tokenizer, images, max_length, rotation=rotation, class_mask=mask)
 
+    def read_with_attention(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *,
+                            rotation: int = 0, allowlist: Allowlist = None) -> Tuple[Tensor, Tensor]:
+        """`forward` plus where the decoder looked: (logits, maps) with logits exactly forward's and maps fp32
+        [N, S, gh, gw] (S = logits.shape[1], (gh, gw) the patch grid): maps[b, i] is the cross-attention of the decoder's
+        last layer for the query that produced logits[b, i], averaged over the heads as nn.MultiheadAttention averages
+        them, from the last refinement pass, the NAR pass, or AR step i when there is no refinement.  Each map sums to
+        1 over the grid.  Inputs and result devices as in forward."""
+        mask = self.allowlist_mask(allowlist, len(images) if isinstance(images, (list, tuple)) else images.shape[0])
+        logits, _, maps = self.model.forward_with_attention(images, max_length, rotation=rotation, class_mask=mask)
+        gh, gw = self.model.cfg.grid
+        return logits, maps.view(maps.shape[0], maps.shape[1], gh, gw)
+
+    def locate(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *, rotation: int = 0,
+               allowlist: Allowlist = None, threshold: float = 0.5):
+        """Where each character was read: (labels, confidences, centers, boxes).  labels / confidences are postprocess's
+        of the forward logits; centers[b] fp32 [n_b, 2] = (x, y) and boxes[b] fp32 [n_b, 4] = (x0, y0, x1, y1), one row
+        per character of labels[b], from its map of read_with_attention: the map-weighted centroid of the patch-cell
+        centres, and the extent of the cells whose weight is >= threshold * the map's maximum.  Coordinates are pixels of
+        the input: of the img_size image for tensors, of each original crop for raw crops (the resize scale and the
+        rotation undone).  Results on the device of the outputs, as forward returns them."""
+        logits, maps = self.read_with_attention(images, max_length, rotation=rotation, allowlist=allowlist)
+        labels, confs = self.postprocess(logits.to(self.device))
+        cfg = self.model.cfg
+        crops = isinstance(images, (list, tuple))
+        centers: List[Tensor] = []
+        boxes: List[Tensor] = []
+        for b, label in enumerate(labels):
+            c, bx = attention_centers_boxes(maps[b, :len(label)], cfg.patch_size, threshold)
+            if crops:
+                hw = _crop_hw(images[b])
+                c = unrotate_points(c, hw, cfg.img_size, rotation)
+                bx = unrotate_boxes(bx, hw, cfg.img_size, rotation)
+            centers.append(c)
+            boxes.append(bx)
+        return labels, confs, centers, boxes
+
 
 class ViTSTR(_System):
     """Mirror of `strhub.models.vitstr.system.ViTSTR` (vitstr/system.py:29-71), inference side."""
@@ -807,6 +931,13 @@ class ViTSTR(_System):
         """`allowlist` as in PARSeq.forward: it constrains the argmax of every token position."""
         mask = self.allowlist_mask(allowlist, len(images) if isinstance(images, (list, tuple)) else images.shape[0])
         return self.model.forward_tokens(images, max_length, rotation=rotation, class_mask=mask)
+
+    def read_with_attention(self, *args, **kwargs):
+        raise NotImplementedError("ViTSTR has no decoder cross-attention: its characters are read from the encoder's "
+                                  "own tokens, so there are no per-character maps to return")
+
+    def locate(self, *args, **kwargs):
+        raise NotImplementedError("ViTSTR has no decoder cross-attention, so characters cannot be located from it")
 
     @classmethod
     def load_from_checkpoint(cls, checkpoint_path: str, map_location="cpu", **kwargs):

@@ -637,7 +637,7 @@ struct parseq_engine {
   unsigned int* ar_bar = nullptr;
   unsigned long long* ar_prof = nullptr;   // [32][16] phase time stamps of the AR kernel (debug option "ar_prof"; DESIGN.md 4)
   bool ar_prof_on = false;
-  cudaEvent_t ev_enc = nullptr;
+  cudaEvent_t ev_enc = nullptr;     // `main`'s work so far, which the stage streams wait for (fan_out)
   struct Stage {
     __nv_bfloat16 *sa = nullptr, *yn = nullptr, *ca = nullptr, *hd = nullptr;
     float *y = nullptr, *qc = nullptr;
@@ -647,12 +647,9 @@ struct parseq_engine {
     float* cx = nullptr;
     std::vector<__nv_bfloat16*> kvc;
     // candidate scoring (parseq_score), allocated by the first score call: per-tile log-sum-exp partials
-    // [dec_chunk * L][ceil(C / 128)] and target logits of the chain's rows; while a group is decoded, cand_off (device,
-    // candidates of each of its images) routes the cross-attention rows to their image (dec_layer_rest)
+    // [dec_chunk * L][ceil(C / 128)] and target logits of the chain's rows
     float2* lse_part = nullptr;
     float* lse_tlogit = nullptr;
-    const int* cand_off = nullptr;
-    int cand_imgs = 0, cand_max_rows = 0;
     // beam search (parseq_beam_search), allocated by the first beam call: double-buffered state of `rows` beam rows
     // (ids [rows][ids_ld], score, len, st; kernels.cuh beam_select_kernel), the parent row of each new beam, what the
     // head leaves of one step's rows (ViTSTR: of `rows / BEAM_MAX` images' positions) - the logits at <= 128 classes, the
@@ -674,7 +671,7 @@ struct parseq_engine {
       int* node[2] = {nullptr, nullptr};
     } bm;
     cudaStream_t stream = nullptr;
-    cudaEvent_t ev_enc = nullptr, ev_done = nullptr;
+    cudaEvent_t ev_done = nullptr;
   };
   std::vector<Stage> stages;
   int max_batch = 512;              // images per graph / super-chunk = stages.size() * chunk
@@ -703,7 +700,7 @@ struct parseq_engine {
   float2* sc_vt_part = nullptr;
   long long beam_bytes = 0;         // device bytes of the beam-search buffers (0 until the first beam call)
   int* lex_roots = nullptr;         // the lexicon call's roots [lex_roots_cap] (grown on demand)
-  int lex_roots_cap = 0;
+  long long lex_roots_cap = 0;
   bool use_graph = true;
   struct GraphEntry { cudaGraphExec_t exec; long long kernels; };
   std::map<std::vector<int>, GraphEntry> graphs;
@@ -737,6 +734,48 @@ int dev_alloc(Tp** p, long long n) {
   PQ_CUDA(cudaMalloc(reinterpret_cast<void**>(p), static_cast<size_t>(n) * sizeof(Tp)));
   return PARSEQ_OK;
 }
+
+// A buffer of a call's inputs that grows on demand to n elements (*cap: its size).  The kernels of the previous call,
+// on `main` or `copy`, may still read the old one: both streams are drained before it is freed.
+template <typename Tp>
+int grow(parseq_engine* e, Tp** p, long long* cap, long long n) {
+  if (n <= *cap) return PARSEQ_OK;
+  if (*p != nullptr) {
+    PQ_CUDA(cudaStreamSynchronize(e->main));
+    PQ_CUDA(cudaStreamSynchronize(e->copy));
+    cudaFree(*p);
+    *p = nullptr;
+    *cap = 0;
+  }
+  PQ_TRY(dev_alloc(p, n));
+  *cap = n;
+  return PARSEQ_OK;
+}
+
+// The handle can run a call: not null, its workspace allocated, and (`weights`) its weights finalized.
+int check_ready(const parseq_engine* e, bool weights = true) {
+  if (e == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
+  if (weights && !e->finalized)
+    return fail(PARSEQ_ERR_STATE, "parseq_finalize has not been called after the last weight update");
+  return PARSEQ_OK;
+}
+
+// The stream bracket of an entry point: the engine's work runs on `main` after what the caller enqueued on `user`
+// before the call (enter_main), and the caller's later work runs after it (leave_main; not reached on an error).
+int enter_main(parseq_engine* e, cudaStream_t user) {
+  PQ_CUDA(cudaEventRecord(e->ev_in, user));
+  PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_in, 0));
+  return PARSEQ_OK;
+}
+int leave_main(parseq_engine* e, cudaStream_t user) {
+  PQ_CUDA(cudaEventRecord(e->ev_out, e->main));
+  PQ_CUDA(cudaStreamWaitEvent(user, e->ev_out, 0));
+  return PARSEQ_OK;
+}
+
+// Bytes per input image: fp32 NCHW or uint8 HWC
+long long image_bytes(const parseq_engine* e, bool u8) { return 3ll * e->cfg.img_h * e->cfg.img_w * (u8 ? 1 : 4); }
 
 int alloc_workspace(parseq_engine* e) {
   const long long R = static_cast<long long>(e->chunk) * e->T;          // encoder rows per chunk
@@ -783,7 +822,6 @@ int alloc_workspace(parseq_engine* e) {
       for (auto& c : sg.kvc) PQ_TRY(dev_alloc(&c, Rd * 2 * D));
     }
     PQ_CUDA(cudaStreamCreateWithFlags(&sg.stream, cudaStreamNonBlocking));
-    PQ_CUDA(cudaEventCreateWithFlags(&sg.ev_enc, cudaEventDisableTiming));
     PQ_CUDA(cudaEventCreateWithFlags(&sg.ev_done, cudaEventDisableTiming));
   }
   const long long NB = e->max_batch;
@@ -844,7 +882,6 @@ void free_workspace(parseq_engine* e) {
     for (auto p : sg.kvc)
       if (p) cudaFree(p);
     if (sg.stream) cudaStreamDestroy(sg.stream);
-    if (sg.ev_enc) cudaEventDestroy(sg.ev_enc);
     if (sg.ev_done) cudaEventDestroy(sg.ev_done);
   }
   e->stages.clear();
@@ -1045,7 +1082,12 @@ struct DecodeExtras {
   float* out_norm = nullptr;             // [B*nq, D] fp32: decoder.norm(y) is the result (no head)
   const int* lse_tgt = nullptr;          // [B*nq] target class per row: the head runs with the LSE epilogue into the
                                          // stage's lse_part / lse_tlogit (candidate scoring), no logits are stored
-  int beam = 1;                          // beam search: B counts beam rows, `beam` consecutive rows per image; the rows'
+  // candidate scoring: the B rows are candidates of cand_imgs images, image j's candidates [cand_off[j], cand_off[j + 1])
+  // (device), at most cand_max_rows query rows per image; every cross-attention of the pass serves a candidate's rows
+  // from its image (dec_cross_attn3_grouped_kernel)
+  const int* cand_off = nullptr;
+  int cand_imgs = 0, cand_max_rows = 0;
+  int beam = 1;                         // beam search: B counts beam rows, `beam` consecutive rows per image; the rows'
                                          // self-attention reads their own ids, their cross-attention their image
   // beam search above 128 classes: the head GEMM runs the top-K epilogue (beam_k keys per row and tile, the images'
   // allowlist rows beam_mask) into these, and no logits are stored
@@ -1078,10 +1120,13 @@ int self_attn_rows(parseq_engine* e, const float* q, const __nv_bfloat16* kv, bo
 
 // The rest of decoder layer `l` after its self-attention (modules.py:72-78) on a residual stream x [B*nq, D] (fp32, in
 // place): x += out_proj(sa); x += cross_attn(norm1(x)); x += MLP(norm2(x)).  add != null: x holds no residual yet,
-// the base is the broadcast table / caller rows `add` (row r adds add[r % add_mod]).
+// the base is the broadcast table / caller rows `add` (row r adds add[r % add_mod]).  `ex` (may be null): the
+// candidates' row map, and with `maps_layer` the maps of this layer's query rows.
 int dec_layer_rest(parseq_engine* e, parseq_engine::Stage& sg, int l, int b_first, int B, int nq, float* x, const float* add,
-                   int add_mod, cudaStream_t st, float* maps = nullptr, bool maps_only = false) {
+                   int add_mod, cudaStream_t st, const DecodeExtras* ex, bool maps_layer) {
   const int D = e->D, M = B * nq;
+  float* const maps = ex != nullptr && maps_layer ? ex->maps : nullptr;
+  const int* const cand_off = ex != nullptr ? ex->cand_off : nullptr;
   const std::string Ly = "decoder.layers." + std::to_string(l) + ".";
   const float qscale = 1.0f / std::sqrt(static_cast<float>(e->dh_dec));
   if (add != nullptr) {
@@ -1108,21 +1153,21 @@ int dec_layer_rest(parseq_engine* e, parseq_engine::Stage& sg, int l, int b_firs
     else
       PQ_TRY(launch_k(e->lo, pq::dec_cross_attn_maps_kernel<8>, grid, dim3(pq::AMAP_THREADS), 0, st, static_cast<const float*>(sg.qc),
                       ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, maps));
-    if (maps_only) return PARSEQ_OK;
+    if (ex->maps_only) return PARSEQ_OK;
   }
   {
     TimedScope ts(e, st, CAT_DEC_ATTN, 4.0 * M * e->T * D);
     const long long kv_rows = 1ll * e->max_batch * e->T;
-    if (sg.cand_off != nullptr) {
+    if (cand_off != nullptr) {
       // candidate scoring: the rows of each image's candidates attend to that image (64 rows per CTA)
       constexpr int kRows = 64;
-      const dim3 grid(static_cast<unsigned>(sg.cand_imgs * e->cfg.dec_num_heads), static_cast<unsigned>((sg.cand_max_rows + kRows - 1) / kRows));
+      const dim3 grid(static_cast<unsigned>(ex->cand_imgs * e->cfg.dec_num_heads), static_cast<unsigned>((ex->cand_max_rows + kRows - 1) / kRows));
       if (e->T <= 128)
         PQ_TRY(launch_k(e->lo, pq::dec_cross_attn3_grouped_kernel<4>, grid, dim3(128), 0, st, static_cast<const float*>(sg.qc),
-                        ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, sg.cand_off, kRows, sg.ca));
+                        ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, cand_off, kRows, sg.ca));
       else
         PQ_TRY(launch_k(e->lo, pq::dec_cross_attn3_grouped_kernel<8>, grid, dim3(128), 0, st, static_cast<const float*>(sg.qc),
-                        ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, sg.cand_off, kRows, sg.ca));
+                        ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, cand_off, kRows, sg.ca));
     } else if (e->T <= 128)
       PQ_TRY(launch_k(e->lo, pq::dec_cross_attn3_kernel<4>, dim3(B * e->cfg.dec_num_heads), dim3(128), 0, st,
                       static_cast<const float*>(sg.qc), ckv_of(e, l), kv_rows, b_first, e->T, D,
@@ -1146,12 +1191,13 @@ int dec_layer_rest(parseq_engine* e, parseq_engine::Stage& sg, int l, int b_firs
 // layers 0..depth-2, each appending its K/V rows of the next layer to that layer's cache (row b * pitch + k).  nc is 1
 // (an AR step, pitch L: the causal content rows of earlier positions do not change as the context grows) or nkeys = pitch
 // (a whole pass).  The content rows attend to keys 0..nkeys-1 under `mode` (0: all, 1: cloze + first EOS), or under the
-// caller's content / padding masks (decode API).
+// caller's content / padding masks (decode API, `ex`), whose candidates' row map (scoring) routes the cross-attention.
 // rpi > 1 (beam search, nc = 1): the B rows are rpi consecutive beams of each of B / rpi images.
 int content_stream(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, int k0, int nc, int nkeys, int pitch,
-                   int mode, const int* ids, const unsigned char* cmask, const unsigned char* pmask, cudaStream_t st,
-                   int rpi = 1) {
+                   int mode, const int* ids, const DecodeExtras* ex, cudaStream_t st, int rpi) {
   const int D = e->D, M = B * nc;
+  const unsigned char* cmask = ex != nullptr ? ex->cmask : nullptr;
+  const unsigned char* pmask = ex != nullptr ? ex->pmask : nullptr;
   const float qscale = 1.0f / std::sqrt(static_cast<float>(e->dh_dec));
   {
     TimedScope ts(e, st, CAT_MISC, 0.0);
@@ -1170,7 +1216,7 @@ int content_stream(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int 
                 pq::EPI_F32, qscale, nullptr, 0, 0, sg.qc, D, st));
     PQ_TRY(self_attn_rows(e, sg.qc, l == 0 ? e->kvtab : sg.kvc[l - 1], l > 0, pitch, ids, B, nc, k0, nkeys, mode, cmask, pmask,
                           sg.sa, st));
-    PQ_TRY(dec_layer_rest(e, sg, l, b_first, B / rpi, nc * rpi, sg.cx, nullptr, 0, st));
+    PQ_TRY(dec_layer_rest(e, sg, l, b_first, B / rpi, nc * rpi, sg.cx, nullptr, 0, st, ex, false));
     // K/V of layer l + 1 = W_kv norm_c_{l+1}(content_{l+1}) + b_kv, into rows k0.. of its cache
     const std::string Ln = "decoder.layers." + std::to_string(l + 1) + ".";
     PQ_TRY(layernorm(e, sg.cx, Ln + "norm_c", 1e-5f, M, sg.yn, nullptr, st));
@@ -1193,8 +1239,7 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
   const int kv_pitch = ar_step ? e->L : nkeys;
   const int rpi = ex != nullptr ? ex->beam : 1;   // rows per image of the cross-attention (beam search)
   if (e->cfg.dec_depth > 1)
-    PQ_TRY(content_stream(e, sg, b_first, B, ar_step ? q0 : 0, ar_step ? 1 : nkeys, nkeys, kv_pitch, mode, ids,
-                          ex != nullptr ? ex->cmask : nullptr, ex != nullptr ? ex->pmask : nullptr, st, rpi));
+    PQ_TRY(content_stream(e, sg, b_first, B, ar_step ? q0 : 0, ar_step ? 1 : nkeys, nkeys, kv_pitch, mode, ids, ex, st, rpi));
   const float* qself = e->qs;            // [L, D] table of W_q LN_q(pos_queries), pre-scaled
   const unsigned char *qmask = nullptr, *pmask = nullptr;
   if (ex != nullptr && ex->query != nullptr) {
@@ -1231,10 +1276,8 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
   const bool own_q = ex != nullptr && ex->query != nullptr;
   const float* resid = own_q ? ex->query : e->wf("pos_queries") + static_cast<long long>(q0) * D;
   const int last = e->cfg.dec_depth - 1;
-  float* maps = ex != nullptr ? ex->maps : nullptr;
-  const bool maps_only = maps != nullptr && ex->maps_only;
-  PQ_TRY(dec_layer_rest(e, sg, 0, b_first, B / rpi, nq * rpi, sg.y, resid, own_q ? M : nq, st, last == 0 ? maps : nullptr,
-                        maps_only));
+  const bool maps_only = ex != nullptr && ex->maps != nullptr && ex->maps_only;
+  PQ_TRY(dec_layer_rest(e, sg, 0, b_first, B / rpi, nq * rpi, sg.y, resid, own_q ? M : nq, st, ex, last == 0));
   // query stream of layers >= 1 (modules.py:91-93): its residual base is the previous layer's output, its keys the
   // layer's content K/V cache
   for (int l = 1; l < e->cfg.dec_depth; ++l) {
@@ -1243,7 +1286,7 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
     PQ_TRY(gemm(e, sg.yn, D, e->w(Ll + "self_attn.in_proj_weight"), D, e->wf(Ll + "self_attn.in_proj_bias"), M, D, D,
                 pq::EPI_F32, qscale, nullptr, 0, 0, sg.qc, D, st));
     PQ_TRY(self_attn_rows(e, sg.qc, sg.kvc[l - 1], true, kv_pitch, ids, B, nq, q0, nkeys, mode, qmask, pmask, sg.sa, st));
-    PQ_TRY(dec_layer_rest(e, sg, l, b_first, B / rpi, nq * rpi, sg.y, nullptr, 0, st, l == last ? maps : nullptr, maps_only));
+    PQ_TRY(dec_layer_rest(e, sg, l, b_first, B / rpi, nq * rpi, sg.y, nullptr, 0, st, ex, l == last));
   }
   if (maps_only) {
     // the map pass of an AR-only schedule stops after the last layer's maps
@@ -1313,6 +1356,14 @@ int ar_maps_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B,
   return decode_pass(e, sg, b_first, B, L, 0, L, 0, ids, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, st, &ex);
 }
 
+// id rows [B, ids_ld] = BOS, PAD, PAD, ...: the context of a first AR step or of a NAR / refinement pass
+int fill_ids(parseq_engine* e, int* ids, int B, cudaStream_t st) {
+  PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * e->ids_ld + 255) / 256), dim3(256), 0, st, ids, B, e->ids_ld, e->V - 2,
+                  e->V - 1));
+  e->launches++;
+  return PARSEQ_OK;
+}
+
 // Decoder chain of one group of B <= dec_chunk images (their cross K/V is at `ckv`): AR loop / NAR pass, cloze
 // refinement, final argmax.  model.py:113-169.  `mask`: the group's class allowlist rows, or null.  Every head output
 // that the multi-query passes (and the chain's large-head AR steps) leave unmasked is masked by the argmax that reads it,
@@ -1326,15 +1377,12 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
   const DecodeExtras* last_ex = maps != nullptr ? &mx : nullptr;
   // b_first: index of the group's first image inside the super-chunk (row of the K/V cache); b0: inside the caller's batch
   const int C = e->C;
-  const int bos = e->V - 2, pad = e->V - 1;
   const bool testing = a->max_length < 0;
   const long long LC = static_cast<long long>(L) * C;
   if (a->decode_ar && ar_done) {
     // the AR loop of the whole super-chunk already ran in the persistent kernel (ar_decode)
   } else if (a->decode_ar) {
-    PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * e->ids_ld + 255) / 256), dim3(256), 0, st, sg.ids_ar, B, e->ids_ld,
-                    bos, pad));
-    e->launches++;
+    PQ_TRY(fill_ids(e, sg.ids_ar, B, st));
     const int* forced = a->forced_ids ? a->forced_ids + static_cast<long long>(b0) * L : nullptr;
     for (int i = 0; i < L; ++i) {
       // step i: context ids[:, :i+1], query position i; the fused tail writes ids[:, i+1] = argmax (model.py:142)
@@ -1347,16 +1395,12 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
       e->launches++;
     }
   } else {
-    PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * e->ids_ld + 255) / 256), dim3(256), 0, st, sg.ids_ctx, B, e->ids_ld,
-                    bos, pad));
-    e->launches++;
+    PQ_TRY(fill_ids(e, sg.ids_ctx, B, st));
     PQ_TRY(decode_pass(e, sg, b_first, B, L, 0, 1, 0, sg.ids_ctx, logits, C, nullptr, 0, nullptr, 0, mask, st,
                        a->refine_iters == 0 ? last_ex : nullptr));
   }
   for (int it = 0; it < a->refine_iters; ++it) {
-    PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * e->ids_ld + 255) / 256), dim3(256), 0, st, sg.ids_ctx, B, e->ids_ld,
-                    bos, pad));
-    e->launches++;
+    PQ_TRY(fill_ids(e, sg.ids_ctx, B, st));
     const int* forced = a->forced_refine
                             ? a->forced_refine + (static_cast<long long>(it) * a->batch + b0) * L
                             : nullptr;
@@ -1505,9 +1549,7 @@ int ar_decode(parseq_engine* e, ArPath path, const parseq_forward_args* a, int b
               const uint32_t* mask, cudaStream_t st) {
   const int D = e->D;
   const std::string Ly = "decoder.layers.0.";
-  PQ_TRY(launch_k(e->lo, pq::fill_ids_kernel, dim3((B * e->ids_ld + 255) / 256), dim3(256), 0, st, e->ar_ids, B, e->ids_ld,
-                  e->V - 2, e->V - 1));
-  e->launches++;
+  PQ_TRY(fill_ids(e, e->ar_ids, B, st));
   // what both kernels read: the decoder's tables, bias and LayerNorm vectors, the id rows and the logits
   auto common = [&](auto& p) {
     p.B = B; p.L = L; p.V = e->V; p.C = e->C; p.T = e->T;
@@ -1569,13 +1611,6 @@ int ar_decode(parseq_engine* e, ArPath path, const parseq_forward_args* a, int b
   return PARSEQ_OK;
 }
 
-// One super-chunk (B <= max_batch images): `main` encodes everything (in `chunk`-image pieces) and projects the cross
-// K/V of the whole super-chunk; then the decoder - a latency-bound chain of small kernels - runs as ceil(B/dec_chunk)
-// independent chains on their own streams, concurrently (event fork/join, capturable into a CUDA graph).
-// part 0: the whole super-chunk.  part 1 / 2 (host entry points, PARSeq only): the encoder of images [0, split) alone /
-// the encoder of images [split, B) and everything after it - two graphs, so that the second half of the input is still
-// uploading while the first half is being encoded.
-// `mask`: the super-chunk's class allowlist rows (mask_ld words per image), or null.
 // Cross-attention K/V of every decoder layer from the memory of the super-chunk's B images, once per image (the
 // reference recomputes it in every decode call).
 int cross_kv(parseq_engine* e, int B) {
@@ -1593,33 +1628,80 @@ int cross_kv(parseq_engine* e, int B) {
   return PARSEQ_OK;
 }
 
+// PARSeq: images [0, B) of a super-chunk -> e->mem, encoded in `chunk`-image pieces, and their cross K/V.  The kernel
+// regime (fused GEMM + LayerNorm or not) follows the super-chunk, not `chunk`, so that the memory bits do not depend on
+// `chunk` and every entry point (forward, score, beam search) reads the same memory of an image.
+int encode_super(parseq_engine* e, const void* images, bool u8, int B) {
+  for (int o = 0; o < B; o += e->chunk)
+    PQ_TRY(encode_chunk(e, static_cast<const char*>(images) + o * image_bytes(e, u8), u8, std::min(B - o, e->chunk),
+                        e->mem + 1ll * o * e->T * e->D, nullptr, e->main, true, B));
+  return cross_kv(e, B);
+}
+
+// ViTSTR: the encoder blocks of images [0, B) in `chunk`-image pieces; after each piece, tail(o, Bs) runs on the final
+// tokens of its images [o, o + Bs) (in e->x) - the norm and head of the kept rows.
+template <typename Tail>
+int vitstr_chunks(parseq_engine* e, const void* images, bool u8, int B, Tail&& tail) {
+  for (int o = 0; o < B; o += e->chunk) {
+    const int Bs = std::min(B - o, e->chunk);
+    PQ_TRY(encode_chunk(e, static_cast<const char*>(images) + o * image_bytes(e, u8), u8, Bs, nullptr, nullptr, e->main, false));
+    PQ_TRY(tail(o, Bs));
+  }
+  return PARSEQ_OK;
+}
+
+// n decoder groups, group i on stage i % stages: group(i, stage, stream).  With more than one stage in use the stages'
+// streams run concurrently: each waits for `main`'s work so far, and `main` waits for all of them at the end (event
+// fork / join, capturable into a CUDA graph).  Otherwise, and in timing mode (isolated kernel times), every group runs
+// on `main`.
+template <typename Group>
+int fan_out(parseq_engine* e, int n, Group&& group) {
+  const int ns = static_cast<int>(e->stages.size());
+  const int used = std::min(n, ns);
+  const bool fork = used > 1 && !e->timing;
+  if (fork) {
+    PQ_CUDA(cudaEventRecord(e->ev_enc, e->main));
+    for (int s = 0; s < used; ++s) PQ_CUDA(cudaStreamWaitEvent(e->stages[static_cast<size_t>(s)].stream, e->ev_enc, 0));
+  }
+  for (int i = 0; i < n; ++i) {
+    parseq_engine::Stage& sg = e->stages[static_cast<size_t>(i % ns)];
+    PQ_TRY(group(i, sg, fork ? sg.stream : e->main));
+  }
+  if (fork) {
+    for (int s = 0; s < used; ++s) {
+      parseq_engine::Stage& sg = e->stages[static_cast<size_t>(s)];
+      PQ_CUDA(cudaEventRecord(sg.ev_done, sg.stream));
+      PQ_CUDA(cudaStreamWaitEvent(e->main, sg.ev_done, 0));
+    }
+  }
+  return PARSEQ_OK;
+}
+
+// One super-chunk (B <= max_batch images): `main` encodes everything (in `chunk`-image pieces) and projects the cross
+// K/V of the whole super-chunk; then the decoder - a latency-bound chain of small kernels - runs as ceil(B/dec_chunk)
+// independent chains on their own streams, concurrently (fan_out).
+// part 0: the whole super-chunk.  part 1 / 2 (host entry points, PARSeq only): the encoder of images [0, split) alone /
+// the encoder of images [split, B) and everything after it - two graphs, so that the second half of the input is still
+// uploading while the first half is being encoded.
+// `mask`: the super-chunk's class allowlist rows (mask_ld words per image), or null.
 int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B, int L, const void* images, bool u8,
                   float* logits, int* ids_out, int* steps, const uint32_t* mask, float* maps, int part = 0, int split = 0) {
-  const long long img_sz = 3ll * e->cfg.img_h * e->cfg.img_w * (u8 ? 1 : 4);   // bytes per image
   const int D = e->D, T = e->T;
   if (part == 1)
     return encode_chunk(e, images, u8, split, e->mem, nullptr, e->main, true, B);
   if (e->arch == 1) {               // ViTSTR: encoder blocks, then norm + head on the kept token rows of each chunk
-    for (int o = 0; o < B; o += e->chunk) {
-      const int Bs = (B - o < e->chunk) ? (B - o) : e->chunk;
-      PQ_TRY(encode_chunk(e, static_cast<const char*>(images) + o * img_sz, u8, Bs, nullptr, nullptr, e->main, false));
-      PQ_TRY(vitstr_tail(e, Bs, L, logits + 1ll * o * L * e->C, ids_out ? ids_out + 1ll * o * L : nullptr,
-                         mask ? mask + 1ll * o * e->mask_ld : nullptr, e->main));
-    }
-    return PARSEQ_OK;
+    return vitstr_chunks(e, images, u8, B, [&](int o, int Bs) -> int {
+      return vitstr_tail(e, Bs, L, logits + 1ll * o * L * e->C, ids_out ? ids_out + 1ll * o * L : nullptr,
+                         mask ? mask + 1ll * o * e->mask_ld : nullptr, e->main);
+    });
   }
   if (part == 2) {
-    PQ_TRY(encode_chunk(e, static_cast<const char*>(images) + split * img_sz, u8, B - split, e->mem + 1ll * split * T * D, nullptr,
-                        e->main, true, B));
+    PQ_TRY(encode_chunk(e, static_cast<const char*>(images) + split * image_bytes(e, u8), u8, B - split,
+                        e->mem + 1ll * split * T * D, nullptr, e->main, true, B));
+    PQ_TRY(cross_kv(e, B));
   } else {
-    for (int o = 0; o < B; o += e->chunk) {
-      const int Bs = (B - o < e->chunk) ? (B - o) : e->chunk;
-      // kernel regime (fused GEMM + LayerNorm or not) from the super-chunk, so that it does not depend on `chunk`
-      PQ_TRY(encode_chunk(e, static_cast<const char*>(images) + o * img_sz, u8, Bs, e->mem + 1ll * o * T * D, nullptr, e->main,
-                          true, B));
-    }
+    PQ_TRY(encode_super(e, images, u8, B));
   }
-  PQ_TRY(cross_kv(e, B));
   const ArPath path = ar_path(e);
   const bool ar_done = a->decode_ar && path != ArPath::Chain;
   e->ar_last_path = a->decode_ar ? static_cast<int>(path) : -1;
@@ -1633,23 +1715,13 @@ int forward_super(parseq_engine* e, const parseq_forward_args* a, int b0, int B,
       return PARSEQ_OK;
     }
   }
-  const int n = (B + e->dec_chunk - 1) / e->dec_chunk;
-  const bool fork = (n > 1) && !e->timing;      // timing mode: everything on `main` (isolated kernel times)
-  if (fork) PQ_CUDA(cudaEventRecord(e->ev_enc, e->main));
-  for (int s = 0; s < n; ++s) {
-    parseq_engine::Stage& sg = e->stages[static_cast<size_t>(s)];
+  // one decoder chain per dec_chunk images (B <= max_batch: one per stage at most)
+  return fan_out(e, (B + e->dec_chunk - 1) / e->dec_chunk, [&](int s, parseq_engine::Stage& sg, cudaStream_t ds) -> int {
     const int o = s * e->dec_chunk;
-    const int Bs = (B - o < e->dec_chunk) ? (B - o) : e->dec_chunk;
-    cudaStream_t ds = fork ? sg.stream : e->main;
-    if (fork) PQ_CUDA(cudaStreamWaitEvent(ds, e->ev_enc, 0));
-    PQ_TRY(decode_stage(e, sg, o, a, b0 + o, Bs, L, logits + 1ll * o * L * e->C,
+    return decode_stage(e, sg, o, a, b0 + o, std::min(B - o, e->dec_chunk), L, logits + 1ll * o * L * e->C,
                         ids_out ? ids_out + 1ll * o * L : nullptr, steps, mask ? mask + 1ll * o * e->mask_ld : nullptr, ds,
-                        ar_done, maps ? maps + 1ll * o * L * T : nullptr));
-    if (fork) PQ_CUDA(cudaEventRecord(sg.ev_done, ds));
-  }
-  if (fork)
-    for (int s = 0; s < n; ++s) PQ_CUDA(cudaStreamWaitEvent(e->main, e->stages[static_cast<size_t>(s)].ev_done, 0));
-  return PARSEQ_OK;
+                        ar_done, maps ? maps + 1ll * o * L * T : nullptr);
+  });
 }
 
 int num_steps_of(const parseq_engine* e, int max_length) {
@@ -1768,15 +1840,7 @@ int crops_reserve(parseq_engine* e, const CropBatch& cb, int batch) {
     crop_range(cb.c, b0, (batch - b0 < e->max_batch) ? batch : b0 + e->max_batch, &lo, &hi);
     need = hi - lo > need ? hi - lo : need;
   }
-  if (need <= e->crop_stage_bytes) return PARSEQ_OK;
-  PQ_CUDA(cudaStreamSynchronize(e->main));
-  PQ_CUDA(cudaStreamSynchronize(e->copy));
-  if (e->crop_stage) cudaFree(e->crop_stage);
-  e->crop_stage = nullptr;
-  e->crop_stage_bytes = 0;
-  PQ_TRY(dev_alloc(&e->crop_stage, need));
-  e->crop_stage_bytes = need;
-  return PARSEQ_OK;
+  return grow(e, &e->crop_stage, &e->crop_stage_bytes, need);
 }
 
 // Uploads the crop table of super-chunk [b0, b0 + Bc) on `st`.
@@ -1824,9 +1888,8 @@ int check_crops_call(parseq_engine* e, const parseq_forward_args* a, const parse
   if (a->forced_ids != nullptr || a->forced_refine != nullptr)
     return fail(PARSEQ_ERR_INVALID_ARG, "teacher forcing is a device-pointer API (parseq_forward)");
   PQ_TRY(check_crops(a->batch, crops));
-  if (e == nullptr || logits == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
-  if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
-  if (!e->finalized) return fail(PARSEQ_ERR_STATE, "parseq_finalize has not been called after the last weight update");
+  if (logits == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  PQ_TRY(check_ready(e));
   return check_crop_smem(e, a->batch, crops);
 }
 
@@ -1866,7 +1929,7 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
   }
   const int L = num_steps_of(e, a->max_length);
   const bool testing = a->max_length < 0;
-  const long long img_sz = 3ll * e->cfg.img_h * e->cfg.img_w * (u8 ? 1 : 4);   // bytes per image
+  const long long img_sz = image_bytes(e, u8);
   const char* images = static_cast<const char*>(images_any);
   void* in_static = u8 ? static_cast<void*>(e->in_images_u8) : static_cast<void*>(e->in_images);
   const bool eager = !e->use_graph || e->timing || a->forced_ids != nullptr || a->forced_refine != nullptr;
@@ -1887,9 +1950,7 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
     PQ_CUDA(cudaMemcpyAsync(maps + 1ll * b0 * L * e->T, e->out_maps, static_cast<size_t>(1ll * Bc * L * e->T) * 4, kout, e->main));
     return PARSEQ_OK;
   };
-  // user stream -> main
-  PQ_CUDA(cudaEventRecord(e->ev_in, user));
-  PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_in, 0));
+  PQ_TRY(enter_main(e, user));
   PQ_TRY(launch_k(e->lo, pq::set_int_kernel, dim3(1), dim3(32), 0, e->main, e->out_steps,
                   (testing && a->decode_ar && e->arch == 0) ? 0 : L));
   e->launches++;
@@ -1957,9 +2018,22 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
     PQ_TRY(copy_maps(b0, Bc));
   }
   if (steps) PQ_CUDA(cudaMemcpyAsync(steps, e->out_steps, 4, kout, e->main));
-  // main -> user stream
-  PQ_CUDA(cudaEventRecord(e->ev_out, e->main));
-  PQ_CUDA(cudaStreamWaitEvent(user, e->ev_out, 0));
+  return leave_main(e, user);
+}
+
+// parseq_forward / _host / _u8 / _host_u8: `host` (host buffers; the call returns once the outputs are there) and `u8`
+// (uint8 HWC images) as in forward_impl.  Teacher forcing is a device-pointer API.
+int forward_call(parseq_engine* e, const parseq_forward_args* a, const void* images, float* logits, int32_t* ids,
+                 int32_t* steps, parseq_stream_t stream, bool host, bool u8) {
+  if (a == nullptr || images == nullptr || logits == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  PQ_TRY(check_ready(e));
+  if (a->batch < 0 || a->refine_iters < 0) return fail(PARSEQ_ERR_INVALID_ARG, "negative batch / refine_iters");
+  if (a->batch == 0) return PARSEQ_OK;
+  if (host && (a->forced_ids != nullptr || a->forced_refine != nullptr))
+    return fail(PARSEQ_ERR_INVALID_ARG, "teacher forcing is a device-pointer API (parseq_forward)");
+  PQ_CUDA(cudaSetDevice(e->cfg.device));
+  PQ_TRY(forward_impl(e, a, images, logits, ids, steps, reinterpret_cast<cudaStream_t>(stream), host, u8));
+  if (host) PQ_CUDA(cudaStreamSynchronize(e->main));
   return PARSEQ_OK;
 }
 
@@ -2032,10 +2106,10 @@ struct ScoreGroup {
 // and a gather per candidate (ViTSTR).
 int score_impl(parseq_engine* e, const parseq_score_args* a, const void* images_any, bool u8, float* scores, float* token_lp,
                cudaStream_t user) {
-  const int L = e->L, D = e->D, T = e->T, N = a->batch, M = a->num_candidates;
+  const int L = e->L, D = e->D, N = a->batch, M = a->num_candidates;
   const int bos = e->V - 2, pad = e->V - 1;
   const int ntiles = (e->C + pq::GEMM_BLOCK_N - 1) / pq::GEMM_BLOCK_N;
-  const long long img_sz = 3ll * e->cfg.img_h * e->cfg.img_w * (u8 ? 1 : 4);
+  const long long img_sz = image_bytes(e, u8);
   const char* images = static_cast<const char*>(images_any);
   PQ_TRY(score_reserve(e));
   // host metadata: lengths [M], then per arch the candidates' targets / images or the groups' ids, targets, offsets
@@ -2088,26 +2162,17 @@ int score_impl(parseq_engine* e, const parseq_score_args* a, const void* images_
       }
     }
   }
-  if (static_cast<long long>(h.size()) > e->sc_meta_ints) {
-    PQ_CUDA(cudaStreamSynchronize(e->main));                          // the previous call's kernels may still read it
-    if (e->sc_meta) cudaFree(e->sc_meta);
-    e->sc_meta = nullptr;
-    e->sc_meta_ints = 0;
-    PQ_TRY(dev_alloc(&e->sc_meta, static_cast<long long>(h.size())));
-    e->sc_meta_ints = static_cast<long long>(h.size());
-  }
+  PQ_TRY(grow(e, &e->sc_meta, &e->sc_meta_ints, static_cast<long long>(h.size())));
   const int* meta = e->sc_meta;
-  PQ_CUDA(cudaEventRecord(e->ev_in, user));
-  PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_in, 0));
+  PQ_TRY(enter_main(e, user));
   // pageable source: the copy is staged before the call returns, so `h` may go
   PQ_CUDA(cudaMemcpyAsync(e->sc_meta, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice, e->main));
   size_t gi = 0;
   for (int b0 = 0; b0 < N; b0 += e->max_batch) {
     const int Bc = std::min(N - b0, e->max_batch);
     if (e->arch == 1) {
-      for (int o = 0; o < Bc; o += e->chunk) {
-        const int Bs = std::min(Bc - o, e->chunk), b = b0 + o;
-        PQ_TRY(encode_chunk(e, images + b * img_sz, u8, Bs, nullptr, nullptr, e->main, false));
+      PQ_TRY(vitstr_chunks(e, images + b0 * img_sz, u8, Bc, [&](int o, int Bs) -> int {
+        const int b = b0 + o;
         PQ_TRY(vitstr_rows(e, Bs, L, e->main));
         {
           TimedScope ts(e, e->main, CAT_SCORE, 2.0 * Bs * L * e->C * D);
@@ -2116,72 +2181,47 @@ int score_impl(parseq_engine* e, const parseq_score_args* a, const void* images_
         }
         const int m0 = first[b], nc = first[b + Bs] - m0;
         TimedScope ts(e, e->main, CAT_SCORE, 0.0);
-        PQ_TRY(launch_k(e->lo, pq::score_reduce_kernel, dim3(static_cast<unsigned>(nc)), dim3(64), 0, e->main,
+        return launch_k(e->lo, pq::score_reduce_kernel, dim3(static_cast<unsigned>(nc)), dim3(64), 0, e->main,
                         static_cast<const float2*>(e->sc_vt_part), ntiles, static_cast<const float*>(nullptr),
                         meta + vt_tgt_off + 1ll * m0 * L, meta + len_off, meta + vt_img_off, m0, b, L,
-                        static_cast<const __nv_bfloat16*>(e->xn), e->wb("head.weight"), e->wf("head.bias"), D, scores, token_lp, L));
-      }
+                        static_cast<const __nv_bfloat16*>(e->xn), e->wb("head.weight"), e->wf("head.bias"), D, scores, token_lp, L);
+      }));
       continue;
     }
-    for (int o = 0; o < Bc; o += e->chunk) {
-      const int Bs = std::min(Bc - o, e->chunk);
-      // kernel regime from the super-chunk, as forward_super: the memory bits equal the forward's
-      PQ_TRY(encode_chunk(e, images + (b0 + o) * img_sz, u8, Bs, e->mem + 1ll * o * T * D, nullptr, e->main, true, Bc));
-    }
-    PQ_TRY(cross_kv(e, Bc));
+    PQ_TRY(encode_super(e, images + b0 * img_sz, u8, Bc));
     size_t g_end = gi;
     while (g_end < groups.size() && groups[g_end].b_lo < b0 + Bc) ++g_end;
-    const int ns = static_cast<int>(e->stages.size());
-    const int used = static_cast<int>(std::min<size_t>(g_end - gi, static_cast<size_t>(ns)));
-    const bool fork = used > 1 && !e->timing;            // timing mode: everything on `main` (isolated kernel times)
-    if (fork) PQ_CUDA(cudaEventRecord(e->ev_enc, e->main));
-    for (int s = 0; s < used; ++s)
-      if (fork) PQ_CUDA(cudaStreamWaitEvent(e->stages[static_cast<size_t>(s)].stream, e->ev_enc, 0));
-    for (size_t k = gi; k < g_end; ++k) {
-      const ScoreGroup& g = groups[k];
-      parseq_engine::Stage& sg = e->stages[(k - gi) % static_cast<size_t>(ns)];
-      cudaStream_t ds = fork ? sg.stream : e->main;
+    PQ_TRY(fan_out(e, static_cast<int>(g_end - gi), [&](int k, parseq_engine::Stage& sg, cudaStream_t ds) -> int {
+      const ScoreGroup& g = groups[gi + static_cast<size_t>(k)];
       const int B = g.m1 - g.m0;
       const unsigned char* causal = e->sc_causal + 1ll * (g.P - 1) * L * L;
       DecodeExtras ex;
       ex.qmask = causal;
       ex.cmask = e->cfg.dec_depth > 1 ? causal : nullptr;
       ex.lse_tgt = meta + g.tgt_off;
-      sg.cand_off = meta + g.cand_off;
-      sg.cand_imgs = g.nimg;
-      sg.cand_max_rows = g.max_rows;
-      const int rc = decode_pass(e, sg, g.b_lo - b0, B, g.P, 0, g.P, 0, meta + g.ids_off, nullptr, 0, nullptr, 0, nullptr, 0,
-                                 nullptr, ds, &ex);
-      sg.cand_off = nullptr;
-      PQ_TRY(rc);
+      ex.cand_off = meta + g.cand_off;
+      ex.cand_imgs = g.nimg;
+      ex.cand_max_rows = g.max_rows;
+      PQ_TRY(decode_pass(e, sg, g.b_lo - b0, B, g.P, 0, g.P, 0, meta + g.ids_off, nullptr, 0, nullptr, 0, nullptr, 0, nullptr,
+                         ds, &ex));
       TimedScope ts(e, ds, CAT_SCORE, 0.0);
-      PQ_TRY(launch_k(e->lo, pq::score_reduce_kernel, dim3(static_cast<unsigned>(B)), dim3(64), 0, ds,
+      return launch_k(e->lo, pq::score_reduce_kernel, dim3(static_cast<unsigned>(B)), dim3(64), 0, ds,
                       static_cast<const float2*>(sg.lse_part), ntiles, static_cast<const float*>(sg.lse_tlogit),
                       static_cast<const int*>(nullptr), meta + len_off, static_cast<const int*>(nullptr), g.m0, 0, g.P,
                       static_cast<const __nv_bfloat16*>(nullptr), static_cast<const __nv_bfloat16*>(nullptr),
-                      static_cast<const float*>(nullptr), D, scores, token_lp, L));
-    }
-    if (fork) {
-      for (int s = 0; s < used; ++s) {
-        parseq_engine::Stage& sg = e->stages[static_cast<size_t>(s)];
-        PQ_CUDA(cudaEventRecord(sg.ev_done, sg.stream));
-        PQ_CUDA(cudaStreamWaitEvent(e->main, sg.ev_done, 0));
-      }
-    }
+                      static_cast<const float*>(nullptr), D, scores, token_lp, L);
+    }));
     gi = g_end;
   }
-  PQ_CUDA(cudaEventRecord(e->ev_out, e->main));
-  PQ_CUDA(cudaStreamWaitEvent(user, e->ev_out, 0));
-  return PARSEQ_OK;
+  return leave_main(e, user);
 }
 
 // Shared checks of the score entry points: the counts first (a NULL handle is enough for them), then the handle, then
 // the targets against its configuration.
 int check_score_call(parseq_engine* e, const parseq_score_args* a, const void* images, const float* scores) {
   PQ_TRY(check_score(a, -1, 0));
-  if (e == nullptr || images == nullptr || scores == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
-  if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
-  if (!e->finalized) return fail(PARSEQ_ERR_STATE, "parseq_finalize has not been called after the last weight update");
+  if (images == nullptr || scores == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  PQ_TRY(check_ready(e));
   return check_score(a, e->cfg.max_label_length, e->C);
 }
 
@@ -2189,39 +2229,42 @@ int check_score_call(parseq_engine* e, const parseq_score_args* a, const void* i
 // ViTSTR: images whose [L, C] logits one beam group holds (the head runs once per group, the selection once per position)
 int beam_vt_images(const parseq_engine* e) { return std::min(e->chunk, 32); }
 
+// A beam-search buffer of n elements, on first use (counted in beam_bytes)
+template <typename Tp>
+int beam_alloc(parseq_engine* e, Tp** p, long long n) {
+  if (*p != nullptr) return PARSEQ_OK;
+  PQ_TRY(dev_alloc(p, n));
+  e->beam_bytes += n * static_cast<long long>(sizeof(Tp));
+  return PARSEQ_OK;
+}
+
 // Beam buffers, on the first beam call (an engine that never beam-searches allocates none of them).  PARSeq: every stage
 // holds dec_chunk beam rows, whatever the beam width; ViTSTR: stage 0 holds beam_vt_images images of BEAM_MAX slots.
 int beam_reserve(parseq_engine* e) {
   const size_t nst = e->arch == 0 ? e->stages.size() : 1;
   const int D = e->D;
-  auto grab = [&](auto** p, long long n) -> int {
-    if (*p != nullptr) return PARSEQ_OK;
-    PQ_TRY(dev_alloc(p, n));
-    e->beam_bytes += n * static_cast<long long>(sizeof(**p));
-    return PARSEQ_OK;
-  };
   for (size_t s = 0; s < nst; ++s) {
     parseq_engine::Stage::Beam& bm = e->stages[s].bm;
     if (bm.rows > 0) continue;
     const int rows = e->arch == 0 ? e->dec_chunk : beam_vt_images(e) * pq::BEAM_MAX;
     const long long lrows = e->arch == 0 ? rows : 1ll * beam_vt_images(e) * e->L;
     for (int h = 0; h < 2; ++h) {
-      PQ_TRY(grab(&bm.ids[h], 1ll * rows * e->ids_ld));
-      PQ_TRY(grab(&bm.score[h], rows));
-      PQ_TRY(grab(&bm.len[h], rows));
-      PQ_TRY(grab(&bm.st[h], rows));
+      PQ_TRY(beam_alloc(e, &bm.ids[h], 1ll * rows * e->ids_ld));
+      PQ_TRY(beam_alloc(e, &bm.score[h], rows));
+      PQ_TRY(beam_alloc(e, &bm.len[h], rows));
+      PQ_TRY(beam_alloc(e, &bm.st[h], rows));
     }
-    PQ_TRY(grab(&bm.parent, rows));
+    PQ_TRY(beam_alloc(e, &bm.parent, rows));
     const long long ntiles = (e->C + pq::GEMM_BLOCK_N - 1) / pq::GEMM_BLOCK_N;
     if (e->C <= 128) {
-      PQ_TRY(grab(&bm.logits, lrows * e->C));
+      PQ_TRY(beam_alloc(e, &bm.logits, lrows * e->C));
     } else {
-      PQ_TRY(grab(&bm.part, lrows * ntiles));
-      PQ_TRY(grab(&bm.keys, lrows * ntiles * pq::BEAM_TOPK_LD));
+      PQ_TRY(beam_alloc(e, &bm.part, lrows * ntiles));
+      PQ_TRY(beam_alloc(e, &bm.keys, lrows * ntiles * pq::BEAM_TOPK_LD));
     }
     if (e->arch == 0 && e->cfg.dec_depth > 1) {
       bm.kvc.resize(static_cast<size_t>(e->cfg.dec_depth - 1), nullptr);
-      for (auto& c : bm.kvc) PQ_TRY(grab(&c, 1ll * e->dec_chunk * e->L * 2 * D));
+      for (auto& c : bm.kvc) PQ_TRY(beam_alloc(e, &c, 1ll * e->dec_chunk * e->L * 2 * D));
     }
     bm.rows = rows;
   }
@@ -2241,17 +2284,11 @@ int beam_lex_vt_images(const parseq_engine* e) {
 // and dec_chunk 128; ViTSTR: beam_lex_vt_images images' L positions).
 int lexicon_reserve(parseq_engine* e) {
   const size_t nst = e->arch == 0 ? e->stages.size() : 1;
-  auto grab = [&](auto** p, long long n) -> int {
-    if (*p != nullptr) return PARSEQ_OK;
-    PQ_TRY(dev_alloc(p, n));
-    e->beam_bytes += n * static_cast<long long>(sizeof(**p));
-    return PARSEQ_OK;
-  };
   for (size_t s = 0; s < nst; ++s) {
     parseq_engine::Stage::Beam& bm = e->stages[s].bm;
-    for (int h = 0; h < 2; ++h) PQ_TRY(grab(&bm.node[h], bm.rows));
+    for (int h = 0; h < 2; ++h) PQ_TRY(beam_alloc(e, &bm.node[h], bm.rows));
     const long long lrows = e->arch == 0 ? e->dec_chunk : 1ll * beam_lex_vt_images(e) * e->L;
-    PQ_TRY(grab(&bm.logits, lrows * e->C));
+    PQ_TRY(beam_alloc(e, &bm.logits, lrows * e->C));
   }
   return PARSEQ_OK;
 }
@@ -2263,9 +2300,9 @@ int lexicon_reserve(parseq_engine* e) {
 // beam_select_kernel once per position.
 int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_any, bool u8, int* ids, int* lengths,
               float* scores, cudaStream_t user, const parseq_lexicon* lx = nullptr, const int* roots = nullptr) {
-  const int N = a->batch, K = a->beam_width, D = e->D, T = e->T, C = e->C, L = e->L;
+  const int N = a->batch, K = a->beam_width, D = e->D, C = e->C, L = e->L;
   const int S = num_steps_of(e, a->max_length);
-  const long long img_sz = 3ll * e->cfg.img_h * e->cfg.img_w * (u8 ? 1 : 4);
+  const long long img_sz = image_bytes(e, u8);
   const char* images = static_cast<const char*>(images_any);
   PQ_TRY(beam_reserve(e));
   if (lx != nullptr) PQ_TRY(lexicon_reserve(e));
@@ -2281,18 +2318,10 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
   const int ntiles = (C + pq::GEMM_BLOCK_N - 1) / pq::GEMM_BLOCK_N;
   if (lx != nullptr && roots != nullptr) {
     // `roots`: the checked host copy of the call's roots (beam_lexicon_call), uploaded below
-    if (e->lex_roots_cap < N) {
-      if (e->lex_roots != nullptr) {
-        PQ_CUDA(cudaStreamSynchronize(e->main));                      // the previous call's kernels may still read it
-        PQ_CUDA(cudaFree(e->lex_roots));
-        e->beam_bytes -= 4ll * e->lex_roots_cap;
-        e->lex_roots = nullptr;
-        e->lex_roots_cap = 0;
-      }
-      PQ_TRY(dev_alloc(&e->lex_roots, N));
-      e->lex_roots_cap = N;
-      e->beam_bytes += 4ll * N;
-    }
+    const long long cap0 = e->lex_roots_cap;
+    const int rc = grow(e, &e->lex_roots, &e->lex_roots_cap, N);
+    e->beam_bytes += 4ll * (e->lex_roots_cap - cap0);
+    PQ_TRY(rc);
   }
   auto select = [&](parseq_engine::Stage::Beam& bm, int B, int step, long long row0, long long img_stride,
                     long long slot_stride, int g0, cudaStream_t st) {
@@ -2311,8 +2340,7 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
                     bm.len[nxt], bm.st[nxt], bm.parent, e->ids_ld, ids + 1ll * g0 * K * S, lengths + 1ll * g0 * K,
                     scores + 1ll * g0 * K, bl);
   };
-  PQ_CUDA(cudaEventRecord(e->ev_in, user));
-  PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_in, 0));
+  PQ_TRY(enter_main(e, user));
   // pageable source (a std::vector of beam_lexicon_call): the copy is staged before the call returns
   if (lx != nullptr && roots != nullptr)
     PQ_CUDA(cudaMemcpyAsync(e->lex_roots, roots, 4ull * N, cudaMemcpyHostToDevice, e->main));
@@ -2321,9 +2349,7 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
     if (e->arch == 1) {
       parseq_engine::Stage::Beam& bm = e->stages[0].bm;
       const int G = lx != nullptr ? beam_lex_vt_images(e) : beam_vt_images(e);
-      for (int o = 0; o < Bc; o += e->chunk) {
-        const int Bs = std::min(Bc - o, e->chunk);
-        PQ_TRY(encode_chunk(e, images + (b0 + o) * img_sz, u8, Bs, nullptr, nullptr, e->main, false));
+      PQ_TRY(vitstr_chunks(e, images + b0 * img_sz, u8, Bc, [&](int o, int Bs) -> int {
         PQ_TRY(vitstr_rows(e, Bs, L, e->main));
         for (int g = 0; g < Bs; g += G) {
           const int Bg = std::min(G, Bs - g);
@@ -2340,28 +2366,14 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
           PQ_TRY(init(bm, Bg, e->main));
           for (int step = 0; step < S; ++step) PQ_TRY(select(bm, Bg, step, step, L, 0, b0 + o + g, e->main));
         }
-      }
+        return PARSEQ_OK;
+      }));
       continue;
     }
-    for (int o = 0; o < Bc; o += e->chunk) {
-      const int Bs = std::min(Bc - o, e->chunk);
-      // kernel regime from the super-chunk, as forward_super: the memory bits equal the forward's
-      PQ_TRY(encode_chunk(e, images + (b0 + o) * img_sz, u8, Bs, e->mem + 1ll * o * T * D, nullptr, e->main, true, Bc));
-    }
-    PQ_TRY(cross_kv(e, Bc));
+    PQ_TRY(encode_super(e, images + b0 * img_sz, u8, Bc));
     const int G = e->dec_chunk / K;                    // images per group: G * K beam rows fill a stage's buffers
-    const int ngroups = (Bc + G - 1) / G;
-    const int ns = static_cast<int>(e->stages.size());
-    const int used = std::min(ngroups, ns);
-    const bool fork = used > 1 && !e->timing;            // timing mode: everything on `main` (isolated kernel times)
-    if (fork) {
-      PQ_CUDA(cudaEventRecord(e->ev_enc, e->main));
-      for (int s = 0; s < used; ++s) PQ_CUDA(cudaStreamWaitEvent(e->stages[static_cast<size_t>(s)].stream, e->ev_enc, 0));
-    }
-    for (int gi = 0; gi < ngroups; ++gi) {
-      parseq_engine::Stage& sg = e->stages[static_cast<size_t>(gi % ns)];
+    PQ_TRY(fan_out(e, (Bc + G - 1) / G, [&](int gi, parseq_engine::Stage& sg, cudaStream_t ds) -> int {
       parseq_engine::Stage::Beam& bm = sg.bm;
-      cudaStream_t ds = fork ? sg.stream : e->main;
       const int g0 = gi * G, Bg = std::min(G, Bc - g0), R = Bg * K;
       PQ_TRY(init(bm, Bg, ds));
       DecodeExtras ex;
@@ -2397,19 +2409,10 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
       // the stage's own cache pointers back (their contents are scratch between calls)
       for (size_t l = 0; l < sg.kvc.size(); ++l)
         if (sg.kvc[l] != kvc0[l]) std::swap(sg.kvc[l], bm.kvc[l]);
-      PQ_TRY(rc);
-    }
-    if (fork) {
-      for (int s = 0; s < used; ++s) {
-        parseq_engine::Stage& sg = e->stages[static_cast<size_t>(s)];
-        PQ_CUDA(cudaEventRecord(sg.ev_done, sg.stream));
-        PQ_CUDA(cudaStreamWaitEvent(e->main, sg.ev_done, 0));
-      }
-    }
+      return rc;
+    }));
   }
-  PQ_CUDA(cudaEventRecord(e->ev_out, e->main));
-  PQ_CUDA(cudaStreamWaitEvent(user, e->ev_out, 0));
-  return PARSEQ_OK;
+  return leave_main(e, user);
 }
 
 // The host checks of a lexicon (parseq_lexicon_check) against C head classes and labels of at most max_label_length
@@ -2454,10 +2457,9 @@ int check_beam_call(parseq_engine* e, const parseq_beam_args* a, const void* ima
   if (a->beam_width < 1 || a->beam_width > pq::BEAM_MAX)
     return fail(PARSEQ_ERR_INVALID_ARG, "beam_width " + std::to_string(a->beam_width) + " outside [1, 16]");
   if (a->max_length < -1) return fail(PARSEQ_ERR_INVALID_ARG, "max_length must be -1 (None) or >= 0");
-  if (e == nullptr || (a->batch > 0 && (images == nullptr || ids == nullptr || lengths == nullptr || scores == nullptr)))
+  if (a->batch > 0 && (images == nullptr || ids == nullptr || lengths == nullptr || scores == nullptr))
     return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
-  if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
-  if (!e->finalized) return fail(PARSEQ_ERR_STATE, "parseq_finalize has not been called after the last weight update");
+  PQ_TRY(check_ready(e));
   if (e->arch == 0 && a->beam_width > e->dec_chunk)
     return fail(PARSEQ_ERR_INVALID_ARG, "beam_width " + std::to_string(a->beam_width) + " exceeds the decoder chunk (option "
                                         "dec_chunk = " + std::to_string(e->dec_chunk) + ")");
@@ -2745,81 +2747,41 @@ int parseq_finalize(parseq_engine* e, parseq_stream_t stream) {
 
 int parseq_forward(parseq_engine* e, const parseq_forward_args* a, const float* images, float* logits, int32_t* ids,
                    int32_t* steps, parseq_stream_t stream) {
-  if (e == nullptr || a == nullptr || images == nullptr || logits == nullptr)
-    return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
-  if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
-  if (!e->finalized) return fail(PARSEQ_ERR_STATE, "parseq_finalize has not been called after the last weight update");
-  if (a->batch < 0 || a->refine_iters < 0) return fail(PARSEQ_ERR_INVALID_ARG, "negative batch / refine_iters");
-  if (a->batch == 0) return PARSEQ_OK;
-  PQ_CUDA(cudaSetDevice(e->cfg.device));
-  return forward_impl(e, a, images, logits, ids, steps, reinterpret_cast<cudaStream_t>(stream), false);
+  return forward_call(e, a, images, logits, ids, steps, stream, false, false);
 }
 
 int parseq_forward_host(parseq_engine* e, const parseq_forward_args* a, const float* images_host, float* logits_host,
                         int32_t* ids_host, int32_t* steps_host, parseq_stream_t stream) {
-  if (e == nullptr || a == nullptr || images_host == nullptr || logits_host == nullptr)
-    return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
-  if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
-  if (!e->finalized) return fail(PARSEQ_ERR_STATE, "parseq_finalize has not been called after the last weight update");
-  if (a->batch < 0 || a->refine_iters < 0) return fail(PARSEQ_ERR_INVALID_ARG, "negative batch / refine_iters");
-  if (a->batch == 0) return PARSEQ_OK;
-  if (a->forced_ids != nullptr || a->forced_refine != nullptr)
-    return fail(PARSEQ_ERR_INVALID_ARG, "teacher forcing is a device-pointer API (parseq_forward)");
-  PQ_CUDA(cudaSetDevice(e->cfg.device));
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  PQ_TRY(forward_impl(e, a, images_host, logits_host, ids_host, steps_host, st, true));
-  PQ_CUDA(cudaStreamSynchronize(e->main));
-  return PARSEQ_OK;
+  return forward_call(e, a, images_host, logits_host, ids_host, steps_host, stream, true, false);
 }
 
 int parseq_forward_u8(parseq_engine* e, const parseq_forward_args* a, const uint8_t* images_hwc, float* logits, int32_t* ids,
                       int32_t* steps, parseq_stream_t stream) {
-  if (e == nullptr || a == nullptr || images_hwc == nullptr || logits == nullptr)
-    return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
-  if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
-  if (!e->finalized) return fail(PARSEQ_ERR_STATE, "parseq_finalize has not been called after the last weight update");
-  if (a->batch < 0 || a->refine_iters < 0) return fail(PARSEQ_ERR_INVALID_ARG, "negative batch / refine_iters");
-  if (a->batch == 0) return PARSEQ_OK;
-  PQ_CUDA(cudaSetDevice(e->cfg.device));
-  return forward_impl(e, a, images_hwc, logits, ids, steps, reinterpret_cast<cudaStream_t>(stream), false, true);
+  return forward_call(e, a, images_hwc, logits, ids, steps, stream, false, true);
 }
 
 int parseq_forward_host_u8(parseq_engine* e, const parseq_forward_args* a, const uint8_t* images_hwc_host, float* logits_host,
                            int32_t* ids_host, int32_t* steps_host, parseq_stream_t stream) {
-  if (e == nullptr || a == nullptr || images_hwc_host == nullptr || logits_host == nullptr)
-    return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
-  if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
-  if (!e->finalized) return fail(PARSEQ_ERR_STATE, "parseq_finalize has not been called after the last weight update");
-  if (a->batch < 0 || a->refine_iters < 0) return fail(PARSEQ_ERR_INVALID_ARG, "negative batch / refine_iters");
-  if (a->batch == 0) return PARSEQ_OK;
-  if (a->forced_ids != nullptr || a->forced_refine != nullptr)
-    return fail(PARSEQ_ERR_INVALID_ARG, "teacher forcing is a device-pointer API (parseq_forward)");
-  PQ_CUDA(cudaSetDevice(e->cfg.device));
-  PQ_TRY(forward_impl(e, a, images_hwc_host, logits_host, ids_host, steps_host, reinterpret_cast<cudaStream_t>(stream), true, true));
-  PQ_CUDA(cudaStreamSynchronize(e->main));
-  return PARSEQ_OK;
+  return forward_call(e, a, images_hwc_host, logits_host, ids_host, steps_host, stream, true, true);
 }
 
 int parseq_resize_crops(parseq_engine* e, int32_t batch, const parseq_crops* crops, uint8_t* out_hwc, parseq_stream_t stream) {
   if (batch < 0) return fail(PARSEQ_ERR_INVALID_ARG, "negative batch");
   PQ_TRY(check_crops(batch, crops));
-  if (e == nullptr || out_hwc == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
-  if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
+  if (out_hwc == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  PQ_TRY(check_ready(e, false));
   PQ_TRY(check_crop_smem(e, batch, crops));
   if (batch == 0) return PARSEQ_OK;
   PQ_CUDA(cudaSetDevice(e->cfg.device));
   cudaStream_t user = reinterpret_cast<cudaStream_t>(stream);
   const CropBatch cb{crops, false};
-  PQ_CUDA(cudaEventRecord(e->ev_in, user));
-  PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_in, 0));
+  PQ_TRY(enter_main(e, user));
   for (int b0 = 0; b0 < batch; b0 += e->max_batch) {
     const int Bc = (batch - b0 < e->max_batch) ? (batch - b0) : e->max_batch;
     PQ_TRY(crops_table(e, cb, b0, Bc, e->main));
     PQ_TRY(crops_resize(e, cb, b0, 0, Bc, out_hwc + 3ll * e->cfg.img_h * e->cfg.img_w * b0, e->main));
   }
-  PQ_CUDA(cudaEventRecord(e->ev_out, e->main));
-  PQ_CUDA(cudaStreamWaitEvent(user, e->ev_out, 0));
-  return PARSEQ_OK;
+  return leave_main(e, user);
 }
 
 int parseq_forward_crops(parseq_engine* e, const parseq_forward_args* a, const parseq_crops* crops, float* logits, int32_t* ids,
@@ -2947,21 +2909,17 @@ int parseq_postprocess(const float* logits, int32_t batch, int32_t num_steps, in
 }
 
 int parseq_encode(parseq_engine* e, int32_t batch, const float* images, float* memory, parseq_stream_t stream) {
-  if (e == nullptr || images == nullptr || memory == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
-  if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
-  if (!e->finalized) return fail(PARSEQ_ERR_STATE, "parseq_finalize has not been called");
+  if (images == nullptr || memory == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  PQ_TRY(check_ready(e));
   PQ_CUDA(cudaSetDevice(e->cfg.device));
   cudaStream_t user = reinterpret_cast<cudaStream_t>(stream);
-  PQ_CUDA(cudaEventRecord(e->ev_in, user));
-  PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_in, 0));
+  PQ_TRY(enter_main(e, user));
   const long long img_sz = 3ll * e->cfg.img_h * e->cfg.img_w;
   for (int b0 = 0; b0 < batch; b0 += e->chunk) {
     const int B = (batch - b0 < e->chunk) ? (batch - b0) : e->chunk;
     PQ_TRY(encode_chunk(e, images + b0 * img_sz, false, B, e->mem, memory + 1ll * b0 * e->T * e->D, e->main));
   }
-  PQ_CUDA(cudaEventRecord(e->ev_out, e->main));
-  PQ_CUDA(cudaStreamWaitEvent(user, e->ev_out, 0));
-  return PARSEQ_OK;
+  return leave_main(e, user);
 }
 
 int parseq_decode(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t num_queries, const int32_t* tgt, const float* memory,
@@ -2973,17 +2931,15 @@ int parseq_decode(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t num_
 int parseq_decode_ex(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t num_queries, const int32_t* tgt,
                      const float* memory, const float* query, const uint8_t* query_mask, const uint8_t* padding_mask,
                      const uint8_t* content_mask, float* out, parseq_stream_t stream) {
-  if (e == nullptr || tgt == nullptr || memory == nullptr || out == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
-  if (e->broken) return fail(PARSEQ_ERR_STATE, "engine workspace is gone (a failed resize): destroy the handle");
-  if (!e->finalized) return fail(PARSEQ_ERR_STATE, "parseq_finalize has not been called");
+  if (tgt == nullptr || memory == nullptr || out == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  PQ_TRY(check_ready(e));
   if (e->arch != 0) return fail(PARSEQ_ERR_UNSUPPORTED, "decode: PARSeq only");
   if (batch < 0 || ctx_len < 1 || ctx_len > e->L || num_queries < 1 || num_queries > e->L)
     return fail(PARSEQ_ERR_INVALID_ARG, "decode: 1 <= context length, queries <= max_label_length + 1");
   if (batch == 0) return PARSEQ_OK;
   PQ_CUDA(cudaSetDevice(e->cfg.device));
   cudaStream_t user = reinterpret_cast<cudaStream_t>(stream);
-  PQ_CUDA(cudaEventRecord(e->ev_in, user));
-  PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_in, 0));
+  PQ_TRY(enter_main(e, user));
   const int D = e->D, T = e->T, J = ctx_len, NQ = num_queries;
   parseq_engine::Stage& sg = e->stages[0];
   cudaStream_t st = e->main;
@@ -2994,13 +2950,7 @@ int parseq_decode_ex(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t n
     pq::f32_to_bf16_kernel<<<static_cast<unsigned>(std::min<long long>((n4 + 255) / 256, 132ll * 8)), 256, 0, st>>>(
         reinterpret_cast<const float4*>(memory + 1ll * b0 * T * D), reinterpret_cast<uint2*>(e->mem), n4);
     PQ_CUDA(cudaGetLastError());
-    e->cur_cat = CAT_DEC_GEMM;
-    for (int l = 0; l < e->cfg.dec_depth; ++l) {
-      const std::string Ly = "decoder.layers." + std::to_string(l) + ".";
-      PQ_TRY(gemm(e, e->mem, D, e->wb(Ly + "cross_attn.in_proj_weight") + static_cast<long long>(D) * D, D,
-                  e->wf(Ly + "cross_attn.in_proj_bias") + D, Bc * T, 2 * D, D, pq::EPI_BF16, 1.0f, nullptr, 0, 0,
-                  const_cast<__nv_bfloat16*>(ckv_of(e, l)), 2 * D, st, 1ll * e->max_batch * T));
-    }
+    PQ_TRY(cross_kv(e, Bc));
     pq::copy_ids_kernel<<<(Bc * e->ids_ld + 255) / 256, 256, 0, st>>>(tgt + 1ll * b0 * J, J, sg.ids_ctx, Bc, e->ids_ld);
     PQ_CUDA(cudaGetLastError());
     e->launches += 2;
@@ -3012,19 +2962,16 @@ int parseq_decode_ex(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t n
     ex.out_norm = out + 1ll * b0 * NQ * D;
     PQ_TRY(decode_pass(e, sg, 0, Bc, NQ, 0, J, 0, sg.ids_ctx, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, st, &ex));
   }
-  PQ_CUDA(cudaEventRecord(e->ev_out, e->main));
-  PQ_CUDA(cudaStreamWaitEvent(user, e->ev_out, 0));
-  return PARSEQ_OK;
+  return leave_main(e, user);
 }
 
 int parseq_head(parseq_engine* e, int32_t rows, const float* x, float* logits, parseq_stream_t stream) {
-  if (e == nullptr || x == nullptr || logits == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
-  if (e->broken || !e->finalized) return fail(PARSEQ_ERR_STATE, "engine not ready");
+  if (x == nullptr || logits == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  PQ_TRY(check_ready(e));
   if (rows <= 0) return rows == 0 ? PARSEQ_OK : fail(PARSEQ_ERR_INVALID_ARG, "negative rows");
   PQ_CUDA(cudaSetDevice(e->cfg.device));
   cudaStream_t user = reinterpret_cast<cudaStream_t>(stream);
-  PQ_CUDA(cudaEventRecord(e->ev_in, user));
-  PQ_CUDA(cudaStreamWaitEvent(e->main, e->ev_in, 0));
+  PQ_TRY(enter_main(e, user));
   const int D = e->D;
   const int cap = e->dec_chunk * e->L;                 // rows of the bf16 staging buffer of a decoder chain
   parseq_engine::Stage& sg = e->stages[0];
@@ -3039,9 +2986,7 @@ int parseq_head(parseq_engine* e, int32_t rows, const float* x, float* logits, p
     PQ_TRY(gemm(e, sg.yn, D, e->w("head.weight"), D, e->wf("head.bias"), n, e->C, D, pq::EPI_F32, 1.0f, nullptr, 0, 0,
                 logits + 1ll * r0 * e->C, e->C, e->main));
   }
-  PQ_CUDA(cudaEventRecord(e->ev_out, e->main));
-  PQ_CUDA(cudaStreamWaitEvent(user, e->ev_out, 0));
-  return PARSEQ_OK;
+  return leave_main(e, user);
 }
 
 int parseq_text_embed(parseq_engine* e, int32_t n, const int32_t* ids, float* out, parseq_stream_t stream) {

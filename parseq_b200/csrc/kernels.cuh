@@ -685,28 +685,18 @@ __global__ void gather_ctx_rows_kernel(const float* __restrict__ emb, const floa
 }
 
 // ---------------------------------------------------------------------------------------------
-// Decoder cross-attention: one CTA per (image, head), 4 warps.  The head's K (padded pitch, lane = key reads are
-// conflict-free) and V tiles are staged once in shared memory, so the per-image K/V cache is read once per decode
-// pass; the nq queries are distributed over the warps and each query is handled entirely inside one warp (scores
-// for 4 keys per lane, shuffle softmax, lane = channel for P.V): no block-level synchronisation after the load.
-// q fp32 [B*nq, D] pre-scaled by 1/sqrt(32); kv bf16 [B, T, 2D]; out bf16 [B*nq, D].  T <= 128, head dim 32.
-template <int NR>   // keys per lane: T <= 32 * NR (NR = 4: T <= 128, NR = 8: T <= 256)
-__global__ void __launch_bounds__(128) dec_cross_attn3_kernel(const float* __restrict__ q,
-                                                              const __nv_bfloat16* __restrict__ kv, long long kv_rows,
-                                                              int b_first, int T, int D, int heads, int nq,
-                                                              __nv_bfloat16* __restrict__ out) {
-  // kv: column-blocked cross K/V cache [2D/64][kv_rows][64] (ptx.cuh: blocked_off), row = image * T + key; the
-  // queries / outputs of this launch belong to images b_first, b_first + 1, ...
-  constexpr int TK = 32 * NR;
-  __shared__ uint32_t sK[TK * 17];                        // bf16x2 words, pitch 17 (odd)
-  __shared__ __align__(16) __nv_bfloat16 sV[TK * 32];
-  grid_dep_launch();
-  grid_dep_wait();
-  const int b = blockIdx.x / heads, h = blockIdx.x % heads;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const long long row_b = static_cast<long long>(b_first + b) * T;
-  for (int t = tid; t < TK; t += 128) {
-    uint4* vd = reinterpret_cast<uint4*>(sV + t * 32);
+// Decoder cross-attention over the cached image K/V, head dim 32.  The pieces below are shared by the three kernels
+// that compute a cross-attention row's probabilities, so that they are computed one way: dec_cross_attn3_kernel (the
+// decoder's passes), dec_cross_attn3_grouped_kernel (candidate scoring) and dec_cross_attn_maps_kernel (the maps, which
+// must be bitwise the probabilities the P.V of the other two uses).
+// kv: column-blocked cross K/V cache [2D/64][kv_rows][64] (ptx.cuh: blocked_off), row = image * T + key.
+
+// Stages head h's K of keys [0, 32 * NR) of the image whose first cache row is row_b into sK (bf16x2 words, pitch 17:
+// odd, so that lane = key reads are conflict-free), and with V its V into sV [32 * NR][32]; keys >= T are zero.
+template <int NR, int NT, bool V>
+__device__ __forceinline__ void cross_stage_kv(uint32_t* sK, __nv_bfloat16* sV, const __nv_bfloat16* __restrict__ kv,
+                                               long long kv_rows, long long row_b, int T, int D, int h, int tid) {
+  for (int t = tid; t < 32 * NR; t += NT) {
     if (t < T) {
       const uint4* kr = reinterpret_cast<const uint4*>(kv + blocked_off(kv_rows, row_b + t, h * 32));
       const uint4* vr = reinterpret_cast<const uint4*>(kv + blocked_off(kv_rows, row_b + t, D + h * 32));
@@ -715,199 +705,155 @@ __global__ void __launch_bounds__(128) dec_cross_attn3_kernel(const float* __res
         const uint4 u = __ldg(kr + j);
         sK[t * 17 + j * 4 + 0] = u.x; sK[t * 17 + j * 4 + 1] = u.y;
         sK[t * 17 + j * 4 + 2] = u.z; sK[t * 17 + j * 4 + 3] = u.w;
-        vd[j] = __ldg(vr + j);
+        if (V) reinterpret_cast<uint4*>(sV + t * 32)[j] = __ldg(vr + j);
       }
     } else {
 #pragma unroll
       for (int j = 0; j < 16; ++j) sK[t * 17 + j] = 0u;
+      if (V) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) vd[j] = make_uint4(0u, 0u, 0u, 0u);
-    }
-  }
-  __syncthreads();
-  for (int qi = warp; qi < nq; qi += 4) {
-    const long long row = static_cast<long long>(b) * nq + qi;
-    const float qv = q[row * D + h * 32 + lane];          // lane j holds q_j
-    float sc[NR];
-#pragma unroll
-    for (int r = 0; r < NR; ++r) sc[r] = 0.f;
-#pragma unroll
-    for (int w = 0; w < 16; ++w) {
-      const float qa = __shfl_sync(0xffffffffu, qv, 2 * w), qb = __shfl_sync(0xffffffffu, qv, 2 * w + 1);
-#pragma unroll
-      for (int r = 0; r < NR; ++r) {
-        const uint32_t kw = sK[(r * 32 + lane) * 17 + w];
-        sc[r] = fmaf(qb, __uint_as_float(kw & 0xffff0000u), fmaf(qa, __uint_as_float(kw << 16), sc[r]));
+        for (int j = 0; j < 4; ++j) reinterpret_cast<uint4*>(sV + t * 32)[j] = make_uint4(0u, 0u, 0u, 0u);
       }
-    }
-    float mx = -INFINITY;
-#pragma unroll
-    for (int r = 0; r < NR; ++r) {
-      if (r * 32 + lane >= T) sc[r] = -INFINITY;
-      mx = fmaxf(mx, sc[r]);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    float sum = 0.f;
-#pragma unroll
-    for (int r = 0; r < NR; ++r) {
-      sc[r] = expf(sc[r] - mx);
-      sum += sc[r];
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    // P.V with 16-byte smem reads: lane = (key group kg = lane>>2, 8-channel chunk cc = lane&3); 4*NR iterations cover
-    // the keys; the 8 key groups are then summed with xor-shuffles and lanes 0..3 hold the 32 output channels.
-    const int kg = lane >> 2, cc = lane & 3;
-    float o[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) o[j] = 0.f;
-#pragma unroll
-    for (int it = 0; it < 4 * NR; ++it) {              // key = it*8 + kg -> register sc[it>>2], source lane (it&3)*8 + kg
-      const int key = it * 8 + kg;
-      const uint4 vvv = *reinterpret_cast<const uint4*>(sV + key * 32 + cc * 8);
-      const float pk = __shfl_sync(0xffffffffu, sc[it >> 2], (it & 3) * 8 + kg);
-      const __nv_bfloat162* p2 = reinterpret_cast<const __nv_bfloat162*>(&vvv);
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float2 f = __bfloat1622float2(p2[e]);
-        o[e * 2] = fmaf(pk, f.x, o[e * 2]);
-        o[e * 2 + 1] = fmaf(pk, f.y, o[e * 2 + 1]);
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      o[j] += __shfl_xor_sync(0xffffffffu, o[j], 4);
-      o[j] += __shfl_xor_sync(0xffffffffu, o[j], 8);
-      o[j] += __shfl_xor_sync(0xffffffffu, o[j], 16);
-    }
-    if (kg == 0) {
-      const float inv = 1.0f / sum;
-      uint4 q4;
-      q4.x = pack_bf16(o[0] * inv, o[1] * inv); q4.y = pack_bf16(o[2] * inv, o[3] * inv);
-      q4.z = pack_bf16(o[4] * inv, o[5] * inv); q4.w = pack_bf16(o[6] * inv, o[7] * inv);
-      *reinterpret_cast<uint4*>(out + row * D + h * 32 + cc * 8) = q4;
     }
   }
 }
 
-// Candidate scoring: the query rows of image b_first + j are rows [cand_off[j] * nq, cand_off[j + 1] * nq) (candidates
-// are image-major, nq rows each).  CTA (j * heads + h, y) stages the image's K/V of head h once and serves rows
-// [y * rows_per_cta, (y + 1) * rows_per_cta) of the image, grid.y covering the image with the most rows.  Apart from
-// that row mapping this is dec_cross_attn3_kernel line for line (kept separate so that the existing kernel's code is
-// untouched), so every row is computed as there and its bits do not depend on how many candidates share its image.
+// One query row against the staged keys (qv: lane j holds q_j): sc[r] = exp(s - max) of key r * 32 + lane (0 for keys
+// >= T), in a fixed fmaf order over the 16 bf16x2 words; returns the xor-shuffle sum of the exponentials.
+template <int NR>
+__device__ __forceinline__ float cross_row_exp(const uint32_t* sK, float qv, int T, int lane, float (&sc)[NR]) {
+#pragma unroll
+  for (int r = 0; r < NR; ++r) sc[r] = 0.f;
+#pragma unroll
+  for (int w = 0; w < 16; ++w) {
+    const float qa = __shfl_sync(0xffffffffu, qv, 2 * w), qb = __shfl_sync(0xffffffffu, qv, 2 * w + 1);
+#pragma unroll
+    for (int r = 0; r < NR; ++r) {
+      const uint32_t kw = sK[(r * 32 + lane) * 17 + w];
+      sc[r] = fmaf(qb, __uint_as_float(kw & 0xffff0000u), fmaf(qa, __uint_as_float(kw << 16), sc[r]));
+    }
+  }
+  float mx = -INFINITY;
+#pragma unroll
+  for (int r = 0; r < NR; ++r) {
+    if (r * 32 + lane >= T) sc[r] = -INFINITY;
+    mx = fmaxf(mx, sc[r]);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  float sum = 0.f;
+#pragma unroll
+  for (int r = 0; r < NR; ++r) {
+    sc[r] = expf(sc[r] - mx);
+    sum += sc[r];
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  return sum;
+}
+
+// out[0, 32) = bf16(sum_k sc_k v_k / sum) of one row.  P.V with 16-byte smem reads: lane = (key group kg = lane>>2,
+// 8-channel chunk cc = lane&3); 4*NR iterations cover the keys; the 8 key groups are then summed with xor-shuffles and
+// lanes 0..3 hold the 32 output channels.
+template <int NR>
+__device__ __forceinline__ void cross_row_pv(const __nv_bfloat16* sV, const float (&sc)[NR], float sum, int lane,
+                                             __nv_bfloat16* __restrict__ out) {
+  const int kg = lane >> 2, cc = lane & 3;
+  float o[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) o[j] = 0.f;
+#pragma unroll
+  for (int it = 0; it < 4 * NR; ++it) {              // key = it*8 + kg -> register sc[it>>2], source lane (it&3)*8 + kg
+    const int key = it * 8 + kg;
+    const uint4 vvv = *reinterpret_cast<const uint4*>(sV + key * 32 + cc * 8);
+    const float pk = __shfl_sync(0xffffffffu, sc[it >> 2], (it & 3) * 8 + kg);
+    const __nv_bfloat162* p2 = reinterpret_cast<const __nv_bfloat162*>(&vvv);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float2 f = __bfloat1622float2(p2[e]);
+      o[e * 2] = fmaf(pk, f.x, o[e * 2]);
+      o[e * 2 + 1] = fmaf(pk, f.y, o[e * 2 + 1]);
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    o[j] += __shfl_xor_sync(0xffffffffu, o[j], 4);
+    o[j] += __shfl_xor_sync(0xffffffffu, o[j], 8);
+    o[j] += __shfl_xor_sync(0xffffffffu, o[j], 16);
+  }
+  if (kg == 0) {
+    const float inv = 1.0f / sum;
+    uint4 q4;
+    q4.x = pack_bf16(o[0] * inv, o[1] * inv); q4.y = pack_bf16(o[2] * inv, o[3] * inv);
+    q4.z = pack_bf16(o[4] * inv, o[5] * inv); q4.w = pack_bf16(o[6] * inv, o[7] * inv);
+    *reinterpret_cast<uint4*>(out + cc * 8) = q4;
+  }
+}
+
+// One CTA per (image, head), 4 warps.  The head's K and V tiles are staged once in shared memory, so the per-image K/V
+// cache is read once per decode pass; the query rows are distributed over the warps and each row is handled entirely
+// inside one warp (scores for NR keys per lane, shuffle softmax, P.V): no block-level synchronisation after the load.
+// q fp32 [rows, D] pre-scaled by 1/sqrt(32); out bf16 [rows, D]; the rows of this launch belong to images b_first,
+// b_first + 1, ...
+// GROUPED (candidate scoring): the query rows of image b_first + j are rows [cand_off[j] * nq, cand_off[j + 1] * nq)
+// (candidates are image-major, nq rows each); CTA (j * heads + h, y) serves rows [y * rows_per_cta, (y + 1) *
+// rows_per_cta) of the image, grid.y covering the image with the most rows.  Otherwise image j's rows are
+// [j * nq, (j + 1) * nq).  Every row is computed the same way in both, so its bits do not depend on how many candidates
+// share its image.
+template <int NR, bool GROUPED>
+__device__ __forceinline__ void dec_cross_attn3_body(const float* __restrict__ q, const __nv_bfloat16* __restrict__ kv,
+                                                     long long kv_rows, int b_first, int T, int D, int heads, int nq,
+                                                     const int* __restrict__ cand_off, int rows_per_cta,
+                                                     __nv_bfloat16* __restrict__ out) {
+  constexpr int TK = 32 * NR;
+  __shared__ uint32_t sK[TK * 17];
+  __shared__ __align__(16) __nv_bfloat16 sV[TK * 32];
+  grid_dep_launch();
+  grid_dep_wait();
+  const int b = blockIdx.x / heads, h = blockIdx.x % heads;
+  long long row0 = static_cast<long long>(b) * nq;
+  int q_begin = 0, q_end = nq;
+  if (GROUPED) {
+    row0 = static_cast<long long>(cand_off[b]) * nq;
+    const int rows = (cand_off[b + 1] - cand_off[b]) * nq;
+    q_begin = static_cast<int>(blockIdx.y) * rows_per_cta;
+    if (q_begin >= rows) return;
+    q_end = q_begin + rows_per_cta < rows ? q_begin + rows_per_cta : rows;
+  }
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  cross_stage_kv<NR, 128, true>(sK, sV, kv, kv_rows, static_cast<long long>(b_first + b) * T, T, D, h, tid);
+  __syncthreads();
+  for (int qi = q_begin + warp; qi < q_end; qi += 4) {
+    const long long row = row0 + qi;
+    float sc[NR];
+    const float sum = cross_row_exp<NR>(sK, q[row * D + h * 32 + lane], T, lane, sc);
+    cross_row_pv<NR>(sV, sc, sum, lane, out + row * D + h * 32);
+  }
+}
+
+template <int NR>   // keys per lane: T <= 32 * NR (NR = 4: T <= 128, NR = 8: T <= 256)
+__global__ void __launch_bounds__(128) dec_cross_attn3_kernel(const float* __restrict__ q,
+                                                              const __nv_bfloat16* __restrict__ kv, long long kv_rows,
+                                                              int b_first, int T, int D, int heads, int nq,
+                                                              __nv_bfloat16* __restrict__ out) {
+  dec_cross_attn3_body<NR, false>(q, kv, kv_rows, b_first, T, D, heads, nq, nullptr, 0, out);
+}
+
 template <int NR>
 __global__ void __launch_bounds__(128) dec_cross_attn3_grouped_kernel(const float* __restrict__ q,
                                                                       const __nv_bfloat16* __restrict__ kv, long long kv_rows,
                                                                       int b_first, int T, int D, int heads, int nq,
                                                                       const int* __restrict__ cand_off, int rows_per_cta,
                                                                       __nv_bfloat16* __restrict__ out) {
-  constexpr int TK = 32 * NR;
-  __shared__ uint32_t sK[TK * 17];                        // bf16x2 words, pitch 17 (odd)
-  __shared__ __align__(16) __nv_bfloat16 sV[TK * 32];
-  grid_dep_launch();
-  grid_dep_wait();
-  const int b = blockIdx.x / heads, h = blockIdx.x % heads;
-  const long long row0 = static_cast<long long>(cand_off[b]) * nq;
-  const int rows = (cand_off[b + 1] - cand_off[b]) * nq;
-  const int q_begin = static_cast<int>(blockIdx.y) * rows_per_cta;
-  if (q_begin >= rows) return;
-  const int q_end = q_begin + rows_per_cta < rows ? q_begin + rows_per_cta : rows;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const long long row_b = static_cast<long long>(b_first + b) * T;
-  for (int t = tid; t < TK; t += 128) {
-    uint4* vd = reinterpret_cast<uint4*>(sV + t * 32);
-    if (t < T) {
-      const uint4* kr = reinterpret_cast<const uint4*>(kv + blocked_off(kv_rows, row_b + t, h * 32));
-      const uint4* vr = reinterpret_cast<const uint4*>(kv + blocked_off(kv_rows, row_b + t, D + h * 32));
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const uint4 u = __ldg(kr + j);
-        sK[t * 17 + j * 4 + 0] = u.x; sK[t * 17 + j * 4 + 1] = u.y;
-        sK[t * 17 + j * 4 + 2] = u.z; sK[t * 17 + j * 4 + 3] = u.w;
-        vd[j] = __ldg(vr + j);
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 16; ++j) sK[t * 17 + j] = 0u;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) vd[j] = make_uint4(0u, 0u, 0u, 0u);
-    }
-  }
-  __syncthreads();
-  for (int qi = q_begin + warp; qi < q_end; qi += 4) {
-    const long long row = row0 + qi;
-    const float qv = q[row * D + h * 32 + lane];          // lane j holds q_j
-    float sc[NR];
-#pragma unroll
-    for (int r = 0; r < NR; ++r) sc[r] = 0.f;
-#pragma unroll
-    for (int w = 0; w < 16; ++w) {
-      const float qa = __shfl_sync(0xffffffffu, qv, 2 * w), qb = __shfl_sync(0xffffffffu, qv, 2 * w + 1);
-#pragma unroll
-      for (int r = 0; r < NR; ++r) {
-        const uint32_t kw = sK[(r * 32 + lane) * 17 + w];
-        sc[r] = fmaf(qb, __uint_as_float(kw & 0xffff0000u), fmaf(qa, __uint_as_float(kw << 16), sc[r]));
-      }
-    }
-    float mx = -INFINITY;
-#pragma unroll
-    for (int r = 0; r < NR; ++r) {
-      if (r * 32 + lane >= T) sc[r] = -INFINITY;
-      mx = fmaxf(mx, sc[r]);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    float sum = 0.f;
-#pragma unroll
-    for (int r = 0; r < NR; ++r) {
-      sc[r] = expf(sc[r] - mx);
-      sum += sc[r];
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    // P.V with 16-byte smem reads: lane = (key group kg = lane>>2, 8-channel chunk cc = lane&3); 4*NR iterations cover
-    // the keys; the 8 key groups are then summed with xor-shuffles and lanes 0..3 hold the 32 output channels.
-    const int kg = lane >> 2, cc = lane & 3;
-    float o[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) o[j] = 0.f;
-#pragma unroll
-    for (int it = 0; it < 4 * NR; ++it) {              // key = it*8 + kg -> register sc[it>>2], source lane (it&3)*8 + kg
-      const int key = it * 8 + kg;
-      const uint4 vvv = *reinterpret_cast<const uint4*>(sV + key * 32 + cc * 8);
-      const float pk = __shfl_sync(0xffffffffu, sc[it >> 2], (it & 3) * 8 + kg);
-      const __nv_bfloat162* p2 = reinterpret_cast<const __nv_bfloat162*>(&vvv);
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float2 f = __bfloat1622float2(p2[e]);
-        o[e * 2] = fmaf(pk, f.x, o[e * 2]);
-        o[e * 2 + 1] = fmaf(pk, f.y, o[e * 2 + 1]);
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      o[j] += __shfl_xor_sync(0xffffffffu, o[j], 4);
-      o[j] += __shfl_xor_sync(0xffffffffu, o[j], 8);
-      o[j] += __shfl_xor_sync(0xffffffffu, o[j], 16);
-    }
-    if (kg == 0) {
-      const float inv = 1.0f / sum;
-      uint4 q4;
-      q4.x = pack_bf16(o[0] * inv, o[1] * inv); q4.y = pack_bf16(o[2] * inv, o[3] * inv);
-      q4.z = pack_bf16(o[4] * inv, o[5] * inv); q4.w = pack_bf16(o[6] * inv, o[7] * inv);
-      *reinterpret_cast<uint4*>(out + row * D + h * 32 + cc * 8) = q4;
-    }
-  }
+  dec_cross_attn3_body<NR, true>(q, kv, kv_rows, b_first, T, D, heads, nq, cand_off, rows_per_cta, out);
 }
 
 // ---------------------------------------------------------------------------------------------
 // Cross-attention maps (parseq_forward_args.attn_maps): maps[row, t] = (1 / heads) * sum_h softmax_t(q_h . k_h,t) of
 // the query rows of one decoder pass, the head-averaged weights nn.MultiheadAttention returns.  One CTA of 8 warps per
-// (image, block of AMAP_ROWS query rows); the heads are visited in order, each head's K staged as dec_cross_attn3_kernel
-// stages it, and the probabilities are computed with that kernel's arithmetic (the fmaf order over the 16 bf16x2 words,
-// expf(s - max), the xor-shuffle sum): the exponentials and their sum are bitwise those of its P.V, which scales
-// sum(e * v) by 1 / sum where this kernel stores p = e * (1 / sum) per key.
+// (image, block of AMAP_ROWS query rows); the heads are visited in order, each head's K staged and each row's
+// exponentials and their sum computed by the pieces dec_cross_attn3_kernel uses (cross_stage_kv, cross_row_exp): they are
+// bitwise those of its P.V, which scales sum(e * v) by 1 / sum where this kernel stores p = e * (1 / sum) per key.
 // Each warp keeps its AMAP_ROWS / 8 rows' running sums in registers; the heads are summed in fixed order, so the maps
 // are bitwise reproducible and independent of the batch.  q fp32 [B*nq, D] pre-scaled; maps fp32 [B*nq, T].
 constexpr int AMAP_ROWS = 32;
@@ -918,7 +864,7 @@ __global__ void __launch_bounds__(AMAP_THREADS, 1) dec_cross_attn_maps_kernel(co
                                                                          long long kv_rows, int b_first, int T, int D,
                                                                          int heads, int nq, float* __restrict__ maps) {
   constexpr int TK = 32 * NR, WARPS = AMAP_THREADS / 32, RPW = AMAP_ROWS / WARPS;
-  __shared__ uint32_t sK[TK * 17];                        // bf16x2 words, pitch 17 (odd)
+  __shared__ uint32_t sK[TK * 17];
   grid_dep_launch();
   grid_dep_wait();
   const int b = blockIdx.x, q_begin = static_cast<int>(blockIdx.y) * AMAP_ROWS;
@@ -931,55 +877,15 @@ __global__ void __launch_bounds__(AMAP_THREADS, 1) dec_cross_attn_maps_kernel(co
     for (int r = 0; r < NR; ++r) acc[j][r] = 0.f;
   for (int h = 0; h < heads; ++h) {
     if (h > 0) __syncthreads();                          // every warp is done with the previous head's K
-    for (int t = tid; t < TK; t += AMAP_THREADS) {
-      if (t < T) {
-        const uint4* kr = reinterpret_cast<const uint4*>(kv + blocked_off(kv_rows, row_b + t, h * 32));
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const uint4 u = __ldg(kr + j);
-          sK[t * 17 + j * 4 + 0] = u.x; sK[t * 17 + j * 4 + 1] = u.y;
-          sK[t * 17 + j * 4 + 2] = u.z; sK[t * 17 + j * 4 + 3] = u.w;
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) sK[t * 17 + j] = 0u;
-      }
-    }
+    cross_stage_kv<NR, AMAP_THREADS, false>(sK, nullptr, kv, kv_rows, row_b, T, D, h, tid);
     __syncthreads();
 #pragma unroll
     for (int j = 0; j < RPW; ++j) {
       const int qi = q_begin + warp + j * WARPS;
       if (qi >= nq) continue;                            // warp-uniform
       const long long row = static_cast<long long>(b) * nq + qi;
-      const float qv = q[row * D + h * 32 + lane];        // lane j holds q_j
       float sc[NR];
-#pragma unroll
-      for (int r = 0; r < NR; ++r) sc[r] = 0.f;
-#pragma unroll
-      for (int w = 0; w < 16; ++w) {
-        const float qa = __shfl_sync(0xffffffffu, qv, 2 * w), qb = __shfl_sync(0xffffffffu, qv, 2 * w + 1);
-#pragma unroll
-        for (int r = 0; r < NR; ++r) {
-          const uint32_t kw = sK[(r * 32 + lane) * 17 + w];
-          sc[r] = fmaf(qb, __uint_as_float(kw & 0xffff0000u), fmaf(qa, __uint_as_float(kw << 16), sc[r]));
-        }
-      }
-      float mx = -INFINITY;
-#pragma unroll
-      for (int r = 0; r < NR; ++r) {
-        if (r * 32 + lane >= T) sc[r] = -INFINITY;
-        mx = fmaxf(mx, sc[r]);
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-      float sum = 0.f;
-#pragma unroll
-      for (int r = 0; r < NR; ++r) {
-        sc[r] = expf(sc[r] - mx);
-        sum += sc[r];
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+      const float sum = cross_row_exp<NR>(sK, q[row * D + h * 32 + lane], T, lane, sc);
       const float inv = 1.0f / sum;
 #pragma unroll
       for (int r = 0; r < NR; ++r) acc[j][r] += sc[r] * inv;

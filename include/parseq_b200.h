@@ -361,6 +361,61 @@ int parseq_enc_attention(const void* qkv_bf16, int B, int T, int D, int heads, v
  * returns PARSEQ_ERR_UNSUPPORTED. */
 int parseq_qkv_attention_bf16(const void* xn_bf16, const void* W_qkv, const float* b_qkv, int B, int T, int D,
                               int heads, void* out_bf16, parseq_stream_t stream);
+/* The head GEMM of parseq_score with its log-sum-exp epilogue: the logits v = A[M,K] * W[N,K]^T + bias (bias may be NULL)
+ * never reach memory.  part: fp32 [M][ceil(N / 128)][2], per row and 128-column tile (max, sum of exp(v - max)) over the
+ * tile's columns < N (a tile whose max is -inf sums exp(v)); tlogit[r] = v[r][tgt[r]] for tgt[r] in 0..N-1 (tgt and
+ * tlogit both NULL: partials only).  Rows >= M are not written. */
+int parseq_head_lse_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, const float* bias, int M, int N, int K,
+                         const int32_t* tgt, float* part, float* tlogit, parseq_stream_t stream);
+/* The head GEMM of parseq_beam_search above 128 classes with its top-K epilogue: part as parseq_head_lse_bf16 over the
+ * allowed classes (a masked class counts as -inf), and keys: uint64 [M][ceil(N / 128)][16], the tile's k best allowed
+ * classes in the beam order (see parseq_beam_select), 0 after the last; -inf logits are never listed.  1 <= k <= 16.
+ * mask: allowlist words (parseq_forward_args.class_mask), row r reads row r / mask_div (mask_div >= 1), or NULL. */
+int parseq_head_topk_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, const float* bias, int M, int N, int K,
+                          int k, const uint32_t* mask, int mask_div, float* part, uint64_t* keys, parseq_stream_t stream);
+/* One step of parseq_beam_search's selection for `batch` images (one launch of the selection kernel).  An image's state
+ * has one row r = b * beam_width + k per slot: ids [rows][ids_ld] (BOS, c_1.., then anything), score, len (characters, -1
+ * empty) and st (0 active, 1 finished, 2 empty).  The logits row of slot (b, k) is row0 + b * img_stride + k *
+ * slot_stride; it is read from `logits` [rows][num_classes], or, when keys != NULL and there is no lexicon, from the
+ * partials and keys of parseq_head_topk_bf16 (part [rows][ntiles][2], keys [rows][ntiles][16], k = beam_width).  A key
+ * orders a row's classes: NaN logits first, then the logit descending, ties to the lower class, -0 as +0.  The new
+ * state goes to the *_out arrays, parent[r] = the state row slot r came from; at the last step (step + 1 == num_steps)
+ * also out_ids [rows][num_steps], out_len [rows] and out_score [rows] as parseq_beam_search returns them.  With
+ * first_edge != NULL the step walks a lexicon DAG (parseq_lexicon_desc arrays on the device; roots [batch] or NULL for
+ * node 0, read at step 0; node_in read at step > 0; node_out written).  All pointers DEVICE.  Checked on the host
+ * (PARSEQ_ERR_INVALID_ARG, nothing launched): 1 <= beam_width <= 16, ntiles == ceil(num_classes / 128), 0 <= step <
+ * num_steps, ids_ld > num_steps, and logits present without keys or with a lexicon. */
+typedef struct parseq_beam_select_args {
+  const float* logits;                   /* [rows][num_classes] or NULL */
+  const float* part;                     /* [rows][ntiles][2] or NULL */
+  const uint64_t* keys;                  /* [rows][ntiles][16] or NULL */
+  int32_t ntiles;
+  int64_t row0, img_stride, slot_stride;
+  int32_t batch, num_classes, beam_width, step, num_steps;
+  const uint32_t* class_mask;            /* [batch][mask_ld] or NULL */
+  int32_t mask_ld;
+  const int32_t* ids_in;
+  const float* score_in;
+  const int32_t* len_in;
+  const int32_t* st_in;
+  int32_t* ids_out;
+  float* score_out;
+  int32_t* len_out;
+  int32_t* st_out;
+  int32_t* parent;
+  int32_t ids_ld;
+  int32_t* out_ids;
+  int32_t* out_len;
+  float* out_score;
+  const int32_t* first_edge;             /* lexicon, or NULL */
+  const int32_t* edge_class;
+  const int32_t* edge_child;
+  const uint8_t* terminal;
+  const int32_t* roots;
+  const int32_t* node_in;
+  int32_t* node_out;
+} parseq_beam_select_args;
+int parseq_beam_select(const parseq_beam_select_args* a, parseq_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -3215,5 +3215,56 @@ int parseq_qkv_attention_bf16(const void* xn_bf16, const void* W_qkv, const floa
   PQ_TRY(ensure_kernel_attributes());
   return qkv_attn_launch(g_default_opts, xn_bf16, W_qkv, b_qkv, B, T, D, heads, out_bf16, reinterpret_cast<cudaStream_t>(stream));
 }
+int parseq_head_lse_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, const float* bias, int M, int N, int K,
+                         const int32_t* tgt, float* part, float* tlogit, parseq_stream_t stream) {
+  if (part == nullptr || (tgt == nullptr) != (tlogit == nullptr))
+    return fail(PARSEQ_ERR_INVALID_ARG, "head_lse: part is required, tgt and tlogit go together");
+  PQ_TRY(ensure_kernel_attributes());
+  return gemm_lse_launch(g_default_opts, A, lda, W, ldw, bias, M, N, K, tgt, reinterpret_cast<float2*>(part), tlogit,
+                         reinterpret_cast<cudaStream_t>(stream));
+}
+int parseq_head_topk_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, const float* bias, int M, int N, int K,
+                          int k, const uint32_t* mask, int mask_div, float* part, uint64_t* keys, parseq_stream_t stream) {
+  if (k < 1 || k > pq::BEAM_TOPK_LD) return fail(PARSEQ_ERR_INVALID_ARG, "head_topk: k must be in 1..16");
+  if (part == nullptr || keys == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "head_topk: part and keys are required");
+  if (mask != nullptr && mask_div < 1) return fail(PARSEQ_ERR_INVALID_ARG, "head_topk: mask_div must be >= 1");
+  PQ_TRY(ensure_kernel_attributes());
+  return gemm_topk_launch(g_default_opts, A, lda, W, ldw, bias, M, N, K, k, mask, mask != nullptr ? mask_div : 1,
+                          reinterpret_cast<float2*>(part), reinterpret_cast<unsigned long long*>(keys),
+                          reinterpret_cast<cudaStream_t>(stream));
+}
+int parseq_beam_select(const parseq_beam_select_args* a, parseq_stream_t stream) {
+  if (a == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "beam_select: null arguments");
+  const int C = a->num_classes, K = a->beam_width;
+  const bool lex = a->first_edge != nullptr;
+  if (a->batch < 1 || C < 1) return fail(PARSEQ_ERR_INVALID_ARG, "beam_select: batch and num_classes must be >= 1");
+  if (K < 1 || K > pq::BEAM_MAX) return fail(PARSEQ_ERR_INVALID_ARG, "beam_select: beam_width must be in 1..16");
+  if (a->ntiles != (C + pq::GEMM_BLOCK_N - 1) / pq::GEMM_BLOCK_N)
+    return fail(PARSEQ_ERR_INVALID_ARG, "beam_select: ntiles must be ceil(num_classes / 128)");
+  if (a->step < 0 || a->step >= a->num_steps) return fail(PARSEQ_ERR_INVALID_ARG, "beam_select: need 0 <= step < num_steps");
+  if (a->ids_ld <= a->num_steps) return fail(PARSEQ_ERR_INVALID_ARG, "beam_select: ids_ld must exceed num_steps");
+  if (a->logits == nullptr && (a->keys == nullptr || lex))
+    return fail(PARSEQ_ERR_INVALID_ARG, "beam_select: logits are required without keys and with a lexicon");
+  if (a->keys != nullptr && a->part == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "beam_select: keys need part");
+  if (a->class_mask != nullptr && a->mask_ld < (C + 31) / 32)
+    return fail(PARSEQ_ERR_INVALID_ARG, "beam_select: mask_ld must be >= ceil(num_classes / 32)");
+  if (a->ids_in == nullptr || a->score_in == nullptr || a->len_in == nullptr || a->st_in == nullptr || a->ids_out == nullptr ||
+      a->score_out == nullptr || a->len_out == nullptr || a->st_out == nullptr || a->parent == nullptr ||
+      (a->step + 1 == a->num_steps && (a->out_ids == nullptr || a->out_len == nullptr || a->out_score == nullptr)))
+    return fail(PARSEQ_ERR_INVALID_ARG, "beam_select: missing state or output array");
+  if (lex && (a->edge_class == nullptr || a->edge_child == nullptr || a->terminal == nullptr || a->node_out == nullptr ||
+              (a->step > 0 && a->node_in == nullptr)))
+    return fail(PARSEQ_ERR_INVALID_ARG, "beam_select: incomplete lexicon");
+  PQ_TRY(ensure_kernel_attributes());
+  pq::BeamLex bl{};
+  if (lex) bl = pq::BeamLex{a->first_edge, a->edge_class, a->edge_child, a->terminal, a->roots, a->node_in, a->node_out};
+  return launch_k(g_default_opts, lex ? pq::beam_select_kernel<true> : pq::beam_select_kernel<false>,
+                  dim3(static_cast<unsigned>(a->batch)), dim3(pq::BEAM_THREADS), 0, reinterpret_cast<cudaStream_t>(stream),
+                  a->logits, reinterpret_cast<const float2*>(a->part),
+                  reinterpret_cast<const unsigned long long*>(lex ? nullptr : a->keys), a->ntiles, static_cast<long long>(a->row0),
+                  static_cast<long long>(a->img_stride), static_cast<long long>(a->slot_stride), C, K, a->step, a->num_steps,
+                  a->class_mask, a->mask_ld, a->ids_in, a->score_in, a->len_in, a->st_in, a->ids_out, a->score_out, a->len_out,
+                  a->st_out, a->parent, a->ids_ld, a->out_ids, a->out_len, a->out_score, bl);
+}
 
 }  // extern "C"

@@ -43,6 +43,19 @@ class LexiconDescC(C.Structure):
                 ("edge_child", C.c_void_p), ("terminal", C.c_void_p)]
 
 
+class BeamSelectArgsC(C.Structure):
+    _fields_ = [("logits", C.c_void_p), ("part", C.c_void_p), ("keys", C.c_void_p), ("ntiles", C.c_int32),
+                ("row0", C.c_int64), ("img_stride", C.c_int64), ("slot_stride", C.c_int64),
+                ("batch", C.c_int32), ("num_classes", C.c_int32), ("beam_width", C.c_int32), ("step", C.c_int32),
+                ("num_steps", C.c_int32), ("class_mask", C.c_void_p), ("mask_ld", C.c_int32),
+                ("ids_in", C.c_void_p), ("score_in", C.c_void_p), ("len_in", C.c_void_p), ("st_in", C.c_void_p),
+                ("ids_out", C.c_void_p), ("score_out", C.c_void_p), ("len_out", C.c_void_p), ("st_out", C.c_void_p),
+                ("parent", C.c_void_p), ("ids_ld", C.c_int32), ("out_ids", C.c_void_p), ("out_len", C.c_void_p),
+                ("out_score", C.c_void_p), ("first_edge", C.c_void_p), ("edge_class", C.c_void_p),
+                ("edge_child", C.c_void_p), ("terminal", C.c_void_p), ("roots", C.c_void_p), ("node_in", C.c_void_p),
+                ("node_out", C.c_void_p)]
+
+
 def lexicon_desc(first_edge, edge_class, edge_child, terminal) -> LexiconDescC:
     """parseq_lexicon_desc over contiguous numpy arrays (int32, int32, int32, uint8); the caller keeps them alive."""
     return LexiconDescC(int(terminal.shape[0]), int(edge_class.shape[0]), first_edge.ctypes.data, edge_class.ctypes.data,
@@ -73,7 +86,8 @@ EXPORTS = [
     "parseq_beam_search_lexicon_u8",
     "parseq_postprocess", "parseq_encode", "parseq_decode", "parseq_decode_ex", "parseq_head", "parseq_text_embed", "parseq_kernel_launches", "parseq_debug_int", "parseq_bench_tma_stream",
     "parseq_set_option", "parseq_get_timing", "parseq_get_ar_profile", "parseq_last_error", "parseq_version", "parseq_gemm_bf16", "parseq_gemm_ln_bf16", "parseq_mlp_ln_bf16", "parseq_layernorm_bf16",
-    "parseq_enc_attention", "parseq_qkv_attention_bf16",
+    "parseq_enc_attention", "parseq_qkv_attention_bf16", "parseq_head_lse_bf16", "parseq_head_topk_bf16",
+    "parseq_beam_select",
 ]
 
 
@@ -147,6 +161,11 @@ def load_library(path: Optional[str] = None):
     lib.parseq_enc_attention.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     lib.parseq_qkv_attention_bf16.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                               C.c_void_p, C.c_void_p]
+    lib.parseq_head_lse_bf16.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.parseq_head_topk_bf16.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                          C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.parseq_beam_select.argtypes = [C.POINTER(BeamSelectArgsC), C.c_void_p]
     if path is None:
         _lib = lib
     return lib

@@ -73,9 +73,10 @@ def budget_stats(got: torch.Tensor, ref: torch.Tensor) -> Dict[str, float]:
             "p99": d.kthvalue(max(1, math.ceil(0.99 * n))).values.item() / sigma, "max": d.max().item() / sigma}
 
 
-def excess(stats: Dict[str, float], key: Tuple[int, int]) -> Dict[str, float]:
-    """stat / bound for every bounded statistic of BOUNDS[(embed_dim, dec_depth)]: <= 1 inside the budget."""
-    return {k: stats[k] / b for k, b in BOUNDS[key].items()}
+def excess(stats: Dict[str, float], key: Tuple[int, int], bounds=None) -> Dict[str, float]:
+    """stat / bound for every bounded statistic of BOUNDS[(embed_dim, dec_depth)] (or of bounds[key], another module's
+    table): <= 1 inside the budget."""
+    return {k: stats[k] / b for k, b in (BOUNDS if bounds is None else bounds)[key].items()}
 
 
 def format_stats(name: str, s: Dict[str, float]) -> str:

@@ -33,6 +33,7 @@ SHAPES = [
     (128, 128, 64), (128, 128, 384), (256, 384, 384), (1024, 1152, 384), (512, 1536, 384), (384, 384, 1536),
     (1, 384, 384), (26, 384, 384), (52, 1536, 384), (300, 95, 384), (2522, 768, 384), (640, 384, 96),
     (130, 576, 192), (129, 192, 768), (20000, 384, 384), (4096, 768, 384),
+    (700, 1536, 384), (8192, 1152, 384), (1000, 384, 1536), (130, 95, 384),
 ]
 
 
@@ -46,26 +47,6 @@ def test_gemm_f32_bias(lib, M, N, K):
     out = _gemm(lib, A, W, bias, 0)
     err = (out - ref).abs().max().item()
     assert err <= 2e-4 * max(1.0, ref.abs().max().item()), err
-
-
-@pytest.mark.parametrize("cta_group,block_n", [(1, 64), (1, 128), (1, 256), (2, 128), (2, 192), (2, 256)])
-@pytest.mark.parametrize("M,N,K", [(700, 1536, 384), (8192, 1152, 384), (1000, 384, 1536), (130, 95, 384)])
-def test_gemm_tile_variants(lib, cta_group, block_n, M, N, K):
-    """Single-CTA tiles and CTA-pair tiles (a cluster of two on 256 rows, W tile multicast) of every width, ragged M / N."""
-    from parseq_b200.engine import check
-    check(lib, lib.parseq_set_option(None, b"block_n", block_n))
-    check(lib, lib.parseq_set_option(None, b"cta_group", cta_group))
-    try:
-        g = torch.Generator(device="cuda").manual_seed(block_n + M)
-        A = torch.randn((M, K), device="cuda", generator=g).bfloat16()
-        W = (torch.randn((N, K), device="cuda", generator=g) * 0.05).bfloat16()
-        bias = torch.randn((N,), device="cuda", generator=g)
-        ref = A.float() @ W.float().t() + bias
-        out = _gemm(lib, A, W, bias, 0)
-        assert (out - ref).abs().max().item() <= 2e-4 * ref.abs().max().item()
-    finally:
-        check(lib, lib.parseq_set_option(None, b"block_n", 0))
-        check(lib, lib.parseq_set_option(None, b"cta_group", 0))
 
 
 @pytest.mark.parametrize("N,K,mode", [(1152, 384, 1), (384, 384, 0), (1536, 384, 2), (384, 1536, 0)])

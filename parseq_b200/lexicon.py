@@ -80,6 +80,8 @@ class Lexicon:
     def __init__(self, tokenizer: Tokenizer, candidates, max_label_length: int, num_classes: int):
         shared, rows = lexicon_rows(candidates)
         check_words(tokenizer, {s for r in rows for s in r}, max_label_length, num_classes)
+        # what the trie's class ids mean and how long a word may be: beam_search refuses a model that differs
+        self.charset = "".join(tokenizer._itos[1:tokenizer.bos_id])
         self.num_classes = num_classes
         self.max_label_length = max_label_length
         distinct: Dict[frozenset, int] = {}

@@ -258,8 +258,24 @@ def unrotate_boxes(boxes: Tensor, crop_hw: Sequence[int], img_size: Sequence[int
     return torch.cat([torch.minimum(a, b), torch.maximum(a, b)], dim=-1)
 
 
+def _weights_changed(module: nn.Module, *_):
+    """Makes the _EngineModule that owns `module` (module.__dict__["_owner"], a weak reference) walk its parameters
+    again and upload them on its next engine call.  Runs when a parameter is registered or replaced (which also covers
+    load_state_dict(assign=True)) and after every load_state_dict (a load_state_dict post hook): an in-place reload of
+    inference tensors changes no version counter and no parameter identity, so the signature alone cannot see it."""
+    ref = module.__dict__.get("_owner")
+    owner = ref() if ref is not None else None
+    if owner is not None:
+        owner.__dict__.pop("_plist", None)
+        owner.__dict__["_engine_sig"] = None
+
+
 class _Holder(nn.Module):
     """Parameter container; nested so that state_dict keys equal the reference's."""
+
+    def register_parameter(self, name: str, param: Optional[nn.Parameter]) -> None:
+        super().register_parameter(name, param)
+        _weights_changed(self)
 
 
 class _HeadModule(_Holder):
@@ -319,19 +335,26 @@ class _EngineModule(nn.Module):
         import weakref
         for name, cls in (("head", _HeadModule), ("text_embed", _TextEmbedModule)):
             if hasattr(self, name):
-                mod = getattr(self, name)
-                mod.__class__ = cls
-                mod.__dict__["_owner"] = weakref.ref(self)
+                getattr(self, name).__class__ = cls
+        # every module of the tree reports parameter replacements and reloads to this one (_weights_changed)
+        for mod in self.modules():
+            mod.__dict__["_owner"] = weakref.ref(self)
+            mod.register_load_state_dict_post_hook(_weights_changed)
 
     # ---- engine plumbing -------------------------------------------------------------------
     @property
     def _device(self) -> torch.device:
         return next(self.parameters()).device
 
+    def register_parameter(self, name: str, param: Optional[nn.Parameter]) -> None:
+        super().register_parameter(name, param)
+        _weights_changed(self)
+
     def _signature(self):
-        """Cheap staleness check of the engine's weight copy: version counters of every parameter (in-place updates,
-        load_state_dict) + the storage addresses of the first / last one (`.to()` moves).  The parameter list is cached:
-        walking the module tree costs more than a bs=1 forward's launch overhead."""
+        """Cheap staleness check of the engine's weight copy: version counters of every parameter (in-place updates)
+        + the storage addresses of the first / last one (`.to()` moves).  The parameter list is cached: walking the
+        module tree costs more than a bs=1 forward's launch overhead.  Replaced parameters and load_state_dict reach
+        the engine through _weights_changed, which drops the cached list and the signature."""
         pl = self.__dict__.get("_plist")
         if pl is None:
             pl = list(self.parameters())
@@ -349,6 +372,12 @@ class _EngineModule(nn.Module):
         return out
 
     def engine(self) -> Engine:
+        """The engine handle, with the current weights uploaded.  The next call after any of these computes with the
+        new weights: load_state_dict in any form (strict or not, assign=True, inside or outside inference mode, on
+        inference-tensor parameters), replacing a parameter, an in-place update of ordinary parameters (an optimizer
+        step), and `.to()`.  Otherwise nothing is uploaded.  One change cannot be seen without reading the weights: an
+        in-place write into a parameter that is an inference tensor (built or loaded under torch.inference_mode),
+        made outside load_state_dict.  After such a write, call load_state_dict again."""
         dev = self._device
         if dev.type != "cuda":
             raise RuntimeError("parseq_b200 runs on a CUDA (sm_90a, H100) device only; move the model with .to('cuda') "
@@ -367,9 +396,9 @@ class _EngineModule(nn.Module):
 
     def set_engine_option(self, name: str, value: int):
         """Engine tuning knobs: "max_batch", "chunk", "use_graph" (see include/parseq_b200.h)."""
-        self._options[name] = int(value)
         if self._engine is not None:
             self._engine.set_option(name, value)
+        self._options[name] = int(value)          # a refused option is not replayed on a later handle
 
     def _check_images(self, images: Tensor) -> Tensor:
         if images.device.type != "cuda":
@@ -452,6 +481,15 @@ class _EngineModule(nn.Module):
             raise ValueError("roots need a lexicon")
         if max_length is not None and int(max_length) < 0:
             raise ValueError(f"max_length must be None or >= 0, got {max_length}")
+        if lexicon is not None:
+            # the trie holds class ids of one charset (which fixes the class count), its words at most one
+            # max_label_length long
+            if lexicon.charset != self.cfg.charset_train:
+                raise ValueError(f"lexicon was compiled for another charset_train ({lexicon.num_classes} classes) than "
+                                 f"the model's ({self.cfg.num_classes} classes)")
+            if lexicon.max_label_length != self.cfg.max_label_length:
+                raise ValueError(f"lexicon was compiled for max_label_length = {lexicon.max_label_length}, the model "
+                                 f"has {self.cfg.max_label_length}")
         eng = self.engine()
         if isinstance(images, (list, tuple)):
             images = self.preprocess(images, rotation)
@@ -469,9 +507,6 @@ class _EngineModule(nn.Module):
         scores = torch.empty((N, K), dtype=torch.float32, device=dev)
         lex = None
         if lexicon is not None:
-            if lexicon.num_classes != self.cfg.num_classes:
-                raise ValueError(f"lexicon was compiled for {lexicon.num_classes} classes, the model has "
-                                 f"{self.cfg.num_classes}")
             lex = lexicon.handle(eng)
             if roots is not None:
                 roots = roots.to(device="cpu", dtype=torch.int32).contiguous()

@@ -297,7 +297,9 @@ int parseq_bench_tma_stream(void* buf, int64_t bytes, int cluster, int ctas, int
  * "ar_last_ids_pitch"; "ar_last_path": the AR loop of the last PARSeq forward, 0 the chain of separate kernels, 1 the
  * grid-barrier kernel, 2 the cluster kernel, -1 no AR loop; "ln_clusters": the clusters the persistent GEMM + LayerNorm
  * kernel runs on, 0 before its first launch, also with e = NULL for the bare kernel exports; "beam_bytes": device bytes of
- * the beam-search buffers, 0 until the first parseq_beam_search call); -1 if unknown. */
+ * the beam-search buffers, 0 until the first parseq_beam_search call; process-wide, also with e = NULL:
+ * "live_device_bytes" and "live_cuda_objects", the device bytes and the streams, events and graph execs that every live
+ * handle and lexicon holds); -1 if unknown. */
 int64_t parseq_debug_int(parseq_engine* e, const char* name);
 /* Options: "max_batch" (images per super-chunk = one CUDA graph), "chunk" (images per encoder pass inside a
  * super-chunk), "dec_chunk" (images per decoder chain; the chains of a super-chunk run concurrently on their own

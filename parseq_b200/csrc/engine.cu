@@ -26,6 +26,7 @@
 #include "attn_wgmma.cuh"
 #include "qkv_attn.cuh"
 #include "crops.cuh"
+#include "owners.h"
 
 namespace {
 
@@ -187,13 +188,13 @@ struct LaunchConfig {
 };
 
 template <typename... KArgs, typename... Args>
-int launch_ex(const LaunchConfig& lc, void (*kern)(KArgs...), Args... args) {
+int launch_ex(const LaunchConfig& lc, void (*kern)(KArgs...), const Args&... args) {
   PQ_CUDA(cudaLaunchKernelEx(&lc.cfg, kern, static_cast<KArgs>(args)...));
   return PARSEQ_OK;
 }
 // a launch without a cluster attribute, with PDL as the options say
 template <typename... KArgs, typename... Args>
-int launch_k(const LaunchOpts& lo, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
+int launch_k(const LaunchOpts& lo, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, const Args&... args) {
   return launch_ex(LaunchConfig(grid, block, smem, st, 0, lo.use_pdl), kern, args...);
 }
 // PDL on a launch of cg-CTA clusters of the forward chain: CTA pairs take it only with the "pair_pdl" option
@@ -576,24 +577,110 @@ int qkv_attn_launch(LaunchOpts& lo, const void* xn, const void* W, const float* 
   return launch_k(lo, pq::enc_qkv_attn_kernel<384>, grid, dim3(pq::QA_THREADS), pq::QkvAttnCfg::kSmemBytes, st, tx, tw, bias, o, items);
 }
 
+// The engine's streams are non-blocking, its events untimed (the timing events come from pool_event)
+int make_stream(Stream* s) {
+  cudaStream_t h = nullptr;
+  PQ_CUDA(cudaStreamCreateWithFlags(&h, cudaStreamNonBlocking));
+  *s = Stream(h);
+  return PARSEQ_OK;
+}
+int make_event(Event* ev) {
+  cudaEvent_t h = nullptr;
+  PQ_CUDA(cudaEventCreateWithFlags(&h, cudaEventDisableTiming));
+  *ev = Event(h);
+  return PARSEQ_OK;
+}
+
 struct Slot {
   std::string key;   // internal name (PARSeq state_dict key)
   std::string pub;   // state_dict key of the served architecture (== key for PARSeq; ViTSTR drops the "encoder." prefix)
   long long numel;
   bool bf16;
-  void* dev;
+  DevBuf<unsigned char> dev;
   bool set;
+};
+
+// What the engine allocates for its sizes (max_batch, chunk, dec_chunk): the buffers alloc_workspace creates and those
+// that calls reserve on first use.  A resize replaces all of it (free_workspace); the weights, the tables derived from
+// them and the host-crop staging buffer stay.
+struct Workspace {
+  // encoder workspace (one pipeline stage = `chunk` images; the encoder runs serialised on `main`)
+  DevBuf<__nv_bfloat16> a_pe, xn, qkv, att, hid;
+  DevBuf<float> x;
+  DevBuf<float> vt_rows;                            // ViTSTR tail: gathered token rows [chunk * L, D] fp32
+  // per-stage decoder state: the decoder of stage s runs on its own stream while `main` encodes stage s+1
+  DevBuf<__nv_bfloat16> mem, ckv;                   // [max_batch*T, D] encoder output, [max_batch*T, 2D] cross K/V
+  std::vector<DevBuf<__nv_bfloat16>> ckv_deep;      // cross K/V of decoder layers 1..dec_depth-1, laid out as ckv
+  // persistent AR-loop kernel state (whole super-chunk)
+  DevBuf<__nv_bfloat16> ar_sa, ar_ca, ar_hd;
+  DevBuf<float> ar_y, ar_qc, ar_part;
+  DevBuf<int> ar_ids;               // [max_batch, ids_ld]
+  DevBuf<unsigned int> ar_bar;
+  DevBuf<unsigned long long> ar_prof;   // [32][16] phase time stamps of the AR kernel (debug option "ar_prof"; DESIGN.md 4)
+  Event ev_enc;                     // `main`'s work so far, which the stage streams wait for (fan_out)
+  struct Stage {
+    DevBuf<__nv_bfloat16> sa, yn, ca, hd;
+    DevBuf<float> y, qc;
+    DevBuf<int> ids_ar, ids_ctx;    // [dec_chunk, ids_ld]
+    // decoders of depth >= 2: content residual stream [dec_chunk * L, D] fp32, and the content K/V of layers
+    // 1..dec_depth-1, one [dec_chunk, L, 2D] bf16 cache per layer (layer 0 reads the (position, token) table)
+    DevBuf<float> cx;
+    std::vector<DevBuf<__nv_bfloat16>> kvc;
+    // candidate scoring (parseq_score), allocated by the first score call: per-tile log-sum-exp partials
+    // [dec_chunk * L][ceil(C / 128)] and target logits of the chain's rows
+    DevBuf<float2> lse_part;
+    DevBuf<float> lse_tlogit;
+    // beam search (parseq_beam_search), allocated by the first beam call: double-buffered state of `rows` beam rows
+    // (ids [rows][ids_ld], score, len, st; kernels.cuh beam_select_kernel), the parent row of each new beam, what the
+    // head leaves of one step's rows (ViTSTR: of `rows / BEAM_MAX` images' positions) - the logits at <= 128 classes, the
+    // top-K epilogue's partials and keys above - and at depth >= 2 a second content K/V cache per layer that the parents'
+    // rows are gathered into
+    struct Beam {
+      int rows = 0;
+      DevBuf<int> ids[2];
+      DevBuf<float> score[2];
+      DevBuf<int> len[2];
+      DevBuf<int> st[2];
+      DevBuf<int> parent;
+      DevBuf<float> logits;              // <= 128 classes: the step's logits
+      DevBuf<float2> part;               // > 128 classes: the top-K epilogue's LSE partials [lrows][ceil(C / 128)]
+      DevBuf<unsigned long long> keys;   //   and keys [lrows][ceil(C / 128)][BEAM_TOPK_LD]
+      std::vector<DevBuf<__nv_bfloat16>> kvc;
+      // lexicon search (parseq_beam_search_lexicon), allocated by the first lexicon call: each beam row's lexicon node,
+      // double-buffered; above 128 classes `logits` is allocated then as well (the lexicon step reads whole rows)
+      DevBuf<int> node[2];
+    } bm;
+    Stream stream;
+    Event ev_done;
+  };
+  std::vector<Stage> stages;
+  // static I/O buffers the CUDA graphs are captured on
+  DevBuf<float> in_images, out_logits;
+  DevBuf<int> out_ids, out_steps;
+  DevBuf<float> out_maps;           // [max_batch, L, T] cross-attention maps, allocated by the first call that asks for them
+  DevBuf<uint8_t> in_images_u8;     // static input of the uint8 HWC entry points
+  DevBuf<uint32_t> in_mask;         // [max_batch, mask_ld] class allowlist rows of the super-chunk (graphs, host entry points)
+  DevBuf<pq::CropDesc> crop_tab;    // the resize kernel's crop table [max_batch] (raw-crop entry points, crops.cuh)
+  // candidate scoring: the call's metadata (ids, targets, row tables; grown on demand), one causal [P][P] mask per
+  // P = 1..L (mask of P at sc_causal + (P - 1) * L * L), and ViTSTR's LSE partials of a chunk's (image, position) rows
+  DevBuf<int> sc_meta;
+  DevBuf<unsigned char> sc_causal;
+  DevBuf<float2> sc_vt_part;
+  long long beam_bytes = 0;         // device bytes of the beam-search buffers (0 until the first beam call)
+  DevBuf<int> lex_roots;            // the lexicon call's roots (grown on demand)
 };
 
 }  // namespace
 
-struct parseq_engine {
+// The engine derives from its workspace so that the call sites name its buffers directly (e->x, e->stages).  Its own
+// members are destroyed before the workspace base, and `graphs` before every other member: the graphs go before the
+// buffers they captured.
+struct parseq_engine : Workspace {
   parseq_config cfg;
   int D, T, Kp, Me, Md, L, V, C, gh, gw, dh_dec;   // T: tokens per image in the encoder (patches + class token if any)
   int ids_ld = 32;                                   // row pitch of the decoder's id buffers: 32 (L <= 32) or 64 (L <= 64)
   int arch = 0, Tp = 0;                              // arch 1 = ViTSTR; Tp = gh * gw patches
   std::map<std::string, int> pub_index;
-  float* vt_rows = nullptr;                          // ViTSTR tail: gathered token rows [chunk * L, D] fp32
   int chunk;
   std::vector<Slot> slots;
   std::map<std::string, int> index;
@@ -603,19 +690,13 @@ struct parseq_engine {
   long long launches = 0;
   // optional per-category device timing (bench.py roofline pass; off on the throughput pass)
   bool timing = false;
-  struct TimedLaunch { int cat; double flops; cudaEvent_t a, b; };
+  struct TimedLaunch { int cat; double flops; Event a, b; };
   std::vector<TimedLaunch> timed;
-  std::vector<cudaEvent_t> event_pool;
+  std::vector<Event> event_pool;
   int cur_cat = 5;
   // derived tables
-  __nv_bfloat16* kvtab = nullptr;   // [L*V, 2D]
-  float* qs = nullptr;              // [L, D]
-  // encoder workspace (one pipeline stage = `chunk` images; the encoder runs serialised on `main`)
-  __nv_bfloat16 *a_pe = nullptr, *xn = nullptr, *qkv = nullptr, *att = nullptr, *hid = nullptr;
-  float* x = nullptr;
-  // per-stage decoder state: the decoder of stage s runs on its own stream while `main` encodes stage s+1
-  __nv_bfloat16 *mem = nullptr, *ckv = nullptr;   // [max_batch*T, D] encoder output, [max_batch*T, 2D] cross K/V
-  std::vector<__nv_bfloat16*> ckv_deep;           // cross K/V of decoder layers 1..dec_depth-1, laid out as ckv
+  DevBuf<__nv_bfloat16> kvtab;      // [L*V, 2D]
+  DevBuf<float> qs;                 // [L, D]
   int dec_chunk = 128;              // images per decoder chain (each chain runs on its own stream)
   // persistent AR-loop kernel state (whole super-chunk)
   int ar_kernel = 2;                // option "ar_kernel": 0 chain, 1 grid-barrier kernel, 2 cluster kernel where it applies (ar_path)
@@ -631,79 +712,21 @@ struct parseq_engine {
   int ar_clusters_override = 0;     // option "ar_clusters": clusters the AR kernel spreads a batch over (0 = derived)
   int fuse_mlp = 0;                 // fc1 + GELU + fc2 + residual + LayerNorm in one kernel (mlp_ln.cuh) where fuse_ln bit 1 applies
   int fuse_ln = 3;                  // bit 0: attn.proj, bit 1: mlp.fc2 also produce the LayerNorm that follows (gemm_ln.cuh)
-  __nv_bfloat16 *ar_sa = nullptr, *ar_ca = nullptr, *ar_hd = nullptr;
-  float *ar_y = nullptr, *ar_qc = nullptr, *ar_part = nullptr;
-  int* ar_ids = nullptr;            // [max_batch, ids_ld]
-  unsigned int* ar_bar = nullptr;
-  unsigned long long* ar_prof = nullptr;   // [32][16] phase time stamps of the AR kernel (debug option "ar_prof"; DESIGN.md 4)
   bool ar_prof_on = false;
-  cudaEvent_t ev_enc = nullptr;     // `main`'s work so far, which the stage streams wait for (fan_out)
-  struct Stage {
-    __nv_bfloat16 *sa = nullptr, *yn = nullptr, *ca = nullptr, *hd = nullptr;
-    float *y = nullptr, *qc = nullptr;
-    int *ids_ar = nullptr, *ids_ctx = nullptr;    // [dec_chunk, ids_ld]
-    // decoders of depth >= 2: content residual stream [dec_chunk * L, D] fp32, and the content K/V of layers
-    // 1..dec_depth-1, one [dec_chunk, L, 2D] bf16 cache per layer (layer 0 reads the (position, token) table)
-    float* cx = nullptr;
-    std::vector<__nv_bfloat16*> kvc;
-    // candidate scoring (parseq_score), allocated by the first score call: per-tile log-sum-exp partials
-    // [dec_chunk * L][ceil(C / 128)] and target logits of the chain's rows
-    float2* lse_part = nullptr;
-    float* lse_tlogit = nullptr;
-    // beam search (parseq_beam_search), allocated by the first beam call: double-buffered state of `rows` beam rows
-    // (ids [rows][ids_ld], score, len, st; kernels.cuh beam_select_kernel), the parent row of each new beam, what the
-    // head leaves of one step's rows (ViTSTR: of `rows / BEAM_MAX` images' positions) - the logits at <= 128 classes, the
-    // top-K epilogue's partials and keys above - and at depth >= 2 a second content K/V cache per layer that the parents'
-    // rows are gathered into
-    struct Beam {
-      int rows = 0;
-      int* ids[2] = {nullptr, nullptr};
-      float* score[2] = {nullptr, nullptr};
-      int* len[2] = {nullptr, nullptr};
-      int* st[2] = {nullptr, nullptr};
-      int* parent = nullptr;
-      float* logits = nullptr;              // <= 128 classes: the step's logits
-      float2* part = nullptr;               // > 128 classes: the top-K epilogue's LSE partials [lrows][ceil(C / 128)]
-      unsigned long long* keys = nullptr;   //   and keys [lrows][ceil(C / 128)][BEAM_TOPK_LD]
-      std::vector<__nv_bfloat16*> kvc;
-      // lexicon search (parseq_beam_search_lexicon), allocated by the first lexicon call: each beam row's lexicon node,
-      // double-buffered; above 128 classes `logits` is allocated then as well (the lexicon step reads whole rows)
-      int* node[2] = {nullptr, nullptr};
-    } bm;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev_done = nullptr;
-  };
-  std::vector<Stage> stages;
   int max_batch = 512;              // images per graph / super-chunk = stages.size() * chunk
-  cudaStream_t main = nullptr;      // engine-owned: user stream -> (event) -> main -> (event) -> user stream
-  cudaStream_t copy = nullptr;      // host entry points: input upload in two halves, overlapped with the first half's encoder
-  cudaEvent_t ev_c[3] = {nullptr, nullptr, nullptr};
-  cudaEvent_t ev_in = nullptr, ev_out = nullptr;
-  // static I/O buffers the CUDA graphs are captured on
-  float* in_images = nullptr; float* out_logits = nullptr; int* out_ids = nullptr; int* out_steps = nullptr;
-  float* out_maps = nullptr;        // [max_batch, L, T] cross-attention maps, allocated by the first call that asks for them
-  uint8_t* in_images_u8 = nullptr;  // static input of the uint8 HWC entry points
-  uint32_t* in_mask = nullptr;      // [max_batch, mask_ld] class allowlist rows of the super-chunk (graphs, host entry points)
+  Stream main;                      // engine-owned: user stream -> (event) -> main -> (event) -> user stream
+  Stream copy;                      // host entry points: input upload in two halves, overlapped with the first half's encoder
+  Event ev_c[3];
+  Event ev_in, ev_out;
   int mask_ld = 0;                  // words per allowlist row: ceil(C / 32)
-  // raw-crop entry points (crops.cuh): the resize kernel's crop table [max_batch], its host copy for the current
-  // super-chunk, and the device copy of a super-chunk's packed bytes for the host entry point (grown on demand)
-  pq::CropDesc* crop_tab = nullptr;
+  // raw-crop entry points (crops.cuh): the host copy of the crop table of the current super-chunk, and the device copy
+  // of a super-chunk's packed bytes for the host entry point (grown on demand)
   std::vector<pq::CropDesc> crop_descs;
   long long crop_base = 0;
-  uint8_t* crop_stage = nullptr;
-  long long crop_stage_bytes = 0;
-  // candidate scoring: the call's metadata (ids, targets, row tables; grown on demand), one causal [P][P] mask per
-  // P = 1..L (mask of P at sc_causal + (P - 1) * L * L), and ViTSTR's LSE partials of a chunk's (image, position) rows
-  int* sc_meta = nullptr;
-  long long sc_meta_ints = 0;
-  unsigned char* sc_causal = nullptr;
-  float2* sc_vt_part = nullptr;
-  long long beam_bytes = 0;         // device bytes of the beam-search buffers (0 until the first beam call)
-  int* lex_roots = nullptr;         // the lexicon call's roots [lex_roots_cap] (grown on demand)
-  long long lex_roots_cap = 0;
+  DevBuf<uint8_t> crop_stage;
   bool use_graph = true;
-  struct GraphEntry { cudaGraphExec_t exec; long long kernels; };
-  std::map<std::vector<int>, GraphEntry> graphs;
+  struct GraphEntry { GraphExec exec; long long kernels; };
+  std::map<std::vector<int>, GraphEntry> graphs;   // last member: destroyed first
 
   void* w(const std::string& k) const { return slots[index.at(k)].dev; }
   const float* wf(const std::string& k) const { return reinterpret_cast<const float*>(w(k)); }
@@ -713,11 +736,32 @@ struct parseq_engine {
 // A lexicon DAG on one device (parseq_lexicon_create): the CSR arrays of parseq_lexicon_desc
 struct parseq_lexicon {
   int device = 0, C = 0, V = 0, E = 0;
-  int* first_edge = nullptr;        // [V + 1]
-  int* edge_class = nullptr;        // [max(E, 1)]
-  int* edge_child = nullptr;        // [max(E, 1)]
-  unsigned char* terminal = nullptr;   // [V]
+  DevBuf<int> first_edge;           // [V + 1]
+  DevBuf<int> edge_class;           // [max(E, 1)]
+  DevBuf<int> edge_child;           // [max(E, 1)]
+  DevBuf<unsigned char> terminal;   // [V]
 };
+
+template <typename T>
+int DevBuf<T>::alloc(long long n) {
+  reset();
+  void* p = nullptr;
+  PQ_CUDA(cudaMalloc(&p, static_cast<size_t>(n) * sizeof(T)));
+  p_ = static_cast<T*>(p);
+  n_ = n;
+  g_live_bytes += bytes();
+  return PARSEQ_OK;
+}
+
+template <typename T>
+int DevBuf<T>::grow(const parseq_engine* e, long long n) {
+  if (n <= n_) return PARSEQ_OK;
+  if (p_ != nullptr) {
+    PQ_CUDA(cudaStreamSynchronize(e->main));
+    PQ_CUDA(cudaStreamSynchronize(e->copy));
+  }
+  return alloc(n);
+}
 
 namespace {
 
@@ -726,30 +770,7 @@ void add_slot(parseq_engine* e, const std::string& key, long long numel, bool bf
   if (e->arch == 1 && key.rfind("encoder.", 0) == 0) pub = key.substr(8);
   e->index[key] = static_cast<int>(e->slots.size());
   e->pub_index[pub] = static_cast<int>(e->slots.size());
-  e->slots.push_back(Slot{key, pub, numel, bf16, nullptr, false});
-}
-
-template <typename Tp>
-int dev_alloc(Tp** p, long long n) {
-  PQ_CUDA(cudaMalloc(reinterpret_cast<void**>(p), static_cast<size_t>(n) * sizeof(Tp)));
-  return PARSEQ_OK;
-}
-
-// A buffer of a call's inputs that grows on demand to n elements (*cap: its size).  The kernels of the previous call,
-// on `main` or `copy`, may still read the old one: both streams are drained before it is freed.
-template <typename Tp>
-int grow(parseq_engine* e, Tp** p, long long* cap, long long n) {
-  if (n <= *cap) return PARSEQ_OK;
-  if (*p != nullptr) {
-    PQ_CUDA(cudaStreamSynchronize(e->main));
-    PQ_CUDA(cudaStreamSynchronize(e->copy));
-    cudaFree(*p);
-    *p = nullptr;
-    *cap = 0;
-  }
-  PQ_TRY(dev_alloc(p, n));
-  *cap = n;
-  return PARSEQ_OK;
+  e->slots.push_back(Slot{key, pub, numel, bf16, {}, false});
 }
 
 // The handle can run a call: not null, its workspace allocated, and (`weights`) its weights finalized.
@@ -782,109 +803,65 @@ int alloc_workspace(parseq_engine* e) {
   const long long RB = static_cast<long long>(e->max_batch) * e->T;     // rows of a whole super-chunk
   const long long Rd = static_cast<long long>(e->dec_chunk) * e->L;     // decoder rows per chain
   const int D = e->D;
-  PQ_TRY(dev_alloc(&e->a_pe, R * e->Kp));
-  PQ_TRY(dev_alloc(&e->x, R * D));
-  PQ_TRY(dev_alloc(&e->xn, R * D));
-  PQ_TRY(dev_alloc(&e->qkv, R * 3 * D));
-  PQ_TRY(dev_alloc(&e->att, R * D));
-  PQ_TRY(dev_alloc(&e->hid, R * e->Me));
-  PQ_TRY(dev_alloc(&e->mem, RB * D));
-  PQ_TRY(dev_alloc(&e->ckv, RB * 2 * D));
+  PQ_TRY(e->a_pe.alloc(R * e->Kp));
+  PQ_TRY(e->x.alloc(R * D));
+  PQ_TRY(e->xn.alloc(R * D));
+  PQ_TRY(e->qkv.alloc(R * 3 * D));
+  PQ_TRY(e->att.alloc(R * D));
+  PQ_TRY(e->hid.alloc(R * e->Me));
+  PQ_TRY(e->mem.alloc(RB * D));
+  PQ_TRY(e->ckv.alloc(RB * 2 * D));
   if (e->cfg.dec_depth > 1) {
-    e->ckv_deep.assign(static_cast<size_t>(e->cfg.dec_depth - 1), nullptr);
-    for (auto& c : e->ckv_deep) PQ_TRY(dev_alloc(&c, RB * 2 * D));
+    e->ckv_deep.resize(static_cast<size_t>(e->cfg.dec_depth - 1));
+    for (auto& c : e->ckv_deep) PQ_TRY(c.alloc(RB * 2 * D));
   }
-  PQ_TRY(dev_alloc(&e->ar_sa, 1ll * e->max_batch * D));
-  PQ_TRY(dev_alloc(&e->ar_ca, 1ll * e->max_batch * D));
-  PQ_TRY(dev_alloc(&e->ar_hd, 1ll * e->max_batch * e->Md));
-  PQ_TRY(dev_alloc(&e->ar_y, 1ll * e->max_batch * D));
-  PQ_TRY(dev_alloc(&e->ar_qc, 1ll * e->max_batch * D));
-  PQ_TRY(dev_alloc(&e->ar_part, 3ll * e->max_batch * D));
-  PQ_TRY(dev_alloc(&e->ar_ids, 1ll * e->max_batch * e->ids_ld));
-  PQ_TRY(dev_alloc(&e->ar_bar, 64));
-  PQ_TRY(dev_alloc(&e->ar_prof, 32 * 16));
-  if (e->arch == 1) PQ_TRY(dev_alloc(&e->vt_rows, 1ll * e->chunk * e->L * D));
-  PQ_CUDA(cudaEventCreateWithFlags(&e->ev_enc, cudaEventDisableTiming));
+  PQ_TRY(e->ar_sa.alloc(1ll * e->max_batch * D));
+  PQ_TRY(e->ar_ca.alloc(1ll * e->max_batch * D));
+  PQ_TRY(e->ar_hd.alloc(1ll * e->max_batch * e->Md));
+  PQ_TRY(e->ar_y.alloc(1ll * e->max_batch * D));
+  PQ_TRY(e->ar_qc.alloc(1ll * e->max_batch * D));
+  PQ_TRY(e->ar_part.alloc(3ll * e->max_batch * D));
+  PQ_TRY(e->ar_ids.alloc(1ll * e->max_batch * e->ids_ld));
+  PQ_TRY(e->ar_bar.alloc(64));
+  PQ_TRY(e->ar_prof.alloc(32 * 16));
+  if (e->arch == 1) PQ_TRY(e->vt_rows.alloc(1ll * e->chunk * e->L * D));
+  PQ_TRY(make_event(&e->ev_enc));
   const int n_stages = (e->max_batch + e->dec_chunk - 1) / e->dec_chunk;
   e->stages.resize(static_cast<size_t>(n_stages));
   for (auto& sg : e->stages) {
-    PQ_TRY(dev_alloc(&sg.sa, Rd * D));
-    PQ_TRY(dev_alloc(&sg.yn, Rd * D));
-    PQ_TRY(dev_alloc(&sg.ca, Rd * D));
-    PQ_TRY(dev_alloc(&sg.hd, Rd * e->Md));
-    PQ_TRY(dev_alloc(&sg.y, Rd * D));
-    PQ_TRY(dev_alloc(&sg.qc, Rd * D));
-    PQ_TRY(dev_alloc(&sg.ids_ar, static_cast<long long>(e->dec_chunk) * e->ids_ld));
-    PQ_TRY(dev_alloc(&sg.ids_ctx, static_cast<long long>(e->dec_chunk) * e->ids_ld));
+    PQ_TRY(sg.sa.alloc(Rd * D));
+    PQ_TRY(sg.yn.alloc(Rd * D));
+    PQ_TRY(sg.ca.alloc(Rd * D));
+    PQ_TRY(sg.hd.alloc(Rd * e->Md));
+    PQ_TRY(sg.y.alloc(Rd * D));
+    PQ_TRY(sg.qc.alloc(Rd * D));
+    PQ_TRY(sg.ids_ar.alloc(static_cast<long long>(e->dec_chunk) * e->ids_ld));
+    PQ_TRY(sg.ids_ctx.alloc(static_cast<long long>(e->dec_chunk) * e->ids_ld));
     if (e->cfg.dec_depth > 1) {
-      PQ_TRY(dev_alloc(&sg.cx, Rd * D));
-      sg.kvc.assign(static_cast<size_t>(e->cfg.dec_depth - 1), nullptr);
-      for (auto& c : sg.kvc) PQ_TRY(dev_alloc(&c, Rd * 2 * D));
+      PQ_TRY(sg.cx.alloc(Rd * D));
+      sg.kvc.resize(static_cast<size_t>(e->cfg.dec_depth - 1));
+      for (auto& c : sg.kvc) PQ_TRY(c.alloc(Rd * 2 * D));
     }
-    PQ_CUDA(cudaStreamCreateWithFlags(&sg.stream, cudaStreamNonBlocking));
-    PQ_CUDA(cudaEventCreateWithFlags(&sg.ev_done, cudaEventDisableTiming));
+    PQ_TRY(make_stream(&sg.stream));
+    PQ_TRY(make_event(&sg.ev_done));
   }
   const long long NB = e->max_batch;
-  PQ_TRY(dev_alloc(&e->in_images, NB * 3 * e->cfg.img_h * e->cfg.img_w));
-  PQ_TRY(dev_alloc(&e->in_images_u8, NB * 3 * e->cfg.img_h * e->cfg.img_w));
-  PQ_TRY(dev_alloc(&e->crop_tab, NB));
-  PQ_TRY(dev_alloc(&e->in_mask, NB * e->mask_ld));
-  PQ_TRY(dev_alloc(&e->out_logits, NB * e->L * e->C));
-  PQ_TRY(dev_alloc(&e->out_ids, NB * e->L));
-  PQ_TRY(dev_alloc(&e->out_steps, 4));
+  PQ_TRY(e->in_images.alloc(NB * 3 * e->cfg.img_h * e->cfg.img_w));
+  PQ_TRY(e->in_images_u8.alloc(NB * 3 * e->cfg.img_h * e->cfg.img_w));
+  PQ_TRY(e->crop_tab.alloc(NB));
+  PQ_TRY(e->in_mask.alloc(NB * e->mask_ld));
+  PQ_TRY(e->out_logits.alloc(NB * e->L * e->C));
+  PQ_TRY(e->out_ids.alloc(NB * e->L));
+  PQ_TRY(e->out_steps.alloc(4));
   return PARSEQ_OK;
 }
 
-void drop_graphs(parseq_engine* e) {
-  for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second.exec);
-  e->graphs.clear();
-}
-
+// Back to no workspace: the graphs first (they captured its buffers), and the cluster AR kernel's tensor maps, which hold
+// the address of the K/V cache.
 void free_workspace(parseq_engine* e) {
-  drop_graphs(e);
-  e->ar2_maps_ok = false;           // holds the address of the K/V cache
-  void* ptrs[] = {e->a_pe, e->x, e->xn, e->qkv, e->att, e->hid, e->mem, e->ckv, e->in_images, e->out_logits, e->out_ids,
-                  e->out_steps, e->in_images_u8, e->crop_tab, e->in_mask, e->ar_sa, e->ar_ca, e->ar_hd, e->ar_y, e->ar_qc, e->ar_part,
-                  e->ar_ids, e->ar_bar, e->ar_prof};
-  e->ar_part = nullptr; e->ar_prof = nullptr; e->in_images_u8 = nullptr; e->crop_tab = nullptr; e->in_mask = nullptr;
-  if (e->vt_rows) { cudaFree(e->vt_rows); e->vt_rows = nullptr; }
-  e->ar_sa = e->ar_ca = e->ar_hd = nullptr; e->ar_y = e->ar_qc = nullptr; e->ar_ids = nullptr; e->ar_bar = nullptr;
-  for (void* p : ptrs)
-    if (p) cudaFree(p);
-  for (auto p : e->ckv_deep)
-    if (p) cudaFree(p);
-  e->ckv_deep.clear();
-  void* sc[] = {e->sc_meta, e->sc_causal, e->sc_vt_part};
-  for (void* p : sc)
-    if (p) cudaFree(p);
-  e->sc_meta = nullptr; e->sc_meta_ints = 0; e->sc_causal = nullptr; e->sc_vt_part = nullptr;
-  e->beam_bytes = 0;
-  if (e->out_maps) { cudaFree(e->out_maps); e->out_maps = nullptr; }
-  if (e->lex_roots) { cudaFree(e->lex_roots); e->lex_roots = nullptr; }
-  e->lex_roots_cap = 0;
-  if (e->ev_enc) { cudaEventDestroy(e->ev_enc); e->ev_enc = nullptr; }
-  e->a_pe = e->xn = e->qkv = e->att = e->hid = e->mem = e->ckv = nullptr;
-  e->x = e->in_images = e->out_logits = nullptr;
-  e->out_ids = e->out_steps = nullptr;
-  for (auto& sg : e->stages) {
-    void* q[] = {sg.sa, sg.yn, sg.ca, sg.hd, sg.y, sg.qc, sg.ids_ar, sg.ids_ctx};
-    for (void* p : q)
-      if (p) cudaFree(p);
-    if (sg.cx) cudaFree(sg.cx);
-    if (sg.lse_part) cudaFree(sg.lse_part);
-    if (sg.lse_tlogit) cudaFree(sg.lse_tlogit);
-    void* bq[] = {sg.bm.ids[0], sg.bm.ids[1], sg.bm.score[0], sg.bm.score[1], sg.bm.len[0], sg.bm.len[1], sg.bm.st[0],
-                  sg.bm.st[1], sg.bm.parent, sg.bm.logits, sg.bm.part, sg.bm.keys, sg.bm.node[0], sg.bm.node[1]};
-    for (void* p : bq)
-      if (p) cudaFree(p);
-    for (auto p : sg.bm.kvc)
-      if (p) cudaFree(p);
-    for (auto p : sg.kvc)
-      if (p) cudaFree(p);
-    if (sg.stream) cudaStreamDestroy(sg.stream);
-    if (sg.ev_done) cudaEventDestroy(sg.ev_done);
-  }
-  e->stages.clear();
+  e->graphs.clear();
+  e->ar2_maps_ok = false;
+  static_cast<Workspace&>(*e) = Workspace();
 }
 
 // categories: 0 encoder GEMM, 1 encoder attention, 2 LayerNorm, 3 decoder GEMM, 4 decoder attention, 5 other,
@@ -894,9 +871,9 @@ void free_workspace(parseq_engine* e) {
 enum { CAT_ENC_GEMM = 0, CAT_ENC_ATTN = 1, CAT_LN = 2, CAT_DEC_GEMM = 3, CAT_DEC_ATTN = 4, CAT_MISC = 5, CAT_ENC_GEMM_LN = 6, CAT_DEC_AR = 7,
        CAT_SCORE = 8, CAT_BEAM = 9, CAT_MAPS = 10, CAT_COUNT = 11 };
 
-cudaEvent_t pool_event(parseq_engine* e) {
-  if (!e->event_pool.empty()) { cudaEvent_t ev = e->event_pool.back(); e->event_pool.pop_back(); return ev; }
-  cudaEvent_t ev; cudaEventCreate(&ev); return ev;
+Event pool_event(parseq_engine* e) {
+  if (!e->event_pool.empty()) { Event ev = std::move(e->event_pool.back()); e->event_pool.pop_back(); return ev; }
+  cudaEvent_t ev = nullptr; cudaEventCreate(&ev); return Event(ev);
 }
 struct TimedScope {   // records a CUDA-event pair around the launches issued in its lifetime
   parseq_engine* e; cudaStream_t st; int idx = -1;
@@ -905,7 +882,7 @@ struct TimedScope {   // records a CUDA-event pair around the launches issued in
     if (!e->timing) return;
     parseq_engine::TimedLaunch t{cat, flops, pool_event(e), pool_event(e)};
     cudaEventRecord(t.a, st);
-    e->timed.push_back(t);
+    e->timed.push_back(std::move(t));
     idx = static_cast<int>(e->timed.size()) - 1;
   }
   ~TimedScope() { if (idx >= 0) cudaEventRecord(e->timed[idx].b, st); }
@@ -965,7 +942,7 @@ int encode_chunk(parseq_engine* e, const void* images_any, bool u8, int B, __nv_
                 e->x, D, st));
   } else {
     // timm _pos_embed with a class token: x = cat(cls_token, patches * Wpe^T + bpe) + pos_embed[0..Tp]
-    float* tmp = reinterpret_cast<float*>(e->hid);      // [B*Tp, D] fp32 fits the (still unused) [B*T, 4D] bf16 MLP buffer
+    float* tmp = reinterpret_cast<float*>(e->hid.get());      // [B*Tp, D] fp32 fits the (still unused) [B*T, 4D] bf16 MLP buffer
     PQ_TRY(gemm(e, e->a_pe, e->Kp, e->w("encoder.patch_embed.proj.weight"), e->Kp,
                 e->wf("encoder.patch_embed.proj.bias"), B * e->Tp, D, e->Kp, pq::EPI_F32, 1.0f,
                 e->wf("encoder.pos_embed") + D, D, e->Tp, tmp, D, st));
@@ -974,7 +951,7 @@ int encode_chunk(parseq_engine* e, const void* images_any, bool u8, int B, __nv_
     const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, 132ll * 16));
     PQ_TRY(launch_k(e->lo, pq::cls_assemble_kernel, dim3(grid), dim3(256), 0, st, reinterpret_cast<const float4*>(tmp),
                     reinterpret_cast<const float4*>(e->wf("encoder.cls_token")),
-                    reinterpret_cast<const float4*>(e->wf("encoder.pos_embed")), reinterpret_cast<float4*>(e->x), B, e->Tp,
+                    reinterpret_cast<const float4*>(e->wf("encoder.pos_embed")), reinterpret_cast<float4*>(e->x.get()), B, e->Tp,
                     D / 4));
   }
   // With fuse_ln the two residual GEMMs of a block also emit the LayerNorm that consumes their result (norm2 after
@@ -1054,8 +1031,8 @@ int vitstr_rows(parseq_engine* e, int B, int L, cudaStream_t st) {
     TimedScope ts(e, st, CAT_MISC, 0.0);
     const long long total = 1ll * M * (D / 4);
     const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, 132ll * 16));
-    PQ_TRY(launch_k(e->lo, pq::gather_token_rows_kernel, dim3(grid), dim3(256), 0, st, reinterpret_cast<const float4*>(e->x),
-                    reinterpret_cast<float4*>(e->vt_rows), B, e->T, 1, L, D / 4));
+    PQ_TRY(launch_k(e->lo, pq::gather_token_rows_kernel, dim3(grid), dim3(256), 0, st, reinterpret_cast<const float4*>(e->x.get()),
+                    reinterpret_cast<float4*>(e->vt_rows.get()), B, e->T, 1, L, D / 4));
   }
   return layernorm(e, e->vt_rows, "encoder.norm", 1e-6f, M, e->xn, nullptr, st);
 }
@@ -1258,7 +1235,7 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
       const int n4 = nq * D / 4;
       PQ_TRY(launch_ex(LaunchConfig(dim3(static_cast<unsigned>(std::min((B * n4 + 255) / 256, 132 * 8))), dim3(256), 0, st, 0, false),
                        pq::bcast_rows_kernel, reinterpret_cast<const float4*>(e->qs + static_cast<long long>(q0) * D),
-                       reinterpret_cast<float4*>(sg.qc), n4, B));
+                       reinterpret_cast<float4*>(sg.qc.get()), n4, B));
       e->launches++;
       qself = sg.qc;
       mode = 2;
@@ -1387,7 +1364,7 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
     for (int i = 0; i < L; ++i) {
       // step i: context ids[:, :i+1], query position i; the fused tail writes ids[:, i+1] = argmax (model.py:142)
       PQ_TRY(decode_pass(e, sg, b_first, B, 1, i, i + 1, 0, sg.ids_ar, logits + static_cast<long long>(i) * C, LC,
-                         (i + 1 < L) ? sg.ids_ar : nullptr, i + 1, forced, L, mask, st, nullptr, /*ar_step*/ true));
+                         (i + 1 < L) ? sg.ids_ar.get() : nullptr, i + 1, forced, L, mask, st, nullptr, /*ar_step*/ true));
     }
     if (testing && steps != nullptr) {
       PQ_TRY(launch_k(e->lo, pq::ar_steps_kernel, dim3(1), dim3(256), 0, st, static_cast<const int*>(sg.ids_ar), e->ids_ld, B, L,
@@ -1565,7 +1542,7 @@ int ar_decode(parseq_engine* e, ArPath path, const parseq_forward_args* a, int b
     p.forced = a->forced_ids ? a->forced_ids + static_cast<long long>(b0) * L : nullptr;
     p.forced_ld = L;
     p.mask = mask;
-    p.prof = e->ar_prof_on ? e->ar_prof : nullptr;
+    p.prof = e->ar_prof_on ? e->ar_prof.get() : nullptr;
   };
   pq::DecAr2Params q;
   pq::DecArParams p;
@@ -1747,8 +1724,8 @@ int run_graph(parseq_engine* e, const parseq_forward_args* a, int Bc, int L, boo
     const long long before = e->launches;
     PQ_CUDA(cudaStreamBeginCapture(e->main, cudaStreamCaptureModeThreadLocal));
     int r = forward_super(e, &aa, 0, Bc, L, u8 ? static_cast<const void*>(e->in_images_u8) : static_cast<const void*>(e->in_images),
-                          u8, e->out_logits, e->out_ids, e->out_steps, masked ? e->in_mask : nullptr,
-                          a->attn_maps != nullptr ? e->out_maps : nullptr, part, split);
+                          u8, e->out_logits, e->out_ids, e->out_steps, masked ? e->in_mask.get() : nullptr,
+                          a->attn_maps != nullptr ? e->out_maps.get() : nullptr, part, split);
     cudaGraph_t g = nullptr;
     cudaError_t ce = cudaStreamEndCapture(e->main, &g);
     if (r != PARSEQ_OK) { if (g) cudaGraphDestroy(g); return r; }
@@ -1757,9 +1734,9 @@ int run_graph(parseq_engine* e, const parseq_forward_args* a, int Bc, int L, boo
     ce = cudaGraphInstantiate(&exec, g, 0);
     cudaGraphDestroy(g);
     if (ce != cudaSuccess) return fail(PARSEQ_ERR_CUDA, std::string("graph instantiate: ") + cudaGetErrorString(ce));
-    parseq_engine::GraphEntry ge{exec, e->launches - before};
+    parseq_engine::GraphEntry ge{GraphExec(exec), e->launches - before};
     e->launches = before;
-    it = e->graphs.emplace(key, ge).first;
+    it = e->graphs.emplace(key, std::move(ge)).first;
   }
   PQ_CUDA(cudaGraphLaunch(it->second.exec, e->main));
   e->launches += it->second.kernels;
@@ -1840,7 +1817,7 @@ int crops_reserve(parseq_engine* e, const CropBatch& cb, int batch) {
     crop_range(cb.c, b0, (batch - b0 < e->max_batch) ? batch : b0 + e->max_batch, &lo, &hi);
     need = hi - lo > need ? hi - lo : need;
   }
-  return grow(e, &e->crop_stage, &e->crop_stage_bytes, need);
+  return e->crop_stage.grow(e, need);
 }
 
 // Uploads the crop table of super-chunk [b0, b0 + Bc) on `st`.
@@ -1902,7 +1879,7 @@ int causal_reserve(parseq_engine* e) {
   for (int P = 1; P <= L; ++P)
     for (int q = 0; q < P; ++q)
       for (int k = 0; k < P; ++k) h[static_cast<size_t>(P - 1) * L * L + static_cast<size_t>(q) * P + k] = k > q ? 1 : 0;
-  PQ_TRY(dev_alloc(&e->sc_causal, static_cast<long long>(h.size())));
+  PQ_TRY(e->sc_causal.alloc(static_cast<long long>(h.size())));
   PQ_CUDA(cudaMemcpy(e->sc_causal, h.data(), h.size(), cudaMemcpyHostToDevice));
   return PARSEQ_OK;
 }
@@ -1910,7 +1887,7 @@ int causal_reserve(parseq_engine* e) {
 // Cross-attention map buffers, on the first call that asks for maps: the static maps the graphs write, and the causal
 // masks only for an AR-only schedule (the one whose map pass reads them).
 int maps_reserve(parseq_engine* e, const parseq_forward_args* a) {
-  if (e->out_maps == nullptr) PQ_TRY(dev_alloc(&e->out_maps, 1ll * e->max_batch * e->L * e->T));
+  PQ_TRY(e->out_maps.reserve(1ll * e->max_batch * e->L * e->T));
   return a->decode_ar && a->refine_iters == 0 ? causal_reserve(e) : PARSEQ_OK;
 }
 
@@ -1957,7 +1934,7 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
   for (int b0 = 0; b0 < a->batch; b0 += e->max_batch) {
     const int Bc = (a->batch - b0 < e->max_batch) ? (a->batch - b0) : e->max_batch;
     if (eager && !host) {
-      const char* in = reinterpret_cast<const char*>(e->in_images_u8);
+      const char* in = reinterpret_cast<const char*>(e->in_images_u8.get());
       if (crops) {
         PQ_TRY(crops_table(e, *crops, b0, Bc, e->main));
         PQ_TRY(crops_resize(e, *crops, b0, 0, Bc, e->in_images_u8, e->main));
@@ -2008,7 +1985,7 @@ int forward_impl(parseq_engine* e, const parseq_forward_args* a, const void* ima
     PQ_TRY(stage_mask(b0, Bc));
     if (eager) {
       PQ_TRY(forward_super(e, a, b0, Bc, L, in_static, u8, e->out_logits, e->out_ids, e->out_steps,
-                           a->class_mask ? e->in_mask : nullptr, maps ? e->out_maps : nullptr));
+                           a->class_mask ? e->in_mask.get() : nullptr, maps ? e->out_maps.get() : nullptr));
     } else {
       PQ_TRY(run_graph(e, a, Bc, L, u8));
     }
@@ -2083,13 +2060,12 @@ int score_reserve(parseq_engine* e) {
   const long long Rd = 1ll * e->dec_chunk * L;
   if (e->arch == 0) {
     for (auto& sg : e->stages) {
-      if (sg.lse_part != nullptr) continue;
-      PQ_TRY(dev_alloc(&sg.lse_part, Rd * ntiles));
-      PQ_TRY(dev_alloc(&sg.lse_tlogit, Rd));
+      PQ_TRY(sg.lse_part.reserve(Rd * ntiles));
+      PQ_TRY(sg.lse_tlogit.reserve(Rd));
     }
     PQ_TRY(causal_reserve(e));
-  } else if (e->sc_vt_part == nullptr) {
-    PQ_TRY(dev_alloc(&e->sc_vt_part, 1ll * e->chunk * L * ntiles));
+  } else {
+    PQ_TRY(e->sc_vt_part.reserve(1ll * e->chunk * L * ntiles));
   }
   return PARSEQ_OK;
 }
@@ -2162,7 +2138,7 @@ int score_impl(parseq_engine* e, const parseq_score_args* a, const void* images_
       }
     }
   }
-  PQ_TRY(grow(e, &e->sc_meta, &e->sc_meta_ints, static_cast<long long>(h.size())));
+  PQ_TRY(e->sc_meta.grow(e, static_cast<long long>(h.size())));
   const int* meta = e->sc_meta;
   PQ_TRY(enter_main(e, user));
   // pageable source: the copy is staged before the call returns, so `h` may go
@@ -2229,15 +2205,6 @@ int check_score_call(parseq_engine* e, const parseq_score_args* a, const void* i
 // ViTSTR: images whose [L, C] logits one beam group holds (the head runs once per group, the selection once per position)
 int beam_vt_images(const parseq_engine* e) { return std::min(e->chunk, 32); }
 
-// A beam-search buffer of n elements, on first use (counted in beam_bytes)
-template <typename Tp>
-int beam_alloc(parseq_engine* e, Tp** p, long long n) {
-  if (*p != nullptr) return PARSEQ_OK;
-  PQ_TRY(dev_alloc(p, n));
-  e->beam_bytes += n * static_cast<long long>(sizeof(Tp));
-  return PARSEQ_OK;
-}
-
 // Beam buffers, on the first beam call (an engine that never beam-searches allocates none of them).  PARSeq: every stage
 // holds dec_chunk beam rows, whatever the beam width; ViTSTR: stage 0 holds beam_vt_images images of BEAM_MAX slots.
 int beam_reserve(parseq_engine* e) {
@@ -2249,22 +2216,22 @@ int beam_reserve(parseq_engine* e) {
     const int rows = e->arch == 0 ? e->dec_chunk : beam_vt_images(e) * pq::BEAM_MAX;
     const long long lrows = e->arch == 0 ? rows : 1ll * beam_vt_images(e) * e->L;
     for (int h = 0; h < 2; ++h) {
-      PQ_TRY(beam_alloc(e, &bm.ids[h], 1ll * rows * e->ids_ld));
-      PQ_TRY(beam_alloc(e, &bm.score[h], rows));
-      PQ_TRY(beam_alloc(e, &bm.len[h], rows));
-      PQ_TRY(beam_alloc(e, &bm.st[h], rows));
+      PQ_TRY(bm.ids[h].reserve(1ll * rows * e->ids_ld, &e->beam_bytes));
+      PQ_TRY(bm.score[h].reserve(rows, &e->beam_bytes));
+      PQ_TRY(bm.len[h].reserve(rows, &e->beam_bytes));
+      PQ_TRY(bm.st[h].reserve(rows, &e->beam_bytes));
     }
-    PQ_TRY(beam_alloc(e, &bm.parent, rows));
+    PQ_TRY(bm.parent.reserve(rows, &e->beam_bytes));
     const long long ntiles = (e->C + pq::GEMM_BLOCK_N - 1) / pq::GEMM_BLOCK_N;
     if (e->C <= 128) {
-      PQ_TRY(beam_alloc(e, &bm.logits, lrows * e->C));
+      PQ_TRY(bm.logits.reserve(lrows * e->C, &e->beam_bytes));
     } else {
-      PQ_TRY(beam_alloc(e, &bm.part, lrows * ntiles));
-      PQ_TRY(beam_alloc(e, &bm.keys, lrows * ntiles * pq::BEAM_TOPK_LD));
+      PQ_TRY(bm.part.reserve(lrows * ntiles, &e->beam_bytes));
+      PQ_TRY(bm.keys.reserve(lrows * ntiles * pq::BEAM_TOPK_LD, &e->beam_bytes));
     }
     if (e->arch == 0 && e->cfg.dec_depth > 1) {
-      bm.kvc.resize(static_cast<size_t>(e->cfg.dec_depth - 1), nullptr);
-      for (auto& c : bm.kvc) PQ_TRY(beam_alloc(e, &c, 1ll * e->dec_chunk * e->L * 2 * D));
+      bm.kvc.resize(static_cast<size_t>(e->cfg.dec_depth - 1));
+      for (auto& c : bm.kvc) PQ_TRY(c.reserve(1ll * e->dec_chunk * e->L * 2 * D, &e->beam_bytes));
     }
     bm.rows = rows;
   }
@@ -2286,9 +2253,9 @@ int lexicon_reserve(parseq_engine* e) {
   const size_t nst = e->arch == 0 ? e->stages.size() : 1;
   for (size_t s = 0; s < nst; ++s) {
     parseq_engine::Stage::Beam& bm = e->stages[s].bm;
-    for (int h = 0; h < 2; ++h) PQ_TRY(beam_alloc(e, &bm.node[h], bm.rows));
+    for (int h = 0; h < 2; ++h) PQ_TRY(bm.node[h].reserve(bm.rows, &e->beam_bytes));
     const long long lrows = e->arch == 0 ? e->dec_chunk : 1ll * beam_lex_vt_images(e) * e->L;
-    PQ_TRY(beam_alloc(e, &bm.logits, lrows * e->C));
+    PQ_TRY(bm.logits.reserve(lrows * e->C, &e->beam_bytes));
   }
   return PARSEQ_OK;
 }
@@ -2318,9 +2285,9 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
   const int ntiles = (C + pq::GEMM_BLOCK_N - 1) / pq::GEMM_BLOCK_N;
   if (lx != nullptr && roots != nullptr) {
     // `roots`: the checked host copy of the call's roots (beam_lexicon_call), uploaded below
-    const long long cap0 = e->lex_roots_cap;
-    const int rc = grow(e, &e->lex_roots, &e->lex_roots_cap, N);
-    e->beam_bytes += 4ll * (e->lex_roots_cap - cap0);
+    const long long cap0 = e->lex_roots.size();
+    const int rc = e->lex_roots.grow(e, N);
+    e->beam_bytes += 4ll * (e->lex_roots.size() - cap0);
     PQ_TRY(rc);
   }
   auto select = [&](parseq_engine::Stage::Beam& bm, int B, int step, long long row0, long long img_stride,
@@ -2334,7 +2301,7 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
     return launch_k(e->lo, lx != nullptr ? pq::beam_select_kernel<true> : pq::beam_select_kernel<false>,
                     dim3(static_cast<unsigned>(B)), dim3(pq::BEAM_THREADS), 0, st,
                     static_cast<const float*>(bm.logits), static_cast<const float2*>(bm.part),
-                    static_cast<const unsigned long long*>(topk ? bm.keys : nullptr), ntiles, row0, img_stride, slot_stride, C, K, step, S, a->class_mask ? a->class_mask + 1ll * g0 * e->mask_ld : nullptr, e->mask_ld,
+                    static_cast<const unsigned long long*>(topk ? bm.keys.get() : nullptr), ntiles, row0, img_stride, slot_stride, C, K, step, S, a->class_mask ? a->class_mask + 1ll * g0 * e->mask_ld : nullptr, e->mask_ld,
                     static_cast<const int*>(bm.ids[cur]), static_cast<const float*>(bm.score[cur]),
                     static_cast<const int*>(bm.len[cur]), static_cast<const int*>(bm.st[cur]), bm.ids[nxt], bm.score[nxt],
                     bm.len[nxt], bm.st[nxt], bm.parent, e->ids_ld, ids + 1ll * g0 * K * S, lengths + 1ll * g0 * K,
@@ -2384,7 +2351,7 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
         ex.beam_k = K;
         ex.beam_mask = a->class_mask ? a->class_mask + 1ll * (b0 + g0) * e->mask_ld : nullptr;
       }
-      const std::vector<__nv_bfloat16*> kvc0 = sg.kvc;
+      const std::vector<__nv_bfloat16*> kvc0(sg.kvc.begin(), sg.kvc.end());
       int rc = PARSEQ_OK;
       for (int step = 0; step < S && rc == PARSEQ_OK; ++step) {
         // query position `step` over keys 0..step of every beam row; the head leaves row r's logits at bm.logits + r * C
@@ -2401,7 +2368,7 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
         for (size_t l = 0; l < sg.kvc.size() && rc == PARSEQ_OK; ++l) {
           const long long total = 1ll * R * n4;
           rc = launch_k(e->lo, pq::beam_kv_gather_kernel, dim3(static_cast<unsigned>(std::min<long long>((total + 255) / 256, 132ll * 8))),
-                        dim3(256), 0, ds, reinterpret_cast<const uint4*>(sg.kvc[l]), reinterpret_cast<uint4*>(bm.kvc[l]),
+                        dim3(256), 0, ds, reinterpret_cast<const uint4*>(sg.kvc[l].get()), reinterpret_cast<uint4*>(bm.kvc[l].get()),
                         static_cast<const int*>(bm.parent), R, pitch4, n4);
           std::swap(sg.kvc[l], bm.kvc[l]);
         }
@@ -2630,19 +2597,16 @@ int parseq_create(const parseq_config* cfg, parseq_engine** out) {
     // +64 elements of slack: head.bias (95 floats) is read with float4 only when in range, but keep
     // every buffer 16-byte padded
     const size_t bytes = static_cast<size_t>(s.numel + 64) * (s.bf16 ? 2 : 4);
-    if (cudaMalloc(&s.dev, bytes) != cudaSuccess) { parseq_destroy(e); return fail(PARSEQ_ERR_CUDA, "cudaMalloc weights"); }
+    if (s.dev.alloc(static_cast<long long>(bytes)) != PARSEQ_OK) { parseq_destroy(e); return fail(PARSEQ_ERR_CUDA, "cudaMalloc weights"); }
     cudaMemset(s.dev, 0, bytes);
   }
-  int r = dev_alloc(&e->kvtab, 1ll * e->L * e->V * 2 * D);
-  if (r == PARSEQ_OK) r = dev_alloc(&e->qs, 1ll * e->L * D);
+  int r = e->kvtab.alloc(1ll * e->L * e->V * 2 * D);
+  if (r == PARSEQ_OK) r = e->qs.alloc(1ll * e->L * D);
   if (r == PARSEQ_OK) r = alloc_workspace(e);
-  if (r == PARSEQ_OK && cudaStreamCreateWithFlags(&e->main, cudaStreamNonBlocking) != cudaSuccess) r = fail(PARSEQ_ERR_CUDA, "stream");
-  if (r == PARSEQ_OK && cudaStreamCreateWithFlags(&e->copy, cudaStreamNonBlocking) != cudaSuccess) r = fail(PARSEQ_ERR_CUDA, "stream");
-  for (int i = 0; i < 3 && r == PARSEQ_OK; ++i)
-    if (cudaEventCreateWithFlags(&e->ev_c[i], cudaEventDisableTiming) != cudaSuccess) r = fail(PARSEQ_ERR_CUDA, "event");
-  if (r == PARSEQ_OK && (cudaEventCreateWithFlags(&e->ev_in, cudaEventDisableTiming) != cudaSuccess ||
-                         cudaEventCreateWithFlags(&e->ev_out, cudaEventDisableTiming) != cudaSuccess))
-    r = fail(PARSEQ_ERR_CUDA, "event");
+  if (r == PARSEQ_OK) r = make_stream(&e->main);
+  if (r == PARSEQ_OK) r = make_stream(&e->copy);
+  for (Event* ev : {&e->ev_c[0], &e->ev_c[1], &e->ev_c[2], &e->ev_in, &e->ev_out})
+    if (r == PARSEQ_OK) r = make_event(ev);
   if (r != PARSEQ_OK) { parseq_destroy(e); return r; }
   *out = e;
   return PARSEQ_OK;
@@ -2652,19 +2616,6 @@ void parseq_destroy(parseq_engine* e) {
   if (e == nullptr) return;
   cudaSetDevice(e->cfg.device);
   cudaDeviceSynchronize();
-  for (auto& s : e->slots)
-    if (s.dev) cudaFree(s.dev);
-  if (e->kvtab) cudaFree(e->kvtab);
-  if (e->qs) cudaFree(e->qs);
-  if (e->crop_stage) cudaFree(e->crop_stage);
-  free_workspace(e);
-  if (e->main) cudaStreamDestroy(e->main);
-  if (e->copy) cudaStreamDestroy(e->copy);
-  for (auto ev : e->ev_c) if (ev) cudaEventDestroy(ev);
-  if (e->ev_in) cudaEventDestroy(e->ev_in);
-  if (e->ev_out) cudaEventDestroy(e->ev_out);
-  for (auto& t : e->timed) { cudaEventDestroy(t.a); cudaEventDestroy(t.b); }
-  for (auto ev : e->event_pool) cudaEventDestroy(ev);
   delete e;
 }
 
@@ -2709,13 +2660,12 @@ int parseq_finalize(parseq_engine* e, parseq_stream_t stream) {
   const int D = e->D, L = e->L, V = e->V;
   const std::string Ly = "decoder.layers.0.";
   const long long rows = 1ll * L * V;
-  float* ctx = nullptr;
-  __nv_bfloat16* ctxn = nullptr;
-  __nv_bfloat16* qn = nullptr;
-  int r = dev_alloc(&ctx, rows * D);
-  if (r == PARSEQ_OK) r = dev_alloc(&ctxn, rows * D);
-  if (r == PARSEQ_OK) r = dev_alloc(&qn, 1ll * L * D);
-  if (r != PARSEQ_OK) { cudaFree(ctx); cudaFree(ctxn); cudaFree(qn); return r; }
+  DevBuf<float> ctx;                // temporaries, freed on return (after the synchronise below)
+  DevBuf<__nv_bfloat16> ctxn, qn;
+  PQ_TRY(ctx.alloc(rows * D));
+  PQ_TRY(ctxn.alloc(rows * D));
+  PQ_TRY(qn.alloc(1ll * L * D));
+  int r = PARSEQ_OK;
   pq::build_ctx_rows_kernel<<<1024, 256, 0, st>>>(e->wf("text_embed.embedding.weight"), e->wf("pos_queries"), ctx, L, V, D,
                                                   std::sqrt(static_cast<float>(D)));
   if (cudaGetLastError() != cudaSuccess) r = fail(PARSEQ_ERR_CUDA, "build_ctx_rows_kernel launch");
@@ -2734,9 +2684,6 @@ int parseq_finalize(parseq_engine* e, parseq_stream_t stream) {
     r = gemm_launch(e->lo, qn, D, e->wb(Ly + "self_attn.in_proj_weight"), D, e->wf(Ly + "self_attn.in_proj_bias"), L, D, D,
                     pq::EPI_F32, 1.0f / std::sqrt(static_cast<float>(e->dh_dec)), nullptr, 0, 0, e->qs, D, st);
   cudaError_t ce = cudaStreamSynchronize(st);
-  cudaFree(ctx);
-  cudaFree(ctxn);
-  cudaFree(qn);
   if (r != PARSEQ_OK) return r;
   if (ce != cudaSuccess) return fail(PARSEQ_ERR_CUDA, std::string("finalize: ") + cudaGetErrorString(ce));
   e->ar2_maps_ok = false;
@@ -2856,10 +2803,10 @@ int parseq_lexicon_create(parseq_engine* e, const parseq_lexicon_desc* d, parseq
   lx->device = e->cfg.device; lx->C = e->C; lx->V = d->num_nodes; lx->E = d->num_edges;
   const long long E1 = std::max(d->num_edges, 1);
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  int rc = dev_alloc(&lx->first_edge, lx->V + 1ll);
-  if (rc == PARSEQ_OK) rc = dev_alloc(&lx->edge_class, E1);
-  if (rc == PARSEQ_OK) rc = dev_alloc(&lx->edge_child, E1);
-  if (rc == PARSEQ_OK) rc = dev_alloc(&lx->terminal, lx->V);
+  int rc = lx->first_edge.alloc(lx->V + 1ll);
+  if (rc == PARSEQ_OK) rc = lx->edge_class.alloc(E1);
+  if (rc == PARSEQ_OK) rc = lx->edge_child.alloc(E1);
+  if (rc == PARSEQ_OK) rc = lx->terminal.alloc(lx->V);
   auto up = [&](void* dst, const void* src, long long bytes) {
     if (rc == PARSEQ_OK && bytes > 0 && cudaMemcpyAsync(dst, src, static_cast<size_t>(bytes), cudaMemcpyHostToDevice, st) != cudaSuccess)
       rc = fail(PARSEQ_ERR_CUDA, "lexicon upload failed");
@@ -2870,7 +2817,7 @@ int parseq_lexicon_create(parseq_engine* e, const parseq_lexicon_desc* d, parseq
   up(lx->terminal, d->terminal, lx->V);
   if (rc == PARSEQ_OK && cudaStreamSynchronize(st) != cudaSuccess) rc = fail(PARSEQ_ERR_CUDA, "lexicon upload failed");
   if (rc != PARSEQ_OK) {
-    parseq_lexicon_destroy(lx);
+    delete lx;
     return rc;
   }
   *out = lx;
@@ -2880,9 +2827,6 @@ int parseq_lexicon_create(parseq_engine* e, const parseq_lexicon_desc* d, parseq
 void parseq_lexicon_destroy(parseq_lexicon* lx) {
   if (lx == nullptr) return;
   cudaSetDevice(lx->device);
-  void* p[] = {lx->first_edge, lx->edge_class, lx->edge_child, lx->terminal};
-  for (void* q : p)
-    if (q) cudaFree(q);
   delete lx;
 }
 
@@ -2948,7 +2892,7 @@ int parseq_decode_ex(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t n
     // memory (fp32, caller's) -> bf16 operand -> cross K/V cache rows [0, Bc * T)
     const long long n4 = 1ll * Bc * T * D / 4;
     pq::f32_to_bf16_kernel<<<static_cast<unsigned>(std::min<long long>((n4 + 255) / 256, 132ll * 8)), 256, 0, st>>>(
-        reinterpret_cast<const float4*>(memory + 1ll * b0 * T * D), reinterpret_cast<uint2*>(e->mem), n4);
+        reinterpret_cast<const float4*>(memory + 1ll * b0 * T * D), reinterpret_cast<uint2*>(e->mem.get()), n4);
     PQ_CUDA(cudaGetLastError());
     PQ_TRY(cross_kv(e, Bc));
     pq::copy_ids_kernel<<<(Bc * e->ids_ld + 255) / 256, 256, 0, st>>>(tgt + 1ll * b0 * J, J, sg.ids_ctx, Bc, e->ids_ld);
@@ -2979,7 +2923,7 @@ int parseq_head(parseq_engine* e, int32_t rows, const float* x, float* logits, p
     const int n = (rows - r0 < cap) ? (rows - r0) : cap;
     const long long n4 = 1ll * n * D / 4;
     pq::f32_to_bf16_kernel<<<static_cast<unsigned>(std::min<long long>((n4 + 255) / 256, 132ll * 8)), 256, 0, e->main>>>(
-        reinterpret_cast<const float4*>(x + 1ll * r0 * D), reinterpret_cast<uint2*>(sg.yn), n4);
+        reinterpret_cast<const float4*>(x + 1ll * r0 * D), reinterpret_cast<uint2*>(sg.yn.get()), n4);
     PQ_CUDA(cudaGetLastError());
     e->launches++;
     e->cur_cat = CAT_DEC_GEMM;
@@ -3024,6 +2968,8 @@ int64_t parseq_debug_int(parseq_engine* e, const char* name) {
   const std::string n(name);
   // launch options: per handle, or (NULL handle) those of the bare kernel exports; 0 until the first MODE 2 launch
   if (n == "ln_clusters") return (e ? e->lo : g_default_opts).ln_clusters;
+  if (n == "live_device_bytes") return g_live_bytes;      // process-wide: every handle and lexicon
+  if (n == "live_cuda_objects") return g_live_objects;
   if (e == nullptr) return -1;
   if (n == "ar2_occupancy_mt1_cs8") return e->ar2_occ[1][0];
   if (n == "ar2_occupancy_mt2_cs8") return e->ar2_occ[2][0];
@@ -3059,66 +3005,66 @@ int parseq_set_option(parseq_engine* e, const char* name, int64_t value) {
     if (value < 0 || value > 2) return fail(PARSEQ_ERR_INVALID_ARG, "cta_group: 0 (auto) / 1 / 2");
     return PARSEQ_OK;
   }
-  if (n == "attn_impl") { lo.attn_impl = value != 0 ? 1 : 0; if (e) drop_graphs(e); return PARSEQ_OK; }
-  if (n == "pdl") { lo.use_pdl = value != 0; if (e) drop_graphs(e); return PARSEQ_OK; }
+  if (n == "attn_impl") { lo.attn_impl = value != 0 ? 1 : 0; if (e) e->graphs.clear(); return PARSEQ_OK; }
+  if (n == "pdl") { lo.use_pdl = value != 0; if (e) e->graphs.clear(); return PARSEQ_OK; }
   if (n == "gemm_stages") {
     // the MMA warpgroups release a stage once the next k-block's MMAs are queued: a ring needs at least two slots
     if (value < 0 || value == 1) return fail(PARSEQ_ERR_INVALID_ARG, "gemm_stages: 0 (full ring) or >= 2");
     lo.gemm_stages = static_cast<int>(value);
-    if (e) drop_graphs(e);
+    if (e) e->graphs.clear();
     return PARSEQ_OK;
   }
   if (n == "ln_cta_group") {
     if (value < 0 || value > 2) return fail(PARSEQ_ERR_INVALID_ARG, "ln_cta_group: 0 (auto) / 1 / 2");
     lo.ln_cta_group = static_cast<int>(value);
-    if (e) drop_graphs(e);
+    if (e) e->graphs.clear();
     return PARSEQ_OK;
   }
   if (n == "ln_split") {
     if (value < 0 || value > 2) return fail(PARSEQ_ERR_INVALID_ARG, "ln_split: 0 (auto) / 1 (off) / 2 (on)");
     lo.ln_split = static_cast<int>(value);
-    if (e) drop_graphs(e);
+    if (e) e->graphs.clear();
     return PARSEQ_OK;
   }
   if (n == "mlp_cta_group") {
     if (value < 0 || value > 2) return fail(PARSEQ_ERR_INVALID_ARG, "mlp_cta_group: 0 (auto) / 1 / 2");
     lo.mlp_cta_group = static_cast<int>(value);
-    if (e) drop_graphs(e);
+    if (e) e->graphs.clear();
     return PARSEQ_OK;
   }
-  if (n == "pair_pdl") { lo.pair_pdl = value != 0; if (e) drop_graphs(e); return PARSEQ_OK; }
+  if (n == "pair_pdl") { lo.pair_pdl = value != 0; if (e) e->graphs.clear(); return PARSEQ_OK; }
   if (n == "fuse_mlp") {
     if (e == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null engine");
     e->fuse_mlp = value != 0 ? 1 : 0;
-    drop_graphs(e);
+    e->graphs.clear();
     return PARSEQ_OK;
   }
   if (n == "fuse_ln") {
     if (e == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null engine");
     e->fuse_ln = static_cast<int>(value) & 7;
-    drop_graphs(e);
+    e->graphs.clear();
     return PARSEQ_OK;
   }
   if (e == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null engine");
   if (n == "timing") {
     e->timing = value != 0;
-    for (auto& t : e->timed) { e->event_pool.push_back(t.a); e->event_pool.push_back(t.b); }
+    for (auto& t : e->timed) { e->event_pool.push_back(std::move(t.a)); e->event_pool.push_back(std::move(t.b)); }
     e->timed.clear();
     return PARSEQ_OK;
   }
   if (n == "use_graph") { e->use_graph = value != 0; return PARSEQ_OK; }
-  if (n == "ar_prof") { e->ar_prof_on = value != 0; drop_graphs(e); return PARSEQ_OK; }
+  if (n == "ar_prof") { e->ar_prof_on = value != 0; e->graphs.clear(); return PARSEQ_OK; }
   if (n == "ar_clusters") {
     if (value < 0 || value > 1024) return fail(PARSEQ_ERR_INVALID_ARG, "ar_clusters out of range");
     e->ar_clusters_override = static_cast<int>(value);
     for (auto& r : e->ar2_clusters) r[0] = r[1] = 0;
-    drop_graphs(e);
+    e->graphs.clear();
     return PARSEQ_OK;
   }
   if (n == "ar_cluster_size") {
     if (value != 0 && value != 6 && value != 8) return fail(PARSEQ_ERR_INVALID_ARG, "ar_cluster_size: 0 (auto) / 6 / 8");
     e->ar_cs = static_cast<int>(value);
-    drop_graphs(e);
+    e->graphs.clear();
     return PARSEQ_OK;
   }
   if (n == "ar_kernel") {           // 0: AR loop as separate kernels, 1: grid-barrier kernel, 2: cluster kernel (ar_path)
@@ -3126,7 +3072,7 @@ int parseq_set_option(parseq_engine* e, const char* name, int64_t value) {
     if (value == 1)
       if (const char* why = grid_barrier_limit(e)) return fail(PARSEQ_ERR_UNSUPPORTED, why);
     e->ar_kernel = static_cast<int>(value);
-    drop_graphs(e);
+    e->graphs.clear();
     return PARSEQ_OK;
   }
   if (n == "chunk" || n == "max_batch" || n == "dec_chunk") {

@@ -10,7 +10,8 @@
  *
  * Threading / streams: an engine handle is NOT thread-safe (one handle per device and stream user).
  * All work is enqueued on the caller's stream; the only host synchronisation is inside
- * parseq_forward_host (which must return host-visible results) and parseq_finalize.
+ * parseq_forward_host (which must return host-visible results), parseq_finalize and a
+ * parseq_forward_crops_oriented call with a min_confidence.
  */
 #ifndef PARSEQ_B200_H_
 #define PARSEQ_B200_H_
@@ -143,6 +144,9 @@ typedef struct parseq_crops {
   const int64_t* offsets;  /* HOST int64 [N]: byte offset of crop i in data */
   const int32_t* sizes;    /* HOST int32 [N][2]: (h, w) of crop i before rotation, 1 <= h, w <= 8192 */
   int32_t rotation;        /* 0, 90, 180, 270: PIL Image.rotate(r, expand=True), counter-clockwise */
+  const int32_t* rotations;  /* HOST int32 [N]: crop i's own rotation (each 0, 90, 180 or 270), or NULL: `rotation` for
+                                every crop.  A row's results do not depend on the other crops of the call, so crop i
+                                reads exactly as in a call with rotation = rotations[i]. */
 } parseq_crops;
 /* out_hwc: DEVICE uint8 [N, img_h, img_w, 3], what T.Resize(img_size, BICUBIC) makes of each (rotated) crop.  The
  * metadata is checked on the host before anything is launched (PARSEQ_ERR_INVALID_ARG). */
@@ -153,6 +157,41 @@ int parseq_forward_crops(parseq_engine* e, const parseq_forward_args* args, cons
                          int32_t* ids, int32_t* steps, parseq_stream_t stream);
 int parseq_forward_host_crops(parseq_engine* e, const parseq_forward_args* args, const parseq_crops* crops,
                               float* logits_host, int32_t* ids_host, int32_t* steps_host, parseq_stream_t stream);
+/* Orientation search: each crop read in the orientation the model is most confident of.
+ * Rule.  The caller lists orientations o_0 .. o_{R-1} (1 <= R <= 4, distinct, each 0, 90, 180 or 270) and optionally a
+ * threshold t (min_confidence; NaN = none).  Every crop is read at o_0; a crop whose confidence is >= t keeps that
+ * reading.  Every other crop (every crop without t) is also read at o_1 .. o_{R-1} and takes the reading of highest
+ * confidence; ties go to the earlier orientation of the list, and NaN ranks below every number.  A reading's confidence
+ * is parseq_postprocess's, in its fp32 order: parseq_postprocess of the returned logits gives the returned confidence
+ * bit for bit.  Each reading is bit-identical to parseq_forward_crops's at that rotation.
+ * Schedule.  Pass 1 is parseq_forward_crops of all N crops at o_0, into the caller's outputs.  A confidence kernel then
+ * writes o_0 and its confidence c_0 for every crop.  With t, c_0 is copied to the host, which lists the crops below t:
+ * this is the call's one host synchronisation, so a call with t cannot be captured in a CUDA graph.  Pass 2 reads the
+ * listed crops at the other R - 1 orientations: super-chunks of floor(max_batch / (R - 1)) crops, each crop's R - 1
+ * readings in one super-chunk, the reading count rounded up to a power of two (at most max_batch) with copies of the
+ * last reading, so a call adds graphs of power-of-two or max_batch readings only.  After each pass-2 super-chunk the
+ * confidence kernel (one CTA per reading) scores every reading, and the orientation select kernel (one CTA per listed
+ * crop, no atomics) compares a crop's readings and, when one wins, copies its logits, ids and maps into the crop's
+ * outputs.
+ * Outputs are those of parseq_forward_crops (DEVICE logits / ids / steps, attn_maps), plus rotation_out DEVICE int32 [N]
+ * (the chosen orientation) and confidence_out DEVICE fp32 [N].  steps is the maximum over both passes.  Where the steps
+ * shape the result (max_length = -1, decode_ar, refine_iters = 0, PARSeq), the rows of a crop's logits, ids and maps
+ * from the step count of the pass (pass 2: of the super-chunk) that produced its reading are 0: they lie after that
+ * reading's EOS.  crops->data may be device or host memory: host crops are staged per super-chunk, so the staging
+ * buffer holds at most max_batch crops of pass 1 or the floor(max_batch / (R - 1)) largest crops; crops->rotations must
+ * be NULL.  class_mask (DEVICE rows) and attn_maps as in parseq_forward_crops; each pass-2 reading uses its crop's mask
+ * row.  Every argument is checked on the host before anything is enqueued (PARSEQ_ERR_INVALID_ARG; the orientations and
+ * outputs also without a handle); max_batch must be >= R - 1. */
+typedef struct parseq_orient_args {
+  int32_t num_orientations;   /* R, 1..4 */
+  int32_t orientations[4];    /* o_0 .. o_{R-1} */
+  float min_confidence;       /* t, or NaN for none */
+  int32_t* rotation_out;      /* DEVICE int32 [N] */
+  float* confidence_out;      /* DEVICE fp32 [N] */
+} parseq_orient_args;
+int parseq_forward_crops_oriented(parseq_engine* e, const parseq_forward_args* args, const parseq_crops* crops,
+                                  const parseq_orient_args* orient, float* logits, int32_t* ids, int32_t* steps,
+                                  parseq_stream_t stream);
 /* Candidate scoring: the log-likelihood of given labels for each image, e.g. to pick the best word of a lexicon.
  * PARSeq: score(x, c) = sum_{i=0..n} log_softmax(head(decode(tgt_in, memory, content_mask, query_mask)))[i, t_i] with
  * tgt_in = [BOS, c_1..c_n] (Tokenizer.encode, strhub/data/utils.py:113-118, without its last column), the targets
@@ -299,7 +338,8 @@ int parseq_bench_tma_stream(void* buf, int64_t bytes, int cluster, int ctas, int
  * kernel runs on, 0 before its first launch, also with e = NULL for the bare kernel exports; "beam_bytes": device bytes of
  * the beam-search buffers, 0 until the first parseq_beam_search call; process-wide, also with e = NULL:
  * "live_device_bytes" and "live_cuda_objects", the device bytes and the streams, events and graph execs that every live
- * handle and lexicon holds); -1 if unknown. */
+ * handle and lexicon holds); "orient_rereads": the crops pass 2 of the last parseq_forward_crops_oriented call re-read,
+ * and "orient_readings": the readings it ran, padding included; -1 if unknown. */
 int64_t parseq_debug_int(parseq_engine* e, const char* name);
 /* Options: "max_batch" (images per super-chunk = one CUDA graph), "chunk" (images per encoder pass inside a
  * super-chunk), "dec_chunk" (images per decoder chain; the chains of a super-chunk run concurrently on their own
@@ -323,7 +363,8 @@ int parseq_set_option(parseq_engine* e, const char* name, int64_t value);
  * 6 encoder residual GEMM fused with LayerNorm, 7 persistent AR-loop kernel, 8 scoring tail (head GEMM with the log-sum-exp
  * epilogue and the per-candidate reduce of parseq_score), 9 beam selection (the selection kernel and, at dec_depth >= 2,
  * the K/V cache gather of parseq_beam_search), 10 cross-attention maps (the maps kernel of parseq_forward_args.attn_maps;
- * the AR-only map pass's other kernels count in their own categories). */
+ * the AR-only map pass's other kernels count in their own categories), 11 orientation search (the confidence and
+ * select kernels and the pass-2 allowlist gather of parseq_forward_crops_oriented). */
 int parseq_get_timing(parseq_engine* e, int category, double* ms, double* flops, int64_t* count);
 /* Debug: after a forward with option "ar_prof"=1, copies the [32 steps][16 slots] globaltimer (ns) stamps that block 0 of
  * the persistent AR kernel recorded at its phase boundaries.  Row 26 holds extra stamps of step 1 of the cluster kernel;

@@ -5,10 +5,12 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <mutex>
 #include <set>
@@ -26,6 +28,7 @@
 #include "attn_wgmma.cuh"
 #include "qkv_attn.cuh"
 #include "crops.cuh"
+#include "orient.cuh"
 #include "owners.h"
 
 namespace {
@@ -668,6 +671,10 @@ struct Workspace {
   DevBuf<float2> sc_vt_part;
   long long beam_bytes = 0;         // device bytes of the beam-search buffers (0 until the first beam call)
   DevBuf<int> lex_roots;            // the lexicon call's roots (grown on demand)
+  // orientation search (parseq_forward_crops_oriented), allocated by the first oriented call: the crop of each pass-2
+  // reading of a super-chunk [max_batch], the readings' confidences [max_batch], and the running step count of the call
+  DevBuf<int> or_rd, or_steps;
+  DevBuf<float> or_conf;
 };
 
 }  // namespace
@@ -725,6 +732,7 @@ struct parseq_engine : Workspace {
   long long crop_base = 0;
   DevBuf<uint8_t> crop_stage;
   bool use_graph = true;
+  long long orient_rereads = 0, orient_readings = 0;   // pass 2 of the last oriented call: crops re-read, readings run
   struct GraphEntry { GraphExec exec; long long kernels; };
   std::map<std::vector<int>, GraphEntry> graphs;   // last member: destroyed first
 
@@ -867,9 +875,9 @@ void free_workspace(parseq_engine* e) {
 // categories: 0 encoder GEMM, 1 encoder attention, 2 LayerNorm, 3 decoder GEMM, 4 decoder attention, 5 other,
 // 6 encoder residual GEMM + LayerNorm, 7 AR-loop kernel, 8 scoring tail (head GEMM with the LSE epilogue + reduce),
 // 9 beam selection (beam_select_kernel and the K/V gather of parseq_beam_search), 10 cross-attention maps
-// (dec_cross_attn_maps_kernel)
+// (dec_cross_attn_maps_kernel), 11 orientation search (orient.cuh: confidence, select, pass-2 allowlist gather)
 enum { CAT_ENC_GEMM = 0, CAT_ENC_ATTN = 1, CAT_LN = 2, CAT_DEC_GEMM = 3, CAT_DEC_ATTN = 4, CAT_MISC = 5, CAT_ENC_GEMM_LN = 6, CAT_DEC_AR = 7,
-       CAT_SCORE = 8, CAT_BEAM = 9, CAT_MAPS = 10, CAT_COUNT = 11 };
+       CAT_SCORE = 8, CAT_BEAM = 9, CAT_MAPS = 10, CAT_ORIENT = 11, CAT_COUNT = 12 };
 
 Event pool_event(parseq_engine* e) {
   if (!e->event_pool.empty()) { Event ev = std::move(e->event_pool.back()); e->event_pool.pop_back(); return ev; }
@@ -1750,6 +1758,10 @@ struct CropBatch {
   bool host;                        // c->data is host memory: each super-chunk's bytes are staged in e->crop_stage
 };
 
+bool valid_rotation(int r) { return r == 0 || r == 90 || r == 180 || r == 270; }
+// Crop i's rotation: its own (rotations) or the call's
+int crop_rot(const parseq_crops* c, int i) { return c->rotations != nullptr ? c->rotations[i] : c->rotation; }
+
 // The crop metadata, on the host alone (no handle or device needed).  These checks, and check_crop_smem, run before
 // the first launch of a call: on failure nothing is enqueued.
 int check_crops(int batch, const parseq_crops* c) {
@@ -1757,9 +1769,12 @@ int check_crops(int batch, const parseq_crops* c) {
   if (batch == 0) return PARSEQ_OK;
   if (c->data == nullptr || c->offsets == nullptr || c->sizes == nullptr)
     return fail(PARSEQ_ERR_INVALID_ARG, "null crop data, offsets or sizes");
-  if (c->rotation != 0 && c->rotation != 90 && c->rotation != 180 && c->rotation != 270)
+  if (c->rotations == nullptr && !valid_rotation(c->rotation))
     return fail(PARSEQ_ERR_INVALID_ARG, "rotation must be 0, 90, 180 or 270");
   for (int i = 0; i < batch; ++i) {
+    if (c->rotations != nullptr && !valid_rotation(c->rotations[i]))
+      return fail(PARSEQ_ERR_INVALID_ARG, "crop " + std::to_string(i) + ": rotation must be 0, 90, 180 or 270, got " +
+                                              std::to_string(c->rotations[i]));
     const int h = c->sizes[2 * i], w = c->sizes[2 * i + 1];
     if (h < 1 || w < 1 || h > pq::CROP_MAX_SIDE || w > pq::CROP_MAX_SIDE)
       return fail(PARSEQ_ERR_INVALID_ARG, "crop " + std::to_string(i) + ": size " + std::to_string(h) + " x " +
@@ -1774,21 +1789,21 @@ int check_crops(int batch, const parseq_crops* c) {
 int check_crop_smem(const parseq_engine* e, int batch, const parseq_crops* c) {
   int optin = 0;
   PQ_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, e->cfg.device));
-  const bool turn = c->rotation == 90 || c->rotation == 270;
   for (int i = 0; i < batch; ++i) {
     const int h = c->sizes[2 * i], w = c->sizes[2 * i + 1];
+    const bool turn = crop_rot(c, i) == 90 || crop_rot(c, i) == 270;
     if (4ll * pq::crop_smem_ints(turn ? w : h, turn ? h : w, e->cfg.img_h, e->cfg.img_w) > optin)
       return fail(PARSEQ_ERR_UNSUPPORTED, "crop " + std::to_string(i) + ": resize tables exceed shared memory at this img_size");
   }
   return PARSEQ_OK;
 }
 
-// Crop i as the kernel reads it, rotated counter-clockwise by c->rotation (np.rot90(crop, rotation / 90)), its bytes
-// at data + offsets[i] - base.
-pq::CropDesc crop_desc(const parseq_crops* c, int i, long long base) {
+// Crop i as the kernel reads it, rotated counter-clockwise by `rot` (np.rot90(crop, rot / 90)), its bytes at
+// data + offsets[i] - base.
+pq::CropDesc crop_desc(const parseq_crops* c, int i, long long base, int rot) {
   const int h = c->sizes[2 * i], w = c->sizes[2 * i + 1], row = 3 * w;
   const long long o = c->offsets[i] - base;
-  switch (c->rotation) {
+  switch (rot) {
     case 90: return pq::CropDesc{o + 3ll * (w - 1), -3, row, w, h};
     case 180: return pq::CropDesc{o + 1ll * row * (h - 1) + 3ll * (w - 1), -row, -3, h, w};
     case 270: return pq::CropDesc{o + 1ll * row * (h - 1), 3, -row, w, h};
@@ -1826,7 +1841,7 @@ int crops_table(parseq_engine* e, const CropBatch& cb, int b0, int Bc, cudaStrea
   if (cb.host) crop_range(cb.c, b0, b0 + Bc, &lo, &hi);
   e->crop_base = lo;
   e->crop_descs.resize(static_cast<size_t>(Bc));
-  for (int i = 0; i < Bc; ++i) e->crop_descs[static_cast<size_t>(i)] = crop_desc(cb.c, b0 + i, lo);
+  for (int i = 0; i < Bc; ++i) e->crop_descs[static_cast<size_t>(i)] = crop_desc(cb.c, b0 + i, lo, crop_rot(cb.c, b0 + i));
   // pageable source: the call returns once the table is staged, so crop_descs may change afterwards
   PQ_CUDA(cudaMemcpyAsync(e->crop_tab, e->crop_descs.data(), sizeof(pq::CropDesc) * Bc, cudaMemcpyHostToDevice, st));
   return PARSEQ_OK;
@@ -2012,6 +2027,145 @@ int forward_call(parseq_engine* e, const parseq_forward_args* a, const void* ima
   PQ_TRY(forward_impl(e, a, images, logits, ids, steps, reinterpret_cast<cudaStream_t>(stream), host, u8));
   if (host) PQ_CUDA(cudaStreamSynchronize(e->main));
   return PARSEQ_OK;
+}
+
+// ---------------------------------------------------------------- orientation search (parseq_forward_crops_oriented)
+// The orientation arguments, on the host alone (no handle or device needed).
+int check_orient(const parseq_orient_args* o) {
+  if (o == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  const int R = o->num_orientations;
+  if (R < 1 || R > 4) return fail(PARSEQ_ERR_INVALID_ARG, "num_orientations must be in [1, 4], got " + std::to_string(R));
+  for (int r = 0; r < R; ++r) {
+    if (!valid_rotation(o->orientations[r]))
+      return fail(PARSEQ_ERR_INVALID_ARG, "orientations must be 0, 90, 180 or 270, got " + std::to_string(o->orientations[r]));
+    for (int q = 0; q < r; ++q)
+      if (o->orientations[q] == o->orientations[r])
+        return fail(PARSEQ_ERR_INVALID_ARG, "orientations must be distinct, " + std::to_string(o->orientations[r]) + " repeats");
+  }
+  if (o->rotation_out == nullptr || o->confidence_out == nullptr)
+    return fail(PARSEQ_ERR_INVALID_ARG, "null rotation_out or confidence_out");
+  return PARSEQ_OK;
+}
+
+// Pass 1 over all crops at o_0 (forward_impl), the confidence kernel, the list of crops to re-read (with a threshold:
+// after the call's one host synchronisation), then pass 2 in super-chunks of whole crops, each followed by the select
+// kernel.  `c`: the crops at rotation o_0; `host`: their bytes are in host memory, staged in e->crop_stage per pass-1
+// super-chunk and per pass-2 super-chunk (which packs its listed crops one after another).
+int orient_impl(parseq_engine* e, const parseq_forward_args* a, const parseq_crops& c, bool host, const parseq_orient_args* o,
+                float* logits, int32_t* ids, int32_t* steps, cudaStream_t user) {
+  const int N = a->batch, R = o->num_orientations, R1 = R - 1;
+  const int L = num_steps_of(e, a->max_length);
+  const bool testing = a->max_length < 0;
+  // the rows past the step count are dropped with the shape (forward returns [N, S, C]) only here
+  const bool zero_tail = testing && a->decode_ar && a->refine_iters == 0 && e->arch == 0;
+  float* const maps = a->attn_maps;
+  PQ_TRY(e->or_rd.reserve(e->max_batch));
+  PQ_TRY(e->or_steps.reserve(1));
+  PQ_TRY(e->or_conf.reserve(e->max_batch));
+  const CropBatch cb{&c, host};
+  PQ_TRY(forward_impl(e, a, nullptr, logits, ids, nullptr, user, false, true, &cb));
+  PQ_TRY(enter_main(e, user));
+  {
+    TimedScope ts(e, e->main, CAT_ORIENT, 0.0);
+    PQ_TRY(launch_ex(LaunchConfig(dim3(N), dim3(pq::ORIENT_THREADS), 0, e->main, 0, false), pq::orient_init_kernel, logits,
+                     static_cast<int*>(ids), maps, L, e->C, e->T, o->orientations[0], static_cast<const int*>(e->out_steps),
+                     zero_tail, static_cast<int*>(e->or_steps), static_cast<int*>(o->rotation_out), o->confidence_out));
+  }
+  std::vector<int> list;
+  if (R > 1) {
+    if (std::isnan(o->min_confidence)) {
+      list.resize(static_cast<size_t>(N));
+      for (int b = 0; b < N; ++b) list[static_cast<size_t>(b)] = b;
+    } else {
+      std::vector<float> c0(static_cast<size_t>(N));
+      PQ_CUDA(cudaMemcpyAsync(c0.data(), o->confidence_out, 4ull * N, cudaMemcpyDeviceToHost, e->main));
+      PQ_CUDA(cudaStreamSynchronize(e->main));
+      for (int b = 0; b < N; ++b)
+        if (!(c0[static_cast<size_t>(b)] >= o->min_confidence)) list.push_back(b);
+    }
+  }
+  e->orient_rereads = static_cast<long long>(list.size());
+  e->orient_readings = 0;
+  const bool eager = !e->use_graph || e->timing;
+  pq::OrientList rest{{0, 0, 0, 0}};
+  for (int r = 1; r < R; ++r) rest.o[r - 1] = o->orientations[r];
+  const int per = R1 > 0 ? e->max_batch / R1 : 0;        // whole crops per pass-2 super-chunk
+  std::vector<int> rd;
+  std::vector<int64_t> poff;
+  std::vector<int32_t> psz;
+  for (size_t k0 = 0; k0 < list.size(); k0 += static_cast<size_t>(per)) {
+    const int nk = static_cast<int>(std::min(list.size() - k0, static_cast<size_t>(per)));
+    const int n = nk * R1;
+    int nb = 1;                                            // a power of two (or max_batch): few distinct graphs
+    while (nb < n) nb <<= 1;
+    nb = std::min(nb, e->max_batch);
+    e->orient_readings += nb;
+    rd.resize(static_cast<size_t>(nb));
+    e->crop_descs.resize(static_cast<size_t>(nb));
+    e->crop_base = 0;
+    parseq_crops pc = c;                                   // the crops the super-chunk's table points into
+    if (host) {
+      poff.resize(static_cast<size_t>(nk));
+      psz.resize(2 * static_cast<size_t>(nk));
+      long long off = 0;
+      for (int k = 0; k < nk; ++k) {
+        const int b = list[k0 + static_cast<size_t>(k)];
+        const long long bytes = 3ll * c.sizes[2 * b] * c.sizes[2 * b + 1];
+        PQ_CUDA(cudaMemcpyAsync(e->crop_stage + off, c.data + c.offsets[b], static_cast<size_t>(bytes), cudaMemcpyHostToDevice,
+                                e->main));
+        poff[static_cast<size_t>(k)] = off;
+        psz[2 * static_cast<size_t>(k)] = c.sizes[2 * b];
+        psz[2 * static_cast<size_t>(k) + 1] = c.sizes[2 * b + 1];
+        off += bytes;
+      }
+      pc.data = e->crop_stage;
+      pc.data_bytes = off;
+      pc.offsets = poff.data();
+      pc.sizes = psz.data();
+    }
+    for (int j = 0; j < nb; ++j) {
+      const int jj = std::min(j, n - 1);                   // padding: copies of the last reading
+      const int k = jj / R1;
+      const int b = list[k0 + static_cast<size_t>(k)];
+      rd[static_cast<size_t>(j)] = b;
+      e->crop_descs[static_cast<size_t>(j)] = crop_desc(&pc, host ? k : b, 0, rest.o[jj % R1]);
+    }
+    // pageable sources: the calls return once the tables are staged, so rd and crop_descs may change afterwards
+    PQ_CUDA(cudaMemcpyAsync(e->or_rd, rd.data(), 4ull * nb, cudaMemcpyHostToDevice, e->main));
+    PQ_CUDA(cudaMemcpyAsync(e->crop_tab, e->crop_descs.data(), sizeof(pq::CropDesc) * nb, cudaMemcpyHostToDevice, e->main));
+    PQ_TRY(launch_k(e->lo, pq::set_int_kernel, dim3(1), dim3(32), 0, e->main, static_cast<int*>(e->out_steps),
+                    (testing && a->decode_ar && e->arch == 0) ? 0 : L));
+    e->launches++;
+    PQ_TRY(crops_resize(e, CropBatch{&pc, false}, 0, 0, nb, e->in_images_u8, e->main));
+    if (a->class_mask != nullptr) {
+      TimedScope ts(e, e->main, CAT_ORIENT, 0.0);
+      PQ_TRY(launch_ex(LaunchConfig(dim3((nb * e->mask_ld + 255) / 256), dim3(256), 0, e->main, 0, false),
+                       pq::gather_rows_kernel, a->class_mask, static_cast<const int*>(e->or_rd), nb, e->mask_ld,
+                       static_cast<uint32_t*>(e->in_mask)));
+    }
+    parseq_forward_args a2 = *a;
+    a2.batch = nb;
+    if (eager) {
+      PQ_TRY(forward_super(e, &a2, 0, nb, L, e->in_images_u8, true, e->out_logits, e->out_ids, e->out_steps,
+                           a->class_mask ? e->in_mask.get() : nullptr, maps ? e->out_maps.get() : nullptr));
+    } else {
+      PQ_TRY(run_graph(e, &a2, nb, L, true));
+    }
+    {
+      TimedScope ts(e, e->main, CAT_ORIENT, 0.0);
+      PQ_TRY(launch_ex(LaunchConfig(dim3(n), dim3(pq::ORIENT_THREADS), 0, e->main, 0, false), pq::orient_conf_kernel,
+                       static_cast<const float*>(e->out_logits), L, e->C, static_cast<float*>(e->or_conf)));
+    }
+    TimedScope ts(e, e->main, CAT_ORIENT, 0.0);
+    PQ_TRY(launch_ex(LaunchConfig(dim3(nk), dim3(pq::ORIENT_THREADS), 0, e->main, 0, false), pq::orient_select_kernel,
+                     static_cast<const float*>(e->out_logits), static_cast<const int*>(e->out_ids),
+                     static_cast<const float*>(maps ? e->out_maps.get() : nullptr), static_cast<const float*>(e->or_conf),
+                     static_cast<const int*>(e->or_rd), R1, rest, L, e->C, e->T, static_cast<const int*>(e->out_steps), zero_tail,
+                     static_cast<int*>(e->or_steps), logits, static_cast<int*>(ids), maps,
+                     static_cast<int*>(o->rotation_out), o->confidence_out));
+  }
+  if (steps) PQ_CUDA(cudaMemcpyAsync(steps, e->or_steps, 4, cudaMemcpyDeviceToDevice, e->main));
+  return leave_main(e, user);
 }
 
 // ---------------------------------------------------------------- candidate scoring (parseq_score)
@@ -2752,6 +2906,52 @@ int parseq_forward_host_crops(parseq_engine* e, const parseq_forward_args* a, co
   return PARSEQ_OK;
 }
 
+int parseq_forward_crops_oriented(parseq_engine* e, const parseq_forward_args* a, const parseq_crops* crops,
+                                  const parseq_orient_args* o, float* logits, int32_t* ids, int32_t* steps,
+                                  parseq_stream_t stream) {
+  PQ_TRY(check_orient(o));
+  if (crops == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  if (crops->rotations != nullptr)
+    return fail(PARSEQ_ERR_INVALID_ARG, "rotations must be NULL: the oriented call chooses each crop's rotation");
+  parseq_crops c = *crops;
+  c.rotation = o->orientations[0];
+  PQ_TRY(check_crops_call(e, a, &c, logits));
+  const int R = o->num_orientations;
+  if (e->max_batch < R - 1)
+    return fail(PARSEQ_ERR_INVALID_ARG, "max_batch (" + std::to_string(e->max_batch) + ") must be >= num_orientations - 1 (" +
+                                            std::to_string(R - 1) + "): a crop's readings share one super-chunk");
+  if (a->attn_maps != nullptr && e->arch != 0)
+    return fail(PARSEQ_ERR_UNSUPPORTED, "attn_maps: ViTSTR has no decoder cross-attention");
+  for (int r = 1; r < R; ++r) {
+    parseq_crops cr = c;
+    cr.rotation = o->orientations[r];
+    PQ_TRY(check_crop_smem(e, a->batch, &cr));
+  }
+  if (a->batch == 0) return PARSEQ_OK;
+  PQ_CUDA(cudaSetDevice(e->cfg.device));
+  const cudaStream_t user = reinterpret_cast<cudaStream_t>(stream);
+  cudaPointerAttributes pa{};
+  const bool on_device = cudaPointerGetAttributes(&pa, c.data) == cudaSuccess &&
+                         (pa.type == cudaMemoryTypeDevice || pa.type == cudaMemoryTypeManaged);
+  cudaGetLastError();
+  if (!on_device) {
+    // host crops: the staging buffer holds one super-chunk's bytes at a time - pass 1's span of max_batch crops, or the
+    // listed crops of a pass-2 super-chunk, at most the floor(max_batch / (R - 1)) largest crops
+    const CropBatch cb{&c, true};
+    PQ_TRY(crops_reserve(e, cb, a->batch));
+    if (R > 1) {
+      std::vector<long long> bytes(static_cast<size_t>(a->batch));
+      for (int i = 0; i < a->batch; ++i) bytes[static_cast<size_t>(i)] = 3ll * c.sizes[2 * i] * c.sizes[2 * i + 1];
+      const size_t per = std::min(bytes.size(), static_cast<size_t>(e->max_batch / (R - 1)));
+      std::partial_sort(bytes.begin(), bytes.begin() + static_cast<long>(per), bytes.end(), std::greater<long long>());
+      long long need = 0;
+      for (size_t i = 0; i < per; ++i) need += bytes[i];
+      PQ_TRY(e->crop_stage.grow(e, need));
+    }
+  }
+  return orient_impl(e, a, c, !on_device, o, logits, ids, steps, user);
+}
+
 int parseq_score_check(const parseq_config* cfg, const parseq_score_args* a) {
   if (cfg == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
   return check_score(a, cfg->max_label_length, cfg->num_tokens - 2);
@@ -2985,6 +3185,8 @@ int64_t parseq_debug_int(parseq_engine* e, const char* name) {
   if (n == "ar_last_path") return e->ar_last_path;
   if (n == "sm_count") return e->lo.sm_count;
   if (n == "beam_bytes") return e->beam_bytes;
+  if (n == "orient_rereads") return e->orient_rereads;
+  if (n == "orient_readings") return e->orient_readings;
   return -1;
 }
 int64_t parseq_kernel_launches(const parseq_engine* e) { return e ? e->launches : 0; }

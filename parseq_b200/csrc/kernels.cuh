@@ -1423,6 +1423,29 @@ __global__ void __launch_bounds__(384) dec_ln_head_argmax_kernel(
 }
 
 // ---------------------------------------------------------------------------------------------
+// row_max_prob_warp: the max softmax probability of one row (NaN where its maximum is not finite) and its id, the same
+// bits in every lane of the warp (the butterfly sums are commutative).  The confidence is the product of these factors in
+// row order through the first EOS; orient.cuh computes the rows of one image on several warps and multiplies the same
+// factors in the same order.
+__device__ __forceinline__ float row_max_prob_warp(const float* __restrict__ row, int C, int* id) {
+  const int lane = threadIdx.x & 31;
+  float best = -INFINITY;
+  int bi = ARGMAX_NONE;
+  for (int j = lane; j < C; j += 32) argmax_scan(best, bi, row[j], j);
+  bi = argmax_finish(best, bi, row, C, lane);
+  best = row[bi];
+  // torch's softmax of a row whose maximum is not finite (it holds a NaN or a +inf, or is all -inf) is all NaN, and
+  // max() over it gives index 0 with probability NaN
+  const bool finite = isfinite(best);
+  float se = 0.f;
+  if (finite)
+    for (int j = lane; j < C; j += 32) se += expf(row[j] - best);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
+  *id = finite ? bi : 0;
+  return finite ? 1.0f / se : __int_as_float(0x7fc00000);
+}
+
 // Fused post-processing of the reference's test path (strhub/models/base.py:132-142 + Tokenizer._filter,
 // strhub/data/utils.py:120-129): per image  ids[i] = argmax_c logits[i, c]  (first maximum),  length = index of the
 // first EOS (L if none),  confidence = prod_{i <= min(length, L-1)} max_c softmax(logits[i])_c  (the EOS probability is
@@ -1437,24 +1460,11 @@ __global__ void postprocess_kernel(const float* __restrict__ logits, int B, int 
   int len = L;
   bool done = false;
   for (int i = 0; i < L; ++i) {
-    const float* row = logits + (static_cast<long long>(b) * L + i) * C;
-    float best = -INFINITY;
-    int bi = ARGMAX_NONE;
-    for (int j = lane; j < C; j += 32) argmax_scan(best, bi, row[j], j);
-    bi = argmax_finish(best, bi, row, C, lane);
-    best = row[bi];
-    // torch's softmax of a row whose maximum is not finite (it holds a NaN or a +inf, or is all -inf) is all NaN, and
-    // max() over it gives index 0 with probability NaN
-    const bool finite = isfinite(best);
-    float se = 0.f;
-    if (finite)
-      for (int j = lane; j < C; j += 32) se += expf(row[j] - best);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
-    const int id = finite ? bi : 0;
+    int id;
+    const float p = row_max_prob_warp(logits + (static_cast<long long>(b) * L + i) * C, C, &id);
     if (lane == 0) ids[static_cast<long long>(b) * L + i] = id;
     if (!done) {
-      conf *= finite ? 1.0f / se : __int_as_float(0x7fc00000);   // max softmax probability of position i
+      conf *= p;                    // max softmax probability of position i
       if (id == eos_id) { len = i; done = true; }
     }
   }

@@ -26,7 +26,19 @@ class ForwardArgsC(C.Structure):
 
 class CropsC(C.Structure):
     _fields_ = [("data", C.c_void_p), ("data_bytes", C.c_int64), ("offsets", C.c_void_p), ("sizes", C.c_void_p),
-                ("rotation", C.c_int32)]
+                ("rotation", C.c_int32), ("rotations", C.c_void_p)]
+
+
+class OrientArgsC(C.Structure):
+    _fields_ = [("num_orientations", C.c_int32), ("orientations", C.c_int32 * 4), ("min_confidence", C.c_float),
+                ("rotation_out", C.c_void_p), ("confidence_out", C.c_void_p)]
+
+
+def orient_args(orientations, min_confidence, rotation_ptr, confidence_ptr) -> OrientArgsC:
+    """parseq_orient_args: up to four orientations, min_confidence None for none (NaN)."""
+    o = list(orientations)
+    return OrientArgsC(len(o), (C.c_int32 * 4)(*(o + [0] * (4 - len(o)))[:4]),
+                       float("nan") if min_confidence is None else float(min_confidence), rotation_ptr, confidence_ptr)
 
 
 class ScoreArgsC(C.Structure):
@@ -80,7 +92,7 @@ class LexiconHandle:
 EXPORTS = [
     "parseq_create", "parseq_destroy", "parseq_set_weight", "parseq_num_weights", "parseq_weight_key",
     "parseq_finalize", "parseq_forward", "parseq_forward_host", "parseq_forward_u8", "parseq_forward_host_u8",
-    "parseq_resize_crops", "parseq_forward_crops", "parseq_forward_host_crops",
+    "parseq_resize_crops", "parseq_forward_crops", "parseq_forward_host_crops", "parseq_forward_crops_oriented",
     "parseq_score", "parseq_score_u8", "parseq_score_check", "parseq_beam_search", "parseq_beam_search_u8",
     "parseq_lexicon_check", "parseq_lexicon_create", "parseq_lexicon_destroy", "parseq_beam_search_lexicon",
     "parseq_beam_search_lexicon_u8",
@@ -124,6 +136,8 @@ def load_library(path: Optional[str] = None):
     lib.parseq_forward_crops.argtypes = [C.c_void_p, C.POINTER(ForwardArgsC), C.POINTER(CropsC), C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p]
     lib.parseq_forward_host_crops.argtypes = lib.parseq_forward_crops.argtypes
+    lib.parseq_forward_crops_oriented.argtypes = [C.c_void_p, C.POINTER(ForwardArgsC), C.POINTER(CropsC),
+                                                  C.POINTER(OrientArgsC), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.parseq_score.argtypes = [C.c_void_p, C.POINTER(ScoreArgsC), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.parseq_score_u8.argtypes = lib.parseq_score.argtypes
     lib.parseq_score_check.argtypes = [C.POINTER(ParseqConfigC), C.POINTER(ScoreArgsC)]
@@ -237,7 +251,7 @@ class Engine:
         check(self.lib, self.lib.parseq_set_option(self.handle, name.encode(), int(value)))
 
     TIMING_CATEGORIES = ("enc_gemm", "enc_attn", "layernorm", "dec_gemm", "dec_attn", "other", "enc_gemm_ln", "dec_ar",
-                         "score_tail", "beam_select", "attn_maps")
+                         "score_tail", "beam_select", "attn_maps", "orient")
 
     def get_timing(self):
         out = {}
@@ -299,6 +313,16 @@ class Engine:
         a = self._args(batch, max_length, decode_ar, refine_iters, class_mask=class_mask_ptr, attn_maps=attn_maps_ptr)
         fn = self.lib.parseq_forward_host_crops if host else self.lib.parseq_forward_crops
         check(self.lib, fn(self.handle, C.byref(a), C.byref(crops), logits_ptr, ids_ptr, steps_ptr, stream))
+
+    # orientation search (parseq_forward_crops_oriented): crops in device or host memory, every output on the device;
+    # rotation_ptr int32 [batch] / confidence_ptr fp32 [batch] the chosen orientation and its confidence
+    def forward_crops_oriented(self, crops: CropsC, batch, orientations, min_confidence, logits_ptr, ids_ptr, steps_ptr,
+                               rotation_ptr, confidence_ptr, stream, max_length=None, decode_ar=True, refine_iters=1,
+                               class_mask_ptr=None, attn_maps_ptr=None):
+        a = self._args(batch, max_length, decode_ar, refine_iters, class_mask=class_mask_ptr, attn_maps=attn_maps_ptr)
+        o = orient_args(orientations, min_confidence, rotation_ptr, confidence_ptr)
+        check(self.lib, self.lib.parseq_forward_crops_oriented(self.handle, C.byref(a), C.byref(crops), C.byref(o),
+                                                               logits_ptr, ids_ptr, steps_ptr, stream))
 
     # per_image / targets / lengths: CPU int32 tensors (parseq_score_args); scores / token_lp: device pointers
     def score(self, images_ptr, batch, per_image, targets, lengths, scores_ptr, token_lp_ptr, stream, u8=False):

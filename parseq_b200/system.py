@@ -12,6 +12,7 @@ fallback: calling forward with non-CUDA tensors raises.
 from __future__ import annotations
 
 import math
+import numbers
 from dataclasses import dataclass
 from types import SimpleNamespace
 from typing import Any, Dict, List, Optional, Sequence, Tuple, Union
@@ -190,8 +191,53 @@ def _ptr(t: Optional[Tensor]):
     return t.data_ptr() if t is not None else None
 
 
-def _crops_c(data: Tensor, offsets: Tensor, sizes: Tensor, rotation: int) -> CropsC:
-    return CropsC(data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), int(rotation))
+def _crops_c(data: Tensor, offsets: Tensor, sizes: Tensor, rotation: int, *, rotations: Optional[Tensor] = None) -> CropsC:
+    """parseq_crops of packed crops; `rotations`: CPU int32 [N], each crop's own rotation (kept alive by the result)."""
+    c = CropsC(data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), int(rotation), _ptr(rotations))
+    c._rotations = rotations
+    return c
+
+
+Rotation = Union[int, Sequence[int]]
+ORIENTATIONS = (0, 90, 180, 270)
+
+
+def _is_rotation_list(rotation: Rotation) -> bool:
+    """A sequence of per-crop rotations, as opposed to one number (an int, a numpy scalar, a 0-d array or tensor)."""
+    if getattr(rotation, "ndim", None) == 0:
+        return False
+    return isinstance(rotation, (list, tuple, Tensor)) or hasattr(rotation, "__len__")
+
+
+def _crop_rotations(rotation: Rotation, n: int) -> Tuple[int, Optional[Tensor]]:
+    """`rotation=` of a call on raw crops: one int for every crop, or a sequence of n ints, one per crop -> the
+    parseq_crops (rotation, rotations) pair (rotations a CPU int32 [n] tensor, or None)."""
+    if not _is_rotation_list(rotation):
+        return int(rotation), None
+    r = [int(x) for x in (rotation.tolist() if isinstance(rotation, Tensor) else rotation)]
+    if len(r) != n:
+        raise ValueError(f"rotation must be an int or a sequence of one int per crop ({n}), got {len(r)} values")
+    return 0, torch.tensor(r, dtype=torch.int32)
+
+
+def _rotation_of(rotation: Rotation, b: int) -> int:
+    """Crop b's rotation of a `rotation=` argument."""
+    if not _is_rotation_list(rotation):
+        return int(rotation)
+    return int(rotation[b])
+
+
+def _reject_tensor_rotation(rotation: Rotation):
+    if _is_rotation_list(rotation) or rotation:
+        raise ValueError("rotation applies to lists of raw crops; a tensor input is already at img_size")
+
+
+def check_orientations(orientations: Sequence[int]) -> Tuple[int, ...]:
+    """The orientations of an orientation search: 1 to 4 distinct values of 0, 90, 180, 270 (ValueError otherwise)."""
+    o = tuple(orientations)
+    if not 1 <= len(o) <= 4 or any(isinstance(x, bool) or x not in ORIENTATIONS for x in o) or len(set(o)) != len(o):
+        raise ValueError(f"orientations must be 1 to 4 distinct values of {ORIENTATIONS}, got {orientations!r}")
+    return tuple(int(x) for x in o)
 
 
 def _crop_hw(c) -> Tuple[int, int]:
@@ -423,9 +469,10 @@ class _EngineModule(nn.Module):
         eng.encode(img.data_ptr(), img.shape[0], mem.data_ptr(), torch.cuda.current_stream(img.device).cuda_stream)
         return mem
 
-    def preprocess(self, crops: Sequence[Any], rotation: int = 0) -> Tensor:
-        """CUDA uint8 [N, H, W, 3]: each crop rotated by `rotation` (counter-clockwise) and resized to img_size on the
-        device, byte-identical to the reference's Image.rotate(rotation, expand=True) + T.Resize(img_size, BICUBIC)."""
+    def preprocess(self, crops: Sequence[Any], rotation: Rotation = 0) -> Tensor:
+        """CUDA uint8 [N, H, W, 3]: each crop rotated by `rotation` (counter-clockwise; one int for every crop or one
+        per crop) and resized to img_size on the device, byte-identical to the reference's Image.rotate(rotation,
+        expand=True) + T.Resize(img_size, BICUBIC)."""
         eng = self.engine()
         dev = self._device
         data, offsets, sizes = pack_crops(crops, pin_memory=True)
@@ -434,12 +481,13 @@ class _EngineModule(nn.Module):
         data = data.to(dev, non_blocking=True)
         H, W = self.cfg.img_size
         out = torch.empty((len(crops), H, W, 3), dtype=torch.uint8, device=dev)
-        eng.resize_crops(_crops_c(data, offsets, sizes, rotation), len(crops), out.data_ptr(),
+        rot, rots = _crop_rotations(rotation, len(crops))
+        eng.resize_crops(_crops_c(data, offsets, sizes, rot, rotations=rots), len(crops), out.data_ptr(),
                          torch.cuda.current_stream(dev).cuda_stream)
         return out
 
     def score(self, images: Union[Tensor, List[Any]], targets: Tensor, lengths: Tensor, per_image: Tensor, *,
-              rotation: int = 0, return_token_logprobs: bool = False):
+              rotation: Rotation = 0, return_token_logprobs: bool = False):
         """Log-likelihoods of candidate labels (parseq_score): `targets` int32 [M, max_label_length + 1] (c_1..c_n, EOS),
         `lengths` [M], `per_image` [N] as pack_candidates makes them (CPU).  Returns fp32 scores [M] on the device, and
         with return_token_logprobs the per-position terms [M, max_label_length + 1] (0 past each label's EOS).
@@ -447,8 +495,8 @@ class _EngineModule(nn.Module):
         eng = self.engine()
         if isinstance(images, (list, tuple)):
             images = self.preprocess(images, rotation)
-        elif rotation:
-            raise ValueError("rotation applies to lists of raw crops; a tensor input is already at img_size")
+        else:
+            _reject_tensor_rotation(rotation)
         images = self._check_images(images)
         dev = images.device
         L = self.cfg.max_label_length + 1
@@ -468,7 +516,7 @@ class _EngineModule(nn.Module):
         return (scores, tlp) if return_token_logprobs else scores
 
     def beam_search(self, images: Union[Tensor, List[Any]], beam_width: int = 5, max_length: Optional[int] = None, *,
-                    rotation: int = 0, class_mask: Optional[Tensor] = None, lexicon: Optional[Lexicon] = None,
+                    rotation: Rotation = 0, class_mask: Optional[Tensor] = None, lexicon: Optional[Lexicon] = None,
                     roots: Optional[Tensor] = None):
         """Beam search (parseq_beam_search): the `beam_width` most likely readings of each image, best first, as raw
         (ids int32 [N, K, num_steps] = c_1..c_n then 0, lengths int32 [N, K] (-1: no hypothesis), scores fp32 [N, K]
@@ -493,8 +541,8 @@ class _EngineModule(nn.Module):
         eng = self.engine()
         if isinstance(images, (list, tuple)):
             images = self.preprocess(images, rotation)
-        elif rotation:
-            raise ValueError("rotation applies to lists of raw crops; a tensor input is already at img_size")
+        else:
+            _reject_tensor_rotation(rotation)
         images = self._check_images(images)
         dev = images.device
         N, K, S = images.shape[0], int(beam_width), eng.num_steps(max_length)
@@ -538,13 +586,14 @@ class _EngineModule(nn.Module):
                 if attn_maps else None)
         if class_mask is not None:
             class_mask = class_mask.pin_memory() if host else class_mask.to(dev, non_blocking=True)
-        eng.forward_crops(_crops_c(data, offsets, sizes, rotation), N, logits.data_ptr(), ids.data_ptr(), steps.data_ptr(),
+        rot, rots = _crop_rotations(rotation, N)
+        eng.forward_crops(_crops_c(data, offsets, sizes, rot, rotations=rots), N, logits.data_ptr(), ids.data_ptr(), steps.data_ptr(),
                           torch.cuda.current_stream(dev).cuda_stream, max_length, decode_ar, refine_iters, host=host,
                           class_mask_ptr=_mask_ptr(class_mask), attn_maps_ptr=_ptr(maps))
         return logits, ids, steps, maps
 
     def _run(self, images: Union[Tensor, List[Any]], max_length, decode_ar, refine_iters, forced_ids=None,
-             forced_refine=None, rotation: int = 0, class_mask: Optional[Tensor] = None, attn_maps: bool = False):
+             forced_refine=None, rotation: Rotation = 0, class_mask: Optional[Tensor] = None, attn_maps: bool = False):
         """(logits, ids, steps, maps) of one engine forward; maps is None unless attn_maps."""
         if class_mask is not None and (forced_ids is not None or forced_refine is not None):
             raise ValueError("an allowlist cannot be combined with teacher forcing")
@@ -554,8 +603,7 @@ class _EngineModule(nn.Module):
             if forced_ids is not None or forced_refine is not None:
                 raise ValueError("teacher forcing takes normalised float images")
             return self._run_crops(images, max_length, decode_ar, refine_iters, rotation, class_mask, attn_maps)
-        if rotation:
-            raise ValueError("rotation applies to lists of raw crops; a tensor input is already at img_size")
+        _reject_tensor_rotation(rotation)
         eng = self.engine()
         images = self._check_images(images)
         dev = images.device
@@ -580,6 +628,47 @@ class _EngineModule(nn.Module):
                         decode_ar, refine_iters, fi.data_ptr() if fi is not None else None,
                         fr.data_ptr() if fr is not None else None, _mask_ptr(class_mask), _ptr(maps))
         return logits, ids, steps, maps
+
+    def _run_oriented(self, crops, orientations, min_confidence, max_length, decode_ar, refine_iters, class_mask=None,
+                      attn_maps=False):
+        """Orientation search over raw crops (parseq_forward_crops_oriented): (logits, ids, steps, maps, rotation int32,
+        confidence fp32), on the device for CUDA crops and on the CPU for CPU crops; maps None unless attn_maps."""
+        if not isinstance(crops, (list, tuple)):
+            raise ValueError("orientation search takes a list of raw crops; a tensor input is already at img_size")
+        orientations = check_orientations(orientations)
+        if min_confidence is not None:
+            scalar = isinstance(min_confidence, numbers.Real) or getattr(min_confidence, "ndim", None) == 0
+            if isinstance(min_confidence, bool) or not scalar or getattr(min_confidence, "dtype", None) == torch.bool:
+                raise ValueError(f"min_confidence must be None or a real number, got {min_confidence!r}")
+            min_confidence = float(min_confidence)
+        mb = self._options.get("max_batch")
+        if mb is not None and 0 < mb < len(orientations) - 1:
+            raise ValueError(f"max_batch ({mb}) must be >= len(orientations) - 1 ({len(orientations) - 1}): a crop's "
+                             "readings share one super-chunk")
+        eng = self.engine()
+        dev = self._device
+        data, offsets, sizes = pack_crops(crops, pin_memory=True)
+        host = data.device.type != "cuda"
+        if not host and data.device != dev:
+            raise ValueError(f"crops are on {data.device}, the model on {dev}")
+        N = len(crops)
+        L = eng.num_steps(max_length)
+        logits = torch.empty((N, L, self.cfg.num_classes), dtype=torch.float32, device=dev)
+        ids = torch.empty((N, L), dtype=torch.int32, device=dev)
+        steps = torch.empty((1,), dtype=torch.int32, device=dev)
+        rotation = torch.empty((N,), dtype=torch.int32, device=dev)
+        confidence = torch.empty((N,), dtype=torch.float32, device=dev)
+        maps = torch.empty((N, L, self.cfg.enc_tokens), dtype=torch.float32, device=dev) if attn_maps else None
+        if class_mask is not None:
+            class_mask = class_mask.to(dev, non_blocking=True).contiguous()
+        eng.forward_crops_oriented(_crops_c(data, offsets, sizes, orientations[0]), N, orientations, min_confidence,
+                                   logits.data_ptr(), ids.data_ptr(), steps.data_ptr(), rotation.data_ptr(),
+                                   confidence.data_ptr(), torch.cuda.current_stream(dev).cuda_stream, max_length,
+                                   decode_ar, refine_iters, class_mask_ptr=_mask_ptr(class_mask), attn_maps_ptr=_ptr(maps))
+        out = (logits, ids, steps, maps, rotation, confidence)
+        if host:                       # the copies also wait for the call, which reads the pinned crop bytes
+            out = tuple(t.cpu() if t is not None else None for t in out)
+        return out
 
 
 class ParseqModel(_EngineModule):
@@ -641,7 +730,7 @@ class ParseqModel(_EngineModule):
 
     def forward(self, tokenizer: Tokenizer, images: Union[Tensor, List[Any]], max_length: Optional[int] = None,
                 return_ids: bool = False, forced_ids: Optional[Tensor] = None,
-                forced_refine: Optional[Tensor] = None, *, rotation: int = 0, class_mask: Optional[Tensor] = None):
+                forced_refine: Optional[Tensor] = None, *, rotation: Rotation = 0, class_mask: Optional[Tensor] = None):
         """`images`: normalised float [N, 3, H, W], uint8 [N, H, W, 3] at img_size, or a list of raw crops of any size
         (uint8 [h, w, 3] tensors, all CUDA or all CPU, or PIL images in mode RGB) that the engine rotates by `rotation`
         and resizes as the reference's test transform does.  `class_mask`: per-image allowlist words (allowlist_mask)."""
@@ -656,7 +745,7 @@ class ParseqModel(_EngineModule):
         return logits
 
     def forward_with_attention(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *,
-                               rotation: int = 0, class_mask: Optional[Tensor] = None):
+                               rotation: Rotation = 0, class_mask: Optional[Tensor] = None):
         """forward(tokenizer, images, max_length, return_ids=True) plus the cross-attention maps of the decoder's last
         layer (parseq_forward_args.attn_maps): (logits [N, S, C], ids [N, S], maps fp32 [N, S, T]), maps[b, i] the
         head-averaged weights over the T image tokens of the query that produced logits[b, i].  The logits and ids are
@@ -668,6 +757,22 @@ class ParseqModel(_EngineModule):
             logits, ids, maps = logits[:, :S], ids[:, :S], maps[:, :S]
         return logits, ids, maps
 
+    def read_oriented(self, crops: List[Any], orientations: Sequence[int] = ORIENTATIONS,
+                      min_confidence: Optional[float] = None, max_length: Optional[int] = None, *,
+                      class_mask: Optional[Tensor] = None, attn_maps: bool = False):
+        """Orientation search (parseq_forward_crops_oriented): each raw crop read at orientations[0] and, unless its
+        confidence is >= min_confidence, at the others too, keeping the most confident reading (ties to the earlier
+        orientation, NaN last).  (logits [N, S, C], ids [N, S], rotation int64 [N], confidence [N], maps [N, S, T] or
+        None); logits and ids as forward returns them, each crop's bit-identical to forward(rotation=rotation[b]) up to
+        its EOS."""
+        logits, ids, steps, maps, rot, conf = self._run_oriented(crops, orientations, min_confidence, max_length,
+                                                                 self.decode_ar, self.refine_iters, class_mask, attn_maps)
+        if max_length is None and self.decode_ar and not self.refine_iters:
+            S = int(steps.item())
+            logits, ids = logits[:, :S], ids[:, :S]
+            maps = maps[:, :S] if maps is not None else None
+        return logits, ids, rot.long(), conf, maps
+
 
 class VitstrModel(_EngineModule):
     """Mirror of `strhub.models.vitstr.model.ViTSTR` (vitstr/model.py:14-28): a timm ViT with class token whose head is
@@ -677,11 +782,20 @@ class VitstrModel(_EngineModule):
         return self._features(x)
 
     def forward_tokens(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, return_ids: bool = False,
-                       *, rotation: int = 0, class_mask: Optional[Tensor] = None):
+                       *, rotation: Rotation = 0, class_mask: Optional[Tensor] = None):
         """`self.forward(images, max_length + 2)[:, 1:]` (vitstr/system.py:65-71) in one engine call; `images` and
         `class_mask` as in ParseqModel.forward."""
         logits, ids, _, _ = self._run(images, max_length, False, 0, rotation=rotation, class_mask=class_mask)
         return (logits, ids) if return_ids else logits
+
+    def read_oriented(self, crops: List[Any], orientations: Sequence[int] = ORIENTATIONS,
+                      min_confidence: Optional[float] = None, max_length: Optional[int] = None, *,
+                      class_mask: Optional[Tensor] = None):
+        """ParseqModel.read_oriented over forward_tokens' logits: (logits, ids, rotation int64 [N], confidence [N],
+        None)."""
+        logits, ids, _, _, rot, conf = self._run_oriented(crops, orientations, min_confidence, max_length, False, 0,
+                                                          class_mask)
+        return logits, ids, rot.long(), conf, None
 
     def forward(self, x: Tensor, seqlen: int = 25) -> Tensor:
         raise NotImplementedError(
@@ -713,7 +827,7 @@ class _System(nn.Module):
     def device(self) -> torch.device:
         return self.model._device
 
-    def preprocess(self, crops: Sequence[Any], rotation: int = 0) -> Tensor:
+    def preprocess(self, crops: Sequence[Any], rotation: Rotation = 0) -> Tensor:
         """The reference's test transform up to the uint8 image (module.py:69-82: rotate, T.Resize(img_size, BICUBIC)) of
         a list of raw crops, on the device: CUDA uint8 [N, H, W, 3], what `forward` takes as a tensor."""
         return self.model.preprocess(crops, rotation)
@@ -738,7 +852,23 @@ class _System(nn.Module):
         labels = [self.tokenizer._ids2tok(row[:n], True) for row, n in zip(ids_h, len_h)]
         return labels, conf_h
 
-    def score(self, images: Union[Tensor, List[Any]], candidates: Candidates, *, rotation: int = 0,
+    def read_oriented(self, crops: List[Any], orientations: Sequence[int] = ORIENTATIONS,
+                      min_confidence: Optional[float] = None, max_length: Optional[int] = None,
+                      allowlist: Allowlist = None) -> Tuple[Tensor, Tensor, Tensor]:
+        """Reads each raw crop the right way up: (logits, rotation int64 [N], confidence fp32 [N]).  Every crop is
+        read at orientations[0]; a crop whose confidence (postprocess's) is below `min_confidence`, or every crop when
+        it is None, is also read at the other orientations (1 to 4 distinct values of 0, 90, 180, 270, counter-
+        clockwise as `rotation`) and keeps the reading of highest confidence: ties go to the earlier orientation, NaN
+        ranks below every number.  Each crop's logits are forward(rotation=rotation[b])'s up to its EOS (rows from the
+        step count of the pass that produced the reading are 0), and postprocess(logits) returns `confidence` exactly.
+        The search runs on the device; with min_confidence the engine synchronises once to list the crops to re-read.
+        CUDA crops give CUDA results, CPU crops CPU results."""
+        mask = self.allowlist_mask(allowlist, len(crops) if isinstance(crops, (list, tuple)) else crops.shape[0])
+        logits, _, rotation, confidence, _ = self.model.read_oriented(crops, orientations, min_confidence, max_length,
+                                                                      class_mask=mask)
+        return logits, rotation, confidence
+
+    def score(self, images: Union[Tensor, List[Any]], candidates: Candidates, *, rotation: Rotation = 0,
               return_token_logprobs: bool = False):
         """Log-likelihood of each candidate label for each image: fp32 [N, Kmax], -inf past an image's own candidates.
         PARSeq: sum over i = 0..n of log_softmax(head(decode(...)))[i, t_i] under the canonical left-to-right masks, with
@@ -780,7 +910,7 @@ class _System(nn.Module):
         return Lexicon(self.tokenizer, candidates, cfg.max_label_length, cfg.num_classes)
 
     def lexicon_decode(self, images: Union[Tensor, List[Any]], lexicon: Union[Candidates, Lexicon], *,
-                       rotation: int = 0, beam_width: Optional[int] = None):
+                       rotation: Rotation = 0, beam_width: Optional[int] = None):
         """Lexicon-constrained recognition: for each image the candidate the model rates most likely (score), as
         (labels, log_probs).  The pick is torch.argmax of the image's scores: the first maximum, or the first NaN.
         With `beam_width` the pick is the best hypothesis of a lexicon-constrained beam search of that width instead,
@@ -801,7 +931,7 @@ class _System(nn.Module):
         return labels, scores.gather(1, best[:, None])[:, 0]
 
     def beam_search(self, images: Union[Tensor, List[Any]], beam_width: int = 5, max_length: Optional[int] = None, *,
-                    rotation: int = 0, allowlist: Allowlist = None, lexicon: Union[Candidates, Lexicon, None] = None):
+                    rotation: Rotation = 0, allowlist: Allowlist = None, lexicon: Union[Candidates, Lexicon, None] = None):
         """The `beam_width` most likely readings of each image by beam search on the device, as (labels, scores):
         labels[b] lists image b's hypotheses best first (fewer than beam_width when fewer exist), scores is fp32
         [N, beam_width], -inf padded, with each hypothesis's AR log-likelihood (what `score` returns for that label).
@@ -890,7 +1020,7 @@ class PARSeq(_System):
         except EngineError as e:  # pragma: no cover
             raise InvalidModelError(str(e)) from e
 
-    def forward(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *, rotation: int = 0,
+    def forward(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *, rotation: Rotation = 0,
                 allowlist: Allowlist = None) -> Tensor:
         """`images`: a tensor, as the reference takes, or a list of raw crops of any size (ParseqModel.forward).
         `allowlist`: None, one string for every image, or one Optional[str] per image: the characters each image may
@@ -900,7 +1030,7 @@ class PARSeq(_System):
         return self.model.forward(self.tokenizer, images, max_length, rotation=rotation, class_mask=mask)
 
     def read_with_attention(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *,
-                            rotation: int = 0, allowlist: Allowlist = None) -> Tuple[Tensor, Tensor]:
+                            rotation: Rotation = 0, allowlist: Allowlist = None) -> Tuple[Tensor, Tensor]:
         """`forward` plus where the decoder looked: (logits, maps) with logits exactly forward's and maps fp32
         [N, S, gh, gw] (S = logits.shape[1], (gh, gw) the patch grid): maps[b, i] is the cross-attention of the decoder's
         last layer for the query that produced logits[b, i], averaged over the heads as nn.MultiheadAttention averages
@@ -911,15 +1041,30 @@ class PARSeq(_System):
         gh, gw = self.model.cfg.grid
         return logits, maps.view(maps.shape[0], maps.shape[1], gh, gw)
 
-    def locate(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *, rotation: int = 0,
-               allowlist: Allowlist = None, threshold: float = 0.5):
+    def locate(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *, rotation: Rotation = 0,
+               allowlist: Allowlist = None, threshold: float = 0.5, orientations: Optional[Sequence[int]] = None,
+               min_confidence: Optional[float] = None):
         """Where each character was read: (labels, confidences, centers, boxes).  labels / confidences are postprocess's
         of the forward logits; centers[b] fp32 [n_b, 2] = (x, y) and boxes[b] fp32 [n_b, 4] = (x0, y0, x1, y1), one row
         per character of labels[b], from its map of read_with_attention: the map-weighted centroid of the patch-cell
         centres, and the extent of the cells whose weight is >= threshold * the map's maximum.  Coordinates are pixels of
-        the input: of the img_size image for tensors, of each original crop for raw crops (the resize scale and the
-        rotation undone).  Results on the device of the outputs, as forward returns them."""
-        logits, maps = self.read_with_attention(images, max_length, rotation=rotation, allowlist=allowlist)
+        the input: of the img_size image for tensors, of each original crop for raw crops (the resize scale and each
+        crop's rotation undone).  Results on the device of the outputs, as forward returns them.  With `orientations`
+        (raw crops only) each crop is read in the orientation read_oriented chooses, and its points are mapped back
+        under that rotation."""
+        if orientations is None:
+            if min_confidence is not None:
+                raise ValueError("min_confidence needs orientations")
+            logits, maps = self.read_with_attention(images, max_length, rotation=rotation, allowlist=allowlist)
+        else:
+            if _is_rotation_list(rotation) or rotation:
+                raise ValueError("rotation and orientations cannot be combined: the search chooses each crop's rotation")
+            mask = self.allowlist_mask(allowlist, len(images) if isinstance(images, (list, tuple)) else images.shape[0])
+            logits, _, rot, _, maps = self.model.read_oriented(images, orientations, min_confidence, max_length,
+                                                               class_mask=mask, attn_maps=True)
+            gh, gw = self.model.cfg.grid
+            maps = maps.view(maps.shape[0], maps.shape[1], gh, gw)
+            rotation = rot.tolist()
         labels, confs = self.postprocess(logits.to(self.device))
         cfg = self.model.cfg
         crops = isinstance(images, (list, tuple))
@@ -929,8 +1074,8 @@ class PARSeq(_System):
             c, bx = attention_centers_boxes(maps[b, :len(label)], cfg.patch_size, threshold)
             if crops:
                 hw = _crop_hw(images[b])
-                c = unrotate_points(c, hw, cfg.img_size, rotation)
-                bx = unrotate_boxes(bx, hw, cfg.img_size, rotation)
+                c = unrotate_points(c, hw, cfg.img_size, _rotation_of(rotation, b))
+                bx = unrotate_boxes(bx, hw, cfg.img_size, _rotation_of(rotation, b))
             centers.append(c)
             boxes.append(bx)
         return labels, confs, centers, boxes
@@ -961,7 +1106,7 @@ class ViTSTR(_System):
         except EngineError as e:  # pragma: no cover
             raise InvalidModelError(str(e)) from e
 
-    def forward(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *, rotation: int = 0,
+    def forward(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *, rotation: Rotation = 0,
                 allowlist: Allowlist = None) -> Tensor:
         """`allowlist` as in PARSeq.forward: it constrains the argmax of every token position."""
         mask = self.allowlist_mask(allowlist, len(images) if isinstance(images, (list, tuple)) else images.shape[0])

@@ -208,6 +208,7 @@ typedef struct parseq_score_args {
   const int32_t* per_image;    /* HOST int32 [N]: candidates of image b, >= 1; candidates are image-major */
   const int32_t* targets;      /* HOST int32 [M][max_label_length + 1]: c_1..c_n (head classes 1..C-1), EOS (0), rest ignored */
   const int32_t* lengths;      /* HOST int32 [M]: n, 0 <= n <= max_label_length */
+  float* attn_maps;            /* DEVICE fp32 [M][max_label_length + 1][T] or NULL: see below */
 } parseq_score_args;
 /* images as parseq_forward / parseq_forward_u8 take them; scores DEVICE fp32 [M]; token_logprobs DEVICE fp32
  * [M][max_label_length + 1] or NULL (term i of candidate m, 0 past n).  All metadata is checked on the host before anything
@@ -217,6 +218,11 @@ int parseq_score(parseq_engine* e, const parseq_score_args* a, const float* imag
                  parseq_stream_t stream);
 int parseq_score_u8(parseq_engine* e, const parseq_score_args* a, const uint8_t* images_hwc, float* scores,
                     float* token_logprobs, parseq_stream_t stream);
+/* attn_maps (PARSeq; ViTSTR has no decoder cross-attention: PARSEQ_ERR_UNSUPPORTED): row i <= n of candidate m is the
+ * cross-attention of the decoder's last layer for the query that predicts t_i in the teacher-forced pass above (the
+ * head-averaged weights nn.MultiheadAttention returns, as parseq_forward_args.attn_maps), rows past n are 0.  The maps are
+ * written in the pass that computes the scores, which stay bit-identical to the call without maps; a row's bits do not
+ * depend on the other candidates of its image or on the batch.  No buffer is allocated for them. */
 /* The host checks of parseq_score against a configuration, without a handle or a device. */
 int parseq_score_check(const parseq_config* cfg, const parseq_score_args* a);
 
@@ -239,10 +245,16 @@ int parseq_score_check(const parseq_config* cfg, const parseq_score_args* a);
 typedef struct parseq_beam_args {
   int32_t batch, beam_width, max_length;   /* 1 <= beam_width <= 16 (PARSeq: and <= option dec_chunk); max_length -1 = None */
   const uint32_t* class_mask;              /* DEVICE allowlist rows as parseq_forward_args.class_mask, or NULL */
+  float* attn_maps;                        /* DEVICE fp32 [N][K][num_steps][T] or NULL: see below */
 } parseq_beam_args;
 /* images as parseq_forward / parseq_forward_u8 take them; all outputs DEVICE, hypotheses best first:
  * ids int32 [N][K][num_steps] = c_1..c_n, then 0 (EOS / padding); lengths int32 [N][K] = n, -1 for a missing hypothesis;
- * scores fp32 [N][K], -inf for a missing hypothesis (e.g. allowlist "": the only reading is "" with score 0). */
+ * scores fp32 [N][K], -inf for a missing hypothesis (e.g. allowlist "": the only reading is "" with score 0).
+ * attn_maps (PARSeq, also under a lexicon; ViTSTR: PARSEQ_ERR_UNSUPPORTED): row i <= n of hypothesis k is the
+ * cross-attention map parseq_score_args.attn_maps gives row i of that hypothesis's label, bit for bit; rows past n, and
+ * every row of a missing hypothesis, are 0.  After a group's last selection one teacher-forced pass over its final
+ * hypotheses (context [BOS, c_1..c_{num_steps-1}] under the causal masks) computes them on the device; the ids, lengths
+ * and scores are bit-identical to the call without maps. */
 int parseq_beam_search(parseq_engine* e, const parseq_beam_args* a, const float* images, int32_t* ids, int32_t* lengths,
                        float* scores, parseq_stream_t stream);
 int parseq_beam_search_u8(parseq_engine* e, const parseq_beam_args* a, const uint8_t* images_hwc, int32_t* ids,
@@ -362,8 +374,9 @@ int parseq_set_option(parseq_engine* e, const char* name, int64_t value);
  * category 0 encoder GEMM, 1 encoder attention, 2 LayerNorm, 3 decoder GEMM, 4 decoder attention, 5 other,
  * 6 encoder residual GEMM fused with LayerNorm, 7 persistent AR-loop kernel, 8 scoring tail (head GEMM with the log-sum-exp
  * epilogue and the per-candidate reduce of parseq_score), 9 beam selection (the selection kernel and, at dec_depth >= 2,
- * the K/V cache gather of parseq_beam_search), 10 cross-attention maps (the maps kernel of parseq_forward_args.attn_maps;
- * the AR-only map pass's other kernels count in their own categories), 11 orientation search (the confidence and
+ * the K/V cache gather of parseq_beam_search), 10 cross-attention maps (the maps kernels of parseq_forward_args,
+ * parseq_score_args and parseq_beam_args.attn_maps and the beam maps' tail fill; the teacher-forced map passes' other
+ * kernels count in their own categories), 11 orientation search (the confidence and
  * select kernels and the pass-2 allowlist gather of parseq_forward_crops_oriented). */
 int parseq_get_timing(parseq_engine* e, int category, double* ms, double* flops, int64_t* count);
 /* Debug: after a forward with option "ar_prof"=1, copies the [32 steps][16 slots] globaltimer (ns) stamps that block 0 of

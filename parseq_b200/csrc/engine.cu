@@ -875,7 +875,8 @@ void free_workspace(parseq_engine* e) {
 // categories: 0 encoder GEMM, 1 encoder attention, 2 LayerNorm, 3 decoder GEMM, 4 decoder attention, 5 other,
 // 6 encoder residual GEMM + LayerNorm, 7 AR-loop kernel, 8 scoring tail (head GEMM with the LSE epilogue + reduce),
 // 9 beam selection (beam_select_kernel and the K/V gather of parseq_beam_search), 10 cross-attention maps
-// (dec_cross_attn_maps_kernel), 11 orientation search (orient.cuh: confidence, select, pass-2 allowlist gather)
+// (dec_cross_attn_maps_kernel, its grouped form, maps_zero_tail_kernel), 11 orientation search (orient.cuh:
+// confidence, select, pass-2 allowlist gather)
 enum { CAT_ENC_GEMM = 0, CAT_ENC_ATTN = 1, CAT_LN = 2, CAT_DEC_GEMM = 3, CAT_DEC_ATTN = 4, CAT_MISC = 5, CAT_ENC_GEMM_LN = 6, CAT_DEC_AR = 7,
        CAT_SCORE = 8, CAT_BEAM = 9, CAT_MAPS = 10, CAT_ORIENT = 11, CAT_COUNT = 12 };
 
@@ -1085,6 +1086,10 @@ struct DecodeExtras {
   // or head)
   float* maps = nullptr;
   bool maps_only = false;
+  // with cand_off (candidate scoring): the maps have maps_ld rows per candidate, rows past maps_len[c] (the group's
+  // candidate lengths, device) written as 0 (dec_cross_attn_maps_grouped_kernel)
+  const int* maps_len = nullptr;
+  int maps_ld = 0;
 };
 
 const __nv_bfloat16* ckv_of(const parseq_engine* e, int layer) { return layer == 0 ? e->ckv : e->ckv_deep[layer - 1]; }
@@ -1130,14 +1135,23 @@ int dec_layer_rest(parseq_engine* e, parseq_engine::Stage& sg, int l, int b_firs
   if (maps != nullptr) {
     // the head-averaged weights of these query rows, from the q just projected and the layer's K (reads only)
     TimedScope ts(e, st, CAT_MAPS, 2.0 * M * e->T * D);
-    const dim3 grid(static_cast<unsigned>(B), static_cast<unsigned>((nq + pq::AMAP_ROWS - 1) / pq::AMAP_ROWS));
     const long long kv_rows = 1ll * e->max_batch * e->T;
-    if (e->T <= 128)
-      PQ_TRY(launch_k(e->lo, pq::dec_cross_attn_maps_kernel<4>, grid, dim3(pq::AMAP_THREADS), 0, st, static_cast<const float*>(sg.qc),
-                      ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, maps));
-    else
-      PQ_TRY(launch_k(e->lo, pq::dec_cross_attn_maps_kernel<8>, grid, dim3(pq::AMAP_THREADS), 0, st, static_cast<const float*>(sg.qc),
-                      ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, maps));
+    if (cand_off != nullptr) {
+      // candidate scoring: every image's candidates' maps_ld map rows, at most cand_max_rows / nq candidates per image
+      const int max_rows = ex->cand_max_rows / nq * ex->maps_ld;
+      const dim3 grid(static_cast<unsigned>(ex->cand_imgs), static_cast<unsigned>((max_rows + pq::AMAP_ROWS - 1) / pq::AMAP_ROWS));
+      PQ_TRY(launch_k(e->lo, e->T <= 128 ? pq::dec_cross_attn_maps_grouped_kernel<4> : pq::dec_cross_attn_maps_grouped_kernel<8>,
+                      grid, dim3(pq::AMAP_THREADS), 0, st, static_cast<const float*>(sg.qc), ckv_of(e, l), kv_rows, b_first,
+                      e->T, D, e->cfg.dec_num_heads, nq, cand_off, ex->maps_len, ex->maps_ld, maps));
+    } else {
+      const dim3 grid(static_cast<unsigned>(B), static_cast<unsigned>((nq + pq::AMAP_ROWS - 1) / pq::AMAP_ROWS));
+      if (e->T <= 128)
+        PQ_TRY(launch_k(e->lo, pq::dec_cross_attn_maps_kernel<4>, grid, dim3(pq::AMAP_THREADS), 0, st, static_cast<const float*>(sg.qc),
+                        ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, maps));
+      else
+        PQ_TRY(launch_k(e->lo, pq::dec_cross_attn_maps_kernel<8>, grid, dim3(pq::AMAP_THREADS), 0, st, static_cast<const float*>(sg.qc),
+                        ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, maps));
+    }
     if (ex->maps_only) return PARSEQ_OK;
   }
   {
@@ -2332,6 +2346,12 @@ int score_impl(parseq_engine* e, const parseq_score_args* a, const void* images_
       ex.cand_off = meta + g.cand_off;
       ex.cand_imgs = g.nimg;
       ex.cand_max_rows = g.max_rows;
+      if (a->attn_maps != nullptr) {
+        // the last layer's query rows of this pass, under each candidate's L map rows (0 past its EOS)
+        ex.maps = a->attn_maps + 1ll * g.m0 * L * e->T;
+        ex.maps_len = meta + len_off + g.m0;
+        ex.maps_ld = L;
+      }
       PQ_TRY(decode_pass(e, sg, g.b_lo - b0, B, g.P, 0, g.P, 0, meta + g.ids_off, nullptr, 0, nullptr, 0, nullptr, 0, nullptr,
                          ds, &ex));
       TimedScope ts(e, ds, CAT_SCORE, 0.0);
@@ -2352,6 +2372,8 @@ int check_score_call(parseq_engine* e, const parseq_score_args* a, const void* i
   PQ_TRY(check_score(a, -1, 0));
   if (images == nullptr || scores == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
   PQ_TRY(check_ready(e));
+  if (a->attn_maps != nullptr && e->arch != 0)
+    return fail(PARSEQ_ERR_UNSUPPORTED, "attn_maps: ViTSTR has no decoder cross-attention");
   return check_score(a, e->cfg.max_label_length, e->C);
 }
 
@@ -2427,6 +2449,7 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
   const char* images = static_cast<const char*>(images_any);
   PQ_TRY(beam_reserve(e));
   if (lx != nullptr) PQ_TRY(lexicon_reserve(e));
+  if (a->attn_maps != nullptr) PQ_TRY(causal_reserve(e));
   auto init = [&](parseq_engine::Stage::Beam& bm, int B, cudaStream_t st) {
     const int n = B * K * e->ids_ld;
     e->launches++;
@@ -2530,7 +2553,22 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
       // the stage's own cache pointers back (their contents are scratch between calls)
       for (size_t l = 0; l < sg.kvc.size(); ++l)
         if (sg.kvc[l] != kvc0[l]) std::swap(sg.kvc[l], bm.kvc[l]);
-      return rc;
+      if (rc != PARSEQ_OK || a->attn_maps == nullptr) return rc;
+      // the final hypotheses' maps: the last selection left each row's [BOS, c_1..] in bm.ids[S & 1] (valid ids
+      // everywhere), so one teacher-forced pass over the rows' first S ids under the causal masks computes every step's
+      // query (ar_maps_pass over beam rows); image j's K * S query rows are contiguous
+      float* const maps = a->attn_maps + 1ll * (b0 + g0) * K * S * e->T;
+      const unsigned char* causal = e->sc_causal + 1ll * (S - 1) * L * L;
+      DecodeExtras mx;
+      mx.beam = K;
+      mx.qmask = causal;
+      mx.cmask = e->cfg.dec_depth > 1 ? causal : nullptr;
+      mx.maps = maps;
+      mx.maps_only = true;
+      PQ_TRY(decode_pass(e, sg, g0, R, S, 0, S, 0, bm.ids[S & 1], nullptr, 0, nullptr, 0, nullptr, 0, nullptr, ds, &mx));
+      TimedScope ts(e, ds, CAT_MAPS, 0.0);
+      return launch_k(e->lo, pq::maps_zero_tail_kernel, dim3(static_cast<unsigned>(R)), dim3(256), 0, ds, maps,
+                      static_cast<const int*>(lengths + 1ll * (b0 + g0) * K), S, e->T);
     }));
   }
   return leave_main(e, user);
@@ -2581,6 +2619,8 @@ int check_beam_call(parseq_engine* e, const parseq_beam_args* a, const void* ima
   if (a->batch > 0 && (images == nullptr || ids == nullptr || lengths == nullptr || scores == nullptr))
     return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
   PQ_TRY(check_ready(e));
+  if (a->attn_maps != nullptr && e->arch != 0)
+    return fail(PARSEQ_ERR_UNSUPPORTED, "attn_maps: ViTSTR has no decoder cross-attention");
   if (e->arch == 0 && a->beam_width > e->dec_chunk)
     return fail(PARSEQ_ERR_INVALID_ARG, "beam_width " + std::to_string(a->beam_width) + " exceeds the decoder chunk (option "
                                         "dec_chunk = " + std::to_string(e->dec_chunk) + ")");
@@ -2954,6 +2994,8 @@ int parseq_forward_crops_oriented(parseq_engine* e, const parseq_forward_args* a
 
 int parseq_score_check(const parseq_config* cfg, const parseq_score_args* a) {
   if (cfg == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null argument");
+  if (a != nullptr && a->attn_maps != nullptr && cfg->arch != 0)
+    return fail(PARSEQ_ERR_UNSUPPORTED, "attn_maps: ViTSTR has no decoder cross-attention");
   return check_score(a, cfg->max_label_length, cfg->num_tokens - 2);
 }
 

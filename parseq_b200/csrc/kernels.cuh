@@ -856,18 +856,29 @@ __global__ void __launch_bounds__(128) dec_cross_attn3_grouped_kernel(const floa
 // bitwise those of its P.V, which scales sum(e * v) by 1 / sum where this kernel stores p = e * (1 / sum) per key.
 // Each warp keeps its AMAP_ROWS / 8 rows' running sums in registers; the heads are summed in fixed order, so the maps
 // are bitwise reproducible and independent of the batch.  q fp32 [B*nq, D] pre-scaled; maps fp32 [B*nq, T].
+// GROUPED (candidate scoring, parseq_score_args.attn_maps): the maps have out_ld rows per candidate, candidate c's
+// query rows are q rows [c * nq, c * nq + nq) (nq <= out_ld), and image j owns the map rows [cand_off[j] * out_ld,
+// cand_off[j + 1] * out_ld); CTA (j, y) writes AMAP_ROWS of them, grid.y covering the image with the most.  Row i of
+// candidate c is computed for i <= lengths[c] and written as 0 past it (its sums stay 0), so rows past a label's EOS
+// cost no exponentials.  A computed row's bits are those of the non-grouped kernel for the same q row.
 constexpr int AMAP_ROWS = 32;
 constexpr int AMAP_THREADS = 256;
-template <int NR>   // keys per lane: T <= 32 * NR
-__global__ void __launch_bounds__(AMAP_THREADS, 1) dec_cross_attn_maps_kernel(const float* __restrict__ q,
-                                                                         const __nv_bfloat16* __restrict__ kv,
-                                                                         long long kv_rows, int b_first, int T, int D,
-                                                                         int heads, int nq, float* __restrict__ maps) {
+template <int NR, bool GROUPED>
+__device__ __forceinline__ void dec_cross_attn_maps_body(const float* __restrict__ q, const __nv_bfloat16* __restrict__ kv,
+                                                         long long kv_rows, int b_first, int T, int D, int heads, int nq,
+                                                         const int* __restrict__ cand_off, const int* __restrict__ lengths,
+                                                         int out_ld, float* __restrict__ maps) {
   constexpr int TK = 32 * NR, WARPS = AMAP_THREADS / 32, RPW = AMAP_ROWS / WARPS;
   __shared__ uint32_t sK[TK * 17];
   grid_dep_launch();
   grid_dep_wait();
   const int b = blockIdx.x, q_begin = static_cast<int>(blockIdx.y) * AMAP_ROWS;
+  int rows = nq, out0 = 0;
+  if (GROUPED) {
+    out0 = cand_off[b] * out_ld;
+    rows = cand_off[b + 1] * out_ld - out0;
+    if (q_begin >= rows) return;                       // CTA-uniform, before any barrier
+  }
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const long long row_b = static_cast<long long>(b_first + b) * T;
   float acc[RPW][NR];
@@ -882,8 +893,13 @@ __global__ void __launch_bounds__(AMAP_THREADS, 1) dec_cross_attn_maps_kernel(co
 #pragma unroll
     for (int j = 0; j < RPW; ++j) {
       const int qi = q_begin + warp + j * WARPS;
-      if (qi >= nq) continue;                            // warp-uniform
-      const long long row = static_cast<long long>(b) * nq + qi;
+      if (qi >= (GROUPED ? rows : nq)) continue;         // warp-uniform
+      long long row = static_cast<long long>(b) * nq + qi;
+      if (GROUPED) {
+        const int c = (out0 + qi) / out_ld, i = out0 + qi - c * out_ld;
+        if (i > lengths[c]) continue;                    // warp-uniform: past the label's EOS
+        row = static_cast<long long>(c) * nq + i;
+      }
       float sc[NR];
       const float sum = cross_row_exp<NR>(sK, q[row * D + h * 32 + lane], T, lane, sc);
       const float inv = 1.0f / sum;
@@ -895,12 +911,39 @@ __global__ void __launch_bounds__(AMAP_THREADS, 1) dec_cross_attn_maps_kernel(co
 #pragma unroll
   for (int j = 0; j < RPW; ++j) {
     const int qi = q_begin + warp + j * WARPS;
-    if (qi >= nq) continue;
-    float* out = maps + (static_cast<long long>(b) * nq + qi) * T;
+    if (qi >= (GROUPED ? rows : nq)) continue;
+    float* out = maps + ((GROUPED ? static_cast<long long>(out0) : static_cast<long long>(b) * nq) + qi) * T;
 #pragma unroll
     for (int r = 0; r < NR; ++r)
       if (r * 32 + lane < T) out[r * 32 + lane] = acc[j][r] / rh;
   }
+}
+
+template <int NR>   // keys per lane: T <= 32 * NR
+__global__ void __launch_bounds__(AMAP_THREADS, 1) dec_cross_attn_maps_kernel(const float* __restrict__ q,
+                                                                         const __nv_bfloat16* __restrict__ kv,
+                                                                         long long kv_rows, int b_first, int T, int D,
+                                                                         int heads, int nq, float* __restrict__ maps) {
+  dec_cross_attn_maps_body<NR, false>(q, kv, kv_rows, b_first, T, D, heads, nq, nullptr, nullptr, 0, maps);
+}
+
+template <int NR>
+__global__ void __launch_bounds__(AMAP_THREADS, 1) dec_cross_attn_maps_grouped_kernel(
+    const float* __restrict__ q, const __nv_bfloat16* __restrict__ kv, long long kv_rows, int b_first, int T, int D,
+    int heads, int nq, const int* __restrict__ cand_off, const int* __restrict__ lengths, int out_ld,
+    float* __restrict__ maps) {
+  dec_cross_attn_maps_body<NR, true>(q, kv, kv_rows, b_first, T, D, heads, nq, cand_off, lengths, out_ld, maps);
+}
+
+// Rows past each hypothesis's length of the beam maps (parseq_beam_args.attn_maps) to 0: one CTA per hypothesis h of
+// rows_per map rows, rows i > lengths[h] (every row of a missing hypothesis, length -1).
+__global__ void maps_zero_tail_kernel(float* __restrict__ maps, const int* __restrict__ lengths, int rows_per, int T) {
+  grid_dep_wait();
+  const int h = blockIdx.x;
+  const int first = lengths[h] + 1 > 0 ? lengths[h] + 1 : 0;
+  float* m = maps + (static_cast<long long>(h) * rows_per + first) * T;
+  const int n = (rows_per - first) * T;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) m[i] = 0.f;
 }
 
 // ---------------------------------------------------------------------------------------------

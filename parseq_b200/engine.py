@@ -43,11 +43,12 @@ def orient_args(orientations, min_confidence, rotation_ptr, confidence_ptr) -> O
 
 class ScoreArgsC(C.Structure):
     _fields_ = [("batch", C.c_int32), ("num_candidates", C.c_int32), ("per_image", C.c_void_p), ("targets", C.c_void_p),
-                ("lengths", C.c_void_p)]
+                ("lengths", C.c_void_p), ("attn_maps", C.c_void_p)]
 
 
 class BeamArgsC(C.Structure):
-    _fields_ = [("batch", C.c_int32), ("beam_width", C.c_int32), ("max_length", C.c_int32), ("class_mask", C.c_void_p)]
+    _fields_ = [("batch", C.c_int32), ("beam_width", C.c_int32), ("max_length", C.c_int32), ("class_mask", C.c_void_p),
+                ("attn_maps", C.c_void_p)]
 
 
 class LexiconDescC(C.Structure):
@@ -324,17 +325,20 @@ class Engine:
         check(self.lib, self.lib.parseq_forward_crops_oriented(self.handle, C.byref(a), C.byref(crops), C.byref(o),
                                                                logits_ptr, ids_ptr, steps_ptr, stream))
 
-    # per_image / targets / lengths: CPU int32 tensors (parseq_score_args); scores / token_lp: device pointers
-    def score(self, images_ptr, batch, per_image, targets, lengths, scores_ptr, token_lp_ptr, stream, u8=False):
-        a = ScoreArgsC(batch, int(targets.shape[0]), per_image.data_ptr(), targets.data_ptr(), lengths.data_ptr())
+    # per_image / targets / lengths: CPU int32 tensors (parseq_score_args); scores / token_lp / attn_maps: device pointers
+    def score(self, images_ptr, batch, per_image, targets, lengths, scores_ptr, token_lp_ptr, stream, u8=False,
+              attn_maps_ptr=None):
+        a = ScoreArgsC(batch, int(targets.shape[0]), per_image.data_ptr(), targets.data_ptr(), lengths.data_ptr(),
+                       attn_maps_ptr)
         fn = self.lib.parseq_score_u8 if u8 else self.lib.parseq_score
         check(self.lib, fn(self.handle, C.byref(a), images_ptr, scores_ptr, token_lp_ptr, stream))
 
-    # ids [N, K, num_steps] / lengths [N, K] / scores [N, K]: device pointers; class_mask_ptr as in forward; lexicon: a
-    # LexiconHandle of this engine's device, roots a CPU int32 tensor [N] or None
+    # ids [N, K, num_steps] / lengths [N, K] / scores [N, K] / attn_maps [N, K, num_steps, T]: device pointers;
+    # class_mask_ptr as in forward; lexicon: a LexiconHandle of this engine's device, roots a CPU int32 tensor [N] or None
     def beam_search(self, images_ptr, batch, beam_width, ids_ptr, lengths_ptr, scores_ptr, stream, max_length=None,
-                    class_mask_ptr=None, u8=False, lexicon=None, roots=None):
-        a = BeamArgsC(batch, int(beam_width), -1 if max_length is None else int(max_length), class_mask_ptr)
+                    class_mask_ptr=None, u8=False, lexicon=None, roots=None, attn_maps_ptr=None):
+        a = BeamArgsC(batch, int(beam_width), -1 if max_length is None else int(max_length), class_mask_ptr,
+                      attn_maps_ptr)
         if lexicon is None:
             fn = self.lib.parseq_beam_search_u8 if u8 else self.lib.parseq_beam_search
             check(self.lib, fn(self.handle, C.byref(a), images_ptr, ids_ptr, lengths_ptr, scores_ptr, stream))

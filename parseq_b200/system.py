@@ -487,10 +487,12 @@ class _EngineModule(nn.Module):
         return out
 
     def score(self, images: Union[Tensor, List[Any]], targets: Tensor, lengths: Tensor, per_image: Tensor, *,
-              rotation: Rotation = 0, return_token_logprobs: bool = False):
+              rotation: Rotation = 0, return_token_logprobs: bool = False, return_attention: bool = False):
         """Log-likelihoods of candidate labels (parseq_score): `targets` int32 [M, max_label_length + 1] (c_1..c_n, EOS),
         `lengths` [M], `per_image` [N] as pack_candidates makes them (CPU).  Returns fp32 scores [M] on the device, and
-        with return_token_logprobs the per-position terms [M, max_label_length + 1] (0 past each label's EOS).
+        with return_token_logprobs the per-position terms [M, max_label_length + 1] (0 past each label's EOS), with
+        return_attention the cross-attention maps fp32 [M, max_label_length + 1, T] (parseq_score_args.attn_maps: row i
+        the map of the query predicting t_i, 0 past each label's EOS), in that order.
         `images` as forward takes them; raw crops are resized on the device first (preprocess)."""
         eng = self.engine()
         if isinstance(images, (list, tuple)):
@@ -510,20 +512,24 @@ class _EngineModule(nn.Module):
         M = targets.shape[0]
         scores = torch.empty((M,), dtype=torch.float32, device=dev)
         tlp = torch.empty((M, L), dtype=torch.float32, device=dev) if return_token_logprobs else None
+        maps = torch.empty((M, L, self.cfg.enc_tokens), dtype=torch.float32, device=dev) if return_attention else None
         eng.score(images.data_ptr(), images.shape[0], per_image, targets, lengths, scores.data_ptr(),
                   tlp.data_ptr() if tlp is not None else None, torch.cuda.current_stream(dev).cuda_stream,
-                  u8=images.dtype == torch.uint8)
-        return (scores, tlp) if return_token_logprobs else scores
+                  u8=images.dtype == torch.uint8, attn_maps_ptr=_ptr(maps))
+        out = (scores,) + ((tlp,) if return_token_logprobs else ()) + ((maps,) if return_attention else ())
+        return out if len(out) > 1 else scores
 
     def beam_search(self, images: Union[Tensor, List[Any]], beam_width: int = 5, max_length: Optional[int] = None, *,
                     rotation: Rotation = 0, class_mask: Optional[Tensor] = None, lexicon: Optional[Lexicon] = None,
-                    roots: Optional[Tensor] = None):
+                    roots: Optional[Tensor] = None, return_attention: bool = False):
         """Beam search (parseq_beam_search): the `beam_width` most likely readings of each image, best first, as raw
         (ids int32 [N, K, num_steps] = c_1..c_n then 0, lengths int32 [N, K] (-1: no hypothesis), scores fp32 [N, K]
         (-inf: no hypothesis)) on the device.  A hypothesis's score is its AR log-likelihood, the quantity `score`
         computes.  `images` as forward takes them; `class_mask`: per-image allowlist words (allowlist_mask).
         `lexicon` (a compiled Lexicon) restricts every hypothesis to its words (parseq_beam_search_lexicon); `roots`:
-        CPU int32 [N], the node each image starts at (Lexicon.roots_for), or None for node 0."""
+        CPU int32 [N], the node each image starts at (Lexicon.roots_for), or None for node 0.  return_attention: also
+        the hypotheses' cross-attention maps fp32 [N, K, num_steps, T] (parseq_beam_args.attn_maps: `score`'s maps of
+        each hypothesis's label, 0 past its EOS and for a missing hypothesis)."""
         check_beam_width(beam_width)
         if lexicon is None and roots is not None:
             raise ValueError("roots need a lexicon")
@@ -553,6 +559,7 @@ class _EngineModule(nn.Module):
         ids = torch.empty((N, K, S), dtype=torch.int32, device=dev)
         lengths = torch.empty((N, K), dtype=torch.int32, device=dev)
         scores = torch.empty((N, K), dtype=torch.float32, device=dev)
+        maps = torch.empty((N, K, S, self.cfg.enc_tokens), dtype=torch.float32, device=dev) if return_attention else None
         lex = None
         if lexicon is not None:
             lex = lexicon.handle(eng)
@@ -562,8 +569,8 @@ class _EngineModule(nn.Module):
                     raise ValueError(f"roots must be int32 [{N}]")
         eng.beam_search(images.data_ptr(), N, K, ids.data_ptr(), lengths.data_ptr(), scores.data_ptr(),
                         torch.cuda.current_stream(dev).cuda_stream, max_length, _mask_ptr(class_mask),
-                        u8=images.dtype == torch.uint8, lexicon=lex, roots=roots)
-        return ids, lengths, scores
+                        u8=images.dtype == torch.uint8, lexicon=lex, roots=roots, attn_maps_ptr=_ptr(maps))
+        return (ids, lengths, scores, maps) if return_attention else (ids, lengths, scores)
 
     def _run_crops(self, crops, max_length, decode_ar, refine_iters, rotation, class_mask=None, attn_maps=False):
         """Raw crops of any size: CUDA crops run parseq_forward_crops and return CUDA tensors; CPU crops and PIL images
@@ -817,6 +824,18 @@ class _HParams(SimpleNamespace):
 class _System(nn.Module):
     """The inference-side surface of `strhub.models.base.CrossEntropySystem` (base.py:36-44,112-143,179-207)."""
 
+    # why return_attention is refused, or None where the decoder has cross-attention maps
+    _no_attention: Optional[str] = None
+
+    def _check_attention(self, return_attention: bool):
+        if return_attention and self._no_attention is not None:
+            raise NotImplementedError(self._no_attention)
+
+    def _grid_maps(self, maps: Tensor) -> Tensor:
+        """fp32 [..., T] maps as [..., gh, gw] over the patch grid."""
+        gh, gw = self.model.cfg.grid
+        return maps.view(*maps.shape[:-1], gh, gw)
+
     def _init_base(self, charset_train, charset_test, batch_size, lr, warmup_pct, weight_decay):
         self.tokenizer = Tokenizer(charset_train)
         self.charset_adapter = CharsetAdapter(charset_test)
@@ -869,20 +888,27 @@ class _System(nn.Module):
         return logits, rotation, confidence
 
     def score(self, images: Union[Tensor, List[Any]], candidates: Candidates, *, rotation: Rotation = 0,
-              return_token_logprobs: bool = False):
+              return_token_logprobs: bool = False, return_attention: bool = False):
         """Log-likelihood of each candidate label for each image: fp32 [N, Kmax], -inf past an image's own candidates.
         PARSeq: sum over i = 0..n of log_softmax(head(decode(...)))[i, t_i] under the canonical left-to-right masks, with
         targets t = (c_1..c_n, EOS) - minus the summed cross-entropy of permutation 0 of the reference's training_step.
         ViTSTR: the same sum over its per-token logits.  `candidates`: one list of strings for every image (a lexicon),
         or one non-empty list per image.  With return_token_logprobs also the terms [N, Kmax, max_label_length + 1]
-        (0 past each label's EOS and past an image's candidates).  `images` as forward takes them; the result is on
-        the images' device (CPU for CPU crops)."""
+        (0 past each label's EOS and past an image's candidates).  With return_attention (PARSeq) also the maps fp32
+        [N, Kmax, max_label_length + 1, gh, gw]: [b, k, i] is the cross-attention of the decoder's last layer for the
+        query that predicts character i of candidate k (i = n: its EOS), in the teacher-forced pass the score comes
+        from, averaged over the heads as in read_with_attention; 0 past each label's EOS and past an image's candidates.
+        `images` as forward takes them; the result is on the images' device (CPU for CPU crops)."""
+        self._check_attention(return_attention)
         N = len(images) if isinstance(images, (list, tuple)) else images.shape[0]
         cfg = self.model.cfg
         targets, lengths, per_image = pack_candidates(self.tokenizer, candidates, N, cfg.max_label_length, cfg.num_classes)
         out = self.model.score(images, targets, lengths, per_image, rotation=rotation,
-                               return_token_logprobs=return_token_logprobs)
-        scores, tlp = out if return_token_logprobs else (out, None)
+                               return_token_logprobs=return_token_logprobs, return_attention=return_attention)
+        out = out if isinstance(out, tuple) else (out,)
+        scores = out[0]
+        tlp = out[1] if return_token_logprobs else None
+        maps = out[-1] if return_attention else None
         K = int(per_image.max())
         dev = scores.device
         img = torch.repeat_interleave(torch.arange(N), per_image.long())
@@ -894,12 +920,15 @@ class _System(nn.Module):
         if isinstance(images, (list, tuple)) and all(not (isinstance(c, Tensor) and c.is_cuda) for c in images):
             dev = torch.device("cpu")
         grid = grid.view(N, K).to(dev)
-        if not return_token_logprobs:
-            return grid
-        L = cfg.max_label_length + 1
-        terms = torch.zeros((N * K, L), dtype=torch.float32, device=tlp.device)
-        terms[idx] = tlp
-        return grid, terms.view(N, K, L).to(dev)
+        res = (grid,)
+        for rows in (tlp, maps):
+            if rows is not None:                     # [M, L, ...] -> [N, Kmax, L, ...], zero past an image's candidates
+                full = torch.zeros((N * K,) + tuple(rows.shape[1:]), dtype=torch.float32, device=rows.device)
+                full[idx] = rows
+                res += (full.view((N, K) + tuple(rows.shape[1:])).to(dev),)
+        if maps is not None:
+            res = res[:-1] + (self._grid_maps(res[-1]),)
+        return res if len(res) > 1 else grid
 
     def compile_lexicon(self, candidates: Candidates) -> Lexicon:
         """A word list (shared by every image) or one list per image, compiled for beam_search(lexicon=) and
@@ -910,28 +939,38 @@ class _System(nn.Module):
         return Lexicon(self.tokenizer, candidates, cfg.max_label_length, cfg.num_classes)
 
     def lexicon_decode(self, images: Union[Tensor, List[Any]], lexicon: Union[Candidates, Lexicon], *,
-                       rotation: Rotation = 0, beam_width: Optional[int] = None):
+                       rotation: Rotation = 0, beam_width: Optional[int] = None, return_attention: bool = False):
         """Lexicon-constrained recognition: for each image the candidate the model rates most likely (score), as
         (labels, log_probs).  The pick is torch.argmax of the image's scores: the first maximum, or the first NaN.
         With `beam_width` the pick is the best hypothesis of a lexicon-constrained beam search of that width instead,
         at a cost that does not grow with the lexicon (`lexicon` may then be a compiled Lexicon); an image with no
-        reachable word gets label None and -inf."""
+        reachable word gets label None and -inf.  With return_attention (PARSeq) also the chosen word's maps fp32
+        [N, max_label_length + 1, gh, gw], as score returns them (0 for an image with no word)."""
+        self._check_attention(return_attention)
         if beam_width is not None:
-            labels, scores = self.beam_search(images, beam_width, rotation=rotation, lexicon=lexicon)
-            return [h[0] if h else None for h in labels], scores[:, 0]
+            out = self.beam_search(images, beam_width, rotation=rotation, lexicon=lexicon,
+                                   return_attention=return_attention)
+            labels = [h[0] if h else None for h in out[0]]
+            return (labels, out[1][:, 0]) + ((out[2][:, 0],) if return_attention else ())
         if isinstance(lexicon, Lexicon):
             raise TypeError("a compiled Lexicon serves the beam search only: pass beam_width, or the word lists to score "
                             "every word")
-        scores = self.score(images, lexicon, rotation=rotation)
+        out = self.score(images, lexicon, rotation=rotation, return_attention=return_attention)
+        scores = out[0] if return_attention else out
         N = scores.shape[0]
         rows = [lexicon] * N if all(isinstance(c, str) for c in lexicon) else list(lexicon)
         best = scores.argmax(-1)
         best_h = best.tolist()
         labels = [rows[b][k] for b, k in enumerate(best_h)]
-        return labels, scores.gather(1, best[:, None])[:, 0]
+        res = (labels, scores.gather(1, best[:, None])[:, 0])
+        if not return_attention:
+            return res
+        maps = out[1]
+        return res + (maps[torch.arange(N, device=maps.device), best.to(maps.device)],)
 
     def beam_search(self, images: Union[Tensor, List[Any]], beam_width: int = 5, max_length: Optional[int] = None, *,
-                    rotation: Rotation = 0, allowlist: Allowlist = None, lexicon: Union[Candidates, Lexicon, None] = None):
+                    rotation: Rotation = 0, allowlist: Allowlist = None, lexicon: Union[Candidates, Lexicon, None] = None,
+                    return_attention: bool = False):
         """The `beam_width` most likely readings of each image by beam search on the device, as (labels, scores):
         labels[b] lists image b's hypotheses best first (fewer than beam_width when fewer exist), scores is fp32
         [N, beam_width], -inf padded, with each hypothesis's AR log-likelihood (what `score` returns for that label).
@@ -940,8 +979,11 @@ class _System(nn.Module):
         `allowlist` as in forward.  The scores are on the images' device (CPU for CPU crops).
         `lexicon` (a word list for every image, one list per image, or a compiled Lexicon) restricts every hypothesis to
         a word of the image's list that ends with EOS within max_length characters; the log-sum-exp of each step stays
-        over all allowed classes, so a score is still `score`'s for that word."""
+        over all allowed classes, so a score is still `score`'s for that word.  With return_attention (PARSeq) also the
+        hypotheses' maps fp32 [N, beam_width, num_steps, gh, gw]: hypothesis k's are `score`'s maps of its label, bit for
+        bit, 0 past its EOS and for a missing hypothesis."""
         check_beam_width(beam_width)
+        self._check_attention(return_attention)
         N = len(images) if isinstance(images, (list, tuple)) else images.shape[0]
         mask = self.allowlist_mask(allowlist, N)
         roots = None
@@ -950,14 +992,17 @@ class _System(nn.Module):
                 lexicon_rows(lexicon, N)                   # the image count of per-image lists, before the trie build
                 lexicon = self.compile_lexicon(lexicon)
             roots = lexicon.roots_for(N)
-        ids, lengths, scores = self.model.beam_search(images, beam_width, max_length, rotation=rotation, class_mask=mask,
-                                                      lexicon=lexicon, roots=roots)
+        out = self.model.beam_search(images, beam_width, max_length, rotation=rotation, class_mask=mask,
+                                     lexicon=lexicon, roots=roots, return_attention=return_attention)
+        ids, lengths, scores = out[:3]
         ids_h, len_h = ids.cpu().tolist(), lengths.cpu().tolist()
         labels = [[self.tokenizer._ids2tok(ids_h[b][k][:n], True) for k, n in enumerate(len_h[b]) if n >= 0]
                   for b in range(N)]
+        maps = self._grid_maps(out[3]) if return_attention else None
         if isinstance(images, (list, tuple)) and all(not (isinstance(c, Tensor) and c.is_cuda) for c in images):
             scores = scores.cpu()
-        return labels, scores
+            maps = maps.cpu() if maps is not None else None
+        return (labels, scores, maps) if return_attention else (labels, scores)
 
     # base.py:112-143,179-180 (test path only; validation loss is a training concern)
     def _eval_step(self, batch, validation: bool = False):
@@ -1043,7 +1088,7 @@ class PARSeq(_System):
 
     def locate(self, images: Union[Tensor, List[Any]], max_length: Optional[int] = None, *, rotation: Rotation = 0,
                allowlist: Allowlist = None, threshold: float = 0.5, orientations: Optional[Sequence[int]] = None,
-               min_confidence: Optional[float] = None):
+               min_confidence: Optional[float] = None, text: Union[None, str, Sequence[str]] = None):
         """Where each character was read: (labels, confidences, centers, boxes).  labels / confidences are postprocess's
         of the forward logits; centers[b] fp32 [n_b, 2] = (x, y) and boxes[b] fp32 [n_b, 4] = (x0, y0, x1, y1), one row
         per character of labels[b], from its map of read_with_attention: the map-weighted centroid of the patch-cell
@@ -1051,7 +1096,26 @@ class PARSeq(_System):
         the input: of the img_size image for tensors, of each original crop for raw crops (the resize scale and each
         crop's rotation undone).  Results on the device of the outputs, as forward returns them.  With `orientations`
         (raw crops only) each crop is read in the orientation read_oriented chooses, and its points are mapped back
-        under that rotation."""
+        under that rotation.
+        With `text` (one string for every image, or one per image) the characters located are those of the given text
+        rather than of the model's reading (forced alignment): (labels = the texts, log-likelihoods fp32 [N] as score
+        gives them, centers, boxes), each character's map the one score(return_attention=True) gives it.  The text's
+        characters must be in charset_train (ValueError otherwise, as in score); it takes the place of max_length,
+        allowlist and orientations."""
+        if text is not None:
+            if max_length is not None or allowlist is not None or orientations is not None or min_confidence is not None:
+                raise ValueError("text fixes the characters to locate: it cannot be combined with max_length, "
+                                 "allowlist, orientations or min_confidence")
+            N = len(images) if isinstance(images, (list, tuple)) else images.shape[0]
+            if isinstance(text, str):
+                texts = [text] * N
+            elif isinstance(text, (list, tuple)) and len(text) == N and all(isinstance(t, str) for t in text):
+                texts = list(text)
+            else:
+                raise ValueError(f"text must be one string or a list of {N} strings (one per image)")
+            scores, maps = self.score(images, [[t] for t in texts], rotation=rotation, return_attention=True)
+            centers, boxes = self._locate_maps(images, maps[:, 0], [len(t) for t in texts], rotation, threshold)
+            return texts, scores[:, 0], centers, boxes
         if orientations is None:
             if min_confidence is not None:
                 raise ValueError("min_confidence needs orientations")
@@ -1066,23 +1130,32 @@ class PARSeq(_System):
             maps = maps.view(maps.shape[0], maps.shape[1], gh, gw)
             rotation = rot.tolist()
         labels, confs = self.postprocess(logits.to(self.device))
+        centers, boxes = self._locate_maps(images, maps, [len(label) for label in labels], rotation, threshold)
+        return labels, confs, centers, boxes
+
+    def _locate_maps(self, images, maps: Tensor, counts: Sequence[int], rotation: Rotation, threshold: float):
+        """(centers, boxes) of the first counts[b] maps of each image (maps [N, S, gh, gw]) as locate returns them: in
+        pixels of the img_size image for tensors, of each original crop for raw crops (its resize and rotation undone)."""
         cfg = self.model.cfg
         crops = isinstance(images, (list, tuple))
         centers: List[Tensor] = []
         boxes: List[Tensor] = []
-        for b, label in enumerate(labels):
-            c, bx = attention_centers_boxes(maps[b, :len(label)], cfg.patch_size, threshold)
+        for b, n in enumerate(counts):
+            c, bx = attention_centers_boxes(maps[b, :n], cfg.patch_size, threshold)
             if crops:
                 hw = _crop_hw(images[b])
                 c = unrotate_points(c, hw, cfg.img_size, _rotation_of(rotation, b))
                 bx = unrotate_boxes(bx, hw, cfg.img_size, _rotation_of(rotation, b))
             centers.append(c)
             boxes.append(bx)
-        return labels, confs, centers, boxes
+        return centers, boxes
 
 
 class ViTSTR(_System):
     """Mirror of `strhub.models.vitstr.system.ViTSTR` (vitstr/system.py:29-71), inference side."""
+
+    _no_attention = ("ViTSTR has no decoder cross-attention: its characters are read from the encoder's own tokens, so "
+                     "there are no per-character maps to return")
 
     def __init__(self, charset_train: str, charset_test: str, max_label_length: int, batch_size: int = 384,
                  lr: float = 8.9e-4, warmup_pct: float = 0.075, weight_decay: float = 0.0,

@@ -41,6 +41,15 @@ BUGS = {
     "pos_query_shift": "context row k adds pos_queries[k] instead of pos_queries[k - 1]",
     "no_linear2_bias": "the decoder MLP's linear2 bias is dropped",
     "no_head_bias": "the head bias is dropped",
+    "self_extra_zero_key": "every self-attention query also sees one key whose K and V are zero (an unwritten cache slot, "
+                           "or a lane past nkeys)",
+    "self_drop_own_key": "AR query i >= 1 does not see key i (query 0 keeps BOS)",
+    "cloze_mask_shift": "the refinement hides key i from query i >= 1 instead of key i + 1 (query 0 keeps every key)",
+    "eos_mask_eos_only": "the refinement's padding mask hides the EOS keys only, not every key from the first EOS on",
+    "norm_qc_eps": "norm_q and norm_c use eps 1e-6 instead of 1e-5 (every layer; at depth 1 the (position, token) table "
+                   "and the query table)",
+    "self_q_bf16": "the self-attention query (the pre-scaled query table; at depth >= 2 the query GEMM output) is rounded "
+                   "to bf16",
 }
 
 # Bounds on |engine - model| over the logits of one decoder pass, relative to the standard deviation sigma of the model's
@@ -158,6 +167,8 @@ class _RoundingPointModel:
     def _ln(self, x, prefix, eps):
         if self.bug == "ln_eps" and prefix.startswith("decoder.") and prefix.endswith(("norm1", "norm2", "decoder.norm")):
             eps = 1e-6
+        if self.bug == "norm_qc_eps" and prefix.endswith(("norm_q", "norm_c")):
+            eps = 1e-6
         return super()._ln(x, prefix, eps)
 
     def _context(self, ids):
@@ -171,7 +182,7 @@ class _RoundingPointModel:
         return emb
 
     def _mha(self, prefix, q_in, kv_in, mask):
-        """ParseqOracle._mha with the cross-attention bugs."""
+        """ParseqOracle._mha with the cross- and self-attention bugs."""
         p, cfg = self.p, self.cfg
         D, h = cfg.embed_dim, cfg.dec_num_heads
         d = D // h
@@ -186,6 +197,13 @@ class _RoundingPointModel:
                 kv = torch.cat([kv, kv.new_zeros((B, 1, 2 * D))], dim=1)
             elif self.bug == "cross_drop_last_key":
                 kv = kv[:, :-1]
+        elif prefix.endswith("self_attn"):
+            if self.bug == "self_q_bf16":
+                q = self.r(q)
+            elif self.bug == "self_extra_zero_key":
+                kv = torch.cat([kv, kv.new_zeros((B, 1, 2 * D))], dim=1)
+                if mask is not None:
+                    mask = torch.cat([mask, mask.new_zeros((B, nq, 1))], dim=2)
         nk = kv.shape[1]
         k, v = kv[..., :D], kv[..., D:]
         q = q.reshape(B, nq, h, d).transpose(1, 2)
@@ -228,12 +246,19 @@ class _RoundingPointModel:
 
     def _causal(self, L):
         """Query i sees keys 0..i (model.py:130-136)."""
-        return torch.triu(torch.ones((L, L), dtype=torch.bool, device=self.device), 2 if self.bug == "self_mask_leak" else 1)
+        m = torch.triu(torch.ones((L, L), dtype=torch.bool, device=self.device), 2 if self.bug == "self_mask_leak" else 1)
+        if self.bug == "self_drop_own_key":
+            i = torch.arange(1, L, device=self.device)
+            m[i, i] = True
+        return m
 
     def _cloze(self, L):
         """Query i sees every key but i + 1 (model.py:157)."""
         m = torch.zeros((L, L), dtype=torch.bool, device=self.device)
-        if self.bug != "self_mask_leak":
+        if self.bug == "cloze_mask_shift":
+            i = torch.arange(1, L, device=self.device)
+            m[i, i] = True
+        elif self.bug != "self_mask_leak":
             i = torch.arange(L - 1, device=self.device)
             m[i, i + 1] = True
         return m
@@ -254,7 +279,9 @@ class _RoundingPointModel:
         ids = ctx_ids.to(device=self.device, dtype=torch.long)
         B, L = ids.shape
         pad = (ids == EOS_ID).int().cumsum(-1) > 0
-        if self.bug == "eos_mask_off_by_one":
+        if self.bug == "eos_mask_eos_only":
+            pad = ids == EOS_ID
+        elif self.bug == "eos_mask_off_by_one":
             pad = torch.cat([pad.new_zeros((B, 1)), pad[:, :-1]], dim=1)
         return self._decode(ids, self._memory(memory), self._pos(B, L), self._cloze(L), pad)
 

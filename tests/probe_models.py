@@ -92,6 +92,9 @@ class Probe:
     forced: Optional[torch.Tensor] = None
     context: Optional[torch.Tensor] = None
     over: dict = field(default_factory=dict)    # create_model overrides
+    # BUGS name -> the decoder passes it moves (DEC_PASSES names); a bug not listed moves every pass, and the passes a
+    # listed bug leaves out stay bit-identical in the fp64 model
+    moves: dict = field(default_factory=dict)
 
     # -- the fp64 model and the output it is compared on ----------------------------------------------------------------
     def encoder_model(self, accum=torch.float64, bug=None, device="cpu"):
@@ -114,6 +117,24 @@ class Probe:
         if pass_ == "refine":
             return m.refine(mem, self.context)
         return m.nar(mem, self.cfg.max_label_length + 1)
+
+    def score_terms(self, logits=None, **kw):
+        """The terms `score` returns for the teacher-forced candidates of the AR pass: candidate b is forced[b, 1:] up to
+        its first EOS (c_1..c_n), and term i <= n is log_softmax(logits[b, i])[t_i] with t = (c_1..c_n, EOS); 0 past n."""
+        lg = self.expected(pass_="ar", **kw) if logits is None else logits
+        return teacher_forced_terms(lg, self.forced)
+
+
+def teacher_forced_terms(logits: torch.Tensor, forced: torch.Tensor) -> torch.Tensor:
+    """[B, L] terms of the AR logits [B, L, C] under teacher forcing `forced` [B, L] (BOS first): see Probe.score_terms."""
+    B, L, _ = logits.shape
+    f = forced.to(logits.device).long()
+    t = torch.cat([f[:, 1:], torch.zeros_like(f[:, :1])], dim=1)          # EOS = 0 after the last position
+    eos = (t == 0).int()
+    n = torch.where(eos.any(1), eos.argmax(1), torch.full((B,), L - 1, device=f.device))
+    t[torch.arange(B), n] = 0
+    lp = torch.log_softmax(logits.double(), dim=-1).gather(-1, t[..., None])[..., 0]
+    return torch.where(torch.arange(L, device=f.device)[None] <= n[:, None], lp, torch.zeros_like(lp))
 
 
 # ---- the encoder --------------------------------------------------------------------------------------------------
@@ -149,14 +170,18 @@ def _encoder_base(cfg, seed: int, amp: float, tied=()):
     return sd, n, pat
 
 
-def _loud_head(sd, depth):
-    """Head columns of the flip pairs at +-1/4, so that a flip moves every logit by 1."""
+def _loud_head(sd, depth, classwise=False):
+    """Head columns of the flip pairs at +-1/4, so that a flip moves every logit by 1.  classwise: the column of flip
+    pair (l, i) is +1/4 for class c when bit (4 l + i) mod 6 of c is set and -1/4 otherwise, so that a flip moves the
+    classes' logits apart and log_softmax (scoring) sees it; every logit still moves by 1."""
     W = sd["head.weight"]
+    c = torch.arange(W.shape[0])
     for l in range(depth):
         for i in range(4):
             r = 2 * _flip_pair(l, i)
-            W[:, r] = 0.25
-            W[:, r + 1] = -0.25
+            w = torch.where((c >> ((4 * l + i) % 6)) & 1 == 1, 0.25, -0.25) if classwise else 0.25
+            W[:, r] = w
+            W[:, r + 1] = -w
 
 
 def _config(key, **over):
@@ -344,19 +369,20 @@ def _decoder_base(key, seed, amp, T=None, extra_chars=0, mll=25):
     s = _pattern(1, D, seed)[0]
     s[: 2 * (_TIED + 1)] = torch.tensor([1.0, -1.0, 1.0, -1.0])
     sd["pos_queries"] = (amp * s).expand(1, L, D).clone()
-    _loud_head(sd, depth)
+    _loud_head(sd, depth, classwise=True)
     return cfg, sd, over
 
 
-def _dec_probe(name, key, cfg, sd, covers, tol, over, seed) -> Probe:
-    B, L, C = 2, cfg.max_label_length + 1, cfg.num_classes
+def _dec_probe(name, key, cfg, sd, covers, tol, over, seed, B=2, ctx=None, moves=None) -> Probe:
+    L, C = cfg.max_label_length + 1, cfg.num_classes
     bos = cfg.num_tokens - 2
     forced = forced_ar_ids(B, L, C, bos, 100 + seed)
-    ctx = refine_context(B, L, C, bos, [3, None], 200 + seed)
+    if ctx is None:
+        ctx = refine_context(B, L, C, bos, [3, None], 200 + seed)
     tag = (f"-T{cfg.num_patches}" if "img_size" in over else "") + (f"-C{C}" if "charset_train" in over else "") + \
         (f"-L{L}" if "max_label_length" in over else "")
-    return Probe(f"{name}-{_kname(key)}{tag}", key, cfg, sd, _images(cfg), covers, tol, decoder=True, forced=forced,
-                 context=ctx, over=over)
+    return Probe(f"{name}-{_kname(key)}{tag}", key, cfg, sd, _images(cfg, B), covers, tol, decoder=True, forced=forced,
+                 context=ctx, over=over, moves=moves or {})
 
 
 def dec_cross(key, T=None, extra_chars=0, mll=25, seed=5) -> Probe:
@@ -424,6 +450,169 @@ def dec_ln_eps(key, T=None, extra_chars=0, mll=25, seed=6) -> Probe:
     return _dec_probe("dec_ln_eps", key, cfg, sd, [("ln_eps", key)], 1e-4, over, seed)
 
 
+# ---- the decoder self-attention --------------------------------------------------------------------------------------
+# pairs of the self-attention probes: a 7-bit position code (bit j on pair _CODE + j) and one token-indicator pair
+_CODE, _NBITS = _flip_pair(2, 0), 7
+_TOK = _CODE + _NBITS
+SELF_B = 7                      # images per self-attention probe, each with its own ids and its own first EOS
+SELF_EOS = {26: (3, 1, 12, 24, 25, 8, None), 64: (1, 31, 32, 33, 63, 8, None)}     # first EOS of image b (b mod 7)
+_AR, _REFINE, _NAR = ("ar", "ar-cluster", "score"), ("refine",), ("nar",)
+
+
+def marked(ids: torch.Tensor) -> torch.Tensor:
+    """The token indicator of dec_self_order: odd ids (EOS = 0 is unmarked, BOS has its own row)."""
+    return ids % 2 == 1
+
+
+def self_context(B, L, C, bos, first_eos, seed):
+    """Refinement contexts [B, L] without EOS but at first_eos[b % len(first_eos)] (None: no EOS).  Where the last key
+    has the parity of the key before the first EOS, it is an EOS too, so that the latest key a padding mask with a hole
+    lets through has the other parity."""
+    g = torch.Generator().manual_seed(seed)
+    ids = torch.randint(1, max(C, 2), (B, L), generator=g, dtype=torch.int32)
+    for b in range(B):
+        e = first_eos[b % len(first_eos)]
+        if e is not None:
+            ids[b, e] = 0
+            if e < L - 2 and (L - 1) % 2 == (e - 1) % 2:
+                ids[b, L - 1] = 0
+    ids[:, 0] = bos
+    return ids
+
+
+def _self_rows(sd, cfg):
+    """pos_queries[j] carries the code of j + 1 on the code pairs and -1 on the token pair; BOS's embedding the full row
+    with code 0, every other token's embedding +-2 on the token pair where marked() and 0 elsewhere, so that context row
+    k (BOS, or sqrt(D) E[id] + pos_queries[k - 1]) is a +-1 pattern whose code is k and whose token pair is +1 on
+    marked ids."""
+    D = cfg.embed_dim
+    L = cfg.max_label_length + 1
+    s = sd["pos_queries"][0].view(L, D // 2, 2)[:, :, 0].clone()       # every row the shared pattern
+    for j in range(_NBITS):
+        s[:, _CODE + j] = torch.tensor([1.0 if ((q + 1) >> j) & 1 else -1.0 for q in range(L)])
+    s[:, _TOK] = -1.0
+    sd["pos_queries"] = torch.stack([s, -s], dim=-1).reshape(1, L, D).float().contiguous()
+    E = torch.zeros_like(sd["text_embed.embedding.weight"])
+    rs = math.sqrt(D)
+    m = marked(torch.arange(E.shape[0]))
+    E[m, 2 * _TOK] = 2.0 / rs
+    E[m, 2 * _TOK + 1] = -2.0 / rs
+    bos = s[0].clone()
+    bos[_CODE: _CODE + _NBITS] = -1.0
+    E[cfg.num_tokens - 2] = torch.stack([bos, -bos], dim=-1).reshape(D) / rs
+    sd["text_embed.embedding.weight"] = E
+
+
+def dec_self_order(key, T=None, extra_chars=0, mll=25, seed=7) -> Probe:
+    """Which keys the self-attention sees.  Context row k carries the 7-bit code of k (BOS 0) and a token indicator.
+    Every layer l, three heads with queries from the bias alone:
+      head 0: key k scores 64 (k - 64), so the latest visible key wins by e^-64; v = the parity of k: flips pair (l, 0)
+              when the latest visible key is odd;
+      head 1: the same scores, v = the token indicator of the latest visible key (the image's own id there): pair (l, 1);
+      head 2: key k scores -64 (k + 1), the earliest visible key (BOS) wins and the running max never moves; v = 1 on
+              even keys: pair (l, 2);
+      head 3 (layers l >= 1): head 0's scores, v = 1 where the key's content row kept pair (l - 1, 0) unflipped in
+              layer l - 1, i.e. where the latest key that content row saw under the content mask was even: pair (l, 3).
+              So a content mask off by one key moves the output at depth >= 2.
+    A mask that lets a later key through or hides the latest one (a causal leak, a dropped own key, a padding mask
+    starting one late or hiding only EOS keys, a cloze mask on the wrong key) moves the latest visible key, and an
+    extra zero key (score 0) takes every head's weight.  Ids and first EOS differ per image, so a read of another
+    image's ids, table rows or cache rows flips head 1."""
+    cfg, sd, over = _decoder_base(key, seed, 1.0, T, extra_chars, mll)
+    D, h = cfg.embed_dim, cfg.dec_num_heads
+    d = D // h
+    rs = math.sqrt(d)
+    L, C = cfg.max_label_length + 1, cfg.num_classes
+    _self_rows(sd, cfg)
+    top = 32 * (2 ** _NBITS - 1)                             # sum of the code weights 32 * 2^j
+    for l in range(cfg.dec_depth):
+        p = f"decoder.layers.{l}.self_attn."
+        W, b = sd[p + "in_proj_weight"], sd[p + "in_proj_bias"]
+        for hd, sign, offset in ((0, 1.0, 32.0), (1, 1.0, 32.0), (2, -1.0, top + 64.0)):
+            o = hd * d
+            for j in range(_NBITS):
+                b[o + j] = sign * 32.0 * 2 ** j * rs         # score = sum_j 32 * 2^j * (+-1) - offset
+                W[D + o + j, 2 * (_CODE + j)] = 1.0
+            b[o + _NBITS] = -offset * rs
+            b[D + o + _NBITS] = 1.0
+        W[2 * D: 2 * D + d, 2 * _CODE], b[2 * D: 2 * D + d] = 0.5, 0.5                  # parity
+        W[2 * D + d: 2 * D + 2 * d, 2 * _TOK], b[2 * D + d: 2 * D + 2 * d] = 0.5, 0.5    # token indicator
+        W[2 * D + 2 * d: 2 * D + 3 * d, 2 * _CODE], b[2 * D + 2 * d: 2 * D + 3 * d] = -0.5, 0.5   # even
+        heads = 3
+        if l >= 1:                                           # head 3: the content stream's own result of layer l - 1
+            heads = 4
+            o = 3 * d
+            for j in range(_NBITS):
+                b[o + j] = 32.0 * 2 ** j * rs
+                W[D + o + j, 2 * (_CODE + j)] = 1.0
+            b[o + _NBITS] = -32.0 * rs
+            b[D + o + _NBITS] = 1.0
+            W[2 * D + o: 2 * D + o + d, 2 * _flip_pair(l - 1, 0)], b[2 * D + o: 2 * D + o + d] = 0.5, 0.5
+        Wo = sd[p + "out_proj.weight"]
+        for hd in range(heads):
+            r = 2 * _flip_pair(l, hd)
+            Wo[r, hd * d: (hd + 1) * d] = -2.0 / d           # (+1, -1) + 2 v (-1, +1): flips when v = 1
+            Wo[r + 1, hd * d: (hd + 1) * d] = 2.0 / d
+    ctx = self_context(SELF_B, L, C, cfg.num_tokens - 2, SELF_EOS[26 if L <= 32 else 64], 300 + seed)
+    bugs = {"self_extra_zero_key": _AR + _REFINE + _NAR, "self_mask_leak": _AR + _REFINE, "self_drop_own_key": _AR,
+            "cloze_mask_shift": _REFINE, "eos_mask_off_by_one": _REFINE, "eos_mask_eos_only": _REFINE}
+    return _dec_probe("dec_self_order", key, cfg, sd, [(bug, key) for bug in bugs], 1e-4, over, seed, B=SELF_B,
+                      ctx=ctx, moves=bugs)
+
+
+def dec_self_query(key, T=None, extra_chars=0, mll=25, seed=8) -> Probe:
+    """The self-attention's LayerNorms and query precision.  The query stream and the context rows at amplitude delta
+    (row variance ~ 2e-5), where eps 1e-6 instead of 1e-5 raises the LayerNorm gain from 0.81 to 0.98; BOS's row has
+    the key indicator (pair 0) at -1, every other context row at +1.  Every layer l:
+      head 0: the query reads norm_q's gain through the shared pattern and scores every key but BOS 113 or more below
+              BOS at the right gain, above it at the bug's; v = (norm_c's key indicator + 0.8125) / 2, which is 0 on BOS
+              at norm_c's right gain only: adds 2^-4 sum(v) to pair (l, 0);
+      head 1: q = (1 + 2^-9, -1, 1) against keys -2^14 (s, s) and 16 s of the indicator s: BOS scores 13 and the others
+              -13: q's bits below bf16 carry 2^14 * 2^-9 = 32 of the dot product with each key's indicator, 26 at
+              gain 0.8125, which decides the sign; a bf16 q lets the others win by 26.  Same v and output, on pair
+              (l, 1).
+    With a single key (NAR, AR query 0) only norm_c's gain is seen, through v."""
+    cfg, sd, over = _decoder_base(key, seed, 1.0, T, extra_chars, mll)
+    eps, eps_bug = 1e-5, 1e-6
+    dl, A, Ab = _ln_amplitude(eps, eps_bug)
+    D, h = cfg.embed_dim, cfg.dec_num_heads
+    d = D // h
+    rs = math.sqrt(d)
+    s = sd["pos_queries"][0, 0].clone()
+    s[: 2 * (_TIED + 1)] = 0.0
+    sd["pos_queries"] = (dl * sd["pos_queries"]).float()
+    E = torch.zeros_like(sd["text_embed.embedding.weight"])
+    bos = sd["pos_queries"][0, 0].clone()
+    bos[2 * _KEY], bos[2 * _KEY + 1] = -dl, dl
+    E[cfg.num_tokens - 2] = bos / math.sqrt(D)
+    sd["text_embed.embedding.weight"] = E
+    Ah, Abh = float(_bf(A)), float(_bf(Ab))
+    mid = (Ah + Abh) / 2
+    ns = float(s.abs().sum())
+    kappa = 64.0
+    for l in range(cfg.dec_depth):
+        p = f"decoder.layers.{l}.self_attn."
+        W, b = sd[p + "in_proj_weight"], sd[p + "in_proj_bias"]
+        # q_0 (scaled) = g (gain_q - mid) < 0; k_0 = kappa gain_c s_key: the other keys score q_0 * 2 kappa gain_c
+        # against BOS, at least 120 below it at the right gains and 120 above it at norm_q's bug
+        g = 120.0 / (2 * kappa * Ah) / min(mid - Ah, Abh - mid)
+        w = float(_bf(g * rs / ns))
+        W[0] = w * s
+        b[0] = -w * ns * mid
+        W[D, 2 * _KEY] = kappa
+        b[d], b[d + 1], b[d + 2] = (1 + 2.0 ** -9) * rs, -1.0 * rs, 1.0 * rs
+        W[D + d, 2 * _KEY], W[D + d + 1, 2 * _KEY], W[D + d + 2, 2 * _KEY] = -2.0 ** 14, -2.0 ** 14, 16.0
+        W[2 * D: 2 * D + 2 * d, 2 * _KEY], b[2 * D: 2 * D + 2 * d] = 0.5, 0.5 * Ah
+        Wo = sd[p + "out_proj.weight"]
+        Wo[2 * _flip_pair(l, 0), :d] = 2.0 ** -4
+        Wo[2 * _flip_pair(l, 1), d: 2 * d] = 2.0 ** -4
+    L, C = cfg.max_label_length + 1, cfg.num_classes
+    ctx = self_context(SELF_B, L, C, cfg.num_tokens - 2, SELF_EOS[26 if L <= 32 else 64], 400 + seed)
+    bugs = {"norm_qc_eps": _AR + _REFINE + _NAR, "self_q_bf16": _AR + _REFINE}
+    return _dec_probe("dec_self_query", key, cfg, sd, [(bug, key) for bug in bugs], 1e-4, over, seed, B=SELF_B,
+                      ctx=ctx, moves=bugs)
+
+
 def _kname(key):
     return f"{'D' if isinstance(key[0], int) else ''}{key[0]}-depth{key[1]}"
 
@@ -434,6 +623,8 @@ WIDE_EXTRA = 100                # 195 head classes: the cluster kernel's class-s
 # T = 32, 65, 130 and 240 put key T inside a K/V box (zero-filled rows past the last key); at 256 the last key ends the
 # last box, where a dropped last key, not an extra one, is what could go wrong
 CROSS_T = (32, 65, 130, 240, 256)
+SELF_KINDS = (dec_self_order, dec_self_query)
+DEC_KINDS = (dec_cross, dec_ln_eps) + SELF_KINDS
 
 
 def all_probes():
@@ -444,10 +635,11 @@ def all_probes():
         if key[0] in ("vitstr", "vitstr-tail"):
             out.append((vitstr_rounding, (key,)))
     for key in DECODER_KEYS:
-        out += [(dec_cross, (key,)), (dec_ln_eps, (key,))]
+        out += [(fn, (key,)) for fn in DEC_KINDS]
+        out += [(fn, (key, None, 0, 63)) for fn in SELF_KINDS if key[1] > 1]    # depth 2 at L = 64
     for D in (192, 384, 768):                   # the class-sliced head (195 classes) and ids pitch 64 (L = 64)
         for extra, mll in ((WIDE_EXTRA, 25), (0, 63), (WIDE_EXTRA, 63)):
-            out += [(dec_cross, ((D, 1), None, extra, mll)), (dec_ln_eps, ((D, 1), None, extra, mll))]
+            out += [(fn, ((D, 1), None, extra, mll)) for fn in DEC_KINDS]
     for T in CROSS_T:
         out.append((dec_cross, ((384, 1), T)))
     return out

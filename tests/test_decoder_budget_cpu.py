@@ -7,9 +7,11 @@ pass over random ids.  Two kinds of variant are compared with it, pass by pass, 
     like: it must stay within half of every bound of decoder_reference.BOUNDS;
   * each injected bug of decoder_reference.BUGS: it must exceed some bound by 2x or more in some pass.
 So the bounds that tests/test_gpu_decoder_isolated.py holds the engine to sit at least 2x above the stand-in's noise and
-at least 2x below each of these mistakes, except where EXCLUDED says, with the numbers, that no bound can be:
-the three smallest bugs at D >= 384 and at depth 2, where a correct decoder's noise is within 2x of them.  At D = 192
-they exceed the bounds by 2x to 2.7x while the engine stays 1.8x or more below them."""
+at least 2x below each of these mistakes, except where EXCLUDED says, with the numbers, that no bound can be: at
+D >= 384 and at depth 2 the three smallest bugs (ln_eps, cross_extra_zero_key, cross_q_bf16) and self_q_bf16, and at
+depth 2 also norm_qc_eps, where a correct decoder's noise is within 2x of them.  At D = 192 they exceed the bounds by
+2x or more while the engine stays 1.8x or more below them.  The probes of tests/probe_models.py cover every excluded
+entry (tests/test_probe_separation_cpu.py)."""
 import functools
 
 import pytest
@@ -26,14 +28,17 @@ B, L = 8, 26
 _SMALL = ("ln_eps", "cross_extra_zero_key", "cross_q_bf16")
 EXCLUDED = {
     # bugs 2.23e-3 / 2.15e-3 / 2.29e-3; the stand-in's median is 4e-7, but the engine's reaches 1.07e-3 (the 2-class head;
-    # 3e-4 to 6e-4 elsewhere), so the median bound is 1.6e-3 and these bugs exceed it by 1.3x to 1.4x only
-    (384, 1): _SMALL,
+    # 3e-4 to 6e-4 elsewhere), so the median bound is 1.6e-3 and these bugs exceed it by 1.3x to 1.4x only.
+    # self_q_bf16: median 3.03e-3, 1.9x the bound
+    (384, 1): _SMALL + ("self_q_bf16",),
     # bugs 2.05e-3 / 9.1e-4 / 2.61e-3; stand-in 2.2e-4; the engine reaches 1.9e-3 (chain at L = 64), so the median
-    # bound is 2.6e-3 and the bugs' means (2.5e-3 / 1.3e-3 / 3.1e-3) stay under the engine's 2.4e-3 x 1.5 too
-    (768, 1): _SMALL,
+    # bound is 2.6e-3 and the bugs' means (2.5e-3 / 1.3e-3 / 3.1e-3) stay under the engine's 2.4e-3 x 1.5 too.
+    # self_q_bf16: median 3.86e-3, 1.5x the bound
+    (768, 1): _SMALL + ("self_q_bf16",),
     # bugs 3.1e-3 / 3.1e-3 / 3.2e-3; the stand-in's own median is 1.7e-3: a second layer carries the flips of the first
-    # into every row, so the bound cannot be below 3.5e-3
-    (384, 2): _SMALL,
+    # into every row, so the bound cannot be below 3.5e-3.  norm_qc_eps: median 5.74e-3, 1.6x the bound;
+    # self_q_bf16: median 3.82e-3, 1.1x
+    (384, 2): _SMALL + ("norm_qc_eps", "self_q_bf16"),
 }
 CASES = sorted(BOUNDS)
 

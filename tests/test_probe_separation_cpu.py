@@ -2,7 +2,9 @@
 
 For every probe, on the CPU: the fp32 stand-in (the probe's fp64 model with fp32 arithmetic, i.e. what a correct engine
 looks like) is within 1/10 of the probe's tolerance, and each bug the probe covers moves its output by 10x the tolerance
-or more, in every decoder pass (AR with and without the cluster kernel's hi + lo operands, refinement, NAR).  And the
+or more, in every decoder output (AR with and without the cluster kernel's hi + lo operands, refinement, NAR, and the
+log_softmax terms `score` returns for the AR pass's teacher-forced candidates) or in the outputs the probe lists for it (`Probe.moves`: a mask bug of the refinement cannot touch AR); every pass it leaves out
+stays bit-identical, so the list cannot go stale.  And the
 probes cover every bug the budget tests leave out: each (budget key, bug) pair of the EXCLUDED tables of
 test_encoder_budget_cpu.py and test_decoder_budget_cpu.py is covered by some probe at that key, so an entry added there
 without a probe fails here."""
@@ -37,7 +39,9 @@ def _outputs(p, **kw):
     if not p.decoder:
         return {"encoder": p.expected(**kw)}
     mem = p.memory()
-    return {f"{ps}{'-cluster' if cl else ''}": p.expected(pass_=ps, cluster=cl, memory=mem, **kw) for ps, cl in DEC_PASSES}
+    out = {f"{ps}{'-cluster' if cl else ''}": p.expected(pass_=ps, cluster=cl, memory=mem, **kw) for ps, cl in DEC_PASSES}
+    out["score"] = pm.teacher_forced_terms(out["ar"], p.forced)
+    return out
 
 
 @functools.lru_cache(maxsize=None)
@@ -71,10 +75,15 @@ def test_every_covered_bug_is_10x_over_the_tolerance(entry):
     ref = _reference(*entry)
     for bug in sorted({b for b, _ in p.covers}):
         got = _outputs(p, bug=bug)
+        moved = p.moves.get(bug, tuple(ref))
+        assert set(moved) <= set(ref), (bug, moved)
         for k in ref:
             e = _err(got[k], ref[k])
             print(f"{p.name} {bug} {k}: {e:.2e} = {e / p.tol:.0f}x the tolerance")
-            assert e >= 10 * p.tol, (bug, k, e)
+            if k in moved:
+                assert e >= 10 * p.tol, (bug, k, e)
+            else:
+                assert torch.equal(got[k], ref[k]), (bug, k, "moves a pass the probe does not list", e)
 
 
 def test_every_excluded_bug_is_covered_by_a_probe():

@@ -151,6 +151,35 @@ typedef struct parseq_crops {
 /* out_hwc: DEVICE uint8 [N, img_h, img_w, 3], what T.Resize(img_size, BICUBIC) makes of each (rotated) crop.  The
  * metadata is checked on the host before anything is launched (PARSEQ_ERR_INVALID_ARG). */
 int parseq_resize_crops(parseq_engine* e, int32_t batch, const parseq_crops* crops, uint8_t* out_hwc, parseq_stream_t stream);
+/* Text regions of full frames (a detector's quadrilaterals) -> rectified crops that every raw-crop entry point takes.
+ * Region i is crop size (h_i, w_i) and the 8 coefficients a0..a7 of PIL's PERSPECTIVE transform, which map output
+ * point (u, v) to frame point x = (a0 u + a1 v + a2) / (a6 u + a7 v + 1), y = (a3 u + a4 v + a5) / (a6 u + a7 v + 1).
+ * Its bytes are exactly frame.transform((w, h), Image.Transform.PERSPECTIVE, coeffs, Image.Resampling.BICUBIC) of the
+ * RGB frame (Pillow's Geometry.c): per output pixel (x, y) the point (x + .5, y + .5) is mapped in fp64 in that order;
+ * a point outside [0, W) x [0, H) gives 0; otherwise the 4 x 4 BICUBIC of Geometry.c (rows first, taps clamped to the
+ * frame) gives v, written as 0 if v <= 0, 255 if v >= 255, else (uint8)v (truncation).  For a quadrilateral TL, TR, BR,
+ * BL the Python layer derives (h, w) and the coefficients (Heckbert's square-to-quad map, parseq_b200/regions.py); an
+ * integer box gives a = (1, 0, x0, 0, 1, y0, 0, 0), the crop frame[y0:y1, x0:x1] with 0 outside the frame.
+ * One kernel thread per output pixel; a crop's bytes depend only on its own frame, size and coefficients. */
+typedef struct parseq_regions {
+  const uint8_t* frames;         /* DEVICE packed HWC RGB bytes of all frames */
+  int64_t frames_bytes;
+  const int64_t* frame_offsets;  /* HOST int64 [F]: byte offset of frame f in frames */
+  const int32_t* frame_sizes;    /* HOST int32 [F][2]: (H, W) of frame f, 1 <= H, W <= 32768 */
+  int32_t num_frames;            /* F */
+  const int32_t* frame_index;    /* HOST int32 [M]: the frame of region i */
+  const int32_t* sizes;          /* HOST int32 [M][2]: (h, w) of crop i, 1 <= h, w <= 8192 */
+  const double* coeffs;          /* HOST double [M][8]: PIL PERSPECTIVE order, output (x + .5, y + .5) -> frame */
+} parseq_regions;
+/* out: DEVICE uint8, the M crops [h_i, w_i, 3] back to back (crop i at byte sum_{j<i} 3 h_j w_j), out_bytes at least
+ * that sum.  Checked on the host before anything is enqueued, also without a handle (PARSEQ_ERR_INVALID_ARG): null
+ * pointers, count < 0, frame sides outside [1, 32768] or frame bytes past frames_bytes, frame_index out of range, crop
+ * sides outside [1, 8192], non-finite coefficients, a denominator a6 x + a7 y + 1 that is not positive at one of the
+ * four corner pixel centres (then it is positive at every pixel centre), and out_bytes too small.  The region table is
+ * uploaded per chunk of max_batch regions; the call runs on the engine's main stream, ordered after the caller's
+ * earlier work on `stream`, and needs no weights. */
+int parseq_warp_regions(parseq_engine* e, int32_t count, const parseq_regions* regions, uint8_t* out, int64_t out_bytes,
+                        parseq_stream_t stream);
 /* parseq_forward_u8 / parseq_forward_host_u8 on the resized crops; args->batch = N.  No teacher forcing.  The host
  * variant uploads each super-chunk's bytes on the engine's copy stream (in two halves from 256 crops up, PARSeq). */
 int parseq_forward_crops(parseq_engine* e, const parseq_forward_args* args, const parseq_crops* crops, float* logits,

@@ -10,7 +10,7 @@ CSRC = os.path.join(PKG, "csrc")
 LIB_DIR = os.path.join(PKG, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libparseq_b200.so")
 SOURCES = ["engine.cu"]
-HEADERS = ["ptx.cuh", "gemm.cuh", "gemm_body.inc", "kernels.cuh", "dec_ar.cuh", "dec_ar2.cuh", "gemm_ln.cuh", "mlp_ln.cuh", "attn_wgmma.cuh", "qkv_attn.cuh", "crops.cuh", "orient.cuh", "owners.h", os.path.join("..", "..", "include", "parseq_b200.h")]
+HEADERS = ["ptx.cuh", "gemm.cuh", "gemm_body.inc", "kernels.cuh", "dec_ar.cuh", "dec_ar2.cuh", "gemm_ln.cuh", "mlp_ln.cuh", "attn_wgmma.cuh", "qkv_attn.cuh", "crops.cuh", "regions.cuh", "orient.cuh", "owners.h", os.path.join("..", "..", "include", "parseq_b200.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

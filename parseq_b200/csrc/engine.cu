@@ -28,6 +28,7 @@
 #include "attn_wgmma.cuh"
 #include "qkv_attn.cuh"
 #include "crops.cuh"
+#include "regions.cuh"
 #include "orient.cuh"
 #include "owners.h"
 
@@ -664,6 +665,7 @@ struct Workspace {
   DevBuf<uint8_t> in_images_u8;     // static input of the uint8 HWC entry points
   DevBuf<uint32_t> in_mask;         // [max_batch, mask_ld] class allowlist rows of the super-chunk (graphs, host entry points)
   DevBuf<pq::CropDesc> crop_tab;    // the resize kernel's crop table [max_batch] (raw-crop entry points, crops.cuh)
+  DevBuf<pq::RegionDesc> reg_tab;   // the warp kernel's region table [max_batch], allocated by the first parseq_warp_regions
   // candidate scoring: the call's metadata (ids, targets, row tables; grown on demand), one causal [P][P] mask per
   // P = 1..L (mask of P at sc_causal + (P - 1) * L * L), and ViTSTR's LSE partials of a chunk's (image, position) rows
   DevBuf<int> sc_meta;
@@ -730,6 +732,7 @@ struct parseq_engine : Workspace {
   // of a super-chunk's packed bytes for the host entry point (grown on demand)
   std::vector<pq::CropDesc> crop_descs;
   long long crop_base = 0;
+  std::vector<pq::RegionDesc> reg_descs;   // parseq_warp_regions: the host copy of a chunk's region table (regions.cuh)
   DevBuf<uint8_t> crop_stage;
   bool use_graph = true;
   long long orient_rereads = 0, orient_readings = 0;   // pass 2 of the last oriented call: crops re-read, readings run
@@ -1899,6 +1902,51 @@ int check_crops_call(parseq_engine* e, const parseq_forward_args* a, const parse
   return check_crop_smem(e, a->batch, crops);
 }
 
+// ---------------------------------------------------------------- text regions of full frames (regions.cuh)
+// The metadata of a parseq_warp_regions call, on the host alone (no handle or device needed), before anything is
+// enqueued.  *packed: the bytes of all rectified crops, sum of 3 h w.
+int check_regions(int count, const parseq_regions* r, const uint8_t* out, long long out_bytes, long long* packed) {
+  if (r == nullptr || count < 0) return fail(PARSEQ_ERR_INVALID_ARG, "null argument or negative count");
+  *packed = 0;
+  if (count == 0) return PARSEQ_OK;
+  if (r->frames == nullptr || r->frame_offsets == nullptr || r->frame_sizes == nullptr || r->frame_index == nullptr ||
+      r->sizes == nullptr || r->coeffs == nullptr || out == nullptr)
+    return fail(PARSEQ_ERR_INVALID_ARG, "null frames, frame_offsets, frame_sizes, frame_index, sizes, coeffs or out");
+  if (r->num_frames < 1) return fail(PARSEQ_ERR_INVALID_ARG, "num_frames must be >= 1");
+  for (int f = 0; f < r->num_frames; ++f) {
+    const int H = r->frame_sizes[2 * f], W = r->frame_sizes[2 * f + 1];
+    if (H < 1 || W < 1 || H > pq::REGION_MAX_FRAME_SIDE || W > pq::REGION_MAX_FRAME_SIDE)
+      return fail(PARSEQ_ERR_INVALID_ARG, "frame " + std::to_string(f) + ": size " + std::to_string(H) + " x " +
+                                              std::to_string(W) + ", sides must be in [1, 32768]");
+    if (r->frame_offsets[f] < 0 || r->frame_offsets[f] > r->frames_bytes - 3ll * H * W)
+      return fail(PARSEQ_ERR_INVALID_ARG, "frame " + std::to_string(f) + ": offset + 3 H W exceeds frames_bytes");
+  }
+  for (int i = 0; i < count; ++i) {
+    const std::string at = "region " + std::to_string(i) + ": ";
+    if (r->frame_index[i] < 0 || r->frame_index[i] >= r->num_frames)
+      return fail(PARSEQ_ERR_INVALID_ARG, at + "frame_index " + std::to_string(r->frame_index[i]) + " out of range");
+    const int h = r->sizes[2 * i], w = r->sizes[2 * i + 1];
+    if (h < 1 || w < 1 || h > pq::REGION_MAX_SIDE || w > pq::REGION_MAX_SIDE)
+      return fail(PARSEQ_ERR_INVALID_ARG, at + "size " + std::to_string(h) + " x " + std::to_string(w) +
+                                              ", sides must be in [1, 8192]");
+    const double* a = r->coeffs + 8ll * i;
+    for (int k = 0; k < 8; ++k)
+      if (!std::isfinite(a[k])) return fail(PARSEQ_ERR_INVALID_ARG, at + "non-finite coefficient");
+    // the denominator is affine in the output point: positive at the four corner pixel centres, it is positive at
+    // every pixel centre, so the kernel's divisions never meet 0 or a sign change
+    for (int k = 0; k < 4; ++k) {
+      const double xin = (k & 1) ? w - 0.5 : 0.5, yin = (k & 2) ? h - 0.5 : 0.5;
+      if (!(a[6] * xin + a[7] * yin + 1.0 > 0.0))
+        return fail(PARSEQ_ERR_INVALID_ARG, at + "the map's denominator a6 x + a7 y + 1 is not positive at a corner");
+    }
+    *packed += 3ll * h * w;
+  }
+  if (out_bytes < *packed)
+    return fail(PARSEQ_ERR_INVALID_ARG, "out_bytes (" + std::to_string(out_bytes) + ") is smaller than the packed crops (" +
+                                            std::to_string(*packed) + ")");
+  return PARSEQ_OK;
+}
+
 // The causal masks of every row count P (scoring, and the map pass of AR-only schedules), on first use.
 int causal_reserve(parseq_engine* e) {
   if (e->sc_causal != nullptr) return PARSEQ_OK;
@@ -2921,6 +2969,45 @@ int parseq_resize_crops(parseq_engine* e, int32_t batch, const parseq_crops* cro
     const int Bc = (batch - b0 < e->max_batch) ? (batch - b0) : e->max_batch;
     PQ_TRY(crops_table(e, cb, b0, Bc, e->main));
     PQ_TRY(crops_resize(e, cb, b0, 0, Bc, out_hwc + 3ll * e->cfg.img_h * e->cfg.img_w * b0, e->main));
+  }
+  return leave_main(e, user);
+}
+
+int parseq_warp_regions(parseq_engine* e, int32_t count, const parseq_regions* r, uint8_t* out, int64_t out_bytes,
+                        parseq_stream_t stream) {
+  long long packed = 0;
+  PQ_TRY(check_regions(count, r, out, out_bytes, &packed));
+  PQ_TRY(check_ready(e, false));
+  if (count == 0) return PARSEQ_OK;
+  PQ_CUDA(cudaSetDevice(e->cfg.device));
+  PQ_TRY(e->reg_tab.grow(e, e->max_batch));
+  cudaStream_t user = reinterpret_cast<cudaStream_t>(stream);
+  PQ_TRY(enter_main(e, user));
+  long long dst = 0;
+  for (int b0 = 0; b0 < count; b0 += e->max_batch) {
+    const int Bc = (count - b0 < e->max_batch) ? (count - b0) : e->max_batch;
+    e->reg_descs.resize(static_cast<size_t>(Bc));
+    long long pixels = 0;                  // of the largest region of the chunk: the grid's tile count
+    for (int i = 0; i < Bc; ++i) {
+      const int g = b0 + i, f = r->frame_index[g];
+      pq::RegionDesc& d = e->reg_descs[static_cast<size_t>(i)];
+      std::memcpy(d.a, r->coeffs + 8ll * g, sizeof(d.a));
+      d.src = r->frame_offsets[f];
+      d.dst = dst;
+      d.fh = r->frame_sizes[2 * f];
+      d.fw = r->frame_sizes[2 * f + 1];
+      d.h = r->sizes[2 * g];
+      d.w = r->sizes[2 * g + 1];
+      dst += 3ll * d.h * d.w;
+      pixels = std::max(pixels, 1ll * d.h * d.w);
+    }
+    // pageable source: the copy is staged when it returns, so reg_descs may change for the next chunk
+    PQ_CUDA(cudaMemcpyAsync(e->reg_tab, e->reg_descs.data(), sizeof(pq::RegionDesc) * Bc, cudaMemcpyHostToDevice, e->main));
+    const dim3 grid(static_cast<unsigned>((pixels + pq::REGION_THREADS - 1) / pq::REGION_THREADS), static_cast<unsigned>(Bc));
+    TimedScope ts(e, e->main, CAT_MISC, 0.0);
+    // no PDL: the kernel reads the table copy and the caller's frames
+    PQ_TRY(launch_ex(LaunchConfig(grid, dim3(pq::REGION_THREADS), 0, e->main, 0, false), pq::region_warp_kernel,
+                     r->frames, static_cast<const pq::RegionDesc*>(e->reg_tab), out));
   }
   return leave_main(e, user);
 }

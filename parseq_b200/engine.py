@@ -29,6 +29,12 @@ class CropsC(C.Structure):
                 ("rotation", C.c_int32), ("rotations", C.c_void_p)]
 
 
+class RegionsC(C.Structure):
+    _fields_ = [("frames", C.c_void_p), ("frames_bytes", C.c_int64), ("frame_offsets", C.c_void_p),
+                ("frame_sizes", C.c_void_p), ("num_frames", C.c_int32), ("frame_index", C.c_void_p), ("sizes", C.c_void_p),
+                ("coeffs", C.c_void_p)]
+
+
 class OrientArgsC(C.Structure):
     _fields_ = [("num_orientations", C.c_int32), ("orientations", C.c_int32 * 4), ("min_confidence", C.c_float),
                 ("rotation_out", C.c_void_p), ("confidence_out", C.c_void_p)]
@@ -93,7 +99,7 @@ class LexiconHandle:
 EXPORTS = [
     "parseq_create", "parseq_destroy", "parseq_set_weight", "parseq_num_weights", "parseq_weight_key",
     "parseq_finalize", "parseq_forward", "parseq_forward_host", "parseq_forward_u8", "parseq_forward_host_u8",
-    "parseq_resize_crops", "parseq_forward_crops", "parseq_forward_host_crops", "parseq_forward_crops_oriented",
+    "parseq_resize_crops", "parseq_warp_regions", "parseq_forward_crops", "parseq_forward_host_crops", "parseq_forward_crops_oriented",
     "parseq_score", "parseq_score_u8", "parseq_score_check", "parseq_beam_search", "parseq_beam_search_u8",
     "parseq_lexicon_check", "parseq_lexicon_create", "parseq_lexicon_destroy", "parseq_beam_search_lexicon",
     "parseq_beam_search_lexicon_u8",
@@ -134,6 +140,7 @@ def load_library(path: Optional[str] = None):
     lib.parseq_forward_u8.argtypes = lib.parseq_forward.argtypes
     lib.parseq_forward_host_u8.argtypes = lib.parseq_forward.argtypes
     lib.parseq_resize_crops.argtypes = [C.c_void_p, C.c_int32, C.POINTER(CropsC), C.c_void_p, C.c_void_p]
+    lib.parseq_warp_regions.argtypes = [C.c_void_p, C.c_int32, C.POINTER(RegionsC), C.c_void_p, C.c_int64, C.c_void_p]
     lib.parseq_forward_crops.argtypes = [C.c_void_p, C.POINTER(ForwardArgsC), C.POINTER(CropsC), C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p]
     lib.parseq_forward_host_crops.argtypes = lib.parseq_forward_crops.argtypes
@@ -308,6 +315,9 @@ class Engine:
 
     def resize_crops(self, crops: CropsC, batch, out_ptr, stream):
         check(self.lib, self.lib.parseq_resize_crops(self.handle, batch, C.byref(crops), out_ptr, stream))
+
+    def warp_regions(self, regions: RegionsC, count, out_ptr, out_bytes, stream):
+        check(self.lib, self.lib.parseq_warp_regions(self.handle, count, C.byref(regions), out_ptr, out_bytes, stream))
 
     def forward_crops(self, crops: CropsC, batch, logits_ptr, ids_ptr, steps_ptr, stream, max_length=None, decode_ar=True,
                       refine_iters=1, host=False, class_mask_ptr=None, attn_maps_ptr=None):

@@ -76,10 +76,42 @@ def _crop_tensor(c) -> Tensor:
     raise TypeError(f"a crop must be a uint8 [h, w, 3] tensor or a PIL image, got {type(c).__name__}")
 
 
+class RegionCrops(list):
+    """The rectified crops of crop_regions: a list of M CUDA uint8 [h, w, 3] views into one packed buffer, so it goes
+    wherever a list of raw crops goes (pack_crops then passes the buffer on without a copy).  Also holds each region's
+    `quads` (float64 [M, 4, 2], TL, TR, BR, BL in frame pixels), `coeffs` (float64 [M, 8], PIL PERSPECTIVE order) and
+    `frame_index` (int64 [M])."""
+
+    def __init__(self, views: List[Tensor], data: Tensor, offsets: Tensor, sizes: Tensor, quads: Tensor, coeffs: Tensor,
+                 frame_index: Tensor):
+        super().__init__(views)
+        self._views = tuple(views)
+        self.data, self.offsets, self.sizes = data, offsets, sizes
+        self.quads, self.coeffs, self.frame_index = quads, coeffs, frame_index
+
+    def packed(self) -> bool:
+        """The list still holds exactly the views of `data` it was made with."""
+        return len(self) == len(self._views) and all(a is b for a, b in zip(self, self._views))
+
+    def to_frame(self, points, i: int) -> Tensor:
+        """Points (x, y) [..., 2] in the pixels of crop i (pixel j covers [j, j + 1); e.g. locate's centres, or the
+        corners of a box) -> the same points in frame pixels, float64, through region i's map."""
+        from .regions import map_points
+        p = points if isinstance(points, Tensor) else torch.as_tensor(points)
+        p = p.to(torch.float64)
+        if p.shape[-1] != 2:
+            raise ValueError(f"points must be [..., 2], got {tuple(p.shape)}")
+        x, y = map_points(self.coeffs[int(i)].tolist(), p[..., 0], p[..., 1])
+        return torch.stack([x, y], dim=-1)
+
+
 def pack_crops(crops: Sequence[Any], pin_memory: bool = False) -> Tuple[Tensor, Tensor, Tensor]:
     """Packs a list of raw crops of any size for the engine's crop entry points: (data, offsets, sizes), with data the
     crops' HWC bytes back to back on the crops' device (pinned if asked, for CPU crops), offsets int64 [N] and sizes
-    int32 [N, 2] = (h, w) on the CPU.  All crops must be on one device; PIL images count as CPU crops."""
+    int32 [N, 2] = (h, w) on the CPU.  All crops must be on one device; PIL images count as CPU crops.  The crops of
+    crop_regions are already packed: their buffer is returned as it is."""
+    if isinstance(crops, RegionCrops) and crops.packed():
+        return crops.data, crops.offsets, crops.sizes
     if not isinstance(crops, (list, tuple)):
         raise TypeError("crops must be a list of uint8 [h, w, 3] tensors or PIL images")
     if len(crops) == 0:
@@ -238,6 +270,26 @@ def check_orientations(orientations: Sequence[int]) -> Tuple[int, ...]:
     if not 1 <= len(o) <= 4 or any(isinstance(x, bool) or x not in ORIENTATIONS for x in o) or len(set(o)) != len(o):
         raise ValueError(f"orientations must be 1 to 4 distinct values of {ORIENTATIONS}, got {orientations!r}")
     return tuple(int(x) for x in o)
+
+
+def _region_quads(regions) -> List[List[Tuple[float, float]]]:
+    """`regions` of crop_regions as M quads of Python floats: corners [M, 4, 2] (TL, TR, BR, BL; any real dtype), or
+    integer boxes [M, 4] = (x0, y0, x1, y1) with x1 > x0 and y1 > y0."""
+    import numpy as np
+    from .regions import box_quad
+    r = regions.detach().cpu().numpy() if isinstance(regions, Tensor) else np.asarray(regions)
+    if r.dtype.kind not in "iuf":
+        raise ValueError(f"regions must be real corners [M, 4, 2] or integer boxes [M, 4], got dtype {r.dtype}")
+    if r.ndim == 3 and r.shape[1:] == (4, 2) and r.shape[0] > 0:
+        return [[(float(x), float(y)) for x, y in q] for q in r.astype(np.float64)]
+    if r.ndim == 2 and r.shape[1] == 4 and r.shape[0] > 0:
+        if r.dtype.kind == "f":
+            raise ValueError("boxes [M, 4] must be integers; give real-valued regions as corners [M, 4, 2]")
+        bad = np.nonzero((r[:, 2] <= r[:, 0]) | (r[:, 3] <= r[:, 1]))[0]
+        if bad.size:
+            raise ValueError(f"box {int(bad[0])}: {r[bad[0]].tolist()} needs x1 > x0 and y1 > y0")
+        return [box_quad(b) for b in r.tolist()]
+    raise ValueError(f"regions must be corners [M, 4, 2] or boxes [M, 4] with M >= 1, got shape {tuple(r.shape)}")
 
 
 def _crop_hw(c) -> Tuple[int, int]:
@@ -485,6 +537,66 @@ class _EngineModule(nn.Module):
         eng.resize_crops(_crops_c(data, offsets, sizes, rot, rotations=rots), len(crops), out.data_ptr(),
                          torch.cuda.current_stream(dev).cuda_stream)
         return out
+
+    def crop_regions(self, frames, regions, frame_index=None) -> RegionCrops:
+        """Text regions of full frames, rectified on the device (parseq_warp_regions): see _System.crop_regions."""
+        from .engine import RegionsC
+        from .regions import check_quad, quad_coeffs, quad_size
+        import numpy as np
+        frame_list = list(frames) if isinstance(frames, (list, tuple)) else [frames]
+        if not frame_list:
+            raise ValueError("no frames")
+        quads = _region_quads(regions)
+        M, F = len(quads), len(frame_list)
+        if frame_index is None:
+            if F > 1:
+                raise ValueError(f"frame_index is required with more than one frame ({F})")
+            fidx = np.zeros(M, dtype=np.int64)
+        else:
+            fi = frame_index.cpu().numpy() if isinstance(frame_index, Tensor) else np.asarray(frame_index)
+            if fi.shape != (M,) or fi.dtype.kind not in "iu":
+                raise ValueError(f"frame_index must be integer [{M}], got {fi.dtype} {tuple(fi.shape)}")
+            if M and (fi.min() < 0 or fi.max() >= F):
+                raise ValueError(f"frame_index must be in [0, {F}), got values in [{fi.min()}, {fi.max()}]")
+            fidx = fi.astype(np.int64)
+        sizes, coeffs = [], []
+        for i, q in enumerate(quads):
+            check_quad(q, i)
+            h, w = quad_size(q)
+            sizes.append((h, w))
+            coeffs.append(quad_coeffs(q, h, w))
+        for f, fr in enumerate(frame_list):
+            if isinstance(fr, Tensor) and (fr.dtype != torch.uint8 or fr.dim() != 3 or fr.shape[2] != 3):
+                raise ValueError(f"frame {f} must be uint8 [H, W, 3] (HWC RGB), got {fr.dtype} {tuple(fr.shape)}")
+            if not isinstance(fr, Tensor) and getattr(fr, "mode", "RGB") != "RGB":
+                raise ValueError(f"frame {f}: a PIL frame must be in mode RGB, got {fr.mode}")
+        eng = self.engine()
+        dev = self._device
+        one = frame_list[0]
+        if F == 1 and isinstance(one, Tensor) and one.is_cuda:
+            fdata = one.contiguous().view(-1)
+            foffsets = torch.zeros(1, dtype=torch.int64)
+            fsizes = torch.tensor([[one.shape[0], one.shape[1]]], dtype=torch.int32)
+        else:
+            fdata, foffsets, fsizes = pack_crops(frame_list, pin_memory=True)
+        if fdata.device.type == "cuda" and fdata.device != dev:
+            raise ValueError(f"frames are on {fdata.device}, the model on {dev}")
+        fdata = fdata.to(dev, non_blocking=True)
+        sz = torch.tensor(sizes, dtype=torch.int32).reshape(M, 2)
+        nbytes = 3 * sz[:, 0].to(torch.int64) * sz[:, 1].to(torch.int64)
+        offsets = torch.zeros(M, dtype=torch.int64)
+        if M > 1:
+            offsets[1:] = torch.cumsum(nbytes, 0)[:-1]
+        total = int(nbytes.sum())
+        out = torch.empty(total, dtype=torch.uint8, device=dev)
+        cf = torch.tensor(coeffs, dtype=torch.float64).reshape(M, 8)
+        fi32 = torch.from_numpy(fidx.astype(np.int32))
+        rc = RegionsC(fdata.data_ptr(), fdata.numel(), foffsets.data_ptr(), fsizes.data_ptr(), F, fi32.data_ptr(),
+                      sz.data_ptr(), cf.data_ptr())
+        eng.warp_regions(rc, M, out.data_ptr(), total, torch.cuda.current_stream(dev).cuda_stream)
+        views = [out[o:o + 3 * h * w].view(h, w, 3) for o, (h, w) in zip(offsets.tolist(), sizes)]
+        return RegionCrops(views, out, offsets, sz, torch.tensor(quads, dtype=torch.float64).reshape(M, 4, 2), cf,
+                           torch.from_numpy(fidx))
 
     def score(self, images: Union[Tensor, List[Any]], targets: Tensor, lengths: Tensor, per_image: Tensor, *,
               rotation: Rotation = 0, return_token_logprobs: bool = False, return_attention: bool = False):
@@ -850,6 +962,21 @@ class _System(nn.Module):
         """The reference's test transform up to the uint8 image (module.py:69-82: rotate, T.Resize(img_size, BICUBIC)) of
         a list of raw crops, on the device: CUDA uint8 [N, H, W, 3], what `forward` takes as a tensor."""
         return self.model.preprocess(crops, rotation)
+
+    def crop_regions(self, frames, regions, frame_index=None) -> RegionCrops:
+        """Text regions of full frames (a detector's output), rectified on the device into crops that forward,
+        read_oriented, score, beam_search, lexicon_decode, preprocess and locate take as raw crops.
+        `frames`: one frame or a list of frames, each a uint8 [H, W, 3] tensor (CUDA or CPU) or an RGB PIL image; CPU
+        and PIL frames are uploaded to the model's device.  `regions`: float corners [M, 4, 2] in reading order (TL, TR,
+        BR, BL, frame pixels; pixel i covers [i, i + 1)), or integer boxes [M, 4] = (x0, y0, x1, y1), as a tensor or
+        array.  `frame_index`: int [M], the frame of each region (required with more than one frame).
+        Crop i is w = max(1, round(max(|TR - TL|, |BR - BL|))) by h = max(1, round(max(|BL - TL|, |BR - TR|))) pixels
+        (round half up), exactly frame.transform((w, h), PERSPECTIVE, coeffs, BICUBIC) of PIL with the closed-form
+        square-to-quad coefficients (parseq_b200/regions.py), 0 outside the frame; a box gives frame[y0:y1, x0:x1].
+        ValueError for non-finite corners, degenerate, self-intersecting or non-convex quads, crop sides over 8192, and
+        bad shapes or dtypes.  Returns a RegionCrops: the M CUDA crops, with .quads, .coeffs, .frame_index and
+        .to_frame(points, i), which maps points of crop i (such as locate's centres) back into its frame."""
+        return self.model.crop_regions(frames, regions, frame_index)
 
     def allowlist_mask(self, allowlist: Allowlist, batch: int) -> Optional[Tensor]:
         """`allowlist` of `forward` as the engine's per-image class mask (module function allowlist_mask)."""

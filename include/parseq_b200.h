@@ -180,6 +180,42 @@ typedef struct parseq_regions {
  * earlier work on `stream`, and needs no weights. */
 int parseq_warp_regions(parseq_engine* e, int32_t count, const parseq_regions* regions, uint8_t* out, int64_t out_bytes,
                         parseq_stream_t stream);
+/* Curved text regions: polygons of F = 2k points, 3 <= k <= 32, in frame pixels (pixel i covers [i, i + 1)), rectified
+ * by the thin-plate spline of TRBA's GridGenerator (RARE) with the polygon as its fiducial points C'.  The callers'
+ * Total-Text / CTW1500 order (top edge p_0..p_{k-1} left to right, then bottom edge q_0..q_{k-1} right to left) becomes
+ * the engine order C'_j = p_j, C'_{k+j} = b_j = q_{k-1-j} in Python; the C ABI takes the engine order.
+ *   Crop size (the Python layer): w = max(1, floor(max(sum |p_{j+1} - p_j|, sum |b_{j+1} - b_j|) + 0.5)),
+ *   h = max(1, floor(max_j |p_j - b_j| + 0.5)); with k = 2 this is the quad rule.
+ *   Map, fp64: C_x = numpy.linspace(-1, 1, k) bit for bit, C_y = -1 (top) / +1 (bottom); T = inv_delta_C . [C'; 0]
+ *   (parseq_tps_coeffs); output pixel (x, y) has xn = (2x + 1 - w) / w, yn = (2y + 1 - h) / h, r_m = |(xn, yn) - C_m|,
+ *   phi_m = (r_m r_m) ln(r_m + 1e-6), and goes to X = T0 + T1 xn + T2 yn + sum_m T_{3+m} phi_m (that order, one rounding
+ *   per operation, no FMA), Y likewise; (X, Y) then goes through parseq_warp_regions' sampler unchanged.
+ *   Exactness: every operation is IEEE round-to-nearest except ln, which the device does not round as numpy does.  The
+ *   bytes equal an fp64 restatement with numpy's log (tests/tps_warp_oracle.py) except at pixels whose byte changes when
+ *   the mapped point moves by 1e-7 px; they are not PIL-exact as the quad warp is. */
+typedef struct parseq_polygons {
+  const uint8_t* frames;         /* DEVICE packed HWC RGB bytes of all frames */
+  int64_t frames_bytes;
+  const int64_t* frame_offsets;  /* HOST int64 [F]: byte offset of frame f in frames */
+  const int32_t* frame_sizes;    /* HOST int32 [F][2]: (H, W) of frame f, 1 <= H, W <= 32768 */
+  int32_t num_frames;            /* F */
+  const int32_t* frame_index;    /* HOST int32 [M]: the frame of region i */
+  const int32_t* sizes;          /* HOST int32 [M][2]: (h, w) of crop i, 1 <= h, w <= 8192 */
+  const int32_t* num_points;     /* HOST int32 [M]: 2k_i points of region i, even, 6..64 (k may differ per region) */
+  const double* points;          /* HOST double: the regions' points (x, y) back to back, engine order */
+} parseq_polygons;
+/* coeffs [F + 3][2] = T of the map above for the F = num_points points [F][2] (engine order): the host solve the warp
+ * uses, with inv_delta_C computed once per k (Gauss-Jordan with partial pivoting, fp64, thread-safe cache).  No handle
+ * or device.  PARSEQ_ERR_INVALID_ARG for null pointers, a count that is odd or outside [6, 64], non-finite points. */
+int parseq_tps_coeffs(int32_t num_points, const double* points, double* coeffs);
+/* out: DEVICE uint8, the M crops [h_i, w_i, 3] back to back (crop i at byte sum_{j<i} 3 h_j w_j), out_bytes at least
+ * that sum.  Checked on the host before anything is enqueued, also without a handle (PARSEQ_ERR_INVALID_ARG): null
+ * pointers, count < 0, the frame checks of parseq_warp_regions, frame_index out of range, crop sides outside [1, 8192],
+ * point counts odd or outside [6, 64], non-finite points, and out_bytes too small.  Per chunk of max_batch regions the
+ * coefficients are solved on the host and the table (descriptor, T and C_x per region) uploaded; region_tps_kernel runs
+ * on the engine's main stream, ordered after the caller's earlier work on `stream`, and needs no weights. */
+int parseq_warp_polygons(parseq_engine* e, int32_t count, const parseq_polygons* polygons, uint8_t* out,
+                         int64_t out_bytes, parseq_stream_t stream);
 /* parseq_forward_u8 / parseq_forward_host_u8 on the resized crops; args->batch = N.  No teacher forcing.  The host
  * variant uploads each super-chunk's bytes on the engine's copy stream (in two halves from 256 crops up, PARSeq). */
 int parseq_forward_crops(parseq_engine* e, const parseq_forward_args* args, const parseq_crops* crops, float* logits,

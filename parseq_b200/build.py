@@ -14,7 +14,7 @@ HEADERS = ["ptx.cuh", "gemm.cuh", "gemm_body.inc", "kernels.cuh", "dec_ar.cuh", 
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
-    "-Xcompiler", "-fPIC", "-shared",
+    "-Xcompiler", "-fPIC", "-Xcompiler", "-ffp-contract=off", "-shared",
 ]
 
 

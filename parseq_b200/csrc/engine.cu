@@ -666,6 +666,7 @@ struct Workspace {
   DevBuf<uint32_t> in_mask;         // [max_batch, mask_ld] class allowlist rows of the super-chunk (graphs, host entry points)
   DevBuf<pq::CropDesc> crop_tab;    // the resize kernel's crop table [max_batch] (raw-crop entry points, crops.cuh)
   DevBuf<pq::RegionDesc> reg_tab;   // the warp kernel's region table [max_batch], allocated by the first parseq_warp_regions
+  DevBuf<pq::TpsDesc> tps_tab;      // the TPS kernel's polygon table [max_batch], allocated by the first parseq_warp_polygons
   // candidate scoring: the call's metadata (ids, targets, row tables; grown on demand), one causal [P][P] mask per
   // P = 1..L (mask of P at sc_causal + (P - 1) * L * L), and ViTSTR's LSE partials of a chunk's (image, position) rows
   DevBuf<int> sc_meta;
@@ -733,6 +734,7 @@ struct parseq_engine : Workspace {
   std::vector<pq::CropDesc> crop_descs;
   long long crop_base = 0;
   std::vector<pq::RegionDesc> reg_descs;   // parseq_warp_regions: the host copy of a chunk's region table (regions.cuh)
+  std::vector<pq::TpsDesc> tps_descs;      // parseq_warp_polygons: the host copy of a chunk's polygon table
   DevBuf<uint8_t> crop_stage;
   bool use_graph = true;
   long long orient_rereads = 0, orient_readings = 0;   // pass 2 of the last oriented call: crops re-read, readings run
@@ -1905,6 +1907,31 @@ int check_crops_call(parseq_engine* e, const parseq_forward_args* a, const parse
 // ---------------------------------------------------------------- text regions of full frames (regions.cuh)
 // The metadata of a parseq_warp_regions call, on the host alone (no handle or device needed), before anything is
 // enqueued.  *packed: the bytes of all rectified crops, sum of 3 h w.
+// The frames of a region call, and region i's frame index and crop size; the checks parseq_warp_regions and
+// parseq_warp_polygons share.
+int check_region_frames(int64_t frames_bytes, const int64_t* frame_offsets, const int32_t* frame_sizes, int num_frames) {
+  if (num_frames < 1) return fail(PARSEQ_ERR_INVALID_ARG, "num_frames must be >= 1");
+  for (int f = 0; f < num_frames; ++f) {
+    const int H = frame_sizes[2 * f], W = frame_sizes[2 * f + 1];
+    if (H < 1 || W < 1 || H > pq::REGION_MAX_FRAME_SIDE || W > pq::REGION_MAX_FRAME_SIDE)
+      return fail(PARSEQ_ERR_INVALID_ARG, "frame " + std::to_string(f) + ": size " + std::to_string(H) + " x " +
+                                              std::to_string(W) + ", sides must be in [1, 32768]");
+    if (frame_offsets[f] < 0 || frame_offsets[f] > frames_bytes - 3ll * H * W)
+      return fail(PARSEQ_ERR_INVALID_ARG, "frame " + std::to_string(f) + ": offset + 3 H W exceeds frames_bytes");
+  }
+  return PARSEQ_OK;
+}
+
+int check_region_crop(const std::string& at, const int32_t* frame_index, const int32_t* sizes, int num_frames, int i) {
+  if (frame_index[i] < 0 || frame_index[i] >= num_frames)
+    return fail(PARSEQ_ERR_INVALID_ARG, at + "frame_index " + std::to_string(frame_index[i]) + " out of range");
+  const int h = sizes[2 * i], w = sizes[2 * i + 1];
+  if (h < 1 || w < 1 || h > pq::REGION_MAX_SIDE || w > pq::REGION_MAX_SIDE)
+    return fail(PARSEQ_ERR_INVALID_ARG, at + "size " + std::to_string(h) + " x " + std::to_string(w) +
+                                            ", sides must be in [1, 8192]");
+  return PARSEQ_OK;
+}
+
 int check_regions(int count, const parseq_regions* r, const uint8_t* out, long long out_bytes, long long* packed) {
   if (r == nullptr || count < 0) return fail(PARSEQ_ERR_INVALID_ARG, "null argument or negative count");
   *packed = 0;
@@ -1912,23 +1939,11 @@ int check_regions(int count, const parseq_regions* r, const uint8_t* out, long l
   if (r->frames == nullptr || r->frame_offsets == nullptr || r->frame_sizes == nullptr || r->frame_index == nullptr ||
       r->sizes == nullptr || r->coeffs == nullptr || out == nullptr)
     return fail(PARSEQ_ERR_INVALID_ARG, "null frames, frame_offsets, frame_sizes, frame_index, sizes, coeffs or out");
-  if (r->num_frames < 1) return fail(PARSEQ_ERR_INVALID_ARG, "num_frames must be >= 1");
-  for (int f = 0; f < r->num_frames; ++f) {
-    const int H = r->frame_sizes[2 * f], W = r->frame_sizes[2 * f + 1];
-    if (H < 1 || W < 1 || H > pq::REGION_MAX_FRAME_SIDE || W > pq::REGION_MAX_FRAME_SIDE)
-      return fail(PARSEQ_ERR_INVALID_ARG, "frame " + std::to_string(f) + ": size " + std::to_string(H) + " x " +
-                                              std::to_string(W) + ", sides must be in [1, 32768]");
-    if (r->frame_offsets[f] < 0 || r->frame_offsets[f] > r->frames_bytes - 3ll * H * W)
-      return fail(PARSEQ_ERR_INVALID_ARG, "frame " + std::to_string(f) + ": offset + 3 H W exceeds frames_bytes");
-  }
+  PQ_TRY(check_region_frames(r->frames_bytes, r->frame_offsets, r->frame_sizes, r->num_frames));
   for (int i = 0; i < count; ++i) {
     const std::string at = "region " + std::to_string(i) + ": ";
-    if (r->frame_index[i] < 0 || r->frame_index[i] >= r->num_frames)
-      return fail(PARSEQ_ERR_INVALID_ARG, at + "frame_index " + std::to_string(r->frame_index[i]) + " out of range");
+    PQ_TRY(check_region_crop(at, r->frame_index, r->sizes, r->num_frames, i));
     const int h = r->sizes[2 * i], w = r->sizes[2 * i + 1];
-    if (h < 1 || w < 1 || h > pq::REGION_MAX_SIDE || w > pq::REGION_MAX_SIDE)
-      return fail(PARSEQ_ERR_INVALID_ARG, at + "size " + std::to_string(h) + " x " + std::to_string(w) +
-                                              ", sides must be in [1, 8192]");
     const double* a = r->coeffs + 8ll * i;
     for (int k = 0; k < 8; ++k)
       if (!std::isfinite(a[k])) return fail(PARSEQ_ERR_INVALID_ARG, at + "non-finite coefficient");
@@ -1940,6 +1955,118 @@ int check_regions(int count, const parseq_regions* r, const uint8_t* out, long l
         return fail(PARSEQ_ERR_INVALID_ARG, at + "the map's denominator a6 x + a7 y + 1 is not positive at a corner");
     }
     *packed += 3ll * h * w;
+  }
+  if (out_bytes < *packed)
+    return fail(PARSEQ_ERR_INVALID_ARG, "out_bytes (" + std::to_string(out_bytes) + ") is smaller than the packed crops (" +
+                                            std::to_string(*packed) + ")");
+  return PARSEQ_OK;
+}
+
+// ---------------------------------------------------------------- curved regions: thin-plate splines (regions.cuh)
+// TRBA's GridGenerator (RARE's TPS) with F = 2k fiducials C at C_x = numpy.linspace(-1, 1, k), C_y = -1 (top) and +1
+// (bottom).  delta_C [F + 3][F + 3] is _build_inv_delta_C's matrix: rows m < F are (1, C_x[m], C_y[m], hat_C[m][.]) with
+// hat_C = r^2 ln r off the diagonal and 0 on it, then the rows (0, 0, 0, C_x), (0, 0, 0, C_y) and (0, 0, 0, 1).  Its
+// inverse depends only on k: it is computed once per k by Gauss-Jordan elimination with partial pivoting (first
+// largest pivot in row order) and kept for the process.  The library is built with -ffp-contract=off, so the host
+// arithmetic here is one rounding per operation on every host compiler.
+
+// numpy.linspace(-1, 1, k) bit for bit: j * (2 / (k - 1)) + (-1), the last point exactly 1
+void tps_cx(int k, double* cx) {
+  const double step = 2.0 / static_cast<double>(k - 1);
+  for (int j = 0; j < k - 1; ++j) cx[j] = static_cast<double>(j) * step + (-1.0);
+  cx[k - 1] = 1.0;
+}
+
+const std::vector<double>& tps_inv_delta_c(int k) {
+  static std::mutex mu;
+  static std::map<int, std::vector<double>> cache;
+  std::lock_guard<std::mutex> lock(mu);
+  auto it = cache.find(k);
+  if (it != cache.end()) return it->second;
+  const int F = 2 * k, n = F + 3;
+  double cx[pq::TPS_MAX_K];
+  tps_cx(k, cx);
+  std::vector<double> a(static_cast<size_t>(n) * n, 0.0), inv(static_cast<size_t>(n) * n, 0.0);
+  auto fx = [&](int m) { return cx[m % k]; };
+  auto fy = [&](int m) { return m < k ? -1.0 : 1.0; };
+  for (int i = 0; i < F; ++i) {
+    a[i * n + 0] = 1.0;
+    a[i * n + 1] = fx(i);
+    a[i * n + 2] = fy(i);
+    for (int j = 0; j < F; ++j) {
+      if (i == j) continue;
+      const double dx = fx(i) - fx(j), dy = fy(i) - fy(j);
+      const double r = std::sqrt(dx * dx + dy * dy);
+      a[i * n + 3 + j] = (r * r) * std::log(r);
+    }
+    a[(F + 0) * n + 3 + i] = fx(i);
+    a[(F + 1) * n + 3 + i] = fy(i);
+    a[(F + 2) * n + 3 + i] = 1.0;
+  }
+  for (int i = 0; i < n; ++i) inv[i * n + i] = 1.0;
+  for (int c = 0; c < n; ++c) {
+    int piv = c;
+    for (int r = c + 1; r < n; ++r)
+      if (std::fabs(a[r * n + c]) > std::fabs(a[piv * n + c])) piv = r;
+    if (piv != c)
+      for (int j = 0; j < n; ++j) {
+        std::swap(a[c * n + j], a[piv * n + j]);
+        std::swap(inv[c * n + j], inv[piv * n + j]);
+      }
+    const double p = a[c * n + c];
+    for (int j = 0; j < n; ++j) {
+      a[c * n + j] /= p;
+      inv[c * n + j] /= p;
+    }
+    for (int r = 0; r < n; ++r) {
+      const double f = a[r * n + c];
+      if (r == c || f == 0.0) continue;
+      for (int j = 0; j < n; ++j) {
+        a[r * n + j] -= f * a[c * n + j];
+        inv[r * n + j] -= f * inv[c * n + j];
+      }
+    }
+  }
+  return cache.emplace(k, std::move(inv)).first->second;
+}
+
+// T [F + 3][2] = inv_delta_C [F + 3][F + 3] . [C'; 0], summed in index order; points: C' [F][2], engine order.
+void tps_solve(int k, const double* points, double* coeffs) {
+  const std::vector<double>& inv = tps_inv_delta_c(k);
+  const int F = 2 * k, n = F + 3;
+  for (int i = 0; i < n; ++i)
+    for (int c = 0; c < 2; ++c) {
+      double acc = 0.0;
+      for (int j = 0; j < F; ++j) acc += inv[static_cast<size_t>(i) * n + j] * points[2 * j + c];
+      coeffs[2 * i + c] = acc;
+    }
+}
+
+int check_polygon_points(const std::string& at, int num_points, const double* points) {
+  if (num_points % 2 != 0 || num_points < 2 * pq::TPS_MIN_K || num_points > 2 * pq::TPS_MAX_K)
+    return fail(PARSEQ_ERR_INVALID_ARG, at + std::to_string(num_points) + " points, a polygon needs an even count in [6, 64]");
+  for (int j = 0; j < 2 * num_points; ++j)
+    if (!std::isfinite(points[j])) return fail(PARSEQ_ERR_INVALID_ARG, at + "non-finite point");
+  return PARSEQ_OK;
+}
+
+// The metadata of a parseq_warp_polygons call, on the host alone (no handle or device needed), before anything is
+// enqueued.  *packed: the bytes of all rectified crops, sum of 3 h w.
+int check_polygons(int count, const parseq_polygons* r, const uint8_t* out, long long out_bytes, long long* packed) {
+  if (r == nullptr || count < 0) return fail(PARSEQ_ERR_INVALID_ARG, "null argument or negative count");
+  *packed = 0;
+  if (count == 0) return PARSEQ_OK;
+  if (r->frames == nullptr || r->frame_offsets == nullptr || r->frame_sizes == nullptr || r->frame_index == nullptr ||
+      r->sizes == nullptr || r->num_points == nullptr || r->points == nullptr || out == nullptr)
+    return fail(PARSEQ_ERR_INVALID_ARG, "null frames, frame_offsets, frame_sizes, frame_index, sizes, num_points, points or out");
+  PQ_TRY(check_region_frames(r->frames_bytes, r->frame_offsets, r->frame_sizes, r->num_frames));
+  long long first = 0;                     // the region's first point in `points`
+  for (int i = 0; i < count; ++i) {
+    const std::string at = "region " + std::to_string(i) + ": ";
+    PQ_TRY(check_region_crop(at, r->frame_index, r->sizes, r->num_frames, i));
+    PQ_TRY(check_polygon_points(at, r->num_points[i], r->points + 2 * first));
+    first += r->num_points[i];
+    *packed += 3ll * r->sizes[2 * i] * r->sizes[2 * i + 1];
   }
   if (out_bytes < *packed)
     return fail(PARSEQ_ERR_INVALID_ARG, "out_bytes (" + std::to_string(out_bytes) + ") is smaller than the packed crops (" +
@@ -3008,6 +3135,56 @@ int parseq_warp_regions(parseq_engine* e, int32_t count, const parseq_regions* r
     // no PDL: the kernel reads the table copy and the caller's frames
     PQ_TRY(launch_ex(LaunchConfig(grid, dim3(pq::REGION_THREADS), 0, e->main, 0, false), pq::region_warp_kernel,
                      r->frames, static_cast<const pq::RegionDesc*>(e->reg_tab), out));
+  }
+  return leave_main(e, user);
+}
+
+int parseq_tps_coeffs(int32_t num_points, const double* points, double* coeffs) {
+  if (points == nullptr || coeffs == nullptr) return fail(PARSEQ_ERR_INVALID_ARG, "null points or coeffs");
+  PQ_TRY(check_polygon_points("", num_points, points));
+  tps_solve(num_points / 2, points, coeffs);
+  return PARSEQ_OK;
+}
+
+int parseq_warp_polygons(parseq_engine* e, int32_t count, const parseq_polygons* r, uint8_t* out, int64_t out_bytes,
+                         parseq_stream_t stream) {
+  long long packed = 0;
+  PQ_TRY(check_polygons(count, r, out, out_bytes, &packed));
+  PQ_TRY(check_ready(e, false));
+  if (count == 0) return PARSEQ_OK;
+  PQ_CUDA(cudaSetDevice(e->cfg.device));
+  PQ_TRY(e->tps_tab.grow(e, e->max_batch));
+  cudaStream_t user = reinterpret_cast<cudaStream_t>(stream);
+  PQ_TRY(enter_main(e, user));
+  long long dst = 0, first = 0;
+  for (int b0 = 0; b0 < count; b0 += e->max_batch) {
+    const int Bc = (count - b0 < e->max_batch) ? (count - b0) : e->max_batch;
+    e->tps_descs.resize(static_cast<size_t>(Bc));
+    long long pixels = 0;                  // of the largest region of the chunk: the grid's tile count
+    for (int i = 0; i < Bc; ++i) {
+      const int g = b0 + i, f = r->frame_index[g];
+      pq::TpsDesc& d = e->tps_descs[static_cast<size_t>(i)];
+      std::memset(&d, 0, sizeof(d));
+      d.k = r->num_points[g] / 2;
+      tps_solve(d.k, r->points + 2 * first, d.t);
+      tps_cx(d.k, d.cx);
+      first += r->num_points[g];
+      d.src = r->frame_offsets[f];
+      d.dst = dst;
+      d.fh = r->frame_sizes[2 * f];
+      d.fw = r->frame_sizes[2 * f + 1];
+      d.h = r->sizes[2 * g];
+      d.w = r->sizes[2 * g + 1];
+      dst += 3ll * d.h * d.w;
+      pixels = std::max(pixels, 1ll * d.h * d.w);
+    }
+    // pageable source: the copy is staged when it returns, so tps_descs may change for the next chunk
+    PQ_CUDA(cudaMemcpyAsync(e->tps_tab, e->tps_descs.data(), sizeof(pq::TpsDesc) * Bc, cudaMemcpyHostToDevice, e->main));
+    const dim3 grid(static_cast<unsigned>((pixels + pq::REGION_THREADS - 1) / pq::REGION_THREADS), static_cast<unsigned>(Bc));
+    TimedScope ts(e, e->main, CAT_MISC, 0.0);
+    // no PDL: the kernel reads the table copy and the caller's frames
+    PQ_TRY(launch_ex(LaunchConfig(grid, dim3(pq::REGION_THREADS), 0, e->main, 0, false), pq::region_tps_kernel,
+                     r->frames, static_cast<const pq::TpsDesc*>(e->tps_tab), out));
   }
   return leave_main(e, user);
 }

@@ -35,6 +35,12 @@ class RegionsC(C.Structure):
                 ("coeffs", C.c_void_p)]
 
 
+class PolygonsC(C.Structure):
+    _fields_ = [("frames", C.c_void_p), ("frames_bytes", C.c_int64), ("frame_offsets", C.c_void_p),
+                ("frame_sizes", C.c_void_p), ("num_frames", C.c_int32), ("frame_index", C.c_void_p), ("sizes", C.c_void_p),
+                ("num_points", C.c_void_p), ("points", C.c_void_p)]
+
+
 class OrientArgsC(C.Structure):
     _fields_ = [("num_orientations", C.c_int32), ("orientations", C.c_int32 * 4), ("min_confidence", C.c_float),
                 ("rotation_out", C.c_void_p), ("confidence_out", C.c_void_p)]
@@ -99,7 +105,8 @@ class LexiconHandle:
 EXPORTS = [
     "parseq_create", "parseq_destroy", "parseq_set_weight", "parseq_num_weights", "parseq_weight_key",
     "parseq_finalize", "parseq_forward", "parseq_forward_host", "parseq_forward_u8", "parseq_forward_host_u8",
-    "parseq_resize_crops", "parseq_warp_regions", "parseq_forward_crops", "parseq_forward_host_crops", "parseq_forward_crops_oriented",
+    "parseq_resize_crops", "parseq_warp_regions", "parseq_tps_coeffs", "parseq_warp_polygons",
+    "parseq_forward_crops", "parseq_forward_host_crops", "parseq_forward_crops_oriented",
     "parseq_score", "parseq_score_u8", "parseq_score_check", "parseq_beam_search", "parseq_beam_search_u8",
     "parseq_lexicon_check", "parseq_lexicon_create", "parseq_lexicon_destroy", "parseq_beam_search_lexicon",
     "parseq_beam_search_lexicon_u8",
@@ -141,6 +148,8 @@ def load_library(path: Optional[str] = None):
     lib.parseq_forward_host_u8.argtypes = lib.parseq_forward.argtypes
     lib.parseq_resize_crops.argtypes = [C.c_void_p, C.c_int32, C.POINTER(CropsC), C.c_void_p, C.c_void_p]
     lib.parseq_warp_regions.argtypes = [C.c_void_p, C.c_int32, C.POINTER(RegionsC), C.c_void_p, C.c_int64, C.c_void_p]
+    lib.parseq_tps_coeffs.argtypes = [C.c_int32, C.c_void_p, C.c_void_p]
+    lib.parseq_warp_polygons.argtypes = [C.c_void_p, C.c_int32, C.POINTER(PolygonsC), C.c_void_p, C.c_int64, C.c_void_p]
     lib.parseq_forward_crops.argtypes = [C.c_void_p, C.POINTER(ForwardArgsC), C.POINTER(CropsC), C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p]
     lib.parseq_forward_host_crops.argtypes = lib.parseq_forward_crops.argtypes
@@ -200,6 +209,17 @@ class EngineError(RuntimeError):
 def check(lib, rc: int):
     if rc != 0:
         raise EngineError(f"parseq_b200 error {rc}: {lib.parseq_last_error().decode()}")
+
+
+def tps_coeffs(points, lib=None):
+    """parseq_tps_coeffs: the TPS coefficients T float64 [F + 3, 2] of F polygon points [F, 2] in engine order (top edge,
+    then bottom edge, each left to right).  Needs the library, not a device."""
+    import numpy as np
+    lib = lib or load_library()
+    p = np.ascontiguousarray(points, dtype=np.float64).reshape(-1, 2)
+    t = np.empty((len(p) + 3, 2), dtype=np.float64)
+    check(lib, lib.parseq_tps_coeffs(len(p), p.ctypes.data, t.ctypes.data))
+    return t
 
 
 def config_c(cfg, device: int = 0, max_batch: int = 0) -> ParseqConfigC:
@@ -318,6 +338,9 @@ class Engine:
 
     def warp_regions(self, regions: RegionsC, count, out_ptr, out_bytes, stream):
         check(self.lib, self.lib.parseq_warp_regions(self.handle, count, C.byref(regions), out_ptr, out_bytes, stream))
+
+    def warp_polygons(self, polygons: PolygonsC, count, out_ptr, out_bytes, stream):
+        check(self.lib, self.lib.parseq_warp_polygons(self.handle, count, C.byref(polygons), out_ptr, out_bytes, stream))
 
     def forward_crops(self, crops: CropsC, batch, logits_ptr, ids_ptr, steps_ptr, stream, max_length=None, decode_ar=True,
                       refine_iters=1, host=False, class_mask_ptr=None, attn_maps_ptr=None):

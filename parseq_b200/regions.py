@@ -73,3 +73,90 @@ def map_points(coeffs: Sequence[float], u, v):
     a0, a1, a2, a3, a4, a5, a6, a7 = coeffs
     den = a6 * u + a7 * v + 1.0
     return (a0 * u + a1 * v + a2) / den, (a3 * u + a4 * v + a5) / den
+
+
+# ---------------------------------------------------------------- curved regions (parseq_warp_polygons)
+# A polygon of 2k points, 3 <= k <= 32, in the Total-Text / CTW1500 clockwise order: the top edge p_0..p_{k-1} left to
+# right, then the bottom edge q_0..q_{k-1} right to left.  The engine takes TRBA's fiducial order, both edges left to
+# right: C'_j = p_j, C'_{k+j} = b_j = q_{k-1-j}.  The crop is w = max(1, floor(max(sum |p_{j+1} - p_j|,
+# sum |b_{j+1} - b_j|) + 0.5)) wide and h = max(1, floor(max_j |p_j - b_j| + 0.5)) tall; with k = 2 that is quad_size.
+# The map is the thin-plate spline of include/parseq_b200.h (parseq_tps_coeffs, map_tps).
+MIN_K, MAX_K = 3, 32
+
+
+def engine_points(poly: Quad) -> List[Tuple[float, float]]:
+    """Caller order (top left to right, bottom right to left) -> engine order (both edges left to right)."""
+    pts = [(float(p[0]), float(p[1])) for p in poly]
+    k = len(pts) // 2
+    return pts[:k] + pts[k:][::-1]
+
+
+def polygon_size(points: Quad) -> Tuple[int, int]:
+    """(h, w) of the crop of a polygon given in engine order (top then bottom, each left to right)."""
+    pts = [(float(p[0]), float(p[1])) for p in points]
+    k = len(pts) // 2
+    top, bot = pts[:k], pts[k:]
+    lt = lb = hh = 0.0
+    for j in range(k - 1):
+        lt += math.hypot(top[j + 1][0] - top[j][0], top[j + 1][1] - top[j][1])
+        lb += math.hypot(bot[j + 1][0] - bot[j][0], bot[j + 1][1] - bot[j][1])
+    for j in range(k):
+        hh = max(hh, math.hypot(bot[j][0] - top[j][0], bot[j][1] - top[j][1]))
+    return max(1, math.floor(hh + 0.5)), max(1, math.floor(max(lt, lb) + 0.5))
+
+
+def check_polygon(poly: Quad, i: int = 0):
+    """ValueError unless poly (caller order) is 6..64 finite points, an even count, of a simple polygon (no zero-length
+    edge, no two edges that meet other than adjacent ones at their shared point), crop sides <= 8192."""
+    import numpy as np
+    n = len(poly)
+    if n % 2 or n < 2 * MIN_K or n > 2 * MAX_K:
+        raise ValueError(f"region {i}: {n} points, a polygon needs an even count of 6 to 64 points")
+    p = np.asarray([(float(a[0]), float(a[1])) for a in poly], dtype=np.float64)
+    if not np.isfinite(p).all():
+        raise ValueError(f"region {i}: non-finite point")
+    a, b = p, np.roll(p, -1, axis=0)                     # edge e = (a[e], b[e]), the closed boundary
+    d = b - a
+    if ((d[:, 0] == 0.0) & (d[:, 1] == 0.0)).any():
+        raise ValueError(f"region {i}: the polygon is degenerate (a repeated point)")
+
+    def orient(o, u, v):                                  # cross(u - o, v - o) over all (edge, edge) pairs
+        return (u[..., 0] - o[..., 0]) * (v[..., 1] - o[..., 1]) - (u[..., 1] - o[..., 1]) * (v[..., 0] - o[..., 0])
+    A, B, Cq, D = a[:, None], b[:, None], a[None, :], b[None, :]
+    o1, o2, o3, o4 = orient(A, B, Cq), orient(A, B, D), orient(Cq, D, A), orient(Cq, D, B)
+    col = (o1 == 0.0) & (o2 == 0.0)
+    lo, hi = np.minimum(a, b), np.maximum(a, b)
+    # overlapping bounding boxes: needed for any meeting, and what decides it for (nearly) collinear edges
+    overlap = ((np.maximum(lo[:, None], lo[None, :]) <= np.minimum(hi[:, None], hi[None, :])).all(-1))
+    meet = (o1 * o2 <= 0.0) & (o3 * o4 <= 0.0) & overlap
+    e = np.arange(n)
+    gap = (e[None, :] - e[:, None]) % n
+    nonadjacent = (gap >= 2) & (gap <= n - 2)
+    # adjacent edges may only share their point: folding back along the same line is a self-intersection
+    fold = (gap == 1) & col & ((d[:, None] * d[None, :]).sum(-1) < 0.0)
+    if (meet & nonadjacent).any() or fold.any():
+        raise ValueError(f"region {i}: the polygon is self-intersecting")
+    h, w = polygon_size(engine_points(poly))
+    if h > MAX_SIDE or w > MAX_SIDE:
+        raise ValueError(f"region {i}: crop size {h} x {w}, sides must be at most {MAX_SIDE}")
+
+
+def map_tps(tps, h: int, w: int, u, v):
+    """Crop points (u, v) of an h x w crop -> frame points (x, y) through the TPS coefficients tps [F + 3][2]: xn =
+    2u / w - 1, yn = 2v / h - 1, then the map of include/parseq_b200.h in its order (float64 tensors)."""
+    import numpy as np
+    import torch
+    t = torch.as_tensor(tps, dtype=torch.float64)
+    k = (t.shape[0] - 3) // 2
+    cx = torch.from_numpy(np.linspace(-1.0, 1.0, k))
+    xn = 2.0 * torch.as_tensor(u, dtype=torch.float64) / w - 1.0
+    yn = 2.0 * torch.as_tensor(v, dtype=torch.float64) / h - 1.0
+    x = t[0, 0] + t[1, 0] * xn + t[2, 0] * yn
+    y = t[0, 1] + t[1, 1] * xn + t[2, 1] * yn
+    for m in range(2 * k):
+        dx, dy = xn - cx[m % k], yn - (-1.0 if m < k else 1.0)
+        r = torch.sqrt(dx * dx + dy * dy)
+        phi = (r * r) * torch.log(r + 1e-6)
+        x = x + t[3 + m, 0] * phi
+        y = y + t[3 + m, 1] * phi
+    return x, y

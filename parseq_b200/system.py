@@ -79,15 +79,21 @@ def _crop_tensor(c) -> Tensor:
 class RegionCrops(list):
     """The rectified crops of crop_regions: a list of M CUDA uint8 [h, w, 3] views into one packed buffer, so it goes
     wherever a list of raw crops goes (pack_crops then passes the buffer on without a copy).  Also holds each region's
-    `quads` (float64 [M, 4, 2], TL, TR, BR, BL in frame pixels), `coeffs` (float64 [M, 8], PIL PERSPECTIVE order) and
-    `frame_index` (int64 [M])."""
+    `quads` (float64 [M, 4, 2], TL, TR, BR, BL in frame pixels; for a polygon p_0, p_{k-1}, q_0, q_{k-1}), `coeffs`
+    (float64 [M, 8], PIL PERSPECTIVE order; NaN for a polygon), `frame_index` (int64 [M]), `polygons` (per region the
+    caller's float64 [2k, 2] points of a polygon, else None) and `tps` (per region its TPS coefficients float64
+    [2k + 3, 2], else None).  In a call that mixes quads and polygons the quad crops come first in the buffer, so
+    `offsets` need not increase."""
 
     def __init__(self, views: List[Tensor], data: Tensor, offsets: Tensor, sizes: Tensor, quads: Tensor, coeffs: Tensor,
-                 frame_index: Tensor):
+                 frame_index: Tensor, polygons: Optional[List[Optional[Tensor]]] = None,
+                 tps: Optional[List[Optional[Tensor]]] = None):
         super().__init__(views)
         self._views = tuple(views)
         self.data, self.offsets, self.sizes = data, offsets, sizes
         self.quads, self.coeffs, self.frame_index = quads, coeffs, frame_index
+        self.polygons = list(polygons) if polygons is not None else [None] * len(views)
+        self.tps = list(tps) if tps is not None else [None] * len(views)
 
     def packed(self) -> bool:
         """The list still holds exactly the views of `data` it was made with."""
@@ -95,13 +101,19 @@ class RegionCrops(list):
 
     def to_frame(self, points, i: int) -> Tensor:
         """Points (x, y) [..., 2] in the pixels of crop i (pixel j covers [j, j + 1); e.g. locate's centres, or the
-        corners of a box) -> the same points in frame pixels, float64, through region i's map."""
-        from .regions import map_points
+        corners of a box) -> the same points in frame pixels, float64, through region i's map (the thin-plate spline
+        of a polygon region)."""
+        from .regions import map_points, map_tps
         p = points if isinstance(points, Tensor) else torch.as_tensor(points)
         p = p.to(torch.float64)
         if p.shape[-1] != 2:
             raise ValueError(f"points must be [..., 2], got {tuple(p.shape)}")
-        x, y = map_points(self.coeffs[int(i)].tolist(), p[..., 0], p[..., 1])
+        i = int(i)
+        if self.tps[i] is not None:
+            h, w = (int(v) for v in self.sizes[i])
+            x, y = map_tps(self.tps[i], h, w, p[..., 0], p[..., 1])
+        else:
+            x, y = map_points(self.coeffs[i].tolist(), p[..., 0], p[..., 1])
         return torch.stack([x, y], dim=-1)
 
 
@@ -272,16 +284,39 @@ def check_orientations(orientations: Sequence[int]) -> Tuple[int, ...]:
     return tuple(int(x) for x in o)
 
 
-def _region_quads(regions) -> List[List[Tuple[float, float]]]:
-    """`regions` of crop_regions as M quads of Python floats: corners [M, 4, 2] (TL, TR, BR, BL; any real dtype), or
-    integer boxes [M, 4] = (x0, y0, x1, y1) with x1 > x0 and y1 > y0."""
+_REGION_FORMS = ("regions must be corners [M, 4, 2], polygons [M, 2k, 2] with 3 <= k <= 32, integer boxes [M, 4], or "
+                 "a list of M point arrays [n_i, 2], with M >= 1")
+
+
+def _region_points(regions) -> List[List[Tuple[float, float]]]:
+    """`regions` of crop_regions as M lists of Python float points: a quad (TL, TR, BR, BL) or a polygon of 2k points in
+    the caller's order.  Forms: corners [M, 4, 2] or polygons [M, 2k, 2] (any real dtype); integer boxes [M, 4] =
+    (x0, y0, x1, y1) with x1 > x0 and y1 > y0; a list of per-region point arrays [n_i, 2] of different lengths."""
     import numpy as np
     from .regions import box_quad
-    r = regions.detach().cpu().numpy() if isinstance(regions, Tensor) else np.asarray(regions)
+
+    def arr(r):
+        return r.detach().cpu().numpy() if isinstance(r, Tensor) else np.asarray(r)
+
+    if isinstance(regions, (list, tuple)) and len(regions) > 1 and len({np.shape(arr(r)) for r in regions}) > 1:
+        out = []
+        for i, r in enumerate(regions):
+            a = arr(r)
+            if a.dtype.kind not in "iuf" or a.ndim != 2 or a.shape[1] != 2:
+                raise ValueError(f"region {i}: points must be real [n, 2], got {a.dtype} of shape {tuple(a.shape)}")
+            if a.shape[0] != 4 and (a.shape[0] % 2 or not 6 <= a.shape[0] <= 64):
+                raise ValueError(f"region {i}: {a.shape[0]} points, a region needs 4 corners or an even count of 6 to "
+                                 f"64 polygon points")
+            out.append([(float(x), float(y)) for x, y in a.astype(np.float64)])
+        return out
+    r = arr(regions)
     if r.dtype.kind not in "iuf":
         raise ValueError(f"regions must be real corners [M, 4, 2] or integer boxes [M, 4], got dtype {r.dtype}")
-    if r.ndim == 3 and r.shape[1:] == (4, 2) and r.shape[0] > 0:
-        return [[(float(x), float(y)) for x, y in q] for q in r.astype(np.float64)]
+    if r.ndim == 3 and r.shape[2] == 2 and r.shape[0] > 0:
+        n = r.shape[1]
+        if n == 4 or (n % 2 == 0 and 6 <= n <= 64):
+            return [[(float(x), float(y)) for x, y in q] for q in r.astype(np.float64)]
+        raise ValueError(f"region 0: {n} points; {_REGION_FORMS}, got shape {tuple(r.shape)}")
     if r.ndim == 2 and r.shape[1] == 4 and r.shape[0] > 0:
         if r.dtype.kind == "f":
             raise ValueError("boxes [M, 4] must be integers; give real-valued regions as corners [M, 4, 2]")
@@ -289,7 +324,7 @@ def _region_quads(regions) -> List[List[Tuple[float, float]]]:
         if bad.size:
             raise ValueError(f"box {int(bad[0])}: {r[bad[0]].tolist()} needs x1 > x0 and y1 > y0")
         return [box_quad(b) for b in r.tolist()]
-    raise ValueError(f"regions must be corners [M, 4, 2] or boxes [M, 4] with M >= 1, got shape {tuple(r.shape)}")
+    raise ValueError(f"{_REGION_FORMS}, got shape {tuple(r.shape)}")
 
 
 def _crop_hw(c) -> Tuple[int, int]:
@@ -539,15 +574,16 @@ class _EngineModule(nn.Module):
         return out
 
     def crop_regions(self, frames, regions, frame_index=None) -> RegionCrops:
-        """Text regions of full frames, rectified on the device (parseq_warp_regions): see _System.crop_regions."""
-        from .engine import RegionsC
-        from .regions import check_quad, quad_coeffs, quad_size
+        """Text regions of full frames, rectified on the device (parseq_warp_regions for quads and boxes,
+        parseq_warp_polygons for polygons): see _System.crop_regions."""
+        from .engine import PolygonsC, RegionsC, tps_coeffs
+        from .regions import check_polygon, check_quad, engine_points, polygon_size, quad_coeffs, quad_size
         import numpy as np
         frame_list = list(frames) if isinstance(frames, (list, tuple)) else [frames]
         if not frame_list:
             raise ValueError("no frames")
-        quads = _region_quads(regions)
-        M, F = len(quads), len(frame_list)
+        regs = _region_points(regions)
+        M, F = len(regs), len(frame_list)
         if frame_index is None:
             if F > 1:
                 raise ValueError(f"frame_index is required with more than one frame ({F})")
@@ -559,12 +595,23 @@ class _EngineModule(nn.Module):
             if M and (fi.min() < 0 or fi.max() >= F):
                 raise ValueError(f"frame_index must be in [0, {F}), got values in [{fi.min()}, {fi.max()}]")
             fidx = fi.astype(np.int64)
-        sizes, coeffs = [], []
-        for i, q in enumerate(quads):
-            check_quad(q, i)
-            h, w = quad_size(q)
+        sizes, coeffs, quads, epts = [], [], [], []
+        for i, q in enumerate(regs):
+            if len(q) == 4:
+                check_quad(q, i)
+                h, w = quad_size(q)
+                coeffs.append(quad_coeffs(q, h, w))
+                quads.append(q)
+                epts.append(None)
+            else:
+                check_polygon(q, i)
+                e = engine_points(q)
+                h, w = polygon_size(e)
+                k = len(q) // 2
+                coeffs.append((math.nan,) * 8)
+                quads.append([q[0], q[k - 1], q[k], q[-1]])
+                epts.append(e)
             sizes.append((h, w))
-            coeffs.append(quad_coeffs(q, h, w))
         for f, fr in enumerate(frame_list):
             if isinstance(fr, Tensor) and (fr.dtype != torch.uint8 or fr.dim() != 3 or fr.shape[2] != 3):
                 raise ValueError(f"frame {f} must be uint8 [H, W, 3] (HWC RGB), got {fr.dtype} {tuple(fr.shape)}")
@@ -582,21 +629,43 @@ class _EngineModule(nn.Module):
         if fdata.device.type == "cuda" and fdata.device != dev:
             raise ValueError(f"frames are on {fdata.device}, the model on {dev}")
         fdata = fdata.to(dev, non_blocking=True)
+        # quad crops first, then polygon crops, each group in region order
+        qi = [i for i in range(M) if epts[i] is None]
+        pi = [i for i in range(M) if epts[i] is not None]
         sz = torch.tensor(sizes, dtype=torch.int32).reshape(M, 2)
         nbytes = 3 * sz[:, 0].to(torch.int64) * sz[:, 1].to(torch.int64)
+        order = torch.tensor(qi + pi, dtype=torch.int64)
         offsets = torch.zeros(M, dtype=torch.int64)
         if M > 1:
-            offsets[1:] = torch.cumsum(nbytes, 0)[:-1]
+            offsets[order[1:]] = torch.cumsum(nbytes[order], 0)[:-1]
         total = int(nbytes.sum())
+        qbytes = int(nbytes[qi].sum()) if qi else 0
         out = torch.empty(total, dtype=torch.uint8, device=dev)
         cf = torch.tensor(coeffs, dtype=torch.float64).reshape(M, 8)
-        fi32 = torch.from_numpy(fidx.astype(np.int32))
-        rc = RegionsC(fdata.data_ptr(), fdata.numel(), foffsets.data_ptr(), fsizes.data_ptr(), F, fi32.data_ptr(),
-                      sz.data_ptr(), cf.data_ptr())
-        eng.warp_regions(rc, M, out.data_ptr(), total, torch.cuda.current_stream(dev).cuda_stream)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        if qi:
+            q_sz = sz[qi].contiguous()
+            q_cf = cf[qi].contiguous()
+            q_fi = torch.from_numpy(fidx[qi].astype(np.int32))
+            rc = RegionsC(fdata.data_ptr(), fdata.numel(), foffsets.data_ptr(), fsizes.data_ptr(), F, q_fi.data_ptr(),
+                          q_sz.data_ptr(), q_cf.data_ptr())
+            eng.warp_regions(rc, len(qi), out.data_ptr(), qbytes, stream)
+        tps = [None] * M
+        polys = [None] * M
+        if pi:
+            p_sz = sz[pi].contiguous()
+            p_fi = torch.from_numpy(fidx[pi].astype(np.int32))
+            p_np = torch.tensor([len(epts[i]) for i in pi], dtype=torch.int32)
+            p_pts = torch.tensor([xy for i in pi for xy in epts[i]], dtype=torch.float64)
+            pc = PolygonsC(fdata.data_ptr(), fdata.numel(), foffsets.data_ptr(), fsizes.data_ptr(), F, p_fi.data_ptr(),
+                           p_sz.data_ptr(), p_np.data_ptr(), p_pts.data_ptr())
+            eng.warp_polygons(pc, len(pi), out.data_ptr() + qbytes, total - qbytes, stream)
+            for i in pi:
+                polys[i] = torch.tensor(regs[i], dtype=torch.float64)
+                tps[i] = torch.from_numpy(tps_coeffs(epts[i], eng.lib))
         views = [out[o:o + 3 * h * w].view(h, w, 3) for o, (h, w) in zip(offsets.tolist(), sizes)]
         return RegionCrops(views, out, offsets, sz, torch.tensor(quads, dtype=torch.float64).reshape(M, 4, 2), cf,
-                           torch.from_numpy(fidx))
+                           torch.from_numpy(fidx), polys, tps)
 
     def score(self, images: Union[Tensor, List[Any]], targets: Tensor, lengths: Tensor, per_image: Tensor, *,
               rotation: Rotation = 0, return_token_logprobs: bool = False, return_attention: bool = False):
@@ -967,15 +1036,25 @@ class _System(nn.Module):
         """Text regions of full frames (a detector's output), rectified on the device into crops that forward,
         read_oriented, score, beam_search, lexicon_decode, preprocess and locate take as raw crops.
         `frames`: one frame or a list of frames, each a uint8 [H, W, 3] tensor (CUDA or CPU) or an RGB PIL image; CPU
-        and PIL frames are uploaded to the model's device.  `regions`: float corners [M, 4, 2] in reading order (TL, TR,
-        BR, BL, frame pixels; pixel i covers [i, i + 1)), or integer boxes [M, 4] = (x0, y0, x1, y1), as a tensor or
-        array.  `frame_index`: int [M], the frame of each region (required with more than one frame).
-        Crop i is w = max(1, round(max(|TR - TL|, |BR - BL|))) by h = max(1, round(max(|BL - TL|, |BR - TR|))) pixels
-        (round half up), exactly frame.transform((w, h), PERSPECTIVE, coeffs, BICUBIC) of PIL with the closed-form
-        square-to-quad coefficients (parseq_b200/regions.py), 0 outside the frame; a box gives frame[y0:y1, x0:x1].
-        ValueError for non-finite corners, degenerate, self-intersecting or non-convex quads, crop sides over 8192, and
-        bad shapes or dtypes.  Returns a RegionCrops: the M CUDA crops, with .quads, .coeffs, .frame_index and
-        .to_frame(points, i), which maps points of crop i (such as locate's centres) back into its frame."""
+        and PIL frames are uploaded to the model's device.  `regions`, as a tensor, array or list: float corners
+        [M, 4, 2] in reading order (TL, TR, BR, BL, frame pixels; pixel i covers [i, i + 1)); integer boxes [M, 4] =
+        (x0, y0, x1, y1); polygons of curved text [M, 2k, 2], 3 <= k <= 32; or a list of M point arrays [n_i, 2] that
+        mixes quads (n_i = 4) and polygons of different even lengths.  `frame_index`: int [M], the frame of each region
+        (required with more than one frame).
+        Quads: crop i is w = max(1, round(max(|TR - TL|, |BR - BL|))) by h = max(1, round(max(|BL - TL|, |BR - TR|)))
+        pixels (round half up), exactly frame.transform((w, h), PERSPECTIVE, coeffs, BICUBIC) of PIL with the
+        closed-form square-to-quad coefficients (parseq_b200/regions.py), 0 outside the frame; a box gives
+        frame[y0:y1, x0:x1].
+        Polygons are in the Total-Text / CTW1500 order: the top edge p_0..p_{k-1} left to right, then the bottom edge
+        q_0..q_{k-1} right to left (FCENet, TextSnake, PAN and ABCNet-style outputs).  A DBNet-style contour has to be
+        split into those two edges by the caller.  The crop is as long as the longer edge and as tall as the widest
+        p_j - q_{k-1-j} gap (rounded half up) and is rectified by the thin-plate spline of TRBA's GridGenerator with
+        the polygon as its fiducial points, then sampled like a quad (include/parseq_b200.h, parseq_warp_polygons).
+        ValueError, with the region's index, for non-finite points; degenerate, self-intersecting or non-convex quads;
+        polygons of an odd count, fewer than 6 or more than 64 points, or self-intersecting; crop sides over 8192; and
+        bad shapes or dtypes.  Returns a RegionCrops: the M CUDA crops, with .quads, .coeffs, .polygons, .tps,
+        .frame_index and .to_frame(points, i), which maps points of crop i (such as locate's centres) back into its
+        frame, through the thin-plate spline for a polygon."""
         return self.model.crop_regions(frames, regions, frame_index)
 
     def allowlist_mask(self, allowlist: Allowlist, batch: int) -> Optional[Tensor]:

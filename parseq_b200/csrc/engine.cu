@@ -1061,67 +1061,100 @@ int vitstr_tail(parseq_engine* e, int B, int L, float* logits, int* ids_out, con
 }
 
 // ---------------------------------------------------------------- one Decoder call (model.py:86-103, modules.py:55-125)
-// rows are (b, qi), qi in [0,nq); query position q0+qi; context ids[b, 0..nkeys-1].
-// Tail: LayerNorm(decoder.norm) + head + (optionally) greedy argmax -> ids_dst[b*ids_ld + dst_off + qi] in one kernel.
-// Caller-supplied pieces of PARSeq.decode (model.py:86-103) that the inference loops never use: explicit query rows,
-// explicit masks, decoder output instead of logits.
-struct DecodeExtras {
+// The self-attention mask (the int the kernels take): keys 0..nkeys-1 (AR step, NAR), the cloze mask + first EOS
+// (refinement), or the caller's masks over one query row per (image, query) (PARSeq.decode), which only self_mask picks.
+enum class SelfMask : int { Keys = 0, Cloze = 1, Caller = 2 };
+// What a pass ends with after the last layer: decoder.norm, then the head into logits (+ greedy ids), the head GEMM's
+// LSE or top-K epilogue (no logits stored), or nothing more (Norm); or it stops after the last layer's maps (MapsOnly:
+// no cross-attention output, MLP or decoder.norm)
+enum class Tail { Head, LogSumExp, TopK, Norm, MapsOnly };
+
+// One decoder pass: rows (b, qi), qi in [0, nq), of images b_first.. of the super-chunk (rows of the cross K/V cache);
+// query position q0 + qi; context ids[b, 0..nkeys-1] (id rows [B, ids_ld]).  Callers assign the fields they use.
+struct DecodePass {
+  int b_first = 0, B = 0, nq = 0, q0 = 0, nkeys = 0;
+  const int* ids = nullptr;
+  // an AR step (nq = 1, keys 0..q0): the content stream computes row q0 only and appends it to the caches of pitch L;
+  // otherwise it computes the whole context (nkeys rows per image, pitch nkeys)
+  bool ar_step = false;
+  int kv_pitch(const parseq_engine* e) const { return ar_step ? e->L : nkeys; }
+  int beam = 1;                          // beam search: B counts beam rows, `beam` consecutive rows per image; the rows'
+                                         // self-attention reads their own ids, their cross-attention their image
+  SelfMask self_mask = SelfMask::Keys;
+  // caller inputs of PARSeq.decode (model.py:86-103) that the inference loops never use
   const float* query = nullptr;          // [B*nq, D] fp32 raw queries (residual base); null -> pos_queries[q0 + qi]
   const unsigned char* qmask = nullptr;  // [nq, nkeys], 1 = masked
   const unsigned char* pmask = nullptr;  // [B, nkeys], 1 = masked
   const unsigned char* cmask = nullptr;  // [nkeys, nkeys] content-stream mask (`tgt_mask`), 1 = masked; depth >= 2 only
-  float* out_norm = nullptr;             // [B*nq, D] fp32: decoder.norm(y) is the result (no head)
-  const int* lse_tgt = nullptr;          // [B*nq] target class per row: the head runs with the LSE epilogue into the
-                                         // stage's lse_part / lse_tlogit (candidate scoring), no logits are stored
   // candidate scoring: the B rows are candidates of cand_imgs images, image j's candidates [cand_off[j], cand_off[j + 1])
   // (device), at most cand_max_rows query rows per image; every cross-attention of the pass serves a candidate's rows
   // from its image (dec_cross_attn3_grouped_kernel)
   const int* cand_off = nullptr;
   int cand_imgs = 0, cand_max_rows = 0;
-  int beam = 1;                         // beam search: B counts beam rows, `beam` consecutive rows per image; the rows'
-                                         // self-attention reads their own ids, their cross-attention their image
-  // beam search above 128 classes: the head GEMM runs the top-K epilogue (beam_k keys per row and tile, the images'
-  // allowlist rows beam_mask) into these, and no logits are stored
-  float2* beam_part = nullptr;
-  unsigned long long* beam_keys = nullptr;
-  int beam_k = 0;
-  const uint32_t* beam_mask = nullptr;
   // cross-attention maps (parseq_forward_args.attn_maps): the query stream of the last layer writes the head-averaged
-  // weights of row (b, qi) to maps + (b * nq + qi) * T; maps_only: the pass ends there (no cross-attention output, MLP
-  // or head)
+  // weights of row (b, qi) to maps + (b * nq + qi) * T.  With cand_off the maps have maps_ld rows per candidate, rows
+  // past maps_len[c] (the group's candidate lengths, device) written as 0 (dec_cross_attn_maps_grouped_kernel)
   float* maps = nullptr;
-  bool maps_only = false;
-  // with cand_off (candidate scoring): the maps have maps_ld rows per candidate, rows past maps_len[c] (the group's
-  // candidate lengths, device) written as 0 (dec_cross_attn_maps_grouped_kernel)
   const int* maps_len = nullptr;
   int maps_ld = 0;
+  Tail tail = Tail::Head;
+  // Head: row r's logits at logits + r * logits_ld; with ids_dst the greedy id of row (b, qi) goes to
+  // ids_dst[b * ids_ld + dst_off + qi], or with `forced` (teacher forcing) forced[b * forced_ld + dst_off + qi].
+  // Head and TopK: `mask` holds the images' class allowlist rows, or null
+  float* logits = nullptr;
+  long long logits_ld = 0;
+  const uint32_t* mask = nullptr;
+  int* ids_dst = nullptr;
+  const int* forced = nullptr;
+  int dst_off = 0, forced_ld = 0;
+  const int* lse_tgt = nullptr;          // LogSumExp: [B*nq] target class per row
+  float2* part = nullptr;                // TopK: k keys per row and 128-class tile, the allowlist row of r is image r / beam
+  unsigned long long* keys = nullptr;
+  int k = 0;
+  float* out_norm = nullptr;             // Norm: [B*nq, D] fp32
 };
+
+// A stream's self-attention mask: Caller where the pass has a padding mask or the stream's own mask (content stream:
+// cmask, query stream: qmask), or in the query stream the caller's queries; else the pass's own
+SelfMask self_mask(const DecodePass& p, bool content) {
+  const bool caller = p.pmask != nullptr || (content ? p.cmask != nullptr : p.qmask != nullptr || p.query != nullptr);
+  return caller ? SelfMask::Caller : p.self_mask;
+}
 
 const __nv_bfloat16* ckv_of(const parseq_engine* e, int layer) { return layer == 0 ? e->ckv : e->ckv_deep[layer - 1]; }
 
-// Self-attention with one query row per (image, query) (decoders of depth >= 2): over the (position, token) table
-// (kv = kvtab, layer 0) or over a content K/V cache of `pitch` key rows per image (cache = true).
-int self_attn_rows(parseq_engine* e, const float* q, const __nv_bfloat16* kv, bool cache, int pitch, const int* ids, int B,
-                   int nq, int q0, int nkeys, int mode, const unsigned char* qmask, const unsigned char* pmask,
-                   __nv_bfloat16* out, cudaStream_t st) {
-  const int D = e->D;
-  TimedScope ts(e, st, CAT_DEC_ATTN, 4.0 * B * nq * nkeys * D);
-  const int qsplit = (nq >= 8) ? 4 : 1;
-  auto kern = e->ids_ld == 32 ? (cache ? pq::dec_self_attn2_rows_kernel<true> : pq::dec_self_attn2_rows_kernel<false>)
-                              : (cache ? pq::dec_self_attn2_rows_long_kernel<true> : pq::dec_self_attn2_rows_long_kernel<false>);
-  return launch_k(e->lo, kern, dim3(B * qsplit), dim3(D < 384 ? D : 384), 0, st, q, kv, ids, e->ids_ld, cache ? pitch : e->V, D,
-                  nq, q0, nkeys, mode, /*eos*/ 0, out, qsplit, qmask, pmask);
+// Calls f(std::integral_constant<int, TB>) with the 128-token blocks of the image memory that the decoder's
+// cross-attention kernels are instantiated for: TB = 1 up to 128 tokens, else 2 (NR = 4 TB keys per lane)
+template <typename F>
+int dispatch_tokens(int T, F&& f) {
+  return T <= 128 ? f(std::integral_constant<int, 1>{}) : f(std::integral_constant<int, 2>{});
 }
 
-// The rest of decoder layer `l` after its self-attention (modules.py:72-78) on a residual stream x [B*nq, D] (fp32, in
-// place): x += out_proj(sa); x += cross_attn(norm1(x)); x += MLP(norm2(x)).  add != null: x holds no residual yet,
-// the base is the broadcast table / caller rows `add` (row r adds add[r % add_mod]).  `ex` (may be null): the
-// candidates' row map, and with `maps_layer` the maps of this layer's query rows.
-int dec_layer_rest(parseq_engine* e, parseq_engine::Stage& sg, int l, int b_first, int B, int nq, float* x, const float* add,
-                   int add_mod, cudaStream_t st, const DecodeExtras* ex, bool maps_layer) {
-  const int D = e->D, M = B * nq;
-  float* const maps = ex != nullptr && maps_layer ? ex->maps : nullptr;
-  const int* const cand_off = ex != nullptr ? ex->cand_off : nullptr;
+// Self-attention sg.qc -> sg.sa of layer l with one query row per (image, query) (decoders of depth >= 2), nq rows per
+// image from position q0 of the content or query stream, over the (position, token) table (l = 0) or the layer's cache.
+int self_attn_rows(parseq_engine* e, parseq_engine::Stage& sg, const DecodePass& p, int l, bool content, int nq, int q0,
+                   cudaStream_t st) {
+  const int D = e->D;
+  TimedScope ts(e, st, CAT_DEC_ATTN, 4.0 * p.B * nq * p.nkeys * D);
+  const int qsplit = (nq >= 8) ? 4 : 1;
+  const bool cache = l > 0;
+  auto kern = e->ids_ld == 32 ? (cache ? pq::dec_self_attn2_rows_kernel<true> : pq::dec_self_attn2_rows_kernel<false>)
+                              : (cache ? pq::dec_self_attn2_rows_long_kernel<true> : pq::dec_self_attn2_rows_long_kernel<false>);
+  const __nv_bfloat16* kv = cache ? sg.kvc[l - 1] : e->kvtab;
+  return launch_k(e->lo, kern, dim3(p.B * qsplit), dim3(D < 384 ? D : 384), 0, st, static_cast<const float*>(sg.qc), kv, p.ids,
+                  e->ids_ld, cache ? p.kv_pitch(e) : e->V, D, nq, q0, p.nkeys, static_cast<int>(self_mask(p, content)),
+                  /*eos*/ 0, sg.sa, qsplit, content ? p.cmask : p.qmask, p.pmask);
+}
+
+// The rest of decoder layer `l` after its self-attention (modules.py:72-78) on a residual stream x [p.B * nq, D] (fp32, in
+// place): x += out_proj(sa); x += cross_attn(norm1(x)); x += MLP(norm2(x)).  add != null: x holds no residual yet, the
+// base is the broadcast table / caller rows `add` (row r adds add[r % add_mod]).  With `maps_layer` the layer writes the
+// pass's maps (a MapsOnly pass ends there).
+int dec_layer_rest(parseq_engine* e, parseq_engine::Stage& sg, const DecodePass& p, int l, int nq, float* x, const float* add,
+                   int add_mod, bool maps_layer, cudaStream_t st) {
+  const int D = e->D, M = p.B * nq;
+  const int B = p.B / p.beam;             // images; each has p.beam * nq query rows
+  nq *= p.beam;
   const std::string Ly = "decoder.layers." + std::to_string(l) + ".";
   const float qscale = 1.0f / std::sqrt(static_cast<float>(e->dh_dec));
   if (add != nullptr) {
@@ -1137,49 +1170,41 @@ int dec_layer_rest(parseq_engine* e, parseq_engine::Stage& sg, int l, int b_firs
   }
   PQ_TRY(gemm(e, sg.yn, D, e->wb(Ly + "cross_attn.in_proj_weight"), D, e->wf(Ly + "cross_attn.in_proj_bias"), M, D, D,
               pq::EPI_F32, qscale, nullptr, 0, 0, sg.qc, D, st));
-  if (maps != nullptr) {
+  const long long kv_rows = 1ll * e->max_batch * e->T;
+  const int H = e->cfg.dec_num_heads;
+  const float* q = sg.qc;
+  if (maps_layer && p.maps != nullptr) {
     // the head-averaged weights of these query rows, from the q just projected and the layer's K (reads only)
     TimedScope ts(e, st, CAT_MAPS, 2.0 * M * e->T * D);
-    const long long kv_rows = 1ll * e->max_batch * e->T;
-    if (cand_off != nullptr) {
-      // candidate scoring: every image's candidates' maps_ld map rows, at most cand_max_rows / nq candidates per image
-      const int max_rows = ex->cand_max_rows / nq * ex->maps_ld;
-      const dim3 grid(static_cast<unsigned>(ex->cand_imgs), static_cast<unsigned>((max_rows + pq::AMAP_ROWS - 1) / pq::AMAP_ROWS));
-      PQ_TRY(launch_k(e->lo, e->T <= 128 ? pq::dec_cross_attn_maps_grouped_kernel<4> : pq::dec_cross_attn_maps_grouped_kernel<8>,
-                      grid, dim3(pq::AMAP_THREADS), 0, st, static_cast<const float*>(sg.qc), ckv_of(e, l), kv_rows, b_first,
-                      e->T, D, e->cfg.dec_num_heads, nq, cand_off, ex->maps_len, ex->maps_ld, maps));
-    } else {
+    PQ_TRY(dispatch_tokens(e->T, [&](auto tb) {
+      constexpr int NR = 4 * decltype(tb)::value;
+      if (p.cand_off != nullptr) {
+        // candidate scoring: every image's candidates' maps_ld map rows, at most cand_max_rows / nq candidates per image
+        const int max_rows = p.cand_max_rows / nq * p.maps_ld;
+        const dim3 grid(static_cast<unsigned>(p.cand_imgs), static_cast<unsigned>((max_rows + pq::AMAP_ROWS - 1) / pq::AMAP_ROWS));
+        return launch_k(e->lo, pq::dec_cross_attn_maps_grouped_kernel<NR>, grid, dim3(pq::AMAP_THREADS), 0, st, q, ckv_of(e, l),
+                        kv_rows, p.b_first, e->T, D, H, nq, p.cand_off, p.maps_len, p.maps_ld, p.maps);
+      }
       const dim3 grid(static_cast<unsigned>(B), static_cast<unsigned>((nq + pq::AMAP_ROWS - 1) / pq::AMAP_ROWS));
-      if (e->T <= 128)
-        PQ_TRY(launch_k(e->lo, pq::dec_cross_attn_maps_kernel<4>, grid, dim3(pq::AMAP_THREADS), 0, st, static_cast<const float*>(sg.qc),
-                        ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, maps));
-      else
-        PQ_TRY(launch_k(e->lo, pq::dec_cross_attn_maps_kernel<8>, grid, dim3(pq::AMAP_THREADS), 0, st, static_cast<const float*>(sg.qc),
-                        ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, maps));
-    }
-    if (ex->maps_only) return PARSEQ_OK;
+      return launch_k(e->lo, pq::dec_cross_attn_maps_kernel<NR>, grid, dim3(pq::AMAP_THREADS), 0, st, q, ckv_of(e, l), kv_rows,
+                      p.b_first, e->T, D, H, nq, p.maps);
+    }));
+    if (p.tail == Tail::MapsOnly) return PARSEQ_OK;
   }
   {
     TimedScope ts(e, st, CAT_DEC_ATTN, 4.0 * M * e->T * D);
-    const long long kv_rows = 1ll * e->max_batch * e->T;
-    if (cand_off != nullptr) {
-      // candidate scoring: the rows of each image's candidates attend to that image (64 rows per CTA)
-      constexpr int kRows = 64;
-      const dim3 grid(static_cast<unsigned>(ex->cand_imgs * e->cfg.dec_num_heads), static_cast<unsigned>((ex->cand_max_rows + kRows - 1) / kRows));
-      if (e->T <= 128)
-        PQ_TRY(launch_k(e->lo, pq::dec_cross_attn3_grouped_kernel<4>, grid, dim3(128), 0, st, static_cast<const float*>(sg.qc),
-                        ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, cand_off, kRows, sg.ca));
-      else
-        PQ_TRY(launch_k(e->lo, pq::dec_cross_attn3_grouped_kernel<8>, grid, dim3(128), 0, st, static_cast<const float*>(sg.qc),
-                        ckv_of(e, l), kv_rows, b_first, e->T, D, e->cfg.dec_num_heads, nq, cand_off, kRows, sg.ca));
-    } else if (e->T <= 128)
-      PQ_TRY(launch_k(e->lo, pq::dec_cross_attn3_kernel<4>, dim3(B * e->cfg.dec_num_heads), dim3(128), 0, st,
-                      static_cast<const float*>(sg.qc), ckv_of(e, l), kv_rows, b_first, e->T, D,
-                      e->cfg.dec_num_heads, nq, sg.ca));
-    else
-      PQ_TRY(launch_k(e->lo, pq::dec_cross_attn3_kernel<8>, dim3(B * e->cfg.dec_num_heads), dim3(128), 0, st,
-                      static_cast<const float*>(sg.qc), ckv_of(e, l), kv_rows, b_first, e->T, D,
-                      e->cfg.dec_num_heads, nq, sg.ca));
+    PQ_TRY(dispatch_tokens(e->T, [&](auto tb) {
+      constexpr int NR = 4 * decltype(tb)::value;
+      if (p.cand_off != nullptr) {
+        // candidate scoring: the rows of each image's candidates attend to that image (64 rows per CTA)
+        constexpr int kRows = 64;
+        const dim3 grid(static_cast<unsigned>(p.cand_imgs * H), static_cast<unsigned>((p.cand_max_rows + kRows - 1) / kRows));
+        return launch_k(e->lo, pq::dec_cross_attn3_grouped_kernel<NR>, grid, dim3(128), 0, st, q, ckv_of(e, l), kv_rows,
+                        p.b_first, e->T, D, H, nq, p.cand_off, kRows, sg.ca);
+      }
+      return launch_k(e->lo, pq::dec_cross_attn3_kernel<NR>, dim3(B * H), dim3(128), 0, st, q, ckv_of(e, l), kv_rows, p.b_first,
+                      e->T, D, H, nq, sg.ca);
+    }));
   }
   PQ_TRY(gemm(e, sg.ca, D, e->w(Ly + "cross_attn.out_proj.weight"), D, e->wf(Ly + "cross_attn.out_proj.bias"), M, D, D,
               pq::EPI_F32, 1.0f, x, D, 0, x, D, st));
@@ -1191,26 +1216,23 @@ int dec_layer_rest(parseq_engine* e, parseq_engine::Stage& sg, int l, int b_firs
   return PARSEQ_OK;
 }
 
-// Content stream of a decoder of depth >= 2 (modules.py:94-97, 119-123): context rows [k0, k0 + nc) of B images through
-// layers 0..depth-2, each appending its K/V rows of the next layer to that layer's cache (row b * pitch + k).  nc is 1
-// (an AR step, pitch L: the causal content rows of earlier positions do not change as the context grows) or nkeys = pitch
-// (a whole pass).  The content rows attend to keys 0..nkeys-1 under `mode` (0: all, 1: cloze + first EOS), or under the
-// caller's content / padding masks (decode API, `ex`), whose candidates' row map (scoring) routes the cross-attention.
-// rpi > 1 (beam search, nc = 1): the B rows are rpi consecutive beams of each of B / rpi images.
-int content_stream(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, int k0, int nc, int nkeys, int pitch,
-                   int mode, const int* ids, const DecodeExtras* ex, cudaStream_t st, int rpi) {
-  const int D = e->D, M = B * nc;
-  const unsigned char* cmask = ex != nullptr ? ex->cmask : nullptr;
-  const unsigned char* pmask = ex != nullptr ? ex->pmask : nullptr;
+// Content stream of a decoder of depth >= 2 (modules.py:94-97, 119-123): context rows [k0, k0 + nc) of the pass's B
+// rows through layers 0..depth-2, each appending its K/V rows of the next layer to that layer's cache (row b * pitch + k).
+// An AR step computes its own position's row (nc = 1, pitch L: the causal content rows of earlier positions do not change
+// as the context grows), any other pass its whole context (nc = nkeys = pitch).  The content rows attend to keys
+// 0..nkeys-1 under the pass's mask, or under the caller's content / padding masks (self_mask).  Beam rows (nc = 1) are
+// p.beam consecutive rows per image.
+int content_stream(parseq_engine* e, parseq_engine::Stage& sg, const DecodePass& p, cudaStream_t st) {
+  const int k0 = p.ar_step ? p.q0 : 0, nc = p.ar_step ? 1 : p.nkeys, pitch = p.kv_pitch(e);
+  const int D = e->D, M = p.B * nc;
   const float qscale = 1.0f / std::sqrt(static_cast<float>(e->dh_dec));
   {
     TimedScope ts(e, st, CAT_MISC, 0.0);
     const long long total = 1ll * M * D;
     PQ_TRY(launch_k(e->lo, pq::gather_ctx_rows_kernel, dim3(static_cast<unsigned>(std::min<long long>((total + 255) / 256, 132ll * 8))),
-                    dim3(256), 0, st, e->wf("text_embed.embedding.weight"), e->wf("pos_queries"), ids, e->ids_ld, B, k0, nc, D,
+                    dim3(256), 0, st, e->wf("text_embed.embedding.weight"), e->wf("pos_queries"), p.ids, e->ids_ld, p.B, k0, nc, D,
                     std::sqrt(static_cast<float>(D)), sg.cx));
   }
-  if (cmask != nullptr || pmask != nullptr) mode = 2;
   PQ_TRY(layernorm(e, sg.cx, "decoder.layers.0.norm_c", 1e-5f, M, sg.yn, nullptr, st));
   const long long ldo = (nc == pitch ? 1ll : pitch) * 2 * D;
   for (int l = 0; l + 1 < e->cfg.dec_depth; ++l) {
@@ -1218,9 +1240,8 @@ int content_stream(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int 
     const std::string Ly = "decoder.layers." + std::to_string(l) + ".";
     PQ_TRY(gemm(e, sg.yn, D, e->w(Ly + "self_attn.in_proj_weight"), D, e->wf(Ly + "self_attn.in_proj_bias"), M, D, D,
                 pq::EPI_F32, qscale, nullptr, 0, 0, sg.qc, D, st));
-    PQ_TRY(self_attn_rows(e, sg.qc, l == 0 ? e->kvtab : sg.kvc[l - 1], l > 0, pitch, ids, B, nc, k0, nkeys, mode, cmask, pmask,
-                          sg.sa, st));
-    PQ_TRY(dec_layer_rest(e, sg, l, b_first, B / rpi, nc * rpi, sg.cx, nullptr, 0, st, ex, false));
+    PQ_TRY(self_attn_rows(e, sg, p, l, /*content*/ true, nc, k0, st));
+    PQ_TRY(dec_layer_rest(e, sg, p, l, nc, sg.cx, nullptr, 0, /*maps_layer*/ false, st));
     // K/V of layer l + 1 = W_kv norm_c_{l+1}(content_{l+1}) + b_kv, into rows k0.. of its cache
     const std::string Ln = "decoder.layers." + std::to_string(l + 1) + ".";
     PQ_TRY(layernorm(e, sg.cx, Ln + "norm_c", 1e-5f, M, sg.yn, nullptr, st));
@@ -1230,58 +1251,45 @@ int content_stream(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int 
   return PARSEQ_OK;
 }
 
-// ar_step: an AR step (nq = 1, query position q0, keys 0..q0): the content stream computes row q0 only and appends it to
-// the caches of pitch L; otherwise it computes the whole context (nkeys rows per image, pitch nkeys)
-int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, int nq, int q0, int nkeys,
-                int mode, const int* ids, float* logits_out, long long logits_ld, int* ids_dst, int dst_off,
-                const int* forced, int forced_ld, const uint32_t* mask, cudaStream_t st, const DecodeExtras* ex = nullptr,
-                bool ar_step = false) {
-  const int D = e->D, M = B * nq;
+// The decoder on the pass's rows: the content stream (depth >= 2), the query stream of every layer, then the tail.
+int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, const DecodePass& p, cudaStream_t st) {
+  if (p.tail == Tail::MapsOnly && p.maps == nullptr) return fail(PARSEQ_ERR_STATE, "decode_pass: a maps-only pass needs maps");
+  const int D = e->D, B = p.B, nq = p.nq, M = B * nq;
   const std::string Ly = "decoder.layers.0.";
   const float qscale = 1.0f / std::sqrt(static_cast<float>(e->dh_dec));
   e->cur_cat = CAT_DEC_GEMM;
-  const int kv_pitch = ar_step ? e->L : nkeys;
-  const int rpi = ex != nullptr ? ex->beam : 1;   // rows per image of the cross-attention (beam search)
-  if (e->cfg.dec_depth > 1)
-    PQ_TRY(content_stream(e, sg, b_first, B, ar_step ? q0 : 0, ar_step ? 1 : nkeys, nkeys, kv_pitch, mode, ids, ex, st, rpi));
+  if (e->cfg.dec_depth > 1) PQ_TRY(content_stream(e, sg, p, st));
   const float* qself = e->qs;            // [L, D] table of W_q LN_q(pos_queries), pre-scaled
-  const unsigned char *qmask = nullptr, *pmask = nullptr;
-  if (ex != nullptr && ex->query != nullptr) {
+  const SelfMask mode = self_mask(p, /*content*/ false);
+  if (p.query != nullptr) {
     // custom queries: q = scale * (W_q LN_q(query) + b_q), one row per (image, query)
-    PQ_TRY(layernorm(e, ex->query, Ly + "norm_q", 1e-5f, M, sg.yn, nullptr, st));
+    PQ_TRY(layernorm(e, p.query, Ly + "norm_q", 1e-5f, M, sg.yn, nullptr, st));
     PQ_TRY(gemm(e, sg.yn, D, e->w(Ly + "self_attn.in_proj_weight"), D, e->wf(Ly + "self_attn.in_proj_bias"), M, D, D,
                 pq::EPI_F32, qscale, nullptr, 0, 0, sg.qc, D, st));
     qself = sg.qc;
-    mode = 2;
-  }
-  if (ex != nullptr && (ex->qmask != nullptr || ex->pmask != nullptr)) {
-    if (mode != 2) {                     // masks with the default queries: expand the table rows (tiny) so mode 2 applies
-      // launched without PDL: the kernel has no griddepcontrol.wait, so as a PDL launch it could start under the previous
-      // kernel on the stream (an early-triggering GEMM: the cross K/V, or the previous scoring group's head), and every
-      // later kernel of this pass, which waits only for its own predecessor, would lose its order after that kernel
-      const int n4 = nq * D / 4;
-      PQ_TRY(launch_ex(LaunchConfig(dim3(static_cast<unsigned>(std::min((B * n4 + 255) / 256, 132 * 8))), dim3(256), 0, st, 0, false),
-                       pq::bcast_rows_kernel, reinterpret_cast<const float4*>(e->qs + static_cast<long long>(q0) * D),
-                       reinterpret_cast<float4*>(sg.qc.get()), n4, B));
-      e->launches++;
-      qself = sg.qc;
-      mode = 2;
-    }
-    qmask = ex->qmask; pmask = ex->pmask;
+  } else if (mode == SelfMask::Caller) {
+    // masks with the default queries: expand the table rows (tiny) so that mode 2 finds one query row per (image, query).
+    // Launched without PDL: the kernel has no griddepcontrol.wait, so as a PDL launch it could start under the previous
+    // kernel on the stream (an early-triggering GEMM: the cross K/V, or the previous scoring group's head), and every
+    // later kernel of this pass, which waits only for its own predecessor, would lose its order after that kernel
+    const int n4 = nq * D / 4;
+    PQ_TRY(launch_ex(LaunchConfig(dim3(static_cast<unsigned>(std::min((B * n4 + 255) / 256, 132 * 8))), dim3(256), 0, st, 0, false),
+                     pq::bcast_rows_kernel, reinterpret_cast<const float4*>(e->qs + static_cast<long long>(p.q0) * D),
+                     reinterpret_cast<float4*>(sg.qc.get()), n4, B));
+    e->launches++;
+    qself = sg.qc;
   }
   {
-    TimedScope ts(e, st, CAT_DEC_ATTN, 4.0 * M * nkeys * D);
+    TimedScope ts(e, st, CAT_DEC_ATTN, 4.0 * M * p.nkeys * D);
     const int qsplit = (nq >= 8) ? 4 : 1;
     // one key per lane up to 32 keys, two up to 64 (the kernel of the engine's id pitch)
     PQ_TRY(launch_k(e->lo, e->ids_ld == 32 ? pq::dec_self_attn2_kernel : pq::dec_self_attn2_long_kernel, dim3(B * qsplit),
-                    dim3(D < 384 ? D : 384), 0, st, qself, static_cast<const __nv_bfloat16*>(e->kvtab), ids, e->ids_ld, e->V,
-                    D, nq, q0, nkeys, mode, /*eos*/ 0, sg.sa, qsplit, qmask, pmask));
+                    dim3(D < 384 ? D : 384), 0, st, qself, static_cast<const __nv_bfloat16*>(e->kvtab), p.ids, e->ids_ld, e->V,
+                    D, nq, p.q0, p.nkeys, static_cast<int>(mode), /*eos*/ 0, sg.sa, qsplit, p.qmask, p.pmask));
   }
-  const bool own_q = ex != nullptr && ex->query != nullptr;
-  const float* resid = own_q ? ex->query : e->wf("pos_queries") + static_cast<long long>(q0) * D;
+  const float* resid = p.query != nullptr ? p.query : e->wf("pos_queries") + static_cast<long long>(p.q0) * D;
   const int last = e->cfg.dec_depth - 1;
-  const bool maps_only = ex != nullptr && ex->maps != nullptr && ex->maps_only;
-  PQ_TRY(dec_layer_rest(e, sg, 0, b_first, B / rpi, nq * rpi, sg.y, resid, own_q ? M : nq, st, ex, last == 0));
+  PQ_TRY(dec_layer_rest(e, sg, p, 0, nq, sg.y, resid, p.query != nullptr ? M : nq, last == 0, st));
   // query stream of layers >= 1 (modules.py:91-93): its residual base is the previous layer's output, its keys the
   // layer's content K/V cache
   for (int l = 1; l < e->cfg.dec_depth; ++l) {
@@ -1289,47 +1297,39 @@ int decode_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, 
     PQ_TRY(layernorm(e, sg.y, Ll + "norm_q", 1e-5f, M, sg.yn, nullptr, st));
     PQ_TRY(gemm(e, sg.yn, D, e->w(Ll + "self_attn.in_proj_weight"), D, e->wf(Ll + "self_attn.in_proj_bias"), M, D, D,
                 pq::EPI_F32, qscale, nullptr, 0, 0, sg.qc, D, st));
-    PQ_TRY(self_attn_rows(e, sg.qc, sg.kvc[l - 1], true, kv_pitch, ids, B, nq, q0, nkeys, mode, qmask, pmask, sg.sa, st));
-    PQ_TRY(dec_layer_rest(e, sg, l, b_first, B / rpi, nq * rpi, sg.y, nullptr, 0, st, ex, l == last));
+    PQ_TRY(self_attn_rows(e, sg, p, l, /*content*/ false, nq, p.q0, st));
+    PQ_TRY(dec_layer_rest(e, sg, p, l, nq, sg.y, nullptr, 0, l == last, st));
   }
-  if (maps_only) {
-    // the map pass of an AR-only schedule stops after the last layer's maps
-  } else if (ex != nullptr && ex->out_norm != nullptr) {
-    // PARSeq.decode returns the decoder output: final LayerNorm only (modules.py:123-125)
-    PQ_TRY(layernorm(e, sg.y, "decoder.norm", 1e-5f, M, sg.yn, ex->out_norm, st));
-  } else if (ex != nullptr && ex->lse_tgt != nullptr) {
-    // candidate scoring: the multi-query head's LayerNorm, then the head GEMM whose epilogue keeps only the per-row
-    // log-sum-exp partials and target logits (score_reduce_kernel finishes the terms)
-    PQ_TRY(layernorm(e, sg.y, "decoder.norm", 1e-5f, M, sg.yn, nullptr, st));
+  if (p.tail == Tail::MapsOnly) return PARSEQ_OK;   // dec_layer_rest stopped after the last layer's maps
+  if (p.tail == Tail::Head && nq == 1 && e->C <= 128) {
+    TimedScope ts(e, st, CAT_DEC_GEMM, 2.0 * M * e->C * D);
+    return ln_head_argmax_launch(e->lo, sg.y, e->wf("decoder.norm.weight"), e->wf("decoder.norm.bias"), 1e-5f,
+                                 e->wb("head.weight"), e->wf("head.bias"), M, e->C, D, p.logits, p.logits_ld, p.ids_dst,
+                                 e->ids_ld, nq, p.dst_off, p.forced, p.forced_ld, p.mask, st);
+  }
+  // decoder.norm (modules.py:123-125): PARSeq.decode returns it (Norm), every other tail feeds it to the head
+  PQ_TRY(layernorm(e, sg.y, "decoder.norm", 1e-5f, M, sg.yn, p.tail == Tail::Norm ? p.out_norm : nullptr, st));
+  if (p.tail == Tail::Norm) return PARSEQ_OK;
+  if (p.tail == Tail::LogSumExp) {
+    // candidate scoring: the head GEMM's epilogue keeps only the per-row log-sum-exp partials and target logits
+    // (score_reduce_kernel finishes the terms)
     TimedScope ts(e, st, CAT_SCORE, 2.0 * M * e->C * D);
-    PQ_TRY(gemm_lse_launch(e->lo, sg.yn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, ex->lse_tgt, sg.lse_part,
-                           sg.lse_tlogit, st));
-  } else if (ex != nullptr && ex->beam_keys != nullptr) {
-    PQ_TRY(layernorm(e, sg.y, "decoder.norm", 1e-5f, M, sg.yn, nullptr, st));
-    TimedScope ts(e, st, CAT_DEC_GEMM, 2.0 * M * e->C * D);
-    PQ_TRY(gemm_topk_launch(e->lo, sg.yn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, ex->beam_k, ex->beam_mask,
-                            rpi, ex->beam_part, ex->beam_keys, st));
-  } else if (nq > 1 && ids_dst == nullptr) {
-    // multi-query passes (refine / NAR): LayerNorm kernel + wgmma GEMM for the head (weights read once per tile).
-    // Chosen by pass type, not by batch size, so that a row's result does not depend on the batch it is computed in.
-    PQ_TRY(layernorm(e, sg.y, "decoder.norm", 1e-5f, M, sg.yn, nullptr, st));
-    PQ_TRY(gemm(e, sg.yn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, pq::EPI_F32, 1.0f, nullptr, 0, 0,
-                logits_out, logits_ld, st));
-  } else if (e->C > 128) {
-    // single-query tail of a head too large for the fused kernel's shared memory: LayerNorm, the wgmma GEMM and the
-    // greedy argmax (one AR step, nq == 1: row b of the step's logits is at logits_out + b * logits_ld)
-    PQ_TRY(layernorm(e, sg.y, "decoder.norm", 1e-5f, M, sg.yn, nullptr, st));
-    PQ_TRY(gemm(e, sg.yn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, pq::EPI_F32, 1.0f, nullptr, 0, 0,
-                logits_out, logits_ld, st));
-    if (ids_dst != nullptr)
-      PQ_TRY(argmax_rows(e, logits_out, static_cast<int>(logits_ld / e->C), B, nq, 0, ids_dst, e->ids_ld, dst_off, forced,
-                         forced_ld, mask, st));
-  } else {
-    TimedScope ts(e, st, CAT_DEC_GEMM, 2.0 * M * e->C * D);
-    PQ_TRY(ln_head_argmax_launch(e->lo, sg.y, e->wf("decoder.norm.weight"), e->wf("decoder.norm.bias"), 1e-5f, e->wb("head.weight"),
-                                 e->wf("head.bias"), M, e->C, D, logits_out, logits_ld, ids_dst, e->ids_ld, nq, dst_off, forced,
-                                 forced_ld, mask, st));
+    return gemm_lse_launch(e->lo, sg.yn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, p.lse_tgt, sg.lse_part,
+                           sg.lse_tlogit, st);
   }
+  if (p.tail == Tail::TopK) {
+    TimedScope ts(e, st, CAT_DEC_GEMM, 2.0 * M * e->C * D);
+    return gemm_topk_launch(e->lo, sg.yn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, p.k, p.mask, p.beam,
+                            p.part, p.keys, st);
+  }
+  // Head of a multi-query pass (refine / NAR) or too large for the fused kernel's shared memory: the wgmma GEMM (weights
+  // read once per tile), then the greedy argmax if ids are asked for.  Chosen by pass type, not by batch size, so that a
+  // row's result does not depend on the batch it is computed in.
+  PQ_TRY(gemm(e, sg.yn, D, e->w("head.weight"), D, e->wf("head.bias"), M, e->C, D, pq::EPI_F32, 1.0f, nullptr, 0, 0, p.logits,
+              p.logits_ld, st));
+  if (p.ids_dst != nullptr)
+    PQ_TRY(argmax_rows(e, p.logits, static_cast<int>(p.logits_ld / e->C), B, nq, 0, p.ids_dst, e->ids_ld, p.dst_off, p.forced,
+                       p.forced_ld, p.mask, st));
   return PARSEQ_OK;
 }
 
@@ -1348,16 +1348,16 @@ int argmax_rows(parseq_engine* e, float* logits, int L, int B, int nrows, int sr
 // step i is a fixed function of the memory and the context 0..i, so one pass over the AR loop's own ids
 // [BOS, ids[:, :L-1]] (`ids`: its [B, ids_ld] id rows) under the causal query mask, and at depth >= 2 the causal content
 // mask, computes every step's query at once (the argument parseq_score rests on).  It stops after the last layer's maps
-// and writes nothing else the caller sees; whichever AR loop ran, the maps depend only on the ids.
+// and writes nothing else the caller sees; whichever AR loop ran, the maps depend only on the ids.  beam > 1 (beam
+// search): the B rows are `beam` consecutive hypotheses of each image.
 int ar_maps_pass(parseq_engine* e, parseq_engine::Stage& sg, int b_first, int B, int L, const int* ids, float* maps,
-                 cudaStream_t st) {
+                 cudaStream_t st, int beam = 1) {
   const unsigned char* causal = e->sc_causal + 1ll * (L - 1) * e->L * e->L;
-  DecodeExtras ex;
-  ex.qmask = causal;
-  ex.cmask = e->cfg.dec_depth > 1 ? causal : nullptr;
-  ex.maps = maps;
-  ex.maps_only = true;
-  return decode_pass(e, sg, b_first, B, L, 0, L, 0, ids, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, st, &ex);
+  DecodePass p;
+  p.b_first = b_first; p.B = B; p.nq = L; p.nkeys = L; p.ids = ids; p.beam = beam;
+  p.qmask = causal; p.cmask = e->cfg.dec_depth > 1 ? causal : nullptr;
+  p.maps = maps; p.tail = Tail::MapsOnly;
+  return decode_pass(e, sg, p, st);
 }
 
 // id rows [B, ids_ld] = BOS, PAD, PAD, ...: the context of a first AR step or of a NAR / refinement pass
@@ -1376,22 +1376,25 @@ int fill_ids(parseq_engine* e, int* ids, int B, cudaStream_t st) {
 int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const parseq_forward_args* a, int b0,
                  int B, int L, float* logits, int* ids_out, int* steps, const uint32_t* mask, cudaStream_t st, bool ar_done,
                  float* maps) {
-  DecodeExtras mx;                  // the final pass's extras: its maps
-  mx.maps = maps;
-  const DecodeExtras* last_ex = maps != nullptr ? &mx : nullptr;
   // b_first: index of the group's first image inside the super-chunk (row of the K/V cache); b0: inside the caller's batch
   const int C = e->C;
   const bool testing = a->max_length < 0;
-  const long long LC = static_cast<long long>(L) * C;
+  DecodePass chain;                 // what the chain's passes share: their rows, Head tails into [B, L, C] logits
+  chain.b_first = b_first; chain.B = B; chain.logits = logits; chain.logits_ld = C; chain.mask = mask;
   if (a->decode_ar && ar_done) {
     // the AR loop of the whole super-chunk already ran in the persistent kernel (ar_decode)
   } else if (a->decode_ar) {
     PQ_TRY(fill_ids(e, sg.ids_ar, B, st));
-    const int* forced = a->forced_ids ? a->forced_ids + static_cast<long long>(b0) * L : nullptr;
+    DecodePass p = chain;
+    p.nq = 1; p.ids = sg.ids_ar; p.ar_step = true;
+    p.logits_ld = static_cast<long long>(L) * C;
+    p.forced = a->forced_ids ? a->forced_ids + static_cast<long long>(b0) * L : nullptr; p.forced_ld = L;
     for (int i = 0; i < L; ++i) {
-      // step i: context ids[:, :i+1], query position i; the fused tail writes ids[:, i+1] = argmax (model.py:142)
-      PQ_TRY(decode_pass(e, sg, b_first, B, 1, i, i + 1, 0, sg.ids_ar, logits + static_cast<long long>(i) * C, LC,
-                         (i + 1 < L) ? sg.ids_ar.get() : nullptr, i + 1, forced, L, mask, st, nullptr, /*ar_step*/ true));
+      // step i: context ids[:, :i+1], query position i; the head writes ids[:, i+1] = argmax (model.py:142)
+      p.q0 = i; p.nkeys = i + 1;
+      p.logits = logits + static_cast<long long>(i) * C;
+      p.ids_dst = i + 1 < L ? sg.ids_ar.get() : nullptr; p.dst_off = i + 1;
+      PQ_TRY(decode_pass(e, sg, p, st));
     }
     if (testing && steps != nullptr) {
       PQ_TRY(launch_k(e->lo, pq::ar_steps_kernel, dim3(1), dim3(256), 0, st, static_cast<const int*>(sg.ids_ar), e->ids_ld, B, L,
@@ -1400,8 +1403,10 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
     }
   } else {
     PQ_TRY(fill_ids(e, sg.ids_ctx, B, st));
-    PQ_TRY(decode_pass(e, sg, b_first, B, L, 0, 1, 0, sg.ids_ctx, logits, C, nullptr, 0, nullptr, 0, mask, st,
-                       a->refine_iters == 0 ? last_ex : nullptr));
+    DecodePass p = chain;
+    p.nq = L; p.nkeys = 1; p.ids = sg.ids_ctx;
+    p.maps = a->refine_iters == 0 ? maps : nullptr;
+    PQ_TRY(decode_pass(e, sg, p, st));
   }
   for (int it = 0; it < a->refine_iters; ++it) {
     PQ_TRY(fill_ids(e, sg.ids_ctx, B, st));
@@ -1410,8 +1415,10 @@ int decode_stage(parseq_engine* e, parseq_engine::Stage& sg, int b_first, const 
                             : nullptr;
     // ctx = [BOS, argmax(logits[:, :L-1])]  (model.py:161)
     PQ_TRY(argmax_rows(e, logits, L, B, L - 1, 0, sg.ids_ctx, e->ids_ld, 1, forced, L, mask, st));
-    PQ_TRY(decode_pass(e, sg, b_first, B, L, 0, L, 1, sg.ids_ctx, logits, C, nullptr, 0, nullptr, 0, mask, st,
-                       it + 1 == a->refine_iters ? last_ex : nullptr));
+    DecodePass p = chain;
+    p.nq = L; p.nkeys = L; p.ids = sg.ids_ctx; p.self_mask = SelfMask::Cloze;
+    p.maps = it + 1 == a->refine_iters ? maps : nullptr;
+    PQ_TRY(decode_pass(e, sg, p, st));
   }
   if (ids_out != nullptr || mask != nullptr) PQ_TRY(argmax_rows(e, logits, L, B, L, 0, ids_out, L, 0, nullptr, 0, mask, st));
   if (maps != nullptr && a->decode_ar && a->refine_iters == 0) PQ_TRY(ar_maps_pass(e, sg, b_first, B, L, sg.ids_ar, maps, st));
@@ -1601,9 +1608,10 @@ int ar_decode(parseq_engine* e, ArPath path, const parseq_forward_args* a, int b
     } else {
       PQ_TRY(dispatch_width(D, "dec_ar", [&](auto w) {
         constexpr int W = decltype(w)::value;
-        const dim3 grid(static_cast<unsigned>(e->lo.sm_count)), block(pq::DEC_THREADS);
-        return e->T <= 128 ? launch_k(e->lo, pq::dec_ar_kernel<W, 1>, grid, block, pq::dec_ar_smem_bytes<W>(), st, p)
-                           : launch_k(e->lo, pq::dec_ar_kernel<W, 2>, grid, block, pq::dec_ar_smem_bytes<W>(), st, p);
+        return dispatch_tokens(e->T, [&](auto tb) {
+          return launch_k(e->lo, pq::dec_ar_kernel<W, decltype(tb)::value>, dim3(static_cast<unsigned>(e->lo.sm_count)),
+                          dim3(pq::DEC_THREADS), pq::dec_ar_smem_bytes<W>(), st, p);
+        });
       }));
     }
   }
@@ -2514,21 +2522,18 @@ int score_impl(parseq_engine* e, const parseq_score_args* a, const void* images_
       const ScoreGroup& g = groups[gi + static_cast<size_t>(k)];
       const int B = g.m1 - g.m0;
       const unsigned char* causal = e->sc_causal + 1ll * (g.P - 1) * L * L;
-      DecodeExtras ex;
-      ex.qmask = causal;
-      ex.cmask = e->cfg.dec_depth > 1 ? causal : nullptr;
-      ex.lse_tgt = meta + g.tgt_off;
-      ex.cand_off = meta + g.cand_off;
-      ex.cand_imgs = g.nimg;
-      ex.cand_max_rows = g.max_rows;
+      DecodePass p;
+      p.b_first = g.b_lo - b0; p.B = B; p.nq = g.P; p.nkeys = g.P; p.ids = meta + g.ids_off;
+      p.qmask = causal; p.cmask = e->cfg.dec_depth > 1 ? causal : nullptr;
+      p.cand_off = meta + g.cand_off; p.cand_imgs = g.nimg; p.cand_max_rows = g.max_rows;
       if (a->attn_maps != nullptr) {
         // the last layer's query rows of this pass, under each candidate's L map rows (0 past its EOS)
-        ex.maps = a->attn_maps + 1ll * g.m0 * L * e->T;
-        ex.maps_len = meta + len_off + g.m0;
-        ex.maps_ld = L;
+        p.maps = a->attn_maps + 1ll * g.m0 * L * e->T;
+        p.maps_len = meta + len_off + g.m0;
+        p.maps_ld = L;
       }
-      PQ_TRY(decode_pass(e, sg, g.b_lo - b0, B, g.P, 0, g.P, 0, meta + g.ids_off, nullptr, 0, nullptr, 0, nullptr, 0, nullptr,
-                         ds, &ex));
+      p.tail = Tail::LogSumExp; p.lse_tgt = meta + g.tgt_off;
+      PQ_TRY(decode_pass(e, sg, p, ds));
       TimedScope ts(e, ds, CAT_SCORE, 0.0);
       return launch_k(e->lo, pq::score_reduce_kernel, dim3(static_cast<unsigned>(B)), dim3(64), 0, ds,
                       static_cast<const float2*>(sg.lse_part), ntiles, static_cast<const float*>(sg.lse_tlogit),
@@ -2613,7 +2618,7 @@ int lexicon_reserve(parseq_engine* e) {
 
 // Beam search over a batch of images (parseq_beam_search).  PARSeq: the encoder and the cross K/V once per super-chunk as
 // forward_super runs them, then groups of dec_chunk / K images (all K beams of an image in one group) round-robin over
-// the stages' streams; each step is one decoder pass over the group's beam rows (decode_pass with DecodeExtras::beam),
+// the stages' streams; each step is one decoder pass over the group's beam rows (decode_pass with DecodePass::beam),
 // the head's logits of the step, and beam_select_kernel.  ViTSTR: the head once over a group's [B * L] token rows, then
 // beam_select_kernel once per position.
 int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_any, bool u8, int* ids, int* lengths,
@@ -2695,13 +2700,13 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
       parseq_engine::Stage::Beam& bm = sg.bm;
       const int g0 = gi * G, Bg = std::min(G, Bc - g0), R = Bg * K;
       PQ_TRY(init(bm, Bg, ds));
-      DecodeExtras ex;
-      ex.beam = K;
+      DecodePass p;
+      p.b_first = g0; p.B = R; p.nq = 1; p.ar_step = true; p.beam = K;
       if (topk) {
-        ex.beam_part = bm.part;
-        ex.beam_keys = bm.keys;
-        ex.beam_k = K;
-        ex.beam_mask = a->class_mask ? a->class_mask + 1ll * (b0 + g0) * e->mask_ld : nullptr;
+        p.tail = Tail::TopK; p.part = bm.part; p.keys = bm.keys; p.k = K;
+        p.mask = a->class_mask ? a->class_mask + 1ll * (b0 + g0) * e->mask_ld : nullptr;
+      } else {
+        p.logits = bm.logits; p.logits_ld = C;
       }
       const std::vector<__nv_bfloat16*> kvc0(sg.kvc.begin(), sg.kvc.end());
       int rc = PARSEQ_OK;
@@ -2709,8 +2714,8 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
         // query position `step` over keys 0..step of every beam row; the head leaves row r's logits at bm.logits + r * C
         // (<= 128 classes, and at every C under a lexicon: the chain's head GEMM, no argmax) or its partials and top-K
         // keys (above)
-        rc = decode_pass(e, sg, g0, R, 1, step, step + 1, 0, bm.ids[step & 1], bm.logits, C, nullptr, 0, nullptr, 0, nullptr,
-                         ds, &ex, /*ar_step*/ true);
+        p.q0 = step; p.nkeys = step + 1; p.ids = bm.ids[step & 1];
+        rc = decode_pass(e, sg, p, ds);
         if (rc == PARSEQ_OK) rc = select(bm, Bg, step, 0, K, 1, b0 + g0, ds);
         if (rc != PARSEQ_OK || e->cfg.dec_depth == 1 || step + 1 == S) continue;
         // depth >= 2: each new beam row continues its parent's content K/V cache rows 0..step
@@ -2731,16 +2736,9 @@ int beam_impl(parseq_engine* e, const parseq_beam_args* a, const void* images_an
       if (rc != PARSEQ_OK || a->attn_maps == nullptr) return rc;
       // the final hypotheses' maps: the last selection left each row's [BOS, c_1..] in bm.ids[S & 1] (valid ids
       // everywhere), so one teacher-forced pass over the rows' first S ids under the causal masks computes every step's
-      // query (ar_maps_pass over beam rows); image j's K * S query rows are contiguous
+      // query; image j's K * S query rows are contiguous
       float* const maps = a->attn_maps + 1ll * (b0 + g0) * K * S * e->T;
-      const unsigned char* causal = e->sc_causal + 1ll * (S - 1) * L * L;
-      DecodeExtras mx;
-      mx.beam = K;
-      mx.qmask = causal;
-      mx.cmask = e->cfg.dec_depth > 1 ? causal : nullptr;
-      mx.maps = maps;
-      mx.maps_only = true;
-      PQ_TRY(decode_pass(e, sg, g0, R, S, 0, S, 0, bm.ids[S & 1], nullptr, 0, nullptr, 0, nullptr, 0, nullptr, ds, &mx));
+      PQ_TRY(ar_maps_pass(e, sg, g0, R, S, bm.ids[S & 1], maps, ds, K));
       TimedScope ts(e, ds, CAT_MAPS, 0.0);
       return launch_k(e->lo, pq::maps_zero_tail_kernel, dim3(static_cast<unsigned>(R)), dim3(256), 0, ds, maps,
                       static_cast<const int*>(lengths + 1ll * (b0 + g0) * K), S, e->T);
@@ -3404,13 +3402,13 @@ int parseq_decode_ex(parseq_engine* e, int32_t batch, int32_t ctx_len, int32_t n
     pq::copy_ids_kernel<<<(Bc * e->ids_ld + 255) / 256, 256, 0, st>>>(tgt + 1ll * b0 * J, J, sg.ids_ctx, Bc, e->ids_ld);
     PQ_CUDA(cudaGetLastError());
     e->launches += 2;
-    DecodeExtras ex;
-    ex.query = query ? query + 1ll * b0 * NQ * D : nullptr;
-    ex.qmask = query_mask;
-    ex.pmask = padding_mask ? padding_mask + 1ll * b0 * J : nullptr;
-    ex.cmask = content_mask;
-    ex.out_norm = out + 1ll * b0 * NQ * D;
-    PQ_TRY(decode_pass(e, sg, 0, Bc, NQ, 0, J, 0, sg.ids_ctx, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, st, &ex));
+    DecodePass p;
+    p.B = Bc; p.nq = NQ; p.nkeys = J; p.ids = sg.ids_ctx;
+    p.query = query ? query + 1ll * b0 * NQ * D : nullptr;
+    p.qmask = query_mask; p.cmask = content_mask;
+    p.pmask = padding_mask ? padding_mask + 1ll * b0 * J : nullptr;
+    p.tail = Tail::Norm; p.out_norm = out + 1ll * b0 * NQ * D;
+    PQ_TRY(decode_pass(e, sg, p, st));
   }
   return leave_main(e, user);
 }
